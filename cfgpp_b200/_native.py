@@ -12,7 +12,7 @@ from pathlib import Path
 
 import torch
 
-# CFGPP_B200_LIB points at an alternative build of the same library (A/B experiments with tools/build_variant.sh)
+# CFGPP_B200_LIB points at an alternative build of the same library (A/B experiments)
 _LIB_PATH = Path(os.environ.get("CFGPP_B200_LIB") or Path(__file__).resolve().parent / "lib" / "libcfgpp_b200.so")
 _lib = None
 

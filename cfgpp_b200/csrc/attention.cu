@@ -1,23 +1,14 @@
-// cfgpp_b200 — flash-style attention forward for head_dim 64 on tcgen05/TMEM (sm_100a). See attention.cuh.
+// cfgpp_b200 — flash-style attention forward on sm_90a tensor cores (mma.sync m16n8k16). See attention.cuh.
 //
-// One CTA = up to two 128-row query tiles of one (batch, head) ("ping-pong"), looping over 128-wide KV tiles that
-// both query tiles share (K / V are fetched once per pair):
-//   warp 0 lane 0 : TMA producer (Q0, Q1 once; K / V rings, 128B swizzle)
-//   warp 1 lane 0 : MMA issuer   S_q = Q_q K_j^T   (M128 N128 K64, fp32 in TMEM)
-//                                O_q += P_q V_j    (M128 N64 K128; A = P from swizzled smem, B = V MN-major).
-//                   Event driven: QK_q(j+1) is issued as soon as the softmax warps of q have pulled S_q(j) into
-//                   registers (s_free), PV_q(j) as soon as P_q(j) is in shared memory (p_full) — whichever comes
-//                   first — so neither query tile's softmax ever waits for the tensor pipe
-//   warp 2        : TMEM allocator (512 columns: S0 [0,128) S1 [128,256) O0 [256,320) O1 [320,384))
-//   warps 4..7    : softmax of query tile 0, warps 8..11: query tile 1 — one row per thread:
-//                   a single TMEM read of the 128 scores into registers, row max, p = exp2((s - m) * scale*log2e),
-//                   fp32 row sum, P rounded to fp16 into smem. O accumulates in TMEM across KV tiles; the running
-//                   max is only advanced (and O / l rescaled, through tcgen05.ld/st) when the new maximum exceeds
-//                   the reference by more than 2^8 in the exp2 domain — exact after the final 1/l normalisation,
-//                   and p <= 256 stays well inside fp16 / fp32 range.
+// One CTA = one 64-row query tile of one (batch, head), 4 warps of 16 query rows each, looping over 64-row KV tiles:
+//   thread 0 : TMA producer (Q once; K / V into a 2-deep ring, 128B swizzle, mbarrier complete_tx)
+//   all      : S = Q K^T (ldmatrix from the swizzled tiles, fp32 accumulators in registers), online softmax on the
+//              accumulator fragments (running max and sum per row, exp2 with the scale folded in), P rounded to fp16
+//              and fed straight back from registers as the A operand of O += P V (V through ldmatrix.trans).
+// The same kernel serves self-attention (Nkv = Nq) and cross-attention (Nkv = 77 text tokens): a KV tile past Nkv is
+// zero-filled by the TMA and its columns are masked to -inf. Head dims of 40 / 80 / 160 arrive zero-padded to 64 / 128
+// / 192 columns; the padding columns of V are zero, so those of the output are too.
 #include <cmath>
-#include <cstdlib>
-#include <cstring>
 
 #include "attention.cuh"
 #include "common.cuh"
@@ -25,413 +16,210 @@
 namespace cfgpp {
 
 void attn_configure();
-// attention_cross.cu: single-KV-tile (cross-attention) kernel
-void xattn_configure();
-bool xattn_applicable(const AttnOp& op);
-void run_xattn_op(const AttnOp& op, cudaStream_t stream);
-// attention_persist.cu: persistent self-attention for head dim 64 (one CTA per SM, balanced tile ranges)
-void attn_persist_configure();
-bool attn_persist_applicable(const AttnOp& op);
-void run_attn_persist_op(const AttnOp& op, cudaStream_t stream);
 
 namespace {
 
-constexpr int BQ = 128;
-constexpr int BKV = 128;
-constexpr int ATOM_BYTES = 128 * 64 * 2;  // 16 KB: one [128 rows x 64 fp16] swizzle-128B atom
-constexpr int kThreads = 384;
-constexpr uint32_t TMEM_COLS = 512;
-constexpr float kRescaleThreshold = 8.0f;  // log2 units
-constexpr int kDefaultPoly = 0;            // see attn_poly()
-constexpr int kDefaultRowsumMma = 0;       // see attn_rowsum_mma()
-constexpr int kDefaultPbuf = 1;            // see attn_pbuf()
+constexpr int BQ = 64;
+constexpr int BKV = 64;
+constexpr int kThreads = 128;
+constexpr int ATOM_BYTES = 64 * 64 * 2;  // 8 KB: one [64 rows x 64 fp16] swizzle-128B atom
 
-// HD = padded head dim (64 / 128 / 192: heads of 40 / 80 / 160 channels are zero-padded by the QKV projection),
-// NQT = query tiles per CTA, KS = K / V ring depth. TMEM: S_q at [q*128], O_q at [NQT*128 + q*HD].
-// RS: the softmax row sums come out of the P V tensor-core product (a constant "ones" column appended to V: O gets 16
-// extra columns, column HD = sum_j fp16(p_j)) instead of 128 FADDs per thread and tile.
-// PB: P buffers per query tile. With one buffer the softmax of KV tile j+1 must wait for PV(j) to retire before it may
-// write P (a 0.3-0.6 us bubble on every step: issue poll + 8 MMAs + commit); with two it only waits for PV(j-1).
-template <int HD, int NQT, int KS, bool RS = false, int PB = 1>
+template <int HD>
 struct ACfg {
-  static constexpr int NA = HD / 64;                    // swizzle atoms per tile row
-  static constexpr int TILE_BYTES = NA * ATOM_BYTES;    // one Q / K / V tile
-  static constexpr int P_BYTES = 2 * ATOM_BYTES;        // one P tile (128 x 128 fp16)
-  static constexpr int OW = HD + (RS ? 16 : 0);        // accumulator columns per query tile
-  static constexpr int SMEM_BYTES =
-      TILE_BYTES * (NQT + 2 * KS) + P_BYTES * NQT * PB + (RS ? ATOM_BYTES : 0) + 1024 + 256;
-  static constexpr uint32_t O_COL = NQT * 128;
-  static_assert(!RS || HD == 64, "the ones column is implemented for head dim 64");
-  static_assert(NQT * 128 + NQT * OW <= 512, "TMEM overflow");
+  static constexpr int NA = HD / 64;                  // swizzle atoms per tile row
+  static constexpr int TILE_BYTES = NA * ATOM_BYTES;  // one Q / K / V tile
+  static constexpr int SMEM_BYTES = TILE_BYTES * 5 + 1024 + 64;  // Q + 2 x K + 2 x V, alignment slack, barriers
   static_assert(SMEM_BYTES <= 232448, "shared memory overflow");
 };
 
-// POLY: 0 = every exponential on the MUFU pipe; n > 0 = every n-th one through exp2_poly() on the FMA pipe
-template <int HD, int NQT, int KS, int POLY, bool RS, int PB>
-__global__ void __launch_bounds__(kThreads, 1)
+// byte offset of (row, 16-byte chunk) in a tile of NA atoms [64 rows x 128 B] (128B swizzle: chunk ^= row % 8)
+CFGPP_DEVICE uint32_t tile_off(int row, int chunk) {
+  return (chunk >> 3) * ATOM_BYTES + row * 128 + (((chunk & 7) ^ (row & 7)) << 4);
+}
+
+template <int HD>
+__global__ void __launch_bounds__(kThreads)
 attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
             const __grid_constant__ CUtensorMap map_v) {
-  using A = ACfg<HD, NQT, KS, RS, PB>;
-  constexpr int OW = A::OW;
-  constexpr int TILE_BYTES = A::TILE_BYTES;
+  using A = ACfg<HD>;
   constexpr int NA = A::NA;
-  constexpr uint32_t O_COL = A::O_COL;
+  constexpr int TILE_BYTES = A::TILE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint8_t* sQ = smem;                      // NQT tiles
-  uint8_t* sK = sQ + NQT * TILE_BYTES;     // KS tiles
-  uint8_t* sV = sK + KS * TILE_BYTES;      // KS tiles
-  uint8_t* sP = sV + KS * TILE_BYTES;      // NQT query tiles x PB buffers x 2 halves of 64 columns
-  uint8_t* sOnes = sP + NQT * PB * A::P_BYTES;  // RS: [128 kv rows x 64] fp16 MN-major atom whose column 0 is 1.0
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sOnes + (RS ? ATOM_BYTES : 0));
-  uint64_t* q_full = bars;            // [2]
-  uint64_t* k_full = q_full + 2;      // [KS]
-  uint64_t* k_empty = k_full + KS;
-  uint64_t* v_full = k_empty + KS;
-  uint64_t* v_empty = v_full + KS;
-  uint64_t* s_full = v_empty + KS;    // [2]
-  uint64_t* s_free = s_full + 2;      // [2]
-  uint64_t* p_full = s_free + 2;      // [2][PB]: one barrier per P buffer (a buffer's phases cannot alias)
-  uint64_t* pv_done = p_full + 2 * PB;  // [2][PB]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(pv_done + 2 * PB);
+  uint8_t* sQ = smem;
+  uint8_t* sK = sQ + TILE_BYTES;      // 2 tiles
+  uint8_t* sV = sK + 2 * TILE_BYTES;  // 2 tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * TILE_BYTES);
+  uint64_t* q_full = bars;        // [1]
+  uint64_t* kv_full = bars + 1;   // [2]
 
-  const int warp_idx = threadIdx.x >> 5;
+  const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * NQT * BQ;
+  const int q0 = blockIdx.x * BQ;
   const int head = blockIdx.y;
   const int batch = blockIdx.z;
   const int n_tiles = (p.Nkv + BKV - 1) / BKV;
-  const int n_qt = (NQT == 2 && q0 + BQ < p.Nq) ? 2 : 1;  // query tiles handled by this CTA
 
-  if (warp_idx == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_k);
     tma_prefetch_desc(&map_v);
-  }
-  if (warp_idx == 1 && lane == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&q_full[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_free[i], 128);
-      for (int b = 0; b < PB; ++b) {
-        mbar_init(&p_full[i * PB + b], 128);
-        mbar_init(&pv_done[i * PB + b], 1);
-      }
-    }
-    for (int i = 0; i < KS; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], n_qt);  // one tcgen05.commit per query tile that consumed the stage
-      mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], n_qt);
-    }
+    mbar_init(q_full, 1);
+    mbar_init(&kv_full[0], 1);
+    mbar_init(&kv_full[1], 1);
     fence_barrier_init();
   }
-  if (warp_idx == 2) {
-    tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-    tmem_relinquish();
-  }
-  if constexpr (RS) {
-    if (warp_idx == 3) {  // row k: element (k, 0) = 1.0, the 16-byte chunk holding it sits at chunk (0 ^ (k & 7)) (128B swizzle)
-      for (int k = lane; k < 128; k += 32) {
-        uint4* rowp = reinterpret_cast<uint4*>(sOnes + k * 128);
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) rowp[ch] = make_uint4(ch == (k & 7) ? 0x00003C00u : 0u, 0u, 0u, 0u);
-      }
-      fence_proxy_async_smem();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_launch_dependents();
   pdl_wait();
 
-  if (warp_idx == 0) {
-    if (lane == 0) {
-      // ===================== TMA producer =====================
-      for (int qt = 0; qt < n_qt; ++qt) {
-        mbar_arrive_expect_tx(&q_full[qt], TILE_BYTES);
-        for (int a = 0; a < NA; ++a)
-          tma_load_3d(sQ + qt * TILE_BYTES + a * ATOM_BYTES, &map_q, &q_full[qt], head * HD + a * 64, q0 + qt * BQ,
-                      batch);
-      }
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j % KS;
-        const uint32_t ph = (j / KS) & 1;
-        mbar_wait(&k_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&k_full[s], TILE_BYTES);
-        for (int a = 0; a < NA; ++a)
-          tma_load_3d(sK + s * TILE_BYTES + a * ATOM_BYTES, &map_k, &k_full[s], head * HD + a * 64, j * BKV, batch);
-        mbar_wait(&v_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&v_full[s], TILE_BYTES);
-        for (int a = 0; a < NA; ++a)
-          tma_load_3d(sV + s * TILE_BYTES + a * ATOM_BYTES, &map_v, &v_full[s], head * HD + a * 64, j * BKV, batch);
-      }
+  auto load_kv = [&](int j) {  // thread 0
+    const int s = j & 1;
+    mbar_arrive_expect_tx(&kv_full[s], 2 * TILE_BYTES);
+#pragma unroll
+    for (int a = 0; a < NA; ++a) {
+      tma_load_3d(sK + s * TILE_BYTES + a * ATOM_BYTES, &map_k, &kv_full[s], head * HD + a * 64, j * BKV, batch);
+      tma_load_3d(sV + s * TILE_BYTES + a * ATOM_BYTES, &map_v, &kv_full[s], head * HD + a * 64, j * BKV, batch);
     }
-  } else if (warp_idx == 1) {
-    if (lane == 0) {
-      // ===================== MMA issuer =====================
-      constexpr uint32_t idesc_qk = make_idesc_f16(128, BKV, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_f16(128, OW, 0, 1);  // B (= V [+ ones column]) is MN-major
-      auto issue_qk = [&](int qt, int j) {
+  };
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(q_full, TILE_BYTES);
 #pragma unroll
-        for (int a = 0; a < NA; ++a) {  // K dimension = head dim: one 64-wide swizzle atom at a time
-          const uint64_t q_desc = make_sdesc_sw128(smem_u32(sQ + qt * TILE_BYTES + a * ATOM_BYTES), 1024, 0);
-          const uint64_t k_desc = make_sdesc_sw128(smem_u32(sK + (j % KS) * TILE_BYTES + a * ATOM_BYTES), 1024, 0);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_f16(tmem_base + qt * BKV, q_desc + 2 * k, k_desc + 2 * k, idesc_qk, (a | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(&s_full[qt]);
-      };
-      auto issue_pv = [&](int qt, int j) {
-        // V tile: 128 kv rows x HD d as NA atoms of [128 rows x 64 d] (128 B per row, swizzled) = MN-major B operand:
-        // 8-row K groups are 1024 B apart (SBO), 64-wide N atoms 16 KB apart (LBO); a K step of 16 rows advances 2048 B.
-        // (RS: the second 64-wide N atom is the constant ones tile, reached through the leading-dimension byte offset)
-        const uint32_t v_addr = smem_u32(sV + (j % KS) * TILE_BYTES);
-        const uint64_t v_desc = make_sdesc_sw128(v_addr, 1024, RS ? (smem_u32(sOnes) - v_addr) : ATOM_BYTES);
-        const uint8_t* pbuf = sP + (qt * PB + (j % PB)) * A::P_BYTES;
-#pragma unroll
-        for (int k = 0; k < BKV / 16; ++k) {
-          const uint64_t p_desc = make_sdesc_sw128(smem_u32(pbuf + (k >> 2) * ATOM_BYTES), 1024, 0) + 2 * (k & 3);
-          umma_f16(tmem_base + O_COL + qt * OW, p_desc, v_desc + 128 * k, idesc_pv, (j | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(&pv_done[qt * PB + (j % PB)]);
-      };
-      for (int qt = 0; qt < n_qt; ++qt) mbar_wait(&q_full[qt], 0);
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      for (int qt = 0; qt < n_qt; ++qt) {
-        issue_qk(qt, 0);
-        umma_commit(&k_empty[0]);
-      }
-      int next_qk[2] = {1, 1}, next_pv[2] = {0, 0};
-      int remaining = n_qt * (2 * n_tiles - 1);
-      long long t_start = clock64();
-      while (remaining > 0) {
-        bool progressed = false;
-        for (int qt = 0; qt < n_qt; ++qt) {
-          int j = next_pv[qt];
-          if (j < n_tiles && mbar_try_wait(&p_full[qt * PB + (j % PB)], (j / PB) & 1) &&
-              mbar_try_wait(&v_full[j % KS], (j / KS) & 1)) {
-            tc_fence_after();
-            issue_pv(qt, j);
-            umma_commit(&v_empty[j % KS]);
-            ++next_pv[qt];
-            --remaining;
-            progressed = true;
-          }
-          j = next_qk[qt];
-          if (j < n_tiles && mbar_try_wait(&s_free[qt], (j - 1) & 1) && mbar_try_wait(&k_full[j % KS], (j / KS) & 1)) {
-            tc_fence_after();
-            issue_qk(qt, j);
-            umma_commit(&k_empty[j % KS]);
-            ++next_qk[qt];
-            --remaining;
-            progressed = true;
-          }
-        }
-        if (progressed) {
-          t_start = clock64();
-        } else if (clock64() - t_start > 4000000000LL) {
-          printf("cfgpp: attention MMA issuer stalled (block %d,%d,%d)\n", blockIdx.x, blockIdx.y, blockIdx.z);
-          __trap();
-        }
-      }
-    }
-  } else if (warp_idx >= 4) {
-    // ===================== softmax / output =====================
-    const int qt = (warp_idx - 4) >> 2;
-    if (qt < n_qt) {
-      const int qw = warp_idx & 3;  // TMEM lane quarter of this warp
-      const int row = qw * 32 + lane;
-      const uint32_t lane_off = static_cast<uint32_t>(qw * 32) << 16;
-      const uint32_t s_addr = tmem_base + qt * BKV + lane_off;
-      const uint32_t o_addr = tmem_base + O_COL + qt * OW + lane_off;
-      uint8_t* prow0 = sP + qt * PB * A::P_BYTES + row * 128;
-      const float c = p.scale_log2e;
-      float m_ref = -INFINITY, l_run = 0.f;
-
-      for (int j = 0; j < n_tiles; ++j) {
-        const int valid = p.Nkv - j * BKV;  // columns >= valid are padding (last tile only)
-        mbar_wait(&s_full[qt], j & 1);
-        tc_fence_after();
-        uint32_t s[128];
-#pragma unroll
-        for (int g = 0; g < 4; ++g) tmem_ld_x32(s_addr + g * 32, *reinterpret_cast<uint32_t(*)[32]>(&s[g * 32]));
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(&s_free[qt]);  // scores are in registers: the tensor pipe may already produce S_q(j+1)
-        if (valid < BKV) {
-#pragma unroll
-          for (int i = 0; i < 128; ++i)
-            if (i >= valid) s[i] = 0xff800000u;  // -inf
-        }
-        // row maximum: eight independent chains of three-input maxima (two dependent chains of 63 two-input ones
-        // cost ~250 cycles of pure latency per tile)
-        float mxc[8];
-#pragma unroll
-        for (int k8 = 0; k8 < 8; ++k8) mxc[k8] = fmaxf(__uint_as_float(s[k8]), __uint_as_float(s[8 + k8]));
-#pragma unroll
-        for (int i = 16; i < 128; i += 16) {
-#pragma unroll
-          for (int k8 = 0; k8 < 8; ++k8) mxc[k8] = fmax3(mxc[k8], __uint_as_float(s[i + k8]), __uint_as_float(s[i + 8 + k8]));
-        }
-        const float mx = fmax3(fmax3(mxc[0], mxc[1], mxc[2]), fmax3(mxc[3], mxc[4], mxc[5]), fmaxf(mxc[6], mxc[7]));
-        // lazy running max: move the reference only when it would otherwise overflow the comfortable range
-        float alpha = 1.0f;
-        bool need = false;
-        if (j == 0) {
-          m_ref = mx;
-        } else if ((mx - m_ref) * c > kRescaleThreshold) {
-          alpha = fast_exp2((m_ref - mx) * c);
-          m_ref = mx;
-          need = true;
-        }
-        uint8_t* prow = prow0 + (j % PB) * A::P_BYTES;
-        if (j >= PB) {  // PV_q(j-PB) retired: its P buffer is reusable
-          mbar_wait(&pv_done[qt * PB + (j % PB)], ((j - PB) / PB) & 1);
-          tc_fence_after();
-        }
-        if (j > 0 && __any_sync(0xffffffffu, need)) {
-          if constexpr (PB > 1) {  // O_q is only rescalable once EVERY earlier PV has retired (in-order: the latest)
-            mbar_wait(&pv_done[qt * PB + ((j - 1) % PB)], ((j - 1) / PB) & 1);
-            tc_fence_after();
-          }
-#pragma unroll 1
-          for (int h = 0; h < OW / 16; ++h) {  // 16 columns at a time: the 128 scores stay live in registers
-            uint32_t o[16];
-            tmem_ld_x16(o_addr + h * 16, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int d = 0; d < 16; ++d) o[d] = __float_as_uint(__uint_as_float(o[d]) * alpha);
-            tmem_st_x16(o_addr + h * 16, o);
-          }
-          tmem_st_wait();
-          l_run *= alpha;
-        }
-        const float mc = m_ref * c;
-        float rs0 = 0.f, rs1 = 0.f;
-#pragma unroll
-        for (int g = 0; g < 16; ++g) {  // 16-byte chunks of the 256-byte P row (two 128-byte halves)
-          uint32_t pk[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float x0 = __uint_as_float(s[g * 8 + 2 * e]) * c - mc;
-            const float x1 = __uint_as_float(s[g * 8 + 2 * e + 1]) * c - mc;
-            // (g, e are unrolled: the selection folds at compile time)
-            constexpr int kP = POLY > 0 ? POLY : 1;
-            const bool poly0 = POLY > 0 && ((g * 8 + 2 * e) % kP) == kP - 1;
-            const bool poly1 = POLY > 0 && ((g * 8 + 2 * e + 1) % kP) == kP - 1;
-            const float p0 = poly0 ? exp2_poly(x0) : fast_exp2(x0);
-            const float p1 = poly1 ? exp2_poly(x1) : fast_exp2(x1);
-            if constexpr (!RS) {
-              rs0 += p0;
-              rs1 += p1;
-            }
-            pk[e] = pack_half2(p0, p1);
-          }
-          const int half_idx = g >> 3;        // which 64-column half
-          const int ch = (g & 7) ^ (row & 7);  // 128B swizzle
-          *reinterpret_cast<uint4*>(prow + half_idx * ATOM_BYTES + ch * 16) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        }
-        l_run += rs0 + rs1;
-        tc_fence_before();
-        fence_proxy_async_smem();
-        mbar_arrive(&p_full[qt * PB + (j % PB)]);
-      }
-      mbar_wait(&pv_done[qt * PB + ((n_tiles - 1) % PB)], ((n_tiles - 1) / PB) & 1);
-      tc_fence_after();
-      if constexpr (RS) {  // column HD of the accumulator = sum of the fp16-rounded P over all KV tiles
-        uint32_t lcol[16];
-        tmem_ld_x16(o_addr + HD, lcol);
-        tmem_ld_wait();
-        l_run = __uint_as_float(lcol[0]);
-      }
-      const float inv_l = 1.0f / l_run;
-      const int qrow = q0 + qt * BQ + row;
-      __half* dst = p.out + (static_cast<size_t>(batch) * p.Nq + qrow) * p.ldo + head * HD;
-#pragma unroll 1
-      for (int h = 0; h < HD / 32; ++h) {
-        uint32_t o[32];
-        tmem_ld_x32(o_addr + h * 32, o);
-        tmem_ld_wait();
-        if (qrow < p.Nq) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            uint4 w;
-            w.x = pack_half2(__uint_as_float(o[8 * i + 0]) * inv_l, __uint_as_float(o[8 * i + 1]) * inv_l);
-            w.y = pack_half2(__uint_as_float(o[8 * i + 2]) * inv_l, __uint_as_float(o[8 * i + 3]) * inv_l);
-            w.z = pack_half2(__uint_as_float(o[8 * i + 4]) * inv_l, __uint_as_float(o[8 * i + 5]) * inv_l);
-            w.w = pack_half2(__uint_as_float(o[8 * i + 6]) * inv_l, __uint_as_float(o[8 * i + 7]) * inv_l);
-            reinterpret_cast<uint4*>(dst + h * 32)[i] = w;
-          }
-        }
-      }
-    }
+    for (int a = 0; a < NA; ++a) tma_load_3d(sQ + a * ATOM_BYTES, &map_q, q_full, head * HD + a * 64, q0, batch);
+    load_kv(0);
+    if (n_tiles > 1) load_kv(1);
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+  const float c = p.scale_log2e;
+  // accumulator fragment (m16n8): o[n][0..1] = (row lane / 4, cols 8 n + 2 (lane % 4) + {0, 1}), o[n][2..3] = row + 8
+  float o[HD / 8][4];
+#pragma unroll
+  for (int n = 0; n < HD / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const uint32_t q_base = smem_u32(sQ);
+  const int qrow_ld = warp * 16 + (lane & 15);  // ldmatrix row of this lane for the A operand (Q)
+  mbar_wait(q_full, 0);
+
+  for (int j = 0; j < n_tiles; ++j) {
+    const int s = j & 1;
+    mbar_wait(&kv_full[s], (j >> 1) & 1);
+    const uint32_t k_base = smem_u32(sK + s * TILE_BYTES);
+    const uint32_t v_base = smem_u32(sV + s * TILE_BYTES);
+    // ---- S = Q K^T: 16 rows x 64 kv columns per warp ----
+    float sc[BKV / 8][4];
+#pragma unroll
+    for (int n = 0; n < BKV / 8; ++n) sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk) {
+      uint32_t a[4];
+      ldmatrix_x4(q_base + tile_off(qrow_ld, 2 * kk + (lane >> 4)), a[0], a[1], a[2], a[3]);
+#pragma unroll
+      for (int n2 = 0; n2 < BKV / 16; ++n2) {  // two 8-column n tiles per ldmatrix.x4
+        const int krow = n2 * 16 + (lane & 7) + ((lane >> 4) << 3);
+        uint32_t b0, b1, b2, b3;
+        ldmatrix_x4(k_base + tile_off(krow, 2 * kk + ((lane >> 3) & 1)), b0, b1, b2, b3);
+        mma_16816(sc[2 * n2], a, b0, b1);
+        mma_16816(sc[2 * n2 + 1], a, b2, b3);
+      }
+    }
+    // ---- online softmax (rows lane / 4 and lane / 4 + 8; the four lanes of a quad share a row) ----
+    const int valid = p.Nkv - j * BKV;  // columns >= valid are padding (last tile only)
+    if (valid < BKV) {
+#pragma unroll
+      for (int n = 0; n < BKV / 8; ++n) {
+        const int col = n * 8 + 2 * (lane & 3);
+        if (col >= valid) sc[n][0] = sc[n][2] = -INFINITY;
+        if (col + 1 >= valid) sc[n][1] = sc[n][3] = -INFINITY;
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int n = 0; n < BKV / 8; ++n) mx = fmaxf(mx, fmaxf(sc[n][2 * h], sc[n][2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx);  // finite: every tile holds at least one valid column
+      alpha[h] = fast_exp2((m_run[h] - m_new) * c);
+      m_run[h] = m_new;
+    }
+    float rs[2] = {0.f, 0.f};
+    uint32_t pa[BKV / 8][2];  // P rounded to fp16, packed pairs in the accumulator layout
+#pragma unroll
+    for (int n = 0; n < BKV / 8; ++n) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float mc = m_run[h] * c;
+        const float p0 = fast_exp2(sc[n][2 * h] * c - mc);
+        const float p1 = fast_exp2(sc[n][2 * h + 1] * c - mc);
+        rs[h] += p0 + p1;
+        pa[n][h] = pack_half2(p0, p1);
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + rs[h];  // per-lane partial; quad-reduced at the end
+#pragma unroll
+    for (int n = 0; n < HD / 8; ++n) {
+      o[n][0] *= alpha[0];
+      o[n][1] *= alpha[0];
+      o[n][2] *= alpha[1];
+      o[n][3] *= alpha[1];
+    }
+    // ---- O += P V: the m16n8 accumulators of kv columns [16 t, 16 t + 16) are the A fragment of k step t ----
+#pragma unroll
+    for (int t = 0; t < BKV / 16; ++t) {
+      const uint32_t a[4] = {pa[2 * t][0], pa[2 * t][1], pa[2 * t + 1][0], pa[2 * t + 1][1]};
+      const int vrow = t * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
+#pragma unroll
+      for (int d2 = 0; d2 < HD / 16; ++d2) {  // two 8-column d tiles per ldmatrix.x4.trans
+        uint32_t b0, b1, b2, b3;
+        ldmatrix_x4_trans(v_base + tile_off(vrow, 2 * d2 + (lane >> 4)), b0, b1, b2, b3);
+        mma_16816(o[2 * d2], a, b0, b1);
+        mma_16816(o[2 * d2 + 1], a, b2, b3);
+      }
+    }
+    __syncthreads();  // every warp is done with stage s
+    if (threadIdx.x == 0 && j + 2 < n_tiles) load_kv(j + 2);
+  }
+
+  float inv_l[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    inv_l[h] = 1.0f / l;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int qrow = q0 + warp * 16 + (lane >> 2) + 8 * h;
+    if (qrow >= p.Nq) continue;
+    __half* dst = p.out + (static_cast<size_t>(batch) * p.Nq + qrow) * p.ldo + head * HD + 2 * (lane & 3);
+#pragma unroll
+    for (int n = 0; n < HD / 8; ++n)
+      *reinterpret_cast<uint32_t*>(dst + n * 8) = pack_half2(o[n][2 * h] * inv_l[h], o[n][2 * h + 1] * inv_l[h]);
   }
 }
 
 CUtensorMap make_head_map(const __half* base, int ld, int B, int N, int cols) {
   uint64_t dims[3] = {(uint64_t)cols, (uint64_t)N, (uint64_t)B};
   uint64_t strides[2] = {(uint64_t)ld * 2, (uint64_t)N * ld * 2};
-  uint32_t box[3] = {64, 128, 1};
+  uint32_t box[3] = {64, 64, 1};
   return make_tmap_f16(base, 3, dims, strides, box);
 }
 
-template <int HD, int NQT, int KS, int POLY = 0, bool RS = false, int PB = 1>
+template <int HD>
 void configure_one() {
-  CFGPP_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<HD, NQT, KS, POLY, RS, PB>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        ACfg<HD, NQT, KS, RS, PB>::SMEM_BYTES));
+  CFGPP_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        ACfg<HD>::SMEM_BYTES));
 }
 
-template <int HD, int NQT, int KS, int POLY = 0, bool RS = false, int PB = 1>
+template <int HD>
 void launch(const AttnOp& op, cudaStream_t stream) {
-  dim3 grid((op.p.Nq + NQT * BQ - 1) / (NQT * BQ), op.p.H, op.p.B);
-  launch_pdl(attn_kernel<HD, NQT, KS, POLY, RS, PB>, grid, dim3(kThreads), ACfg<HD, NQT, KS, RS, PB>::SMEM_BYTES, stream,
-             op.p, op.map_q, op.map_k, op.map_v);
-}
-
-// CFGPP_ATTN_PBUF=2|1: double-buffered P (K / V ring of 2 instead of 3 to stay inside 227 KB) for head dim 64
-int attn_pbuf() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = std::getenv("CFGPP_ATTN_PBUF");
-    v = e ? atoi(e) : kDefaultPbuf;
-    if (v != 1 && v != 2) v = kDefaultPbuf;
-  }
-  return v;
-}
-
-// CFGPP_ATTN_ROWSUM_MMA=1|0: row sums from the tensor pipe (ones column appended to V) for head dim 64
-bool attn_rowsum_mma() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = std::getenv("CFGPP_ATTN_ROWSUM_MMA");
-    v = e ? (e[0] == '1' ? 1 : 0) : kDefaultRowsumMma;
-  }
-  return v == 1;
-}
-
-// fraction of the exponentials computed on the FMA pipe for head dim 64: CFGPP_ATTN_POLY = 0 (none), 8, 4 or 3 (every n-th)
-int attn_poly() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = std::getenv("CFGPP_ATTN_POLY");
-    v = e ? atoi(e) : kDefaultPoly;
-    if (v != 0 && v != 8 && v != 4 && v != 3) v = kDefaultPoly;
-  }
-  return v;
+  dim3 grid((op.p.Nq + BQ - 1) / BQ, op.p.H, op.p.B);
+  launch_pdl(attn_kernel<HD>, grid, dim3(kThreads), ACfg<HD>::SMEM_BYTES, stream, op.p, op.map_q, op.map_k, op.map_v);
 }
 
 }  // namespace
@@ -458,50 +246,18 @@ AttnOp make_attn_op(const __half* q, int ldq, const __half* k, int ldk, const __
 void attn_configure() {
   static bool done = false;
   if (done) return;
-  configure_one<64, 2, 3>();
-  configure_one<64, 2, 3, 8>();
-  configure_one<64, 2, 3, 4>();
-  configure_one<64, 2, 3, 3>();
-  configure_one<64, 2, 3, 0, true>();
-  configure_one<64, 2, 2, 0, false, 2>();
-  configure_one<128, 1, 2>();
-  configure_one<192, 1, 1>();
-  xattn_configure();
-  attn_persist_configure();
+  configure_one<64>();
+  configure_one<128>();
+  configure_one<192>();
   done = true;
 }
 
 void run_attn_op(const AttnOp& op, cudaStream_t stream) {
   attn_configure();
-  // Nkv <= 128 (the 77 text tokens): K / V resident, query tiles streamed (attention_cross.cu). CFGPP_NO_XATTN=1 keeps
-  // the general flash kernel for A/B runs.
-  static const bool no_x = [] {
-    const char* e = std::getenv("CFGPP_NO_XATTN");
-    return e != nullptr && e[0] == '1';
-  }();
-  if (!no_x && xattn_applicable(op)) return run_xattn_op(op, stream);
-  // Persistent variant (attention_persist.cu: one CTA per SM, balanced tile ranges, two independent pipelines):
-  // correct (the attention tests also run with it) but measured SLOWER than the pair-per-CTA grid on B200 — 54.6 vs
-  // 49.4 us at N = 1024 x 20 heads x 4, 321 vs 274 us at N = 4096 x 10 x 4: what the even tile split saves, the
-  // un-shared K / V fetches and the lock-step of the two pipelines lose again — so it is opt-in (CFGPP_PATTN=1).
-  static const bool use_p = [] {
-    const char* e = std::getenv("CFGPP_PATTN");
-    return e != nullptr && e[0] == '1';
-  }();
-  if (use_p && attn_persist_applicable(op)) return run_attn_persist_op(op, stream);
-  attn_configure();
   switch (op.hd_pad) {
-    case 64:
-      if (attn_pbuf() == 2) return launch<64, 2, 2, 0, false, 2>(op, stream);
-      if (attn_rowsum_mma()) return launch<64, 2, 3, 0, true>(op, stream);
-      switch (attn_poly()) {
-        case 8: return launch<64, 2, 3, 8>(op, stream);
-        case 4: return launch<64, 2, 3, 4>(op, stream);
-        case 3: return launch<64, 2, 3, 3>(op, stream);
-        default: return launch<64, 2, 3>(op, stream);
-      }
-    case 128: return launch<128, 1, 2>(op, stream);
-    case 192: return launch<192, 1, 1>(op, stream);
+    case 64: return launch<64>(op, stream);
+    case 128: return launch<128>(op, stream);
+    case 192: return launch<192>(op, stream);
     default: throw Error(-1, "unsupported padded head dim");
   }
 }

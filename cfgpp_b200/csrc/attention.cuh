@@ -1,4 +1,4 @@
-// cfgpp_b200 — fused scaled-dot-product attention (no mask, no dropout) on tcgen05.
+// cfgpp_b200 — fused scaled-dot-product attention (no mask, no dropout) on the sm_90a tensor cores.
 //   out[b, i, h*P + :] = softmax(q_i k^T / sqrt(d)) v           (AttnProcessor2_0 / F.scaled_dot_product_attention)
 // d = real head dim (SDXL: 64; SD v1.5: 40 / 80 / 160), P = d rounded up to a multiple of 64: the projections that
 // feed this kernel emit each head zero-padded to P columns (and to_out ignores the padded columns), so every tile is

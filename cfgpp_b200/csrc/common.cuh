@@ -1,4 +1,4 @@
-// cfgpp_b200 — shared device-side PTX wrappers for sm_100a (tcgen05 / TMEM / TMA / mbarrier).
+// cfgpp_b200 — shared device-side PTX wrappers for sm_90a (wgmma / mma.sync / TMA / mbarrier).
 // Everything here is raw inline PTX; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
@@ -18,7 +18,7 @@ CFGPP_DEVICE uint32_t smem_u32(const void* p) {
 // ----------------------------------------------------------------------------------------------
 // programmatic dependent launch (PDL): every kernel of the step is launched with the programmatic-stream-
 // serialization attribute. pdl_launch_dependents() lets the next kernel's CTAs start (and run their prologue:
-// barrier init, TMEM alloc, descriptor prefetch) as soon as SM resources free up; pdl_wait() blocks until the
+// barrier init, descriptor prefetch) as soon as SM resources free up; pdl_wait() blocks until the
 // preceding kernel has fully completed and its writes are visible — it must precede the first global access.
 // ----------------------------------------------------------------------------------------------
 CFGPP_DEVICE void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -58,7 +58,7 @@ CFGPP_DEVICE uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity) {
 #define CFGPP_MBAR_SLEEP_NS 1000000
 #endif
 // Probe with a suspend-time hint: the thread may sleep in hardware for up to ~1 ms waiting for the phase, instead
-// of spinning through the issue stage (the epilogue warps of an SM wait for a whole main loop on tmem_full).
+// of spinning through the issue stage (a consumer may wait for a whole main loop of TMA loads).
 CFGPP_DEVICE uint32_t mbar_try_wait_sleep(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -87,6 +87,16 @@ CFGPP_DEVICE void mbar_wait(uint64_t* bar, uint32_t parity) {
              smem_u32(bar), parity);
       __trap();
     }
+  }
+}
+
+// The same wait with the same time-out, but trapping without the printf report: any function call (printf) in a kernel
+// that issues wgmma makes ptxas serialise every wgmma of that kernel.
+CFGPP_DEVICE void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > 4000000000LL) __trap();
   }
 }
 
@@ -132,209 +142,122 @@ CFGPP_DEVICE void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// ---- thread-block clusters ----
-CFGPP_DEVICE uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-CFGPP_DEVICE void cluster_sync_all() {  // all threads of all CTAs in the cluster
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// ---- cta_group::2 (CTA pair) variants -------------------------------------------------------------------------
-// In a pair the even CTA (cluster rank 0) is the leader: it alone issues tcgen05.mma.cta_group::2, which reads A / B
-// from BOTH CTAs' shared memory (same offsets) and writes each CTA's half of the 256-row accumulator into that CTA's
-// TMEM. Clearing bit 24 of a shared::cluster address gives the same offset in the leader CTA.
-constexpr uint32_t kLeaderMask = 0xFEFFFFFFu;
-
-CFGPP_DEVICE void tmem_alloc_cg2(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-CFGPP_DEVICE void tmem_relinquish_cg2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-CFGPP_DEVICE void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA load into this CTA's shared memory, completion signalled on the LEADER CTA's mbarrier (same offset)
-CFGPP_DEVICE void tma_load_2d_cg2(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & kLeaderMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-CFGPP_DEVICE void tma_load_4d_cg2(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
-                                  int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-      "%5, %6}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & kLeaderMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-CFGPP_DEVICE void umma_f16_cg2(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit of the pair's MMAs, arriving on the mbarrier at this offset in both CTAs
-CFGPP_DEVICE void umma_commit_cg2(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-// arrive on the leader CTA's copy of a barrier (works from either CTA of the pair)
-CFGPP_DEVICE void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kLeaderMask)
-               : "memory");
-}
-
-// generic-proxy smem writes -> visible to the async proxy (UMMA / TMA reads)
+// generic-proxy smem writes -> visible to the async proxy (wgmma / TMA reads)
 CFGPP_DEVICE void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM alloc, MMA, commit, ld
+// warpgroup register reallocation (setmaxnreg): the producer warpgroup gives registers back so the two MMA / epilogue
+// warpgroups can hold a 64 x 256 fp32 accumulator each. Executed by all warps of a warpgroup.
 // ----------------------------------------------------------------------------------------------
-CFGPP_DEVICE void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // whole warp, .sync.aligned
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-CFGPP_DEVICE void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-CFGPP_DEVICE void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-CFGPP_DEVICE void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-// One lane of a fully converged warp (elect.sync). Roles that issue TMA / tcgen05 instructions run their loops with the
-// WHOLE warp and predicate only the issue itself on this: the loop state then stays provably warp-uniform, so the
-// compiler keeps descriptors / coordinates in uniform registers instead of wrapping every UTCHMMA / UTMALDG in an
-// ELECT + R2UR + BRA.U.ANY "waterfall" loop (which made the single-thread MMA issuer the bottleneck of the main loop).
-CFGPP_DEVICE bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t"
-      "}"
-      : "=r"(pred));
-  return pred != 0;
-}
-
-CFGPP_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], fp16/bf16 inputs, fp32 accumulate. One thread issues.
-CFGPP_DEVICE void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same with the A operand in TENSOR MEMORY (K-major fp16: lane = row, one 32-bit column = two consecutive K elements,
-// a K = 16 instruction reads 8 columns - verified by tools/bringup/tmem_a_mma.cu).
-CFGPP_DEVICE void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-CFGPP_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 bit, N consecutive columns; thread i of the warp reads lane (base + i).
-CFGPP_DEVICE void tmem_ld_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-CFGPP_DEVICE void tmem_ld_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-CFGPP_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM (32 lanes x 32 consecutive columns)
-CFGPP_DEVICE void tmem_st_x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-CFGPP_DEVICE void tmem_st_x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-CFGPP_DEVICE void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+template <uint32_t N>
+CFGPP_DEVICE void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+CFGPP_DEVICE void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ----------------------------------------------------------------------------------------------
-// UMMA descriptors (see PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor")
+// wgmma (sm_90a warpgroup MMA): D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 in, fp32 accumulate in registers.
+// Both operands come from shared memory through matrix descriptors (K-major, 128B swizzle).
 // ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128B swizzle, K-major operand whose K extent per tile row is exactly
+CFGPP_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+CFGPP_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+CFGPP_DEVICE void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+template <int N>
+CFGPP_DEVICE void fence_acc(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// Shared-memory matrix descriptor (sm_90 wgmma), 128B swizzle, K-major operand whose K extent per tile row is exactly
 // one 128-byte swizzle atom (64 fp16). Rows are 128 B apart; 8-row groups are 1024 B apart (SBO).
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (unused here)
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1 (sm_100)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
-CFGPP_DEVICE uint64_t make_sdesc_sw128(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t lbo_bytes) {
+//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1)
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout type: 1 = SWIZZLE_128B
+// Advancing 16 fp16 (32 B) along K inside the atom is +2 in the start-address field.
+CFGPP_DEVICE uint64_t make_wgmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Instruction descriptor for kind::f16: fp16 A/B (format 0), fp32 accumulate (c_format 1).
-//   bit 15: A major (0 = K-major, 1 = MN-major)   bit 16: B major
-//   bits [17,23): N >> 3                           bits [24,29): M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                      uint32_t b_mn_major) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
+// D[64 x N] (+)= A * B^T from two smem descriptors; scale_d = 0 overwrites D. One instruction per N (inline asm needs
+// literal operand lists), for the tile widths the GEMM instantiates.
+#define CFGPP_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
+                    "+f"(d[i + 6]), "+f"(d[i + 7])
+template <int N>
+CFGPP_DEVICE void wgmma_f16(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d);
+template <>
+CFGPP_DEVICE void wgmma_f16<64>(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\nwgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+               "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,"
+               "%27,%28,%29,%30,%31"
+               "}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+               : CFGPP_D8(0), CFGPP_D8(8), CFGPP_D8(16), CFGPP_D8(24)
+               : "l"(a_desc), "l"(b_desc), "r"(scale_d)
+               : "memory");
+}
+template <>
+CFGPP_DEVICE void wgmma_f16<128>(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\nwgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+               "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,"
+               "%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,"
+               "%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+               "}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+               : CFGPP_D8(0), CFGPP_D8(8), CFGPP_D8(16), CFGPP_D8(24), CFGPP_D8(32), CFGPP_D8(40), CFGPP_D8(48), CFGPP_D8(56)
+               : "l"(a_desc), "l"(b_desc), "r"(scale_d)
+               : "memory");
+}
+template <>
+CFGPP_DEVICE void wgmma_f16<160>(float (&d)[80], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %82, 0;\nwgmma.mma_async.sync.aligned.m64n160k16.f32.f16.f16 {"
+               "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,"
+               "%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,"
+               "%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,"
+               "%77,%78,%79"
+               "}, %80, %81, p, 1, 1, 0, 0;\n}\n"
+               : CFGPP_D8(0), CFGPP_D8(8), CFGPP_D8(16), CFGPP_D8(24), CFGPP_D8(32), CFGPP_D8(40), CFGPP_D8(48), CFGPP_D8(56), CFGPP_D8(64), CFGPP_D8(72)
+               : "l"(a_desc), "l"(b_desc), "r"(scale_d)
+               : "memory");
+}
+template <>
+CFGPP_DEVICE void wgmma_f16<256>(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\nwgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
+               "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,"
+               "%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,"
+               "%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,"
+               "%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,"
+               "%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,"
+               "%121,%122,%123,%124,%125,%126,%127"
+               "}, %128, %129, p, 1, 1, 0, 0;\n}\n"
+               : CFGPP_D8(0), CFGPP_D8(8), CFGPP_D8(16), CFGPP_D8(24), CFGPP_D8(32), CFGPP_D8(40), CFGPP_D8(48), CFGPP_D8(56), CFGPP_D8(64), CFGPP_D8(72), CFGPP_D8(80), CFGPP_D8(88), CFGPP_D8(96), CFGPP_D8(104), CFGPP_D8(112), CFGPP_D8(120)
+               : "l"(a_desc), "l"(b_desc), "r"(scale_d)
+               : "memory");
+}
+#undef CFGPP_D8
+
+// ----------------------------------------------------------------------------------------------
+// warp-level tensor-core MMA (mma.sync m16n8k16) and ldmatrix, used by the attention kernel
+// ----------------------------------------------------------------------------------------------
+CFGPP_DEVICE void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr));
+}
+CFGPP_DEVICE void ldmatrix_x4_trans(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr));
+}
+// D (fp32, 16 x 8) += A (fp16, 16 x 16, row) * B (fp16, 16 x 8, col)
+CFGPP_DEVICE void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -372,27 +295,6 @@ CFGPP_DEVICE float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-// 2^x on the FMA / ALU pipes (no MUFU): round-to-nearest split x = n + r, r in [-0.5, 0.5], degree-3 minimax polynomial
-// for 2^r (max relative error 7.5e-5, a sixth of an fp16 ulp), n added into the exponent field. Valid for x <= ~100;
-// x below -126 (incl. -inf from masking) flushes to ~1e-38. Used for a fraction of the softmax exponentials: the
-// attention kernels are bound by the 16 ex2 / clk / SM of the MUFU pipe, not by the tensor pipe (FA4's trick).
-CFGPP_DEVICE float exp2_poly(float x) {
-  x = fmaxf(x, -126.0f);
-  const float t = x + 12582912.0f;  // 1.5 * 2^23: the integer nearest to x lands in the low mantissa bits
-  const float r = x - (t - 12582912.0f);
-  float p = 0.0551716648042202f;
-  p = fmaf(p, r, 0.2426111251115799f);
-  p = fmaf(p, r, 0.6932609677314758f);
-  p = fmaf(p, r, 0.9999280571937561f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
-}
-// three-input maximum (FMNMX3 on sm_100)
-CFGPP_DEVICE float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
 }
 
 CFGPP_DEVICE uint32_t pack_half2(float a, float b) {

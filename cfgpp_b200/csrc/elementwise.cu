@@ -495,7 +495,7 @@ void run_step_only(const __half* eps_uc, const __half* eps_c, int n, int mode, c
 void run_upsample2x(const __half* x, __half* out, int B, int H, int W, int C, cudaStream_t stream) {
   CFGPP_REQUIRE(C % 8 == 0, "upsample C % 8");
   const size_t total = static_cast<size_t>(B) * 4 * H * W * (C / 8);
-  const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 148 * 16));
+  const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, num_sms() * 16));
   launch_pdl(upsample2x_kernel, dim3(blocks), dim3(256), 0, stream, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(out), B, H,
                                                 W, C / 8);
 }
@@ -503,7 +503,7 @@ void run_upsample2x(const __half* x, __half* out, int B, int H, int W, int C, cu
 void run_im2col_s2(const __half* x, __half* out, int B, int H, int W, int C, cudaStream_t stream) {
   CFGPP_REQUIRE(C % 8 == 0 && H % 2 == 0 && W % 2 == 0, "im2col_s2 shape");
   const size_t total = static_cast<size_t>(B) * (H / 2) * (W / 2) * 9 * (C / 8);
-  const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 148 * 16));
+  const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, num_sms() * 16));
   launch_pdl(im2col_s2_kernel, dim3(blocks), dim3(256), 0, stream, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(out), B, H,
                                                W, C / 8);
 }

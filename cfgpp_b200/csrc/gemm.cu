@@ -1,26 +1,20 @@
-// cfgpp_b200 — persistent, warp-specialised tcgen05 GEMM / implicit-GEMM conv3x3 kernel for sm_100a.
-// See gemm.cuh for the operator contract. Structure per CTA (384 threads, 1 CTA / SM, persistent over tiles):
-//   warps 0..7 : epilogue      (tcgen05.ld 32x32b -> bias/addend/GEGLU/LN-fold -> fp16 smem staging -> TMA store; warp w
-//                               owns TMEM lane quarter w % 4 and the 32-column chunks of parity w / 4, end to end)
-//   warp 8     : TMA producer  (A tile 128x64, B tile BNx64 per stage, 128B swizzle, mbarrier complete_tx)
-//   warp 9     : MMA issuer    (tcgen05.mma kind::f16, M=128 (256 for a CTA pair), N=BN, K=16 x4 per stage)
-//   warp 10    : TMEM allocator
-// The producer and issuer warps run their loops warp-wide and issue from one elected lane (see elect_one()).
-// Pipelines: smem ring full/empty (TMA <-> MMA) and a 2-deep TMEM accumulator ring full/empty (MMA <-> epilogue),
-// so the epilogue of tile i overlaps the main loop of tile i+1.
+// cfgpp_b200 — persistent, warp-specialised wgmma GEMM / implicit-GEMM conv3x3 kernel for sm_90a.
+// See gemm.cuh for the operator contract. Structure per CTA (384 threads = 3 warpgroups, 1 CTA / SM, persistent over
+// tiles):
+//   warpgroups 0, 1 : MMA + epilogue. Warpgroup g owns rows [64 g, 64 g + 64) of the 128 x BN tile: wgmma m64nBNk16
+//                     from the shared-memory ring into a register accumulator, then bias / addend / GEGLU / LN-fold ->
+//                     fp16 into a swizzled smem staging tile -> TMA store. Warp w of the group owns 16 rows end to end.
+//   warp 8          : TMA producer (A tile 128x64, B tile BNx64 per stage, 128B swizzle, mbarrier complete_tx); the
+//                     rest of warpgroup 2 idles. The producer warpgroup hands registers to the MMA warpgroups
+//                     (setmaxnreg), which hold up to 128 fp32 accumulator registers per thread.
+// Pipeline: smem ring full/empty (TMA <-> MMA); the producer runs ahead into the next tile while the epilogue of the
+// current one runs.
 #include <algorithm>
 #include <cstdlib>
 #include <type_traits>
 
 #include "common.cuh"
 #include "gemm.cuh"
-
-#ifdef CFGPP_DIAG_NOTMA  // diagnostic build: operand (and residual) loads disappear; use on ops without a residual
-#define tma_load_2d(...) ((void)0)
-#define tma_load_4d(...) ((void)0)
-#define tma_load_2d_cg2(...) ((void)0)
-#define tma_load_4d_cg2(...) ((void)0)
-#endif
 
 namespace cfgpp {
 
@@ -31,52 +25,37 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int kThreads = 384;
-// Warp roles. Eight epilogue warps: warp w owns TMEM lane quarter w % 4 (rows 32*(w%4) .. +31 of the tile) and the
-// 32-column chunks j with j % 2 == w / 4, so every SM sub-partition hosts two epilogue warps that hide each other's
-// tcgen05.ld / shared-memory latencies. The two issue warps sit above them (the sub-partition arbiter serves the
-// highest warp id first; they sleep on mbarriers most of the time).
-constexpr int kEpiWarps = 8;      // warps 0..7
+constexpr int kEpiWarps = 8;      // warps 0..7: MMA + epilogue (warpgroups 0 and 1)
 constexpr int kProducerWarp = 8;
-constexpr int kMmaWarp = 9;
-constexpr int kAllocWarp = 10;
 constexpr int A_BYTES = BM * BK * 2;
-constexpr int kSkMaxClusters = 256;            // stream-K: flags[c] arrivals, flags[kSkDoneOffset + c] consumers
-constexpr int kSkDoneOffset = kSkMaxClusters;
+constexpr int kSkMaxCtas = 256;            // stream-K: flags[c] arrivals, flags[kSkDoneOffset + c] consumers
+constexpr int kSkDoneOffset = kSkMaxCtas;
 
-template <int BN, bool GEGLU, int CL = 1>
+template <int BN, bool GEGLU>
 struct Cfg {
-  static constexpr int B_BYTES = (BN / CL) * BK * 2;  // per CTA: a CTA pair (CL = 2) holds half of the B tile each
+  static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   // output columns of a tile and its smem staging area: OUT_N / 32 sub-tiles of [128 rows x 64 B], 64B swizzle
   static constexpr int OUT_N = GEGLU ? BN / 2 : BN;
   static constexpr int EPI_SUB = OUT_N / 32;
   static constexpr int EPI_SUB_BYTES = BM * 64;
   static constexpr int EPI_BYTES = EPI_SUB * EPI_SUB_BYTES;
-  static constexpr int STAGES =
-      CL == 2 ? (GEGLU ? 5 : (BN == 256 ? 4 : 6)) : (GEGLU ? 3 : (BN == 256 ? 3 : (BN == 160 ? 4 : 5)));
-  static constexpr int TMEM_COLS = (BN <= 64) ? 128 : (BN <= 128 ? 256 : 512);
-  static constexpr int ACC_STRIDE = TMEM_COLS / 2;
+  static constexpr int STAGES = GEGLU ? 3 : (BN == 256 ? 3 : (BN == 160 ? 4 : 5));
   // per-tile vectors staged for the epilogue: bias + time-embedding row (fp16), LayerNorm-fold s_n / t_n (fp32)
   static constexpr int VEC_ONE = 2 * 256 * 2 + 2 * 256 * 4;
   static constexpr int VEC_BYTES = 2 * VEC_ONE;  // double-buffered by tile parity
   static constexpr int SMEM_BYTES =
       STAGES * STAGE_BYTES + EPI_BYTES + VEC_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB shared memory of an SM");
+  static constexpr int ACC = BN / 2;  // fp32 accumulator registers per thread (m64 x BN over 128 threads)
 };
 
-// CL = 1: one CTA per 128 x BN tile (tcgen05.mma.cta_group::1).
-// CL = 2: a CTA pair (cluster of 2 on one TPC) computes a 256 x BN tile with tcgen05.mma.cta_group::2: each CTA
-//         loads its own 128 rows of A and only HALF of the B (weight) tile; the leader's MMA reads both halves
-//         through the pair's shared memory. Per-SM ingest from L2 (64 B/clk/SM, the measured bound of the 128 x 160
-//         tiles: ~13 TB/s aggregate => ~800 TFLOP/s at 71 FLOP/B) drops from (128 + BN) to (128 + BN/2) rows per
-//         k-block. (A plain TMA-multicast of B inside the cluster was tried first and does not help: every SM still
-//         ingests the full tile.)
-template <int BN, bool GEGLU, int CL>
+template <int BN, bool GEGLU>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_a2,
             const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_out,
             const __grid_constant__ CUtensorMap map_res) {
-  using C = Cfg<BN, GEGLU, CL>;
+  using C = Cfg<BN, GEGLU>;
   extern __shared__ uint8_t smem_raw[];
   // 1024B alignment (required by the 128B swizzle atoms) in the shared address space
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -87,21 +66,15 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
   uint64_t* bars = reinterpret_cast<uint64_t*>(epi_smem + C::EPI_BYTES + C::VEC_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + C::STAGES;
-  uint64_t* tmem_full_bar = bars + 2 * C::STAGES;
-  uint64_t* tmem_empty_bar = bars + 2 * C::STAGES + 2;
-  uint64_t* res_bar = bars + 2 * C::STAGES + 4;  // [kEpiWarps]: each epilogue warp loads its own residual sub-blocks
-  uint64_t* sk_pre_bar = bars + 2 * C::STAGES + 4 + kEpiWarps;  // stream-K: the finishing piece's accumulator is preloaded
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * C::STAGES + 4 + kEpiWarps + 1);
+  uint64_t* res_bar = bars + 2 * C::STAGES;  // [kEpiWarps]: each epilogue warp loads its own residual sub-blocks
 
   const int warp_idx = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);  // provably warp-uniform
   const int lane = threadIdx.x & 31;
   unsigned long long* tl = p.timeline ? p.timeline + static_cast<size_t>(blockIdx.x) * 16 : nullptr;
 #define TL(slot) do { if (tl) tl[slot] = globaltimer_ns(); } while (0)
   if (threadIdx.x == 0) TL(0);
-  const int cta_rank = (CL > 1) ? __shfl_sync(0xffffffffu, static_cast<int>(cluster_ctarank()), 0) : 0;
-  const int cluster_id = blockIdx.x / CL;
-  const int num_clusters = gridDim.x / CL;
-  const bool is_leader_cta = (cta_rank == 0);
+  const int cta_id = blockIdx.x;
+  const int num_ctas = gridDim.x;
 
   if (warp_idx == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&map_a);
@@ -109,78 +82,52 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
     tma_prefetch_desc(&map_b);
     tma_prefetch_desc(&map_out);
     tma_prefetch_desc(&map_res);
-  }
-  if (warp_idx == kMmaWarp && lane == 0) {
     for (int i = 0; i < C::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], CL * kEpiWarps);  // one elected arrive per epilogue warp (pair: of both CTAs)
+      mbar_init(&empty_bar[i], kEpiWarps);  // one arrive per consumer warp once its wgmmas on the stage retired
     }
     for (int i = 0; i < kEpiWarps; ++i) mbar_init(&res_bar[i], 1);
-    mbar_init(sk_pre_bar, CL * kEpiWarps);
     fence_barrier_init();
   }
-  if constexpr (CL > 1) cluster_sync_all();  // both CTAs resident before the pair-wide TMEM allocation
-  if (warp_idx == kAllocWarp) {
-    if constexpr (CL == 2) {
-      tmem_alloc_cg2(tmem_ptr_smem, C::TMEM_COLS);
-      tmem_relinquish_cg2();
-    } else {
-      tmem_alloc(tmem_ptr_smem, C::TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CL > 1) cluster_sync_all();  // peer barriers are initialised before any remote arrive / TMA signal
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_ptr_smem, 0);
-  if (threadIdx.x == 0) TL(1);
   pdl_launch_dependents();  // the next kernel may start its prologue on SMs this grid leaves
   pdl_wait();               // everything above overlapped the previous kernel's tail; its outputs are needed below
   if (threadIdx.x == 0) TL(2);
 
-  // tiles are enumerated as (m-group, n) with CL vertically adjacent M blocks per group; a cluster walks the groups,
-  // CTA `cta_rank` takes M block  group * CL + cta_rank  (possibly a phantom block past M: loads zero-fill, stores clip)
-  const int num_mg = (p.num_m_blocks + CL - 1) / CL;
-  const int num_tiles = num_mg * p.num_n_blocks;
+  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
   const int nkb = p.num_k_blocks;
-  auto tile_m_blk = [&](int tile) { return (p.raster ? tile / p.num_n_blocks : tile % num_mg) * CL + cta_rank; };
-  auto tile_n_blk = [&](int tile) { return p.raster ? tile % p.num_n_blocks : tile / num_mg; };
+  auto tile_m_blk = [&](int tile) { return p.raster ? tile / p.num_n_blocks : tile % p.num_m_blocks; };
+  auto tile_n_blk = [&](int tile) { return p.raster ? tile % p.num_n_blocks : tile / p.num_m_blocks; };
 
   // ---- work schedule: "stream-K for the remainder" -------------------------------------------------------------
-  // D = the tiles that fill whole rounds over the clusters are walked data-parallel (tile = cluster + r * clusters);
-  // the R = T mod clusters left-over tiles would cost a full extra round with most clusters idle, so their
-  // R * nkb k-blocks are split evenly over ALL clusters instead: cluster c owns the contiguous unit range
-  // [c U / P, (c + 1) U / P) of the linearised (tile, k-block) space — at most two pieces, of two adjacent tiles. The
-  // piece that contains a tile's LAST k-block finishes the tile: the fp32 partial accumulators the other pieces
-  // parked in the workspace are summed in a fixed order (deterministic) and preloaded into its TMEM accumulator, its
-  // MMAs accumulate on top and the normal epilogue follows. All clusters of the grid are co-resident (grid <= SMs,
-  // one CTA per SM; a dependent grid is only scheduled after every CTA of this one has started), so the spin-wait
-  // on a peer's flag cannot deadlock; a waits-for edge always points at a lower cluster's FIRST item.
+  // D = the tiles that fill whole rounds over the CTAs are walked data-parallel (tile = cta + r * ctas); the
+  // R = T mod ctas left-over tiles would cost a full extra round with most CTAs idle, so their R * nkb k-blocks are
+  // split evenly over ALL CTAs instead: CTA c owns the contiguous unit range [c U / P, (c + 1) U / P) of the linearised
+  // (tile, k-block) space — at most two pieces, of two adjacent tiles. The piece that contains a tile's LAST k-block
+  // finishes the tile: the fp32 partial accumulators the other pieces parked in the workspace are summed in a fixed
+  // order (deterministic) into its register accumulator before its main loop, and the normal epilogue follows. All
+  // CTAs of the grid are co-resident (grid <= SMs, one CTA per SM; a dependent grid is only scheduled after every CTA
+  // of this one has started), so the spin-wait on a peer's flag cannot deadlock; a waits-for edge always points at a
+  // lower CTA's FIRST item.
   constexpr int kItemFull = 0, kItemPart = 1, kItemFin = 2;
   struct Item {
     int tile, kb0, kb1, kind, c_first;
   };
   int sk_r = 0;  // R
   long sk_units = 0;
-  if (p.sk_ws != nullptr && num_tiles % num_clusters != 0) {
-    sk_r = num_tiles % num_clusters;
+  if (p.sk_ws != nullptr && num_tiles % num_ctas != 0) {
+    sk_r = num_tiles % num_ctas;
     sk_units = static_cast<long>(sk_r) * nkb;
   }
   const int dp_tiles = num_tiles - sk_r;
-  auto sk_u0 = [&](int c) { return static_cast<int>(sk_units * c / num_clusters); };
-  // A cluster's stream-K share is at most one non-finishing piece (`sk_first`, walked FIRST so that its partial is
+  auto sk_u0 = [&](int c) { return static_cast<int>(sk_units * c / num_ctas); };
+  // A CTA's stream-K share is at most one non-finishing piece (`sk_first`, walked FIRST so that its partial is
   // published while everybody still has main-loop work) and at most one finishing piece (`sk_late`, walked just
-  // before the last data-parallel tile — or last when there is only one — so that the flag wait is never exposed,
-  // the heavier fix-up epilogue overlaps a main loop, and the accumulator stage of the parked piece is long free).
+  // before the last data-parallel tile — or last when there is only one — so that the flag wait is rarely exposed).
   Item sk_first{}, sk_late{};
   int n_first = 0, n_late = 0;
   if (sk_r > 0) {
-    const int u0 = sk_u0(cluster_id), u1 = sk_u0(cluster_id + 1);
+    const int u0 = sk_u0(cta_id), u1 = sk_u0(cta_id + 1);
     if (u1 > u0) {
       const int s0 = u0 / nkb;
       const int e0 = (u1 < (s0 + 1) * nkb) ? u1 : (s0 + 1) * nkb;
@@ -189,15 +136,15 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
         it.tile = dp_tiles + s;
         it.kb0 = b - s * nkb;
         it.kb1 = e - s * nkb;
-        it.c_first = cluster_id;
+        it.c_first = cta_id;
         if (it.kb1 < nkb) {
           it.kind = kItemPart;
         } else if (it.kb0 == 0) {
           it.kind = kItemFull;
         } else {
           it.kind = kItemFin;
-          int c = cluster_id;
-          while (c > 0 && sk_u0(c) > s * nkb) --c;  // the cluster whose range holds the tile's first k-block
+          int c = cta_id;
+          while (c > 0 && sk_u0(c) > s * nkb) --c;  // the CTA whose range holds the tile's first k-block
           it.c_first = c;
         }
         return it;
@@ -216,27 +163,28 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
       }
     }
   }
-  const int n_dp = (dp_tiles > cluster_id) ? (dp_tiles - cluster_id + num_clusters - 1) / num_clusters : 0;
+  const int n_dp = (dp_tiles > cta_id) ? (dp_tiles - cta_id + num_ctas - 1) / num_ctas : 0;
   const int n_items = n_first + n_late + n_dp;
   const int late_pos = n_first + (n_dp >= 2 ? n_dp - 1 : n_dp);
   auto item_at = [&](int i) {
     if (i < n_first) return sk_first;
     if (n_late && i == late_pos) return sk_late;
     Item it;
-    it.tile = cluster_id + (i - n_first - ((n_late && i > late_pos) ? 1 : 0)) * num_clusters;
+    it.tile = cta_id + (i - n_first - ((n_late && i > late_pos) ? 1 : 0)) * num_ctas;
     it.kb0 = 0;
     it.kb1 = nkb;
     it.kind = kItemFull;
-    it.c_first = cluster_id;
+    it.c_first = cta_id;
     return it;
   };
-  constexpr unsigned kSkArrivals = CL * kEpiWarps;  // warps that publish / consume one cluster's partial
-  // partial accumulator of (cluster c, CTA rank r): [BN / 32 column chunks][4 lane quarters][8][32 lanes] float4
-  auto sk_ws = [&](int c) { return p.sk_ws + (static_cast<size_t>(c) * CL + cta_rank) * (static_cast<size_t>(BM) * BN); };
+  constexpr unsigned kSkArrivals = kEpiWarps;  // warps that publish / consume one CTA's partial
+  // partial accumulator of CTA c: [BN / 4 register pairs][256 consumer threads] float2 (the register fragment order)
+  auto sk_ws = [&](int c) { return p.sk_ws + static_cast<size_t>(c) * (static_cast<size_t>(BM) * BN); };
 
-  if (warp_idx == kProducerWarp) {
-    {
-      // ===================== TMA producer (whole warp walks the loop, one elected lane issues) ============
+  if (warp_idx >= kEpiWarps) {
+    setmaxnreg_dec<40>();
+    if (warp_idx == kProducerWarp && lane == 0) {
+      // ===================== TMA producer =====================
       int stage = 0;
       uint32_t phase = 0;
       for (int item_i = 0; item_i < n_items; ++item_i) {
@@ -254,67 +202,24 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
           w0 = r - h0 * p.W;
         }
         for (int kb = item.kb0; kb < item.kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * C::STAGE_BYTES;
           uint8_t* sb = sa + A_BYTES;
-          if (!elect_one()) {
-            // non-elected lanes only keep the loop state in step
-          } else if constexpr (CL == 1) {
-            if (item_i == 0 && kb == item.kb0) TL(3);
-#ifdef CFGPP_DIAG_HALFA  // diagnostic build: A arrives on even k-blocks only (the ingest of a tile twice as wide)
-            const bool load_a = !(kb & 1);
-#else
-            const bool load_a = true;
-#endif
-#ifdef CFGPP_DIAG_NOTMA  // diagnostic build (tools/build_variant.sh): no operand traffic, the MMAs run on stale smem
-            mbar_arrive(&full_bar[stage]);
-#else
-            mbar_arrive_expect_tx(&full_bar[stage], load_a ? C::STAGE_BYTES : C::B_BYTES);
-#endif
-            if (!load_a) {
-            } else if (p.conv) {
-              const int tap = kb / p.cpb;
-              const int cb = kb - tap * p.cpb;
-              const int kh = tap / 3, kw = tap - kh * 3;
-              tma_load_4d(sa, &map_a, &full_bar[stage], cb * BK, w0 * p.conv_stride + kw - p.conv_pad, h0 * p.conv_stride + kh - p.conv_pad,
-                          img);
-            } else {
-              const int k0 = kb * BK;
-              if (k0 < p.k_split)
-                tma_load_2d(sa, &map_a, &full_bar[stage], k0, m0);
-              else
-                tma_load_2d(sa, &map_a2, &full_bar[stage], k0 - p.k_split, m0);
-            }
-            tma_load_2d(sb, &map_b, &full_bar[stage], kb * BK, n_blk * BN);
+          mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
+          if (p.conv) {
+            const int tap = kb / p.cpb;
+            const int cb = kb - tap * p.cpb;
+            const int kh = tap / 3, kw = tap - kh * 3;
+            tma_load_4d(sa, &map_a, &full_bar[stage], cb * BK, w0 * p.conv_stride + kw - p.conv_pad,
+                        h0 * p.conv_stride + kh - p.conv_pad, img);
           } else {
-            if (item_i == 0 && kb == item.kb0) TL(3);
-            // both CTAs fill their own smem; all bytes are accounted on the leader's barrier (the MMA issuer's)
-#ifdef CFGPP_DIAG_HALFA
-            const bool load_a = !(kb & 1);
-#else
-            const bool load_a = true;
-#endif
-#ifdef CFGPP_DIAG_NOTMA
-            if (is_leader_cta) mbar_arrive(&full_bar[stage]);
-#else
-            if (is_leader_cta) mbar_arrive_expect_tx(&full_bar[stage], 2 * (load_a ? C::STAGE_BYTES : C::B_BYTES));
-#endif
-            if (!load_a) {
-            } else if (p.conv) {
-              const int tap = kb / p.cpb;
-              const int cb = kb - tap * p.cpb;
-              const int kh = tap / 3, kw = tap - kh * 3;
-              tma_load_4d_cg2(sa, &map_a, &full_bar[stage], cb * BK, w0 * p.conv_stride + kw - p.conv_pad,
-                              h0 * p.conv_stride + kh - p.conv_pad, img);
-            } else {
-              const int k0 = kb * BK;
-              if (k0 < p.k_split)
-                tma_load_2d_cg2(sa, &map_a, &full_bar[stage], k0, m0);
-              else
-                tma_load_2d_cg2(sa, &map_a2, &full_bar[stage], k0 - p.k_split, m0);
-            }
-            tma_load_2d_cg2(sb, &map_b, &full_bar[stage], kb * BK, n_blk * BN + cta_rank * (BN / 2));
+            const int k0 = kb * BK;
+            if (k0 < p.k_split)
+              tma_load_2d(sa, &map_a, &full_bar[stage], k0, m0);
+            else
+              tma_load_2d(sa, &map_a2, &full_bar[stage], k0 - p.k_split, m0);
           }
+          tma_load_2d(sb, &map_b, &full_bar[stage], kb * BK, n_blk * BN);
           if (++stage == C::STAGES) {
             stage = 0;
             phase ^= 1;
@@ -322,86 +227,31 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
         }
       }
     }
-  } else if (warp_idx == kMmaWarp) {
-    if (is_leader_cta) {
-      // ===================== MMA issuer (pair: leader CTA only; whole warp loops, one elected lane issues) ==========
-      constexpr uint32_t idesc = make_idesc_f16(BM * CL, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int it = 0; it < n_items; ++it) {
-        const Item item = item_at(it);
-        const int kb_first = item.kb0, kb_last = item.kb1 - 1;
-        const int as = it & 1;
-        const uint32_t aph = (it >> 1) & 1;
-        mbar_wait(&tmem_empty_bar[as], aph ^ 1);
-        const bool preloaded = (item.kind == kItemFin);  // the epilogue warps stored the other pieces' partial sum
-        if (preloaded) mbar_wait(sk_pre_bar, 0);         // into this accumulator stage: accumulate on top of it
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * C::ACC_STRIDE;
-        for (int kb = kb_first; kb <= kb_last; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES);
-          const uint32_t b_addr = a_addr + A_BYTES;
-          const uint64_t a_desc = make_sdesc_sw128(a_addr, 1024, 0);
-          const uint64_t b_desc = make_sdesc_sw128(b_addr, 1024, 0);
-          if (elect_one()) {
-            if (it == 0 && kb == kb_first) TL(4);
-            if (it == 0 && kb == kb_last) TL(5);
-            if (kb == kb_last) TL(6);
-#ifndef CFGPP_DIAG_NOMMA  // diagnostic build: operand traffic only, the commits below retire at once
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              // advance 16 fp16 = 32 B along K inside the swizzle atom: +2 in the (addr >> 4) field
-              if constexpr (CL == 1)
-                umma_f16(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (preloaded || kb != kb_first || k != 0) ? 1u : 0u);
-              else
-                umma_f16_cg2(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (preloaded || kb != kb_first || k != 0) ? 1u : 0u);
-            }
-#endif
-            // on retirement: free the smem slot (pair: in both CTAs) and, after the last k-block, publish the
-            // accumulator
-            if constexpr (CL == 1) {
-              umma_commit(&empty_bar[stage]);
-              if (kb == kb_last) umma_commit(&tmem_full_bar[as]);
-            } else {
-              umma_commit_cg2(&empty_bar[stage]);
-              if (kb == kb_last) umma_commit_cg2(&tmem_full_bar[as]);
-            }
-          }
-          if (++stage == C::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp_idx < kEpiWarps) {
-    // ===================== epilogue =====================
-    // TMEM -> registers -> (bias / time-embedding row / residual / GEGLU) -> fp16 into the swizzled smem staging
-    // tile -> TMA store (coalesced, clipped at the M / N edges by the hardware). Every warp works on its own
-    // [32 rows x 32 columns] sub-blocks end to end - residual TMA load, arithmetic, TMA store - so the only
-    // cross-warp synchronisation per tile is one named barrier publishing the staged bias / LN vectors.
-    const int q = warp_idx & 3;       // TMEM lane quarter this warp may access
-    const int half = warp_idx >> 2;   // chunk parity this warp handles
-    const int row = q * 32 + lane;
-    const int etid = warp_idx * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(q * 32) << 16;
+  } else {
+    setmaxnreg_inc<232>();
+    // ===================== MMA + epilogue (warpgroups 0 and 1) =====================
+    // Register fragment of the m64nBN accumulator: acc[4 i + e] is (row r0, column 8 i + 2 (lane % 4) + e),
+    // acc[4 i + 2 + e] is (row r0 + 8, same column); r0 = 64 g + 16 (warp % 4) + lane / 4.
+    const int wg = warp_idx >> 2;
+    const int wq = warp_idx & 3;
+    const int slab_row = wg * 64 + wq * 16;       // first tile row of this warp
+    const int r0 = slab_row + (lane >> 2);        // this thread's two rows: r0, r0 + 8
+    const int cq = 2 * (lane & 3);                // column offset inside an 8-column group
+    const int etid = threadIdx.x;                 // 0..255
     const bool leader = (threadIdx.x == 0);
     const bool full_res = (p.addend != nullptr) && (p.add_rows_per_group <= 1);
-    const int sw = (row >> 1) & 3;  // 64B swizzle: 16-byte chunk index ^= (row / 2) % 4
-    uint8_t* my_row = epi_smem + row * 64;
-    uint8_t* my_slab = epi_smem + q * 32 * 64;  // + j * EPI_SUB_BYTES: this warp's [32 x 64 B] block of sub-tile j
+    uint8_t* my_slab = epi_smem + slab_row * 64;  // + j * EPI_SUB_BYTES: this warp's [16 x 64 B] block of sub-tile j
     uint64_t* my_res_bar = &res_bar[warp_idx];
-    const int my_chunks = (C::EPI_SUB - half + 1) / 2;
+    // byte offset of (tile row r, 8-column group q of a 32-column sub-tile) in the 64B-swizzled staging sub-tile
+    auto stage_off = [&](int r, int q) { return r * 64 + ((q ^ ((r >> 1) & 3)) << 4) + (lane & 3) * 4; };
     auto issue_residual = [&](int tile) {  // one lane
       const int m_blk = tile_m_blk(tile);
       const int n_blk = tile_n_blk(tile);
-      mbar_arrive_expect_tx(my_res_bar, my_chunks * 32 * 64);
+      mbar_arrive_expect_tx(my_res_bar, C::EPI_SUB * 16 * 64);
 #pragma unroll 1
-      for (int j = half; j < C::EPI_SUB; j += 2)
+      for (int j = 0; j < C::EPI_SUB; ++j)
         tma_load_2d(my_slab + j * C::EPI_SUB_BYTES, &map_res, my_res_bar, n_blk * C::OUT_N + j * 32,
-                    m_blk * BM + q * 32);
+                    m_blk * BM + slab_row);
     };
     // residual tiles are prefetched one item ahead; stream-K pieces that only park a partial take none
     auto next_res_item = [&](int from) {
@@ -414,67 +264,53 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
       if (i0 < n_items) issue_residual(item_at(i0).tile);
     }
     int res_uses = 0;
-    // Stream-K fix-up: the partial accumulators the other clusters parked for this cluster's finishing piece are summed
-    // (fixed order) and STORED INTO THE TMEM STAGE that piece will use, so its MMAs simply accumulate on top and its
-    // epilogue is the ordinary one. This runs one item early — under the main loop of the data-parallel tile before
-    // the finishing piece — so the L2 round trips of the partial loads (~1 us per chunk and contributor) are hidden.
-    const bool has_fin = n_late && sk_late.kind == kItemFin;
-    const int pre_iter = (late_pos - 1 >= n_first) ? late_pos - 1 : late_pos;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[C::ACC];
+
+    // Stream-K fix-up: the partial accumulators the other CTAs parked for this CTA's finishing piece are summed
+    // (fixed order) into the registers its main loop then accumulates on top of.
     auto sk_preload = [&]() {
       auto contributes = [&](int c) { return sk_u0(c + 1) > sk_u0(c); };
-      if (leader) TL(13);
-      if (lane == 0) {  // acquire: every warp of every contributing cluster has published its partial
-        for (int c = sk_late.c_first; c < cluster_id; ++c) {
+      if (lane == 0) {  // acquire: every warp of every contributing CTA has published its partial
+        for (int c = sk_late.c_first; c < cta_id; ++c) {
           if (!contributes(c)) continue;
           unsigned seen;
+          const long long t0 = clock64();
           do {
             asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(p.sk_flags + c) : "memory");
             if (seen < kSkArrivals) __nanosleep(32);
+            if (clock64() - t0 > 4000000000LL) __trap();  // a peer that never publishes is a scheduling bug
           } while (seen < kSkArrivals);
         }
       }
       __syncwarp();  // the other lanes' partial loads (L2, __ldcg) are ordered after lane 0's acquire
-      if (leader) TL(14);
-      const uint32_t t_base = tmem_base + (late_pos & 1) * C::ACC_STRIDE + lane_off;
-#pragma unroll 1
-      for (int jt = half; jt < BN / 32; jt += 2) {
-        uint32_t v[32];
-        bool first = true;
-        for (int c = sk_late.c_first; c < cluster_id; ++c) {
-          if (!contributes(c)) continue;
-          const float4* src = reinterpret_cast<const float4*>(sk_ws(c)) + (static_cast<size_t>(jt) * 4 + q) * 256 + lane;
+      // the first contributor's partial is assigned, the others are added: a select between the two would keep the
+      // previous item's accumulator live through the loads
+      int c0 = sk_late.c_first;
+      while (!contributes(c0)) ++c0;  // the piece holding the tile's first k-block always contributes
+      auto add_partial = [&](int c, auto assign_c) {
+        constexpr bool ASSIGN = decltype(assign_c)::value;
+        const float2* src = reinterpret_cast<const float2*>(sk_ws(c)) + etid;
 #pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const float4 f = __ldcg(src + e * 32);
-            if (first) {
-              v[4 * e] = __float_as_uint(f.x);
-              v[4 * e + 1] = __float_as_uint(f.y);
-              v[4 * e + 2] = __float_as_uint(f.z);
-              v[4 * e + 3] = __float_as_uint(f.w);
-            } else {
-              v[4 * e] = __float_as_uint(__uint_as_float(v[4 * e]) + f.x);
-              v[4 * e + 1] = __float_as_uint(__uint_as_float(v[4 * e + 1]) + f.y);
-              v[4 * e + 2] = __float_as_uint(__uint_as_float(v[4 * e + 2]) + f.z);
-              v[4 * e + 3] = __float_as_uint(__uint_as_float(v[4 * e + 3]) + f.w);
-            }
-          }
-          first = false;
+        for (int i = 0; i < C::ACC / 2; ++i) {
+          const float2 f = __ldcg(src + i * 256);
+          acc[2 * i] = ASSIGN ? f.x : acc[2 * i] + f.x;
+          acc[2 * i + 1] = ASSIGN ? f.y : acc[2 * i + 1] + f.y;
+          // at most 8 loads in flight: hoisting all of them (BN = 256: 128 registers on top of the 128 of the
+          // accumulator) made ptxas spill
+          if (i % 8 == 7) asm volatile("" ::: "memory");
         }
-        tmem_st_x32(t_base + jt * 32, v);
-      }
-      tmem_st_wait();
-      tc_fence_before();
+      };
+      add_partial(c0, std::true_type{});
+      for (int c = c0 + 1; c < cta_id; ++c)
+        if (contributes(c)) add_partial(c, std::false_type{});
       __syncwarp();
       if (lane == 0) {
-        if constexpr (CL == 2)
-          mbar_arrive_leader(sk_pre_bar);
-        else
-          mbar_arrive(sk_pre_bar);
-        if (leader) TL(7);
         // this warp has consumed the partials: the last of the kSkArrivals consumers re-arms the contributor's flag,
         // so the buffers are back in their initial state when the kernel ends (CUDA-graph replays bake the arguments,
         // an epoch counter is not an option)
-        for (int c = sk_late.c_first; c < cluster_id; ++c) {
+        for (int c = sk_late.c_first; c < cta_id; ++c) {
           if (!contributes(c)) continue;
           const unsigned old = atomicAdd(p.sk_flags + kSkDoneOffset + c, 1u);
           if (old == kSkArrivals - 1) {
@@ -485,64 +321,68 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
       }
       __syncwarp();
     };
+
     for (int it = 0; it < n_items; ++it) {
-      if (has_fin && it == pre_iter) sk_preload();
       const Item item = item_at(it);
       const int tile = item.tile;
-      const int as = it & 1;
-      const uint32_t aph = (it >> 1) & 1;
+      // ---- main loop: wgmma over the smem ring, one k-block kept in flight ----
+      // a finishing stream-K piece starts from the other pieces' partial sum, every other item from zero (scale-d 0)
+      const bool preloaded = item.kind == kItemFin;
+      if (preloaded) sk_preload();
+      for (int kb = item.kb0; kb < item.kb1; ++kb) {
+        mbar_wait_nocall(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES) + wg * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem + stage * C::STAGE_BYTES) + A_BYTES;
+        const uint64_t a_desc = make_wgmma_desc_sw128(a_addr);
+        const uint64_t b_desc = make_wgmma_desc_sw128(b_addr);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_f16<BN>(acc, a_desc + 2 * k, b_desc + 2 * k, (preloaded || kb != item.kb0 || k != 0) ? 1u : 0u);
+        wgmma_commit();
+        // Retire the k-block before the next one (keeping one group in flight across iterations makes ptxas serialise
+        // every wgmma); the producer is STAGES - 1 loads ahead, so only the tensor pipe's drain is exposed.
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == C::STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      fence_acc(acc);
+
       if (item.kind == kItemPart) {
         // ---- stream-K piece that does not finish its tile: park the raw fp32 accumulator, publish, move on ----
-        mbar_wait(&tmem_full_bar[as], aph);
-        tc_fence_after();
-        const uint32_t t_base = tmem_base + as * C::ACC_STRIDE + lane_off;
-        float* ws = sk_ws(cluster_id);
-#pragma unroll 1
-        for (int jt = half; jt < BN / 32; jt += 2) {
-          uint32_t v[32];
-          tmem_ld_x32(t_base + jt * 32, v);
-          tmem_ld_wait();
-          // lane-contiguous: float4 e of lane l sits at [e][l], so one STG.128 of the warp writes 512 contiguous bytes
-          // (a row-contiguous layout - 128 B per lane - makes every store 32 separate L1 wavefronts: 6.5 us per tile)
-          float4* dst = reinterpret_cast<float4*>(ws) + (static_cast<size_t>(jt) * 4 + q) * 256 + lane;
+        // float2 pair i of thread t at [i][t]: one STG.64 of the warp writes 256 contiguous bytes
+        float2* dst = reinterpret_cast<float2*>(sk_ws(cta_id)) + etid;
 #pragma unroll
-          for (int e = 0; e < 8; ++e)
-            dst[e * 32] = make_float4(__uint_as_float(v[4 * e]), __uint_as_float(v[4 * e + 1]),
-                                      __uint_as_float(v[4 * e + 2]), __uint_as_float(v[4 * e + 3]));
-        }
-        tc_fence_before();
+        for (int i = 0; i < C::ACC / 2; ++i) dst[i * 256] = make_float2(acc[2 * i], acc[2 * i + 1]);
         __syncwarp();  // the warp's stores happen-before lane 0's release below (barrier + cumulativity)
-        if (lane == 0) {
-          if constexpr (CL == 2)
-            mbar_arrive_leader(&tmem_empty_bar[as]);
-          else
-            mbar_arrive(&tmem_empty_bar[as]);
-          // ONE release-add per warp publishes its part of the partial. (__threadfence() here — a fence.sc.gpu by all
-          // 256 epilogue threads — cost ~15 us per launch.)
-          asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p.sk_flags + cluster_id) : "memory");
-          if (leader) TL(15);
-        }
+        if (lane == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p.sk_flags + cta_id) : "memory");
         __syncwarp();
         continue;
       }
       const int m_blk = tile_m_blk(tile);
       const int n_blk = tile_n_blk(tile);
-      const int m = m_blk * BM + row;
+      const int mrow[2] = {m_blk * BM + r0, m_blk * BM + r0 + 8};
       __half* s_bias = reinterpret_cast<__half*>(vec_smem + (it & 1) * C::VEC_ONE);  // [256]
       __half* s_temb = s_bias + 256;                                                  // [256]
       float* s_lns = reinterpret_cast<float*>(s_temb + 256);                          // [256]
       float* s_lnt = s_lns + 256;                                                     // [256]
-      // Stage this tile's bias (and, when all 128 rows belong to one sample, its time-embedding row) in shared memory
-      // while the main loop is still running: global loads inside the per-chunk loop would expose ~1 us each. The
-      // buffers alternate with the tile parity, so a warp that runs ahead never overwrites vectors still being read.
-      const __half* add_row = nullptr;  // per-sample row broadcast (ResnetBlock2D time embedding)
+      // Stage this tile's bias (and, when all 128 rows belong to one sample, its time-embedding row) in shared memory.
+      // The buffers alternate with the tile parity, so a warp that runs ahead never overwrites vectors still being read.
+      const __half* add_rows[2] = {nullptr, nullptr};  // per-sample row broadcast (ResnetBlock2D time embedding)
       bool temb_staged = false;
       if (p.addend != nullptr && !full_res) {
         const int m_first = m_blk * BM;
         const int m_last = (m_first + BM - 1 < p.M ? m_first + BM - 1 : p.M - 1);
         temb_staged = (m_first < p.M) && (m_first / p.add_rows_per_group == m_last / p.add_rows_per_group);
-        const int mm = m < p.M ? m : p.M - 1;
-        add_row = p.addend + static_cast<size_t>(mm / p.add_rows_per_group) * p.ld_add;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int mm = mrow[h] < p.M ? mrow[h] : p.M - 1;
+          add_rows[h] = p.addend + static_cast<size_t>(mm / p.add_rows_per_group) * p.ld_add;
+        }
+        if (temb_staged) add_rows[0] = add_rows[1] = p.addend + static_cast<size_t>(m_first / p.add_rows_per_group) * p.ld_add;
       }
       {
         const int ncols = GEGLU ? BN : C::OUT_N;  // GEGLU stages value + gate biases (packed alike)
@@ -551,102 +391,93 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
           const int n = n_base + c;
           const bool ok = n < p.N;
           s_bias[c] = (p.bias && ok) ? p.bias[n] : __float2half(0.f);
-          if (temb_staged) s_temb[c] = ok ? add_row[n] : __float2half(0.f);
+          if (temb_staged) s_temb[c] = ok ? add_rows[0][n] : __float2half(0.f);
           if (p.stats_in) {
             s_lns[c] = ok ? p.ln_s[n] : 0.f;
             s_lnt[c] = ok ? p.ln_t[n] : 0.f;
           }
         }
       }
-      // LayerNorm fold: this row's mean / rstd from the producer's per-N-block partial sums (fixed order)
-      float ln_rstd = 1.f, ln_rm = 0.f;
-      if (p.stats_in && m < p.M) {
-        float sx = 0.f, sxx = 0.f;
-        for (int i = 0; i < p.ln_parts; ++i) {
-          const float2 v = *reinterpret_cast<const float2*>(p.stats_in + (static_cast<size_t>(i) * p.M + m) * 2);
-          sx += v.x;
-          sxx += v.y;
+      // LayerNorm fold: the rows' mean / rstd from the producer's per-N-block partial sums (fixed order)
+      float ln_rstd[2] = {1.f, 1.f}, ln_rm[2] = {0.f, 0.f};
+      if (p.stats_in) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (mrow[h] >= p.M) continue;
+          float sx = 0.f, sxx = 0.f;
+          for (int i = 0; i < p.ln_parts; ++i) {
+            const float2 v = *reinterpret_cast<const float2*>(p.stats_in + (static_cast<size_t>(i) * p.M + mrow[h]) * 2);
+            sx += v.x;
+            sxx += v.y;
+          }
+          const float mean = sx * p.ln_inv_c;
+          const float var = fmaxf(sxx * p.ln_inv_c - mean * mean, 0.f);
+          ln_rstd[h] = rsqrtf(var + p.ln_eps);
+          ln_rm[h] = ln_rstd[h] * mean;
         }
-        const float mean = sx * p.ln_inv_c;
-        const float var = fmaxf(sxx * p.ln_inv_c - mean * mean, 0.f);
-        ln_rstd = rsqrtf(var + p.ln_eps);
-        ln_rm = ln_rstd * mean;
       }
-      float ps = 0.f, pss = 0.f;  // producer side: partial row statistics of this warp's columns of the tile
+      // producer side: partial row statistics [row h][column half] of this thread's columns of the tile
+      float ps[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, pss[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
       named_bar_sync(1, kEpiWarps * 32);  // staged vectors visible to all epilogue threads
-      mbar_wait(&tmem_full_bar[as], aph);
       if (leader) { TL(9); if (tl) tl[12] = it + 1; }
-      tc_fence_after();
-      if (full_res) mbar_wait(my_res_bar, (res_uses++) & 1);
-      const uint32_t t_base = tmem_base + as * C::ACC_STRIDE + lane_off;
+      if (full_res) mbar_wait_nocall(my_res_bar, (res_uses++) & 1);
 
       // The arithmetic variant (LayerNorm fold / kind of addend / row statistics) is chosen ONCE per tile and the chunk
-      // loop is instantiated per variant: with the flags tested inside the unrolled loop the compiler unswitched every
-      // 8-column group into a tree of ~140 branches spread over 50 KB of code, and the epilogue ran at ~1 us per
-      // 32-column chunk (instruction fetch bound) instead of ~0.3 us.
+      // loop is instantiated per variant, so the unrolled loop carries no per-element branches on them.
       if constexpr (!GEGLU) {
         auto chunks = [&](auto ln_c, auto add_c, auto st_c) {
           constexpr bool LN = decltype(ln_c)::value;
           constexpr int ADD = decltype(add_c)::value;  // 0 none, 1 full residual tile, 2 staged row, 3 per-row global
           constexpr bool ST = decltype(st_c)::value;
-#pragma unroll 1
-          for (int j = half; j < C::EPI_SUB; j += 2) {
-            uint32_t v[32];
-            tmem_ld_x32(t_base + j * 32, v);
-            tmem_ld_wait();
-            const int n0 = n_blk * BN + j * 32;
-            uint8_t* srow = my_row + j * C::EPI_SUB_BYTES;
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {  // 8 columns = one 16-byte piece of the output row
-              const int col = j * 32 + c * 8;
-              uint4 r4 = make_uint4(0, 0, 0, 0), b4 = make_uint4(0, 0, 0, 0);
-              if constexpr (ADD == 1) r4 = *reinterpret_cast<const uint4*>(srow + ((c ^ sw) << 4));
-              if constexpr (ADD == 2) r4 = *reinterpret_cast<const uint4*>(s_temb + col);
-              if constexpr (!LN) b4 = *reinterpret_cast<const uint4*>(s_bias + col);  // zeros when there is no bias
-              const __half2* rh = reinterpret_cast<const __half2*>(&r4);
-              const __half2* bh = reinterpret_cast<const __half2*>(&b4);
-              float sv[8], tv[8];
+          for (int i = 0; i < BN / 8; ++i) {  // 8-column group i: sub-tile i / 4, 16-byte piece i % 4
+            const int col = i * 8 + cq;
+            uint8_t* sub = epi_smem + (i >> 2) * C::EPI_SUB_BYTES;
+            float b0 = 0.f, b1 = 0.f, sv0 = 0.f, sv1 = 0.f, tv0 = 0.f, tv1 = 0.f;
+            if constexpr (LN) {
+              sv0 = s_lns[col]; sv1 = s_lns[col + 1];
+              tv0 = s_lnt[col]; tv1 = s_lnt[col + 1];
+            } else {
+              const __half2 bh = *reinterpret_cast<const __half2*>(s_bias + col);  // zeros when there is no bias
+              b0 = __low2float(bh);
+              b1 = __high2float(bh);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int r = r0 + 8 * h;
+              float x0 = acc[4 * i + 2 * h], x1 = acc[4 * i + 2 * h + 1];
               if constexpr (LN) {
-                *reinterpret_cast<float4*>(&sv[0]) = *reinterpret_cast<const float4*>(s_lns + col);
-                *reinterpret_cast<float4*>(&sv[4]) = *reinterpret_cast<const float4*>(s_lns + col + 4);
-                *reinterpret_cast<float4*>(&tv[0]) = *reinterpret_cast<const float4*>(s_lnt + col);
-                *reinterpret_cast<float4*>(&tv[4]) = *reinterpret_cast<const float4*>(s_lnt + col + 4);
+                x0 = x0 * ln_rstd[h] - ln_rm[h] * sv0 + tv0;
+                x1 = x1 * ln_rstd[h] - ln_rm[h] * sv1 + tv1;
+              } else {
+                x0 += b0;
+                x1 += b1;
               }
-              uint32_t o[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int jj = c * 4 + e;  // half2 index within the 32-column chunk
-                float x0 = __uint_as_float(v[2 * jj]), x1 = __uint_as_float(v[2 * jj + 1]);
-                if constexpr (LN) {
-                  x0 = x0 * ln_rstd - ln_rm * sv[2 * e] + tv[2 * e];
-                  x1 = x1 * ln_rstd - ln_rm * sv[2 * e + 1] + tv[2 * e + 1];
-                } else {
-                  x0 += __low2float(bh[e]);
-                  x1 += __high2float(bh[e]);
-                }
-                __half2 t = __floats2half2_rn(x0, x1);
-                if constexpr (ADD == 1 || ADD == 2) {
-                  t = __floats2half2_rn(__low2float(t) + __low2float(rh[e]), __high2float(t) + __high2float(rh[e]));
-                } else if constexpr (ADD == 3) {  // tile spans several samples (tiny latents): per-row global loads
-                  float a0 = 0.f, a1 = 0.f;
-                  if (n0 + 2 * jj < p.N) a0 = __half2float(add_row[n0 + 2 * jj]);
-                  if (n0 + 2 * jj + 1 < p.N) a1 = __half2float(add_row[n0 + 2 * jj + 1]);
-                  t = __floats2half2_rn(__low2float(t) + a0, __high2float(t) + a1);
-                }
-                if constexpr (ST) {
-                  const float f0 = __low2float(t), f1 = __high2float(t);
-                  ps += f0 + f1;
-                  pss += f0 * f0 + f1 * f1;
-                }
-                o[e] = *reinterpret_cast<uint32_t*>(&t);
+              __half2 t = __floats2half2_rn(x0, x1);
+              __half2* sp = reinterpret_cast<__half2*>(sub + stage_off(r, i & 3));
+              if constexpr (ADD == 1 || ADD == 2) {
+                const __half2 rh = ADD == 1 ? *sp : *reinterpret_cast<const __half2*>(s_temb + col);
+                t = __floats2half2_rn(__low2float(t) + __low2float(rh), __high2float(t) + __high2float(rh));
+              } else if constexpr (ADD == 3) {  // tile spans several samples (tiny latents): per-row global loads
+                const int n = n_blk * BN + col;
+                float a0 = 0.f, a1 = 0.f;
+                if (n < p.N) a0 = __half2float(add_rows[h][n]);
+                if (n + 1 < p.N) a1 = __half2float(add_rows[h][n + 1]);
+                t = __floats2half2_rn(__low2float(t) + a0, __high2float(t) + a1);
               }
-              *reinterpret_cast<uint4*>(srow + ((c ^ sw) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
+              if constexpr (ST) {
+                const float f0 = __low2float(t), f1 = __high2float(t);
+                const int hc = (i < BN / 16) ? 0 : 1;
+                ps[h][hc] += f0 + f1;
+                pss[h][hc] += f0 * f0 + f1 * f1;
+              }
+              *sp = t;
             }
           }
         };
         using T = std::true_type;
         using F = std::false_type;
-        const int add_mode = full_res ? 1 : (add_row == nullptr ? 0 : (temb_staged ? 2 : 3));
+        const int add_mode = full_res ? 1 : (p.addend == nullptr ? 0 : (temb_staged ? 2 : 3));
         if (p.stats_in) {  // LayerNorm-fold consumer: bias is inside t_n; no addend, no statistics (host-checked)
           chunks(T{}, std::integral_constant<int, 0>{}, F{});
         } else if (p.stats_out) {
@@ -668,57 +499,40 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
         // value columns [0,128), gate columns [128,256) of this tile -> 128 output columns
         auto chunks = [&](auto ln_c) {
           constexpr bool LN = decltype(ln_c)::value;
-#pragma unroll 1
-          for (int j = half; j < C::EPI_SUB; j += 2) {
-            uint32_t va[32], vg[32];
-            tmem_ld_x32(t_base + j * 32, va);
-            tmem_ld_x32(t_base + BN / 2 + j * 32, vg);
-            tmem_ld_wait();
-            uint8_t* srow = my_row + j * C::EPI_SUB_BYTES;
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const int ia = j * 32 + c * 8, ig = BN / 2 + ia;
-              uint4 ba4 = make_uint4(0, 0, 0, 0), bg4 = make_uint4(0, 0, 0, 0);
-              float sa[8], ta[8], sg[8], tg[8];
+          for (int i = 0; i < BN / 16; ++i) {
+            const int ia = i * 8 + cq, ig = BN / 2 + ia;
+            const int ig_grp = i + BN / 16;
+            uint8_t* sub = epi_smem + (i >> 2) * C::EPI_SUB_BYTES;
+            float ba0 = 0.f, ba1 = 0.f, bg0 = 0.f, bg1 = 0.f;
+            float sa0 = 0.f, sa1 = 0.f, ta0 = 0.f, ta1 = 0.f, sg0 = 0.f, sg1 = 0.f, tg0 = 0.f, tg1 = 0.f;
+            if constexpr (LN) {
+              sa0 = s_lns[ia]; sa1 = s_lns[ia + 1]; ta0 = s_lnt[ia]; ta1 = s_lnt[ia + 1];
+              sg0 = s_lns[ig]; sg1 = s_lns[ig + 1]; tg0 = s_lnt[ig]; tg1 = s_lnt[ig + 1];
+            } else {
+              const __half2 bah = *reinterpret_cast<const __half2*>(s_bias + ia);  // zeros when there is no bias
+              const __half2 bgh = *reinterpret_cast<const __half2*>(s_bias + ig);
+              ba0 = __low2float(bah); ba1 = __high2float(bah);
+              bg0 = __low2float(bgh); bg1 = __high2float(bgh);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float a0 = acc[4 * i + 2 * h], a1 = acc[4 * i + 2 * h + 1];
+              float g0 = acc[4 * ig_grp + 2 * h], g1 = acc[4 * ig_grp + 2 * h + 1];
               if constexpr (LN) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  *reinterpret_cast<float4*>(&sa[4 * h]) = *reinterpret_cast<const float4*>(s_lns + ia + 4 * h);
-                  *reinterpret_cast<float4*>(&ta[4 * h]) = *reinterpret_cast<const float4*>(s_lnt + ia + 4 * h);
-                  *reinterpret_cast<float4*>(&sg[4 * h]) = *reinterpret_cast<const float4*>(s_lns + ig + 4 * h);
-                  *reinterpret_cast<float4*>(&tg[4 * h]) = *reinterpret_cast<const float4*>(s_lnt + ig + 4 * h);
-                }
+                a0 = a0 * ln_rstd[h] - ln_rm[h] * sa0 + ta0;
+                a1 = a1 * ln_rstd[h] - ln_rm[h] * sa1 + ta1;
+                g0 = g0 * ln_rstd[h] - ln_rm[h] * sg0 + tg0;
+                g1 = g1 * ln_rstd[h] - ln_rm[h] * sg1 + tg1;
               } else {
-                ba4 = *reinterpret_cast<const uint4*>(s_bias + ia);  // zeros when there is no bias
-                bg4 = *reinterpret_cast<const uint4*>(s_bias + ig);
+                a0 += ba0; a1 += ba1;
+                g0 += bg0; g1 += bg1;
               }
-              const __half2* bah = reinterpret_cast<const __half2*>(&ba4);
-              const __half2* bgh = reinterpret_cast<const __half2*>(&bg4);
-              uint32_t o[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int jj = c * 4 + e;
-                float a0 = __uint_as_float(va[2 * jj]), a1 = __uint_as_float(va[2 * jj + 1]);
-                float g0 = __uint_as_float(vg[2 * jj]), g1 = __uint_as_float(vg[2 * jj + 1]);
-                if constexpr (LN) {
-                  a0 = a0 * ln_rstd - ln_rm * sa[2 * e] + ta[2 * e];
-                  a1 = a1 * ln_rstd - ln_rm * sa[2 * e + 1] + ta[2 * e + 1];
-                  g0 = g0 * ln_rstd - ln_rm * sg[2 * e] + tg[2 * e];
-                  g1 = g1 * ln_rstd - ln_rm * sg[2 * e + 1] + tg[2 * e + 1];
-                } else {
-                  a0 += __low2float(bah[e]);
-                  a1 += __high2float(bah[e]);
-                  g0 += __low2float(bgh[e]);
-                  g1 += __high2float(bgh[e]);
-                }
-                const __half2 ah = __floats2half2_rn(a0, a1);
-                const __half2 gh = __floats2half2_rn(g0, g1);
-                const __half2 ge = __floats2half2_rn(gelu_erf_fast_f(__low2float(gh)), gelu_erf_fast_f(__high2float(gh)));
-                const __half2 r =
-                    __floats2half2_rn(__low2float(ah) * __low2float(ge), __high2float(ah) * __high2float(ge));
-                o[e] = *reinterpret_cast<const uint32_t*>(&r);
-              }
-              *reinterpret_cast<uint4*>(srow + ((c ^ sw) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
+              const __half2 ah = __floats2half2_rn(a0, a1);
+              const __half2 gh = __floats2half2_rn(g0, g1);
+              const __half2 ge = __floats2half2_rn(gelu_erf_fast_f(__low2float(gh)), gelu_erf_fast_f(__high2float(gh)));
+              *reinterpret_cast<__half2*>(sub + stage_off(r0 + 8 * h, i & 3)) =
+                  __floats2half2_rn(__low2float(ah) * __low2float(ge), __high2float(ah) * __high2float(ge));
             }
           }
         };
@@ -727,18 +541,12 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
         else
           chunks(std::false_type{});
       }
-      tc_fence_before();
       fence_proxy_async_smem();  // this thread's part of the staging tile -> visible to the TMA engine
       __syncwarp();
       if (lane == 0) {
-        // accumulator columns of this warp drained: one arrive per warp (pair: on the leader CTA's barrier)
-        if constexpr (CL == 2)
-          mbar_arrive_leader(&tmem_empty_bar[as]);
-        else
-          mbar_arrive(&tmem_empty_bar[as]);
 #pragma unroll 1
-        for (int j = half; j < C::EPI_SUB; j += 2)
-          tma_store_2d(&map_out, my_slab + j * C::EPI_SUB_BYTES, n_blk * C::OUT_N + j * 32, m_blk * BM + q * 32);
+        for (int j = 0; j < C::EPI_SUB; ++j)
+          tma_store_2d(&map_out, my_slab + j * C::EPI_SUB_BYTES, n_blk * C::OUT_N + j * 32, m_blk * BM + slab_row);
         tma_store_commit();
         if (leader) { if (it == 0) TL(8); TL(10); }
         tma_store_wait_read0();  // this warp's staging blocks have been read out: reusable
@@ -748,53 +556,44 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
         }
       }
       __syncwarp();
-      // (written after the tmem_empty arrive: a global store ahead of that cluster-scope release would delay it)
-      if (p.stats_out && m < p.M)
-        *reinterpret_cast<float2*>(p.stats_out + (static_cast<size_t>(n_blk * 2 + half) * p.M + m) * 2) =
-            make_float2(ps, pss);
+      if constexpr (!GEGLU) {
+        if (p.stats_out) {  // quad reduction (the four lanes of a row), then one float2 per row and column half
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int hc = 0; hc < 2; ++hc) {
+              ps[h][hc] += __shfl_xor_sync(0xffffffffu, ps[h][hc], 1);
+              ps[h][hc] += __shfl_xor_sync(0xffffffffu, ps[h][hc], 2);
+              pss[h][hc] += __shfl_xor_sync(0xffffffffu, pss[h][hc], 1);
+              pss[h][hc] += __shfl_xor_sync(0xffffffffu, pss[h][hc], 2);
+            }
+            if ((lane & 3) == 0 && mrow[h] < p.M) {
+#pragma unroll
+              for (int hc = 0; hc < 2; ++hc)
+                *reinterpret_cast<float2*>(p.stats_out + (static_cast<size_t>(n_blk * 2 + hc) * p.M + mrow[h]) * 2) =
+                    make_float2(ps[h][hc], pss[h][hc]);
+            }
+          }
+        }
+      }
     }
     if (lane == 0) tma_store_wait0();
     if (leader) TL(11);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CL > 1) cluster_sync_all();  // no CTA leaves while its peer may still multicast / arrive into it
-  if (warp_idx == kAllocWarp) {
-    tc_fence_after();
-    if constexpr (CL == 2)
-      tmem_dealloc_cg2(tmem_base, C::TMEM_COLS);
-    else
-      tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
+#undef TL
 }
 
 template <int BN, bool GEGLU>
 void configure_one() {
-  CFGPP_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, GEGLU, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        Cfg<BN, GEGLU, 1>::SMEM_BYTES));
-  CFGPP_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, GEGLU, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        Cfg<BN, GEGLU, 2>::SMEM_BYTES));
+  CFGPP_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, GEGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        Cfg<BN, GEGLU>::SMEM_BYTES));
 }
 
 template <int BN, bool GEGLU>
 void launch(const GemmOp& op, cudaStream_t stream) {
   gemm_configure();
-  if (op.cluster == 2)
-    launch_pdl_cluster(gemm_kernel<BN, GEGLU, 2>, dim3(op.grid), dim3(kThreads), Cfg<BN, GEGLU, 2>::SMEM_BYTES, stream,
-                       2, op.p, op.map_a, op.map_a2, op.map_b, op.map_out, op.map_res);
-  else
-    launch_pdl_cluster(gemm_kernel<BN, GEGLU, 1>, dim3(op.grid), dim3(kThreads), Cfg<BN, GEGLU, 1>::SMEM_BYTES, stream,
-                       1, op.p, op.map_a, op.map_a2, op.map_b, op.map_out, op.map_res);
-}
-
-bool cluster_disabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("CFGPP_NO_CLUSTER");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
+  launch_pdl(gemm_kernel<BN, GEGLU>, dim3(op.grid), dim3(kThreads), Cfg<BN, GEGLU>::SMEM_BYTES, stream, op.p, op.map_a,
+             op.map_a2, op.map_b, op.map_out, op.map_res);
 }
 
 // CFGPP_NO_STREAMK=1 switches the remainder stream-K off (A/B runs); it is also off when the two CFG halves run as
@@ -808,7 +607,7 @@ bool streamk_enabled() {
   }
   return v == 1;
 }
-double streamk_min_saved() {  // k-blocks of main loop the split must save per cluster (CFGPP_STREAMK_MIN overrides)
+double streamk_min_saved() {  // k-blocks of main loop the split must save per CTA (CFGPP_STREAMK_MIN overrides)
   static double v = -1.0;
   if (v < 0) {
     const char* e = getenv("CFGPP_STREAMK_MIN");
@@ -816,10 +615,9 @@ double streamk_min_saved() {  // k-blocks of main loop the split must save per c
   }
   return v;
 }
-// Tile walk of the linear layers: N-fastest, so the clusters running concurrently cover few M groups and every A tile is
-// fetched from HBM once (the activations of the 64 x 64 / 128 x 128 levels — 84 MB at M = 16384, K = 2560 — do not
-// survive num_n_blocks M-fastest passes in the 126 MB L2: 61.8 -> 54.4 us there, 61.2 -> 51.3 us at M = 65536, N = 320;
-// neutral elsewhere, same box). CFGPP_RASTER=0 restores the M-fastest walk; the convolutions keep it (no difference).
+// Tile walk of the linear layers: N-fastest, so the CTAs running concurrently cover few M blocks and every A tile is
+// fetched from HBM about once (large activations do not survive num_n_blocks M-fastest passes through the L2).
+// CFGPP_RASTER=0 restores the M-fastest walk; the convolutions keep it.
 int raster_mode() {
   static int v = -1;
   if (v < 0) {
@@ -844,8 +642,8 @@ double streamk_min_piece() {  // smallest piece as a fraction of a tile's k-bloc
   }
   return v;
 }
-// Stream-K workspace: partial accumulators for up to 148 CTAs ([128 x 256] fp32 each) + the flag words. Launches that
-// share a workspace must be stream-ordered (the flags are per cluster id), so every model handle owns one
+// Stream-K workspace: partial accumulators for up to kSkMaxCtas CTAs ([128 x 256] fp32 each) + the flag words. Launches that
+// share a workspace must be stream-ordered (the flags are per CTA id), so every model handle owns one
 // (StreamKScope around its plan building; a handle runs on one stream at a time) and the operator-level entry points
 // fall back to one buffer per device.
 thread_local float* t_sk_ws = nullptr;
@@ -867,23 +665,20 @@ void streamk_buffers(float** ws, unsigned** flags) {
   *flags = g_flags[dev];
 }
 
-// Tile-width heuristic, fitted to tools/bn_sweep.py (every GEMM / conv shape of the SDXL UNet x every width, timed
-// inside CUDA graphs): time ~ rounds x (BN + 50), rounds = tiles each CTA (pair) walks. The additive term is the
-// per-k-block cost that does not scale with the tile width (A-tile ingest, barrier round trip); 64-wide tiles never
-// reach the tensor pipe's rate (operand fetch bound), hence their floor.
+// Tile-width heuristic: time ~ rounds x (BN + 50), rounds = tiles each CTA walks. The additive term is the per-k-block
+// cost that does not scale with the tile width (A-tile ingest, barrier round trip); 64-wide tiles never reach the
+// tensor pipe's rate (operand fetch bound), hence their floor.
 int choose_bn(int M, int N, bool geglu) {
   if (geglu) return 256;
   const int mb = (M + BM - 1) / BM;
-  const int cl = (mb >= 2 && !cluster_disabled()) ? 2 : 1;
-  const int slots = std::max(1, num_sms() / cl);
-  const int mg = (mb + cl - 1) / cl;
+  const int slots = std::max(1, num_sms());
   const int cand[4] = {256, 160, 128, 64};
   int best = 128;
   double best_cost = 1e30;
   for (int bn : cand) {
     if (bn == 160 && N % 160 != 0) continue;
     const int nb = (N + bn - 1) / bn;
-    const long tiles = static_cast<long>(mg) * nb;
+    const long tiles = static_cast<long>(mb) * nb;
     const long rounds = (tiles + slots - 1) / slots;
     const double tile_cost = (bn < 128 ? 128 * 1.15 : bn) + 50.0;
     const double cost = rounds * tile_cost;
@@ -903,42 +698,35 @@ void finish_op(GemmOp& op, const __half* w, int force_bn) {
   p.num_m_blocks = (p.M + BM - 1) / BM;
   p.num_n_blocks = (p.N + op.bn - 1) / op.bn;
   p.raster = p.conv ? 0 : raster_mode();
-  op.cluster = (p.num_m_blocks >= 2 && !cluster_disabled()) ? 2 : 1;
-  op.map_b = make_tmap_2d(w, p.N, p.K, p.K, op.bn / op.cluster);
+  op.map_b = make_tmap_2d(w, p.N, p.K, p.K, op.bn);
   const int n_out = p.geglu ? p.N / 2 : p.N;
-  op.map_out = make_tmap_2d_sw64(p.out, p.M, n_out, p.ldc, 32);  // one epilogue warp's [32 x 32] block
+  op.map_out = make_tmap_2d_sw64(p.out, p.M, n_out, p.ldc, 16);  // one epilogue warp's [16 x 32] block
   if (p.addend != nullptr && p.add_rows_per_group <= 1) {
     CFGPP_REQUIRE(p.ld_add % 8 == 0, "residual leading dimension must be a multiple of 8");
-    op.map_res = make_tmap_2d_sw64(p.addend, p.M, p.N, p.ld_add, 32);
+    op.map_res = make_tmap_2d_sw64(p.addend, p.M, p.N, p.ld_add, 16);
   } else {
     op.map_res = op.map_out;
   }
-  const int groups = ((p.num_m_blocks + op.cluster - 1) / op.cluster) * p.num_n_blocks;
-  const int max_clusters = num_sms() / op.cluster;
-  op.grid = op.cluster * (groups < max_clusters ? groups : max_clusters);
+  const int groups = p.num_m_blocks * p.num_n_blocks;
+  const int max_ctas = num_sms();
+  op.grid = groups < max_ctas ? groups : max_ctas;
   // stream-K for the remainder tiles (kernel comment "work schedule"): worth it when the left-over round would idle
-  // the clusters for at least a few k-blocks and the pieces are not slivers
+  // the CTAs for at least a few k-blocks and the pieces are not slivers
   p.sk_ws = nullptr;
   p.sk_flags = nullptr;
-  const int rem = groups % max_clusters;
-  if (streamk_enabled() && rem != 0 && max_clusters <= kSkMaxClusters) {
-    // Policy from measurements (tools/diag_kernels.py bench_gemm_graph, graph-timed, same box, with / without):
-    //   conv3x3 1280->1280 @32x32 (180 k-blocks)  119.4 -> 108.7 us     2560->1280  234.7 -> 210.2 us
-    //   conv3x3 640->640 @64x64 (90 k-blocks)     122.1 -> 109.6 us
-    //   linear K = 5120 (80 k-blocks)              47.1 ->  50.2 us     K = 1280 (20)  17.3 -> 25.8 us   GEGLU 82 -> 93
-    // The parked partial + preload cost a fixed ~8 us per launch that only main loops of >= ~90 k-blocks amortise, so
-    // the implicit-GEMM convolutions take the split and the linear layers keep the plain tile walk
+  const int rem = groups % max_ctas;
+  if (streamk_enabled() && rem != 0 && max_ctas <= kSkMaxCtas) {
+    // The parked partial and the fix-up cost a fixed few microseconds per launch that only long main loops amortise,
+    // so the implicit-GEMM convolutions take the split and the linear layers keep the plain tile walk
     // (CFGPP_STREAMK_LINEAR=1 forces it on for them; CFGPP_STREAMK_MIN / _PIECE tune the thresholds).
-    const double piece = static_cast<double>(rem) * p.num_k_blocks / max_clusters;
+    const double piece = static_cast<double>(rem) * p.num_k_blocks / max_ctas;
     const double saved = (p.num_k_blocks - piece) * op.bn / 160.0;
     const bool eligible = p.conv || streamk_linear();
-    // pieces at least half a tile deep: a tile then has at most three pieces, i.e. <= 2 partials to sum per chunk —
-    // unless the saving is large anyway: with fewer tiles than clusters and a long K (SD v1.5's 8 x 8 level: 16 tiles of
-    // 180 k-blocks on 74 clusters, 89 us at 242 TFLOP/s) every cluster takes ~1/5 of a tile and the fix-up sums 4-5
-    // partials per chunk, still a small price for a 4.6x shorter main loop
+    // pieces at least half a tile deep (a tile then has at most three pieces, i.e. <= 2 partials to sum), unless the
+    // saving is large anyway: with fewer tiles than CTAs and a long K every CTA takes a fraction of a tile
     const bool deep_enough = piece >= streamk_min_piece() * p.num_k_blocks || saved >= 60.0;
     if (eligible && saved >= streamk_min_saved() && piece >= 2.0 && deep_enough) {
-      op.grid = op.cluster * max_clusters;  // all clusters take part, also when there are fewer tiles than clusters
+      op.grid = max_ctas;  // all CTAs take part, also when there are fewer tiles than CTAs
       streamk_buffers(&p.sk_ws, &p.sk_flags);
     }
   }
@@ -947,9 +735,9 @@ void finish_op(GemmOp& op, const __half* w, int force_bn) {
 }  // namespace
 
 void streamk_alloc(float** ws, unsigned** flags) {
-  CFGPP_CHECK_CUDA(cudaMalloc(ws, static_cast<size_t>(kSkMaxClusters) * BM * 256 * sizeof(float)));
-  CFGPP_CHECK_CUDA(cudaMalloc(flags, 2 * kSkMaxClusters * sizeof(unsigned)));
-  CFGPP_CHECK_CUDA(cudaMemset(*flags, 0, 2 * kSkMaxClusters * sizeof(unsigned)));
+  CFGPP_CHECK_CUDA(cudaMalloc(ws, static_cast<size_t>(kSkMaxCtas) * BM * 256 * sizeof(float)));
+  CFGPP_CHECK_CUDA(cudaMalloc(flags, 2 * kSkMaxCtas * sizeof(unsigned)));
+  CFGPP_CHECK_CUDA(cudaMemset(*flags, 0, 2 * kSkMaxCtas * sizeof(unsigned)));
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
 }
 void streamk_free(float* ws, unsigned* flags) {

@@ -1,6 +1,6 @@
-// cfgpp_b200 — tcgen05 GEMM / implicit-GEMM conv3x3 operator (host interface).
+// cfgpp_b200 — wgmma GEMM / implicit-GEMM conv3x3 operator (host interface).
 //
-//   out[M,N] = epilogue( A[M,K] * B[N,K]^T )         fp16 in, fp32 accumulate in TMEM, fp16 out
+//   out[M,N] = epilogue( A[M,K] * B[N,K]^T )         fp16 in, fp32 accumulate in registers, fp16 out
 //
 // A is the activation in NHWC (= tokens x channels, K contiguous); B is the packed weight (N x K, K contiguous).
 // Modes:
@@ -51,7 +51,7 @@ struct GemmParams {
   const float* ln_s;       // [N] fp32
   const float* ln_t;       // [N] fp32
   // ---- stream-K for the remainder tiles (see gemm.cu "work schedule"); null = plain data-parallel tile walk ------
-  float* sk_ws;            // per (cluster, CTA rank) partial accumulator, 128 x BN fp32 in the epilogue's lane order
+  float* sk_ws;            // per CTA partial accumulator, 128 x BN fp32 in the accumulator's register order
   unsigned* sk_flags;      // [2 * 256] zero-initialised, self-resetting arrival / consumer counters
 };
 
@@ -60,7 +60,6 @@ struct GemmOp {
   GemmParams p;
   int bn;
   int grid;
-  int cluster;  // thread-block-cluster size along M (1 or 2)
   // FLOP accounting (algorithmic): 2*M*N*K
   double flops() const { return 2.0 * p.M * (double)p.N * p.K; }
 };

@@ -4,7 +4,7 @@
 // `CLIPTextModelWithProjection`: token + position embedding, N pre-LN layers (causal self-attention with 64-wide
 // heads, MLP with quick_gelu or gelu), final LayerNorm, pooled <|endoftext|> row (+ bias-free text_projection).
 // Activations are [batch * tokens][hidden] fp16; the q/k/v projections run as ONE GEMM on a concatenated weight; every
-// projection / MLP GEMM is the tcgen05 kernel of gemm.cu (residual adds in its epilogue), attention / activation /
+// projection / MLP GEMM is the wgmma kernel of gemm.cu (residual adds in its epilogue), attention / activation /
 // embedding are the kernels of text_kernels.cu, LayerNorm is norm.cu's.
 #pragma once
 #include <functional>

@@ -1,7 +1,7 @@
 // cfgpp_b200 — the small kernels of the CLIP text towers (see text_encoder.cuh): token + position embedding, the
 // 77-token causal self-attention (one CTA per (head, prompt); K / V of a head live in shared memory, fp32 scores and
 // probabilities — the sequences are far too short for a tensor-core tile), the MLP activation, and the gather of the
-// pooled (<|endoftext|>) row. The projections and MLP GEMMs run on the tcgen05 GEMM of gemm.cu.
+// pooled (<|endoftext|>) row. The projections and MLP GEMMs run on the wgmma GEMM of gemm.cu.
 #include "common.cuh"
 #include "text_encoder.cuh"
 

@@ -101,7 +101,7 @@ __global__ void fold_ln_kernel(const __half* __restrict__ w, const __half* __res
   }
 }
 
-int grid_for(size_t n) { return static_cast<int>(std::min<size_t>((n + 255) / 256, 148 * 8)); }
+int grid_for(size_t n) { return static_cast<int>(std::min<size_t>((n + 255) / 256, num_sms() * 8)); }
 
 }  // namespace
 
@@ -800,10 +800,10 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
     // ---- body (SURVEY A.2 steps 2-6) ----
     // The unconditional and the conditional halves of the UNet batch never interact before the CFG++ mix, so the body
     // can be built as two launch plans (rows [0,B) and [B,2B)) that run on forked streams inside the captured graph,
-    // one half's GEMM fill / drain, norms and attention overlapping the other half's tensor work (CFGPP_SPLIT=1). That
-    // won 4 % while a GEMM launch lost ~10 us to fill / drain / epilogue; since the issue-loop and epilogue rewrites the
-    // full-batch kernels are faster per row and the single plan is ahead by ~1 % (tools/ab_split.sh), so it is the
-    // default.
+    // one half's GEMM fill / drain, norms and attention overlapping the other half's tensor work (CFGPP_SPLIT=1). The
+    // single full-batch plan stays the default, although on an H100 80GB HBM3 at a 400 W power limit the split measured
+    // 0.452 vs 0.440 img/s (SDXL 1024^2 NFE=50 batch 2, two alternating pairs); the split also turns the stream-K
+    // remainder split of the GEMMs off (gemm.cu streamk_enabled), and a change of default is not validated here.
     const int HW0 = H_ * W_;
     Act h0{g_dry ? nullptr : alloc_act(static_cast<size_t>(NB_) * HW0 * C0), C0};
     if (g_dry) workspace_bytes_ += 2 * static_cast<size_t>(NB_) * HW0 * C0 * sizeof(__half);

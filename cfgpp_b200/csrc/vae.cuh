@@ -1,6 +1,6 @@
 // cfgpp_b200 — AutoencoderKL DECODER executor (SURVEY.md §8 f2): `vae.decode(zt / scaling_factor).sample` of the
 // reference (latent_sdxl.py:155-164 with madebyollin/sdxl-vae-fp16-fix :44; latent_diffusion.py:123-129) on the
-// UNet's kernels: implicit-GEMM conv3x3 and 1x1 / linear GEMMs on tcgen05, GroupNorm(+SiLU), nearest-2x upsample,
+// UNet's kernels: implicit-GEMM conv3x3 and 1x1 / linear GEMMs on wgmma, GroupNorm(+SiLU), nearest-2x upsample,
 // conv_in (4 -> C) — plus the three small kernels of vae_kernels.cu. Structure = diffusers 0.27.1 `Decoder`:
 //   post_quant_conv 1x1 -> conv_in -> mid_block (resnet, single-head attention over all H*W tokens, resnet)
 //   -> up_blocks (layers_per_block + 1 resnets each, nearest-2x + conv between levels) -> GroupNorm + SiLU -> conv_out.

@@ -1,7 +1,7 @@
 // cfgpp_b200 — the three small kernels the AutoencoderKL decoder needs beside the UNet's GEMM / conv / norm kernels
 // (see vae.cuh): latent preparation (1 / scaling_factor + post_quant_conv 1x1), the row softmax of the single-head
-// mid-block attention (head dim = C = 512 does not fit the flash kernel's TMEM budget: S = Q K^T and O = P V run as
-// two tcgen05 GEMMs around it), and conv_out (C -> 3 channels, NHWC -> NCHW).
+// mid-block attention (head dim = C = 512 exceeds the flash kernel's head dims: S = Q K^T and O = P V run as
+// two wgmma GEMMs around it), and conv_out (C -> 3 channels, NHWC -> NCHW).
 #include "common.cuh"
 #include "vae.cuh"
 
@@ -267,7 +267,7 @@ namespace cfgpp {
 void run_vae_image_pad(const void* x, int x_is_half, __half* out, int B, int H, int W, cudaStream_t stream) {
   const size_t HW = static_cast<size_t>(H) * W;
   const size_t total = static_cast<size_t>(B) * 4 * HW;
-  const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 148 * 32));
+  const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, num_sms() * 32));
   launch_pdl(vae_image_pad_kernel, dim3(blocks), dim3(256), 0, stream, x, x_is_half, out, B, HW);
 }
 

@@ -1,7 +1,7 @@
 """NativeUNet — Python owner of one `cfgpp_handle` (one per process and GPU).
 
 Replaces `pipe.unet` of the reference (latent_diffusion.py:67, latent_sdxl.py:50,391) plus the arithmetic between
-UNet calls: everything below goes through the C ABI of libcfgpp_b200.so into hand-written sm_100a kernels.
+UNet calls: everything below goes through the C ABI of libcfgpp_b200.so into hand-written sm_90a kernels.
 PyTorch only owns the tensors and the stream. There is no eager / CPU fallback.
 """
 from __future__ import annotations
@@ -30,7 +30,7 @@ class NativeUNet:
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise nv.NativeError("the cfgpp_b200 backend runs on CUDA (sm_100a) only; use the oracle for CPU runs")
+            raise nv.NativeError("the cfgpp_b200 backend runs on CUDA (sm_90a) only; use the oracle for CPU runs")
         self.lib = nv.load()
         self._h = c_void_p()
         idx = self.device.index if self.device.index is not None else torch.cuda.current_device()

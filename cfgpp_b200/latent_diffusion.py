@@ -3,7 +3,7 @@
 Mirror of the reference's `latent_diffusion.py` solver API for the hot path: registry (:13-26), `StableDiffusion`
 base (:54-241: `alpha`, `get_text_embed`, `encode`, `decode`, `predict_noise`, `inversion`, `initialize_latent`),
 `ddim_cfg++` (:621-679) and `ddim_inversion_cfg++` (:882-957). Same names, argument meaning and errors; the UNet
-forward, CFG++ mix and DDIM update run in hand-written sm_100a CUDA behind include/cfgpp_b200.h.
+forward, CFG++ mix and DDIM update run in hand-written sm_90a CUDA behind include/cfgpp_b200.h.
 SURVEY §8 f1 (the rest of the CFG++ `--method` surface): `ddim_edit_cfg++` (:959-1010) on the same fused step modes;
 `euler_cfg++` (:682-724), `euler_a_cfg++` (:727-768), `dpm++_2s_a_cfg++` (:771-827), `dpm++_2m_cfg++` (:830-879) as
 fused VE-cast trajectories (kdiffusion.py: the ancestral ones with their noise drawn up front); the op-by-op torch

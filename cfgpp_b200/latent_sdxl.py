@@ -5,7 +5,7 @@ Mirror of the reference's `latent_sdxl.py` solver API for the hot path named by 
 (`SDXL.sample` :200-266, `reverse_process` :715-755 / :843-858 / :864-930, `predict_noise` :167-185,
 `initialize_latent` :268-299, `sigma_to_t` :333-346), same errors (ValueError for unknown / duplicate solver,
 AssertionError for Lightning with cfg_guidance != 1, NotImplementedError for unknown init methods) — but the UNet
-forward, the CFG++ guidance mix and the scheduler update run in hand-written sm_100a CUDA behind the C ABI
+forward, the CFG++ guidance mix and the scheduler update run in hand-written sm_90a CUDA behind the C ABI
 (include/cfgpp_b200.h). With `callback_fn=None` a whole trajectory is enqueued as NFE replays of one CUDA graph with
 no host synchronisation; with a callback the un-fused seam (`predict_noise` + `apply_step`) is used so that `z0t` /
 `zt` are materialised and may be replaced by the callback, exactly like the reference loop.
@@ -72,7 +72,7 @@ def resolve_state_dict(model_key: str, cfg: UNetConfig, device):
 def get_engine(model_key: str, cfg: UNetConfig, device, state_dict=None) -> NativeUNet:
     dev = torch.device(device)
     if dev.type != "cuda":
-        raise RuntimeError("cfgpp_b200 solvers run on CUDA (sm_100a) only — there is no CPU fallback on the product "
+        raise RuntimeError("cfgpp_b200 solvers run on CUDA (sm_90a) only — there is no CPU fallback on the product "
                            "path; the CPU eager baseline lives in oracle/ and bench.py")
     idx = dev.index if dev.index is not None else torch.cuda.current_device()
     key = (model_key, cfg.name, idx)

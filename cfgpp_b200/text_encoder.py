@@ -4,7 +4,7 @@ Replaces the reference's prompt conditioning: `self.text_encoder(ids)[0]` (SD v1
 `text_enc(ids, output_hidden_states=True)` -> `hidden_states[-2]` / `[-(clip_skip + 2)]` plus output `[0]` for the two
 SDXL encoders (latent_sdxl.py:77-128) — transformers `CLIPTextModel` (openai/clip-vit-large-patch14) and
 `CLIPTextModelWithProjection` (OpenCLIP ViT-bigG) — through the C ABI (`cfgpp_clip_*`): the projection / MLP GEMMs on
-the tcgen05 GEMM kernel, causal attention / embedding / activation kernels of csrc/text_kernels.cu. Weights use the
+the wgmma GEMM kernel, causal attention / embedding / activation kernels of csrc/text_kernels.cu. Weights use the
 transformers key names (`text_model.*`, `text_projection.weight`); no checkpoint or vocabulary exists offline, so the
 default solver path runs seeded synthetic weights behind the `HashTokenizer` stand-in (tokenizer.py) — pass
 `*.safetensors` + vocab / merges paths for the real models. There is no CPU fallback.
@@ -124,7 +124,7 @@ class NativeCLIPTextEncoder:
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise nv.NativeError("the cfgpp_b200 text encoder runs on CUDA (sm_100a) only; use the oracle for CPU runs")
+            raise nv.NativeError("the cfgpp_b200 text encoder runs on CUDA (sm_90a) only; use the oracle for CPU runs")
         idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
         self.device = torch.device("cuda", idx)
         self.lib = nv.load()

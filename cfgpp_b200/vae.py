@@ -3,7 +3,7 @@
 Replaces `self.vae.decode(zt / self.vae.config.scaling_factor).sample` of the reference (latent_sdxl.py:155-164 with
 `madebyollin/sdxl-vae-fp16-fix`, :44; latent_diffusion.py:123-129 with the SD v1.5 VAE, :64): post_quant_conv, the
 decoder's resnets / mid-block attention / upsamplers and conv_out run through the C ABI (`cfgpp_vae_*`) on the same
-tcgen05 conv / GEMM and GroupNorm kernels as the UNet. Weights use the diffusers AutoencoderKL key names
+wgmma conv / GEMM and GroupNorm kernels as the UNet. Weights use the diffusers AutoencoderKL key names
 (`post_quant_conv.*`, `decoder.*`); no checkpoint exists offline, so the default weights are seeded synthetic ones
 (a `*.safetensors` VAE file is loaded when given). The ENCODER half — `vae.encode(x).latent_dist.sample() *
 scaling_factor`, the front end of the inversion / editing solvers (latent_sdxl.py:151-152, latent_diffusion.py:117-121)
@@ -176,7 +176,7 @@ class NativeVAEDecoder:
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise nv.NativeError("the cfgpp_b200 VAE decoder runs on CUDA (sm_100a) only; use the oracle for CPU runs")
+            raise nv.NativeError("the cfgpp_b200 VAE decoder runs on CUDA (sm_90a) only; use the oracle for CPU runs")
         idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
         self.device = torch.device("cuda", idx)
         self.lib = nv.load()

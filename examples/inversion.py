@@ -2,7 +2,7 @@
 reconstruct / edit it —
     python -m examples.inversion --method ddim_inversion_cfg++ --NFE 10 --cfg_guidance 0.6 --prompt "a cat"
     python -m examples.inversion --method ddim_edit_cfg++ --prompt "a cat" --tgt_prompt "a dog"
-Runs on the Blackwell-native backend (both loops are fused CUDA-graph trajectories). Offline the UNet weights are
+Runs on the Hopper-native (sm_90a) backend (both loops are fused CUDA-graph trajectories). Offline the UNet weights are
 seeded synthetic and the text encoder / VAE are stand-ins (cfgpp_b200/conditioning.py): a plumbing check."""
 import argparse
 from pathlib import Path

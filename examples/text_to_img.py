@@ -1,6 +1,6 @@
 """CLI with the reference's flag surface (examples/text_to_img.py:14-24):
     python -m examples.text_to_img --model sdxl --method ddim_cfg++ --cfg_guidance 0.6 --NFE 50 --prompt "..."
-Runs on the Blackwell-native backend. Without checkpoints (offline) the UNet weights are seeded synthetic and the
+Runs on the Hopper-native (sm_90a) backend. Without checkpoints (offline) the UNet weights are seeded synthetic and the
 text encoder / VAE are stand-ins (cfgpp_b200/conditioning.py), so the PNG is only a plumbing check."""
 import argparse
 from pathlib import Path

@@ -6,7 +6,7 @@
  *                                                                                 latent_sdxl.py:167-185
  * which calls diffusers' UNet2DConditionModel.forward, followed by the hand-written CFG++ update of each solver
  * (latent_diffusion.py:660-666, 904-908; latent_sdxl.py:738-744, 902-919). This library replaces exactly that:
- * the batched (uncond+cond) UNet forward plus the guidance mix and scheduler update, as hand-written sm_100a CUDA.
+ * the batched (uncond+cond) UNet forward plus the guidance mix and scheduler update, as hand-written sm_90a CUDA.
  * The Python mirror of the solver API (cfgpp_b200/latent_diffusion.py, latent_sdxl.py) binds these symbols with
  * ctypes; INTEGRATION.md shows the stub a reference maintainer would add.
  *

@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an sm_90a GPU; select with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

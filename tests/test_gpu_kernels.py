@@ -1,6 +1,6 @@
 """Kernel-level parity (through the C ABI) against torch fp32 references of the same op, with the reference's
 rounding points (fp16(acc+bias) then fp16 add of the residual / time embedding, fp32 norms rounded once).
-Gates are ~5x the error observed on B200 (printed by every test; `pytest -s` shows them): GEMM / conv observe ~3e-5
+Gates are ~5x the error observed on the GPU (printed by every test; `pytest -s` shows them): GEMM / conv observe ~3e-5
 (both sides round the same fp32 sum to fp16, so only accumulation-order flips of the last bit remain) -> 2e-4;
 attention observes 2.5-2.9e-4 (P is rounded to fp16 before PV) -> 1.5e-3; norms observe 5-8e-6 -> 5e-5."""
 import pytest
@@ -62,11 +62,11 @@ def test_linear(M, N, K, hb, ha, bn):
                                               (4096, 3840, 1280, False), (2048, 640, 2560, False),
                                               (8192, 1280, 1280, False), (5000, 1280, 640, False)])
 def test_linear_streamk_shapes_and_repeatability(M, N, K, geglu_like):
-    """Shapes whose tile count is not a multiple of the cluster count CAN take the stream-K remainder path (partials
-    parked in the workspace by other clusters, self-resetting flags; on by default for the convolutions, for linear
-    layers with CFGPP_STREAMK_LINEAR=1 CFGPP_STREAMK_MIN=0 CFGPP_STREAMK_PIECE=0 — the round-2 GPU runs exercise
-    both settings): result vs the fp32 reference, and 12 back-to-back launches must be bit-identical (fixed summation
-    order; flags re-armed by the kernel itself)."""
+    """Shapes whose tile count is not a multiple of the CTA count CAN take the stream-K remainder path (partials
+    parked in the workspace by other CTAs, self-resetting flags; on by default for the convolutions, for linear layers
+    with CFGPP_STREAMK_LINEAR=1 CFGPP_STREAMK_MIN=0 CFGPP_STREAMK_PIECE=0, which
+    test_linear_streamk_forced_in_subprocess sets): result vs the fp32 reference, and 12 back-to-back launches must be
+    bit-identical (fixed summation order; flags re-armed by the kernel itself)."""
     from cfgpp_b200 import _native as nv
     g = torch.Generator().manual_seed(M + N + K)
     a, w, bias, res = rnd(g, M, K), rnd(g, N, K, scale=K ** -0.5), rnd(g, N), rnd(g, M, N)
@@ -74,6 +74,22 @@ def test_linear_streamk_shapes_and_repeatability(M, N, K, geglu_like):
     gate(f'linear(stream-K) {M}x{N}x{K}', first, ref_linear(a, w, bias, res, 1), TOL_GEMM)
     for _ in range(12):
         assert torch.equal(nv.op_linear(a, w, bias, res, 1), first)
+
+
+def test_linear_streamk_forced_in_subprocess():
+    """The stream-K split is off for linear layers by default; re-run the shapes above in a child process with it
+    forced on (the dispatch reads the switches once per process), so the split's partial / fix-up path is covered."""
+    import os
+    import subprocess
+    import sys
+    if os.environ.get("CFGPP_STREAMK_LINEAR") == "1":
+        pytest.skip("already inside the child")
+    env = dict(os.environ, CFGPP_STREAMK_LINEAR="1", CFGPP_STREAMK_MIN="0", CFGPP_STREAMK_PIECE="0")
+    r = subprocess.run([sys.executable, "-m", "pytest", __file__, "-q", "-m", "gpu", "-p", "no:cacheprovider", "-k",
+                        "test_linear_streamk_shapes_and_repeatability", "-x"], env=env, capture_output=True, text=True,
+                       timeout=600)
+    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
+    assert "6 passed" in r.stdout, r.stdout[-2000:]
 
 
 def test_linear_dual_source_and_geglu():
@@ -170,11 +186,9 @@ def test_conv3x3(B, H, W, Cin, Cout, ht, hr):
 
 @pytest.mark.parametrize("B,H,Nq,Nkv", [(1, 1, 128, 128), (1, 4, 64, 64), (2, 5, 1024, 1024), (1, 10, 4096, 4096),
                                         (4, 20, 1024, 77), (1, 2, 200, 333), (1, 1, 1, 1),
-                                        # single-KV-tile (cross-attention) kernel: 80- and 128-column variants,
-                                        # uneven tiles per CTA, a partial last query tile
+                                        # one KV tile (cross-attention): partial KV tiles, a partial last query tile
                                         (4, 10, 4096, 77), (1, 5, 1024, 128), (2, 3, 520, 100), (1, 2, 256, 5),
-                                        # persistent self-attention kernel (>= 2 query tiles per SM): the bench shape,
-                                        # ragged Nq / Nkv, ranges that straddle heads and batches, exactly 2 per SM
+                                        # the bench shape, ragged Nq / Nkv, many heads
                                         (4, 20, 1024, 1024), (3, 13, 1100, 1000), (1, 37, 1024, 640), (2, 31, 700, 333)])
 def test_attention(B, H, Nq, Nkv):
     from cfgpp_b200 import _native as nv
@@ -240,20 +254,3 @@ def test_layernorm(M, Cc):
     x, gamma, beta = rnd(g, M, Cc, scale=3.0, shift=1.0), rnd(g, Cc, scale=0.2, shift=1.0), rnd(g, Cc, scale=0.2)
     ref = torch.nn.functional.layer_norm(x.float(), (Cc,), gamma.float(), beta.float(), 1e-5).half()
     gate(f'layernorm {M}x{Cc}', nv.op_layernorm(x, gamma, beta), ref, TOL_NORM)
-
-
-@pytest.mark.parametrize("switch", ["CFGPP_PATTN=1", "CFGPP_ATTN_POLY=4", "CFGPP_ATTN_ROWSUM_MMA=1", "CFGPP_ATTN_PBUF=2"])
-def test_attention_opt_in_variants_in_subprocess(switch):
-    """The opt-in attention variants of round 2 — persistent kernel, polynomial exp2 on the FMA pipe, row sums on the
-    tensor pipe, double-buffered P: all measured no faster than the default, DESIGN.md §7 — stay validated: the
-    attention parity tests re-run in a child process with the switch set (the dispatch reads it once per process)."""
-    import os
-    import subprocess
-    import sys
-    if os.environ.get("CFGPP_ATTN_CHILD") == "1":
-        pytest.skip("already inside the child")
-    k, v = switch.split("=")
-    env = dict(os.environ, CFGPP_ATTN_CHILD="1", **{k: v})
-    r = subprocess.run([sys.executable, "-m", "pytest", __file__, "-q", "-m", "gpu", "-k",
-                        "test_attention and not subprocess", "-x"], env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]

@@ -23,7 +23,7 @@ for (M, N, K, res, bn) in [(4096, 1280, 1280, False, 0), (4096, 1280, 1280, True
     bias = torch.randn(N, generator=g).half().to(dev) if res else None
     addend = torch.randn(M, N, generator=g).half().to(dev) if res else None
     out = torch.empty(M, N, dtype=torch.float16, device=dev)
-    buf = (C.c_ulonglong * (16 * 148))()
+    buf = (C.c_ulonglong * (16 * 132))()
     grid = C.c_int()
     nv.check(lib.cfgpp_dbg_linear_timeline(nv.ptr(a), C.c_int(K), nv.ptr(w), C.c_int(M), C.c_int(N), C.c_int(K),
                                            nv.ptr(bias), nv.ptr(addend), nv.ptr(out), C.c_int(bn), C.c_int(10), buf,
