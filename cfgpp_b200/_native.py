@@ -58,21 +58,81 @@ def stream_ptr() -> c_void_p:
 # ------------------------------------------------------------------------------------------------
 # operator-level wrappers (one kernel launch each) — used by tests and micro-benchmarks
 # ------------------------------------------------------------------------------------------------
+def _linear_out(out, M, n_out, device):
+    if out is None:
+        return torch.empty((M, n_out), dtype=torch.float16, device=device)
+    assert out.shape == (M, n_out) and out.dtype == torch.float16 and out.is_contiguous()
+    return out
+
+
 def op_linear(a: torch.Tensor, w: torch.Tensor, bias=None, addend=None, add_rows_per_group: int = 1,
-              a2: torch.Tensor | None = None, geglu: bool = False, force_bn: int = 0) -> torch.Tensor:
-    """out = epilogue(cat([a, a2], -1) @ w.T); a [M,K1] fp16, w [N,K] fp16 (already packed for GEGLU)."""
+              a2: torch.Tensor | None = None, geglu: bool = False, force_bn: int = 0,
+              out: torch.Tensor | None = None) -> torch.Tensor:
+    """out = epilogue(cat([a, a2], -1) @ w.T); a [M,K1] fp16, w [N,K] fp16 (already packed for GEGLU). `out` may be
+    given, also as the residual `addend` itself (in-place residual add)."""
     lib = load()
     M, K1 = a.shape
     K = K1 + (a2.shape[1] if a2 is not None else 0)
     N = w.shape[0]
     assert w.shape[1] == K and a.dtype == torch.float16 and w.dtype == torch.float16
     n_out = N // 2 if geglu else N
-    out = torch.empty((M, n_out), dtype=torch.float16, device=a.device)
+    out = _linear_out(out, M, n_out, a.device)
     check(lib.cfgpp_op_linear(ptr(a), c_int(a.stride(0)), ptr(a2), c_int(a2.stride(0) if a2 is not None else 0),
                               c_int(K1), ptr(w), c_int(M), c_int(N), c_int(K), ptr(bias), ptr(addend),
                               c_int(addend.stride(0) if addend is not None else 0), c_int(add_rows_per_group),
                               ptr(out), c_int(n_out), c_int(1 if geglu else 0), c_int(force_bn), stream_ptr()))
     return out
+
+
+def op_linear_stats(a: torch.Tensor, w: torch.Tensor, bn: int, bias=None, addend=None, add_rows_per_group: int = 1,
+                    out: torch.Tensor | None = None):
+    """op_linear that also emits the LayerNorm-fold row statistics of its fp16 output (a transformer block's residual
+    producer). Returns (out, stats): stats [2 * ceil(N / bn), M, 2] fp32 (sum, sum of squares), part 2 j + h over
+    columns [j bn + h bn / 2, j bn + (h + 1) bn / 2)."""
+    lib = load()
+    M, K = a.shape
+    N = w.shape[0]
+    assert a.is_contiguous() and w.shape[1] == K and bn > 0
+    out = _linear_out(out, M, N, a.device)
+    stats = torch.empty((2 * ((N + bn - 1) // bn), M, 2), dtype=torch.float32, device=a.device)
+    check(lib.cfgpp_op_linear_lnfold(ptr(a), ptr(w), c_int(M), c_int(N), c_int(K), ptr(bias), ptr(addend),
+                                     c_int(addend.stride(0) if addend is not None else 0), c_int(add_rows_per_group),
+                                     ptr(out), c_int(N), c_int(0), c_int(bn), ptr(stats), c_void_p(0), c_int(0),
+                                     c_float(0.0), c_void_p(0), c_void_p(0), stream_ptr()))
+    return out, stats
+
+
+def op_linear_lnfold(h: torch.Tensor, wf: torch.Tensor, s: torch.Tensor, t: torch.Tensor, stats: torch.Tensor,
+                     eps: float = 1e-5, geglu: bool = False, force_bn: int = 0, ln_parts: int | None = None,
+                     out: torch.Tensor | None = None) -> torch.Tensor:
+    """LayerNorm(h) @ w.T + bias as the folded GEMM: h [M,C] fp16, (wf, s, t) from op_fold_ln, stats [parts, M, 2]
+    fp32 row (sum, sum of squares) partials of h (op_linear_stats, or any split of the columns)."""
+    lib = load()
+    M, K = h.shape
+    N = wf.shape[0]
+    parts = stats.shape[0] if ln_parts is None else ln_parts
+    assert h.is_contiguous() and wf.shape[1] == K and stats.shape[1:] == (M, 2) and stats.dtype == torch.float32
+    assert s.dtype == torch.float32 and t.dtype == torch.float32 and s.shape == t.shape == (N,)
+    n_out = N // 2 if geglu else N
+    out = _linear_out(out, M, n_out, h.device)
+    check(lib.cfgpp_op_linear_lnfold(ptr(h), ptr(wf), c_int(M), c_int(N), c_int(K), c_void_p(0), c_void_p(0), c_int(0),
+                                     c_int(1), ptr(out), c_int(n_out), c_int(1 if geglu else 0), c_int(force_bn),
+                                     c_void_p(0), ptr(stats), c_int(parts), c_float(eps), ptr(s), ptr(t),
+                                     stream_ptr()))
+    return out
+
+
+def op_fold_ln(w: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, bias: torch.Tensor | None = None):
+    """The LayerNorm fold of w [N,K] (the production weight preparation): (wf = fp16(w * gamma), s [N] fp32 =
+    sum_k wf, t [N] fp32 = w @ beta + bias)."""
+    lib = load()
+    N, K = w.shape
+    wf = torch.empty_like(w)
+    s = torch.empty(N, dtype=torch.float32, device=w.device)
+    t = torch.empty(N, dtype=torch.float32, device=w.device)
+    check(lib.cfgpp_op_fold_ln(ptr(w), ptr(gamma), ptr(beta), ptr(bias), ptr(wf), ptr(s), ptr(t), c_int(N), c_int(K),
+                               stream_ptr()))
+    return wf, s, t
 
 
 def op_conv3x3(x_nhwc: torch.Tensor, w_packed: torch.Tensor, bias=None, addend=None,

@@ -22,6 +22,38 @@ CFGPP_API int cfgpp_op_linear(const void* a, int lda, const void* a2, int lda2, 
   });
 }
 
+CFGPP_API int cfgpp_op_linear_lnfold(const void* a, const void* w, int M, int N, int K, const void* bias,
+                                     const void* addend, int ld_add, int add_rows_per_group, void* out, int ldc,
+                                     int geglu, int force_bn, float* stats_out, const float* stats_in, int ln_parts,
+                                     float ln_eps, const float* ln_s, const float* ln_t, void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE((stats_out != nullptr) != (stats_in != nullptr), "exactly one of stats_out / stats_in");
+    CFGPP_REQUIRE(stats_out == nullptr || force_bn != 0, "a statistics producer needs an explicit tile width");
+    CFGPP_REQUIRE(stats_in == nullptr || (ln_parts >= 1 && ln_s && ln_t), "a LayerNorm-fold consumer needs parts, s, t");
+    GemmOp op = make_linear_op((const __half*)a, K, nullptr, 0, 0, (const __half*)w, M, N, K, (const __half*)bias,
+                               (const __half*)addend, ld_add, add_rows_per_group, (__half*)out, ldc, geglu != 0,
+                               force_bn);
+    op.p.stats_out = stats_out;
+    if (stats_in) {
+      op.p.stats_in = stats_in;
+      op.p.ln_parts = ln_parts;
+      op.p.ln_inv_c = 1.0f / static_cast<float>(K);
+      op.p.ln_eps = ln_eps;
+      op.p.ln_s = ln_s;
+      op.p.ln_t = ln_t;
+    }
+    run_gemm_op(op, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_fold_ln(const void* w, const void* gamma, const void* beta, const void* bias, void* wf,
+                               float* s, float* t, int N, int K, void* stream) {
+  return guarded([&] {
+    run_fold_ln((const __half*)w, (const __half*)gamma, (const __half*)beta, (const __half*)bias, (__half*)wf, s, t, N,
+                K, (cudaStream_t)stream);
+  });
+}
+
 // Debug aid (not in the public header): run the linear op `iters` times and return per-CTA timestamps of the last run.
 CFGPP_API int cfgpp_dbg_linear_timeline(const void* a, int lda, const void* w, int M, int N, int K, const void* bias,
                                         const void* addend, void* out, int force_bn, int iters,

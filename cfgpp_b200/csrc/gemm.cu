@@ -824,6 +824,8 @@ GemmOp make_conv3x3_op(const __half* x, int B, int H, int W, int Cin, const __ha
 void run_gemm_op(const GemmOp& op, cudaStream_t stream) {
   CFGPP_REQUIRE(!(op.p.stats_in && (op.p.addend || op.p.stats_out)),
                 "a LayerNorm-fold consumer GEMM takes no addend and emits no row statistics");
+  CFGPP_REQUIRE(!(op.p.stats_in && op.p.bias),
+                "a LayerNorm-fold consumer GEMM takes its bias inside t_n (run_fold_ln), not as a bias vector");
   CFGPP_REQUIRE(!(op.p.geglu && (op.p.addend || op.p.stats_out)), "the GEGLU epilogue takes no addend / statistics");
   if (op.p.geglu) return launch<256, true>(op, stream);
   switch (op.bn) {

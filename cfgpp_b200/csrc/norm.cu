@@ -4,9 +4,12 @@
 // in fp32 from the fp16 input, and the result is rounded to fp16 exactly once — the point where the reference's
 // fp32 norm output is cast for the following conv / linear.
 //
-// GroupNorm is two launches: (1) per-(sample, pixel-chunk) partial (sum, sum^2) per group — deterministic, no
-// atomics in global memory; (2) apply, which reduces the partials on the fly. Both take an optional second source
-// so that torch.cat([h, skip], dim=1) of the up-blocks is never materialised un-normalised.
+// GroupNorm is two launches: (1) per-(sample, pixel-chunk) partial (sum, sum^2) per group, shifted by a pivot value
+// of the group — deterministic, no atomics in global memory; (2) apply, which reduces the partials on the fly. Both
+// take an optional second source so that torch.cat([h, skip], dim=1) of the up-blocks is never materialised
+// un-normalised.
+//
+// The LayerNorm fold of the transformer blocks (see GemmParams in gemm.cuh) prepares its weights here too.
 #include "common.cuh"
 #include "ops.cuh"
 
@@ -27,62 +30,79 @@ CFGPP_DEVICE uint4 load_vec(const GnSrc& s, size_t pix, int c) {  // c multiple 
   return *reinterpret_cast<const uint4*>(s.x2 + pix * s.C2 + (c - s.C1));
 }
 
+// Shift of group g's sums: its first channel at pixel 0 of the sample. Sums of (x - K) and (x - K)^2 keep
+// var = Q / n - (S / n)^2 free of the cancellation E[x^2] - E[x]^2 suffers when |mean| >> std (fp32 over up to 4 M
+// elements per group); both kernels load the same K.
+CFGPP_DEVICE float gn_pivot(const GnSrc& s, size_t pix0, int g, int cpg) {
+  const int c = g * cpg;
+  return __half2float(c < s.C1 ? s.x1[pix0 * s.C1 + c] : s.x2[pix0 * s.C2 + (c - s.C1)]);
+}
+
 // grid (nchunk, B); block = vpp * k threads (vpp = C / 8 vectors per pixel) so a thread keeps one channel vector.
+// A thread walks up to 2048 pixels of a chunk (VAE levels of 1024^2 pixels); its sums are cascaded (fp32 runs of
+// kRun steps in registers, folded into the thread's shared-memory slot) so that no rounding chain is longer than ~64
+// additions.
 __global__ void gn_stats_kernel(GnSrc src, int HW, int C, int px_per_block, float* __restrict__ partial) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float sm[];  // [pstep][C] sums, then [pstep][C] sums of squares (one slot per thread: no atomics)
   const int vpp = C >> 3;
+  const int cpg = C / GROUPS;
   const int b = blockIdx.y;
   const int chunk = blockIdx.x;
   const int vec = threadIdx.x % vpp;
   const int prow = threadIdx.x / vpp;
   const int pstep = blockDim.x / vpp;
-  float s[8], q[8];
+  float s[8], q[8], piv[8];
+  float* sq = sm + pstep * C;
+  float* my_s = sm + prow * C + vec * 8;
+  float* my_q = sq + prow * C + vec * 8;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) s[i] = q[i] = 0.f;
+  for (int i = 0; i < 8; ++i) {
+    s[i] = q[i] = my_s[i] = my_q[i] = 0.f;
+    piv[i] = gn_pivot(src, static_cast<size_t>(b) * HW, (vec * 8 + i) / cpg, cpg);
+  }
+  // x - K is exact (two nearby fp16 values), and so is its square (<= 24 significant bits)
+  auto accumulate = [&](const uint4& u) {
+    const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float2 f = __half22float2(h[i]);
+      const float d0 = f.x - piv[2 * i], d1 = f.y - piv[2 * i + 1];
+      s[2 * i] += d0;
+      q[2 * i] += d0 * d0;
+      s[2 * i + 1] += d1;
+      q[2 * i + 1] += d1 * d1;
+    }
+  };
+  auto fold = [&]() {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      my_s[i] += s[i];
+      my_q[i] += q[i];
+      s[i] = q[i] = 0.f;
+    }
+  };
   const int p0 = chunk * px_per_block;
   const int pend = min(px_per_block, HW - p0);
   const size_t base = static_cast<size_t>(b) * HW + p0;
   constexpr int U = 4;  // independent 16 B loads in flight per thread
-  int pp = prow;
+  constexpr int kRun = 8;  // steps (U pixels each) per fp32 run
+  int pp = prow, run = 0;
   for (; pp + (U - 1) * pstep < pend; pp += U * pstep) {
     uint4 u[U];
 #pragma unroll
     for (int j = 0; j < U; ++j) u[j] = load_vec(src, base + pp + j * pstep, vec * 8);
 #pragma unroll
-    for (int j = 0; j < U; ++j) {
-      const __half2* h = reinterpret_cast<const __half2*>(&u[j]);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(h[i]);
-        s[2 * i] += f.x;
-        q[2 * i] += f.x * f.x;
-        s[2 * i + 1] += f.y;
-        q[2 * i + 1] += f.y * f.y;
-      }
+    for (int j = 0; j < U; ++j) accumulate(u[j]);
+    if (++run == kRun) {
+      fold();
+      run = 0;
     }
   }
-  for (; pp < pend; pp += pstep) {
-    const uint4 u = load_vec(src, base + pp, vec * 8);
-    const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float2 f = __half22float2(h[i]);
-      s[2 * i] += f.x;
-      q[2 * i] += f.x * f.x;
-      s[2 * i + 1] += f.y;
-      q[2 * i + 1] += f.y * f.y;
-    }
-  }
-  float* sq = sm + pstep * C;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    sm[prow * C + vec * 8 + i] = s[i];
-    sq[prow * C + vec * 8 + i] = q[i];
-  }
+  for (; pp < pend; pp += pstep) accumulate(load_vec(src, base + pp, vec * 8));
+  fold();
   __syncthreads();
-  const int cpg = C / GROUPS;
   if (threadIdx.x < GROUPS) {  // fixed summation order -> bit-reproducible statistics
     float a = 0.f, bsum = 0.f;
     for (int r = 0; r < pstep; ++r)
@@ -97,13 +117,14 @@ __global__ void gn_stats_kernel(GnSrc src, int HW, int C, int px_per_block, floa
 }
 
 // grid (nchunk, B); block = vpp * k threads: a thread owns one 8-channel vector, so the per-channel affine
-// ((x - mean) * rstd) * gamma + beta (the reference's evaluation order) uses 32 registers set up once per thread.
+// (x - mean) * rstd * gamma + beta = (x - K) * a + c (a = rstd * gamma, c = beta - (mean - K) * a) uses 24 registers
+// set up once per thread. x - K is exact (two nearby fp16 values), so a large mean costs no fp32 rounding of its own.
 __global__ void gn_apply_kernel(GnSrc src, int HW, int C, int px_per_block, const float* __restrict__ partial,
                                 int nchunk, const __half* __restrict__ gamma, const __half* __restrict__ beta,
                                 float eps, int silu, __half* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
-  __shared__ float s_mean[GROUPS], s_rstd[GROUPS];
+  __shared__ float s_piv[GROUPS], s_dm[GROUPS], s_rstd[GROUPS];
   __shared__ float2 s_part[8][GROUPS];
   const int b = blockIdx.y;
   // Cross-chunk reduction of the partial sums, spread over 8 x 32 threads (each sums every 8th chunk, loads
@@ -128,10 +149,12 @@ __global__ void gn_apply_kernel(GnSrc src, int HW, int C, int px_per_block, cons
       a += s_part[part][threadIdx.x].x;
       q += s_part[part][threadIdx.x].y;
     }
+    // the partials are sums of (x - K), (x - K)^2 with the group's pivot K (gn_pivot): mean = K + dm
     const float n = static_cast<float>(HW) * (C / GROUPS);
-    const float mean = a / n;
-    const float var = fmaxf(q / n - mean * mean, 0.f);
-    s_mean[threadIdx.x] = mean;
+    const float dm = a / n;
+    const float var = fmaxf(q / n - dm * dm, 0.f);
+    s_piv[threadIdx.x] = gn_pivot(src, static_cast<size_t>(b) * HW, threadIdx.x, C / GROUPS);
+    s_dm[threadIdx.x] = dm;
     s_rstd[threadIdx.x] = rsqrtf(var + eps);
   }
   __syncthreads();
@@ -141,22 +164,17 @@ __global__ void gn_apply_kernel(GnSrc src, int HW, int C, int px_per_block, cons
   const int prow = threadIdx.x / vpp;
   const int pstep = blockDim.x / vpp;
   const int c0 = vec * 8;
-  float scale[8], shift[8];  // rstd / mean of the group each of this thread's 8 channels belongs to
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const int g = (c0 + k) / cpg;
-    scale[k] = s_rstd[g];
-    shift[k] = s_mean[g];
-  }
   const uint4 ug = *reinterpret_cast<const uint4*>(gamma + c0);
   const uint4 ub = *reinterpret_cast<const uint4*>(beta + c0);
   const __half* hg = reinterpret_cast<const __half*>(&ug);
   const __half* hb = reinterpret_cast<const __half*>(&ub);
-  float gm[8], bt[8];
+  float piv[8], sc[8], sh[8];  // pivot K, a, c of each of this thread's 8 channels
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
-    gm[k] = __half2float(hg[k]);
-    bt[k] = __half2float(hb[k]);
+    const int g = (c0 + k) / cpg;
+    piv[k] = s_piv[g];
+    sc[k] = s_rstd[g] * __half2float(hg[k]);
+    sh[k] = __half2float(hb[k]) - s_dm[g] * sc[k];
   }
   const int p0 = blockIdx.x * px_per_block;
   const int pend = min(px_per_block, HW - p0);
@@ -167,7 +185,7 @@ __global__ void gn_apply_kernel(GnSrc src, int HW, int C, int px_per_block, cons
     float y[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      float v = (__half2float(hx[k]) - shift[k]) * scale[k] * gm[k] + bt[k];
+      float v = (__half2float(hx[k]) - piv[k]) * sc[k] + sh[k];
       if (silu) v = silu_f(v);
       y[k] = v;
     }
@@ -256,6 +274,33 @@ __global__ void layernorm_kernel(const __half* __restrict__ x, int M, int C, con
   }
 }
 
+// LayerNorm fold (see GemmParams): one warp per (packed) weight row n
+__global__ void fold_ln_kernel(const __half* __restrict__ w, const __half* __restrict__ gamma,
+                               const __half* __restrict__ beta, const __half* __restrict__ bias,
+                               __half* __restrict__ wf, float* __restrict__ s_out, float* __restrict__ t_out, int N,
+                               int K) {
+  const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (n >= N) return;
+  float s = 0.f, t = 0.f;
+  for (int k = lane; k < K; k += 32) {
+    const float wv = __half2float(w[static_cast<size_t>(n) * K + k]);
+    const __half wg = __float2half_rn(wv * __half2float(gamma[k]));
+    wf[static_cast<size_t>(n) * K + k] = wg;
+    s += __half2float(wg);
+    t += __half2float(beta[k]) * wv;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s += __shfl_xor_sync(0xffffffffu, s, o);
+    t += __shfl_xor_sync(0xffffffffu, t, o);
+  }
+  if (lane == 0) {
+    s_out[n] = s;
+    t_out[n] = t + (bias ? __half2float(bias[n]) : 0.f);
+  }
+}
+
 }  // namespace
 
 // up to 128 pixel chunks per sample (the partial-sum buffer holds 128) so that even the 32x32 level launches
@@ -279,7 +324,8 @@ void run_groupnorm(const __half* x1, int C1, const __half* x2, int C2, int B, in
   if (k < 1) k = 1;
   const int threads = vpp * k;
   CFGPP_REQUIRE(threads <= 1024, "GroupNorm channel count too large");
-  launch_pdl(gn_stats_kernel, dim3(nchunk, B), dim3(threads), 2 * static_cast<size_t>(k) * C * sizeof(float), stream, src, HW, C,
+  const size_t stats_smem = 2 * static_cast<size_t>(k) * C * sizeof(float);
+  launch_pdl(gn_stats_kernel, dim3(nchunk, B), dim3(threads), stats_smem, stream, src, HW, C,
              ppb, partial);
   launch_pdl(gn_apply_kernel, dim3(nchunk, B), dim3(threads), 0, stream, src, HW, C, ppb, partial, nchunk, gamma, beta, eps,
                                                            silu ? 1 : 0, out);
@@ -290,6 +336,13 @@ void run_layernorm(const __half* x, int M, int C, const __half* gamma, const __h
   CFGPP_REQUIRE(C % 8 == 0 && C <= 2048, "LayerNorm needs C % 8 == 0 and C <= 2048");
   const int warps = 8;
   launch_pdl(layernorm_kernel, dim3((M + warps - 1) / warps), dim3(warps * 32), 0, stream, x, M, C, gamma, beta, eps, out);
+}
+
+void run_fold_ln(const __half* w, const __half* gamma, const __half* beta, const __half* bias, __half* wf, float* s,
+                 float* t, int N, int K, cudaStream_t stream) {
+  const int warps = 8;
+  fold_ln_kernel<<<(N + warps - 1) / warps, warps * 32, 0, stream>>>(w, gamma, beta, bias, wf, s, t, N, K);
+  CFGPP_CHECK_CUDA(cudaGetLastError());
 }
 
 }  // namespace cfgpp

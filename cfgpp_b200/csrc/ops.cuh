@@ -14,6 +14,10 @@ void run_groupnorm(const __half* x1, int C1, const __half* x2, int C2, int B, in
                    const __half* beta, float eps, bool silu, float* partial, __half* out, cudaStream_t stream);
 void run_layernorm(const __half* x, int M, int C, const __half* gamma, const __half* beta, float eps, __half* out,
                    cudaStream_t stream);
+// LayerNorm fold of a weight w [N][K] (see GemmParams): wf = fp16(w * gamma), s[n] = sum_k wf[n,k],
+// t[n] = sum_k beta[k] w[n,k] + bias[n] (bias may be null); s, t fp32.
+void run_fold_ln(const __half* w, const __half* gamma, const __half* beta, const __half* bias, __half* wf, float* s,
+                 float* t, int N, int K, cudaStream_t stream);
 
 // ---- elementwise.cu ----------------------------------------------------------------------------------------
 // diffusers get_timestep_embedding(flip_sin_to_cos=True, shift 0): out[i, col_off + (cos | sin)], fp16.

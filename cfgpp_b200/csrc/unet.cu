@@ -74,33 +74,6 @@ __global__ void pack_heads_cols_kernel(const __half* __restrict__ in, __half* __
   }
 }
 
-// LayerNorm fold (see GemmParams): one warp per (packed) weight row n
-__global__ void fold_ln_kernel(const __half* __restrict__ w, const __half* __restrict__ gamma,
-                               const __half* __restrict__ beta, const __half* __restrict__ bias,
-                               __half* __restrict__ wf, float* __restrict__ s_out, float* __restrict__ t_out, int N,
-                               int K) {
-  const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (n >= N) return;
-  float s = 0.f, t = 0.f;
-  for (int k = lane; k < K; k += 32) {
-    const float wv = __half2float(w[static_cast<size_t>(n) * K + k]);
-    const __half wg = __float2half_rn(wv * __half2float(gamma[k]));
-    wf[static_cast<size_t>(n) * K + k] = wg;
-    s += __half2float(wg);
-    t += __half2float(beta[k]) * wv;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    s += __shfl_xor_sync(0xffffffffu, s, o);
-    t += __shfl_xor_sync(0xffffffffu, t, o);
-  }
-  if (lane == 0) {
-    s_out[n] = s;
-    t_out[n] = t + (bias ? __half2float(bias[n]) : 0.f);
-  }
-}
-
 int grid_for(size_t n) { return static_cast<int>(std::min<size_t>((n + 255) / 256, num_sms() * 8)); }
 
 }  // namespace
@@ -284,10 +257,8 @@ Unet::FoldedLN Unet::folded_ln(const std::string& cache_key, const __half* w_pac
   f.w = alloc_weight(static_cast<size_t>(N) * K);
   f.s = reinterpret_cast<float*>(alloc_weight(static_cast<size_t>(N) * 2));
   f.t = reinterpret_cast<float*>(alloc_weight(static_cast<size_t>(N) * 2));
-  const int warps = 8;
-  fold_ln_kernel<<<(N + warps - 1) / warps, warps * 32>>>(w_packed, plain(norm_prefix + ".weight"),
-                                                           plain(norm_prefix + ".bias"), bias_packed, f.w, f.s, f.t, N, K);
-  CFGPP_CHECK_CUDA(cudaGetLastError());
+  run_fold_ln(w_packed, plain(norm_prefix + ".weight"), plain(norm_prefix + ".bias"), bias_packed, f.w, f.s, f.t, N, K,
+              nullptr);
   fold_cache_[cache_key] = f;
   return f;
 }

@@ -216,6 +216,21 @@ int cfgpp_clip_stats(cfgpp_clip_handle* h, double* flops, size_t* workspace_byte
 int cfgpp_op_linear(const void* a, int lda, const void* a2, int lda2, int k_split, const void* w, int M, int N, int K,
                     const void* bias, const void* addend, int ld_add, int add_rows_per_group, void* out, int ldc,
                     int geglu, int force_bn, void* stream);
+/* The LayerNorm-fold variants of cfgpp_op_linear (a [M,K], single source), exactly one of:
+ *  stats_out (producer): besides out, writes per-row partial (sum, sum of squares) of the fp16 output as
+ *    [2 * ceil(N / force_bn)][M] float2 — part 2 j + h covers columns [j BN + h BN / 2, j BN + (h + 1) BN / 2) of N
+ *    block j; force_bn is required. out may alias addend (in-place residual add).
+ *  stats_in (consumer): w is the folded weight of cfgpp_op_fold_ln, the epilogue applies
+ *    rstd * acc - rstd * mean * ln_s[n] + ln_t[n] with mean / rstd over C = K from the first ln_parts parts of
+ *    stats_in ([ln_parts][M] float2); bias and addend must be null (the bias is inside ln_t). */
+int cfgpp_op_linear_lnfold(const void* a, const void* w, int M, int N, int K, const void* bias, const void* addend,
+                           int ld_add, int add_rows_per_group, void* out, int ldc, int geglu, int force_bn,
+                           float* stats_out, const float* stats_in, int ln_parts, float ln_eps, const float* ln_s,
+                           const float* ln_t, void* stream);
+/* LayerNorm fold of w [N,K] fp16 with LayerNorm(K) gamma / beta (fp16) and an optional bias [N]: wf = fp16(w * gamma)
+ * [N,K] fp16, s[n] = sum_k wf[n,k], t[n] = sum_k beta[k] w[n,k] + bias[n] (fp32). */
+int cfgpp_op_fold_ln(const void* w, const void* gamma, const void* beta, const void* bias, void* wf, float* s, float* t,
+                     int N, int K, void* stream);
 int cfgpp_op_conv3x3(const void* x, int B, int H, int W, int Cin, const void* w, int Cout, const void* bias,
                      const void* addend, int ld_add, int add_rows_per_group, void* out, int force_bn, void* stream);
 /* Downsample2D: 3x3, stride 2 on NHWC x [B,H,W,Cin] (even H, W) -> [B,H/2,W/2,Cout]; the A tile is fetched by TMA with
