@@ -208,3 +208,20 @@ def op_cfgpp_step(eps_uc: torch.Tensor, eps_c: torch.Tensor, method: int, coef, 
     check(lib.cfgpp_op_cfgpp_step(ptr(eps_uc), ptr(eps_c), c_int(z.numel()), c_int(method), c_int(code), byref(coef),
                                   ptr(z), ptr(aux), ptr(z0t), ptr(noise), stream_ptr()))
     return z0t
+
+
+def op_cfgpp_step_guided(eps_uc: torch.Tensor, eps_c: torch.Tensor, method: int, coef, z: torch.Tensor,
+                         lambdas: torch.Tensor | None, aux: torch.Tensor | None = None, want_z0t: bool = True,
+                         noise: torch.Tensor | None = None):
+    """op_cfgpp_step with a per-image guidance table: lambdas fp32 [z.shape[0]] on the device, row b of z mixing
+    with lambdas[b]; None falls back to coef.lambda_."""
+    from ctypes import byref
+    lib = load()
+    z0t = torch.empty_like(z) if want_z0t else None
+    code = 0 if z.dtype == torch.float16 else 1
+    if lambdas is not None:
+        assert lambdas.dtype == torch.float32 and lambdas.shape == (z.shape[0],)
+    check(lib.cfgpp_op_cfgpp_step_guided(ptr(eps_uc), ptr(eps_c), c_int(z.numel()), c_int(method), c_int(code),
+                                         byref(coef), ptr(z), ptr(aux), ptr(z0t), ptr(noise), ptr(lambdas),
+                                         c_int(z.shape[0]), stream_ptr()))
+    return z0t

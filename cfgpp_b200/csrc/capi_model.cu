@@ -85,6 +85,10 @@ CFGPP_API int cfgpp_set_noise(cfgpp_handle* h, const void* noise_dev, int slots,
   return guarded([&] { h->unet.set_noise((const __half*)noise_dev, slots, (cudaStream_t)stream); });
 }
 
+CFGPP_API int cfgpp_set_guidance(cfgpp_handle* h, const float* lambda_host, int n, void* stream) {
+  return guarded([&] { h->unet.set_guidance(lambda_host, n, (cudaStream_t)stream); });
+}
+
 CFGPP_API int cfgpp_run_steps(cfgpp_handle* h, int first_step, int nsteps, void* stream) {
   return guarded([&] { h->unet.run_steps(first_step, nsteps, (cudaStream_t)stream); });
 }

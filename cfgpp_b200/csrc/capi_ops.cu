@@ -126,29 +126,52 @@ CFGPP_API int cfgpp_op_layernorm(const void* x, int M, int C, const void* gamma,
   });
 }
 
+namespace {
+// One step-only launch with the coefficients and the two table words (noise, guidance) in a scratch device block.
+void op_step(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype, const cfgpp_step_coef* coef_host,
+             void* z, void* aux, void* z0t_out, const void* noise_dev, const float* lambda_dev, int batch,
+             cudaStream_t stream) {
+  static_assert(sizeof(cfgpp_step_coef) == sizeof(StepCoef), "ABI struct mismatch");
+  static_assert(sizeof(StepCoef) % sizeof(void*) == 0, "the table words are stored right behind the coefficients");
+  const bool guided = lambda_dev != nullptr;
+  CFGPP_REQUIRE(!guided || (batch >= 1 && n % batch == 0), "guidance table: batch must divide n");
+  StepCoef* coef_dev = nullptr;
+  CFGPP_CHECK_CUDA(cudaMalloc(&coef_dev, sizeof(StepCoef) + 2 * sizeof(void*)));
+  const __half** slot = reinterpret_cast<const __half**>(coef_dev + 1);
+  const float** lslot = reinterpret_cast<const float**>(slot + 1);
+  cudaError_t e = cudaMemcpy(coef_dev, coef_host, sizeof(StepCoef), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(slot, &noise_dev, sizeof(void*), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(lslot, &lambda_dev, sizeof(void*), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) {
+    try {
+      run_step_only((const __half*)eps_uc, (const __half*)eps_c, n, method | (state_dtype == CFGPP_F16 ? 0x100 : 0),
+                    coef_dev, z, aux, z0t_out, stream, slot, guided ? lslot : nullptr, guided ? n / batch : 0);
+    } catch (...) {
+      cudaFree(coef_dev);
+      throw;
+    }
+    e = cudaStreamSynchronize(stream);  // test-only entry point
+  }
+  cudaFree(coef_dev);
+  CFGPP_CHECK_CUDA(e);
+}
+}  // namespace
+
 CFGPP_API int cfgpp_op_cfgpp_step(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype,
                                   const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
                                   const void* noise_dev, void* stream) {
   return guarded([&] {
-    static_assert(sizeof(cfgpp_step_coef) == sizeof(StepCoef), "ABI struct mismatch");
-    static_assert(sizeof(StepCoef) % sizeof(void*) == 0, "the noise word is stored right behind the coefficients");
-    StepCoef* coef_dev = nullptr;
-    CFGPP_CHECK_CUDA(cudaMalloc(&coef_dev, sizeof(StepCoef) + sizeof(void*)));
-    const __half** slot = reinterpret_cast<const __half**>(coef_dev + 1);
-    cudaError_t e = cudaMemcpy(coef_dev, coef_host, sizeof(StepCoef), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(slot, &noise_dev, sizeof(void*), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-      try {
-        run_step_only((const __half*)eps_uc, (const __half*)eps_c, n, method | (state_dtype == CFGPP_F16 ? 0x100 : 0),
-                      coef_dev, z, aux, z0t_out, (cudaStream_t)stream, slot);
-      } catch (...) {
-        cudaFree(coef_dev);
-        throw;
-      }
-      e = cudaStreamSynchronize((cudaStream_t)stream);  // test-only entry point
-    }
-    cudaFree(coef_dev);
-    CFGPP_CHECK_CUDA(e);
+    op_step(eps_uc, eps_c, n, method, state_dtype, coef_host, z, aux, z0t_out, noise_dev, nullptr, 0,
+            (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_cfgpp_step_guided(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype,
+                                         const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
+                                         const void* noise_dev, const float* lambda_dev, int batch, void* stream) {
+  return guarded([&] {
+    op_step(eps_uc, eps_c, n, method, state_dtype, coef_host, z, aux, z0t_out, noise_dev, lambda_dev, batch,
+            (cudaStream_t)stream);
   });
 }
 

@@ -203,10 +203,11 @@ CFGPP_DEVICE float rs(float x) {  // round to the state dtype
 }
 
 template <bool kHalfState>
-CFGPP_DEVICE void cfgpp_update(int mode, const StepCoef& k, float eu, float ec, float z, float old_d, float noise,
-                               float& z_new, float& z0t, float& new_old) {
-  // noise_pred = eps_uc + lambda * (eps_c - eps_uc)   (three fp16 tensor ops)
-  const float np = rh(__fadd_rn(eu, rh(__fmul_rn(k.lambda, rh(__fsub_rn(ec, eu))))));
+CFGPP_DEVICE void cfgpp_update(int mode, const StepCoef& k, float lambda, float eu, float ec, float z, float old_d,
+                               float noise, float& z_new, float& z0t, float& new_old) {
+  // noise_pred = eps_uc + lambda * (eps_c - eps_uc)   (three fp16 tensor ops); lambda is k.lambda or the image's entry
+  // of the per-image guidance table
+  const float np = rh(__fadd_rn(eu, rh(__fmul_rn(lambda, rh(__fsub_rn(ec, eu))))));
   new_old = 0.f;
   if (mode == STEP_DDIM_CFGPP || mode == STEP_DDIM_INV_CFGPP || mode == STEP_DDIM_CFG) {
     // Tweedie: guided eps (CFG++ sampling, plain CFG) / eps_uc (CFG++ inversion);
@@ -278,7 +279,8 @@ CFGPP_DEVICE void store_state(void* p, size_t i, bool is_half, float v) {
 }
 
 CFGPP_DEVICE void apply_step_elem(int mode, int half_state, const StepCoef& k, float eu, float ec, void* z, void* aux,
-                                  void* z0t_out, const __half* const* noise_slot, size_t n, size_t i) {
+                                  void* z0t_out, const __half* const* noise_slot, const float* const* lambda_slot,
+                                  size_t sample_elems, size_t n, size_t i) {
   const bool hs = half_state != 0;
   const float zv = load_state(z, i, hs);
   const bool kd = mode == STEP_DPMPP2M_CFGPP;
@@ -290,11 +292,18 @@ CFGPP_DEVICE void apply_step_elem(int mode, int half_state, const StepCoef& k, f
     const __half* base = *noise_slot;
     if (base) noise = __half2float(base[static_cast<size_t>(k.c3) * n + i]);
   }
+  float lambda = k.lambda;
+  if (lambda_slot) {
+    // per-image guidance table [batch]: read through a device word like the noise table, so the captured graph
+    // survives setting and clearing it; a null table means the schedule's scalar
+    const float* table = *lambda_slot;
+    if (table) lambda = table[i / sample_elems];
+  }
   float zn, z0, no;
   if (hs)
-    cfgpp_update<true>(mode, k, eu, ec, zv, old_d, noise, zn, z0, no);
+    cfgpp_update<true>(mode, k, lambda, eu, ec, zv, old_d, noise, zn, z0, no);
   else
-    cfgpp_update<false>(mode, k, eu, ec, zv, old_d, noise, zn, z0, no);
+    cfgpp_update<false>(mode, k, lambda, eu, ec, zv, old_d, noise, zn, z0, no);
   store_state(z, i, hs, zn);
   if (z0t_out) store_state(z0t_out, i, hs, z0);
   if (mode == STEP_DPMPP2M_CFGPP && aux) store_state(aux, i, hs, no);
@@ -305,7 +314,8 @@ __global__ void conv_out_step_kernel(const __half* __restrict__ x, const __half*
                                      const __half* __restrict__ bias, int B, int H, int W, int Cin, int mode,
                                      int half_state, const StepCoef* __restrict__ coef, void* z, void* aux,
                                      void* z0t_out, __half* __restrict__ eps_uc, __half* __restrict__ eps_c,
-                                     const __half* const* __restrict__ noise_slot) {
+                                     const __half* const* __restrict__ noise_slot,
+                                     const float* const* __restrict__ lambda_slot) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ __half swh[];  // [4][9][Cin]
@@ -372,18 +382,21 @@ __global__ void conv_out_step_kernel(const __half* __restrict__ x, const __half*
     if (eps_uc) eps_uc[i] = __float2half_rn(eu);
     if (eps_c) eps_c[i] = __float2half_rn(ec);
     if (mode != STEP_NONE)
-      apply_step_elem(mode, half_state, *coef, eu, ec, z, aux, z0t_out, noise_slot, static_cast<size_t>(B) * 4 * HW, i);
+      apply_step_elem(mode, half_state, *coef, eu, ec, z, aux, z0t_out, noise_slot, lambda_slot,
+                      static_cast<size_t>(4) * HW, static_cast<size_t>(B) * 4 * HW, i);
   }
 }
 
 __global__ void step_only_kernel(const __half* __restrict__ eps_uc, const __half* __restrict__ eps_c, int n, int mode,
                                  int half_state, const StepCoef* __restrict__ coef, void* z, void* aux, void* z0t_out,
-                                 const __half* const* __restrict__ noise_slot) {
+                                 const __half* const* __restrict__ noise_slot,
+                                 const float* const* __restrict__ lambda_slot, int sample_elems) {
   pdl_launch_dependents();
   pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  apply_step_elem(mode, half_state, *coef, __half2float(eps_uc[i]), __half2float(eps_c[i]), z, aux, z0t_out, noise_slot, n, i);
+  apply_step_elem(mode, half_state, *coef, __half2float(eps_uc[i]), __half2float(eps_c[i]), z, aux, z0t_out, noise_slot,
+                  lambda_slot, sample_elems, n, i);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -473,7 +486,7 @@ void run_conv_in(const void* z, int z_is_half, const float* in_scale, const __ha
 // The state dtype travels in bit 8 of `mode` (mode | 0x100 = fp16 sampler state).
 void run_conv_out_step(const __half* x, const __half* w, const __half* bias, int B, int H, int W, int Cin, int mode,
                        const StepCoef* coef_dev, void* z, void* aux, void* z0t_out, __half* eps_uc, __half* eps_c,
-                       cudaStream_t stream, const __half* const* noise_slot) {
+                       cudaStream_t stream, const __half* const* noise_slot, const float* const* lambda_slot) {
   CFGPP_REQUIRE(Cin % 8 == 0, "conv_out Cin must be a multiple of 8");
   const int half_state = (mode & 0x100) ? 1 : 0;
   const int m = mode & 0xff;
@@ -482,14 +495,17 @@ void run_conv_out_step(const __half* x, const __half* w, const __half* bias, int
   const int warps = 8;
   const int total = B * H * W;
   launch_pdl(conv_out_step_kernel, dim3((total + warps - 1) / warps), dim3(warps * 32), smem, stream, 
-      x, w, bias, B, H, W, Cin, m, half_state, coef_dev, z, aux, z0t_out, eps_uc, eps_c, noise_slot);
+      x, w, bias, B, H, W, Cin, m, half_state, coef_dev, z, aux, z0t_out, eps_uc, eps_c, noise_slot, lambda_slot);
 }
 
 void run_step_only(const __half* eps_uc, const __half* eps_c, int n, int mode, const StepCoef* coef_dev, void* z,
-                   void* aux, void* z0t_out, cudaStream_t stream, const __half* const* noise_slot) {
+                   void* aux, void* z0t_out, cudaStream_t stream, const __half* const* noise_slot,
+                   const float* const* lambda_slot, int sample_elems) {
+  CFGPP_REQUIRE(!lambda_slot || (sample_elems > 0 && n % sample_elems == 0),
+                "a guidance table needs the per-image element count (a divisor of n)");
   const int half_state = (mode & 0x100) ? 1 : 0;
   launch_pdl(step_only_kernel, dim3((n + 255) / 256), dim3(256), 0, stream, eps_uc, eps_c, n, mode & 0xff, half_state, coef_dev, z, aux,
-                                                        z0t_out, noise_slot);
+                                                        z0t_out, noise_slot, lambda_slot, sample_elems);
 }
 
 void run_upsample2x(const __half* x, __half* out, int B, int H, int W, int C, cudaStream_t stream) {

@@ -73,15 +73,19 @@ void run_select_step(const StepState* table, int* counter, StepState* cur, cudaS
 
 // conv_out 3x3 (Cin -> 4) on the GroupNorm+SiLU'ed NHWC input x [2B,H,W,Cin] fused with the CFG++ guidance mix and
 // the scheduler update. noise_slot (may be null): device word holding the base of the ancestral noise table
-// [slots][B,4,H,W] fp16. z is the sampler state (NCHW, fp32 for DDIM modes, fp16 for DPM++), updated in place.
+// [slots][B,4,H,W] fp16. lambda_slot (may be null): device word holding the per-image guidance table [B] fp32 or null;
+// while it holds a table, image b mixes with table[b] instead of coef->lambda. z is the sampler state (NCHW, fp32 for
+// DDIM modes, fp16 for DPM++), updated in place.
 void run_conv_out_step(const __half* x, const __half* w /*[4][9][Cin]*/, const __half* bias, int B, int H, int W,
                        int Cin, int mode, const StepCoef* coef_dev, void* z, void* aux /*old_denoised*/,
                        void* z0t_out, __half* eps_uc, __half* eps_c, cudaStream_t stream,
-                       const __half* const* noise_slot = nullptr);
+                       const __half* const* noise_slot = nullptr, const float* const* lambda_slot = nullptr);
 
-// standalone fused CFG++ update from given eps (used when a per-step callback needs the un-fused seam)
+// standalone fused CFG++ update from given eps (used when a per-step callback needs the un-fused seam); with a
+// lambda_slot, element i belongs to image i / sample_elems (sample_elems = 4*H*W)
 void run_step_only(const __half* eps_uc, const __half* eps_c, int n, int mode, const StepCoef* coef_dev, void* z,
-                   void* aux, void* z0t_out, cudaStream_t stream, const __half* const* noise_slot = nullptr);
+                   void* aux, void* z0t_out, cudaStream_t stream, const __half* const* noise_slot = nullptr,
+                   const float* const* lambda_slot = nullptr, int sample_elems = 0);
 
 void run_upsample2x(const __half* x, __half* out, int B, int H, int W, int C, cudaStream_t stream);
 // stride-2 pad-1 3x3 im2col: x [B,H,W,C] -> out [B*(H/2)*(W/2), 9*C] (tap-major, matches the packed weight)

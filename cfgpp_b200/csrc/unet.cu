@@ -703,6 +703,9 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
       z0t_state_ = alloc_bytes(lat * sizeof(float));
       noise_slot_ = static_cast<const __half**>(alloc_bytes(sizeof(__half*)));
       CFGPP_CHECK_CUDA(cudaMemcpy(noise_slot_, &noise_buf_, sizeof(__half*), cudaMemcpyHostToDevice));
+      lambda_buf_ = static_cast<float*>(alloc_bytes(static_cast<size_t>(B_) * sizeof(float)));
+      lambda_slot_ = static_cast<const float**>(alloc_bytes(sizeof(float*)));
+      CFGPP_CHECK_CUDA(cudaMemset(lambda_slot_, 0, sizeof(float*)));  // no table: the schedule's scalar lambda
       fwd_eps_uc_ = alloc_act(lat);
       fwd_eps_c_ = alloc_act(lat);
       temb_w_all_ = packed_cat_rows(temb_w_keys);
@@ -1049,6 +1052,18 @@ void Unet::set_noise(const __half* noise, int slots, cudaStream_t stream) {
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(noise_buf_, noise, n * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
 }
 
+void Unet::set_guidance(const float* lambda, int n, cudaStream_t stream) {
+  CFGPP_REQUIRE(prepared_, "call cfgpp_prepare first");
+  CFGPP_REQUIRE(n == 0 || (lambda != nullptr && n == B_), "guidance table: n = 0 (clear) or one entry per image");
+  // both copies come from pageable host memory, which cudaMemcpyAsync stages before it returns; the stream orders
+  // them after any replay still reading the previous table
+  if (n > 0)
+    CFGPP_CHECK_CUDA(cudaMemcpyAsync(lambda_buf_, lambda, static_cast<size_t>(n) * sizeof(float),
+                                     cudaMemcpyHostToDevice, stream));
+  const float* table = n > 0 ? lambda_buf_ : nullptr;
+  CFGPP_CHECK_CUDA(cudaMemcpyAsync(lambda_slot_, &table, sizeof(table), cudaMemcpyHostToDevice, stream));
+}
+
 void Unet::ensure_graph(cudaStream_t stream) {
   if (graph_valid_) return;
   if (graph_exec_) { cudaGraphExecDestroy(graph_exec_); graph_exec_ = nullptr; }
@@ -1062,7 +1077,7 @@ void Unet::ensure_graph(cudaStream_t stream) {
                 conv_in_out_, B_, H_, W_, d_.block_out_channels[0], 2, capture_stream_);
     run_body(capture_stream_, true);
     run_conv_out_step(final_norm_.p, conv_out_w_, conv_out_b_, B_, H_, W_, final_norm_.C, mode, &cur_state_->coef,
-                      z_state_, aux_state_, z0t_state_, nullptr, nullptr, capture_stream_, noise_slot_);
+                      z_state_, aux_state_, z0t_state_, nullptr, nullptr, capture_stream_, noise_slot_, lambda_slot_);
   } catch (...) {
     cudaGraph_t g = nullptr;
     cudaStreamEndCapture(capture_stream_, &g);
@@ -1094,7 +1109,8 @@ void Unet::apply_step(int step, const __half* eps_uc, const __half* eps_c, cudaS
   CFGPP_REQUIRE(prepared_ && step >= 0 && step < nsteps_, "step outside the schedule");
   const int mode = method_ | (state_dtype_ == CFGPP_F16 ? 0x100 : 0);
   const int n = B_ * 4 * H_ * W_;
-  run_step_only(eps_uc, eps_c, n, mode, &step_table_[step].coef, z_state_, aux_state_, z0t_state_, stream, noise_slot_);
+  run_step_only(eps_uc, eps_c, n, mode, &step_table_[step].coef, z_state_, aux_state_, z0t_state_, stream, noise_slot_,
+                lambda_slot_, 4 * H_ * W_);
 }
 
 }  // namespace cfgpp

@@ -55,6 +55,8 @@ class Unet {
   void set_state(const void* z, int z_dtype, cudaStream_t stream);
   // ancestral samplers: fp16 noise table [slots][B,4,H,W] (device), copied into a handle-owned buffer
   void set_noise(const __half* noise, int slots, cudaStream_t stream);
+  // per-image guidance: lambda_host [batch] (host), or n = 0 to return to the schedule's scalar; prepare() clears it
+  void set_guidance(const float* lambda_host, int n, cudaStream_t stream);
   void run_steps(int first_step, int nsteps, cudaStream_t stream);
   void get_state(int which, void* out, cudaStream_t stream);
   void apply_step(int step, const __half* eps_uc, const __half* eps_c, cudaStream_t stream);
@@ -172,6 +174,8 @@ class Unet {
   const __half** noise_slot_ = nullptr;  // device word holding noise_buf_ (read by the step kernel: graph-stable)
   __half* noise_buf_ = nullptr;          // owned, survives prepare(); re-allocated when a larger table arrives
   size_t noise_cap_ = 0;                 // elements
+  const float** lambda_slot_ = nullptr;  // device word holding lambda_buf_ or null (read by the step kernel)
+  float* lambda_buf_ = nullptr;          // [B] per-image guidance, workspace of the prepared plan
   const void* fwd_z_ = nullptr;  // input of the un-fused forward
   int fwd_z_dtype_ = CFGPP_F32;
   __half *fwd_eps_uc_ = nullptr, *fwd_eps_c_ = nullptr;

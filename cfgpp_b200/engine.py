@@ -167,7 +167,9 @@ class NativeUNet:
         return out
 
     # ---- fused trajectory ------------------------------------------------------------------------------------
-    def set_schedule(self, method: int, state_dtype: torch.dtype, steps: Sequence[StepStateC]):
+    def set_schedule(self, method: int, state_dtype: torch.dtype, steps: Sequence[StepStateC],
+                     guidance: Optional[Sequence[float]] = None):
+        """`guidance`: per-image guidance scales (set_guidance); None leaves the steps' scalar lambda in charge."""
         arr = to_c_array(list(steps))
         code = F16 if state_dtype == torch.float16 else F32
         with torch.cuda.device(self.device):
@@ -175,6 +177,17 @@ class NativeUNet:
                                                  nv.stream_ptr()))
         self._nsteps = len(steps)
         self._state_dtype = state_dtype
+        self.set_guidance(guidance)
+
+    def set_guidance(self, guidance: Optional[Sequence[float]] = None):
+        """One guidance scale per image of the prepared batch, rounded to fp32, used by every following step (fused
+        and `apply_step`) instead of the schedule's scalar; None clears the table."""
+        n = 0 if guidance is None else len(guidance)
+        if guidance is not None and n != self.batch:
+            raise ValueError(f"{n} guidance scales for a prepared batch of {self.batch}")
+        arr = (c_float * n)(*[float(g) for g in guidance]) if n else None
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_set_guidance(self._h, arr, c_int(n), nv.stream_ptr()))
 
     def set_state(self, z: torch.Tensor):
         z = z.to(self.device, self._state_dtype).contiguous()

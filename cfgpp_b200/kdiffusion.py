@@ -18,6 +18,8 @@ from typing import Callable, Optional, Sequence
 
 import torch
 
+from .batching import guidance_mix, guidance_table
+
 
 def get_ancestral_step(sigma_from, sigma_to, eta: float = 1.):
     """(sigma_down, sigma_up) of an ancestral step — latent_diffusion.py:30-37."""
@@ -65,7 +67,7 @@ class KDiffusionMixin:
         """cond = (uc, c) for SD v1.5, (uc, c, add_cond_kwargs) for SDXL. Returns (denoised, uncond_denoised)."""
         xc = self.calculate_input(x, sigma)
         noise_uc, noise_c = self.predict_noise(xc, t, *cond)
-        noise_pred = noise_uc + cfg_guidance * (noise_c - noise_uc)
+        noise_pred = guidance_mix(noise_uc, noise_c, cfg_guidance)
         return self.calculate_denoised(x, noise_pred, sigma), self.calculate_denoised(x, noise_uc, sigma)
 
     def kdiffusion_x_to_denoised(self, x, sigma, uc, c, cfg_guidance, t):
@@ -75,13 +77,13 @@ class KDiffusionMixin:
         return self._k_denoise(x, sigma, t, cfg_guidance, (uc, c, add_cond_kwargs))
 
 
-def _fused_trajectory(solver, x, steps, cond):
+def _fused_trajectory(solver, x, steps, cond, cfg_guidance):
     """Whole VE-cast trajectory on the fused step kernel (UNet + CFG / CFG++ mix + Euler / DPM++2M update in the conv_out
     epilogue, one CUDA-graph replay per step, no elementwise launch or host sync in between). Returns (last denoised, x)."""
     from . import schedule as S
     solver._prepare(x, *cond, force=True)
     eng = solver.unet
-    eng.set_schedule(S.STEP_DPMPP2M_CFGPP, torch.float16, steps)
+    eng.set_schedule(S.STEP_DPMPP2M_CFGPP, torch.float16, steps, guidance_table(cfg_guidance))
     eng.set_state(x)
     eng.run_steps(0, len(steps))
     return eng.get_state(1), eng.get_state(0)
@@ -97,7 +99,7 @@ def _fused_ancestral_trajectory(solver, x, sigmas, cfg_guidance, cond, cfgpp: bo
     eng = solver.unet
     state0 = x.to(eng.device, torch.float16)
     noise = torch.stack([torch.randn_like(state0) for _ in range(slots)]) if slots else None
-    eng.set_schedule(S.STEP_DPMPP2M_CFGPP, torch.float16, steps)
+    eng.set_schedule(S.STEP_DPMPP2M_CFGPP, torch.float16, steps, guidance_table(cfg_guidance))
     eng.set_state(state0)
     if noise is not None:
         eng.set_noise(noise)
@@ -130,7 +132,8 @@ def euler_cfgpp_loop(solver: KDiffusionMixin, x, sigmas, cfg_guidance, cond, cal
         if ancestral:
             return _fused_ancestral_trajectory(solver, x, sigmas, cfg_guidance, cond, cfgpp, two_s=False)
         from . import schedule as S
-        return _fused_trajectory(solver, x, S.kd_steps(sigmas, solver.timestep, cfg_guidance, cfgpp), cond)
+        return _fused_trajectory(solver, x, S.kd_steps(sigmas, solver.timestep, cfg_guidance, cfgpp), cond,
+                                 cfg_guidance)
     denoised = None
     for i in range(len(sigmas) - 1):
         sigma = sigmas[i]
@@ -198,7 +201,7 @@ def dpmpp_2m_cfgpp_karras_loop(solver: KDiffusionMixin, x, sigmas, cfg_guidance,
     if _fusable(solver, callback_fn):
         from . import schedule as S
         return _fused_trajectory(solver, x, S.kd_steps(sigmas, solver.timestep, cfg_guidance, cfgpp, second_order=True,
-                                                       diff_guided=True), cond)
+                                                       diff_guided=True), cond, cfg_guidance)
     t_fn = lambda s: s.log().neg()  # noqa: E731
     old_denoised = None
     denoised = None

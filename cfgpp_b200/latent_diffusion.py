@@ -21,6 +21,7 @@ import torch
 
 from . import kdiffusion as K
 from . import schedule as S
+from .batching import draw_latents, encode_prompts, guidance_table, normalize_batch
 from .conditioning import SyntheticTextEncoder
 from .text_encoder import CLIPTextConfig, get_conditioner
 from .config import UNetConfig, sd15_config
@@ -96,10 +97,22 @@ class StableDiffusion(K.KDiffusionMixin):
         return self._sch.alpha(t)
 
     @torch.no_grad()
-    def get_text_embed(self, null_prompt, prompt):
-        null_text_embed, _ = self.text_encoder(null_prompt, self.device)
-        text_embed, _ = self.text_encoder(prompt, self.device)
+    def get_text_embed(self, null_prompt, prompt, batch: int = 1):
+        """One prompt each (a string is broadcast to `batch` rows) or lists of prompts, one row per prompt."""
+        from .text_encoder import ClipConditioner
+        takes_list = isinstance(self.text_encoder, ClipConditioner)
+        enc = lambda p: self.text_encoder(p, self.device)  # noqa: E731
+        null_text_embed, _ = encode_prompts(enc, null_prompt, batch, takes_list)
+        text_embed, _ = encode_prompts(enc, prompt, batch, takes_list)
         return null_text_embed, text_embed
+
+    def batch_inputs(self, prompt, cfg_guidance, zT=None):
+        """(uc, c, cfg_guidance, zT) of a batched text-to-image call: `prompt[1]` one string or B strings, `prompt[0]`
+        one string (broadcast) or B strings, `cfg_guidance` a float or B floats (one per image, applied in the fused
+        step kernel), `zT` None or (B,4,h,w). Mismatched lengths raise ValueError."""
+        B, p, cfg_guidance = normalize_batch({"prompt[0]": prompt[0], "prompt[1]": prompt[1]}, cfg_guidance, zT)
+        uc, c = self.get_text_embed(null_prompt=p["prompt[0]"], prompt=p["prompt[1]"], batch=B)
+        return uc, c, cfg_guidance, zT
 
     def encode(self, x):
         return self.vae.encode(x, self.dtype)
@@ -119,10 +132,12 @@ class StableDiffusion(K.KDiffusionMixin):
         self._prepare(zt, uc, c)
         return self.unet.predict_noise(zt, float(t))
 
-    def _run(self, method, steps, z_init, uc, c, callback_fn=None):
+    def _run(self, method, steps, z_init, uc, c, callback_fn=None, cfg_guidance=None):
+        """`cfg_guidance`: a per-image sequence goes to the step kernel's guidance table; a float (or None) leaves the
+        steps' scalar in charge."""
         self._prepare(z_init, uc, c, force=True)  # every trajectory re-binds its prompt
         eng = self.unet
-        eng.set_schedule(method, z_init.dtype, steps)
+        eng.set_schedule(method, z_init.dtype, steps, None if cfg_guidance is None else guidance_table(cfg_guidance))
         eng.set_state(z_init)
         z0t = None
         if callback_fn is None:
@@ -155,11 +170,11 @@ class StableDiffusion(K.KDiffusionMixin):
                                cfg_guidance=1.0)
         elif method == 'random':
             size = kwargs.get('latent_dim', (1, 4, self.cfg.sample_size, self.cfg.sample_size))
-            z = torch.randn(size).to(self.device)  # CPU generator, then H2D — latent_diffusion.py:199-200
+            z = draw_latents(size).to(self.device)  # CPU generator, then H2D — latent_diffusion.py:199-200
         elif method == 'random_kdiffusion':
             size = kwargs.get('latent_dim', (1, 4, self.cfg.sample_size, self.cfg.sample_size))
             sigmas = kwargs.get('sigmas', [14.6146])
-            z = torch.randn(size).to(self.device)
+            z = draw_latents(size).to(self.device)
             z = z * (sigmas[0] ** 2 + 1) ** 0.5
         else:
             raise NotImplementedError
@@ -176,14 +191,14 @@ class BaseDDIM(StableDiffusion):
 
     def reverse_process(self, uc, c, cfg_guidance, zt, callback_fn=None):
         steps = S.ddim_cfgpp_steps(self._sch, cfg_guidance, sdxl_indexing=False)
-        z0t, _ = self._run(S.STEP_DDIM_CFG, steps, zt, uc, c, callback_fn)
+        z0t, _ = self._run(S.STEP_DDIM_CFG, steps, zt, uc, c, callback_fn, cfg_guidance)
         return z0t
 
     def sample(self, cfg_guidance=7.5, prompt=["", ""], callback_fn=None, **kwargs):
-        uc, c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[1])
-        zt = kwargs.get('zT')
+        """Batched: see StableDiffusion.batch_inputs. Returns (B, 3, H, W)."""
+        uc, c, cfg_guidance, zt = self.batch_inputs(prompt, cfg_guidance, kwargs.get('zT'))
         if zt is None:
-            zt = self.initialize_latent()
+            zt = self.initialize_latent(latent_dim=(uc.shape[0], 4, self.cfg.sample_size, self.cfg.sample_size))
         z0t = self.reverse_process(uc, c, cfg_guidance, zt, callback_fn)
         img = self.decode(z0t)
         img = (img / 2 + 0.5).clamp(0, 1)
@@ -227,14 +242,14 @@ class BaseDDIMCFGpp(StableDiffusion):
 
     def reverse_process(self, uc, c, cfg_guidance, zt, callback_fn=None):
         steps = S.ddim_cfgpp_steps(self._sch, cfg_guidance, sdxl_indexing=False)
-        z0t, _ = self._run(S.STEP_DDIM_CFGPP, steps, zt, uc, c, callback_fn)
+        z0t, _ = self._run(S.STEP_DDIM_CFGPP, steps, zt, uc, c, callback_fn, cfg_guidance)
         return z0t
 
     def sample(self, cfg_guidance=7.5, prompt=["", ""], callback_fn=None, **kwargs):
-        uc, c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[1])
-        zt = kwargs.get('zT')
+        """Batched: see StableDiffusion.batch_inputs. Returns (B, 3, H, W)."""
+        uc, c, cfg_guidance, zt = self.batch_inputs(prompt, cfg_guidance, kwargs.get('zT'))
         if zt is None:
-            zt = self.initialize_latent()
+            zt = self.initialize_latent(latent_dim=(uc.shape[0], 4, self.cfg.sample_size, self.cfg.sample_size))
         z0t = self.reverse_process(uc, c, cfg_guidance, zt, callback_fn)
         img = self.decode(z0t)
         img = (img / 2 + 0.5).clamp(0, 1)
@@ -296,12 +311,14 @@ class _KarrasCFGpp(StableDiffusion):
             x = noise.to(self.device) * (sigmas[0] ** 2 + 1) ** 0.5
         if x is None:
             x = self.initialize_latent(method="random_kdiffusion", sigmas=sigmas,
-                                       latent_dim=(1, 4, self.cfg.sample_size, self.cfg.sample_size))
+                                       latent_dim=(uc.shape[0], 4, self.cfg.sample_size, self.cfg.sample_size))
         return self._loop(x.to(torch.float16), sigmas, cfg_guidance, (uc, c), callback_fn)
 
     def sample(self, cfg_guidance, prompt=["", ""], callback_fn=None, **kwargs):
-        uc, c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[1])
-        denoised, x = self.reverse_process(uc, c, cfg_guidance, kwargs.get('xT'), callback_fn, kwargs.get('zT'))
+        """Batched: see StableDiffusion.batch_inputs. Ancestral methods draw each step's noise with `randn_like` over
+        the whole batch, as the reference's loop would on a batched x: their images are not the serial runs' images."""
+        uc, c, cfg_guidance, zt = self.batch_inputs(prompt, cfg_guidance, kwargs.get('zT'))
+        denoised, x = self.reverse_process(uc, c, cfg_guidance, kwargs.get('xT'), callback_fn, zt)
         img = self.decode(x if self.decode_state else denoised)
         img = (img / 2 + 0.5).clamp(0, 1)
         return img.detach().cpu()

@@ -25,6 +25,8 @@ import torch
 
 from . import kdiffusion as K
 from . import schedule as S
+from .batching import (draw_latents, encode_prompts, guidance_table, guidance_values, normalize_batch,
+                       sdxl_added_conditions)
 from .conditioning import SyntheticTextEncoder
 from .text_encoder import CLIPTextConfig, ClipConditioner, get_conditioner
 from .config import UNetConfig, sdxl_config
@@ -172,25 +174,26 @@ class SDXL(K.KDiffusionMixin):
         return at
 
     @torch.no_grad()
-    def _text_embed(self, prompt, text_enc, clip_skip):
-        prompt = prompt[0] if isinstance(prompt, (list, tuple)) else prompt
+    def _text_embed(self, prompt, text_enc, clip_skip, batch: int = 1):
+        """One prompt (broadcast to `batch` rows) or a list of prompts, one row each."""
         if isinstance(text_enc, ClipConditioner):
-            return text_enc(prompt, self.device, clip_skip=clip_skip)
-        return text_enc(prompt, self.device)
+            return encode_prompts(lambda p: text_enc(p, self.device, clip_skip=clip_skip), prompt, batch, True)
+        return encode_prompts(lambda p: text_enc(p, self.device), prompt, batch)
 
     @torch.no_grad()
-    def get_text_embed(self, null_prompt_1, prompt_1, null_prompt_2=None, prompt_2=None, clip_skip=None):
-        prompt_embed_1, pool_prompt_embed = self._text_embed(prompt_1, self.text_enc_1, clip_skip)
+    def get_text_embed(self, null_prompt_1, prompt_1, null_prompt_2=None, prompt_2=None, clip_skip=None,
+                       batch: int = 1):
+        prompt_embed_1, pool_prompt_embed = self._text_embed(prompt_1, self.text_enc_1, clip_skip, batch)
         if prompt_2 is None:
             prompt_embed = [prompt_embed_1]
         else:
-            prompt_embed_2, pool_prompt_embed = self._text_embed(prompt_2, self.text_enc_2, clip_skip)
+            prompt_embed_2, pool_prompt_embed = self._text_embed(prompt_2, self.text_enc_2, clip_skip, batch)
             prompt_embed = [prompt_embed_1, prompt_embed_2]
-        null_embed_1, pool_null_embed = self._text_embed(null_prompt_1, self.text_enc_1, clip_skip)
+        null_embed_1, pool_null_embed = self._text_embed(null_prompt_1, self.text_enc_1, clip_skip, batch)
         if null_prompt_2 is None:
             null_embed = [null_embed_1]
         else:
-            null_embed_2, pool_null_embed = self._text_embed(null_prompt_2, self.text_enc_2, clip_skip)
+            null_embed_2, pool_null_embed = self._text_embed(null_prompt_2, self.text_enc_2, clip_skip, batch)
             null_embed = [null_embed_1, null_embed_2]
         null_prompt_embeds = torch.concat(null_embed, dim=-1)
         prompt_embeds = torch.concat(prompt_embed, dim=-1)
@@ -241,15 +244,21 @@ class SDXL(K.KDiffusionMixin):
                negative_target_size: Optional[Tuple[int, int]] = None,
                clip_skip: Optional[int] = None,
                **kwargs):
+        """Batched: `prompt1[1]` / `prompt2[1]` one string or B strings, the null prompts one string (broadcast) or B
+        strings, `cfg_guidance` a float or B floats (one per image, applied in the fused step kernel), `zT` None or
+        (B,4,h,w); without zT the B latents are drawn one image at a time, so image i does not depend on B. Mismatched
+        lengths raise ValueError. Returns (B, 3, H, W)."""
         height = self.default_sample_size * self.vae_scale_factor
         width = self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)
         target_size = target_size or (height, width)
 
+        B, p, cfg_guidance = normalize_batch({"prompt1[0]": prompt1[0], "prompt1[1]": prompt1[1],
+                                              "prompt2[0]": prompt2[0], "prompt2[1]": prompt2[1]},
+                                             cfg_guidance, kwargs.get('zT'))
         (null_prompt_embeds, prompt_embeds, pool_null_embed, pool_prompt_embed) = self.get_text_embed(
-            prompt1[0], prompt1[1], prompt2[0], prompt2[1], clip_skip)
+            p["prompt1[0]"], p["prompt1[1]"], p["prompt2[0]"], p["prompt2[1]"], clip_skip, batch=B)
 
-        add_text_embeds = pool_prompt_embed
         add_time_ids = self._get_add_time_ids(original_size, crops_coords_top_left, target_size,
                                               dtype=prompt_embeds.dtype,
                                               text_encoder_projection_dim=int(pool_prompt_embed.shape[-1]))
@@ -259,11 +268,10 @@ class SDXL(K.KDiffusionMixin):
                                                            text_encoder_projection_dim=int(pool_prompt_embed.shape[-1]))
         else:
             negative_add_time_ids = add_time_ids
-        negative_text_embeds = pool_null_embed
 
-        if cfg_guidance != 0.0 and cfg_guidance != 1.0:
-            add_text_embeds = torch.cat([negative_text_embeds, add_text_embeds], dim=0)
-            add_time_ids = torch.cat([negative_add_time_ids, add_time_ids], dim=0)
+        # per image: the uncond row takes the negative pooled embedding / time ids unless its lambda is 0 or 1
+        add_text_embeds, add_time_ids = sdxl_added_conditions(pool_null_embed, pool_prompt_embed, negative_add_time_ids,
+                                                              add_time_ids, cfg_guidance, B)
 
         add_cond_kwargs = {'text_embeds': add_text_embeds.to(self.device), 'time_ids': add_time_ids.to(self.device)}
 
@@ -278,11 +286,11 @@ class SDXL(K.KDiffusionMixin):
                           add_cond_kwargs: Optional[dict] = None, **kwargs):
         if method == 'random':
             size = kwargs.get('size', (1, 4, 128, 128))
-            z = torch.randn(size).to(self.device)  # CPU generator, then H2D — latent_sdxl.py:288-289
+            z = draw_latents(size).to(self.device)  # CPU generator, then H2D — latent_sdxl.py:288-289
         elif method == 'random_kdiffusion':
             size = kwargs.get('latent_dim', (1, 4, 128, 128))
             sigmas = kwargs.get('sigmas', [14.6146])
-            z = torch.randn(size).to(self.device)
+            z = draw_latents(size).to(self.device)
             z = z * (sigmas[0] ** 2 + 1) ** 0.5
         elif method == 'ddim':
             assert src_img is not None, "src_img must be provided for inversion"
@@ -315,11 +323,13 @@ class SDXL(K.KDiffusionMixin):
         return S.sigma_to_t(self._sch, sigma, quantize)
 
     # ---- shared trajectory driver -------------------------------------------------------------------------------
-    def _run_trajectory(self, method, state_dtype, steps, z_init, uc, c, add_cond_kwargs, callback_fn, result):
-        """`result`: 'z0t' (DDIM family returns the Tweedie estimate of the last step) or 'zt' (DPM++ returns x)."""
+    def _run_trajectory(self, method, state_dtype, steps, z_init, uc, c, add_cond_kwargs, callback_fn, result,
+                        cfg_guidance=None):
+        """`result`: 'z0t' (DDIM family returns the Tweedie estimate of the last step) or 'zt' (DPM++ returns x).
+        `cfg_guidance`: a per-image sequence goes to the step kernel's guidance table."""
         self._prepare(z_init, uc, c, add_cond_kwargs, force=True)  # every trajectory re-binds its prompt
         eng = self.unet
-        eng.set_schedule(method, state_dtype, steps)
+        eng.set_schedule(method, state_dtype, steps, None if cfg_guidance is None else guidance_table(cfg_guidance))
         eng.set_state(z_init)
         if callback_fn is None:
             eng.run_steps(0, len(steps))
@@ -372,7 +382,7 @@ class BaseDDIM(SDXL):
         steps = S.ddim_cfgpp_steps(self._sch, cfg_guidance, sdxl_indexing=True,
                                    tables_on_device=(self.schedule_kind == "lightning"))
         return self._run_trajectory(self.step_mode, torch.float32, steps, zt.float(), null_prompt_embeds,
-                                    prompt_embeds, add_cond_kwargs, callback_fn, 'z0t')
+                                    prompt_embeds, add_cond_kwargs, callback_fn, 'z0t', cfg_guidance)
 
 
 @register_solver('euler')
@@ -389,7 +399,8 @@ class Euler(SDXL):
         if zt is None and kwargs.get('zT') is not None:  # an N(0,1) draw, as every other solver accepts it
             zt = kwargs['zT'].to(self.device) * (sigmas[0] ** 2 + 1) ** 0.5
         if zt is None:
-            zt_dim = (1, 4, shape[1] // self.vae_scale_factor, shape[0] // self.vae_scale_factor)
+            zt_dim = (null_prompt_embeds.shape[0], 4, shape[1] // self.vae_scale_factor,
+                      shape[0] // self.vae_scale_factor)
             zt = self.initialize_latent(method="random_kdiffusion", latent_dim=zt_dim, sigmas=sigmas)
         z0t, _ = K.euler_cfgpp_loop(self, zt.to(torch.float16), sigmas, cfg_guidance,
                                     (null_prompt_embeds, prompt_embeds, add_cond_kwargs), callback_fn, cfgpp=False)
@@ -403,7 +414,7 @@ class BaseDDIMLight(BaseDDIM, SDXLLightning):
 
     def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
                         callback_fn=None, **kwargs):
-        assert cfg_guidance == 1.0, "CFG should be turned off in the lightning version"
+        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
         return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
                                        callback_fn, **kwargs)
 
@@ -417,7 +428,7 @@ class EulerLight(Euler, SDXLLightning):
 
     def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
                         callback_fn=None, **kwargs):
-        assert cfg_guidance == 1.0, "CFG should be turned off in the lightning version"
+        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
         return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
                                        callback_fn, **kwargs)
 
@@ -444,7 +455,7 @@ class BaseDDIMCFGpp(SDXL):
                                    tables_on_device=(self.schedule_kind == "lightning"))
         # fp32 state: zt comes from torch.randn (fp32) and promotes every update (latent_sdxl.py:289, 741-744)
         return self._run_trajectory(S.STEP_DDIM_CFGPP, torch.float32, steps, zt.float(), null_prompt_embeds,
-                                    prompt_embeds, add_cond_kwargs, callback_fn, 'z0t')
+                                    prompt_embeds, add_cond_kwargs, callback_fn, 'z0t', cfg_guidance)
 
 
 @register_solver('ddim_cfg++_lightning')
@@ -460,7 +471,7 @@ class BaseDDIMCFGppLight(BaseDDIMCFGpp, SDXLLightning):
                         shape=(1024, 1024),
                         callback_fn=None,
                         **kwargs):
-        assert cfg_guidance == 1.0, "CFG should be turned off in the lightning version"
+        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
         return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
                                        callback_fn, **kwargs)
 
@@ -486,7 +497,7 @@ class DPMpp2mCFGppSolver(SDXL):
         x = x.to(torch.float16)
         x = x * sigma0  # fp16 tensor x 0-dim fp32 -> fp16 (latent_sdxl.py:882-884)
         return self._run_trajectory(S.STEP_DPMPP2M_CFGPP, torch.float16, steps, x, null_prompt_embeds, prompt_embeds,
-                                    add_cond_kwargs, callback_fn, 'zt')
+                                    add_cond_kwargs, callback_fn, 'zt', cfg_guidance)
 
 
 @register_solver('dpm++_2m_cfgpp_lightning')
@@ -496,7 +507,7 @@ class DPMpp2mCFGppLightningSolver(DPMpp2mCFGppSolver, SDXLLightning):
 
     def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
                         callback_fn=None, **kwargs):
-        assert cfg_guidance == 1.0, "CFG should be turned off in the lightning version"
+        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
         return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
                                        callback_fn, **kwargs)
 
@@ -517,7 +528,8 @@ class EulerCFGpp(SDXL):
         if zt is None and kwargs.get('zT') is not None:  # an N(0,1) draw, as every other solver accepts it
             zt = kwargs['zT'].to(self.device) * (sigmas[0] ** 2 + 1) ** 0.5
         if zt is None:
-            zt_dim = (1, 4, shape[1] // self.vae_scale_factor, shape[0] // self.vae_scale_factor)
+            zt_dim = (null_prompt_embeds.shape[0], 4, shape[1] // self.vae_scale_factor,
+                      shape[0] // self.vae_scale_factor)
             zt = self.initialize_latent(method="random_kdiffusion", latent_dim=zt_dim, sigmas=sigmas)
         z0t, _ = K.euler_cfgpp_loop(self, zt.to(torch.float16), sigmas, cfg_guidance,
                                     (null_prompt_embeds, prompt_embeds, add_cond_kwargs), callback_fn)
@@ -533,7 +545,7 @@ class EulerCFGppLight(EulerCFGpp, SDXLLightning):
 
     def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
                         callback_fn=None, **kwargs):
-        assert cfg_guidance == 1.0, "CFG should be turned off in the lightning version"
+        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
         return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
                                        callback_fn, **kwargs)
 

@@ -19,6 +19,8 @@ from typing import List
 import numpy as np
 import torch
 
+from .batching import schedule_lambda
+
 NUM_TRAIN_TIMESTEPS = 1000
 
 STEP_NONE, STEP_DDIM_CFGPP, STEP_DDIM_INV_CFGPP, STEP_DPMPP2M_CFGPP, STEP_DDIM_CFG = 0, 1, 2, 3, 4
@@ -79,7 +81,7 @@ class Schedule:
 def _state(t: float, in_scale: float, lam: float, c=(0, 0, 0, 0), d=(0, 0, 0, 0), second_order=0) -> StepStateC:
     s = StepStateC()
     s.t, s.in_scale = float(t), float(in_scale)
-    s.coef.lambda_ = float(np.float32(lam))
+    s.coef.lambda_ = float(np.float32(schedule_lambda(lam)))  # a per-image table (cfgpp_set_guidance) overrides it
     s.coef.c0, s.coef.c1, s.coef.c2, s.coef.c3 = (float(x) for x in c)
     s.coef.d0, s.coef.d1, s.coef.d2, s.coef.d3 = (float(x) for x in d)
     s.coef.second_order = int(second_order)

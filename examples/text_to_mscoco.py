@@ -4,7 +4,9 @@
 The reference loops over the prompts on one GPU. Here prompt i goes to rank i % world (SURVEY section 8e): every rank
 holds a full UNet replica, rank 0's weights are broadcast once over NCCL so the replicas are bit-identical, and there
 is no collective inside the sampling loop. Every rank draws the zT of EVERY image from the seeded CPU generator, in
-order, and keeps its own - so image i is the same picture whatever the world size."""
+order, and keeps its own - so image i is the same picture whatever the world size. `--batch_size B` groups each rank's
+prompts into batches of up to B images that share one trajectory (UNet batch 2B, B <= 8); the zT draws stay per image,
+so image i does not depend on B either (its pixels may differ in the last bits: other GEMM shapes)."""
 import argparse
 import os
 from pathlib import Path
@@ -27,6 +29,27 @@ def read_prompts(path: Path, limit: int = 10000):
         return [ln.strip() for ln in f if ln.strip()][:limit]
 
 
+def rank_batches(n_prompts: int, rank: int, world: int, batch_size: int, latent):
+    """Yield (image indices, zT) for this rank: its prompts (i % world == rank) in order, grouped by `batch_size`.
+    zT is drawn from the CPU generator for every image 0..n-1 in order on every rank, and each rank keeps the draws
+    of its own images."""
+    if batch_size < 1:
+        raise ValueError("--batch_size must be >= 1")
+    mine = set(D.shard_indices(n_prompts, rank, world))
+    idx, zs = [], []
+    for i in range(n_prompts):
+        zT = torch.randn(latent)  # CPU generator, advanced for every image on every rank (see module docstring)
+        if i not in mine:
+            continue
+        idx.append(i)
+        zs.append(zT)
+        if len(idx) == batch_size:
+            yield idx, torch.cat(zs)
+            idx, zs = [], []
+    if idx:
+        yield idx, torch.cat(zs)
+
+
 def main():
     parser = argparse.ArgumentParser(description="Latent Diffusion")
     parser.add_argument("--workdir", type=Path, default="examples/workdir/mscoco")
@@ -39,6 +62,8 @@ def main():
     parser.add_argument("--model", type=str, default='sd15', choices=["sd15", "sd20", "sdxl", "sdxl_lightning"])
     parser.add_argument("--NFE", type=int, default=50)
     parser.add_argument("--seed", type=int, default=42)
+    parser.add_argument("--batch_size", type=int, default=1,
+                        help="images per trajectory (1..8); every image keeps its own zT and result file")
     parser.add_argument("--ckpt_dir", type=Path, default=None,
                         help="diffusers-format pipeline directory (unet/, vae/, text_encoder[_2]/, tokenizer[_2]/); "
                              "default: seeded synthetic weights (nothing can be downloaded here)")
@@ -70,24 +95,24 @@ def main():
         kw["state_dict"] = D.broadcast_state_dict(sd, Wt.unet_param_specs(cfg), device, src=0)
     solver = (get_solver_sdxl if sdxl else get_solver)(args.method, solver_config=solver_config, device=device, **kw)
 
-    mine = set(D.shard_indices(len(text_list), rank, world))
     latent = (1, 4, cfg.sample_size, cfg.sample_size)
-    for i, text in enumerate(text_list):
-        zT = torch.randn(latent)  # CPU generator, advanced for every image on every rank (see module docstring)
-        if i not in mine:
-            continue
-        print(f'[rank {rank}] processing {i + 1}/{len(text_list)}: {text}', flush=True)
+    for idx, zT in rank_batches(len(text_list), rank, world, args.batch_size, latent):
+        texts = [text_list[i] for i in idx]
+        for i, text in zip(idx, texts):
+            print(f'[rank {rank}] processing {i + 1}/{len(text_list)}: {text}', flush=True)
         if sdxl:
-            result = solver.sample(prompt1=[args.null_prompt, text], prompt2=[args.null_prompt, text],
-                                   cfg_guidance=args.cfg_guidance, target_size=(1024, 1024), zT=zT)
+            results = solver.sample(prompt1=[args.null_prompt, texts], prompt2=[args.null_prompt, texts],
+                                    cfg_guidance=args.cfg_guidance, target_size=(1024, 1024), zT=zT)
         else:
-            result = solver.sample(prompt=[args.null_prompt, text], cfg_guidance=args.cfg_guidance, zT=zT)
-        torch.save(result, args.workdir.joinpath(f'{str(i).zfill(5)}.pt'))
-        try:
-            from torchvision.utils import save_image
-            save_image(result, args.workdir.joinpath(f'{str(i).zfill(5)}.png'), normalize=True)
-        except Exception:  # torchvision is optional here
-            pass
+            results = solver.sample(prompt=[args.null_prompt, texts], cfg_guidance=args.cfg_guidance, zT=zT)
+        for j, i in enumerate(idx):
+            result = results[j:j + 1]
+            torch.save(result, args.workdir.joinpath(f'{str(i).zfill(5)}.pt'))
+            try:
+                from torchvision.utils import save_image
+                save_image(result, args.workdir.joinpath(f'{str(i).zfill(5)}.png'), normalize=True)
+            except Exception:  # torchvision is optional here
+                pass
     if world > 1:
         import torch.distributed as dist
         dist.barrier()

@@ -139,6 +139,11 @@ int cfgpp_set_state(cfgpp_handle* h, const void* z_dev, int z_dtype, void* strea
 /* Ancestral samplers: the trajectory's fresh noise, drawn up front in the order the reference's loop would draw it
  * (`torch.randn_like(x)` once per step with sigma_next > 0). noise_dev: fp16 [slots][batch,4,h,w]; copied. */
 int cfgpp_set_noise(cfgpp_handle* h, const void* noise_dev, int slots, void* stream);
+/* Per-image guidance: lambda_host is a host array of n = batch fp32 values (copied; the caller may reuse it on
+ * return). While it is set, the guidance mix of every step (fused cfgpp_run_steps and un-fused cfgpp_apply_step, every
+ * method and second_order bit) uses lambda[b] for image b instead of cfgpp_step_coef.lambda_, with the same rounding.
+ * n = 0 clears it; cfgpp_prepare clears it too. Enqueued on `stream`; a captured trajectory graph stays valid. */
+int cfgpp_set_guidance(cfgpp_handle* h, const float* lambda_host, int n, void* stream);
 /* Run `nsteps` consecutive steps starting at schedule index `first_step` on the internal state. */
 int cfgpp_run_steps(cfgpp_handle* h, int first_step, int nsteps, void* stream);
 /* which: 0 = state z (same dtype as the state), 1 = z0t of the last executed step. */
@@ -250,6 +255,11 @@ int cfgpp_op_layernorm(const void* x, int M, int C, const void* gamma, const voi
 int cfgpp_op_cfgpp_step(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype,
                         const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out, const void* noise_dev,
                         void* stream);
+/* cfgpp_op_cfgpp_step with a per-image guidance table: lambda_dev fp32 [batch] (device), element i of the n belongs to
+ * image i / (n / batch) and mixes with lambda_dev[image]; lambda_dev = NULL uses coef_host->lambda_. */
+int cfgpp_op_cfgpp_step_guided(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype,
+                               const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
+                               const void* noise_dev, const float* lambda_dev, int batch, void* stream);
 
 #ifdef __cplusplus
 }
