@@ -225,3 +225,211 @@ def op_cfgpp_step_guided(eps_uc: torch.Tensor, eps_c: torch.Tensor, method: int,
                                          byref(coef), ptr(z), ptr(aux), ptr(z0t), ptr(noise), ptr(lambdas),
                                          c_int(z.shape[0]), stream_ptr()))
     return z0t
+
+
+def op_timestep_embedding(vals: torch.Tensor, n: int, dim: int, out: torch.Tensor | None = None, val_stride: int = 1,
+                          col_off: int = 0) -> torch.Tensor:
+    """Sinusoidal embedding of the fp32 values vals[i * val_stride], i < n: row i of out gets cos at columns
+    [col_off, col_off + dim/2) and sin at [col_off + dim/2, col_off + dim), fp16; other columns are left as they are.
+    Without `out`, returns a fresh [n, dim] tensor."""
+    lib = load()
+    assert vals.dtype == torch.float32 and vals.dim() == 1 and vals.numel() >= (n - 1) * val_stride + 1
+    if out is None:
+        out = torch.empty((n, dim), dtype=torch.float16, device=vals.device)
+    assert out.dtype == torch.float16 and out.dim() == 2 and out.shape[0] >= n and col_off + dim <= out.shape[1]
+    check(lib.cfgpp_op_timestep_embedding(ptr(vals), c_int(val_stride), c_int(n), c_int(dim), ptr(out),
+                                          c_int(out.stride(0)), c_int(col_off), stream_ptr()))
+    return out
+
+
+def op_small_linear(x: torch.Tensor, w: torch.Tensor, bias=None, addend=None, rows: int | None = None,
+                    out_silu: bool = False, want_out2: bool = False):
+    """Tiny-M linear: x [R, K] (or [1, K] broadcast to `rows` rows, the kernel's ld_in = 0), w [N, K] fp16. Returns
+    (out [R, N], out2 [R, N] = fp16(SiLU(out)) or None)."""
+    lib = load()
+    K = x.shape[1]
+    N = w.shape[0]
+    R = x.shape[0] if rows is None else rows
+    ld_in = 0 if rows is not None else K
+    assert rows is None or x.shape[0] == 1
+    assert w.shape[1] == K and (addend is None or addend.shape == (R, N))
+    # NaN-filled, so a row or column the kernel fails to write shows
+    out = torch.full((R, N), float("nan"), dtype=torch.float16, device=x.device)
+    out2 = torch.full_like(out, float("nan")) if want_out2 else None
+    check(lib.cfgpp_op_small_linear(ptr(x), c_int(ld_in), ptr(w), ptr(bias), ptr(addend), c_int(N), ptr(out), c_int(N),
+                                    ptr(out2), c_int(R), c_int(N), c_int(K), c_int(1 if out_silu else 0),
+                                    stream_ptr()))
+    return out, out2
+
+
+def op_copy_rows(src: torch.Tensor, dst: torch.Tensor, rows: int, col_off: int = 0) -> torch.Tensor:
+    """dst[r, col_off:col_off + cols] = src[r % src_rows] for r < rows, in place; src [src_rows, cols] fp16."""
+    lib = load()
+    src_rows, cols = src.shape
+    assert dst.dtype == torch.float16 and dst.shape[0] >= rows and col_off + cols <= dst.shape[1]
+    check(lib.cfgpp_op_copy_rows(ptr(src), c_int(src_rows), c_int(cols), ptr(dst), c_int(dst.stride(0)),
+                                 c_int(col_off), c_int(rows), stream_ptr()))
+    return dst
+
+
+def _dtype_code(t: torch.Tensor) -> int:
+    assert t.dtype in (torch.float16, torch.float32)
+    return 0 if t.dtype == torch.float16 else 1
+
+
+def op_conv_in(z: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, in_scale: torch.Tensor | None = None,
+               reps: int = 1) -> torch.Tensor:
+    """conv_in 3x3 pad 1: z [B,4,H,W] fp16 / fp32 NCHW (times the device scalar in_scale, fp32 [1], when given),
+    w [Cout, 36] fp16 (PyTorch's [Cout,4,3,3] flattened) -> [reps * B, H, W, Cout] NHWC fp16."""
+    lib = load()
+    B, Cin, H, W = z.shape
+    Cout = w.shape[0]
+    assert Cin == 4 and w.shape == (Cout, 36)
+    assert in_scale is None or (in_scale.dtype == torch.float32 and in_scale.numel() == 1)
+    out = torch.empty((reps * B, H, W, Cout), dtype=torch.float16, device=z.device)
+    check(lib.cfgpp_op_conv_in(ptr(z), c_int(_dtype_code(z)), ptr(in_scale), ptr(w), ptr(bias), ptr(out), c_int(B),
+                               c_int(H), c_int(W), c_int(Cout), c_int(reps), stream_ptr()))
+    return out
+
+
+def op_conv_out_step(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, method: int = 0, coef=None,
+                     z: torch.Tensor | None = None, aux: torch.Tensor | None = None, want_z0t: bool = True,
+                     noise: torch.Tensor | None = None, lambdas: torch.Tensor | None = None):
+    """conv_out 3x3 (Cin -> 4) on x [2B,H,W,Cin] NHWC fp16, w [4, 9, Cin] (`w.permute(0, 2, 3, 1)`), fused with the
+    step `method` on the state z [B,4,H,W] (in place). Returns (eps_uc, eps_c, z0t or None); method 0 (STEP_NONE) only
+    writes the eps. noise / lambdas as in op_cfgpp_step_guided."""
+    from ctypes import byref
+    lib = load()
+    B2, H, W, Cin = x.shape
+    B = B2 // 2
+    assert B2 == 2 * B and w.shape == (4, 9, Cin)
+    eps_uc = torch.empty((B, 4, H, W), dtype=torch.float16, device=x.device)
+    eps_c = torch.empty_like(eps_uc)
+    z0t = None
+    code = 1
+    if method != 0:
+        assert z is not None and z.shape == (B, 4, H, W) and coef is not None
+        z0t = torch.empty_like(z) if want_z0t else None
+        code = _dtype_code(z)
+    if lambdas is not None:
+        assert lambdas.dtype == torch.float32 and lambdas.shape == (B,)
+    check(lib.cfgpp_op_conv_out_step(ptr(x), ptr(w), ptr(bias), c_int(B), c_int(H), c_int(W), c_int(Cin),
+                                     c_int(method), c_int(code), byref(coef) if coef is not None else c_void_p(0),
+                                     ptr(z), ptr(aux), ptr(z0t), ptr(eps_uc), ptr(eps_c), ptr(noise), ptr(lambdas),
+                                     stream_ptr()))
+    return eps_uc, eps_c, z0t
+
+
+def op_upsample2x(x: torch.Tensor) -> torch.Tensor:
+    """nearest 2x: x [B,H,W,C] NHWC fp16 -> [B,2H,2W,C]."""
+    lib = load()
+    B, H, W, C = x.shape
+    out = torch.empty((B, 2 * H, 2 * W, C), dtype=torch.float16, device=x.device)
+    check(lib.cfgpp_op_upsample2x(ptr(x), ptr(out), c_int(B), c_int(H), c_int(W), c_int(C), stream_ptr()))
+    return out
+
+
+def op_im2col_s2(x: torch.Tensor) -> torch.Tensor:
+    """stride-2 pad-1 3x3 im2col: x [B,H,W,C] NHWC fp16 -> [B * H/2 * W/2, 9 * C] (tap-major)."""
+    lib = load()
+    B, H, W, C = x.shape
+    out = torch.empty((B * (H // 2) * (W // 2), 9 * C), dtype=torch.float16, device=x.device)
+    check(lib.cfgpp_op_im2col_s2(ptr(x), ptr(out), c_int(B), c_int(H), c_int(W), c_int(C), stream_ptr()))
+    return out
+
+
+def op_vae_latent_prep(z: torch.Tensor, scaling: float, w: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
+    """fp16(w @ fp16(z / scaling) + bias) per pixel: z [B,4,H,W] fp16 / fp32, w [4, 4] fp16 -> [B,4,H,W] fp16."""
+    lib = load()
+    B, C, H, W = z.shape
+    assert C == 4 and w.shape == (4, 4)
+    out = torch.empty((B, 4, H, W), dtype=torch.float16, device=z.device)
+    check(lib.cfgpp_op_vae_latent_prep(ptr(z), c_int(_dtype_code(z)), c_float(scaling), ptr(w), ptr(bias), ptr(out),
+                                       c_int(B), c_int(H * W), stream_ptr()))
+    return out
+
+
+def op_vae_row_softmax(s: torch.Tensor, scale: float) -> torch.Tensor:
+    """In-place softmax(s * scale) over the rows of s [rows, n] fp16."""
+    lib = load()
+    rows, n = s.shape
+    check(lib.cfgpp_op_vae_row_softmax(ptr(s), c_int(rows), c_int(n), c_float(scale), stream_ptr()))
+    return s
+
+
+def op_vae_conv_rgb(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
+    """conv 3x3 pad 1, C -> 3: x [B,H,W,C] NHWC fp16, w [3, 9, C] -> [B,3,H,W] NCHW fp16."""
+    lib = load()
+    B, H, W, C = x.shape
+    assert w.shape == (3, 9, C)
+    out = torch.empty((B, 3, H, W), dtype=torch.float16, device=x.device)
+    check(lib.cfgpp_op_vae_conv_rgb(ptr(x), ptr(w), ptr(bias), ptr(out), c_int(B), c_int(H), c_int(W), c_int(C),
+                                    stream_ptr()))
+    return out
+
+
+def op_vae_image_pad(x: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
+    """image [B,3,H,W] fp16 / fp32 -> [B,4,H,W] fp16 with a zero fourth plane (into `out` when given)."""
+    lib = load()
+    B, C, H, W = x.shape
+    assert C == 3
+    if out is None:
+        out = torch.empty((B, 4, H, W), dtype=torch.float16, device=x.device)
+    assert out.shape == (B, 4, H, W) and out.dtype == torch.float16 and out.is_contiguous()
+    check(lib.cfgpp_op_vae_image_pad(ptr(x), c_int(_dtype_code(x)), ptr(out), c_int(B), c_int(H), c_int(W),
+                                     stream_ptr()))
+    return out
+
+
+def op_vae_moments_sample(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, wq: torch.Tensor, bq: torch.Tensor,
+                          scaling: float, noise: torch.Tensor | None = None) -> torch.Tensor:
+    """Encoder tail: conv 3x3 C -> 8 on x [B,H,W,C] NHWC (w [8, 9, C]), quant_conv (wq [8, 8], bq [8]), then
+    (mean + exp(clamp(logvar, -30, 20) / 2) * noise) * scaling -> [B,4,H,W] fp32; noise [B,4,H,W] fp16 or None."""
+    lib = load()
+    B, H, W, C = x.shape
+    assert w.shape == (8, 9, C) and wq.shape == (8, 8)
+    out = torch.empty((B, 4, H, W), dtype=torch.float32, device=x.device)
+    check(lib.cfgpp_op_vae_moments_sample(ptr(x), ptr(w), ptr(bias), ptr(wq), ptr(bq), ptr(noise), c_float(scaling),
+                                          ptr(out), c_int(B), c_int(H), c_int(W), c_int(C), stream_ptr()))
+    return out
+
+
+def op_clip_embed(ids: torch.Tensor, tok: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
+    """ids [M] int32 -> [M, D] fp16 = fp16(tok[ids[r]] + pos[r % T]); tok [vocab, D], pos [T, D]."""
+    lib = load()
+    vocab, D = tok.shape
+    T = pos.shape[0]
+    assert ids.dtype == torch.int32 and ids.dim() == 1 and pos.shape[1] == D
+    out = torch.empty((ids.numel(), D), dtype=torch.float16, device=tok.device)
+    check(lib.cfgpp_op_clip_embed(ptr(ids), ptr(tok), ptr(pos), ptr(out), c_int(ids.numel()), c_int(T), c_int(D),
+                                  c_int(vocab), stream_ptr()))
+    return out
+
+
+def op_clip_attention(qkv: torch.Tensor, B: int, T: int, heads: int) -> torch.Tensor:
+    """Causal self-attention of the CLIP towers: qkv [B*T, 3D] fp16 (q | k | v, 64-wide heads) -> [B*T, D]."""
+    lib = load()
+    D = qkv.shape[1] // 3
+    assert qkv.shape == (B * T, 3 * D)
+    out = torch.empty((B * T, D), dtype=torch.float16, device=qkv.device)
+    check(lib.cfgpp_op_clip_attention(ptr(qkv), ptr(out), c_int(B), c_int(T), c_int(heads), c_int(D), stream_ptr()))
+    return out
+
+
+def op_clip_activation(x: torch.Tensor, mode: int) -> torch.Tensor:
+    """In place on fp16 x (numel % 8 == 0): mode 0 quick_gelu, 1 gelu (erf)."""
+    lib = load()
+    assert x.dtype == torch.float16
+    check(lib.cfgpp_op_clip_activation(ptr(x), ctypes.c_size_t(x.numel()), c_int(mode), stream_ptr()))
+    return x
+
+
+def op_clip_gather_rows(x: torch.Tensor, index: torch.Tensor, T: int) -> torch.Tensor:
+    """out[b] = x[b * T + index[b]]: x [B*T, D] fp16, index [B] int32 -> [B, D]."""
+    lib = load()
+    BT, D = x.shape
+    B = index.numel()
+    assert index.dtype == torch.int32 and BT == B * T
+    out = torch.empty((B, D), dtype=torch.float16, device=x.device)
+    check(lib.cfgpp_op_clip_gather_rows(ptr(x), ptr(index), ptr(out), c_int(B), c_int(T), c_int(D), stream_ptr()))
+    return out

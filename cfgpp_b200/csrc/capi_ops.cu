@@ -126,36 +126,57 @@ CFGPP_API int cfgpp_op_layernorm(const void* x, int M, int C, const void* gamma,
   });
 }
 
+}  // extern "C"
+
 namespace {
-// One step-only launch with the coefficients and the two table words (noise, guidance) in a scratch device block.
-void op_step(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype, const cfgpp_step_coef* coef_host,
-             void* z, void* aux, void* z0t_out, const void* noise_dev, const float* lambda_dev, int batch,
-             cudaStream_t stream) {
+// Runs one step launch `launch(coef_dev, noise_slot, lambda_slot)` with the coefficients (zeros when coef_host is null)
+// and the two table words (noise, guidance) in a scratch device block, then synchronises and frees the block.
+// lambda_slot is null when there is no guidance table.
+template <class Launch>
+void with_step_block(const cfgpp_step_coef* coef_host, const void* noise_dev, const float* lambda_dev,
+                     cudaStream_t stream, Launch&& launch) {
   static_assert(sizeof(cfgpp_step_coef) == sizeof(StepCoef), "ABI struct mismatch");
   static_assert(sizeof(StepCoef) % sizeof(void*) == 0, "the table words are stored right behind the coefficients");
-  const bool guided = lambda_dev != nullptr;
-  CFGPP_REQUIRE(!guided || (batch >= 1 && n % batch == 0), "guidance table: batch must divide n");
+  const StepCoef zero{};
+  const void* coef_src = coef_host ? static_cast<const void*>(coef_host) : static_cast<const void*>(&zero);
   StepCoef* coef_dev = nullptr;
   CFGPP_CHECK_CUDA(cudaMalloc(&coef_dev, sizeof(StepCoef) + 2 * sizeof(void*)));
   const __half** slot = reinterpret_cast<const __half**>(coef_dev + 1);
   const float** lslot = reinterpret_cast<const float**>(slot + 1);
-  cudaError_t e = cudaMemcpy(coef_dev, coef_host, sizeof(StepCoef), cudaMemcpyHostToDevice);
+  cudaError_t e = cudaMemcpy(coef_dev, coef_src, sizeof(StepCoef), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(slot, &noise_dev, sizeof(void*), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(lslot, &lambda_dev, sizeof(void*), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) {
     try {
-      run_step_only((const __half*)eps_uc, (const __half*)eps_c, n, method | (state_dtype == CFGPP_F16 ? 0x100 : 0),
-                    coef_dev, z, aux, z0t_out, stream, slot, guided ? lslot : nullptr, guided ? n / batch : 0);
+      launch(const_cast<const StepCoef*>(coef_dev), const_cast<const __half* const*>(slot),
+             lambda_dev ? const_cast<const float* const*>(lslot) : nullptr);
     } catch (...) {
       cudaFree(coef_dev);
       throw;
     }
-    e = cudaStreamSynchronize(stream);  // test-only entry point
+    e = cudaStreamSynchronize(stream);  // test-only entry point: scratch freed below
   }
   cudaFree(coef_dev);
   CFGPP_CHECK_CUDA(e);
 }
+
+// One step-only launch from given eps.
+void op_step(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype, const cfgpp_step_coef* coef_host,
+             void* z, void* aux, void* z0t_out, const void* noise_dev, const float* lambda_dev, int batch,
+             cudaStream_t stream) {
+  const bool guided = lambda_dev != nullptr;
+  CFGPP_REQUIRE(!guided || (batch >= 1 && n % batch == 0), "guidance table: batch must divide n");
+  CFGPP_REQUIRE(coef_host != nullptr, "the step needs its coefficients");
+  with_step_block(coef_host, noise_dev, lambda_dev, stream,
+                  [&](const StepCoef* coef_dev, const __half* const* slot, const float* const* lslot) {
+                    run_step_only((const __half*)eps_uc, (const __half*)eps_c, n,
+                                  method | (state_dtype == CFGPP_F16 ? 0x100 : 0), coef_dev, z, aux, z0t_out, stream,
+                                  slot, lslot, guided ? n / batch : 0);
+                  });
+}
 }  // namespace
+
+extern "C" {
 
 CFGPP_API int cfgpp_op_cfgpp_step(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype,
                                   const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
@@ -173,6 +194,61 @@ CFGPP_API int cfgpp_op_cfgpp_step_guided(const void* eps_uc, const void* eps_c, 
     op_step(eps_uc, eps_c, n, method, state_dtype, coef_host, z, aux, z0t_out, noise_dev, lambda_dev, batch,
             (cudaStream_t)stream);
   });
+}
+
+CFGPP_API int cfgpp_op_timestep_embedding(const float* vals, int val_stride, int n, int dim, void* out, int ld,
+                                          int col_off, void* stream) {
+  return guarded([&] {
+    run_sincos_embed(vals, val_stride, n, dim, (__half*)out, ld, col_off, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_small_linear(const void* in, int ld_in, const void* w, const void* bias, const void* addend,
+                                    int ld_add, void* out, int ld_out, void* out2, int R, int N, int K, int out_silu,
+                                    void* stream) {
+  return guarded([&] {
+    run_small_linear((const __half*)in, ld_in, (const __half*)w, (const __half*)bias, (const __half*)addend, ld_add,
+                     (__half*)out, ld_out, (__half*)out2, R, N, K, out_silu != 0, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_copy_rows(const void* src, int src_rows, int cols, void* dst, int ld_dst, int col_off, int R,
+                                 void* stream) {
+  return guarded([&] {
+    run_copy_rows((const __half*)src, src_rows, cols, (__half*)dst, ld_dst, col_off, R, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_conv_in(const void* z, int z_dtype, const float* in_scale_dev, const void* w, const void* bias,
+                               void* out, int B, int H, int W, int Cout, int reps, void* stream) {
+  return guarded([&] {
+    run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, in_scale_dev, (const __half*)w, (const __half*)bias, (__half*)out, B,
+                H, W, Cout, reps, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_conv_out_step(const void* x, const void* w, const void* bias, int B, int H, int W, int Cin,
+                                     int method, int state_dtype, const cfgpp_step_coef* coef_host, void* z, void* aux,
+                                     void* z0t_out, void* eps_uc, void* eps_c, const void* noise_dev,
+                                     const float* lambda_dev, void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(method == CFGPP_STEP_NONE || coef_host != nullptr, "a step method needs its coefficients");
+    const cudaStream_t st = (cudaStream_t)stream;
+    with_step_block(coef_host, noise_dev, lambda_dev, st,
+                    [&](const StepCoef* coef_dev, const __half* const* slot, const float* const* lslot) {
+                      run_conv_out_step((const __half*)x, (const __half*)w, (const __half*)bias, B, H, W, Cin,
+                                        method | (state_dtype == CFGPP_F16 ? 0x100 : 0), coef_dev, z, aux, z0t_out,
+                                        (__half*)eps_uc, (__half*)eps_c, st, slot, lslot);
+                    });
+  });
+}
+
+CFGPP_API int cfgpp_op_upsample2x(const void* x, void* out, int B, int H, int W, int C, void* stream) {
+  return guarded([&] { run_upsample2x((const __half*)x, (__half*)out, B, H, W, C, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_op_im2col_s2(const void* x, void* out, int B, int H, int W, int C, void* stream) {
+  return guarded([&] { run_im2col_s2((const __half*)x, (__half*)out, B, H, W, C, (cudaStream_t)stream); });
 }
 
 }  // extern "C"

@@ -47,4 +47,27 @@ CFGPP_API int cfgpp_clip_stats(cfgpp_clip_handle* h, double* flops, size_t* work
   });
 }
 
+// ---- operator-level entry points (one kernel launch each, on the caller's stream) ----
+CFGPP_API int cfgpp_op_clip_embed(const int32_t* ids, const void* tok, const void* pos, void* out, int M, int T, int D,
+                                  int vocab, void* stream) {
+  return guarded([&] {
+    run_clip_embed(ids, (const __half*)tok, (const __half*)pos, (__half*)out, M, T, D, vocab, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_clip_attention(const void* qkv, void* out, int B, int T, int heads, int D, void* stream) {
+  return guarded([&] { run_clip_attention((const __half*)qkv, (__half*)out, B, T, heads, D, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_op_clip_activation(void* x, size_t n, int mode, void* stream) {
+  return guarded([&] { run_clip_activation((__half*)x, n, mode, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_op_clip_gather_rows(const void* x, const int32_t* index, void* out, int B, int T, int D,
+                                        void* stream) {
+  return guarded([&] {
+    run_clip_gather_rows((const __half*)x, index, (__half*)out, B, T, D, (cudaStream_t)stream);
+  });
+}
+
 }  // extern "C"

@@ -50,4 +50,40 @@ CFGPP_API int cfgpp_vae_stats(cfgpp_vae_handle* h, double* flops, size_t* worksp
   });
 }
 
+// ---- operator-level entry points (one kernel launch each, on the caller's stream) ----
+CFGPP_API int cfgpp_op_vae_latent_prep(const void* z, int z_dtype, float scaling, const void* w, const void* bias,
+                                       void* out, int B, int HW, void* stream) {
+  return guarded([&] {
+    run_vae_latent_prep(z, z_dtype == CFGPP_F16 ? 1 : 0, scaling, (const __half*)w, (const __half*)bias, (__half*)out,
+                        B, HW, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_vae_row_softmax(void* s, int rows, int n, float scale, void* stream) {
+  return guarded([&] {
+    run_vae_row_softmax((__half*)s, rows, n, scale * 1.4426950408889634f, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_vae_conv_rgb(const void* x, const void* w, const void* bias, void* out, int B, int H, int W, int C,
+                                    void* stream) {
+  return guarded([&] {
+    run_vae_conv_rgb((const __half*)x, (const __half*)w, (const __half*)bias, (__half*)out, B, H, W, C,
+                     (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_vae_image_pad(const void* x, int x_dtype, void* out, int B, int H, int W, void* stream) {
+  return guarded([&] { run_vae_image_pad(x, x_dtype == CFGPP_F16 ? 1 : 0, (__half*)out, B, H, W, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_op_vae_moments_sample(const void* x, const void* w, const void* bias, const void* wq, const void* bq,
+                                          const void* noise, float scaling, float* out, int B, int H, int W, int C,
+                                          void* stream) {
+  return guarded([&] {
+    run_vae_moments_sample((const __half*)x, (const __half*)w, (const __half*)bias, (const __half*)wq,
+                           (const __half*)bq, (const __half*)noise, scaling, out, B, H, W, C, (cudaStream_t)stream);
+  });
+}
+
 }  // extern "C"

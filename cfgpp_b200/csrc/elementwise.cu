@@ -21,7 +21,11 @@ __global__ void sincos_kernel(const float* __restrict__ vals, int val_stride, in
   if (idx >= n * half_dim) return;
   const int i = idx / half_dim;
   const int k = idx - i * half_dim;
-  const float freq = expf((-9.210340371976184f * static_cast<float>(k)) / static_cast<float>(half_dim));
+  // diffusers divides the exponent by half_dim, a Python scalar, on the GPU, where torch multiplies by its fp32
+  // reciprocal instead; a true division moves the frequency by up to 1 ulp of the exponent when half_dim is not a
+  // power of two (320, 1280)
+  const float inv_half = 1.0f / static_cast<float>(half_dim);
+  const float freq = expf(__fmul_rn(-9.210340371976184f * static_cast<float>(k), inv_half));
   const float arg = vals[static_cast<size_t>(i) * val_stride] * freq;
   out[static_cast<size_t>(i) * ld + col_off + k] = __float2half_rn(cosf(arg));
   out[static_cast<size_t>(i) * ld + col_off + half_dim + k] = __float2half_rn(sinf(arg));

@@ -109,6 +109,14 @@ __global__ void __launch_bounds__(128) clip_attn_kernel(const __half* __restrict
   }
 }
 
+// quick_gelu as transformers' QuickGELUActivation runs it on an fp16 module, `x * torch.sigmoid(1.702 * x)`: three fp16
+// tensor ops, each computed in fp32 and rounded to fp16 (torch's sigmoid is 1 / (1 + exp(-a)) with the precise expf).
+CFGPP_DEVICE float quick_gelu_f16(float x) {
+  const float a = __half2float(__float2half_rn(1.702f * x));
+  const float s = __half2float(__float2half_rn(1.f / (1.f + expf(-a))));
+  return x * s;  // exact in fp32 (two 11-bit significands); the caller's rounding is the third fp16 op
+}
+
 // In-place MLP activation on fp16: 0 = quick_gelu x * sigmoid(1.702 x) (OpenAI CLIP), 1 = gelu (erf; OpenCLIP bigG)
 __global__ void clip_act_kernel(uint4* __restrict__ x, size_t nvec, int mode) {
   pdl_launch_dependents();
@@ -121,8 +129,8 @@ __global__ void clip_act_kernel(uint4* __restrict__ x, size_t nvec, int mode) {
     for (int k = 0; k < 4; ++k) {
       float2 f = __half22float2(h[k]);
       if (mode == 0) {
-        f.x = f.x / (1.f + __expf(-1.702f * f.x));
-        f.y = f.y / (1.f + __expf(-1.702f * f.y));
+        f.x = quick_gelu_f16(f.x);
+        f.y = quick_gelu_f16(f.y);
       } else {
         f.x = 0.5f * f.x * (1.f + erff(f.x * 0.70710678118654752f));
         f.y = 0.5f * f.y * (1.f + erff(f.y * 0.70710678118654752f));

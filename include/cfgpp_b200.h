@@ -260,6 +260,57 @@ int cfgpp_op_cfgpp_step(const void* eps_uc, const void* eps_c, int n, int method
 int cfgpp_op_cfgpp_step_guided(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype,
                                const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
                                const void* noise_dev, const float* lambda_dev, int batch, void* stream);
+/* Sinusoidal embedding (diffusers get_timestep_embedding, flip_sin_to_cos): value i = vals_dev[i * val_stride] (fp32)
+ * -> out[i * ld + col_off + (0 .. dim/2)] = cos, [.. + dim/2 .. dim) = sin, fp16; other columns are not written. */
+int cfgpp_op_timestep_embedding(const float* vals_dev, int val_stride, int n, int dim, void* out, int ld, int col_off,
+                                void* stream);
+/* Tiny-M linear, R <= 16 rows: in [R, K] with row stride ld_in (0: one row for all R), w [N, K] (K % 8 == 0):
+ * out = fp16(in . w + bias) (+ addend[r * ld_add + n] in fp16), replaced by fp16(SiLU(out)) with out_silu;
+ * out [R, ld_out]; out2 (may be null, same layout) = fp16(SiLU(out)). */
+int cfgpp_op_small_linear(const void* in, int ld_in, const void* w, const void* bias, const void* addend, int ld_add,
+                          void* out, int ld_out, void* out2, int R, int N, int K, int out_silu, void* stream);
+/* dst[r * ld_dst + col_off + c] = src[(r % src_rows) * cols + c], r < R, c < cols (fp16). */
+int cfgpp_op_copy_rows(const void* src, int src_rows, int cols, void* dst, int ld_dst, int col_off, int R, void* stream);
+/* conv_in 3x3 pad 1, 4 -> Cout (Cout % 8 == 0, W % 4 == 0): z [B,4,H,W] NCHW of z_dtype, times *in_scale_dev when
+ * given (fp16 arithmetic for fp16 z), w [Cout][36] fp16, bias [Cout] -> out [reps * B, H, W, Cout] NHWC fp16, the same
+ * B images written reps times. */
+int cfgpp_op_conv_in(const void* z, int z_dtype, const float* in_scale_dev, const void* w, const void* bias, void* out,
+                     int B, int H, int W, int Cout, int reps, void* stream);
+/* conv_out 3x3 pad 1, Cin -> 4 on x [2B,H,W,Cin] NHWC fp16 (rows [0, B) uncond, [B, 2B) cond), w [4][9][Cin] fp16,
+ * fused with the step `method` (CFGPP_STEP_NONE: no update; coef_host may then be null) on the state z [B,4,H,W] of
+ * state_dtype. eps_uc / eps_c (may be null): the conv outputs [B,4,H,W] fp16. noise_dev / lambda_dev as in
+ * cfgpp_op_cfgpp_step_guided (lambda_dev has B entries). Synchronises the stream. */
+int cfgpp_op_conv_out_step(const void* x, const void* w, const void* bias, int B, int H, int W, int Cin, int method,
+                           int state_dtype, const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
+                           void* eps_uc, void* eps_c, const void* noise_dev, const float* lambda_dev, void* stream);
+/* nearest 2x upsample: x [B,H,W,C] NHWC fp16 (C % 8 == 0) -> out [B,2H,2W,C]. */
+int cfgpp_op_upsample2x(const void* x, void* out, int B, int H, int W, int C, void* stream);
+/* stride-2 pad-1 3x3 im2col: x [B,H,W,C] (even H, W; C % 8 == 0) -> out [B * H/2 * W/2, 9 * C], tap-major. */
+int cfgpp_op_im2col_s2(const void* x, void* out, int B, int H, int W, int C, void* stream);
+/* AutoencoderKL decoder front: z [B,4,HW] of z_dtype -> fp16(w . fp16(z / scaling) + bias), w [4][4], out [B,4,HW]. */
+int cfgpp_op_vae_latent_prep(const void* z, int z_dtype, float scaling, const void* w, const void* bias, void* out,
+                             int B, int HW, void* stream);
+/* In-place softmax of every row of s [rows, n] fp16 (n % 8 == 0) of scores * scale. */
+int cfgpp_op_vae_row_softmax(void* s, int rows, int n, float scale, void* stream);
+/* AutoencoderKL decoder conv_out: 3x3 pad 1, C -> 3 on x [B,H,W,C] NHWC, w [3][9][C] -> out [B,3,H,W] NCHW fp16. */
+int cfgpp_op_vae_conv_rgb(const void* x, const void* w, const void* bias, void* out, int B, int H, int W, int C,
+                          void* stream);
+/* image [B,3,H,W] NCHW of x_dtype -> [B,4,H,W] fp16 with a zero fourth plane. */
+int cfgpp_op_vae_image_pad(const void* x, int x_dtype, void* out, int B, int H, int W, void* stream);
+/* AutoencoderKL encoder tail: conv_out 3x3 (C -> 8, w [8][9][C]) on x [B,H,W,C] NHWC, quant_conv (wq [8][8], bq [8]),
+ * logvar clamped to [-30, 20], out [B,4,H,W] fp32 = (mean + exp(logvar / 2) * noise) * scaling; noise [B,4,H,W] fp16
+ * or null (the mean). */
+int cfgpp_op_vae_moments_sample(const void* x, const void* w, const void* bias, const void* wq, const void* bq,
+                                const void* noise, float scaling, float* out, int B, int H, int W, int C, void* stream);
+/* CLIP token + position embedding: out[r] = fp16(tok[ids[r]] + pos[r % T]), r < M; tok [vocab, D], pos [T, D]. */
+int cfgpp_op_clip_embed(const int32_t* ids, const void* tok, const void* pos, void* out, int M, int T, int D, int vocab,
+                        void* stream);
+/* CLIP causal self-attention: qkv [B*T, 3D] (q | k | v, 64-wide heads, D = 64 heads, T <= 128) -> out [B*T, D]. */
+int cfgpp_op_clip_attention(const void* qkv, void* out, int B, int T, int heads, int D, void* stream);
+/* In-place CLIP MLP activation on n fp16 values (n % 8 == 0): mode 0 quick_gelu, 1 gelu (erf). */
+int cfgpp_op_clip_activation(void* x, size_t n, int mode, void* stream);
+/* out[b] = x[b * T + index[b]], x [B*T, D] fp16, out [B, D]. */
+int cfgpp_op_clip_gather_rows(const void* x, const int32_t* index, void* out, int B, int T, int D, void* stream);
 
 #ifdef __cplusplus
 }

@@ -10,7 +10,7 @@ from types import SimpleNamespace
 import pytest
 import torch
 
-from helpers import build_pair, make_inputs, rel_l2
+from helpers import build_pair, coef_variants, make_inputs, rel_l2
 
 pytestmark = pytest.mark.gpu
 dev = torch.device("cuda:0")
@@ -43,37 +43,13 @@ class LatentVAE:
 
 # ---- 1. step kernel: the guidance table reaches every mode and bit, bitwise ---------------------------------------
 
-def _coef_variants():
-    """(method, state dtype, coef, uses aux, noise slots) over every step mode and second_order bit."""
-    from cfgpp_b200 import kdiffusion as K, schedule as S
-    sch = S.Schedule.make(20)
-    out = []
-    for dt in (torch.float32, torch.float16):
-        out.append((S.STEP_DDIM_CFGPP, dt, S.ddim_cfgpp_steps(sch, 0.6, True)[7].coef, False, 0))
-        out.append((S.STEP_DDIM_INV_CFGPP, dt, S.ddim_inversion_cfgpp_steps(sch, 0.6)[5].coef, False, 0))
-        out.append((S.STEP_DDIM_CFG, dt, S.ddim_cfgpp_steps(sch, 0.6, True)[11].coef, False, 0))
-        sigmas = K.get_sigmas_karras(6, 0.03, 14.6, rho=7.)
-        ts = lambda s: torch.tensor(500)  # noqa: E731
-        for cfgpp in (True, False):
-            for second, diff in ((False, False), (True, False), (True, True)):
-                for st in S.kd_steps(sigmas, ts, 0.6, cfgpp, second_order=second, diff_guided=diff)[:3]:
-                    out.append((S.STEP_DPMPP2M_CFGPP, dt, st.coef, True, 0))
-            for two_s in (False, True):
-                steps, slots = S.kd_ancestral_steps(sigmas, ts, 0.6, cfgpp, two_s)
-                for st in steps[:3]:
-                    out.append((S.STEP_DPMPP2M_CFGPP, dt, st.coef, True, slots))
-    bits = {v[2].second_order for v in out if v[0] == S.STEP_DPMPP2M_CFGPP}
-    assert {b_ for b in bits for b_ in (1, 2, 4, 8, 16, 32) if b & b_} == {1, 2, 4, 8, 16, 32}
-    return out
-
-
 def test_step_kernel_guidance_table_bitwise_per_row():
     from cfgpp_b200 import _native as nv
     lams = [0.0, 0.6, 1.0, 7.5]
     shape = (len(lams), 4, 16, 24)
     g = torch.Generator().manual_seed(0)
     lam_dev = torch.tensor(lams, dtype=torch.float32, device=dev)
-    for k, (method, dt, coef, uses_aux, slots) in enumerate(_coef_variants()):
+    for k, (method, dt, coef, uses_aux, slots) in enumerate(coef_variants()):
         eu = torch.randn(shape, generator=g).half().to(dev)
         ec = torch.randn(shape, generator=g).half().to(dev)
         z0 = (torch.randn(shape, generator=g) * 3).to(dt).to(dev)
