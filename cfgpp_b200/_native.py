@@ -67,9 +67,10 @@ def _linear_out(out, M, n_out, device):
 
 def op_linear(a: torch.Tensor, w: torch.Tensor, bias=None, addend=None, add_rows_per_group: int = 1,
               a2: torch.Tensor | None = None, geglu: bool = False, force_bn: int = 0,
-              out: torch.Tensor | None = None) -> torch.Tensor:
+              out: torch.Tensor | None = None, force_streamk: bool = False) -> torch.Tensor:
     """out = epilogue(cat([a, a2], -1) @ w.T); a [M,K1] fp16, w [N,K] fp16 (already packed for GEGLU). `out` may be
-    given, also as the residual `addend` itself (in-place residual add)."""
+    given, also as the residual `addend` itself (in-place residual add). `force_streamk` takes the stream-K remainder
+    split that linear layers otherwise skip (tests of its fix-up path)."""
     lib = load()
     M, K1 = a.shape
     K = K1 + (a2.shape[1] if a2 is not None else 0)
@@ -80,12 +81,13 @@ def op_linear(a: torch.Tensor, w: torch.Tensor, bias=None, addend=None, add_rows
     check(lib.cfgpp_op_linear(ptr(a), c_int(a.stride(0)), ptr(a2), c_int(a2.stride(0) if a2 is not None else 0),
                               c_int(K1), ptr(w), c_int(M), c_int(N), c_int(K), ptr(bias), ptr(addend),
                               c_int(addend.stride(0) if addend is not None else 0), c_int(add_rows_per_group),
-                              ptr(out), c_int(n_out), c_int(1 if geglu else 0), c_int(force_bn), stream_ptr()))
+                              ptr(out), c_int(n_out), c_int(1 if geglu else 0), c_int(force_bn),
+                              c_int(1 if force_streamk else 0), stream_ptr()))
     return out
 
 
 def op_linear_stats(a: torch.Tensor, w: torch.Tensor, bn: int, bias=None, addend=None, add_rows_per_group: int = 1,
-                    out: torch.Tensor | None = None):
+                    out: torch.Tensor | None = None, force_streamk: bool = False):
     """op_linear that also emits the LayerNorm-fold row statistics of its fp16 output (a transformer block's residual
     producer). Returns (out, stats): stats [2 * ceil(N / bn), M, 2] fp32 (sum, sum of squares), part 2 j + h over
     columns [j bn + h bn / 2, j bn + (h + 1) bn / 2)."""
@@ -97,14 +99,15 @@ def op_linear_stats(a: torch.Tensor, w: torch.Tensor, bn: int, bias=None, addend
     stats = torch.empty((2 * ((N + bn - 1) // bn), M, 2), dtype=torch.float32, device=a.device)
     check(lib.cfgpp_op_linear_lnfold(ptr(a), ptr(w), c_int(M), c_int(N), c_int(K), ptr(bias), ptr(addend),
                                      c_int(addend.stride(0) if addend is not None else 0), c_int(add_rows_per_group),
-                                     ptr(out), c_int(N), c_int(0), c_int(bn), ptr(stats), c_void_p(0), c_int(0),
-                                     c_float(0.0), c_void_p(0), c_void_p(0), stream_ptr()))
+                                     ptr(out), c_int(N), c_int(0), c_int(bn), c_int(1 if force_streamk else 0),
+                                     ptr(stats), c_void_p(0), c_int(0), c_float(0.0), c_void_p(0), c_void_p(0),
+                                     stream_ptr()))
     return out, stats
 
 
 def op_linear_lnfold(h: torch.Tensor, wf: torch.Tensor, s: torch.Tensor, t: torch.Tensor, stats: torch.Tensor,
                      eps: float = 1e-5, geglu: bool = False, force_bn: int = 0, ln_parts: int | None = None,
-                     out: torch.Tensor | None = None) -> torch.Tensor:
+                     out: torch.Tensor | None = None, force_streamk: bool = False) -> torch.Tensor:
     """LayerNorm(h) @ w.T + bias as the folded GEMM: h [M,C] fp16, (wf, s, t) from op_fold_ln, stats [parts, M, 2]
     fp32 row (sum, sum of squares) partials of h (op_linear_stats, or any split of the columns)."""
     lib = load()
@@ -117,8 +120,8 @@ def op_linear_lnfold(h: torch.Tensor, wf: torch.Tensor, s: torch.Tensor, t: torc
     out = _linear_out(out, M, n_out, h.device)
     check(lib.cfgpp_op_linear_lnfold(ptr(h), ptr(wf), c_int(M), c_int(N), c_int(K), c_void_p(0), c_void_p(0), c_int(0),
                                      c_int(1), ptr(out), c_int(n_out), c_int(1 if geglu else 0), c_int(force_bn),
-                                     c_void_p(0), ptr(stats), c_int(parts), c_float(eps), ptr(s), ptr(t),
-                                     stream_ptr()))
+                                     c_int(1 if force_streamk else 0), c_void_p(0), ptr(stats), c_int(parts),
+                                     c_float(eps), ptr(s), ptr(t), stream_ptr()))
     return out
 
 
@@ -326,15 +329,6 @@ def op_upsample2x(x: torch.Tensor) -> torch.Tensor:
     B, H, W, C = x.shape
     out = torch.empty((B, 2 * H, 2 * W, C), dtype=torch.float16, device=x.device)
     check(lib.cfgpp_op_upsample2x(ptr(x), ptr(out), c_int(B), c_int(H), c_int(W), c_int(C), stream_ptr()))
-    return out
-
-
-def op_im2col_s2(x: torch.Tensor) -> torch.Tensor:
-    """stride-2 pad-1 3x3 im2col: x [B,H,W,C] NHWC fp16 -> [B * H/2 * W/2, 9 * C] (tap-major)."""
-    lib = load()
-    B, H, W, C = x.shape
-    out = torch.empty((B * (H // 2) * (W // 2), 9 * C), dtype=torch.float16, device=x.device)
-    check(lib.cfgpp_op_im2col_s2(ptr(x), ptr(out), c_int(B), c_int(H), c_int(W), c_int(C), stream_ptr()))
     return out
 
 

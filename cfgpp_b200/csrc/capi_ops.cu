@@ -13,26 +13,27 @@ extern "C" {
 
 CFGPP_API int cfgpp_op_linear(const void* a, int lda, const void* a2, int lda2, int k_split, const void* w, int M,
                               int N, int K, const void* bias, const void* addend, int ld_add,
-                              int add_rows_per_group, void* out, int ldc, int geglu, int force_bn, void* stream) {
+                              int add_rows_per_group, void* out, int ldc, int geglu, int force_bn, int force_streamk,
+                              void* stream) {
   return guarded([&] {
     GemmOp op = make_linear_op((const __half*)a, lda, (const __half*)a2, lda2, k_split, (const __half*)w, M, N, K,
                                (const __half*)bias, (const __half*)addend, ld_add, add_rows_per_group, (__half*)out,
-                               ldc, geglu != 0, force_bn);
+                               ldc, geglu != 0, force_bn, force_streamk != 0);
     run_gemm_op(op, (cudaStream_t)stream);
   });
 }
 
 CFGPP_API int cfgpp_op_linear_lnfold(const void* a, const void* w, int M, int N, int K, const void* bias,
                                      const void* addend, int ld_add, int add_rows_per_group, void* out, int ldc,
-                                     int geglu, int force_bn, float* stats_out, const float* stats_in, int ln_parts,
-                                     float ln_eps, const float* ln_s, const float* ln_t, void* stream) {
+                                     int geglu, int force_bn, int force_streamk, float* stats_out, const float* stats_in,
+                                     int ln_parts, float ln_eps, const float* ln_s, const float* ln_t, void* stream) {
   return guarded([&] {
     CFGPP_REQUIRE((stats_out != nullptr) != (stats_in != nullptr), "exactly one of stats_out / stats_in");
     CFGPP_REQUIRE(stats_out == nullptr || force_bn != 0, "a statistics producer needs an explicit tile width");
     CFGPP_REQUIRE(stats_in == nullptr || (ln_parts >= 1 && ln_s && ln_t), "a LayerNorm-fold consumer needs parts, s, t");
     GemmOp op = make_linear_op((const __half*)a, K, nullptr, 0, 0, (const __half*)w, M, N, K, (const __half*)bias,
                                (const __half*)addend, ld_add, add_rows_per_group, (__half*)out, ldc, geglu != 0,
-                               force_bn);
+                               force_bn, force_streamk != 0);
     op.p.stats_out = stats_out;
     if (stats_in) {
       op.p.stats_in = stats_in;
@@ -245,10 +246,6 @@ CFGPP_API int cfgpp_op_conv_out_step(const void* x, const void* w, const void* b
 
 CFGPP_API int cfgpp_op_upsample2x(const void* x, void* out, int B, int H, int W, int C, void* stream) {
   return guarded([&] { run_upsample2x((const __half*)x, (__half*)out, B, H, W, C, (cudaStream_t)stream); });
-}
-
-CFGPP_API int cfgpp_op_im2col_s2(const void* x, void* out, int B, int H, int W, int C, void* stream) {
-  return guarded([&] { run_im2col_s2((const __half*)x, (__half*)out, B, H, W, C, (cudaStream_t)stream); });
 }
 
 }  // extern "C"

@@ -1,5 +1,5 @@
 // cfgpp_b200 — small / HBM-bound kernels of the UNet step: timestep embeddings, tiny-M linears, conv_in, conv_out fused
-// with the CFG++ guidance mix + scheduler update, nearest-2x upsample, stride-2 im2col. See ops.cuh.
+// with the CFG++ guidance mix + scheduler update, nearest-2x upsample. See ops.cuh.
 #include <algorithm>
 
 #include "common.cuh"
@@ -422,28 +422,6 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict
   }
 }
 
-__global__ void im2col_s2_kernel(const uint4* __restrict__ x, uint4* __restrict__ out, int B, int H, int W, int Cv) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const int Ho = H >> 1, Wo = W >> 1;
-  const size_t total = static_cast<size_t>(B) * Ho * Wo * 9 * Cv;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int cv = i % Cv;
-    size_t t = i / Cv;
-    const int tap = t % 9;
-    t /= 9;
-    const int ow = t % Wo;
-    t /= Wo;
-    const int oh = t % Ho;
-    const int b = t / Ho;
-    const int hh = 2 * oh + tap / 3 - 1, ww = 2 * ow + tap % 3 - 1;
-    uint4 v = make_uint4(0, 0, 0, 0);
-    if (hh >= 0 && hh < H && ww >= 0 && ww < W) v = x[((static_cast<size_t>(b) * H + hh) * W + ww) * Cv + cv];
-    out[i] = v;
-  }
-}
-
 }  // namespace
 
 void run_sincos_embed(const float* vals, int val_stride, int n, int dim, __half* out, int ld, int col_off,
@@ -518,14 +496,6 @@ void run_upsample2x(const __half* x, __half* out, int B, int H, int W, int C, cu
   const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, num_sms() * 16));
   launch_pdl(upsample2x_kernel, dim3(blocks), dim3(256), 0, stream, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(out), B, H,
                                                 W, C / 8);
-}
-
-void run_im2col_s2(const __half* x, __half* out, int B, int H, int W, int C, cudaStream_t stream) {
-  CFGPP_REQUIRE(C % 8 == 0 && H % 2 == 0 && W % 2 == 0, "im2col_s2 shape");
-  const size_t total = static_cast<size_t>(B) * (H / 2) * (W / 2) * 9 * (C / 8);
-  const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, num_sms() * 16));
-  launch_pdl(im2col_s2_kernel, dim3(blocks), dim3(256), 0, stream, reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(out), B, H,
-                                               W, C / 8);
 }
 
 }  // namespace cfgpp

@@ -596,52 +596,9 @@ void launch(const GemmOp& op, cudaStream_t stream) {
              op.map_a2, op.map_b, op.map_out, op.map_res);
 }
 
-// CFGPP_NO_STREAMK=1 switches the remainder stream-K off (A/B runs); it is also off when the two CFG halves run as
-// concurrent launch plans (CFGPP_SPLIT=1), because the partial-accumulator workspace is shared by all launches of a stream.
-bool streamk_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("CFGPP_NO_STREAMK");
-    const char* sp = getenv("CFGPP_SPLIT");
-    v = ((e && e[0] == '1') || (sp && sp[0] == '1')) ? 0 : 1;
-  }
-  return v == 1;
-}
-double streamk_min_saved() {  // k-blocks of main loop the split must save per CTA (CFGPP_STREAMK_MIN overrides)
-  static double v = -1.0;
-  if (v < 0) {
-    const char* e = getenv("CFGPP_STREAMK_MIN");
-    v = e ? atof(e) : 4.0;
-  }
-  return v;
-}
-// Tile walk of the linear layers: N-fastest, so the CTAs running concurrently cover few M blocks and every A tile is
-// fetched from HBM about once (large activations do not survive num_n_blocks M-fastest passes through the L2).
-// CFGPP_RASTER=0 restores the M-fastest walk; the convolutions keep it.
-int raster_mode() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("CFGPP_RASTER");
-    v = e ? atoi(e) : 1;
-  }
-  return v;
-}
-bool streamk_linear() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("CFGPP_STREAMK_LINEAR");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
-}
-double streamk_min_piece() {  // smallest piece as a fraction of a tile's k-blocks (CFGPP_STREAMK_PIECE overrides)
-  static double v = -1.0;
-  if (v < 0) {
-    const char* e = getenv("CFGPP_STREAMK_PIECE");
-    v = e ? atof(e) : 0.5;
-  }
-  return v;
-}
+constexpr double kSkMinSaved = 4.0;  // k-blocks of main loop the split must save per CTA
+constexpr double kSkMinPiece = 0.5;  // smallest piece as a fraction of a tile's k-blocks
+
 // Stream-K workspace: partial accumulators for up to kSkMaxCtas CTAs ([128 x 256] fp32 each) + the flag words. Launches that
 // share a workspace must be stream-ordered (the flags are per CTA id), so every model handle owns one
 // (StreamKScope around its plan building; a handle runs on one stream at a time) and the operator-level entry points
@@ -690,14 +647,17 @@ int choose_bn(int M, int N, bool geglu) {
   return best;
 }
 
-void finish_op(GemmOp& op, const __half* w, int force_bn) {
+void finish_op(GemmOp& op, const __half* w, int force_bn, bool force_streamk) {
   GemmParams& p = op.p;
   op.bn = force_bn ? force_bn : choose_bn(p.M, p.N, p.geglu != 0);
   CFGPP_REQUIRE(op.bn == 64 || op.bn == 128 || op.bn == 160 || op.bn == 256, "unsupported BN");
   if (p.geglu) CFGPP_REQUIRE(op.bn == 256 && p.N % 256 == 0, "GEGLU needs N % 256 == 0");
   p.num_m_blocks = (p.M + BM - 1) / BM;
   p.num_n_blocks = (p.N + op.bn - 1) / op.bn;
-  p.raster = p.conv ? 0 : raster_mode();
+  // Tile walk of the linear layers: N-fastest, so the CTAs running concurrently cover few M blocks and every A tile is
+  // fetched from HBM about once (large activations do not survive num_n_blocks M-fastest passes through the L2). The
+  // convolutions keep the M-fastest walk.
+  p.raster = p.conv ? 0 : 1;
   op.map_b = make_tmap_2d(w, p.N, p.K, p.K, op.bn);
   const int n_out = p.geglu ? p.N / 2 : p.N;
   op.map_out = make_tmap_2d_sw64(p.out, p.M, n_out, p.ldc, 16);  // one epilogue warp's [16 x 32] block
@@ -715,17 +675,16 @@ void finish_op(GemmOp& op, const __half* w, int force_bn) {
   p.sk_ws = nullptr;
   p.sk_flags = nullptr;
   const int rem = groups % max_ctas;
-  if (streamk_enabled() && rem != 0 && max_ctas <= kSkMaxCtas) {
+  if (rem != 0 && max_ctas <= kSkMaxCtas) {
     // The parked partial and the fix-up cost a fixed few microseconds per launch that only long main loops amortise,
     // so the implicit-GEMM convolutions take the split and the linear layers keep the plain tile walk
-    // (CFGPP_STREAMK_LINEAR=1 forces it on for them; CFGPP_STREAMK_MIN / _PIECE tune the thresholds).
+    // (force_streamk, for tests, takes the split for any op whose pieces are at least 2 k-blocks deep).
     const double piece = static_cast<double>(rem) * p.num_k_blocks / max_ctas;
     const double saved = (p.num_k_blocks - piece) * op.bn / 160.0;
-    const bool eligible = p.conv || streamk_linear();
     // pieces at least half a tile deep (a tile then has at most three pieces, i.e. <= 2 partials to sum), unless the
     // saving is large anyway: with fewer tiles than CTAs and a long K every CTA takes a fraction of a tile
-    const bool deep_enough = piece >= streamk_min_piece() * p.num_k_blocks || saved >= 60.0;
-    if (eligible && saved >= streamk_min_saved() && piece >= 2.0 && deep_enough) {
+    const bool deep_enough = piece >= kSkMinPiece * p.num_k_blocks || saved >= 60.0;
+    if (piece >= 2.0 && (force_streamk || (p.conv && saved >= kSkMinSaved && deep_enough))) {
       op.grid = max_ctas;  // all CTAs take part, also when there are fewer tiles than CTAs
       streamk_buffers(&p.sk_ws, &p.sk_flags);
     }
@@ -767,7 +726,7 @@ void gemm_configure() {
 
 GemmOp make_linear_op(const __half* a, int lda, const __half* a2, int lda2, int k_split, const __half* w, int M,
                       int N, int K, const __half* bias, const __half* addend, int ld_add, int add_rows_per_group,
-                      __half* out, int ldc, bool geglu, int force_bn) {
+                      __half* out, int ldc, bool geglu, int force_bn, bool force_streamk) {
   GemmOp op{};
   GemmParams& p = op.p;
   CFGPP_REQUIRE(K % BK == 0, "linear K must be a multiple of 64");
@@ -782,7 +741,7 @@ GemmOp make_linear_op(const __half* a, int lda, const __half* a2, int lda2, int 
   p.out = out; p.ldc = ldc; p.geglu = geglu ? 1 : 0;
   op.map_a = make_tmap_2d(a, M, a2 ? k_split : K, lda, BM);
   op.map_a2 = a2 ? make_tmap_2d(a2, M, K - k_split, lda2, BM) : op.map_a;
-  finish_op(op, w, force_bn);
+  finish_op(op, w, force_bn, force_streamk);
   return op;
 }
 
@@ -817,7 +776,7 @@ GemmOp make_conv3x3_op(const __half* x, int B, int H, int W, int Cin, const __ha
   uint32_t estr[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
   op.map_a = make_tmap_f16(x, 4, dims, strides, box, 128, estr);
   op.map_a2 = op.map_a;
-  finish_op(op, w, force_bn);
+  finish_op(op, w, force_bn, false);
   return op;
 }
 

@@ -65,9 +65,10 @@ struct GemmOp {
 };
 
 // Linear: A [M,K] with leading dim lda (elements). Optional second source a2 (cols k_split..K) with lda2.
+// force_streamk (tests only): take the stream-K remainder split whenever the pieces are at least 2 k-blocks deep.
 GemmOp make_linear_op(const __half* a, int lda, const __half* a2, int lda2, int k_split, const __half* w, int M,
                       int N, int K, const __half* bias, const __half* addend, int ld_add, int add_rows_per_group,
-                      __half* out, int ldc, bool geglu, int force_bn = 0);
+                      __half* out, int ldc, bool geglu, int force_bn = 0, bool force_streamk = false);
 
 // Conv3x3 stride 1 pad 1 on NHWC input x [B,H,W,Cin], weight [Cout][9][Cin], out NHWC [B,H,W,Cout].
 // stride 2: x is [B,H,W,Cin] with even H, W; out is [B,H/2,W/2,Cout]; pad 1 (UNet Downsample2D) or pad 0 (the

@@ -3,7 +3,6 @@
 
 #include <cudaTypedefs.h>
 
-#include <cstdlib>
 #include <mutex>
 
 namespace cfgpp {
@@ -14,19 +13,8 @@ int num_sms() {
     int dev = 0;
     CFGPP_CHECK_CUDA(cudaGetDevice(&dev));
     CFGPP_CHECK_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
-    const char* cap = getenv("CFGPP_SM_CAP");  // experiment knob: persistent grids use at most this many SMs
-    if (cap && atoi(cap) > 0 && atoi(cap) < n) n = atoi(cap);
   }
   return n;
-}
-
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("CFGPP_NO_PDL");
-    v = (e && e[0] == '1') ? 0 : 1;
-  }
-  return v == 1;
 }
 
 static PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {

@@ -33,40 +33,22 @@ struct Error : public std::runtime_error {
   } while (0)
 
 int num_sms();
-bool pdl_enabled();  // false when CFGPP_NO_PDL=1 is set in the environment (A/B switch)
 
 // Launch with programmatic dependent launch enabled (see common.cuh). Capturable into CUDA graphs.
 template <typename... KArgs, typename... Args>
-inline void launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                               int cluster_x, Args&&... args) {
+inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                       Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int n = 0;
-  if (cluster_x > 1) {
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = cluster_x;
-    attr[n].val.clusterDim.y = 1;
-    attr[n].val.clusterDim.z = 1;
-    ++n;
-  }
-  if (pdl_enabled()) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = n;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
   CFGPP_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(std::forward<Args>(args))...));
-}
-
-template <typename... KArgs, typename... Args>
-inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                       Args&&... args) {
-  launch_pdl_cluster(kernel, grid, block, smem, stream, 1, std::forward<Args>(args)...);
 }
 
 // Generic fp16 tiled tensor map, 128B swizzle. dims/strides innermost first; strides[i] is the byte

@@ -88,7 +88,5 @@ void run_step_only(const __half* eps_uc, const __half* eps_c, int n, int mode, c
                    const float* const* lambda_slot = nullptr, int sample_elems = 0);
 
 void run_upsample2x(const __half* x, __half* out, int B, int H, int W, int C, cudaStream_t stream);
-// stride-2 pad-1 3x3 im2col: x [B,H,W,C] -> out [B*(H/2)*(W/2), 9*C] (tap-major, matches the packed weight)
-void run_im2col_s2(const __half* x, __half* out, int B, int H, int W, int C, cudaStream_t stream);
 
 }  // namespace cfgpp

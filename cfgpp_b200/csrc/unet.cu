@@ -3,7 +3,6 @@
 #include "unet.cuh"
 
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
 
 #include "common.cuh"
@@ -102,18 +101,12 @@ Unet::Unet(const cfgpp_model_desc& d, int device) : d_(d), device_(device) {
   attn_configure();
   streamk_alloc(&sk_ws_, &sk_flags_);
   CFGPP_CHECK_CUDA(cudaStreamCreateWithFlags(&capture_stream_, cudaStreamNonBlocking));
-  CFGPP_CHECK_CUDA(cudaStreamCreateWithFlags(&capture_stream2_, cudaStreamNonBlocking));
-  CFGPP_CHECK_CUDA(cudaEventCreateWithFlags(&fork_ev_, cudaEventDisableTiming));
-  CFGPP_CHECK_CUDA(cudaEventCreateWithFlags(&join_ev_, cudaEventDisableTiming));
 }
 
 Unet::~Unet() {
   if (graph_exec_) cudaGraphExecDestroy(graph_exec_);
   if (graph_) cudaGraphDestroy(graph_);
   if (capture_stream_) cudaStreamDestroy(capture_stream_);
-  if (capture_stream2_) cudaStreamDestroy(capture_stream2_);
-  if (fork_ev_) cudaEventDestroy(fork_ev_);
-  if (join_ev_) cudaEventDestroy(join_ev_);
   for (auto& kv : raw_) cudaFree(kv.second.p);
   for (void* p : weight_allocs_) cudaFree(p);
   for (void* p : act_allocs_) cudaFree(p);
@@ -132,7 +125,6 @@ void Unet::load_weight(const std::string& key, const void* data, const int64_t* 
   t.shape.assign(shape, shape + ndim);
   const size_t n = t.numel();
   CFGPP_CHECK_CUDA(cudaMalloc(&t.p, std::max<size_t>(n, 8) * sizeof(__half)));
-  weight_bytes_ += n * sizeof(__half);
   if (dtype == CFGPP_F16) {
     CFGPP_CHECK_CUDA(cudaMemcpyAsync(t.p, data, n * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
   } else {
@@ -157,7 +149,6 @@ __half* Unet::alloc_weight(size_t numel) {
   void* p = nullptr;
   CFGPP_CHECK_CUDA(cudaMalloc(&p, std::max<size_t>(numel, 8) * sizeof(__half)));
   weight_allocs_.push_back(p);
-  weight_bytes_ += numel * sizeof(__half);
   return static_cast<__half*>(p);
 }
 
@@ -263,15 +254,6 @@ Unet::FoldedLN Unet::folded_ln(const std::string& cache_key, const __half* w_pac
   return f;
 }
 
-bool Unet::lnfold_disabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("CFGPP_NO_LNFOLD");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
-}
-
 void Unet::finalize_weights(cudaStream_t stream) {
   CFGPP_CHECK_CUDA(cudaStreamSynchronize(stream));
   // structural validation: every key the plan will touch must exist (dry walk at a nominal size)
@@ -350,12 +332,11 @@ void Unet::add_attn(const std::string& name, const AttnOp& op) {
 Unet::Act Unet::build_resnet(const std::string& prefix, Act x1, const Act* x2, int Cout, int H, int W, int temb_off) {
   const int C1 = x1.C, C2 = x2 ? x2->C : 0, Cin = C1 + C2;
   const int HW = H * W;
-  const size_t M = static_cast<size_t>(bnb_) * HW;
-  Scratch* s_norm = scratch(btag_ + "norm", M * std::max(Cin, Cout));
-  Scratch* s_h1 = scratch(btag_ + "h1", M * Cout);
-  Scratch* s_sc = (Cin != Cout) ? scratch(btag_ + "shortcut", M * Cout) : nullptr;
-  __half* out = g_dry ? nullptr : (out_override_ ? out_override_ : alloc_act(M * Cout));
-  out_override_ = nullptr;
+  const size_t M = static_cast<size_t>(NB_) * HW;
+  Scratch* s_norm = scratch("norm", M * std::max(Cin, Cout));
+  Scratch* s_h1 = scratch("h1", M * Cout);
+  Scratch* s_sc = (Cin != Cout) ? scratch("shortcut", M * Cout) : nullptr;
+  __half* out = g_dry ? nullptr : alloc_act(M * Cout);
   if (g_dry) {
     // validate keys
     raw(prefix + ".norm1.weight"); raw(prefix + ".norm1.bias"); raw(prefix + ".conv1.weight");
@@ -370,17 +351,16 @@ Unet::Act Unet::build_resnet(const std::string& prefix, Act x1, const Act* x2, i
   const __half *g1 = plain(prefix + ".norm1.weight"), *b1 = plain(prefix + ".norm1.bias");
   const __half *g2 = plain(prefix + ".norm2.weight"), *b2 = plain(prefix + ".norm2.bias");
   const float eps = d_.norm_eps;
-  float* partial = bgn_partial_;
-  const int NB = bnb_;
+  float* partial = gn_partial_;
+  const int NB = NB_;
   __half* normp = s_norm->p;
   __half* h1p = s_h1->p;
   const __half* x1p = x1.p;
   add_step(prefix + ".norm1+silu", [=](cudaStream_t st) {
     run_groupnorm(x1p, C1, x2p, C2, NB, HW, g1, b1, eps, true, partial, normp, st);
   }, 2);
-  add_gemm(prefix + ".conv1", make_conv3x3_op(normp, bnb_, H, W, Cin, packed_conv3x3(prefix + ".conv1.weight"), Cout,
-                                              plain(prefix + ".conv1.bias"), temb_all_ + static_cast<size_t>(brow0_) * temb_total_ + temb_off, temb_total_, HW,
-                                              h1p));
+  add_gemm(prefix + ".conv1", make_conv3x3_op(normp, NB_, H, W, Cin, packed_conv3x3(prefix + ".conv1.weight"), Cout,
+                                              plain(prefix + ".conv1.bias"), temb_all_ + temb_off, temb_total_, HW, h1p));
   add_step(prefix + ".norm2+silu", [=](cudaStream_t st) {
     run_groupnorm(h1p, Cout, nullptr, 0, NB, HW, g2, b2, eps, true, partial, normp, st);
   }, 2);
@@ -391,7 +371,7 @@ Unet::Act Unet::build_resnet(const std::string& prefix, Act x1, const Act* x2, i
                             Cin, plain(prefix + ".conv_shortcut.bias"), nullptr, 0, 1, s_sc->p, Cout, false));
     residual = s_sc->p;
   }
-  add_gemm(prefix + ".conv2", make_conv3x3_op(normp, bnb_, H, W, Cout, packed_conv3x3(prefix + ".conv2.weight"), Cout,
+  add_gemm(prefix + ".conv2", make_conv3x3_op(normp, NB_, H, W, Cout, packed_conv3x3(prefix + ".conv2.weight"), Cout,
                                               plain(prefix + ".conv2.bias"), residual, Cout, 1, out));
   return Act{out, Cout};
 }
@@ -399,7 +379,7 @@ Unet::Act Unet::build_resnet(const std::string& prefix, Act x1, const Act* x2, i
 Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W, int layers, int heads) {
   const int C = x.C;
   const int HW = H * W;
-  const int Mi = bnb_ * HW;
+  const int Mi = NB_ * HW;
   const size_t M = static_cast<size_t>(Mi);
   const int D = d_.cross_attention_dim;
   CFGPP_REQUIRE(C % heads == 0 && C / heads <= 192,
@@ -407,17 +387,17 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
   const int hd = C / heads;
   const int hdp = attn_padded_head_dim(hd);  // heads are zero-padded to a multiple of 64 channels (SD v1.5: 40/80/160)
   const int Cp = heads * hdp;
-  Scratch* s_norm = scratch(btag_ + "norm", M * C);
-  Scratch* s_tok = scratch(btag_ + "tokens", M * C);
-  Scratch* s_qkv = scratch(btag_ + "qkv", M * 3 * Cp);
-  Scratch* s_attn = scratch(btag_ + "attn", M * Cp);
-  Scratch* s_q = scratch(btag_ + "q", M * Cp);
-  Scratch* s_ff = scratch(btag_ + "ff", M * 4 * C);
+  Scratch* s_norm = scratch("norm", M * C);
+  Scratch* s_tok = scratch("tokens", M * C);
+  Scratch* s_qkv = scratch("qkv", M * 3 * Cp);
+  Scratch* s_attn = scratch("attn", M * Cp);
+  Scratch* s_q = scratch("q", M * Cp);
+  Scratch* s_ff = scratch("ff", M * 4 * C);
   Scratch* s_stats[3];
   for (int i = 0; i < 3; ++i)  // [16 N blocks][M] float2 partial row statistics (LayerNorm fold)
-    s_stats[i] = scratch(btag_ + "lnstats" + std::to_string(i), static_cast<size_t>(32) * M * 2 * 2);
+    s_stats[i] = scratch("lnstats" + std::to_string(i), static_cast<size_t>(32) * M * 2 * 2);
   __half* out = g_dry ? nullptr : alloc_act(M * C);
-  const int Mkv = bnb_ * n_ctx_;
+  const int Mkv = NB_ * n_ctx_;
   if (g_dry) {
     raw(prefix + ".norm.weight"); raw(prefix + ".norm.bias"); raw(prefix + ".proj_in.weight");
     raw(prefix + ".proj_in.bias"); raw(prefix + ".proj_out.weight"); raw(prefix + ".proj_out.bias");
@@ -435,32 +415,28 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
     workspace_bytes_ += M * C * sizeof(__half);
     return Act{nullptr, C};
   }
-  const int NB = bnb_;
-  float* partial = bgn_partial_;
+  const int NB = NB_;
+  float* partial = gn_partial_;
   __half *normp = s_norm->p, *tok = s_tok->p, *qkv = s_qkv->p, *attn = s_attn->p, *qb = s_q->p, *ff = s_ff->p;
   // LayerNorm fold: the GEMMs that write the residual stream `tok` also emit per-row partial statistics, and the
   // GEMMs that read LN(tok) run on `tok` with gamma folded into the weight (no LayerNorm launches at all)
-  const bool fold = !lnfold_disabled();
-  float* stats[3] = {nullptr, nullptr, nullptr};
+  float* stats[3];
   int parts[3] = {0, 0, 0};
-  if (fold)
-    for (int i = 0; i < 3; ++i) stats[i] = reinterpret_cast<float*>(s_stats[i]->p);
+  for (int i = 0; i < 3; ++i) stats[i] = reinterpret_cast<float*>(s_stats[i]->p);
   // a producer's N blocks must tile C exactly so that every column contributes to the row statistics
   auto producer = [&](const std::function<GemmOp(int)>& make, int slot) {
     GemmOp op = make(0);
-    if (fold) {
-      if (C % op.bn != 0) {
-        for (int bn : {160, 128, 64})
-          if (C % bn == 0) {
-            op = make(bn);
-            break;
-          }
-      }
-      CFGPP_REQUIRE(C % op.bn == 0 && op.p.num_n_blocks <= 16, "LayerNorm fold: no tile width divides C");
-      // two partial sums per N block: the epilogue splits a tile's columns between two warps per row
-      op.p.stats_out = stats[slot];
-      parts[slot] = 2 * op.p.num_n_blocks;
+    if (C % op.bn != 0) {
+      for (int bn : {160, 128, 64})
+        if (C % bn == 0) {
+          op = make(bn);
+          break;
+        }
     }
+    CFGPP_REQUIRE(C % op.bn == 0 && op.p.num_n_blocks <= 16, "LayerNorm fold: no tile width divides C");
+    // two partial sums per N block: the epilogue splits a tile's columns between two warps per row
+    op.p.stats_out = stats[slot];
+    parts[slot] = 2 * op.p.num_n_blocks;
     return op;
   };
   auto consumer = [&](GemmOp op, const FoldedLN& f, int slot) {
@@ -485,27 +461,16 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
            }, 0));
   for (int k = 0; k < layers; ++k) {
     const std::string b = prefix + ".transformer_blocks." + std::to_string(k);
-    auto add_ln = [&](const std::string& n) {
-      const __half *g = plain(b + n + ".weight"), *be = plain(b + n + ".bias");
-      add_step(b + n, [=](cudaStream_t st) { run_layernorm(tok, Mi, C, g, be, 1e-5f, normp, st); });
-    };
     // --- self-attention ---
     __half* wqkv = packed_heads_rows({b + ".attn1.to_q.weight", b + ".attn1.to_k.weight", b + ".attn1.to_v.weight"},
                                      heads, hd, hdp);
-    if (fold) {
-      const FoldedLN f = folded_ln(b + ".attn1.qkv", wqkv, 3 * Cp, C, b + ".norm1", nullptr);
-      add_gemm(b + ".attn1.to_qkv(+norm1)",
-               consumer(make_linear_op(tok, C, nullptr, 0, 0, f.w, Mi, 3 * Cp, C, nullptr, nullptr, 0, 1, qkv, 3 * Cp, false),
-                        f, 0),
-               2.0 * Mi * 3.0 * C * C);
-    } else {
-      add_ln(".norm1");
-      add_gemm(b + ".attn1.to_qkv",
-               make_linear_op(normp, C, nullptr, 0, 0, wqkv, Mi, 3 * Cp, C, nullptr, nullptr, 0, 1, qkv, 3 * Cp, false),
-               2.0 * Mi * 3.0 * C * C);
-    }
+    const FoldedLN f1 = folded_ln(b + ".attn1.qkv", wqkv, 3 * Cp, C, b + ".norm1", nullptr);
+    add_gemm(b + ".attn1.to_qkv(+norm1)",
+             consumer(make_linear_op(tok, C, nullptr, 0, 0, f1.w, Mi, 3 * Cp, C, nullptr, nullptr, 0, 1, qkv, 3 * Cp, false),
+                      f1, 0),
+             2.0 * Mi * 3.0 * C * C);
     add_attn(b + ".attn1.sdpa",
-             make_attn_op(qkv, 3 * Cp, qkv + Cp, 3 * Cp, qkv + 2 * Cp, 3 * Cp, attn, Cp, bnb_, heads, HW, HW, hd));
+             make_attn_op(qkv, 3 * Cp, qkv + Cp, 3 * Cp, qkv + 2 * Cp, 3 * Cp, attn, Cp, NB_, heads, HW, HW, hd));
     add_gemm(b + ".attn1.to_out", producer([&](int bn) {
                return make_linear_op(attn, Cp, nullptr, 0, 0,
                                      packed_heads_cols(b + ".attn1.to_out.0.weight", heads, hd, hdp), Mi, C, Cp,
@@ -514,29 +479,21 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
              2.0 * Mi * static_cast<double>(C) * C);
     // --- cross-attention (K/V projected once per prompt by the prompt plan) ---
     __half* wq2 = packed_heads_rows({b + ".attn2.to_q.weight"}, heads, hd, hdp);
-    if (fold) {
-      const FoldedLN f = folded_ln(b + ".attn2.q", wq2, Cp, C, b + ".norm2", nullptr);
-      add_gemm(b + ".attn2.to_q(+norm2)",
-               consumer(make_linear_op(tok, C, nullptr, 0, 0, f.w, Mi, Cp, C, nullptr, nullptr, 0, 1, qb, Cp, false), f, 1),
-               2.0 * Mi * static_cast<double>(C) * C);
-    } else {
-      add_ln(".norm2");
-      add_gemm(b + ".attn2.to_q",
-               make_linear_op(normp, C, nullptr, 0, 0, wq2, Mi, Cp, C, nullptr, nullptr, 0, 1, qb, Cp, false),
-               2.0 * Mi * static_cast<double>(C) * C);
-    }
+    const FoldedLN f2 = folded_ln(b + ".attn2.q", wq2, Cp, C, b + ".norm2", nullptr);
+    add_gemm(b + ".attn2.to_q(+norm2)",
+             consumer(make_linear_op(tok, C, nullptr, 0, 0, f2.w, Mi, Cp, C, nullptr, nullptr, 0, 1, qb, Cp, false), f2, 1),
+             2.0 * Mi * static_cast<double>(C) * C);
     __half* kv = alloc_act(static_cast<size_t>(Mkv) * 2 * Cp);
     {
       __half* wkv = packed_heads_rows({b + ".attn2.to_k.weight", b + ".attn2.to_v.weight"}, heads, hd, hdp);
       std::vector<PlanStep>* save = cur_plan_;
       cur_plan_ = &prompt_plan_;
       add_gemm(b + ".attn2.to_kv",
-               make_linear_op(ctx_copy_ + static_cast<size_t>(brow0_) * n_ctx_ * D, D, nullptr, 0, 0, wkv, Mkv, 2 * Cp, D,
-                              nullptr, nullptr, 0, 1, kv, 2 * Cp, false),
+               make_linear_op(ctx_copy_, D, nullptr, 0, 0, wkv, Mkv, 2 * Cp, D, nullptr, nullptr, 0, 1, kv, 2 * Cp, false),
                2.0 * Mkv * 2.0 * C * D);
       cur_plan_ = save;
     }
-    add_attn(b + ".attn2.sdpa", make_attn_op(qb, Cp, kv, 2 * Cp, kv + Cp, 2 * Cp, attn, Cp, bnb_, heads, HW, n_ctx_, hd));
+    add_attn(b + ".attn2.sdpa", make_attn_op(qb, Cp, kv, 2 * Cp, kv + Cp, 2 * Cp, attn, Cp, NB_, heads, HW, n_ctx_, hd));
     add_gemm(b + ".attn2.to_out", producer([&](int bn) {
                return make_linear_op(attn, Cp, nullptr, 0, 0,
                                      packed_heads_cols(b + ".attn2.to_out.0.weight", heads, hd, hdp), Mi, C, Cp,
@@ -546,15 +503,9 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
     // --- GEGLU feed-forward ---
     __half* wg = packed_geglu(b + ".ff.net.0.proj.weight", false);
     __half* bg = packed_geglu(b + ".ff.net.0.proj.bias", true);
-    if (fold) {
-      const FoldedLN f = folded_ln(b + ".ff.geglu", wg, 8 * C, C, b + ".norm3", bg);
-      add_gemm(b + ".ff.geglu(+norm3)",
-               consumer(make_linear_op(tok, C, nullptr, 0, 0, f.w, Mi, 8 * C, C, nullptr, nullptr, 0, 1, ff, 4 * C, true), f, 2));
-    } else {
-      add_ln(".norm3");
-      add_gemm(b + ".ff.geglu",
-               make_linear_op(normp, C, nullptr, 0, 0, wg, Mi, 8 * C, C, bg, nullptr, 0, 1, ff, 4 * C, true));
-    }
+    const FoldedLN f3 = folded_ln(b + ".ff.geglu", wg, 8 * C, C, b + ".norm3", bg);
+    add_gemm(b + ".ff.geglu(+norm3)",
+             consumer(make_linear_op(tok, C, nullptr, 0, 0, f3.w, Mi, 8 * C, C, nullptr, nullptr, 0, 1, ff, 4 * C, true), f3, 2));
     add_gemm(b + ".ff.out", producer([&](int bn) {
                return make_linear_op(ff, 4 * C, nullptr, 0, 0, plain(b + ".ff.net.2.weight"), Mi, C, 4 * C,
                                      plain(b + ".ff.net.2.bias"), tok, C, 1, tok, C, false, bn);
@@ -568,49 +519,34 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
 Unet::Act Unet::build_downsample(const std::string& prefix, Act x, int H, int W) {
   const int C = x.C;
   const int Ho = H / 2, Wo = W / 2;
-  const size_t Mo = static_cast<size_t>(bnb_) * Ho * Wo;
-  static const bool use_im2col = [] {  // CFGPP_NO_S2TMA=1: the round-1 path (materialised stride-2 im2col + plain GEMM)
-    const char* e = getenv("CFGPP_NO_S2TMA");
-    return e != nullptr && e[0] == '1';
-  }();
-  Scratch* s_col = use_im2col ? scratch(btag_ + "im2col", Mo * 9 * C) : nullptr;
+  const size_t Mo = static_cast<size_t>(NB_) * Ho * Wo;
   __half* out = g_dry ? nullptr : alloc_act(Mo * C);
   if (g_dry) {
     raw(prefix + ".conv.weight"); raw(prefix + ".conv.bias");
     workspace_bytes_ += Mo * C * sizeof(__half);
     return Act{nullptr, C};
   }
-  if (!use_im2col) {
-    // stride-2 conv as an implicit GEMM: the A tile of every tap comes through a tensor map with element strides 2
-    add_gemm(prefix + ".conv", make_conv3x3_op(x.p, bnb_, H, W, C, packed_conv3x3(prefix + ".conv.weight"), C,
-                                               plain(prefix + ".conv.bias"), nullptr, 0, 1, out, 0, 2));
-    return Act{out, C};
-  }
-  const int NB = bnb_;
-  const __half* xp = x.p;
-  __half* col = s_col->p;
-  add_step(prefix + ".im2col", [=](cudaStream_t st) { run_im2col_s2(xp, col, NB, H, W, C, st); });
-  add_gemm(prefix + ".conv", make_linear_op(col, 9 * C, nullptr, 0, 0, packed_conv3x3(prefix + ".conv.weight"),
-                                            static_cast<int>(Mo), C, 9 * C, plain(prefix + ".conv.bias"), nullptr, 0, 1,
-                                            out, C, false));
+  // stride-2 conv as an implicit GEMM: the A tile of every tap comes through a tensor map with element strides 2
+  add_gemm(prefix + ".conv", make_conv3x3_op(x.p, NB_, H, W, C, packed_conv3x3(prefix + ".conv.weight"), C,
+                                             plain(prefix + ".conv.bias"), nullptr, 0, 1, out, 0, 2));
   return Act{out, C};
 }
 
 Unet::Act Unet::build_upsample(const std::string& prefix, Act x, int H, int W) {
   const int C = x.C;
-  const size_t Mo = static_cast<size_t>(bnb_) * 4 * H * W;
-  Scratch* s_up = scratch(btag_ + "upsampled", Mo * C);
+  const size_t Mo = static_cast<size_t>(NB_) * 4 * H * W;
+  Scratch* s_up = scratch("upsampled", Mo * C);
   __half* out = g_dry ? nullptr : alloc_act(Mo * C);
   if (g_dry) {
     raw(prefix + ".conv.weight"); raw(prefix + ".conv.bias");
     workspace_bytes_ += Mo * C * sizeof(__half);
     return Act{nullptr, C};
   }
-  const int NB = bnb_;
+  const int NB = NB_;
   const __half* xp = x.p;
   __half* up = s_up->p;
   add_step(prefix + ".nearest2x", [=](cudaStream_t st) { run_upsample2x(xp, up, NB, H, W, C, st); });
-  add_gemm(prefix + ".conv", make_conv3x3_op(up, bnb_, 2 * H, 2 * W, C, packed_conv3x3(prefix + ".conv.weight"), C,
+  add_gemm(prefix + ".conv", make_conv3x3_op(up, NB_, 2 * H, 2 * W, C, packed_conv3x3(prefix + ".conv.weight"), C,
                                              plain(prefix + ".conv.bias"), nullptr, 0, 1, out));
   return Act{out, C};
 }
@@ -639,8 +575,7 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
   act_allocs_.clear();
   scratch_.clear();
   prologue_plan_.clear();
-  branch_plan_[0].clear();
-  branch_plan_[1].clear();
+  body_plan_.clear();
   tail_plan_.clear();
   prompt_plan_.clear();
   workspace_bytes_ = 0;
@@ -772,83 +707,57 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
     }
 
     // ---- body (SURVEY A.2 steps 2-6) ----
-    // The unconditional and the conditional halves of the UNet batch never interact before the CFG++ mix, so the body
-    // can be built as two launch plans (rows [0,B) and [B,2B)) that run on forked streams inside the captured graph,
-    // one half's GEMM fill / drain, norms and attention overlapping the other half's tensor work (CFGPP_SPLIT=1). The
-    // single full-batch plan stays the default, although on an H100 80GB HBM3 at a 400 W power limit the split measured
-    // 0.452 vs 0.440 img/s (SDXL 1024^2 NFE=50 batch 2, two alternating pairs); the split also turns the stream-K
-    // remainder split of the GEMMs off (gemm.cu streamk_enabled), and a change of default is not validated here.
+    cur_plan_ = &body_plan_;
     const int HW0 = H_ * W_;
-    Act h0{g_dry ? nullptr : alloc_act(static_cast<size_t>(NB_) * HW0 * C0), C0};
-    if (g_dry) workspace_bytes_ += 2 * static_cast<size_t>(NB_) * HW0 * C0 * sizeof(__half);
-    __half* final_h = g_dry ? nullptr : alloc_act(static_cast<size_t>(NB_) * HW0 * C0);
-    n_branches_ = (NB_ >= 2 && !split_disabled()) ? 2 : 1;
-    for (int br = 0; br < n_branches_; ++br) {
-      bnb_ = NB_ / n_branches_;
-      brow0_ = br * bnb_;
-      btag_ = "b" + std::to_string(br) + ".";
-      bgn_partial_ = g_dry ? nullptr : gn_partial_ + static_cast<size_t>(br) * bnb_ * 128 * 64;
-      cur_plan_ = &branch_plan_[br];
-      int H = H_, W = W_;
-      Act h{g_dry ? nullptr : h0.p + static_cast<size_t>(brow0_) * HW0 * C0, C0};
-      std::vector<Act> skips{h};
-      for (int i = 0; i < L; ++i) {
-        const std::string blk = "down_blocks." + std::to_string(i);
-        const int Cout = d_.block_out_channels[i];
-        for (int j = 0; j < d_.layers_per_block; ++j) {
-          const std::string rp = blk + ".resnets." + std::to_string(j);
-          h = build_resnet(rp, h, nullptr, Cout, H, W, temb_off(rp));
-          if (d_.down_has_attn[i])
-            h = build_transformer(blk + ".attentions." + std::to_string(j), h, H, W, d_.transformer_layers[i],
-                                  d_.num_heads[i]);
-          skips.push_back(h);
-        }
-        if (i != L - 1) {
-          h = build_downsample(blk + ".downsamplers.0", h, H, W);
-          H /= 2; W /= 2;
-          skips.push_back(h);
-        }
+    const Act h0{g_dry ? nullptr : alloc_act(static_cast<size_t>(NB_) * HW0 * C0), C0};
+    if (g_dry) workspace_bytes_ += static_cast<size_t>(NB_) * HW0 * C0 * sizeof(__half);
+    Act h = h0;
+    int H = H_, W = W_;
+    std::vector<Act> skips{h};
+    for (int i = 0; i < L; ++i) {
+      const std::string blk = "down_blocks." + std::to_string(i);
+      const int Cout = d_.block_out_channels[i];
+      for (int j = 0; j < d_.layers_per_block; ++j) {
+        const std::string rp = blk + ".resnets." + std::to_string(j);
+        h = build_resnet(rp, h, nullptr, Cout, H, W, temb_off(rp));
+        if (d_.down_has_attn[i])
+          h = build_transformer(blk + ".attentions." + std::to_string(j), h, H, W, d_.transformer_layers[i],
+                                d_.num_heads[i]);
+        skips.push_back(h);
       }
-      {
-        const int Cm = d_.block_out_channels[L - 1];
-        h = build_resnet("mid_block.resnets.0", h, nullptr, Cm, H, W, temb_off("mid_block.resnets.0"));
-        h = build_transformer("mid_block.attentions.0", h, H, W, d_.transformer_layers[L - 1], d_.num_heads[L - 1]);
-        h = build_resnet("mid_block.resnets.1", h, nullptr, Cm, H, W, temb_off("mid_block.resnets.1"));
-      }
-      for (int i = 0; i < L; ++i) {
-        const std::string blk = "up_blocks." + std::to_string(i);
-        const int rev = L - 1 - i;
-        const int Cout = d_.block_out_channels[rev];
-        for (int j = 0; j < d_.layers_per_block + 1; ++j) {
-          Act skip = skips.back();
-          skips.pop_back();
-          const std::string rp = blk + ".resnets." + std::to_string(j);
-          const bool last = (i == L - 1) && (j == d_.layers_per_block) && !d_.up_has_attn[i];
-          if (last && !g_dry) out_override_ = final_h + static_cast<size_t>(brow0_) * HW0 * C0;
-          h = build_resnet(rp, h, &skip, Cout, H, W, temb_off(rp));
-          if (d_.up_has_attn[i])
-            h = build_transformer(blk + ".attentions." + std::to_string(j), h, H, W, d_.transformer_layers[rev],
-                                  d_.num_heads[rev]);
-        }
-        if (i != L - 1) {
-          h = build_upsample(blk + ".upsamplers.0", h, H, W);
-          H *= 2; W *= 2;
-        }
-      }
-      CFGPP_REQUIRE(skips.empty() && H == H_ && W == W_, "internal: skip stack mismatch");
-      if (!g_dry && h.p != final_h + static_cast<size_t>(brow0_) * HW0 * C0) {
-        // the last block ended with a transformer: gather its output into the shared tail input
-        const __half* src = h.p;
-        __half* dst = final_h + static_cast<size_t>(brow0_) * HW0 * C0;
-        const size_t bytes = static_cast<size_t>(bnb_) * HW0 * C0 * sizeof(__half);
-        add_step(btag_ + "gather_tail", [=](cudaStream_t st) {
-          CFGPP_CHECK_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st));
-        });
+      if (i != L - 1) {
+        h = build_downsample(blk + ".downsamplers.0", h, H, W);
+        H /= 2; W /= 2;
+        skips.push_back(h);
       }
     }
-    // ---- tail: conv_norm_out + SiLU over the whole batch feeds the fused conv_out / CFG++ step kernel ----
+    {
+      const int Cm = d_.block_out_channels[L - 1];
+      h = build_resnet("mid_block.resnets.0", h, nullptr, Cm, H, W, temb_off("mid_block.resnets.0"));
+      h = build_transformer("mid_block.attentions.0", h, H, W, d_.transformer_layers[L - 1], d_.num_heads[L - 1]);
+      h = build_resnet("mid_block.resnets.1", h, nullptr, Cm, H, W, temb_off("mid_block.resnets.1"));
+    }
+    for (int i = 0; i < L; ++i) {
+      const std::string blk = "up_blocks." + std::to_string(i);
+      const int rev = L - 1 - i;
+      const int Cout = d_.block_out_channels[rev];
+      for (int j = 0; j < d_.layers_per_block + 1; ++j) {
+        Act skip = skips.back();
+        skips.pop_back();
+        const std::string rp = blk + ".resnets." + std::to_string(j);
+        h = build_resnet(rp, h, &skip, Cout, H, W, temb_off(rp));
+        if (d_.up_has_attn[i])
+          h = build_transformer(blk + ".attentions." + std::to_string(j), h, H, W, d_.transformer_layers[rev],
+                                d_.num_heads[rev]);
+      }
+      if (i != L - 1) {
+        h = build_upsample(blk + ".upsamplers.0", h, H, W);
+        H *= 2; W *= 2;
+      }
+    }
+    CFGPP_REQUIRE(skips.empty() && H == H_ && W == W_, "internal: skip stack mismatch");
+    // ---- tail: conv_norm_out + SiLU on the last up block's output feeds the fused conv_out / CFG++ step kernel ----
     cur_plan_ = &tail_plan_;
-    bnb_ = NB_; brow0_ = 0; btag_ = "tail."; bgn_partial_ = gn_partial_;
     Scratch* s_norm = scratch("tail.norm", static_cast<size_t>(NB_) * HW0 * C0);
     if (!g_dry) {
       const __half *g = plain("conv_norm_out.weight"), *b = plain("conv_norm_out.bias");
@@ -856,7 +765,7 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
       const float eps = d_.norm_eps;
       float* partial = gn_partial_;
       __half* normp = s_norm->p;
-      const __half* hp = final_h;
+      const __half* hp = h.p;
       add_step("conv_norm_out+silu", [=](cudaStream_t st) {
         run_groupnorm(hp, C0, nullptr, 0, NB, HW, g, b, eps, true, partial, normp, st);
       }, 2);
@@ -865,7 +774,7 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
     }
     if (g_dry) {
       // discard everything the sizing pass pushed (it pushes nothing) and keep the scratch sizes
-      prologue_plan_.clear(); branch_plan_[0].clear(); branch_plan_[1].clear(); tail_plan_.clear();
+      prologue_plan_.clear(); body_plan_.clear(); tail_plan_.clear();
       prompt_plan_.clear();
     }
   }
@@ -874,7 +783,7 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
   // FLOP / launch accounting (the reference executes the K/V projections every step: count them per forward)
   forward_flops_ = 0.0;
   launches_per_step_ = 3;  // select_step + conv_in + conv_out_step
-  for (auto* pl : {&branch_plan_[0], &branch_plan_[1], &tail_plan_})
+  for (auto* pl : {&body_plan_, &tail_plan_})
     for (auto& s : *pl) { forward_flops_ += s.flops; launches_per_step_ += s.launches; }
   for (auto& s : prologue_plan_) launches_per_step_ += s.launches;
   prompt_flops_ = 0.0;
@@ -899,29 +808,10 @@ void Unet::run_plan(const std::vector<PlanStep>& plan, cudaStream_t stream) {
   for (const auto& s : plan) s.fn(stream);
 }
 
-// Body of the forward. `concurrent`: fork the two CFG halves onto a second stream (used under graph capture, where
-// the fork / join become graph edges); otherwise the halves run back to back on the caller's stream.
-void Unet::run_body(cudaStream_t stream, bool concurrent) {
-  if (n_branches_ == 2 && concurrent) {
-    CFGPP_CHECK_CUDA(cudaEventRecord(fork_ev_, stream));
-    CFGPP_CHECK_CUDA(cudaStreamWaitEvent(capture_stream2_, fork_ev_, 0));
-    run_plan(branch_plan_[0], stream);
-    run_plan(branch_plan_[1], capture_stream2_);
-    CFGPP_CHECK_CUDA(cudaEventRecord(join_ev_, capture_stream2_));
-    CFGPP_CHECK_CUDA(cudaStreamWaitEvent(stream, join_ev_, 0));
-  } else {
-    for (int br = 0; br < n_branches_; ++br) run_plan(branch_plan_[br], stream);
-  }
+// Body of the forward: conv_in output .. conv_norm_out, on the caller's stream.
+void Unet::run_body(cudaStream_t stream) {
+  run_plan(body_plan_, stream);
   run_plan(tail_plan_, stream);
-}
-
-bool Unet::split_disabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("CFGPP_SPLIT");
-    v = (e && e[0] == '1') ? 0 : 1;
-  }
-  return v == 1;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -963,7 +853,7 @@ void Unet::unet_forward(const void* z, int z_dtype, float t, float in_scale, __h
   run_plan(prologue_plan_, stream);
   run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, &cur_state_->in_scale, conv_in_w_, conv_in_b_, conv_in_out_, B_, H_, W_,
               d_.block_out_channels[0], 2, stream);
-  run_body(stream, true);  // the two CFG halves fork onto a side stream and join before the tail
+  run_body(stream);
   run_conv_out_step(final_norm_.p, conv_out_w_, conv_out_b_, B_, H_, W_, final_norm_.C, STEP_NONE, nullptr, nullptr,
                     nullptr, nullptr, eps_uc, eps_c, stream);
 }
@@ -993,7 +883,7 @@ std::vector<Unet::ProfEntry> Unet::profile_forward(const void* z, int z_dtype, f
               d_.block_out_channels[0], 2, stream);
   mark();
   out.push_back({"conv_in", 3, 2.0 * NB_ * H_ * W_ * 36.0 * d_.block_out_channels[0], 0.f});
-  for (auto* pl : {&branch_plan_[0], &branch_plan_[1], &tail_plan_})
+  for (auto* pl : {&body_plan_, &tail_plan_})
     for (const auto& st : *pl) {
       st.fn(stream);
       mark();
@@ -1075,7 +965,7 @@ void Unet::ensure_graph(cudaStream_t stream) {
     run_plan(prologue_plan_, capture_stream_);
     run_conv_in(z_state_, state_dtype_ == CFGPP_F16 ? 1 : 0, &cur_state_->in_scale, conv_in_w_, conv_in_b_,
                 conv_in_out_, B_, H_, W_, d_.block_out_channels[0], 2, capture_stream_);
-    run_body(capture_stream_, true);
+    run_body(capture_stream_);
     run_conv_out_step(final_norm_.p, conv_out_w_, conv_out_b_, B_, H_, W_, final_norm_.C, mode, &cur_state_->coef,
                       z_state_, aux_state_, z0t_state_, nullptr, nullptr, capture_stream_, noise_slot_, lambda_slot_);
   } catch (...) {

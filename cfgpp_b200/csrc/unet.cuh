@@ -86,7 +86,6 @@ class Unet {
   FoldedLN folded_ln(const std::string& cache_key, const __half* w_packed, int N, int K, const std::string& norm_prefix,
                      const __half* bias_packed);
   std::map<std::string, FoldedLN> fold_cache_;
-  static bool lnfold_disabled();
   __half* plain(const std::string& key);
 
   // ---- workspace ----
@@ -109,9 +108,7 @@ class Unet {
   void add_attn(const std::string& name, const AttnOp& op);
   void add_step(const std::string& name, std::function<void(cudaStream_t)> fn, int launches = 1);
   void run_plan(const std::vector<PlanStep>& plan, cudaStream_t stream);
-  void run_body(cudaStream_t stream, bool concurrent);
-  static bool split_disabled();
-  void build_final(int mode_with_dtype, bool expose_eps);
+  void run_body(cudaStream_t stream);
   void ensure_graph(cudaStream_t stream);
 
   cfgpp_model_desc d_;
@@ -120,7 +117,7 @@ class Unet {
   std::map<std::string, DevTensor> raw_;
   std::vector<void*> weight_allocs_;
   std::vector<void*> act_allocs_;
-  size_t workspace_bytes_ = 0, weight_bytes_ = 0;
+  size_t workspace_bytes_ = 0;
 
   // packed weights: resolved lazily during plan building (finalize just validates + packs what is shape-independent)
   std::map<std::string, __half*> packed_cache_;
@@ -134,14 +131,8 @@ class Unet {
   int B_ = 0, NB_ = 0, H_ = 0, W_ = 0;
   std::vector<PlanStep>* cur_plan_ = nullptr;
   std::vector<PlanStep> prologue_plan_;  // timestep embedding -> temb for all resnets
-  std::vector<PlanStep> branch_plan_[2];  // conv_in output .. last up block, one plan per CFG half (uncond / cond)
-  std::vector<PlanStep> tail_plan_;       // conv_norm_out + SiLU over the whole batch
-  int n_branches_ = 1;
-  // branch currently being built (rows [brow0_, brow0_ + bnb_) of the UNet batch)
-  int bnb_ = 0, brow0_ = 0;
-  std::string btag_;
-  float* bgn_partial_ = nullptr;
-  __half* out_override_ = nullptr;
+  std::vector<PlanStep> body_plan_;      // conv_in output .. last up block
+  std::vector<PlanStep> tail_plan_;      // conv_norm_out + SiLU
   std::vector<PlanStep> prompt_plan_;    // cross-attention K/V projections + add-embedding
   double forward_flops_ = 0.0, prompt_flops_ = 0.0;
   int launches_per_step_ = 0, prompt_launches_ = 0;
@@ -151,7 +142,6 @@ class Unet {
   Scratch* scratch(const std::string& name, size_t numel_half);
 
   // conditioning / per-step device state
-  const __half* ctx_ = nullptr;  // caller-owned, valid while the prompt is set
   __half* ctx_copy_ = nullptr;
   int n_ctx_ = 77;
   __half* add_in_ = nullptr;    // [NB][proj_in_dim]
@@ -159,7 +149,6 @@ class Unet {
   __half* aug_emb_ = nullptr;   // [NB][time_embed_dim]
   __half* pooled_copy_ = nullptr;
   float* time_ids_copy_ = nullptr;
-  int add_rows_ = 0;
   bool has_aug_ = false;
   __half *t_sin_ = nullptr, *t_h1_ = nullptr, *emb_ = nullptr, *semb_ = nullptr, *temb_all_ = nullptr;
   float* gn_partial_ = nullptr;
@@ -176,8 +165,6 @@ class Unet {
   size_t noise_cap_ = 0;                 // elements
   const float** lambda_slot_ = nullptr;  // device word holding lambda_buf_ or null (read by the step kernel)
   float* lambda_buf_ = nullptr;          // [B] per-image guidance, workspace of the prepared plan
-  const void* fwd_z_ = nullptr;  // input of the un-fused forward
-  int fwd_z_dtype_ = CFGPP_F32;
   __half *fwd_eps_uc_ = nullptr, *fwd_eps_c_ = nullptr;
   Act final_norm_{nullptr, 0};
   __half* conv_in_out_ = nullptr;
@@ -189,8 +176,6 @@ class Unet {
   cudaGraphExec_t graph_exec_ = nullptr;
   bool graph_valid_ = false;
   cudaStream_t capture_stream_ = nullptr;
-  cudaStream_t capture_stream2_ = nullptr;
-  cudaEvent_t fork_ev_ = nullptr, join_ev_ = nullptr;
 };
 
 }  // namespace cfgpp

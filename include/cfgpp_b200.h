@@ -218,9 +218,11 @@ int cfgpp_clip_encode(cfgpp_clip_handle* h, const int32_t* input_ids_dev, const 
 int cfgpp_clip_stats(cfgpp_clip_handle* h, double* flops, size_t* workspace_bytes);
 
 /* ---- operator-level entry points (one kernel each; used by the kernel parity tests and micro-benchmarks) ----- */
+/* force_streamk (also in cfgpp_op_linear_lnfold): take the stream-K remainder split whenever its pieces are at least 2
+ * k-blocks deep. The linear layers never take it otherwise; this lets tests reach the split's fix-up path. */
 int cfgpp_op_linear(const void* a, int lda, const void* a2, int lda2, int k_split, const void* w, int M, int N, int K,
                     const void* bias, const void* addend, int ld_add, int add_rows_per_group, void* out, int ldc,
-                    int geglu, int force_bn, void* stream);
+                    int geglu, int force_bn, int force_streamk, void* stream);
 /* The LayerNorm-fold variants of cfgpp_op_linear (a [M,K], single source), exactly one of:
  *  stats_out (producer): besides out, writes per-row partial (sum, sum of squares) of the fp16 output as
  *    [2 * ceil(N / force_bn)][M] float2 — part 2 j + h covers columns [j BN + h BN / 2, j BN + (h + 1) BN / 2) of N
@@ -230,8 +232,8 @@ int cfgpp_op_linear(const void* a, int lda, const void* a2, int lda2, int k_spli
  *    stats_in ([ln_parts][M] float2); bias and addend must be null (the bias is inside ln_t). */
 int cfgpp_op_linear_lnfold(const void* a, const void* w, int M, int N, int K, const void* bias, const void* addend,
                            int ld_add, int add_rows_per_group, void* out, int ldc, int geglu, int force_bn,
-                           float* stats_out, const float* stats_in, int ln_parts, float ln_eps, const float* ln_s,
-                           const float* ln_t, void* stream);
+                           int force_streamk, float* stats_out, const float* stats_in, int ln_parts, float ln_eps,
+                           const float* ln_s, const float* ln_t, void* stream);
 /* LayerNorm fold of w [N,K] fp16 with LayerNorm(K) gamma / beta (fp16) and an optional bias [N]: wf = fp16(w * gamma)
  * [N,K] fp16, s[n] = sum_k wf[n,k], t[n] = sum_k beta[k] w[n,k] + bias[n] (fp32). */
 int cfgpp_op_fold_ln(const void* w, const void* gamma, const void* beta, const void* bias, void* wf, float* s, float* t,
@@ -285,8 +287,6 @@ int cfgpp_op_conv_out_step(const void* x, const void* w, const void* bias, int B
                            void* eps_uc, void* eps_c, const void* noise_dev, const float* lambda_dev, void* stream);
 /* nearest 2x upsample: x [B,H,W,C] NHWC fp16 (C % 8 == 0) -> out [B,2H,2W,C]. */
 int cfgpp_op_upsample2x(const void* x, void* out, int B, int H, int W, int C, void* stream);
-/* stride-2 pad-1 3x3 im2col: x [B,H,W,C] (even H, W; C % 8 == 0) -> out [B * H/2 * W/2, 9 * C], tap-major. */
-int cfgpp_op_im2col_s2(const void* x, void* out, int B, int H, int W, int C, void* stream);
 /* AutoencoderKL decoder front: z [B,4,HW] of z_dtype -> fp16(w . fp16(z / scaling) + bias), w [4][4], out [B,4,HW]. */
 int cfgpp_op_vae_latent_prep(const void* z, int z_dtype, float scaling, const void* w, const void* bias, void* out,
                              int B, int HW, void* stream);

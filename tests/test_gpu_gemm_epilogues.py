@@ -97,12 +97,13 @@ def torch_stats(h, parts):
     return torch.stack([x.sum(2), (x * x).sum(2)], 2).permute(1, 0, 2).float().contiguous()
 
 
-def fold_vs_unfused(nv, h, stats, gamma, beta, w, b, geglu, what, ratio, force_bn=0):
+def fold_vs_unfused(nv, h, stats, gamma, beta, w, b, geglu, what, ratio, force_bn=0, force_streamk=False):
     """Runs the fused consumer and the unfused op_layernorm → op_linear path on h; returns (fused out, fused error,
-    unfused error) vs the exact reference, and gates fused ≤ 1.5x unfused + floor (ratio ≤ 30) or the envelope."""
+    unfused error) vs the exact reference, and gates fused ≤ 1.5x unfused + floor (ratio ≤ 30) or the envelope.
+    `force_streamk` applies to the fused consumer only: the unfused path stays the plain tile walk it is judged by."""
     wk, bk = pack_geglu(w, b) if geglu else (w, b)
     wf, s, t = nv.op_fold_ln(wk, gamma, beta, bk)
-    fused = nv.op_linear_lnfold(h, wf, s, t, stats, geglu=geglu, force_bn=force_bn)
+    fused = nv.op_linear_lnfold(h, wf, s, t, stats, geglu=geglu, force_bn=force_bn, force_streamk=force_streamk)
     unfused = nv.op_linear(nv.op_layernorm(h, gamma, beta), wk, bk, geglu=geglu)
     ref = lnlinear_exact(h, gamma, beta, w, b, geglu)
     ef, eu = rel_l2_64(fused, ref), rel_l2_64(unfused, ref)
@@ -225,7 +226,7 @@ def test_lnfold_consumer_rejects_bias():
     out = torch.empty(128, 64, dtype=torch.float16, device=dev)
     lib = nv.load()
     st = lib.cfgpp_op_linear_lnfold(nv.ptr(h), nv.ptr(wf), 128, 64, 64, nv.ptr(bias), None, 0, 1, nv.ptr(out), 64, 0, 0,
-                                    None, nv.ptr(stats), 2, ctypes.c_float(1e-5), nv.ptr(s), nv.ptr(t), nv.stream_ptr())
+                                    0, None, nv.ptr(stats), 2, ctypes.c_float(1e-5), nv.ptr(s), nv.ptr(t), nv.stream_ptr())
     assert st != 0 and b"bias" in lib.cfgpp_last_error()
 
 
@@ -315,18 +316,19 @@ def test_geglu_shapes(C, M, hb):
     gate(f"geglu {M}x{inner}x{C}{' +bias' if hb else ''}", out, ref, TOL_GEMM)
 
 
-# ---- stream-K (test_gpu_kernels.test_linear_streamk_forced_in_subprocess re-runs these with the split forced on) ----
+# ---- stream-K -----------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("force_streamk", [False, True])
 @pytest.mark.parametrize("kind", ["rowstats", "lnfold", "geglu", "lnfold_geglu"])
-def test_epilogue_streamk_repeatable(kind):
+def test_epilogue_streamk_repeatable(kind, force_streamk):
     """Shapes with a remainder of tiles over the 132 SMs (rowstats 32x10 tiles, lnfold 32x15, GEGLU 32x20), so with the
-    stream-K split on the fix-up path feeds each epilogue: result gated, 12 launches bit-identical."""
+    stream-K split forced on the fix-up path feeds each epilogue: result gated, 12 launches bit-identical."""
     from cfgpp_b200 import _native as nv
     g = torch.Generator().manual_seed(len(kind))
     M = 4096
     if kind == "rowstats":
         N, K, bn = 1280, 1280, 128
         a, w, bias, res = rnd(g, M, K), rnd(g, N, K, scale=K ** -0.5), rnd(g, N), rnd(g, M, N)
-        run = lambda: nv.op_linear_stats(a, w, bn, bias, res)
+        run = lambda: nv.op_linear_stats(a, w, bn, bias, res, force_streamk=force_streamk)
         first = run()
         gate(f"rowstats(stream-K) {M}x{N}x{K}", first[0], ref_linear(a, w, bias, res, 1), TOL_GEMM)
         check_stats(first[0], first[1], bn, f"rowstats(stream-K) {M}x{N}x{K}")
@@ -334,7 +336,7 @@ def test_epilogue_streamk_repeatable(kind):
         C = 640
         a, w, b = rnd(g, M, C), rnd(g, 8 * C, C, scale=C ** -0.5), rnd(g, 8 * C)
         wp, bp = pack_geglu(w, b)
-        run = lambda: (nv.op_linear(a, wp, bp, geglu=True),)
+        run = lambda: (nv.op_linear(a, wp, bp, geglu=True, force_streamk=force_streamk),)
         first = run()
         h = ref_linear(a, w, b, None, 1)
         ref = (h[:, :4 * C].float() * torch.nn.functional.gelu(h[:, 4 * C:].float()).half().float()).half()
@@ -347,10 +349,11 @@ def test_epilogue_streamk_repeatable(kind):
         gamma, beta = rnd(g, C, scale=0.2, shift=1.0), rnd(g, C, scale=0.2)
         w, b = rnd(g, N, C, scale=C ** -0.5), rnd(g, N)
         stats = torch_stats(h, C // 32)
-        fused, _, _ = fold_vs_unfused(nv, h, stats, gamma, beta, w, b, geglu, f"lnfold(stream-K) {M}x{N}x{C}", 1)
+        fused, _, _ = fold_vs_unfused(nv, h, stats, gamma, beta, w, b, geglu, f"lnfold(stream-K) {M}x{N}x{C}", 1,
+                                      force_streamk=force_streamk)
         wk, bk = pack_geglu(w, b) if geglu else (w, b)
         wf, s, t = nv.op_fold_ln(wk, gamma, beta, bk)
-        run = lambda: (nv.op_linear_lnfold(h, wf, s, t, stats, geglu=geglu),)
+        run = lambda: (nv.op_linear_lnfold(h, wf, s, t, stats, geglu=geglu, force_streamk=force_streamk),)
         first = run()
         assert torch.equal(first[0], fused)
     for _ in range(12):

@@ -58,41 +58,23 @@ def test_linear(M, N, K, hb, ha, bn):
     gate(f'linear {M}x{N}x{K}', out, ref_linear(a, w, bias, addend, ha), TOL_GEMM)
 
 
+@pytest.mark.parametrize("force_streamk", [False, True])
 @pytest.mark.parametrize("M,N,K,geglu_like", [(4096, 1280, 1280, False), (4096, 1280, 5120, False),
                                               (4096, 3840, 1280, False), (2048, 640, 2560, False),
                                               (8192, 1280, 1280, False), (5000, 1280, 640, False)])
-def test_linear_streamk_shapes_and_repeatability(M, N, K, geglu_like):
+def test_linear_streamk_shapes_and_repeatability(M, N, K, geglu_like, force_streamk):
     """Shapes whose tile count is not a multiple of the CTA count CAN take the stream-K remainder path (partials
-    parked in the workspace by other CTAs, self-resetting flags; on by default for the convolutions, for linear layers
-    with CFGPP_STREAMK_LINEAR=1 CFGPP_STREAMK_MIN=0 CFGPP_STREAMK_PIECE=0, which
-    test_linear_streamk_forced_in_subprocess sets): result vs the fp32 reference, and 12 back-to-back launches must be
-    bit-identical (fixed summation order; flags re-armed by the kernel itself)."""
+    parked in the workspace by other CTAs, self-resetting flags; on by default for the convolutions, off for linear
+    layers unless `force_streamk` is set, so the forced cases cover the split's partial / fix-up path): result vs the
+    fp32 reference, and 12 back-to-back launches must be bit-identical (fixed summation order; flags re-armed by the
+    kernel itself)."""
     from cfgpp_b200 import _native as nv
     g = torch.Generator().manual_seed(M + N + K)
     a, w, bias, res = rnd(g, M, K), rnd(g, N, K, scale=K ** -0.5), rnd(g, N), rnd(g, M, N)
-    first = nv.op_linear(a, w, bias, res, 1)
-    gate(f'linear(stream-K) {M}x{N}x{K}', first, ref_linear(a, w, bias, res, 1), TOL_GEMM)
+    first = nv.op_linear(a, w, bias, res, 1, force_streamk=force_streamk)
+    gate(f'linear(force_streamk={force_streamk}) {M}x{N}x{K}', first, ref_linear(a, w, bias, res, 1), TOL_GEMM)
     for _ in range(12):
-        assert torch.equal(nv.op_linear(a, w, bias, res, 1), first)
-
-
-def test_linear_streamk_forced_in_subprocess():
-    """The stream-K split is off for linear layers by default; re-run the shapes above and the epilogue shapes of
-    test_gpu_gemm_epilogues.py (row statistics, LayerNorm fold, GEGLU) in a child process with it forced on (the
-    dispatch reads the switches once per process), so the split's partial / fix-up path is covered."""
-    import os
-    import subprocess
-    import sys
-    from pathlib import Path
-    if os.environ.get("CFGPP_STREAMK_LINEAR") == "1":
-        pytest.skip("already inside the child")
-    env = dict(os.environ, CFGPP_STREAMK_LINEAR="1", CFGPP_STREAMK_MIN="0", CFGPP_STREAMK_PIECE="0")
-    files = [__file__, str(Path(__file__).with_name("test_gpu_gemm_epilogues.py"))]
-    r = subprocess.run([sys.executable, "-m", "pytest", *files, "-q", "-m", "gpu", "-p", "no:cacheprovider", "-k",
-                        "test_linear_streamk_shapes_and_repeatability or test_epilogue_streamk_repeatable", "-x"],
-                       env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    assert "10 passed" in r.stdout, r.stdout[-2000:]
+        assert torch.equal(nv.op_linear(a, w, bias, res, 1, force_streamk=force_streamk), first)
 
 
 def test_linear_dual_source_and_geglu():

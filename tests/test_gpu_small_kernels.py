@@ -1,6 +1,6 @@
 """Kernel-level tests of the small hand-written kernels every image passes through, through their C-ABI entry points:
-the UNet's timestep embedding, tiny-M linear, row copy, conv_in, conv_out fused with the CFG++ step, nearest-2x upsample
-and stride-2 im2col (`elementwise.cu`); the AutoencoderKL's latent preparation, row softmax, RGB conv_out, image pad and
+the UNet's timestep embedding, tiny-M linear, row copy, conv_in, conv_out fused with the CFG++ step and nearest-2x
+upsample (`elementwise.cu`); the AutoencoderKL's latent preparation, row softmax, RGB conv_out, image pad and
 encoder moments / sample (`vae_kernels.cu`); the CLIP towers' embedding, causal attention, MLP activation and pooled-row
 gather (`text_kernels.cu`).
 
@@ -262,7 +262,7 @@ def test_conv_out_step(B, H, W):
           f"standalone step")
 
 
-# ---- upsample2x, im2col_s2 --------------------------------------------------------------------------------------
+# ---- upsample2x -------------------------------------------------------------------------------------------------
 
 @pytest.mark.parametrize("B,H,W,C", [(2, 5, 7, 8), (1, 9, 13, 320), (3, 16, 24, 320), (2, 8, 3, 1280)])
 def test_upsample2x(B, H, W, C):
@@ -270,17 +270,6 @@ def test_upsample2x(B, H, W, C):
     x = rnd(torch.Generator().manual_seed(B + H + W + C), B, H, W, C)
     ref = x.repeat_interleave(2, 1).repeat_interleave(2, 2)
     assert torch.equal(bits(nv.op_upsample2x(x)), bits(ref))
-
-
-@pytest.mark.parametrize("B,H,W,C", [(2, 6, 10, 8), (1, 16, 12, 320), (3, 14, 22, 320), (1, 8, 8, 1280)])
-def test_im2col_s2(B, H, W, C):
-    from cfgpp_b200 import _native as nv
-    x = rnd(torch.Generator().manual_seed(B + H + W + C), B, H, W, C)
-    Ho, Wo = H // 2, W // 2
-    xp = F.pad(x, (0, 0, 1, 1, 1, 1))
-    taps = [xp[:, kh:kh + 2 * Ho:2, kw:kw + 2 * Wo:2, :] for kh in range(3) for kw in range(3)]
-    ref = torch.stack(taps, 3).reshape(B * Ho * Wo, 9 * C)
-    assert torch.equal(bits(nv.op_im2col_s2(x)), bits(ref))
 
 
 # ---- AutoencoderKL helpers --------------------------------------------------------------------------------------
