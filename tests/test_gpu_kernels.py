@@ -2,7 +2,7 @@
 rounding points (fp16(acc+bias) then fp16 add of the residual / time embedding, fp32 norms rounded once).
 Gates are ~5x the error observed on the GPU (printed by every test; `pytest -s` shows them): GEMM / conv observe ~3e-5
 (both sides round the same fp32 sum to fp16, so only accumulation-order flips of the last bit remain) -> 2e-4;
-attention observes 2.5-2.9e-4 (P is rounded to fp16 before PV) -> 1.5e-3; norms observe 5-8e-6 -> 5e-5."""
+norms observe 5-8e-6 -> 5e-5. Attention is pinned element by element against fp64 in `test_gpu_attention.py`."""
 import pytest
 import torch
 
@@ -18,7 +18,7 @@ def _fp32_refs():
     torch.backends.cuda.matmul.allow_tf32 = False
 
 
-TOL_GEMM, TOL_ATTN, TOL_NORM = 2e-4, 1.5e-3, 5e-5
+TOL_GEMM, TOL_NORM = 2e-4, 5e-5
 
 
 def gate(what, got, ref, tol):
@@ -167,51 +167,6 @@ def test_conv3x3(B, H, W, Cin, Cout, ht, hr):
     edge = torch.zeros(B, H, W, dtype=torch.bool, device=dev)
     edge[:, 0], edge[:, -1], edge[:, :, 0], edge[:, :, -1] = True, True, True, True
     gate('conv3x3 edge pixels', out[edge.reshape(-1)], ref[edge.reshape(-1)], TOL_GEMM)
-
-
-@pytest.mark.parametrize("B,H,Nq,Nkv", [(1, 1, 128, 128), (1, 4, 64, 64), (2, 5, 1024, 1024), (1, 10, 4096, 4096),
-                                        (4, 20, 1024, 77), (1, 2, 200, 333), (1, 1, 1, 1),
-                                        # one KV tile (cross-attention): partial KV tiles, a partial last query tile
-                                        (4, 10, 4096, 77), (1, 5, 1024, 128), (2, 3, 520, 100), (1, 2, 256, 5),
-                                        # the bench shape, ragged Nq / Nkv, many heads
-                                        (4, 20, 1024, 1024), (3, 13, 1100, 1000), (1, 37, 1024, 640), (2, 31, 700, 333)])
-def test_attention(B, H, Nq, Nkv):
-    from cfgpp_b200 import _native as nv
-    g = torch.Generator().manual_seed(Nq + Nkv)
-    Cc = H * 64
-    if Nq == Nkv:
-        qkv = rnd(g, B, Nq, 3 * Cc, scale=1.2)
-        q, k, v = qkv[:, :, :Cc], qkv[:, :, Cc:2 * Cc], qkv[:, :, 2 * Cc:]
-    else:
-        q, kv = rnd(g, B, Nq, Cc, scale=1.2), rnd(g, B, Nkv, 2 * Cc, scale=1.2)
-        k, v = kv[:, :, :Cc], kv[:, :, Cc:]
-    out = nv.op_attention(q, k, v, H)
-    qf, kf, vf = (t.float().reshape(B, -1, H, 64).transpose(1, 2) for t in (q, k, v))
-    ref = torch.nn.functional.scaled_dot_product_attention(qf, kf, vf).transpose(1, 2).reshape(B, Nq, Cc)
-    gate(f'attention B{B} H{H} {Nq}x{Nkv}', out, ref, TOL_ATTN)
-
-
-@pytest.mark.parametrize("B,H,Nq,Nkv,hd", [(2, 8, 1024, 1024, 80), (1, 8, 4096, 4096, 40), (2, 8, 256, 256, 160),
-                                           (2, 8, 64, 77, 160), (1, 3, 300, 77, 40), (2, 8, 1024, 77, 80),
-                                           (2, 8, 256, 77, 160), (1, 4, 4096, 77, 40), (1, 2, 640, 120, 160),
-                                           (2, 8, 4096, 4096, 40)])
-def test_attention_padded_heads(B, H, Nq, Nkv, hd):
-    """SD v1.5 head dims (40 / 80 / 160): heads are zero-padded to a multiple of 64 columns in q / k / v."""
-    from cfgpp_b200 import _native as nv
-    g = torch.Generator().manual_seed(hd + Nq)
-    P = (hd + 63) // 64 * 64
-
-    def padded(n):
-        t = torch.zeros(B, n, H, P)
-        t[..., :hd] = torch.randn(B, n, H, hd, generator=g) * 1.1
-        return t.reshape(B, n, H * P).half().to(dev)
-
-    q, k, v = padded(Nq), padded(Nkv), padded(Nkv)
-    out = nv.op_attention(q, k, v, H, head_dim=hd).reshape(B, Nq, H, P)
-    qf, kf, vf = (t.float().reshape(B, -1, H, P)[..., :hd].transpose(1, 2) for t in (q, k, v))
-    ref = torch.nn.functional.scaled_dot_product_attention(qf, kf, vf).transpose(1, 2)
-    gate(f'attention hd{hd} {Nq}x{Nkv}', out[..., :hd], ref, TOL_ATTN)
-    assert out[..., hd:].abs().max() == 0
 
 
 VAE_HW = 1024 * 1024  # the AutoencoderKL decoder's top level at 1024² (up to 4 M elements per group)
