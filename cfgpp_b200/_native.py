@@ -164,6 +164,24 @@ def op_conv3x3_s2(x_nhwc: torch.Tensor, w_packed: torch.Tensor, bias=None, pad: 
     return out
 
 
+def op_conv3x3_ex(x_nhwc: torch.Tensor, w_packed: torch.Tensor, bias=None, addend=None, add_rows_per_group: int = 1,
+                  stride: int = 1, pad: int = 1, force_im2col: bool = False, force_bn: int = 0) -> torch.Tensor:
+    """The 3x3 convolution in every mode: x [B,H,W,Cin] fp16 NHWC, w_packed [Cout, 9*Cin] (tap-major) ->
+    [B,H/stride,W/stride,Cout]; stride 1 / pad 1, stride 2 / pad 1 (Downsample2D) or stride 2 / pad 0 (one zero row /
+    column after the image). Any H, W: the A tile comes through the im2col tensor map where the tiled box cannot hold
+    128 consecutive output pixels; `force_im2col` takes the im2col map everywhere (mode comparisons)."""
+    lib = load()
+    B, H, W, Cin = x_nhwc.shape
+    Cout = w_packed.shape[0]
+    assert w_packed.shape[1] == 9 * Cin
+    out = torch.empty((B, H // stride, W // stride, Cout), dtype=torch.float16, device=x_nhwc.device)
+    check(lib.cfgpp_op_conv3x3_ex(ptr(x_nhwc), c_int(B), c_int(H), c_int(W), c_int(Cin), ptr(w_packed), c_int(Cout),
+                                  ptr(bias), ptr(addend), c_int(addend.stride(0) if addend is not None else 0),
+                                  c_int(add_rows_per_group), ptr(out), c_int(force_bn), c_int(stride), c_int(pad),
+                                  c_int(1 if force_im2col else 0), stream_ptr()))
+    return out
+
+
 def op_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, head_dim: int = 64) -> torch.Tensor:
     """q [B,Nq,H*P], k/v [B,Nkv,H*P] fp16 (views with a row stride are fine) -> [B,Nq,H*P]; P = head_dim rounded up
     to a multiple of 64, the padding columns of every head being zero."""

@@ -93,6 +93,17 @@ CFGPP_API int cfgpp_op_conv3x3_s2(const void* x, int B, int H, int W, int Cin, c
   });
 }
 
+CFGPP_API int cfgpp_op_conv3x3_ex(const void* x, int B, int H, int W, int Cin, const void* w, int Cout, const void* bias,
+                                  const void* addend, int ld_add, int add_rows_per_group, void* out, int force_bn,
+                                  int stride, int pad, int force_im2col, void* stream) {
+  return guarded([&] {
+    GemmOp op = make_conv3x3_op((const __half*)x, B, H, W, Cin, (const __half*)w, Cout, (const __half*)bias,
+                                (const __half*)addend, ld_add, add_rows_per_group, (__half*)out, force_bn, stride, pad,
+                                force_im2col != 0);
+    run_gemm_op(op, (cudaStream_t)stream);
+  });
+}
+
 CFGPP_API int cfgpp_op_attention(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out,
                                  int ldo, int B, int H, int Nq, int Nkv, int head_dim, void* stream) {
   return guarded([&] {

@@ -127,6 +127,16 @@ CFGPP_DEVICE void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* 
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// im2col load through a rank-4 im2col map (host.h make_tmap_im2col_f16): the pixel walk starts at box coordinate
+// (w, h) of image n, channels [c, c + channels_per_pixel); every pixel read is shifted by (off_w, off_h).
+CFGPP_DEVICE void tma_load_im2col_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h, int n,
+                                     uint16_t off_w, uint16_t off_h) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
+      "[%2], {%7, %8};" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h)
+      : "memory");
+}
 
 // TMA store smem -> global (bulk async-group completion)
 CFGPP_DEVICE void tma_store_2d(const CUtensorMap* map, const void* smem_src, int c0, int c1) {

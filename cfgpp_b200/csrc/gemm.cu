@@ -210,8 +210,13 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
             const int tap = kb / p.cpb;
             const int cb = kb - tap * p.cpb;
             const int kh = tap / 3, kw = tap - kh * 3;
-            tma_load_4d(sa, &map_a, &full_bar[stage], cb * BK, w0 * p.conv_stride + kw - p.conv_pad,
-                        h0 * p.conv_stride + kh - p.conv_pad, img);
+            if (p.conv_im2col)  // the walk starts at the tile's first output pixel; the tap is the load's offset
+              tma_load_im2col_4d(sa, &map_a, &full_bar[stage], cb * BK, w0 * p.conv_stride - p.conv_pad,
+                                 h0 * p.conv_stride - p.conv_pad, img, static_cast<uint16_t>(kw),
+                                 static_cast<uint16_t>(kh));
+            else
+              tma_load_4d(sa, &map_a, &full_bar[stage], cb * BK, w0 * p.conv_stride + kw - p.conv_pad,
+                          h0 * p.conv_stride + kh - p.conv_pad, img);
           } else {
             const int k0 = kb * BK;
             if (k0 < p.k_split)
@@ -747,34 +752,45 @@ GemmOp make_linear_op(const __half* a, int lda, const __half* a2, int lda2, int 
 
 GemmOp make_conv3x3_op(const __half* x, int B, int H, int W, int Cin, const __half* w, int Cout, const __half* bias,
                        const __half* addend, int ld_add, int add_rows_per_group, __half* out, int force_bn, int stride,
-                       int pad) {
+                       int pad, bool force_im2col) {
   GemmOp op{};
   GemmParams& p = op.p;
   CFGPP_REQUIRE(stride == 1 || stride == 2, "conv3x3 stride must be 1 or 2");
   CFGPP_REQUIRE(pad == 1 || (pad == 0 && stride == 2), "conv3x3 pad: 1, or 0 with stride 2 (zero row / column after the image)");
   CFGPP_REQUIRE(Cin % BK == 0, "conv3x3 Cin must be a multiple of 64");
   CFGPP_REQUIRE(Cout % 8 == 0, "conv3x3 Cout must be a multiple of 8");
+  CFGPP_REQUIRE(B >= 1 && H >= stride && W >= stride, "conv3x3 needs a non-empty input");
   CFGPP_REQUIRE(stride == 1 || (H % 2 == 0 && W % 2 == 0), "stride-2 conv3x3 needs even H, W");
   const int Ho = H / stride, Wo = W / stride;  // output size (pad 1, kernel 3)
-  CFGPP_REQUIRE(conv3x3_geometry_supported(Ho, Wo),
-                "conv3x3 needs W % 128 == 0, or a power-of-two W <= 128 with H a multiple of 128 / W (or H * W dividing 128)");
-  const int Wt = Wo < BM ? Wo : BM;
-  const int Ht = (BM / Wt) < Ho ? (BM / Wt) : Ho;
-  const int Nt = BM / (Wt * Ht);
+  const bool im2col = force_im2col || !conv3x3_geometry_supported(Ho, Wo);
   p.M = B * Ho * Wo; p.N = Cout; p.K = 9 * Cin;
   p.num_k_blocks = 9 * (Cin / BK);
   p.conv = 1; p.cpb = Cin / BK; p.H = Ho; p.W = Wo; p.conv_stride = stride; p.conv_pad = pad;
+  p.conv_im2col = im2col ? 1 : 0;
   p.k_split = p.K;
   p.bias = bias; p.addend = addend; p.ld_add = ld_add;
   p.add_rows_per_group = add_rows_per_group < 1 ? 1 : add_rows_per_group;
   p.out = out; p.ldc = Cout; p.geglu = 0;
-  // the A tile of tap (kh, kw): output pixel (y, x) reads input pixel (stride * y + kh - pad, stride * x + kw - pad); the
-  // box spans stride * extent input pixels and the tensor map's element strides pick every stride-th one
+  // the A tile of tap (kh, kw): output pixel (y, x) reads input pixel (stride * y + kh - pad, stride * x + kw - pad)
   uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
   uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-  uint32_t box[4] = {64, (uint32_t)(Wt * stride), (uint32_t)(Ht * stride), (uint32_t)Nt};
   uint32_t estr[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
-  op.map_a = make_tmap_f16(x, 4, dims, strides, box, 128, estr);
+  if (im2col) {
+    // The walk's base pixel of output (y, x) is (stride * y - pad, stride * x - pad): the box starts at -pad and ends
+    // where the last output's base lies, one pixel before the last input pixel (upper corner -1) for all three modes
+    // (stride 1 pad 1: -1 .. W-2; stride 2 pad 1: -1 .. W-2, every 2nd = W/2 pixels; stride 2 pad 0: 0 .. W-2, every
+    // 2nd = W/2 pixels). The taps' offsets (kw, kh) in 0..2 reach up to one pixel past the image: zero fill.
+    const int lower[2] = {-pad, -pad};
+    const int upper[2] = {-1, -1};
+    op.map_a = make_tmap_im2col_f16(x, 4, dims, strides, lower, upper, BK, BM, estr, 128);
+  } else {
+    // the box spans stride * extent input pixels and the tensor map's element strides pick every stride-th one
+    const int Wt = Wo < BM ? Wo : BM;
+    const int Ht = (BM / Wt) < Ho ? (BM / Wt) : Ho;
+    const int Nt = BM / (Wt * Ht);
+    uint32_t box[4] = {64, (uint32_t)(Wt * stride), (uint32_t)(Ht * stride), (uint32_t)Nt};
+    op.map_a = make_tmap_f16(x, 4, dims, strides, box, 128, estr);
+  }
   op.map_a2 = op.map_a;
   finish_op(op, w, force_bn, false);
   return op;

@@ -8,7 +8,12 @@
 //                two tensors, used by the 1x1 shortcut conv on torch.cat([h, skip]) in up-blocks).
 //   conv3x3    : stride 1, pad 1. A through a 4D tensor map (C, W, H, B); the K loop walks the 9 taps and
 //                issues shifted TMA box loads whose out-of-bounds pixels are zero-filled by the hardware
-//                (= the padding). Weight packed as [Cout][tap][Cin].
+//                (= the padding). Weight packed as [Cout][tap][Cin]. Two ways to fetch the A tile (the 128
+//                consecutive output pixels m0 .. m0 + 127 in N·H·W order), chosen by make_conv3x3_op:
+//                  tiled  : a 4-D box (64 ch, Wt, Ht, Nt) of whole row segments / rows / images — only where 128
+//                           pixels form such a box (conv3x3_geometry_supported);
+//                  im2col : an im2col tensor map whose 128-pixel walk wraps across row and image ends, the tap
+//                           being the load's (kw, kh) offset — any geometry. Same smem tile, same k order.
 // Epilogue (mirrors the rounding points of the reference's fp16 autocast graph):
 //   t = fp16(acc + bias[n]);  out = addend ? fp16(float(t) + float(addend)) : t
 //   addend is either a full residual [M, ld_add] or a per-sample row broadcast [M / add_rows_per_group][ld_add]
@@ -29,6 +34,7 @@ struct GemmParams {
   int conv_stride;  // conv: 1, or 2 (Downsample2D: the A tile is fetched through a tensor map with element strides 2)
   int conv_pad;     // conv: 1 (symmetric zero padding), or 0 with stride 2 (the VAE encoder's Downsample2D pads one zero
                     // row / column AFTER the image: taps at 2y + kh, out-of-image reads are the TMA's zero fill)
+  int conv_im2col;  // conv: 0 = A tile through the tiled 4-D box, 1 = through the im2col map (any output geometry)
   int k_split;  // linear: first K index served by the second A map (== K when single-source)
   int raster;   // tile walk: 0 = M-fastest (tile = n * m_groups + m), 1 = N-fastest (tile = m * n_blocks + n)
   const __half* bias;
@@ -73,9 +79,11 @@ GemmOp make_linear_op(const __half* a, int lda, const __half* a2, int lda2, int 
 // Conv3x3 stride 1 pad 1 on NHWC input x [B,H,W,Cin], weight [Cout][9][Cin], out NHWC [B,H,W,Cout].
 // stride 2: x is [B,H,W,Cin] with even H, W; out is [B,H/2,W/2,Cout]; pad 1 (UNet Downsample2D) or pad 0 (the
 // AutoencoderKL encoder's: F.pad(x, (0, 1, 0, 1)) followed by an un-padded stride-2 convolution).
+// The A tile comes through the tiled box where conv3x3_geometry_supported(output H, W) holds, through the im2col map
+// otherwise; force_im2col (tests, A/B timing) takes the im2col map for every geometry.
 GemmOp make_conv3x3_op(const __half* x, int B, int H, int W, int Cin, const __half* w, int Cout,
                        const __half* bias, const __half* addend, int ld_add, int add_rows_per_group, __half* out,
-                       int force_bn = 0, int stride = 1, int pad = 1);
+                       int force_bn = 0, int stride = 1, int pad = 1, bool force_im2col = false);
 
 void run_gemm_op(const GemmOp& op, cudaStream_t stream);
 
@@ -95,7 +103,8 @@ class StreamKScope {
   unsigned* prev_flags_;
 };
 
-// Geometry the implicit-GEMM A tile (a 4-D TMA box of 128 consecutive output pixels) can address:
+// Geometry the tiled A tile (a 4-D TMA box of 128 consecutive output pixels) can address — every other geometry takes
+// the im2col A tile:
 //   W > 128           : W % 128 == 0 (a tile = a 128-pixel row segment), any H;
 //   W <= 128, pow2    : a tile = 128 / W whole rows: H must be a multiple of that (e.g. 96 x 128, 48 x 64, 24 x 32 —
 //                       the landscape aspect buckets), or, for images smaller than a tile, H * W must divide 128
@@ -106,6 +115,14 @@ inline bool conv3x3_geometry_supported(int H, int W) {
   if ((W & (W - 1)) != 0) return false;
   const int rows = 128 / W;
   return H >= rows ? (H % rows == 0) : (128 % (H * W) == 0);
+}
+
+// Latent sizes the model handles accept beyond the tiled geometry: with the im2col A tile any level runs, but the
+// handles take those shapes only for latents of at least 64 x 64 (images of 512 px a side and more — the training
+// resolutions of SD v1.5 / SDXL start there).
+constexpr int kIm2colMinLatentSide = 64;
+inline bool latent_allows_im2col(int h_lat, int w_lat) {
+  return h_lat >= kIm2colMinLatentSide && w_lat >= kIm2colMinLatentSide;
 }
 
 }  // namespace cfgpp

@@ -58,6 +58,16 @@ inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
 CUtensorMap make_tmap_f16(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                           const uint32_t* box, int swizzle_bytes = 128, const uint32_t* elem_strides = nullptr);
 
+// fp16 im2col tensor map (rank 3..5, dims / strides as above, NHWC-like: dim 0 = channels, last dim = images).
+// A load walks `pixels_per_column` consecutive pixels of the bounding box in W, H, (D,) N order — wrapping at row and
+// image ends — and fetches `channels_per_pixel` channels of each. Along each spatial dim the box spans coordinates
+// [lower, dim - 1 + upper] (per-dim arrays, innermost spatial dim first; rank 4: each in [-128, 127]) and the walk
+// takes every elem_strides[i]-th one from `lower`; the load's 16-bit offsets shift every pixel it reads (the filter
+// tap), out-of-bounds pixels are zero-filled.
+CUtensorMap make_tmap_im2col_f16(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                                 const int* lower, const int* upper, uint32_t channels_per_pixel,
+                                 uint32_t pixels_per_column, const uint32_t* elem_strides, int swizzle_bytes = 128);
+
 // 2D row-major [rows][cols] fp16 with leading dimension ld (elements); box = (64 cols, box_rows).
 CUtensorMap make_tmap_2d(const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows);
 // epilogue tiles: box = (32 cols = 64 B, box_rows), 64B swizzle (output stores / residual loads)

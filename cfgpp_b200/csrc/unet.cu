@@ -559,9 +559,15 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
     const int down = 1 << (d_.num_levels - 1);
     CFGPP_REQUIRE(h_lat >= down && w_lat >= down && h_lat % down == 0 && w_lat % down == 0,
                   "latent H, W must be multiples of 2^(num_levels-1)");
+    // every level tiled-addressable (any size), or a latent of at least 64 x 64 whose other levels take the im2col
+    // A tile
+    bool tiled = true;
     for (int i = 0, h = h_lat, w = w_lat; i < d_.num_levels; ++i, h /= 2, w /= 2)
-      CFGPP_REQUIRE(conv3x3_geometry_supported(h, w),
-                    "conv3x3 tiler: unsupported level geometry " + std::to_string(h) + "x" + std::to_string(w));
+      tiled = tiled && conv3x3_geometry_supported(h, w);
+    CFGPP_REQUIRE(tiled || latent_allows_im2col(h_lat, w_lat),
+                  "latent " + std::to_string(h_lat) + "x" + std::to_string(w_lat) +
+                      ": a latent whose levels are not all tiled-addressable (W % 128 == 0, or a power-of-two W <= 128 "
+                      "with H a multiple of 128 / W) must be at least 64 x 64 (512 px images)");
   }
   CFGPP_CHECK_CUDA(cudaSetDevice(device_));
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());

@@ -185,9 +185,11 @@ void VaeDecoder::prepare(int batch, int h_lat, int w_lat) {
   CFGPP_REQUIRE(batch >= 1 && batch <= 16, "decode batch must be 1..16");
   CFGPP_REQUIRE(h_lat >= 8 && w_lat >= 8 && (h_lat * w_lat) % 64 == 0, "latent H * W must be a multiple of 64");
   const int L = d_.num_levels;
-  for (int i = 0, h = h_lat, w = w_lat; i < L; ++i, h *= 2, w *= 2)
-    CFGPP_REQUIRE(conv3x3_geometry_supported(h, w),
-                  "conv3x3 tiler: unsupported decoder level geometry " + std::to_string(h) + "x" + std::to_string(w));
+  bool tiled = true;  // every level tiled-addressable, or a latent of at least 64 x 64 (im2col A tiles elsewhere)
+  for (int i = 0, h = h_lat, w = w_lat; i < L; ++i, h *= 2, w *= 2) tiled = tiled && conv3x3_geometry_supported(h, w);
+  CFGPP_REQUIRE(tiled || latent_allows_im2col(h_lat, w_lat),
+                "latent " + std::to_string(h_lat) + "x" + std::to_string(w_lat) +
+                    ": a latent whose decoder levels are not all tiled-addressable must be at least 64 x 64 (512 px images)");
   CFGPP_CHECK_CUDA(cudaSetDevice(device_));
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
   StreamKScope sk_scope(sk_ws_, sk_flags_);  // the decoder's GEMM ops use its own stream-K workspace
@@ -304,9 +306,14 @@ void VaeDecoder::prepare_encode(int batch, int H, int W) {
   const int f = 1 << (L - 1);
   CFGPP_REQUIRE(H >= 8 * f && W >= 8 * f && H % f == 0 && W % f == 0, "image size must be a multiple of the VAE factor");
   CFGPP_REQUIRE(((H / f) * (W / f)) % 64 == 0, "latent H * W must be a multiple of 64");
-  for (int i = 0, h = H, w = W; i < L; ++i, h /= 2, w /= 2)
-    CFGPP_REQUIRE(conv3x3_geometry_supported(h, w) && w % 4 == 0,
-                  "conv3x3 tiler: unsupported encoder level geometry " + std::to_string(h) + "x" + std::to_string(w));
+  bool tiled = true;  // every level tiled-addressable, or a latent of at least 64 x 64 (im2col A tiles elsewhere)
+  for (int i = 0, h = H, w = W; i < L; ++i, h /= 2, w /= 2) {
+    CFGPP_REQUIRE(w % 4 == 0, "encoder level width " + std::to_string(w) + " must be a multiple of 4");
+    tiled = tiled && conv3x3_geometry_supported(h, w);
+  }
+  CFGPP_REQUIRE(tiled || latent_allows_im2col(H / f, W / f),
+                "image " + std::to_string(H) + "x" + std::to_string(W) +
+                    ": an image whose encoder levels are not all tiled-addressable must be at least 512 x 512 px");
   CFGPP_CHECK_CUDA(cudaSetDevice(device_));
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
   StreamKScope sk_scope(sk_ws_, sk_flags_);

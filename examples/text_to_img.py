@@ -8,6 +8,7 @@ from types import SimpleNamespace
 
 import torch
 
+from cfgpp_b200.batching import draw_latents
 from cfgpp_b200.checkpoints import solver_components
 from cfgpp_b200.latent_diffusion import get_solver
 from cfgpp_b200.latent_sdxl import get_solver as get_solver_sdxl
@@ -28,6 +29,10 @@ def main():
     parser.add_argument("--ckpt_dir", type=Path, default=None,
                         help="diffusers-format pipeline directory (unet/, vae/, text_encoder[_2]/, tokenizer[_2]/); "
                              "default: seeded synthetic weights (nothing can be downloaded here)")
+    parser.add_argument("--height", type=int, default=None,
+                        help="image height in pixels (default: the model's native size, 512 for SD v1.5, 1024 for "
+                             "SDXL); a multiple of 8 * 2^(UNet levels - 1), e.g. 1216 x 832 for an SDXL bucket")
+    parser.add_argument("--width", type=int, default=None, help="image width in pixels (default: native size)")
     args = parser.parse_args()
 
     set_seed(args.seed)
@@ -35,16 +40,22 @@ def main():
     solver_config = SimpleNamespace(num_sampling=args.NFE)  # the reference munchifies {'num_sampling': NFE}
     callback = None
 
-    if args.model in ("sdxl", "sdxl_lightning"):
-        extra = solver_components(args.ckpt_dir, "sdxl", args.device) if args.ckpt_dir else {}
-        solver = get_solver_sdxl(args.method, solver_config=solver_config, device=args.device, **extra)
+    sdxl = args.model in ("sdxl", "sdxl_lightning")
+    extra = solver_components(args.ckpt_dir, "sdxl" if sdxl else "sd15", args.device) if args.ckpt_dir else {}
+    solver = (get_solver_sdxl if sdxl else get_solver)(args.method, solver_config=solver_config, device=args.device,
+                                                       **extra)
+    native = solver.cfg.sample_size * 8
+    height, width = args.height or native, args.width or native
+    if height % 8 or width % 8:
+        raise SystemExit(f"--height / --width must be multiples of 8 (got {height} x {width})")
+    zT = draw_latents((1, 4, height // 8, width // 8))  # N(0, 1) start latent from the seeded CPU generator
+    if sdxl:
         result = solver.sample(prompt1=[args.null_prompt, args.prompt], prompt2=[args.null_prompt, args.prompt],
-                               cfg_guidance=args.cfg_guidance, target_size=(1024, 1024), callback_fn=callback)
+                               cfg_guidance=args.cfg_guidance, original_size=(height, width),
+                               target_size=(height, width), callback_fn=callback, zT=zT)
     else:
-        extra = solver_components(args.ckpt_dir, "sd15", args.device) if args.ckpt_dir else {}
-        solver = get_solver(args.method, solver_config=solver_config, device=args.device, **extra)
         result = solver.sample(prompt=[args.null_prompt, args.prompt], cfg_guidance=args.cfg_guidance,
-                               callback_fn=callback)
+                               callback_fn=callback, zT=zT)
 
     out = args.workdir.joinpath('result/generated.pt')
     torch.save(result, out)

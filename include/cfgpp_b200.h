@@ -245,6 +245,13 @@ int cfgpp_op_conv3x3(const void* x, int B, int H, int W, int Cin, const void* w,
  * (one zero row / column AFTER the image, F.pad(x, (0, 1, 0, 1)) + un-padded convolution). */
 int cfgpp_op_conv3x3_s2(const void* x, int B, int H, int W, int Cin, const void* w, int Cout, const void* bias, int pad,
                         void* out, void* stream);
+/* The implicit-GEMM 3x3 convolution in all its modes: stride 1 / pad 1, stride 2 / pad 1, stride 2 / pad 0 (as above),
+ * with the optional addend of cfgpp_op_conv3x3. The A tile comes through the tiled TMA box where the output geometry
+ * allows it and through the im2col tensor map otherwise (any H, W); force_im2col != 0 takes the im2col map for every
+ * geometry (both modes compute bit-identical results: same tile, same k order). */
+int cfgpp_op_conv3x3_ex(const void* x, int B, int H, int W, int Cin, const void* w, int Cout, const void* bias,
+                        const void* addend, int ld_add, int add_rows_per_group, void* out, int force_bn, int stride,
+                        int pad, int force_im2col, void* stream);
 /* head h of q / k / v / out occupies columns [h*P, h*P + head_dim) with P = head_dim rounded up to a multiple of 64
  * (columns head_dim..P-1 must be zero in q / k / v and come back zero in out). */
 int cfgpp_op_attention(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out, int ldo, int B,
