@@ -4,10 +4,9 @@
 // in fp32 from the fp16 input, and the result is rounded to fp16 exactly once — the point where the reference's
 // fp32 norm output is cast for the following conv / linear.
 //
-// GroupNorm is two launches: (1) per-(sample, pixel-chunk) partial (sum, sum^2) per group, shifted by a pivot value
-// of the group — deterministic, no atomics in global memory; (2) apply, which reduces the partials on the fly. Both
-// take an optional second source so that torch.cat([h, skip], dim=1) of the up-blocks is never materialised
-// un-normalised.
+// GroupNorm is two launches: (1) per-(sample, pixel-chunk) partial (mean, M2) per group — deterministic, no atomics in
+// global memory; (2) apply, which merges the partials on the fly. Both take an optional second source so that
+// torch.cat([h, skip], dim=1) of the up-blocks is never materialised un-normalised.
 //
 // The LayerNorm fold of the transformer blocks (see GemmParams in gemm.cuh) prepares its weights here too.
 #include "common.cuh"
@@ -30,22 +29,44 @@ CFGPP_DEVICE uint4 load_vec(const GnSrc& s, size_t pix, int c) {  // c multiple 
   return *reinterpret_cast<const uint4*>(s.x2 + pix * s.C2 + (c - s.C1));
 }
 
-// Shift of group g's sums: its first channel at pixel 0 of the sample. Sums of (x - K) and (x - K)^2 keep
-// var = Q / n - (S / n)^2 free of the cancellation E[x^2] - E[x]^2 suffers when |mean| >> std (fp32 over up to 4 M
-// elements per group); both kernels load the same K.
-CFGPP_DEVICE float gn_pivot(const GnSrc& s, size_t pix0, int g, int cpg) {
-  const int c = g * cpg;
-  return __half2float(c < s.C1 ? s.x1[pix0 * s.C1 + c] : s.x2[pix0 * s.C2 + (c - s.C1)]);
+// Chan et al.'s pairwise update: a set of na elements absorbs a disjoint set (nb > 0, mean_b, m2_b), m2 being the sum of
+// squared deviations from the set's mean. Every term of the new m2 is >= 0, so nothing cancels. The running mean is
+// kept as ref + off, ref the first set's mean: a chain of merges then rounds at the scale of the spread between the
+// sets' means, not at that of the mean itself (a mean far from 0 would cost one rounding of it per merge).
+CFGPP_DEVICE void chan_merge(float& ref, float& off, float& m2, float na, float nb, float mean_b, float m2_b) {
+  if (na == 0.f) {
+    ref = mean_b;
+    off = 0.f;
+    m2 = m2_b;
+    return;
+  }
+  const float f = __fdividef(nb, na + nb);  // a weight: its 2-ulp error scales d, never the mean itself
+  const float d = (mean_b - ref) - off;
+  off += d * f;
+  m2 += m2_b + d * d * (na * f);
 }
 
-// grid (nchunk, B); block = vpp * k threads (vpp = C / 8 vectors per pixel) so a thread keeps one channel vector.
-// A thread walks up to 2048 pixels of a chunk (VAE levels of 1024^2 pixels); its sums are cascaded (fp32 runs of
-// kRun steps in registers, folded into the thread's shared-memory slot) so that no rounding chain is longer than ~64
-// additions.
-__global__ void gn_stats_kernel(GnSrc src, int HW, int C, int px_per_block, float* __restrict__ partial) {
+// pixels of chunk i, and of the chunks i, i + 8, ... whose partials one of the apply's 8 reduction parts merges
+CFGPP_DEVICE int gn_chunk_pixels(int i, int ppb, int HW) { return min(ppb, HW - i * ppb); }
+CFGPP_DEVICE int gn_part_pixels(int part, int nchunk, int ppb, int HW) {
+  int n = 0;
+  for (int i = part; i < nchunk; i += 8) n += gn_chunk_pixels(i, ppb, HW);
+  return n;
+}
+
+// grid (nchunk, B); block = vpp * k threads (vpp = C / 8 vectors per pixel) so a thread keeps one channel vector and
+// walks every pstep-th pixel of the chunk (up to 2048 of them at the VAE's 1024^2 levels).
+//
+// A thread's statistics come in runs of up to kRunPx pixels: fp32 sums of x - K and (x - K)^2, K the run's own first
+// value, so the shifted sums only cancel over the run's own spread (an outlier of the group costs at most the run it
+// shifts). A finished run becomes (mean, M2) and is merged into the thread's summary by chan_merge; the threads'
+// slots are then merged per group in a fixed order. Counts are never stored: every level recomputes them from the
+// launch geometry. At most 768 threads (C <= 6144, see run_groupnorm), so at most 80 registers a thread.
+__global__ void __launch_bounds__(768)
+    gn_stats_kernel(GnSrc src, int HW, int C, int px_per_block, float* __restrict__ partial) {
   pdl_launch_dependents();
   pdl_wait();
-  extern __shared__ float sm[];  // [pstep][C] sums, then [pstep][C] sums of squares (one slot per thread: no atomics)
+  extern __shared__ float sm[];  // [pstep][C] means, then [pstep][C] M2s (one slot per thread: no atomics)
   const int vpp = C >> 3;
   const int cpg = C / GROUPS;
   const int b = blockIdx.y;
@@ -53,16 +74,16 @@ __global__ void gn_stats_kernel(GnSrc src, int HW, int C, int px_per_block, floa
   const int vec = threadIdx.x % vpp;
   const int prow = threadIdx.x / vpp;
   const int pstep = blockDim.x / vpp;
-  float s[8], q[8], piv[8];
-  float* sq = sm + pstep * C;
-  float* my_s = sm + prow * C + vec * 8;
-  float* my_q = sq + prow * C + vec * 8;
+  float s[8], q[8], piv[8], ref[8], off[8], m2[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    s[i] = q[i] = my_s[i] = my_q[i] = 0.f;
-    piv[i] = gn_pivot(src, static_cast<size_t>(b) * HW, (vec * 8 + i) / cpg, cpg);
-  }
-  // x - K is exact (two nearby fp16 values), and so is its square (<= 24 significant bits)
+  for (int i = 0; i < 8; ++i) s[i] = q[i] = piv[i] = ref[i] = off[i] = m2[i] = 0.f;
+  int nrun = 0, nthr = 0;  // pixels of the open run; pixels already merged into (ref + off, m2)
+  auto set_pivot = [&](const uint4& u) {
+    const __half* h = reinterpret_cast<const __half*>(&u);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) piv[i] = __half2float(h[i]);
+  };
+  // x - K is exact when x and K are within a factor of 2 (Sterbenz); otherwise it rounds once, like any fp32 sum term
   auto accumulate = [&](const uint4& u) {
     const __half2* h = reinterpret_cast<const __half2*>(&u);
 #pragma unroll
@@ -76,90 +97,101 @@ __global__ void gn_stats_kernel(GnSrc src, int HW, int C, int px_per_block, floa
     }
   };
   auto fold = [&]() {
+    if (nrun == 0) return;
+    const float nr = static_cast<float>(nrun), rn = __frcp_rn(nr);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      my_s[i] += s[i];
-      my_q[i] += q[i];
+      const float dm = s[i] * rn;
+      chan_merge(ref[i], off[i], m2[i], static_cast<float>(nthr), nr, piv[i] + dm, fmaxf(q[i] - s[i] * dm, 0.f));
       s[i] = q[i] = 0.f;
     }
+    nthr += nrun;
+    nrun = 0;
   };
   const int p0 = chunk * px_per_block;
   const int pend = min(px_per_block, HW - p0);
   const size_t base = static_cast<size_t>(b) * HW + p0;
-  constexpr int U = 4;  // independent 16 B loads in flight per thread
-  constexpr int kRun = 8;  // steps (U pixels each) per fp32 run
-  int pp = prow, run = 0;
+  constexpr int U = 4;        // independent 16 B loads in flight per thread
+  constexpr int kRunPx = 32;  // pixels per run (a multiple of U; the tail loop below adds at most U - 1)
+  int pp = prow;
   for (; pp + (U - 1) * pstep < pend; pp += U * pstep) {
     uint4 u[U];
 #pragma unroll
     for (int j = 0; j < U; ++j) u[j] = load_vec(src, base + pp + j * pstep, vec * 8);
+    if (nrun == 0) set_pivot(u[0]);
 #pragma unroll
     for (int j = 0; j < U; ++j) accumulate(u[j]);
-    if (++run == kRun) {
-      fold();
-      run = 0;
-    }
+    nrun += U;
+    if (nrun == kRunPx) fold();
   }
-  for (; pp < pend; pp += pstep) accumulate(load_vec(src, base + pp, vec * 8));
+  for (; pp < pend; pp += pstep) {
+    const uint4 u = load_vec(src, base + pp, vec * 8);
+    if (nrun == 0) set_pivot(u);
+    accumulate(u);
+    ++nrun;
+  }
   fold();
+  float* sq = sm + pstep * C;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    sm[prow * C + vec * 8 + i] = ref[i] + off[i];
+    sq[prow * C + vec * 8 + i] = m2[i];
+  }
   __syncthreads();
-  if (threadIdx.x < GROUPS) {  // fixed summation order -> bit-reproducible statistics
-    float a = 0.f, bsum = 0.f;
-    for (int r = 0; r < pstep; ++r)
+  if (threadIdx.x < GROUPS) {  // fixed merge order -> bit-reproducible statistics
+    float a = 0.f, o = 0.f, m = 0.f, n = 0.f;
+    for (int r = 0; r < pstep && r < pend; ++r) {
+      const float nr = static_cast<float>((pend - 1 - r) / pstep + 1);  // pixels of the threads in row r
       for (int i = 0; i < cpg; ++i) {
-        a += sm[r * C + threadIdx.x * cpg + i];
-        bsum += sq[r * C + threadIdx.x * cpg + i];
+        chan_merge(a, o, m, n, nr, sm[r * C + threadIdx.x * cpg + i], sq[r * C + threadIdx.x * cpg + i]);
+        n += nr;
       }
+    }
     float* dst = partial + ((static_cast<size_t>(b) * gridDim.x + chunk) * GROUPS + threadIdx.x) * 2;
-    dst[0] = a;
-    dst[1] = bsum;
+    dst[0] = a + o;
+    dst[1] = m;
   }
 }
 
 // grid (nchunk, B); block = vpp * k threads: a thread owns one 8-channel vector, so the per-channel affine
-// (x - mean) * rstd * gamma + beta = (x - K) * a + c (a = rstd * gamma, c = beta - (mean - K) * a) uses 24 registers
-// set up once per thread. x - K is exact (two nearby fp16 values), so a large mean costs no fp32 rounding of its own.
+// (x - mean) * a + beta (a = rstd * gamma) uses 24 registers set up once per thread.
 __global__ void gn_apply_kernel(GnSrc src, int HW, int C, int px_per_block, const float* __restrict__ partial,
                                 int nchunk, const __half* __restrict__ gamma, const __half* __restrict__ beta,
                                 float eps, int silu, __half* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
-  __shared__ float s_piv[GROUPS], s_dm[GROUPS], s_rstd[GROUPS];
+  __shared__ float s_mean[GROUPS], s_rstd[GROUPS];
   __shared__ float2 s_part[8][GROUPS];
   const int b = blockIdx.y;
-  // Cross-chunk reduction of the partial sums, spread over 8 x 32 threads (each sums every 8th chunk, loads
-  // independent), then combined in a fixed order: a single thread per group walking all (up to 128) chunks exposed
-  // ~10 us of serialised L2 latency at the head of EVERY block.
+  const int cpg = C / GROUPS;
+  // Cross-chunk merge of the partials, spread over 8 x 32 threads (each merges every 8th chunk, loads independent),
+  // then combined in a fixed order: a single thread per group walking all (up to 128) chunks exposed ~10 us of
+  // serialised L2 latency at the head of EVERY block.
   for (int idx = threadIdx.x; idx < 8 * GROUPS; idx += blockDim.x) {
     const int g = idx & (GROUPS - 1), part = idx / GROUPS;
-    float a = 0.f, q = 0.f;
+    float a = 0.f, o = 0.f, m = 0.f, n = 0.f;
     const float* src_p = partial + (static_cast<size_t>(b) * nchunk * GROUPS + g) * 2;
     for (int i = part; i < nchunk; i += 8) {
       const float2 v = *reinterpret_cast<const float2*>(src_p + static_cast<size_t>(i) * GROUPS * 2);
-      a += v.x;
-      q += v.y;
+      const float ni = static_cast<float>(gn_chunk_pixels(i, px_per_block, HW) * cpg);
+      chan_merge(a, o, m, n, ni, v.x, v.y);
+      n += ni;
     }
-    s_part[part][g] = make_float2(a, q);
+    s_part[part][g] = make_float2(a + o, m);
   }
   __syncthreads();
   if (threadIdx.x < GROUPS) {
-    float a = 0.f, q = 0.f;
-#pragma unroll
-    for (int part = 0; part < 8; ++part) {
-      a += s_part[part][threadIdx.x].x;
-      q += s_part[part][threadIdx.x].y;
+    float a = 0.f, o = 0.f, m = 0.f, n = 0.f;
+    for (int part = 0; part < 8 && part < nchunk; ++part) {
+      const float np = static_cast<float>(gn_part_pixels(part, nchunk, px_per_block, HW) * cpg);
+      chan_merge(a, o, m, n, np, s_part[part][threadIdx.x].x, s_part[part][threadIdx.x].y);
+      n += np;
     }
-    // the partials are sums of (x - K), (x - K)^2 with the group's pivot K (gn_pivot): mean = K + dm
-    const float n = static_cast<float>(HW) * (C / GROUPS);
-    const float dm = a / n;
-    const float var = fmaxf(q / n - dm * dm, 0.f);
-    s_piv[threadIdx.x] = gn_pivot(src, static_cast<size_t>(b) * HW, threadIdx.x, C / GROUPS);
-    s_dm[threadIdx.x] = dm;
-    s_rstd[threadIdx.x] = rsqrtf(var + eps);
+    s_mean[threadIdx.x] = a + o;
+    s_rstd[threadIdx.x] = rsqrtf(m / (static_cast<float>(HW) * (C / GROUPS)) + eps);
   }
   __syncthreads();
   const int vpp = C >> 3;
-  const int cpg = C / GROUPS;
   const int vec = threadIdx.x % vpp;
   const int prow = threadIdx.x / vpp;
   const int pstep = blockDim.x / vpp;
@@ -168,13 +200,13 @@ __global__ void gn_apply_kernel(GnSrc src, int HW, int C, int px_per_block, cons
   const uint4 ub = *reinterpret_cast<const uint4*>(beta + c0);
   const __half* hg = reinterpret_cast<const __half*>(&ug);
   const __half* hb = reinterpret_cast<const __half*>(&ub);
-  float piv[8], sc[8], sh[8];  // pivot K, a, c of each of this thread's 8 channels
+  float mu[8], sc[8], sh[8];  // mean, a, beta of each of this thread's 8 channels
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     const int g = (c0 + k) / cpg;
-    piv[k] = s_piv[g];
+    mu[k] = s_mean[g];
     sc[k] = s_rstd[g] * __half2float(hg[k]);
-    sh[k] = __half2float(hb[k]) - s_dm[g] * sc[k];
+    sh[k] = __half2float(hb[k]);
   }
   const int p0 = blockIdx.x * px_per_block;
   const int pend = min(px_per_block, HW - p0);
@@ -185,7 +217,7 @@ __global__ void gn_apply_kernel(GnSrc src, int HW, int C, int px_per_block, cons
     float y[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      float v = (__half2float(hx[k]) - piv[k]) * sc[k] + sh[k];
+      float v = (__half2float(hx[k]) - mu[k]) * sc[k] + sh[k];
       if (silu) v = silu_f(v);
       y[k] = v;
     }
@@ -323,8 +355,10 @@ void run_groupnorm(const __half* x1, int C1, const __half* x2, int C2, int B, in
   int k = 256 / vpp;
   if (k < 1) k = 1;
   const int threads = vpp * k;
-  CFGPP_REQUIRE(threads <= 1024, "GroupNorm channel count too large");
   const size_t stats_smem = 2 * static_cast<size_t>(k) * C * sizeof(float);
+  // gn_stats_kernel keeps one (mean, M2) slot per thread and channel in the default 48 KB of dynamic shared memory
+  // (no opt-in): C <= 6144, far above any model's channel count
+  CFGPP_REQUIRE(threads <= 1024 && stats_smem <= 48 * 1024, "GroupNorm channel count too large (C <= 6144)");
   launch_pdl(gn_stats_kernel, dim3(nchunk, B), dim3(threads), stats_smem, stream, src, HW, C,
              ppb, partial);
   launch_pdl(gn_apply_kernel, dim3(nchunk, B), dim3(threads), 0, stream, src, HW, C, ppb, partial, nchunk, gamma, beta, eps,
