@@ -51,6 +51,15 @@ def ptr(t: torch.Tensor | None) -> c_void_p:
     return c_void_p(t.data_ptr())
 
 
+def rows_ptr(t: torch.Tensor | None) -> c_void_p:
+    """A 2-D operand the kernel addresses by rows with its own leading dimension (t.stride(0)): column slices of a
+    wider buffer are fine, the columns themselves must be contiguous."""
+    if t is None:
+        return c_void_p(0)
+    assert t.is_cuda and t.dim() == 2 and t.stride(1) == 1, "row-addressed operands need contiguous columns"
+    return c_void_p(t.data_ptr())
+
+
 def stream_ptr() -> c_void_p:
     return c_void_p(torch.cuda.current_stream().cuda_stream)
 
@@ -70,7 +79,8 @@ def op_linear(a: torch.Tensor, w: torch.Tensor, bias=None, addend=None, add_rows
               out: torch.Tensor | None = None, force_streamk: bool = False) -> torch.Tensor:
     """out = epilogue(cat([a, a2], -1) @ w.T); a [M,K1] fp16, w [N,K] fp16 (already packed for GEGLU). `out` may be
     given, also as the residual `addend` itself (in-place residual add). `force_streamk` takes the stream-K remainder
-    split that linear layers otherwise skip (tests of its fix-up path)."""
+    split that linear layers otherwise skip (tests of its fix-up path). a, a2 and addend may be column slices of wider
+    buffers (their row stride is passed as the leading dimension)."""
     lib = load()
     M, K1 = a.shape
     K = K1 + (a2.shape[1] if a2 is not None else 0)
@@ -78,12 +88,55 @@ def op_linear(a: torch.Tensor, w: torch.Tensor, bias=None, addend=None, add_rows
     assert w.shape[1] == K and a.dtype == torch.float16 and w.dtype == torch.float16
     n_out = N // 2 if geglu else N
     out = _linear_out(out, M, n_out, a.device)
-    check(lib.cfgpp_op_linear(ptr(a), c_int(a.stride(0)), ptr(a2), c_int(a2.stride(0) if a2 is not None else 0),
-                              c_int(K1), ptr(w), c_int(M), c_int(N), c_int(K), ptr(bias), ptr(addend),
-                              c_int(addend.stride(0) if addend is not None else 0), c_int(add_rows_per_group),
-                              ptr(out), c_int(n_out), c_int(1 if geglu else 0), c_int(force_bn),
-                              c_int(1 if force_streamk else 0), stream_ptr()))
+    check(lib.cfgpp_op_linear(*_linear_args(a, w, bias, addend, add_rows_per_group, a2, geglu, force_bn, ptr(out),
+                                            force_streamk), stream_ptr()))
     return out
+
+
+def _linear_args(a, w, bias, addend, add_rows_per_group, a2, geglu, force_bn, out_ptr, force_streamk):
+    M, K1 = a.shape
+    N, K = w.shape
+    return (rows_ptr(a), c_int(a.stride(0)), rows_ptr(a2), c_int(a2.stride(0) if a2 is not None else 0), c_int(K1),
+            ptr(w), c_int(M), c_int(N), c_int(K), ptr(bias), rows_ptr(addend),
+            c_int(addend.stride(0) if addend is not None else 0), c_int(add_rows_per_group), out_ptr,
+            c_int(N // 2 if geglu else N), c_int(1 if geglu else 0), c_int(force_bn), c_int(1 if force_streamk else 0))
+
+
+_SCHEDULE_FIELDS = ("bn", "grid", "tiles", "streamk", "sk_tiles", "max_pieces", "a_mode", "k_blocks")
+A_MODES = ("linear", "tiled", "im2col")
+
+
+def _schedule(conv, args):
+    info = (c_int * 8)()
+    check(load().cfgpp_dbg_gemm_schedule(c_int(conv), *args, info))
+    s = dict(zip(_SCHEDULE_FIELDS, info))
+    s["streamk"] = bool(s["streamk"])
+    s["a_mode"] = A_MODES[s["a_mode"]]
+    return s
+
+
+def linear_schedule(a: torch.Tensor, w: torch.Tensor, bias=None, addend=None, add_rows_per_group: int = 1,
+                    a2: torch.Tensor | None = None, geglu: bool = False, force_bn: int = 0,
+                    out: torch.Tensor | None = None, force_streamk: bool = False) -> dict:
+    """The schedule op_linear would run with these arguments, without launching it (debug entry point): {bn, grid,
+    tiles, streamk, sk_tiles, max_pieces, a_mode, k_blocks}. It depends on the card's SM count. Nothing is written:
+    without `out`, the output's tensor map is encoded over w's address."""
+    args = _linear_args(a, w, bias, addend, add_rows_per_group, a2, geglu, force_bn, ptr(out if out is not None else w),
+                        force_streamk)
+    return _schedule(0, (*args, c_int(1), c_int(1), c_int(1), c_int(1), c_int(0)))
+
+
+def conv3x3_schedule(x_nhwc: torch.Tensor, w_packed: torch.Tensor, bias=None, addend=None, add_rows_per_group: int = 1,
+                     stride: int = 1, pad: int = 1, force_im2col: bool = False, force_bn: int = 0) -> dict:
+    """The schedule op_conv3x3_ex would run with these arguments, without launching it (see linear_schedule; the
+    output's tensor map is encoded over x's address)."""
+    B, H, W, Cin = x_nhwc.shape
+    Cout = w_packed.shape[0]
+    return _schedule(1, (ptr(x_nhwc), c_int(Cin), c_void_p(0), c_int(0), c_int(0), ptr(w_packed), c_int(B),
+                         c_int(Cout), c_int(9 * Cin), ptr(bias), rows_ptr(addend),
+                         c_int(addend.stride(0) if addend is not None else 0), c_int(add_rows_per_group), ptr(x_nhwc),
+                         c_int(Cout), c_int(0), c_int(force_bn), c_int(0), c_int(H), c_int(W), c_int(stride), c_int(pad),
+                         c_int(1 if force_im2col else 0)))
 
 
 def op_linear_stats(a: torch.Tensor, w: torch.Tensor, bn: int, bias=None, addend=None, add_rows_per_group: int = 1,
@@ -176,7 +229,7 @@ def op_conv3x3_ex(x_nhwc: torch.Tensor, w_packed: torch.Tensor, bias=None, adden
     assert w_packed.shape[1] == 9 * Cin
     out = torch.empty((B, H // stride, W // stride, Cout), dtype=torch.float16, device=x_nhwc.device)
     check(lib.cfgpp_op_conv3x3_ex(ptr(x_nhwc), c_int(B), c_int(H), c_int(W), c_int(Cin), ptr(w_packed), c_int(Cout),
-                                  ptr(bias), ptr(addend), c_int(addend.stride(0) if addend is not None else 0),
+                                  ptr(bias), rows_ptr(addend), c_int(addend.stride(0) if addend is not None else 0),
                                   c_int(add_rows_per_group), ptr(out), c_int(force_bn), c_int(stride), c_int(pad),
                                   c_int(1 if force_im2col else 0), stream_ptr()))
     return out

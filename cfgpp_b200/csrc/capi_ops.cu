@@ -74,6 +74,28 @@ CFGPP_API int cfgpp_dbg_linear_timeline(const void* a, int lda, const void* w, i
   });
 }
 
+// Debug aid (not in the public header): the schedule cfgpp_op_linear (conv == 0) or cfgpp_op_conv3x3_ex (conv == 1)
+// would run with these arguments, without launching it. The conv arguments are ignored for a linear op and the
+// linear-only ones (a2, lda2, k_split, K, ldc, geglu, force_streamk) for a convolution; M, N are the conv's B, Cout and
+// lda its Cin. info[8] = {bn, grid, tiles, streamk, sk_tiles, max_pieces, a_mode, k_blocks} (GemmSchedule).
+CFGPP_API int cfgpp_dbg_gemm_schedule(int conv, const void* a, int lda, const void* a2, int lda2, int k_split,
+                                      const void* w, int M, int N, int K, const void* bias, const void* addend,
+                                      int ld_add, int add_rows_per_group, void* out, int ldc, int geglu, int force_bn,
+                                      int force_streamk, int H, int W, int stride, int pad, int force_im2col,
+                                      int* info) {
+  return guarded([&] {
+    GemmOp op = conv ? make_conv3x3_op((const __half*)a, M, H, W, lda, (const __half*)w, N, (const __half*)bias,
+                                       (const __half*)addend, ld_add, add_rows_per_group, (__half*)out, force_bn,
+                                       stride, pad, force_im2col != 0)
+                     : make_linear_op((const __half*)a, lda, (const __half*)a2, lda2, k_split, (const __half*)w, M, N,
+                                      K, (const __half*)bias, (const __half*)addend, ld_add, add_rows_per_group,
+                                      (__half*)out, ldc, geglu != 0, force_bn, force_streamk != 0);
+    const GemmSchedule s = gemm_schedule(op);
+    const int v[8] = {s.bn, s.grid, s.tiles, s.streamk, s.sk_tiles, s.max_pieces, s.a_mode, s.k_blocks};
+    for (int i = 0; i < 8; ++i) info[i] = v[i];
+  });
+}
+
 CFGPP_API int cfgpp_op_conv3x3(const void* x, int B, int H, int W, int Cin, const void* w, int Cout, const void* bias,
                                const void* addend, int ld_add, int add_rows_per_group, void* out, int force_bn,
                                void* stream) {

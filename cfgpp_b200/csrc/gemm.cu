@@ -796,6 +796,32 @@ GemmOp make_conv3x3_op(const __half* x, int B, int H, int W, int Cin, const __ha
   return op;
 }
 
+GemmSchedule gemm_schedule(const GemmOp& op) {
+  const GemmParams& p = op.p;
+  GemmSchedule s{};
+  s.bn = op.bn;
+  s.grid = op.grid;
+  s.tiles = p.num_m_blocks * p.num_n_blocks;
+  s.streamk = p.sk_ws != nullptr ? 1 : 0;
+  s.a_mode = p.conv ? (p.conv_im2col ? 2 : 1) : 0;
+  s.k_blocks = p.num_k_blocks;
+  s.max_pieces = 1;
+  if (s.streamk && s.tiles % s.grid != 0) {
+    // the kernel's "work schedule": CTA c owns units [c U / P, (c + 1) U / P) of the R * nkb remainder units
+    s.sk_tiles = s.tiles % s.grid;
+    const long units = static_cast<long>(s.sk_tiles) * p.num_k_blocks;
+    auto u0 = [&](int c) { return units * c / s.grid; };
+    for (int t = 0; t < s.sk_tiles; ++t) {
+      const long b = static_cast<long>(t) * p.num_k_blocks, e = b + p.num_k_blocks;
+      int pieces = 0;
+      for (int c = 0; c < s.grid; ++c)
+        if (u0(c + 1) > u0(c) && u0(c) < e && u0(c + 1) > b) ++pieces;
+      s.max_pieces = std::max(s.max_pieces, pieces);
+    }
+  }
+  return s;
+}
+
 void run_gemm_op(const GemmOp& op, cudaStream_t stream) {
   CFGPP_REQUIRE(!(op.p.stats_in && (op.p.addend || op.p.stats_out)),
                 "a LayerNorm-fold consumer GEMM takes no addend and emits no row statistics");

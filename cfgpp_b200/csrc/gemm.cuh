@@ -87,6 +87,17 @@ GemmOp make_conv3x3_op(const __half* x, int B, int H, int W, int Cin, const __ha
 
 void run_gemm_op(const GemmOp& op, cudaStream_t stream);
 
+// The schedule an op will run (tests: which path a launch takes on this card, without launching it).
+struct GemmSchedule {
+  int bn, grid, tiles;
+  int streamk;     // 1: the remainder tiles are split over all CTAs (partials parked in the stream-K workspace)
+  int sk_tiles;    // tiles that take the split (0 without stream-K)
+  int max_pieces;  // the most pieces (CTAs) any tile is split over; 1 without stream-K
+  int a_mode;      // A tile: 0 linear 2-D box, 1 conv tiled 4-D box, 2 conv im2col map
+  int k_blocks;    // 64-wide k-blocks of the main loop
+};
+GemmSchedule gemm_schedule(const GemmOp& op);
+
 // Stream-K workspace ownership (see gemm.cu): a model handle allocates its own buffers and wraps its plan building in a
 // StreamKScope, so ops of different handles — which may run on different streams — never share flags.
 void streamk_alloc(float** ws, unsigned** flags);

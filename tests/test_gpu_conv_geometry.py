@@ -2,29 +2,16 @@
 
 The tiled mode fetches the 128 output pixels of a tile as one 4-D TMA box; the im2col mode walks them through an im2col
 tensor map that wraps across row and image ends, so it addresses any H, W. Both fill the same swizzled smem tile in the
-same k order, so on every shape the tiled mode can address, forcing im2col must give a bit-identical result. On the
-shapes only im2col can address, results are gated against fp32 `conv2d` like `test_gpu_kernels.test_conv3x3` (gate 2e-4
-rel-L2; both sides round the same fp32 sum to fp16), edge pixels gated separately (they read the zero fill)."""
+same k order, so on every shape the tiled mode can address, forcing im2col must give a bit-identical result. Every
+result is also gated element by element against the fp64 reference in the kernel's k order, within the accumulation
+bound of `test_gpu_gemm.py` (edge pixels, which read the zero fill, included)."""
 import pytest
 import torch
 
-from helpers import rel_l2
+from test_gpu_gemm import check_bound, conv_kblocks
 
 pytestmark = pytest.mark.gpu
 dev = torch.device("cuda:0")
-TOL = 2e-4
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _fp32_refs():
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-
-
-def gate(what, got, ref, tol=TOL):
-    e = rel_l2(got, ref)
-    print(f"[conv geometry] {what}: rel-L2 {e:.3e} (gate {tol:.1e})")
-    assert e < tol, f"{what}: rel-L2 {e:.3e} >= {tol:.1e}"
 
 
 def rnd(g, *s, scale=1.0):
@@ -47,20 +34,14 @@ def make_case(seed, B, H, W, Cin, Cout, stride, addend_kind):
     return x, w, bias, addend, rpg, x_nhwc, w_packed
 
 
-def reference(x, w, bias, addend, rpg, stride, pad):
-    """fp32 conv2d, rounded to fp16 at the reference's points: fp16(acc + bias), then fp16(t + addend)."""
-    xf = x.float()
-    if stride == 2 and pad == 0:
-        ref = torch.nn.functional.conv2d(torch.nn.functional.pad(xf, (0, 1, 0, 1)), w.float(), bias.float(), stride=2)
-    else:
-        ref = torch.nn.functional.conv2d(xf, w.float(), bias.float(), stride=stride, padding=1)
-    ref = ref.half()
-    B, Cout, Ho, Wo = ref.shape
-    ref = ref.permute(0, 2, 3, 1).reshape(B * Ho * Wo, Cout)
-    if addend is not None:
-        ad = addend.float().repeat_interleave(rpg, 0) if rpg > 1 else addend.float()
-        ref = (ref.float() + ad).half()
-    return ref
+def gate(what, out, case, stride, pad):
+    """Every element of out within the per-element bound of the fp64 reference (the launch's own schedule decides
+    whether the stream-K term applies)."""
+    from cfgpp_b200 import _native as nv
+    _, _, bias, addend, rpg, x_nhwc, w_packed = case
+    sched = nv.conv3x3_schedule(x_nhwc, w_packed, bias, addend, rpg, stride=stride, pad=pad)
+    check_bound(f"[conv geometry] {what}", out, conv_kblocks(x_nhwc, stride, pad), w_packed, out.shape[0], bias,
+                addend, rpg, sched)
 
 
 def run(nv, case, stride, pad, force_im2col):
@@ -70,12 +51,12 @@ def run(nv, case, stride, pad, force_im2col):
 
 
 # ---- bitwise mode equivalence on tiled-addressable shapes ---------------------------------------------------------
-# every shape of test_gpu_kernels.test_conv3x3 (the last three take the stream-K split), stride 1 / pad 1
+# every shape of test_gpu_gemm.test_conv3x3 (the last three take the stream-K split), stride 1 / pad 1
 TILED_S1 = [(1, 32, 32, 64, 64), (2, 64, 64, 128, 128), (4, 16, 16, 128, 256), (2, 8, 8, 128, 128),
             (1, 128, 128, 320, 320), (4, 32, 32, 1280, 1280), (2, 96, 128, 64, 128), (1, 24, 32, 128, 128),
             (3, 6, 64, 64, 64), (1, 40, 256, 64, 64), (1, 16, 1024, 64, 64), (8, 8, 8, 1280, 1280),
             (8, 8, 8, 2560, 1280)]
-# the stride-2 cases of test_gpu_kernels (pad 1: Downsample2D; pad 0: the AutoencoderKL encoder's pad-after)
+# the stride-2 cases of test_gpu_gemm (pad 1: Downsample2D; pad 0: the AutoencoderKL encoder's pad-after)
 TILED_S2 = [(4, 128, 128, 320, 320, 1), (4, 64, 64, 640, 640, 1), (2, 32, 32, 128, 128, 1), (1, 16, 16, 64, 64, 1),
             (2, 96, 128, 64, 64, 1), (1, 256, 256, 128, 128, 0), (2, 128, 128, 256, 256, 0), (2, 32, 32, 64, 64, 0),
             (1, 64, 128, 128, 128, 0)]
@@ -89,7 +70,7 @@ def test_im2col_equals_tiled_stride1(B, H, W, Cin, Cout, addend_kind):
     tiled = run(nv, case, 1, 1, False)
     im2col = run(nv, case, 1, 1, True)
     assert torch.equal(tiled, im2col), f"{B}x{H}x{W} {Cin}->{Cout} addend={addend_kind}: modes differ"
-    gate(f"tiled {B}x{H}x{W} {Cin}->{Cout} addend={addend_kind}", tiled, reference(*case[:5], 1, 1))
+    gate(f"tiled {B}x{H}x{W} {Cin}->{Cout} addend={addend_kind}", tiled, case, 1, 1)
 
 
 @pytest.mark.parametrize("addend_kind", [None, "temb", "res"])
@@ -100,22 +81,16 @@ def test_im2col_equals_tiled_stride2(B, H, W, Cin, Cout, pad, addend_kind):
     tiled = run(nv, case, 2, pad, False)
     im2col = run(nv, case, 2, pad, True)
     assert torch.equal(tiled, im2col), f"s2 pad {pad} {B}x{H}x{W} {Cin}->{Cout} addend={addend_kind}: modes differ"
-    gate(f"tiled s2 pad {pad} {B}x{H}x{W} {Cin}->{Cout} addend={addend_kind}", tiled, reference(*case[:5], 2, pad))
+    gate(f"tiled s2 pad {pad} {B}x{H}x{W} {Cin}->{Cout} addend={addend_kind}", tiled, case, 2, pad)
 
 
-# ---- geometries only the im2col A tile addresses, against fp32 conv2d ----------------------------------------------
+# ---- geometries only the im2col A tile addresses, against the fp64 reference ------------------------------------------
 def check_new_geometry(B, H, W, Cin, Cout, stride, pad, addend_kind):
     from cfgpp_b200 import _native as nv
     case = make_case(B * 1000 + H * 7 + W + Cin + stride + pad, B, H, W, Cin, Cout, stride, addend_kind)
+    assert nv.conv3x3_schedule(case[5], case[6], stride=stride, pad=pad)["a_mode"] == "im2col"
     out = run(nv, case, stride, pad, False)
-    ref = reference(*case[:5], stride, pad)
-    Ho, Wo = H // stride, W // stride
-    what = f"s{stride} pad {pad} {B}x{H}x{W} {Cin}->{Cout} addend={addend_kind}"
-    assert torch.isfinite(out.float()).all(), what
-    gate(what, out, ref)
-    edge = torch.zeros(B, Ho, Wo, dtype=torch.bool, device=dev)
-    edge[:, 0], edge[:, -1], edge[:, :, 0], edge[:, :, -1] = True, True, True, True
-    gate(what + " edge pixels", out[edge.reshape(-1)], ref[edge.reshape(-1)])
+    gate(f"s{stride} pad {pad} {B}x{H}x{W} {Cin}->{Cout} addend={addend_kind}", out, case, stride, pad)
     return out
 
 

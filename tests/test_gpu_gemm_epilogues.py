@@ -8,12 +8,14 @@
 The statistics are checked against the fp64 sums of the kernel's own fp16 output within the worst-case bound of fp32
 recursive summation, (n − 1)·2⁻²⁴·Σ|x| for n terms (taken as n·2⁻²⁴·Σ|x|). The fold replaces the reference's fp16
 rounding of LayerNorm's output by the rounding of fp16(w·γ), so its error is judged against the exact (fp64)
-LayerNorm → Linear on the same fp16 input, next to the error of the unfused op_layernorm → op_linear path."""
+LayerNorm → Linear on the same fp16 input, next to the error of the unfused op_layernorm → op_linear path. The plain
+fp16 outputs (producer, in place, the chain's to_out, GEGLU) are gated element by element within the accumulation bound
+of `test_gpu_gemm.py`."""
 import numpy as np
 import pytest
 import torch
 
-from test_gpu_kernels import TOL_GEMM, dev, gate, ref_linear, rnd
+from test_gpu_gemm import check_bound, dev, linear_kblocks, rnd
 
 pytestmark = pytest.mark.gpu
 
@@ -113,6 +115,13 @@ def fold_vs_unfused(nv, h, stats, gamma, beta, w, b, geglu, what, ratio, force_b
     return fused, ef, eu
 
 
+def gate_linear(what, out, a, w, bias=None, addend=None, rpg=1, bn=0, geglu=False, force_streamk=False):
+    """op_linear's output gated per element; the launch's schedule decides whether the stream-K term applies."""
+    from cfgpp_b200 import _native as nv
+    sched = nv.linear_schedule(a, w, bias, addend, rpg, geglu=geglu, force_bn=bn, force_streamk=force_streamk)
+    check_bound(what, out, linear_kblocks(a), w, a.shape[0], bias, addend, rpg, sched, geglu)
+
+
 def rel_l2_64(a, ref):
     a, ref = a.double(), ref.double()
     return ((a - ref).norm() / (ref.norm() + 1e-300)).item()
@@ -132,7 +141,7 @@ def test_rowstats_producer(M, mode, bn):
     addend, rpg = addend_for(g, mode, M, N)
     out, stats = nv.op_linear_stats(a, w, bn, bias, addend, rpg)
     what = f"rowstats {M}x{N}x{K} BN{bn} {mode}"
-    gate(what, out, ref_linear(a, w, bias, addend, rpg), TOL_GEMM)
+    gate_linear(what, out, a, w, bias, addend, rpg, bn)
     check_stats(out, stats, bn, what)
     if mode == "none":  # the statistics variant writes what the plain epilogue writes
         assert torch.equal(out, nv.op_linear(a, w, bias, force_bn=bn))
@@ -151,7 +160,7 @@ def test_rowstats_producer_in_place(M, N, K, bn):
     out, stats = nv.op_linear_stats(a, w, bn, bias, tok, out=tok)
     assert out.data_ptr() == tok.data_ptr()
     what = f"rowstats in place {M}x{N}x{K} BN{bn}"
-    gate(what, tok, ref_linear(a, w, bias, tok0, 1), TOL_GEMM)
+    gate_linear(what, tok, a, w, bias, tok0, 1, bn)
     check_stats(tok, stats, bn, what)
     assert torch.equal(tok, oop) and torch.equal(stats, oop_stats)
     tok.copy_(tok0)
@@ -257,7 +266,7 @@ def test_lnfold_chain_as_unet(M, C, Cp, bn):
 
     first = run()
     what = f"chain {M}x{C} Cp{Cp} BN{bn}"
-    gate(what + " to_out", first[0], ref_linear(attn, wo, bo, tok0, 1), TOL_GEMM)
+    gate_linear(what + " to_out", first[0], attn, wo, bo, tok0, 1, bn)
     check_stats(first[0], first[1], bn, what)
     for name, got, w, b, geglu in (("to_qkv", first[2], wqkv, None, False), ("ff.geglu", first[3], wff, bff, True)):
         ref = lnlinear_exact(first[0], gamma, beta, w, b, geglu)
@@ -310,10 +319,9 @@ def test_geglu_shapes(C, M, hb):
     inner = 4 * C
     a, w = rnd(g, M, C), rnd(g, 2 * inner, C, scale=C ** -0.5)
     b = rnd(g, 2 * inner) if hb else None
-    out = nv.op_linear(a, *pack_geglu(w, b), geglu=True)
-    h = ref_linear(a, w, b, None, 1)
-    ref = (h[:, :inner].float() * torch.nn.functional.gelu(h[:, inner:].float()).half().float()).half()
-    gate(f"geglu {M}x{inner}x{C}{' +bias' if hb else ''}", out, ref, TOL_GEMM)
+    wp, bp = pack_geglu(w, b)
+    out = nv.op_linear(a, wp, bp, geglu=True)
+    gate_linear(f"geglu {M}x{inner}x{C}{' +bias' if hb else ''}", out, a, wp, bp, geglu=True)
 
 
 # ---- stream-K -----------------------------------------------------------------------------------------------------
@@ -330,7 +338,7 @@ def test_epilogue_streamk_repeatable(kind, force_streamk):
         a, w, bias, res = rnd(g, M, K), rnd(g, N, K, scale=K ** -0.5), rnd(g, N), rnd(g, M, N)
         run = lambda: nv.op_linear_stats(a, w, bn, bias, res, force_streamk=force_streamk)
         first = run()
-        gate(f"rowstats(stream-K) {M}x{N}x{K}", first[0], ref_linear(a, w, bias, res, 1), TOL_GEMM)
+        gate_linear(f"rowstats(stream-K) {M}x{N}x{K}", first[0], a, w, bias, res, 1, bn, force_streamk=force_streamk)
         check_stats(first[0], first[1], bn, f"rowstats(stream-K) {M}x{N}x{K}")
     elif kind == "geglu":
         C = 640
@@ -338,9 +346,7 @@ def test_epilogue_streamk_repeatable(kind, force_streamk):
         wp, bp = pack_geglu(w, b)
         run = lambda: (nv.op_linear(a, wp, bp, geglu=True, force_streamk=force_streamk),)
         first = run()
-        h = ref_linear(a, w, b, None, 1)
-        ref = (h[:, :4 * C].float() * torch.nn.functional.gelu(h[:, 4 * C:].float()).half().float()).half()
-        gate(f"geglu(stream-K) {M}x{4 * C}x{C}", first[0], ref, TOL_GEMM)
+        gate_linear(f"geglu(stream-K) {M}x{4 * C}x{C}", first[0], a, wp, bp, geglu=True, force_streamk=force_streamk)
     else:
         geglu = kind == "lnfold_geglu"
         C = 640 if geglu else 1280

@@ -19,7 +19,7 @@ from helpers import coef_variants, rel_l2
 pytestmark = pytest.mark.gpu
 dev = torch.device("cuda:0")
 
-TOL_GEMM = 2e-4  # fp32 accumulation vs fp64, both rounded once to fp16: only last-bit flips remain (test_gpu_kernels)
+TOL_GEMM = 2e-4  # fp32 accumulation vs fp64, both rounded once to fp16: only last-bit flips remain
 
 
 def gate(what, got, ref, tol):
