@@ -64,6 +64,60 @@ def stream_ptr() -> c_void_p:
     return c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def dtype_code(t: torch.Tensor) -> int:
+    """The C ABI's dtype code of a tensor: 0 fp16, 1 fp32."""
+    if t.dtype == torch.float16:
+        return 0
+    if t.dtype == torch.float32:
+        return 1
+    raise TypeError(f"unsupported dtype {t.dtype}")
+
+
+class NativeHandle:
+    """Owner of one model handle of the C ABI, whose entry points are cfgpp{_prefix}_create / _load_weight /
+    _finalize_weights / _destroy. `_open` creates it on a CUDA device and streams the weights in; `close` (or garbage
+    collection) destroys it."""
+
+    _prefix = ""
+    _what = ""  # what the handle runs, for the error on a non-CUDA device
+
+    def _entry(self, name: str):
+        return getattr(self.lib, f"cfgpp{self._prefix}_{name}")
+
+    def _open(self, desc: ctypes.Structure, weights, device) -> None:
+        """Create the handle for `desc` on `device`, load the (key, tensor) pairs of `weights` (fp16 or fp32, any
+        device) and finalize."""
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise NativeError(f"the cfgpp_b200 {self._what} runs on CUDA (sm_90a) only; use the oracle for CPU runs")
+        idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        self.device = torch.device("cuda", idx)
+        self.lib = load()
+        self._h = c_void_p()
+        with torch.cuda.device(self.device):
+            check(self._entry("create")(ctypes.byref(desc), c_int(idx), ctypes.byref(self._h)))
+            st = stream_ptr()
+            for key, w in weights:
+                w = w.detach().to(self.device).contiguous()
+                shape = (ctypes.c_int64 * w.dim())(*w.shape)
+                check(self._entry("load_weight")(self._h, key.encode(), ptr(w), shape, c_int(w.dim()),
+                                                 c_int(dtype_code(w)), st))
+                del w
+            torch.cuda.synchronize(self.device)
+            check(self._entry("finalize_weights")(self._h, st))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._entry("destroy")(self._h)
+            self._h = c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # noqa: BLE001
+            pass
+
+
 # ------------------------------------------------------------------------------------------------
 # operator-level wrappers (one kernel launch each) — used by tests and micro-benchmarks
 # ------------------------------------------------------------------------------------------------
@@ -346,11 +400,6 @@ def op_copy_rows(src: torch.Tensor, dst: torch.Tensor, rows: int, col_off: int =
     return dst
 
 
-def _dtype_code(t: torch.Tensor) -> int:
-    assert t.dtype in (torch.float16, torch.float32)
-    return 0 if t.dtype == torch.float16 else 1
-
-
 def op_conv_in(z: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, in_scale: torch.Tensor | None = None,
                reps: int = 1) -> torch.Tensor:
     """conv_in 3x3 pad 1: z [B,4,H,W] fp16 / fp32 NCHW (times the device scalar in_scale, fp32 [1], when given),
@@ -361,7 +410,7 @@ def op_conv_in(z: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, in_scale: t
     assert Cin == 4 and w.shape == (Cout, 36)
     assert in_scale is None or (in_scale.dtype == torch.float32 and in_scale.numel() == 1)
     out = torch.empty((reps * B, H, W, Cout), dtype=torch.float16, device=z.device)
-    check(lib.cfgpp_op_conv_in(ptr(z), c_int(_dtype_code(z)), ptr(in_scale), ptr(w), ptr(bias), ptr(out), c_int(B),
+    check(lib.cfgpp_op_conv_in(ptr(z), c_int(dtype_code(z)), ptr(in_scale), ptr(w), ptr(bias), ptr(out), c_int(B),
                                c_int(H), c_int(W), c_int(Cout), c_int(reps), stream_ptr()))
     return out
 
@@ -384,7 +433,7 @@ def op_conv_out_step(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, metho
     if method != 0:
         assert z is not None and z.shape == (B, 4, H, W) and coef is not None
         z0t = torch.empty_like(z) if want_z0t else None
-        code = _dtype_code(z)
+        code = dtype_code(z)
     if lambdas is not None:
         assert lambdas.dtype == torch.float32 and lambdas.shape == (B,)
     check(lib.cfgpp_op_conv_out_step(ptr(x), ptr(w), ptr(bias), c_int(B), c_int(H), c_int(W), c_int(Cin),
@@ -409,7 +458,7 @@ def op_vae_latent_prep(z: torch.Tensor, scaling: float, w: torch.Tensor, bias: t
     B, C, H, W = z.shape
     assert C == 4 and w.shape == (4, 4)
     out = torch.empty((B, 4, H, W), dtype=torch.float16, device=z.device)
-    check(lib.cfgpp_op_vae_latent_prep(ptr(z), c_int(_dtype_code(z)), c_float(scaling), ptr(w), ptr(bias), ptr(out),
+    check(lib.cfgpp_op_vae_latent_prep(ptr(z), c_int(dtype_code(z)), c_float(scaling), ptr(w), ptr(bias), ptr(out),
                                        c_int(B), c_int(H * W), stream_ptr()))
     return out
 
@@ -441,7 +490,7 @@ def op_vae_image_pad(x: torch.Tensor, out: torch.Tensor | None = None) -> torch.
     if out is None:
         out = torch.empty((B, 4, H, W), dtype=torch.float16, device=x.device)
     assert out.shape == (B, 4, H, W) and out.dtype == torch.float16 and out.is_contiguous()
-    check(lib.cfgpp_op_vae_image_pad(ptr(x), c_int(_dtype_code(x)), ptr(out), c_int(B), c_int(H), c_int(W),
+    check(lib.cfgpp_op_vae_image_pad(ptr(x), c_int(dtype_code(x)), ptr(out), c_int(B), c_int(H), c_int(W),
                                      stream_ptr()))
     return out
 

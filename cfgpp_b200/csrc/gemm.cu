@@ -699,10 +699,19 @@ void finish_op(GemmOp& op, const __half* w, int force_bn, bool force_streamk) {
 }  // namespace
 
 void streamk_alloc(float** ws, unsigned** flags) {
-  CFGPP_CHECK_CUDA(cudaMalloc(ws, static_cast<size_t>(kSkMaxCtas) * BM * 256 * sizeof(float)));
-  CFGPP_CHECK_CUDA(cudaMalloc(flags, 2 * kSkMaxCtas * sizeof(unsigned)));
-  CFGPP_CHECK_CUDA(cudaMemset(*flags, 0, 2 * kSkMaxCtas * sizeof(unsigned)));
-  CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
+  float* w = nullptr;
+  unsigned* f = nullptr;
+  CFGPP_CHECK_CUDA(cudaMalloc(&w, static_cast<size_t>(kSkMaxCtas) * BM * 256 * sizeof(float)));
+  try {
+    CFGPP_CHECK_CUDA(cudaMalloc(&f, 2 * kSkMaxCtas * sizeof(unsigned)));
+    CFGPP_CHECK_CUDA(cudaMemset(f, 0, 2 * kSkMaxCtas * sizeof(unsigned)));
+    CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
+  } catch (...) {
+    streamk_free(w, f);
+    throw;
+  }
+  *ws = w;  // both or neither: the per-device fallback tests ws alone
+  *flags = f;
 }
 void streamk_free(float* ws, unsigned* flags) {
   if (ws) cudaFree(ws);

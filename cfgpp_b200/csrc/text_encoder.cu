@@ -8,7 +8,7 @@ namespace cfgpp {
 
 void gemm_configure();
 
-ClipTextEncoder::ClipTextEncoder(const cfgpp_clip_desc& d, int device) : d_(d), device_(device) {
+ClipTextEncoder::ClipTextEncoder(const cfgpp_clip_desc& d, int device) : d_(d), device_(device), sk_(device) {
   CFGPP_CHECK_CUDA(cudaSetDevice(device));
   CFGPP_REQUIRE(d.vocab_size >= 2 && d.num_layers >= 1 && d.num_layers <= 64, "bad vocab_size / num_layers");
   CFGPP_REQUIRE(d.max_positions >= 1 && d.max_positions <= 128, "max_positions must be 1..128 (CLIP: 77)");
@@ -18,62 +18,12 @@ ClipTextEncoder::ClipTextEncoder(const cfgpp_clip_desc& d, int device) : d_(d), 
   CFGPP_REQUIRE(d.projection_dim >= 0 && d.projection_dim % 8 == 0, "projection_dim must be 0 or a multiple of 8");
   CFGPP_REQUIRE(d.layer_norm_eps > 0.f, "layer_norm_eps must be positive");
   gemm_configure();
-  streamk_alloc(&sk_ws_, &sk_flags_);
-}
-
-ClipTextEncoder::~ClipTextEncoder() {
-  for (auto& kv : raw_) cudaFree(kv.second.p);
-  for (void* p : weight_allocs_) cudaFree(p);
-  for (void* p : act_allocs_) cudaFree(p);
-  streamk_free(sk_ws_, sk_flags_);
 }
 
 void ClipTextEncoder::load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
                                   cudaStream_t stream) {
   CFGPP_REQUIRE(!finalized_, "weights already finalized");
-  CFGPP_REQUIRE(dtype == CFGPP_F16 || dtype == CFGPP_F32, "weight dtype must be fp16 or fp32");
-  Tensor t;
-  t.shape.assign(shape, shape + ndim);
-  const size_t n = t.numel();
-  CFGPP_CHECK_CUDA(cudaMalloc(&t.p, std::max<size_t>(n, 8) * sizeof(__half)));
-  if (dtype == CFGPP_F16) {
-    CFGPP_CHECK_CUDA(cudaMemcpyAsync(t.p, data, n * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
-  } else {
-    run_f32_to_f16(static_cast<const float*>(data), t.p, n, stream);
-  }
-  auto it = raw_.find(key);
-  if (it != raw_.end()) {
-    cudaFree(it->second.p);
-    raw_.erase(it);
-  }
-  raw_[key] = t;
-}
-
-const ClipTextEncoder::Tensor& ClipTextEncoder::raw(const std::string& key) const {
-  auto it = raw_.find(key);
-  if (it == raw_.end()) throw Error(-10, "missing weight: " + key);
-  return it->second;
-}
-
-__half* ClipTextEncoder::plain(const std::string& key, size_t expect_numel) const {
-  const Tensor& t = raw(key);
-  if (t.numel() != expect_numel)
-    throw Error(-11, "weight " + key + " has " + std::to_string(t.numel()) + " elements, expected " +
-                         std::to_string(expect_numel));
-  return t.p;
-}
-
-void* ClipTextEncoder::alloc_bytes(size_t bytes, bool weight) {
-  void* p = nullptr;
-  bytes = (bytes + 255) & ~static_cast<size_t>(255);
-  CFGPP_CHECK_CUDA(cudaMalloc(&p, std::max<size_t>(bytes, 256)));
-  if (weight) {
-    weight_allocs_.push_back(p);
-  } else {
-    act_allocs_.push_back(p);
-    workspace_bytes_ += bytes;
-  }
-  return p;
+  weights_.load(key, data, shape, ndim, dtype, stream);
 }
 
 void ClipTextEncoder::finalize_weights(cudaStream_t stream) {
@@ -83,13 +33,13 @@ void ClipTextEncoder::finalize_weights(cudaStream_t stream) {
   // q | k | v projections of a layer as one [3D][D] operand (one GEMM instead of three)
   for (int l = 0; l < d_.num_layers; ++l) {
     const std::string a = tm + "encoder.layers." + std::to_string(l) + ".self_attn.";
-    __half* w = static_cast<__half*>(alloc_bytes(3 * D * D * sizeof(__half), true));
-    __half* b = static_cast<__half*>(alloc_bytes(3 * D * sizeof(__half), true));
+    __half* w = weights_.alloc(3 * D * D);
+    __half* b = weights_.alloc(3 * D);
     const char* names[3] = {"q_proj", "k_proj", "v_proj"};
     for (int i = 0; i < 3; ++i) {
-      CFGPP_CHECK_CUDA(cudaMemcpyAsync(w + i * D * D, plain(a + names[i] + ".weight", D * D), D * D * sizeof(__half),
+      CFGPP_CHECK_CUDA(cudaMemcpyAsync(w + i * D * D, weights_.plain(a + names[i] + ".weight", D * D), D * D * sizeof(__half),
                                        cudaMemcpyDeviceToDevice, stream));
-      CFGPP_CHECK_CUDA(cudaMemcpyAsync(b + i * D, plain(a + names[i] + ".bias", D), D * sizeof(__half),
+      CFGPP_CHECK_CUDA(cudaMemcpyAsync(b + i * D, weights_.plain(a + names[i] + ".bias", D), D * sizeof(__half),
                                        cudaMemcpyDeviceToDevice, stream));
     }
     qkv_w_.push_back(w);
@@ -111,16 +61,14 @@ void ClipTextEncoder::prepare(int batch, int tokens) {
   CFGPP_REQUIRE(tokens >= 1 && tokens <= d_.max_positions, "token count exceeds max_positions");
   CFGPP_CHECK_CUDA(cudaSetDevice(device_));
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
-  StreamKScope sk_scope(sk_ws_, sk_flags_);
-  for (void* p : act_allocs_) cudaFree(p);
-  act_allocs_.clear();
+  StreamKScope sk_scope(sk_.ws(), sk_.flags());
+  act_.clear();
   layer_plan_.clear();
-  workspace_bytes_ = 0;
   flops_ = 0.0;
   B_ = 0;
   const int D = d_.hidden_size, I = d_.intermediate_size, T = tokens, NB = batch, M = NB * T;
   const size_t sD = D, sI = I;
-  auto act = [&](size_t numel) { return static_cast<__half*>(alloc_bytes(numel * sizeof(__half), false)); };
+  auto act = [&](size_t numel) { return act_.alloc<__half>(numel); };
   x0_ = act(M * sD);
   x1_ = act(M * sD);
   ln_ = act(M * sD);
@@ -130,11 +78,11 @@ void ClipTextEncoder::prepare(int batch, int tokens) {
   last_ = act(M * sD);
   pool_ = act(16 * sD);
   const std::string tm = "text_model.";
-  plain(tm + "embeddings.token_embedding.weight", static_cast<size_t>(d_.vocab_size) * sD);
-  plain(tm + "embeddings.position_embedding.weight", static_cast<size_t>(d_.max_positions) * sD);
-  plain(tm + "final_layer_norm.weight", sD);
-  plain(tm + "final_layer_norm.bias", sD);
-  if (d_.projection_dim > 0) plain("text_projection.weight", static_cast<size_t>(d_.projection_dim) * sD);
+  weights_.plain(tm + "embeddings.token_embedding.weight", static_cast<size_t>(d_.vocab_size) * sD);
+  weights_.plain(tm + "embeddings.position_embedding.weight", static_cast<size_t>(d_.max_positions) * sD);
+  weights_.plain(tm + "final_layer_norm.weight", sD);
+  weights_.plain(tm + "final_layer_norm.bias", sD);
+  if (d_.projection_dim > 0) weights_.plain("text_projection.weight", static_cast<size_t>(d_.projection_dim) * sD);
   const float eps = d_.layer_norm_eps;
   const int heads = d_.num_heads, act_mode = d_.hidden_act;
   __half *x0 = x0_, *x1 = x1_, *ln = ln_, *qkv = qkv_, *att = att_, *mlp = mlp_;
@@ -145,22 +93,22 @@ void ClipTextEncoder::prepare(int batch, int tokens) {
       flops_ += op.flops();
       steps.push_back([op](cudaStream_t st) { run_gemm_op(op, st); });
     };
-    const __half *g1 = plain(p + "layer_norm1.weight", sD), *b1 = plain(p + "layer_norm1.bias", sD);
-    const __half *g2 = plain(p + "layer_norm2.weight", sD), *b2 = plain(p + "layer_norm2.bias", sD);
+    const __half *g1 = weights_.plain(p + "layer_norm1.weight", sD), *b1 = weights_.plain(p + "layer_norm1.bias", sD);
+    const __half *g2 = weights_.plain(p + "layer_norm2.weight", sD), *b2 = weights_.plain(p + "layer_norm2.bias", sD);
     // x1 = x0 + out_proj(attention(q, k, v of LN1(x0)))
     steps.push_back([=](cudaStream_t st) { run_layernorm(x0, M, D, g1, b1, eps, ln, st); });
     add_gemm(make_linear_op(ln, D, nullptr, 0, 0, qkv_w_[l], M, 3 * D, D, qkv_b_[l], nullptr, 0, 1, qkv, 3 * D, false));
     steps.push_back([=](cudaStream_t st) { run_clip_attention(qkv, att, NB, T, heads, D, st); });
     flops_ += 2.0 * NB * heads * static_cast<double>(T) * T * 64.0;  // causal: half of 2 * (QK^T + PV)
-    add_gemm(make_linear_op(att, D, nullptr, 0, 0, plain(p + "self_attn.out_proj.weight", sD * sD), M, D, D,
-                            plain(p + "self_attn.out_proj.bias", sD), x0, D, 1, x1, D, false));
+    add_gemm(make_linear_op(att, D, nullptr, 0, 0, weights_.plain(p + "self_attn.out_proj.weight", sD * sD), M, D, D,
+                            weights_.plain(p + "self_attn.out_proj.bias", sD), x0, D, 1, x1, D, false));
     // x0 = x1 + fc2(act(fc1(LN2(x1))))
     steps.push_back([=](cudaStream_t st) { run_layernorm(x1, M, D, g2, b2, eps, ln, st); });
-    add_gemm(make_linear_op(ln, D, nullptr, 0, 0, plain(p + "mlp.fc1.weight", sI * sD), M, I, D,
-                            plain(p + "mlp.fc1.bias", sI), nullptr, 0, 1, mlp, I, false));
+    add_gemm(make_linear_op(ln, D, nullptr, 0, 0, weights_.plain(p + "mlp.fc1.weight", sI * sD), M, I, D,
+                            weights_.plain(p + "mlp.fc1.bias", sI), nullptr, 0, 1, mlp, I, false));
     steps.push_back([=](cudaStream_t st) { run_clip_activation(mlp, static_cast<size_t>(M) * I, act_mode, st); });
-    add_gemm(make_linear_op(mlp, I, nullptr, 0, 0, plain(p + "mlp.fc2.weight", sD * sI), M, D, I,
-                            plain(p + "mlp.fc2.bias", sD), x1, D, 1, x0, D, false));
+    add_gemm(make_linear_op(mlp, I, nullptr, 0, 0, weights_.plain(p + "mlp.fc2.weight", sD * sI), M, D, I,
+                            weights_.plain(p + "mlp.fc2.bias", sD), x1, D, 1, x0, D, false));
     layer_plan_.push_back(std::move(steps));
   }
   B_ = NB;
@@ -176,7 +124,7 @@ void ClipTextEncoder::encode(const int* ids, const int* pooled_index, int batch,
   if (batch != B_ || tokens != T_) prepare(batch, tokens);
   const int D = d_.hidden_size, M = batch * tokens;
   const std::string tm = "text_model.";
-  run_clip_embed(ids, raw(tm + "embeddings.token_embedding.weight").p, raw(tm + "embeddings.position_embedding.weight").p,
+  run_clip_embed(ids, weights_.plain(tm + "embeddings.token_embedding.weight"), weights_.plain(tm + "embeddings.position_embedding.weight"),
                  x0_, M, tokens, D, d_.vocab_size, stream);
   const bool need_last = last_out != nullptr || pooled_out != nullptr;
   const int wanted = d_.num_layers - skip;  // index into hidden_states
@@ -191,12 +139,12 @@ void ClipTextEncoder::encode(const int* ids, const int* pooled_index, int batch,
   }
   if (!need_last) return;
   __half* last = last_out ? last_out : last_;
-  run_layernorm(x0_, M, D, raw(tm + "final_layer_norm.weight").p, raw(tm + "final_layer_norm.bias").p, d_.layer_norm_eps,
+  run_layernorm(x0_, M, D, weights_.plain(tm + "final_layer_norm.weight"), weights_.plain(tm + "final_layer_norm.bias"), d_.layer_norm_eps,
                 last, stream);
   if (pooled_out) {
     if (d_.projection_dim > 0) {
       run_clip_gather_rows(last, pooled_index, pool_, batch, tokens, D, stream);
-      run_small_linear(pool_, D, raw("text_projection.weight").p, nullptr, nullptr, 0, pooled_out, d_.projection_dim,
+      run_small_linear(pool_, D, weights_.plain("text_projection.weight"), nullptr, nullptr, 0, pooled_out, d_.projection_dim,
                        nullptr, batch, d_.projection_dim, D, false, stream);
     } else {
       run_clip_gather_rows(last, pooled_index, pooled_out, batch, tokens, D, stream);

@@ -13,12 +13,12 @@
 #include <vector>
 
 #include "../../include/cfgpp_b200.h"
+#include "executor.cuh"
 #include "gemm.cuh"
 #include "ops.cuh"
 
 namespace cfgpp {
 
-void run_f32_to_f16(const float* in, __half* out, size_t n, cudaStream_t stream);
 // text_kernels.cu
 void run_clip_embed(const int* ids, const __half* tok, const __half* pos, __half* out, int M, int T, int D, int vocab,
                     cudaStream_t stream);
@@ -29,7 +29,6 @@ void run_clip_gather_rows(const __half* x, const int* index, __half* out, int B,
 class ClipTextEncoder {
  public:
   ClipTextEncoder(const cfgpp_clip_desc& d, int device);
-  ~ClipTextEncoder();
   void load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
                    cudaStream_t stream);
   void finalize_weights(cudaStream_t stream);
@@ -39,30 +38,18 @@ class ClipTextEncoder {
   void encode(const int* ids, const int* pooled_index, int batch, int tokens, int skip, __half* hidden_out,
               __half* last_out, __half* pooled_out, cudaStream_t stream);
   double flops() const { return flops_; }
-  size_t workspace_bytes() const { return workspace_bytes_; }
+  size_t workspace_bytes() const { return act_.bytes(); }
 
  private:
-  struct Tensor {
-    __half* p = nullptr;
-    std::vector<int64_t> shape;
-    size_t numel() const {
-      size_t n = 1;
-      for (auto d : shape) n *= static_cast<size_t>(d);
-      return n;
-    }
-  };
-  const Tensor& raw(const std::string& key) const;
-  __half* plain(const std::string& key, size_t expect_numel) const;
-  void* alloc_bytes(size_t bytes, bool weight);
   void prepare(int batch, int tokens);
 
   cfgpp_clip_desc d_;
   int device_;
   bool finalized_ = false;
-  std::map<std::string, Tensor> raw_;
+  WeightStore weights_;
+  DeviceArena act_;  // workspace of the prepared plan
+  StreamKWorkspace sk_;
   std::vector<__half*> qkv_w_, qkv_b_;  // per layer: [3D][D], [3D]
-  std::vector<void*> weight_allocs_, act_allocs_;
-  size_t workspace_bytes_ = 0;
   double flops_ = 0.0;
   int B_ = 0, T_ = 0;
   using Step = std::function<void(cudaStream_t)>;
@@ -70,8 +57,6 @@ class ClipTextEncoder {
   const int* ids_in_ = nullptr;                 // set per encode() call
   __half *x0_ = nullptr, *x1_ = nullptr, *ln_ = nullptr, *qkv_ = nullptr, *att_ = nullptr, *mlp_ = nullptr;
   __half *last_ = nullptr, *pool_ = nullptr;
-  float* sk_ws_ = nullptr;
-  unsigned* sk_flags_ = nullptr;
 };
 
 }  // namespace cfgpp

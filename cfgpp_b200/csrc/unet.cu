@@ -11,25 +11,6 @@ namespace cfgpp {
 
 namespace {
 
-__global__ void f32_to_f16_kernel(const float* __restrict__ in, __half* __restrict__ out, size_t n) {
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x)
-    out[i] = __float2half_rn(in[i]);
-}
-
-// (Cout, Cin, 3, 3) -> [Cout][tap][Cin]
-__global__ void pack_conv3x3_kernel(const __half* __restrict__ in, __half* __restrict__ out, int Cout, int Cin) {
-  const size_t n = static_cast<size_t>(Cout) * Cin * 9;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int ci = i % Cin;
-    const size_t t = i / Cin;
-    const int tap = t % 9;
-    const int co = t / 9;
-    out[i] = in[(static_cast<size_t>(co) * Cin + ci) * 9 + tap];
-  }
-}
-
 // GEGLU proj rows (2*inner, K): per 128 rows interleave value / gate halves into 256-row tiles
 __global__ void pack_geglu_kernel(const __half* __restrict__ in, __half* __restrict__ out, int inner, int K) {
   const size_t n = static_cast<size_t>(2) * inner * K;
@@ -73,24 +54,12 @@ __global__ void pack_heads_cols_kernel(const __half* __restrict__ in, __half* __
   }
 }
 
-int grid_for(size_t n) { return static_cast<int>(std::min<size_t>((n + 255) / 256, num_sms() * 8)); }
-
 }  // namespace
 
 void gemm_configure();
 void attn_configure();
 
-// shared with vae.cu (weight ingestion helpers)
-void run_f32_to_f16(const float* in, __half* out, size_t n, cudaStream_t stream) {
-  f32_to_f16_kernel<<<grid_for(n), 256, 0, stream>>>(in, out, n);
-  CFGPP_CHECK_CUDA(cudaGetLastError());
-}
-void run_pack_conv3x3(const __half* in, __half* out, int Cout, int Cin, cudaStream_t stream) {
-  pack_conv3x3_kernel<<<grid_for(static_cast<size_t>(Cout) * Cin * 9), 256, 0, stream>>>(in, out, Cout, Cin);
-  CFGPP_CHECK_CUDA(cudaGetLastError());
-}
-
-Unet::Unet(const cfgpp_model_desc& d, int device) : d_(d), device_(device) {
+Unet::Unet(const cfgpp_model_desc& d, int device) : d_(d), device_(device), sk_(device) {
   CFGPP_CHECK_CUDA(cudaSetDevice(device));
   CFGPP_REQUIRE(d.num_levels >= 2 && d.num_levels <= CFGPP_MAX_LEVELS, "num_levels must be 2..4");
   CFGPP_REQUIRE(d.norm_num_groups == 32, "only GroupNorm(32) is implemented");
@@ -99,7 +68,6 @@ Unet::Unet(const cfgpp_model_desc& d, int device) : d_(d), device_(device) {
   has_aug_ = d.addition_time_embed_dim > 0;
   gemm_configure();
   attn_configure();
-  streamk_alloc(&sk_ws_, &sk_flags_);
   CFGPP_CHECK_CUDA(cudaStreamCreateWithFlags(&capture_stream_, cudaStreamNonBlocking));
 }
 
@@ -107,11 +75,7 @@ Unet::~Unet() {
   if (graph_exec_) cudaGraphExecDestroy(graph_exec_);
   if (graph_) cudaGraphDestroy(graph_);
   if (capture_stream_) cudaStreamDestroy(capture_stream_);
-  for (auto& kv : raw_) cudaFree(kv.second.p);
-  for (void* p : weight_allocs_) cudaFree(p);
-  for (void* p : act_allocs_) cudaFree(p);
   if (noise_buf_) cudaFree(noise_buf_);
-  streamk_free(sk_ws_, sk_flags_);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -120,51 +84,7 @@ Unet::~Unet() {
 void Unet::load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
                        cudaStream_t stream) {
   CFGPP_REQUIRE(!finalized_, "weights already finalized");
-  CFGPP_REQUIRE(dtype == CFGPP_F16 || dtype == CFGPP_F32, "weight dtype must be fp16 or fp32");
-  DevTensor t;
-  t.shape.assign(shape, shape + ndim);
-  const size_t n = t.numel();
-  CFGPP_CHECK_CUDA(cudaMalloc(&t.p, std::max<size_t>(n, 8) * sizeof(__half)));
-  if (dtype == CFGPP_F16) {
-    CFGPP_CHECK_CUDA(cudaMemcpyAsync(t.p, data, n * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
-  } else {
-    f32_to_f16_kernel<<<grid_for(n), 256, 0, stream>>>(static_cast<const float*>(data), t.p, n);
-    CFGPP_CHECK_CUDA(cudaGetLastError());
-  }
-  auto it = raw_.find(key);
-  if (it != raw_.end()) {
-    cudaFree(it->second.p);
-    raw_.erase(it);
-  }
-  raw_[key] = t;
-}
-
-const DevTensor& Unet::raw(const std::string& key) const {
-  auto it = raw_.find(key);
-  if (it == raw_.end()) throw Error(-10, "missing weight: " + key);
-  return it->second;
-}
-
-__half* Unet::alloc_weight(size_t numel) {
-  void* p = nullptr;
-  CFGPP_CHECK_CUDA(cudaMalloc(&p, std::max<size_t>(numel, 8) * sizeof(__half)));
-  weight_allocs_.push_back(p);
-  return static_cast<__half*>(p);
-}
-
-__half* Unet::plain(const std::string& key) { return raw(key).p; }
-
-__half* Unet::packed_conv3x3(const std::string& key) {
-  auto it = packed_cache_.find(key);
-  if (it != packed_cache_.end()) return it->second;
-  const DevTensor& t = raw(key);
-  CFGPP_REQUIRE(t.shape.size() == 4 && t.shape[2] == 3 && t.shape[3] == 3, "expected (Cout,Cin,3,3): " + key);
-  const int Cout = static_cast<int>(t.shape[0]), Cin = static_cast<int>(t.shape[1]);
-  __half* out = alloc_weight(t.numel());
-  pack_conv3x3_kernel<<<grid_for(t.numel()), 256>>>(t.p, out, Cout, Cin);
-  CFGPP_CHECK_CUDA(cudaGetLastError());
-  packed_cache_[key] = out;
-  return out;
+  weights_.load(key, data, shape, ndim, dtype, stream);
 }
 
 __half* Unet::packed_cat_rows(const std::vector<std::string>& keys) {
@@ -173,12 +93,12 @@ __half* Unet::packed_cat_rows(const std::vector<std::string>& keys) {
   auto it = packed_cache_.find(name);
   if (it != packed_cache_.end()) return it->second;
   size_t total = 0;
-  for (auto& k : keys) total += raw(k).numel();
-  __half* out = alloc_weight(total);
+  for (auto& k : keys) total += weights_.raw(k).numel();
+  __half* out = weights_.alloc(total);
   size_t off = 0;
   for (auto& k : keys) {
-    const DevTensor& t = raw(k);
-    CFGPP_CHECK_CUDA(cudaMemcpy(out + off, t.p, t.numel() * sizeof(__half), cudaMemcpyDeviceToDevice));
+    const WeightStore::Weight& t = weights_.raw(k);
+    CFGPP_CHECK_CUDA(cudaMemcpy(out + off, t.p(), t.numel() * sizeof(__half), cudaMemcpyDeviceToDevice));
     off += t.numel();
   }
   packed_cache_[name] = out;
@@ -188,35 +108,35 @@ __half* Unet::packed_cat_rows(const std::vector<std::string>& keys) {
 __half* Unet::packed_geglu(const std::string& key, bool is_bias) {
   auto it = packed_cache_.find("geglu:" + key);
   if (it != packed_cache_.end()) return it->second;
-  const DevTensor& t = raw(key);
+  const WeightStore::Weight& t = weights_.raw(key);
   const int rows = static_cast<int>(t.shape[0]);
   const int K = is_bias ? 1 : static_cast<int>(t.shape[1]);
   CFGPP_REQUIRE(rows % 256 == 0, "GEGLU width must be a multiple of 256: " + key);
-  __half* out = alloc_weight(t.numel());
-  pack_geglu_kernel<<<grid_for(t.numel()), 256>>>(t.p, out, rows / 2, K);
+  __half* out = weights_.alloc(t.numel());
+  pack_geglu_kernel<<<grid_for(t.numel()), 256>>>(t.p(), out, rows / 2, K);
   CFGPP_CHECK_CUDA(cudaGetLastError());
   packed_cache_["geglu:" + key] = out;
   return out;
 }
 
 __half* Unet::packed_heads_rows(const std::vector<std::string>& keys, int heads, int hd, int hdp) {
-  if (hd == hdp) return keys.size() == 1 ? plain(keys[0]) : packed_cat_rows(keys);
+  if (hd == hdp) return keys.size() == 1 ? weights_.plain(keys[0]) : packed_cat_rows(keys);
   std::string name = "heads_rows:";
   for (auto& k : keys) name += k + "|";
   auto it = packed_cache_.find(name);
   if (it != packed_cache_.end()) return it->second;
-  const int K = static_cast<int>(raw(keys[0]).shape[1]);
+  const int K = static_cast<int>(weights_.raw(keys[0]).shape[1]);
   std::vector<const __half*> ptrs;
   for (auto& k : keys) {
-    const DevTensor& t = raw(k);
+    const WeightStore::Weight& t = weights_.raw(k);
     CFGPP_REQUIRE(t.shape.size() >= 2 && t.shape[0] == heads * hd && t.shape[1] == K, "unexpected projection shape: " + k);
-    ptrs.push_back(t.p);
+    ptrs.push_back(t.p());
   }
   const __half** dptrs = nullptr;
   CFGPP_CHECK_CUDA(cudaMalloc(&dptrs, ptrs.size() * sizeof(__half*)));
   CFGPP_CHECK_CUDA(cudaMemcpy(dptrs, ptrs.data(), ptrs.size() * sizeof(__half*), cudaMemcpyHostToDevice));
   const size_t total = keys.size() * static_cast<size_t>(heads) * hdp * K;
-  __half* out = alloc_weight(total);
+  __half* out = weights_.alloc(total);
   pack_heads_rows_kernel<<<grid_for(total), 256>>>(dptrs, out, static_cast<int>(keys.size()), heads, hd, hdp, K);
   CFGPP_CHECK_CUDA(cudaGetLastError());
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
@@ -226,15 +146,15 @@ __half* Unet::packed_heads_rows(const std::vector<std::string>& keys, int heads,
 }
 
 __half* Unet::packed_heads_cols(const std::string& key, int heads, int hd, int hdp) {
-  if (hd == hdp) return plain(key);
+  if (hd == hdp) return weights_.plain(key);
   auto it = packed_cache_.find("heads_cols:" + key);
   if (it != packed_cache_.end()) return it->second;
-  const DevTensor& t = raw(key);
+  const WeightStore::Weight& t = weights_.raw(key);
   const int N = static_cast<int>(t.shape[0]);
   CFGPP_REQUIRE(t.shape[1] == heads * hd, "unexpected to_out shape: " + key);
   const size_t total = static_cast<size_t>(N) * heads * hdp;
-  __half* out = alloc_weight(total);
-  pack_heads_cols_kernel<<<grid_for(total), 256>>>(t.p, out, N, heads, hd, hdp);
+  __half* out = weights_.alloc(total);
+  pack_heads_cols_kernel<<<grid_for(total), 256>>>(t.p(), out, N, heads, hd, hdp);
   CFGPP_CHECK_CUDA(cudaGetLastError());
   packed_cache_["heads_cols:" + key] = out;
   return out;
@@ -245,18 +165,18 @@ Unet::FoldedLN Unet::folded_ln(const std::string& cache_key, const __half* w_pac
   auto it = fold_cache_.find(cache_key);
   if (it != fold_cache_.end()) return it->second;
   FoldedLN f;
-  f.w = alloc_weight(static_cast<size_t>(N) * K);
-  f.s = reinterpret_cast<float*>(alloc_weight(static_cast<size_t>(N) * 2));
-  f.t = reinterpret_cast<float*>(alloc_weight(static_cast<size_t>(N) * 2));
-  run_fold_ln(w_packed, plain(norm_prefix + ".weight"), plain(norm_prefix + ".bias"), bias_packed, f.w, f.s, f.t, N, K,
-              nullptr);
+  f.w = weights_.alloc(static_cast<size_t>(N) * K);
+  f.s = weights_.alloc<float>(N);
+  f.t = weights_.alloc<float>(N);
+  run_fold_ln(w_packed, weights_.plain(norm_prefix + ".weight"), weights_.plain(norm_prefix + ".bias"), bias_packed,
+              f.w, f.s, f.t, N, K, nullptr);
   fold_cache_[cache_key] = f;
   return f;
 }
 
 void Unet::finalize_weights(cudaStream_t stream) {
   CFGPP_CHECK_CUDA(cudaStreamSynchronize(stream));
-  // structural validation: every key the plan will touch must exist (dry walk at a nominal size)
+  // structural validation: building a plan at a nominal size reads (and packs) every weight the plan touches
   finalized_ = true;
   try {
     // the smallest latent for which every level keeps a spatial extent (H, W >= 1 at the deepest level)
@@ -272,17 +192,6 @@ void Unet::finalize_weights(cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------------------------
 // workspace
 // ------------------------------------------------------------------------------------------------------------
-void* Unet::alloc_bytes(size_t bytes) {
-  void* p = nullptr;
-  bytes = (bytes + 255) & ~static_cast<size_t>(255);
-  CFGPP_CHECK_CUDA(cudaMalloc(&p, std::max<size_t>(bytes, 256)));
-  act_allocs_.push_back(p);
-  workspace_bytes_ += bytes;
-  return p;
-}
-
-__half* Unet::alloc_act(size_t numel) { return static_cast<__half*>(alloc_bytes(numel * sizeof(__half))); }
-
 Unet::Scratch* Unet::scratch(const std::string& name, size_t numel_half) {
   auto& s = scratch_[name];
   if (!s) s.reset(new Scratch());
@@ -298,12 +207,8 @@ Unet::Scratch* Unet::scratch(const std::string& name, size_t numel_half) {
 // plan building. The structure is walked twice by prepare(): a sizing pass (scratch buffers unallocated: only
 // sizes are recorded, no ops are created) and the real pass.
 // ------------------------------------------------------------------------------------------------------------
-namespace {
-bool g_dry = false;
-}
-
 void Unet::add_step(const std::string& name, std::function<void(cudaStream_t)> fn, int launches) {
-  if (g_dry) return;
+  if (sizing_) return;
   PlanStep s;
   s.name = name;
   s.fn = std::move(fn);
@@ -336,20 +241,11 @@ Unet::Act Unet::build_resnet(const std::string& prefix, Act x1, const Act* x2, i
   Scratch* s_norm = scratch("norm", M * std::max(Cin, Cout));
   Scratch* s_h1 = scratch("h1", M * Cout);
   Scratch* s_sc = (Cin != Cout) ? scratch("shortcut", M * Cout) : nullptr;
-  __half* out = g_dry ? nullptr : alloc_act(M * Cout);
-  if (g_dry) {
-    // validate keys
-    raw(prefix + ".norm1.weight"); raw(prefix + ".norm1.bias"); raw(prefix + ".conv1.weight");
-    raw(prefix + ".conv1.bias"); raw(prefix + ".time_emb_proj.weight"); raw(prefix + ".time_emb_proj.bias");
-    raw(prefix + ".norm2.weight"); raw(prefix + ".norm2.bias"); raw(prefix + ".conv2.weight");
-    raw(prefix + ".conv2.bias");
-    if (Cin != Cout) { raw(prefix + ".conv_shortcut.weight"); raw(prefix + ".conv_shortcut.bias"); }
-    workspace_bytes_ += M * Cout * sizeof(__half);
-    return Act{nullptr, Cout};
-  }
+  if (sizing_) return Act{nullptr, Cout};
+  __half* out = alloc_act(M * Cout);
   const __half* x2p = x2 ? x2->p : nullptr;
-  const __half *g1 = plain(prefix + ".norm1.weight"), *b1 = plain(prefix + ".norm1.bias");
-  const __half *g2 = plain(prefix + ".norm2.weight"), *b2 = plain(prefix + ".norm2.bias");
+  const __half *g1 = weights_.plain(prefix + ".norm1.weight"), *b1 = weights_.plain(prefix + ".norm1.bias");
+  const __half *g2 = weights_.plain(prefix + ".norm2.weight"), *b2 = weights_.plain(prefix + ".norm2.bias");
   const float eps = d_.norm_eps;
   float* partial = gn_partial_;
   const int NB = NB_;
@@ -359,20 +255,20 @@ Unet::Act Unet::build_resnet(const std::string& prefix, Act x1, const Act* x2, i
   add_step(prefix + ".norm1+silu", [=](cudaStream_t st) {
     run_groupnorm(x1p, C1, x2p, C2, NB, HW, g1, b1, eps, true, partial, normp, st);
   }, 2);
-  add_gemm(prefix + ".conv1", make_conv3x3_op(normp, NB_, H, W, Cin, packed_conv3x3(prefix + ".conv1.weight"), Cout,
-                                              plain(prefix + ".conv1.bias"), temb_all_ + temb_off, temb_total_, HW, h1p));
+  add_gemm(prefix + ".conv1", make_conv3x3_op(normp, NB_, H, W, Cin, weights_.packed_conv3x3(prefix + ".conv1.weight"), Cout,
+                                              weights_.plain(prefix + ".conv1.bias"), temb_all_ + temb_off, temb_total_, HW, h1p));
   add_step(prefix + ".norm2+silu", [=](cudaStream_t st) {
     run_groupnorm(h1p, Cout, nullptr, 0, NB, HW, g2, b2, eps, true, partial, normp, st);
   }, 2);
   const __half* residual = x1p;
   if (Cin != Cout) {
     add_gemm(prefix + ".conv_shortcut",
-             make_linear_op(x1p, C1, x2p, C2, C1, plain(prefix + ".conv_shortcut.weight"), static_cast<int>(M), Cout,
-                            Cin, plain(prefix + ".conv_shortcut.bias"), nullptr, 0, 1, s_sc->p, Cout, false));
+             make_linear_op(x1p, C1, x2p, C2, C1, weights_.plain(prefix + ".conv_shortcut.weight"), static_cast<int>(M), Cout,
+                            Cin, weights_.plain(prefix + ".conv_shortcut.bias"), nullptr, 0, 1, s_sc->p, Cout, false));
     residual = s_sc->p;
   }
-  add_gemm(prefix + ".conv2", make_conv3x3_op(normp, NB_, H, W, Cout, packed_conv3x3(prefix + ".conv2.weight"), Cout,
-                                              plain(prefix + ".conv2.bias"), residual, Cout, 1, out));
+  add_gemm(prefix + ".conv2", make_conv3x3_op(normp, NB_, H, W, Cout, weights_.packed_conv3x3(prefix + ".conv2.weight"), Cout,
+                                              weights_.plain(prefix + ".conv2.bias"), residual, Cout, 1, out));
   return Act{out, Cout};
 }
 
@@ -396,25 +292,9 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
   Scratch* s_stats[3];
   for (int i = 0; i < 3; ++i)  // [16 N blocks][M] float2 partial row statistics (LayerNorm fold)
     s_stats[i] = scratch("lnstats" + std::to_string(i), static_cast<size_t>(32) * M * 2 * 2);
-  __half* out = g_dry ? nullptr : alloc_act(M * C);
+  if (sizing_) return Act{nullptr, C};
+  __half* out = alloc_act(M * C);
   const int Mkv = NB_ * n_ctx_;
-  if (g_dry) {
-    raw(prefix + ".norm.weight"); raw(prefix + ".norm.bias"); raw(prefix + ".proj_in.weight");
-    raw(prefix + ".proj_in.bias"); raw(prefix + ".proj_out.weight"); raw(prefix + ".proj_out.bias");
-    for (int k = 0; k < layers; ++k) {
-      const std::string b = prefix + ".transformer_blocks." + std::to_string(k);
-      for (const char* n : {".norm1.weight", ".norm1.bias", ".norm2.weight", ".norm2.bias", ".norm3.weight",
-                            ".norm3.bias", ".attn1.to_q.weight", ".attn1.to_k.weight", ".attn1.to_v.weight",
-                            ".attn1.to_out.0.weight", ".attn1.to_out.0.bias", ".attn2.to_q.weight",
-                            ".attn2.to_k.weight", ".attn2.to_v.weight", ".attn2.to_out.0.weight",
-                            ".attn2.to_out.0.bias", ".ff.net.0.proj.weight", ".ff.net.0.proj.bias",
-                            ".ff.net.2.weight", ".ff.net.2.bias"})
-        raw(b + n);
-      workspace_bytes_ += static_cast<size_t>(Mkv) * 2 * Cp * sizeof(__half);
-    }
-    workspace_bytes_ += M * C * sizeof(__half);
-    return Act{nullptr, C};
-  }
   const int NB = NB_;
   float* partial = gn_partial_;
   __half *normp = s_norm->p, *tok = s_tok->p, *qkv = s_qkv->p, *attn = s_attn->p, *qb = s_q->p, *ff = s_ff->p;
@@ -449,15 +329,15 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
     return op;
   };
   {
-    const __half *g = plain(prefix + ".norm.weight"), *b = plain(prefix + ".norm.bias");
+    const __half *g = weights_.plain(prefix + ".norm.weight"), *b = weights_.plain(prefix + ".norm.bias");
     const __half* xp = x.p;
     add_step(prefix + ".norm", [=](cudaStream_t st) {
       run_groupnorm(xp, C, nullptr, 0, NB, HW, g, b, 1e-6f, false, partial, normp, st);
     }, 2);
   }
   add_gemm(prefix + ".proj_in", producer([&](int bn) {
-             return make_linear_op(normp, C, nullptr, 0, 0, plain(prefix + ".proj_in.weight"), Mi, C, C,
-                                   plain(prefix + ".proj_in.bias"), nullptr, 0, 1, tok, C, false, bn);
+             return make_linear_op(normp, C, nullptr, 0, 0, weights_.plain(prefix + ".proj_in.weight"), Mi, C, C,
+                                   weights_.plain(prefix + ".proj_in.bias"), nullptr, 0, 1, tok, C, false, bn);
            }, 0));
   for (int k = 0; k < layers; ++k) {
     const std::string b = prefix + ".transformer_blocks." + std::to_string(k);
@@ -474,7 +354,7 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
     add_gemm(b + ".attn1.to_out", producer([&](int bn) {
                return make_linear_op(attn, Cp, nullptr, 0, 0,
                                      packed_heads_cols(b + ".attn1.to_out.0.weight", heads, hd, hdp), Mi, C, Cp,
-                                     plain(b + ".attn1.to_out.0.bias"), tok, C, 1, tok, C, false, bn);
+                                     weights_.plain(b + ".attn1.to_out.0.bias"), tok, C, 1, tok, C, false, bn);
              }, 1),
              2.0 * Mi * static_cast<double>(C) * C);
     // --- cross-attention (K/V projected once per prompt by the prompt plan) ---
@@ -497,7 +377,7 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
     add_gemm(b + ".attn2.to_out", producer([&](int bn) {
                return make_linear_op(attn, Cp, nullptr, 0, 0,
                                      packed_heads_cols(b + ".attn2.to_out.0.weight", heads, hd, hdp), Mi, C, Cp,
-                                     plain(b + ".attn2.to_out.0.bias"), tok, C, 1, tok, C, false, bn);
+                                     weights_.plain(b + ".attn2.to_out.0.bias"), tok, C, 1, tok, C, false, bn);
              }, 2),
              2.0 * Mi * static_cast<double>(C) * C);
     // --- GEGLU feed-forward ---
@@ -507,12 +387,12 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
     add_gemm(b + ".ff.geglu(+norm3)",
              consumer(make_linear_op(tok, C, nullptr, 0, 0, f3.w, Mi, 8 * C, C, nullptr, nullptr, 0, 1, ff, 4 * C, true), f3, 2));
     add_gemm(b + ".ff.out", producer([&](int bn) {
-               return make_linear_op(ff, 4 * C, nullptr, 0, 0, plain(b + ".ff.net.2.weight"), Mi, C, 4 * C,
-                                     plain(b + ".ff.net.2.bias"), tok, C, 1, tok, C, false, bn);
+               return make_linear_op(ff, 4 * C, nullptr, 0, 0, weights_.plain(b + ".ff.net.2.weight"), Mi, C, 4 * C,
+                                     weights_.plain(b + ".ff.net.2.bias"), tok, C, 1, tok, C, false, bn);
              }, 0));
   }
-  add_gemm(prefix + ".proj_out", make_linear_op(tok, C, nullptr, 0, 0, plain(prefix + ".proj_out.weight"), Mi, C, C,
-                                                plain(prefix + ".proj_out.bias"), x.p, C, 1, out, C, false));
+  add_gemm(prefix + ".proj_out", make_linear_op(tok, C, nullptr, 0, 0, weights_.plain(prefix + ".proj_out.weight"), Mi, C, C,
+                                                weights_.plain(prefix + ".proj_out.bias"), x.p, C, 1, out, C, false));
   return Act{out, C};
 }
 
@@ -520,15 +400,11 @@ Unet::Act Unet::build_downsample(const std::string& prefix, Act x, int H, int W)
   const int C = x.C;
   const int Ho = H / 2, Wo = W / 2;
   const size_t Mo = static_cast<size_t>(NB_) * Ho * Wo;
-  __half* out = g_dry ? nullptr : alloc_act(Mo * C);
-  if (g_dry) {
-    raw(prefix + ".conv.weight"); raw(prefix + ".conv.bias");
-    workspace_bytes_ += Mo * C * sizeof(__half);
-    return Act{nullptr, C};
-  }
+  if (sizing_) return Act{nullptr, C};
+  __half* out = alloc_act(Mo * C);
   // stride-2 conv as an implicit GEMM: the A tile of every tap comes through a tensor map with element strides 2
-  add_gemm(prefix + ".conv", make_conv3x3_op(x.p, NB_, H, W, C, packed_conv3x3(prefix + ".conv.weight"), C,
-                                             plain(prefix + ".conv.bias"), nullptr, 0, 1, out, 0, 2));
+  add_gemm(prefix + ".conv", make_conv3x3_op(x.p, NB_, H, W, C, weights_.packed_conv3x3(prefix + ".conv.weight"), C,
+                                             weights_.plain(prefix + ".conv.bias"), nullptr, 0, 1, out, 0, 2));
   return Act{out, C};
 }
 
@@ -536,18 +412,14 @@ Unet::Act Unet::build_upsample(const std::string& prefix, Act x, int H, int W) {
   const int C = x.C;
   const size_t Mo = static_cast<size_t>(NB_) * 4 * H * W;
   Scratch* s_up = scratch("upsampled", Mo * C);
-  __half* out = g_dry ? nullptr : alloc_act(Mo * C);
-  if (g_dry) {
-    raw(prefix + ".conv.weight"); raw(prefix + ".conv.bias");
-    workspace_bytes_ += Mo * C * sizeof(__half);
-    return Act{nullptr, C};
-  }
+  if (sizing_) return Act{nullptr, C};
+  __half* out = alloc_act(Mo * C);
   const int NB = NB_;
   const __half* xp = x.p;
   __half* up = s_up->p;
   add_step(prefix + ".nearest2x", [=](cudaStream_t st) { run_upsample2x(xp, up, NB, H, W, C, st); });
-  add_gemm(prefix + ".conv", make_conv3x3_op(up, NB_, 2 * H, 2 * W, C, packed_conv3x3(prefix + ".conv.weight"), C,
-                                             plain(prefix + ".conv.bias"), nullptr, 0, 1, out));
+  add_gemm(prefix + ".conv", make_conv3x3_op(up, NB_, 2 * H, 2 * W, C, weights_.packed_conv3x3(prefix + ".conv.weight"), C,
+                                             weights_.plain(prefix + ".conv.bias"), nullptr, 0, 1, out));
   return Act{out, C};
 }
 
@@ -571,21 +443,18 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
   }
   CFGPP_CHECK_CUDA(cudaSetDevice(device_));
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
-  StreamKScope sk_scope(sk_ws_, sk_flags_);  // every GEMM op built below parks its stream-K partials in OUR workspace
+  StreamKScope sk_scope(sk_.ws(), sk_.flags());  // every GEMM op built below parks its stream-K partials in OUR workspace
   // from here on the old plan is gone: a throw below must not leave the handle looking prepared
   prepared_ = false;
   nsteps_ = 0;
   graph_valid_ = false;
   // drop the previous plan / workspace
-  for (void* p : act_allocs_) cudaFree(p);
-  act_allocs_.clear();
+  act_.clear();
   scratch_.clear();
   prologue_plan_.clear();
   body_plan_.clear();
   tail_plan_.clear();
   prompt_plan_.clear();
-  workspace_bytes_ = 0;
-  graph_valid_ = false;
   B_ = batch; NB_ = 2 * batch; H_ = h_lat; W_ = w_lat;
   const int L = d_.num_levels;
   const int C0 = d_.block_out_channels[0];
@@ -616,12 +485,11 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
   };
 
   for (int pass = 0; pass < 2; ++pass) {
-    g_dry = (pass == 0);
-    if (!g_dry) {
-      workspace_bytes_ = 0;
+    sizing_ = (pass == 0);
+    if (!sizing_) {
       // allocate scratch + fixed buffers now that sizes are known
       for (auto& kv : scratch_) kv.second->p = alloc_act(kv.second->need);
-      gn_partial_ = static_cast<float*>(alloc_bytes(static_cast<size_t>(NB_) * 128 * 64 * sizeof(float)));
+      gn_partial_ = act_.alloc<float>(static_cast<size_t>(NB_) * 128 * 64);
       t_sin_ = alloc_act(C0);
       t_h1_ = alloc_act(TE);
       emb_ = alloc_act(static_cast<size_t>(NB_) * TE);
@@ -633,46 +501,36 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
         add_h1_ = alloc_act(static_cast<size_t>(NB_) * TE);
         aug_emb_ = alloc_act(static_cast<size_t>(NB_) * TE);
         pooled_copy_ = alloc_act(static_cast<size_t>(NB_) * d_.pooled_dim);
-        time_ids_copy_ = static_cast<float*>(alloc_bytes(static_cast<size_t>(NB_) * 6 * sizeof(float)));
+        time_ids_copy_ = act_.alloc<float>(static_cast<size_t>(NB_) * 6);
       }
-      cur_state_ = static_cast<StepState*>(alloc_bytes(sizeof(StepState)));
-      step_counter_ = static_cast<int*>(alloc_bytes(sizeof(int)));
-      step_table_ = static_cast<StepState*>(alloc_bytes(sizeof(StepState) * 1024));
+      cur_state_ = act_.alloc<StepState>(1);
+      step_counter_ = act_.alloc<int>(1);
+      step_table_ = act_.alloc<StepState>(1024);
       const size_t lat = static_cast<size_t>(B_) * 4 * H_ * W_;
-      z_state_ = alloc_bytes(lat * sizeof(float));
-      aux_state_ = alloc_bytes(lat * sizeof(float));
-      z0t_state_ = alloc_bytes(lat * sizeof(float));
-      noise_slot_ = static_cast<const __half**>(alloc_bytes(sizeof(__half*)));
+      z_state_ = act_.alloc<float>(lat);
+      aux_state_ = act_.alloc<float>(lat);
+      z0t_state_ = act_.alloc<float>(lat);
+      noise_slot_ = act_.alloc<const __half*>(1);
       CFGPP_CHECK_CUDA(cudaMemcpy(noise_slot_, &noise_buf_, sizeof(__half*), cudaMemcpyHostToDevice));
-      lambda_buf_ = static_cast<float*>(alloc_bytes(static_cast<size_t>(B_) * sizeof(float)));
-      lambda_slot_ = static_cast<const float**>(alloc_bytes(sizeof(float*)));
+      lambda_buf_ = act_.alloc<float>(B_);
+      lambda_slot_ = act_.alloc<const float*>(1);
       CFGPP_CHECK_CUDA(cudaMemset(lambda_slot_, 0, sizeof(float*)));  // no table: the schedule's scalar lambda
       fwd_eps_uc_ = alloc_act(lat);
       fwd_eps_c_ = alloc_act(lat);
       temb_w_all_ = packed_cat_rows(temb_w_keys);
       temb_b_all_ = packed_cat_rows(temb_b_keys);
-      conv_in_w_ = plain("conv_in.weight");
-      conv_in_b_ = plain("conv_in.bias");
-      conv_out_w_ = packed_conv3x3("conv_out.weight");
-      conv_out_b_ = plain("conv_out.bias");
-    } else {
-      for (const char* k : {"conv_in.weight", "conv_in.bias", "conv_out.weight", "conv_out.bias",
-                            "conv_norm_out.weight", "conv_norm_out.bias", "time_embedding.linear_1.weight",
-                            "time_embedding.linear_1.bias", "time_embedding.linear_2.weight",
-                            "time_embedding.linear_2.bias"})
-        raw(k);
-      if (has_aug_)
-        for (const char* k : {"add_embedding.linear_1.weight", "add_embedding.linear_1.bias",
-                              "add_embedding.linear_2.weight", "add_embedding.linear_2.bias"})
-          raw(k);
+      conv_in_w_ = weights_.plain("conv_in.weight");
+      conv_in_b_ = weights_.plain("conv_in.bias");
+      conv_out_w_ = weights_.packed_conv3x3("conv_out.weight");
+      conv_out_b_ = weights_.plain("conv_out.bias");
     }
 
     // ---- prologue: timestep embedding -> per-resnet time_emb_proj (SURVEY A.2 step 1, ResnetBlock2D temb) ----
     cur_plan_ = &prologue_plan_;
-    if (!g_dry) {
+    if (!sizing_) {
       const int NB = NB_;
-      const __half *w1 = plain("time_embedding.linear_1.weight"), *b1 = plain("time_embedding.linear_1.bias");
-      const __half *w2 = plain("time_embedding.linear_2.weight"), *b2 = plain("time_embedding.linear_2.bias");
+      const __half *w1 = weights_.plain("time_embedding.linear_1.weight"), *b1 = weights_.plain("time_embedding.linear_1.bias");
+      const __half *w2 = weights_.plain("time_embedding.linear_2.weight"), *b2 = weights_.plain("time_embedding.linear_2.bias");
       __half *t_sin = t_sin_, *t_h1 = t_h1_, *emb = emb_, *semb = semb_, *temb_all = temb_all_;
       const __half* aug = has_aug_ ? aug_emb_ : nullptr;
       const StepState* cur = cur_state_;
@@ -692,12 +550,12 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
 
     // ---- prompt plan: add-embedding (SDXL text_time) ----
     cur_plan_ = &prompt_plan_;
-    if (!g_dry && has_aug_) {
+    if (!sizing_ && has_aug_) {
       const int NB = NB_;
       const int ATE = d_.addition_time_embed_dim, PD = d_.pooled_dim, AIN = d_.projection_class_embeddings_input_dim;
       CFGPP_REQUIRE(AIN == PD + 6 * ATE, "projection_class_embeddings_input_dim != pooled_dim + 6*addition_time_embed_dim");
-      const __half *w1 = plain("add_embedding.linear_1.weight"), *b1 = plain("add_embedding.linear_1.bias");
-      const __half *w2 = plain("add_embedding.linear_2.weight"), *b2 = plain("add_embedding.linear_2.bias");
+      const __half *w1 = weights_.plain("add_embedding.linear_1.weight"), *b1 = weights_.plain("add_embedding.linear_1.bias");
+      const __half *w2 = weights_.plain("add_embedding.linear_2.weight"), *b2 = weights_.plain("add_embedding.linear_2.bias");
       __half *add_in = add_in_, *add_h1 = add_h1_, *aug = aug_emb_, *pooled = pooled_copy_;
       float* tids = time_ids_copy_;
       add_step("add_embedding.assemble", [=](cudaStream_t st) {
@@ -715,8 +573,7 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
     // ---- body (SURVEY A.2 steps 2-6) ----
     cur_plan_ = &body_plan_;
     const int HW0 = H_ * W_;
-    const Act h0{g_dry ? nullptr : alloc_act(static_cast<size_t>(NB_) * HW0 * C0), C0};
-    if (g_dry) workspace_bytes_ += static_cast<size_t>(NB_) * HW0 * C0 * sizeof(__half);
+    const Act h0{sizing_ ? nullptr : alloc_act(static_cast<size_t>(NB_) * HW0 * C0), C0};
     Act h = h0;
     int H = H_, W = W_;
     std::vector<Act> skips{h};
@@ -765,8 +622,8 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
     // ---- tail: conv_norm_out + SiLU on the last up block's output feeds the fused conv_out / CFG++ step kernel ----
     cur_plan_ = &tail_plan_;
     Scratch* s_norm = scratch("tail.norm", static_cast<size_t>(NB_) * HW0 * C0);
-    if (!g_dry) {
-      const __half *g = plain("conv_norm_out.weight"), *b = plain("conv_norm_out.bias");
+    if (!sizing_) {
+      const __half *g = weights_.plain("conv_norm_out.weight"), *b = weights_.plain("conv_norm_out.bias");
       const int NB = NB_, HW = HW0;
       const float eps = d_.norm_eps;
       float* partial = gn_partial_;
@@ -778,13 +635,7 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
       final_norm_ = Act{normp, C0};
       conv_in_out_ = h0.p;
     }
-    if (g_dry) {
-      // discard everything the sizing pass pushed (it pushes nothing) and keep the scratch sizes
-      prologue_plan_.clear(); body_plan_.clear(); tail_plan_.clear();
-      prompt_plan_.clear();
-    }
   }
-  g_dry = false;
 
   // FLOP / launch accounting (the reference executes the K/V projections every step: count them per forward)
   forward_flops_ = 0.0;

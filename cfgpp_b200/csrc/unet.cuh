@@ -9,20 +9,11 @@
 
 #include "../../include/cfgpp_b200.h"
 #include "attention.cuh"
+#include "executor.cuh"
 #include "gemm.cuh"
 #include "ops.cuh"
 
 namespace cfgpp {
-
-struct DevTensor {
-  __half* p = nullptr;
-  std::vector<int64_t> shape;
-  size_t numel() const {
-    size_t n = 1;
-    for (auto d : shape) n *= static_cast<size_t>(d);
-    return n;
-  }
-};
 
 struct PlanStep {
   std::string name;
@@ -41,7 +32,7 @@ class Unet {
                    cudaStream_t stream);
   void finalize_weights(cudaStream_t stream);
   void prepare(int batch, int h_lat, int w_lat);
-  size_t workspace_bytes() const { return workspace_bytes_; }
+  size_t workspace_bytes() const { return act_.bytes(); }
   double forward_flops() const { return forward_flops_; }
   int launches_per_step() const { return launches_per_step_; }
   double prompt_flops() const { return prompt_flops_; }
@@ -71,9 +62,6 @@ class Unet {
 
  private:
   // ---- weights ----
-  const DevTensor& raw(const std::string& key) const;
-  __half* alloc_weight(size_t numel);
-  __half* packed_conv3x3(const std::string& key);  // (Cout,Cin,3,3) -> [Cout][9][Cin]
   __half* packed_cat_rows(const std::vector<std::string>& keys);
   __half* packed_geglu(const std::string& key, bool is_bias);
   __half* packed_heads_rows(const std::vector<std::string>& keys, int heads, int hd, int hdp);
@@ -86,11 +74,9 @@ class Unet {
   FoldedLN folded_ln(const std::string& cache_key, const __half* w_packed, int N, int K, const std::string& norm_prefix,
                      const __half* bias_packed);
   std::map<std::string, FoldedLN> fold_cache_;
-  __half* plain(const std::string& key);
 
   // ---- workspace ----
-  __half* alloc_act(size_t numel);
-  void* alloc_bytes(size_t bytes);
+  __half* alloc_act(size_t numel) { return act_.alloc<__half>(numel); }
   struct Scratch {
     size_t need = 0;
     __half* p = nullptr;
@@ -114,10 +100,9 @@ class Unet {
   cfgpp_model_desc d_;
   int device_;
   bool finalized_ = false, prepared_ = false;
-  std::map<std::string, DevTensor> raw_;
-  std::vector<void*> weight_allocs_;
-  std::vector<void*> act_allocs_;
-  size_t workspace_bytes_ = 0;
+  WeightStore weights_;
+  DeviceArena act_;  // workspace of the prepared plan
+  StreamKWorkspace sk_;
 
   // packed weights: resolved lazily during plan building (finalize just validates + packs what is shape-independent)
   std::map<std::string, __half*> packed_cache_;
@@ -129,6 +114,7 @@ class Unet {
 
   // plan
   int B_ = 0, NB_ = 0, H_ = 0, W_ = 0;
+  bool sizing_ = false;  // prepare()'s first pass: records scratch sizes, allocates and pushes nothing
   std::vector<PlanStep>* cur_plan_ = nullptr;
   std::vector<PlanStep> prologue_plan_;  // timestep embedding -> temb for all resnets
   std::vector<PlanStep> body_plan_;      // conv_in output .. last up block
@@ -170,8 +156,6 @@ class Unet {
   __half* conv_in_out_ = nullptr;
   __half *conv_in_w_ = nullptr, *conv_in_b_ = nullptr, *conv_out_w_ = nullptr, *conv_out_b_ = nullptr;
 
-  float* sk_ws_ = nullptr;       // this handle's stream-K workspace (gemm.cuh StreamKScope)
-  unsigned* sk_flags_ = nullptr;
   cudaGraph_t graph_ = nullptr;
   cudaGraphExec_t graph_exec_ = nullptr;
   bool graph_valid_ = false;

@@ -8,7 +8,7 @@ namespace cfgpp {
 
 void gemm_configure();
 
-VaeDecoder::VaeDecoder(const cfgpp_vae_desc& d, int device) : d_(d), device_(device) {
+VaeDecoder::VaeDecoder(const cfgpp_vae_desc& d, int device) : d_(d), device_(device), sk_(device) {
   CFGPP_CHECK_CUDA(cudaSetDevice(device));
   CFGPP_REQUIRE(d.num_levels >= 2 && d.num_levels <= CFGPP_MAX_LEVELS, "num_levels must be 2..4");
   CFGPP_REQUIRE(d.latent_channels == 4 && d.out_channels == 3, "the decoder maps 4 latent channels to 3 image channels");
@@ -17,55 +17,12 @@ VaeDecoder::VaeDecoder(const cfgpp_vae_desc& d, int device) : d_(d), device_(dev
     CFGPP_REQUIRE(d.block_out_channels[i] % 64 == 0, "decoder channel counts must be multiples of 64");
   CFGPP_REQUIRE(d.scaling_factor > 0.f, "scaling_factor must be positive");
   gemm_configure();
-  streamk_alloc(&sk_ws_, &sk_flags_);
-}
-
-VaeDecoder::~VaeDecoder() {
-  for (auto& kv : raw_) cudaFree(kv.second.p);
-  for (void* p : weight_allocs_) cudaFree(p);
-  for (void* p : act_allocs_) cudaFree(p);
-  for (void* p : enc_allocs_) cudaFree(p);
-  streamk_free(sk_ws_, sk_flags_);
 }
 
 void VaeDecoder::load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
                              cudaStream_t stream) {
   CFGPP_REQUIRE(!finalized_, "weights already finalized");
-  CFGPP_REQUIRE(dtype == CFGPP_F16 || dtype == CFGPP_F32, "weight dtype must be fp16 or fp32");
-  Tensor t;
-  t.shape.assign(shape, shape + ndim);
-  const size_t n = t.numel();
-  CFGPP_CHECK_CUDA(cudaMalloc(&t.p, std::max<size_t>(n, 8) * sizeof(__half)));
-  if (dtype == CFGPP_F16) {
-    CFGPP_CHECK_CUDA(cudaMemcpyAsync(t.p, data, n * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
-  } else {
-    run_f32_to_f16(static_cast<const float*>(data), t.p, n, stream);
-  }
-  auto it = raw_.find(key);
-  if (it != raw_.end()) {
-    cudaFree(it->second.p);
-    raw_.erase(it);
-  }
-  raw_[key] = t;
-}
-
-const VaeDecoder::Tensor& VaeDecoder::raw(const std::string& key) const {
-  auto it = raw_.find(key);
-  if (it == raw_.end()) throw Error(-10, "missing weight: " + key);
-  return it->second;
-}
-
-__half* VaeDecoder::packed_conv(const std::string& key) {
-  auto it = packed_.find(key);
-  if (it != packed_.end()) return it->second;
-  const Tensor& t = raw(key);
-  CFGPP_REQUIRE(t.shape.size() == 4 && t.shape[2] == 3 && t.shape[3] == 3, "expected (Cout,Cin,3,3): " + key);
-  void* p = nullptr;
-  CFGPP_CHECK_CUDA(cudaMalloc(&p, std::max<size_t>(t.numel(), 8) * sizeof(__half)));
-  weight_allocs_.push_back(p);
-  run_pack_conv3x3(t.p, static_cast<__half*>(p), static_cast<int>(t.shape[0]), static_cast<int>(t.shape[1]), nullptr);
-  packed_[key] = static_cast<__half*>(p);
-  return static_cast<__half*>(p);
+  weights_.load(key, data, shape, ndim, dtype, stream);
 }
 
 void VaeDecoder::finalize_weights(cudaStream_t stream) {
@@ -74,18 +31,16 @@ void VaeDecoder::finalize_weights(cudaStream_t stream) {
   try {  // structural validation: a dry plan at the smallest latent touches (and packs) every weight
     prepare(1, 16, 16);
     if (has_encoder()) {
-      const Tensor& ci = raw("encoder.conv_in.weight");
+      const WeightStore::Weight& ci = weights_.raw("encoder.conv_in.weight");
       CFGPP_REQUIRE(ci.shape.size() == 4 && ci.shape[1] == 3 && ci.shape[2] == 3 && ci.shape[3] == 3 &&
                         ci.shape[0] == d_.block_out_channels[0],
                     "encoder.conv_in.weight must be (C0,3,3,3)");
       const size_t c0 = static_cast<size_t>(ci.shape[0]);
-      void* p4 = nullptr;
-      CFGPP_CHECK_CUDA(cudaMalloc(&p4, c0 * 36 * sizeof(__half)));
-      weight_allocs_.push_back(p4);
+      __half* p4 = weights_.alloc(c0 * 36);
       CFGPP_CHECK_CUDA(cudaMemset(p4, 0, c0 * 36 * sizeof(__half)));
-      CFGPP_CHECK_CUDA(cudaMemcpy2D(p4, 36 * sizeof(__half), ci.p, 27 * sizeof(__half), 27 * sizeof(__half), c0,
+      CFGPP_CHECK_CUDA(cudaMemcpy2D(p4, 36 * sizeof(__half), ci.p(), 27 * sizeof(__half), 27 * sizeof(__half), c0,
                                     cudaMemcpyDeviceToDevice));
-      conv_in_w4_ = static_cast<__half*>(p4);
+      conv_in_w4_ = p4;
       prepare_encode(1, 128, 128);
     }
   } catch (...) {
@@ -94,13 +49,13 @@ void VaeDecoder::finalize_weights(cudaStream_t stream) {
   }
 }
 
-void* VaeDecoder::alloc_bytes(size_t bytes) {
-  void* p = nullptr;
-  bytes = (bytes + 255) & ~static_cast<size_t>(255);
-  CFGPP_CHECK_CUDA(cudaMalloc(&p, std::max<size_t>(bytes, 256)));
-  cur_allocs_->push_back(p);
-  workspace_bytes_ += bytes;
-  return p;
+// drops `plan` (launches and workspace) and makes it the one the builders append to
+void VaeDecoder::begin_plan(Plan& plan) {
+  plan.steps.clear();
+  plan.arena.clear();
+  plan.flops = 0.0;
+  plan.batch = 0;
+  cur_ = &plan;
 }
 
 __half* VaeDecoder::next_out() {
@@ -112,22 +67,22 @@ __half* VaeDecoder::next_out() {
 __half* VaeDecoder::build_resnet(const std::string& prefix, const __half* x, int Cin, int Cout, int H, int W) {
   const int HW = H * W, NB = nb_;
   const int M = NB * HW;
-  const __half *g1 = plain(prefix + ".norm1.weight"), *b1 = plain(prefix + ".norm1.bias");
-  const __half *g2 = plain(prefix + ".norm2.weight"), *b2 = plain(prefix + ".norm2.bias");
+  const __half *g1 = weights_.plain(prefix + ".norm1.weight"), *b1 = weights_.plain(prefix + ".norm1.bias");
+  const __half *g2 = weights_.plain(prefix + ".norm2.weight"), *b2 = weights_.plain(prefix + ".norm2.bias");
   __half *normp = s_norm_, *h1 = s_h1_;
   float* partial = gn_partial_;
   add([=](cudaStream_t st) { run_groupnorm(x, Cin, nullptr, 0, NB, HW, g1, b1, 1e-6f, true, partial, normp, st); });
-  add_gemm(make_conv3x3_op(normp, NB, H, W, Cin, packed_conv(prefix + ".conv1.weight"), Cout, plain(prefix + ".conv1.bias"),
+  add_gemm(make_conv3x3_op(normp, NB, H, W, Cin, weights_.packed_conv3x3(prefix + ".conv1.weight"), Cout, weights_.plain(prefix + ".conv1.bias"),
                            nullptr, 0, 1, h1));
   add([=](cudaStream_t st) { run_groupnorm(h1, Cout, nullptr, 0, NB, HW, g2, b2, 1e-6f, true, partial, normp, st); });
   const __half* residual = x;
   if (Cin != Cout) {
-    add_gemm(make_linear_op(x, Cin, nullptr, 0, 0, plain(prefix + ".conv_shortcut.weight"), M, Cout, Cin,
-                            plain(prefix + ".conv_shortcut.bias"), nullptr, 0, 1, s_sc_, Cout, false));
+    add_gemm(make_linear_op(x, Cin, nullptr, 0, 0, weights_.plain(prefix + ".conv_shortcut.weight"), M, Cout, Cin,
+                            weights_.plain(prefix + ".conv_shortcut.bias"), nullptr, 0, 1, s_sc_, Cout, false));
     residual = s_sc_;
   }
   __half* out = next_out();
-  add_gemm(make_conv3x3_op(normp, NB, H, W, Cout, packed_conv(prefix + ".conv2.weight"), Cout, plain(prefix + ".conv2.bias"),
+  add_gemm(make_conv3x3_op(normp, NB, H, W, Cout, weights_.packed_conv3x3(prefix + ".conv2.weight"), Cout, weights_.plain(prefix + ".conv2.bias"),
                            residual, Cout, 1, out));
   return out;
 }
@@ -136,16 +91,16 @@ __half* VaeDecoder::build_resnet(const std::string& prefix, const __half* x, int
 __half* VaeDecoder::build_attention(const std::string& prefix, const __half* x, int C, int H, int W) {
   const int N = H * W, NB = nb_;
   CFGPP_REQUIRE(N % 64 == 0, "mid-block attention needs H*W to be a multiple of 64");
-  const __half *g = plain(prefix + ".group_norm.weight"), *b = plain(prefix + ".group_norm.bias");
+  const __half *g = weights_.plain(prefix + ".group_norm.weight"), *b = weights_.plain(prefix + ".group_norm.bias");
   __half *normp = s_norm_, *q = s_q_, *k = s_k_, *vt = s_vt_, *sc = s_scores_, *o = s_o_;
   float* partial = gn_partial_;
   add([=](cudaStream_t st) { run_groupnorm(x, C, nullptr, 0, NB, N, g, b, 1e-6f, false, partial, normp, st); });
-  add_gemm(make_linear_op(normp, C, nullptr, 0, 0, plain(prefix + ".to_q.weight"), NB * N, C, C, plain(prefix + ".to_q.bias"),
+  add_gemm(make_linear_op(normp, C, nullptr, 0, 0, weights_.plain(prefix + ".to_q.weight"), NB * N, C, C, weights_.plain(prefix + ".to_q.bias"),
                           nullptr, 0, 1, q, C, false));
-  add_gemm(make_linear_op(normp, C, nullptr, 0, 0, plain(prefix + ".to_k.weight"), NB * N, C, C, plain(prefix + ".to_k.bias"),
+  add_gemm(make_linear_op(normp, C, nullptr, 0, 0, weights_.plain(prefix + ".to_k.weight"), NB * N, C, C, weights_.plain(prefix + ".to_k.bias"),
                           nullptr, 0, 1, k, C, false));
   const float scale_log2e = (1.0f / sqrtf(static_cast<float>(C))) * 1.4426950408889634f;
-  const __half *wv = plain(prefix + ".to_v.weight"), *bv = plain(prefix + ".to_v.bias");
+  const __half *wv = weights_.plain(prefix + ".to_v.weight"), *bv = weights_.plain(prefix + ".to_v.bias");
   for (int s = 0; s < NB; ++s) {  // the N x N score matrix is materialised one sample at a time
     const __half* qs = q + static_cast<size_t>(s) * N * C;
     const __half* ks = k + static_cast<size_t>(s) * N * C;
@@ -160,8 +115,8 @@ __half* VaeDecoder::build_attention(const std::string& prefix, const __half* x, 
     add_gemm(make_linear_op(sc, N, nullptr, 0, 0, vt, N, C, N, bv, nullptr, 0, 1, os, C, false));
   }
   __half* out = next_out();
-  add_gemm(make_linear_op(o, C, nullptr, 0, 0, plain(prefix + ".to_out.0.weight"), NB * N, C, C,
-                          plain(prefix + ".to_out.0.bias"), x, C, 1, out, C, false));
+  add_gemm(make_linear_op(o, C, nullptr, 0, 0, weights_.plain(prefix + ".to_out.0.weight"), NB * N, C, C,
+                          weights_.plain(prefix + ".to_out.0.bias"), x, C, 1, out, C, false));
   return out;
 }
 
@@ -177,7 +132,7 @@ void VaeDecoder::alloc_scratch(size_t max_act, size_t ntok, int Ct) {
   s_o_ = alloc_act(NB * ntok * Ct);
   s_vt_ = alloc_act(ntok * Ct);
   s_scores_ = alloc_act(ntok * ntok);
-  gn_partial_ = static_cast<float*>(alloc_bytes(NB * 128 * 64 * sizeof(float)));
+  gn_partial_ = cur_->arena.alloc<float>(NB * 128 * 64);
 }
 
 void VaeDecoder::prepare(int batch, int h_lat, int w_lat) {
@@ -192,16 +147,8 @@ void VaeDecoder::prepare(int batch, int h_lat, int w_lat) {
                     ": a latent whose decoder levels are not all tiled-addressable must be at least 64 x 64 (512 px images)");
   CFGPP_CHECK_CUDA(cudaSetDevice(device_));
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
-  StreamKScope sk_scope(sk_ws_, sk_flags_);  // the decoder's GEMM ops use its own stream-K workspace
-  for (void* p : act_allocs_) cudaFree(p);
-  act_allocs_.clear();
-  plan_.clear();
-  cur_allocs_ = &act_allocs_;
-  cur_plan_ = &plan_;
-  cur_flops_ = &flops_;
-  workspace_bytes_ = 0;
-  flops_ = 0.0;
-  B_ = 0;
+  StreamKScope sk_scope(sk_.ws(), sk_.flags());  // the decoder's GEMM ops use its own stream-K workspace
+  begin_plan(dec_);
   const int NB = batch;
   nb_ = NB;
   // sizes: the largest activation of the walk (elements per sample)
@@ -220,7 +167,6 @@ void VaeDecoder::prepare(int batch, int h_lat, int w_lat) {
       }
     }
   }
-  B_ = NB; H_ = h_lat; W_ = w_lat;
   const int Ct = d_.block_out_channels[L - 1];
   const size_t ntok = static_cast<size_t>(h_lat) * w_lat;
   alloc_scratch(max_act, ntok, Ct);
@@ -229,9 +175,9 @@ void VaeDecoder::prepare(int batch, int h_lat, int w_lat) {
 
   // ---- plan ----
   const float scaling = d_.scaling_factor;
-  const __half *wpq = plain("post_quant_conv.weight"), *bpq = plain("post_quant_conv.bias");
-  const __half *wci = plain("decoder.conv_in.weight"), *bci = plain("decoder.conv_in.bias");
-  CFGPP_REQUIRE(raw("post_quant_conv.weight").numel() == 16, "post_quant_conv must be a 4 -> 4 1x1 convolution");
+  const __half *wpq = weights_.plain("post_quant_conv.weight"), *bpq = weights_.plain("post_quant_conv.bias");
+  const __half *wci = weights_.plain("decoder.conv_in.weight"), *bci = weights_.plain("decoder.conv_in.bias");
+  CFGPP_REQUIRE(weights_.raw("post_quant_conv.weight").numel() == 16, "post_quant_conv must be a 4 -> 4 1x1 convolution");
   __half* zq = zq_;
   __half* x0 = rot_[0];
   const int h0 = h_lat, w0 = w_lat;
@@ -239,7 +185,7 @@ void VaeDecoder::prepare(int batch, int h_lat, int w_lat) {
     run_vae_latent_prep(z_in_, z_is_half_, scaling, wpq, bpq, zq, NB, h0 * w0, st);
     run_conv_in(zq, 1, nullptr, wci, bci, x0, NB, h0, w0, Ct, 1, st);
   });
-  flops_ += 2.0 * NB * h0 * w0 * 36.0 * Ct;
+  dec_.flops += 2.0 * NB * h0 * w0 * 36.0 * Ct;
   const __half* x = x0;
   x = build_resnet("decoder.mid_block.resnets.0", x, Ct, Ct, h0, w0);
   x = build_attention("decoder.mid_block.attentions.0", x, Ct, h0, w0);
@@ -260,16 +206,16 @@ void VaeDecoder::prepare(int batch, int h_lat, int w_lat) {
       H *= 2;
       W *= 2;
       __half* out = next_out();
-      add_gemm(make_conv3x3_op(up, NB, H, W, C, packed_conv(blk + ".upsamplers.0.conv.weight"), C,
-                               plain(blk + ".upsamplers.0.conv.bias"), nullptr, 0, 1, out));
+      add_gemm(make_conv3x3_op(up, NB, H, W, C, weights_.packed_conv3x3(blk + ".upsamplers.0.conv.weight"), C,
+                               weights_.plain(blk + ".upsamplers.0.conv.bias"), nullptr, 0, 1, out));
       x = out;
     }
   }
   {
-    const __half *g = plain("decoder.conv_norm_out.weight"), *b = plain("decoder.conv_norm_out.bias");
-    const __half* wco = packed_conv("decoder.conv_out.weight");
-    const __half* bco = plain("decoder.conv_out.bias");
-    CFGPP_REQUIRE(raw("decoder.conv_out.weight").shape[0] == 3, "conv_out must produce 3 channels");
+    const __half *g = weights_.plain("decoder.conv_norm_out.weight"), *b = weights_.plain("decoder.conv_norm_out.bias");
+    const __half* wco = weights_.packed_conv3x3("decoder.conv_out.weight");
+    const __half* bco = weights_.plain("decoder.conv_out.bias");
+    CFGPP_REQUIRE(weights_.raw("decoder.conv_out.weight").shape[0] == 3, "conv_out must produce 3 channels");
     __half* normp = s_norm_;
     float* partial = gn_partial_;
     const __half* xin = x;
@@ -278,19 +224,20 @@ void VaeDecoder::prepare(int batch, int h_lat, int w_lat) {
       run_groupnorm(xin, Cc, nullptr, 0, NB, Hc * Wc, g, b, 1e-6f, true, partial, normp, st);
       run_vae_conv_rgb(normp, wco, bco, image_out_, NB, Hc, Wc, Cc, st);
     });
-    flops_ += 2.0 * NB * Hc * Wc * 27.0 * Cc;
+    dec_.flops += 2.0 * NB * Hc * Wc * 27.0 * Cc;
   }
+  dec_.batch = NB; dec_.h = h_lat; dec_.w = w_lat;
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
 }
 
 void VaeDecoder::decode(const void* z, int z_dtype, int batch, int h_lat, int w_lat, __half* image,
                         cudaStream_t stream) {
   CFGPP_REQUIRE(z_dtype == CFGPP_F16 || z_dtype == CFGPP_F32, "latent dtype must be fp16 or fp32");
-  if (batch != B_ || h_lat != H_ || w_lat != W_) prepare(batch, h_lat, w_lat);
+  if (batch != dec_.batch || h_lat != dec_.h || w_lat != dec_.w) prepare(batch, h_lat, w_lat);
   z_in_ = z;
   z_is_half_ = (z_dtype == CFGPP_F16) ? 1 : 0;
   image_out_ = image;
-  for (auto& fn : plan_) fn(stream);
+  for (auto& fn : dec_.steps) fn(stream);
 }
 
 // ---- encoder ----------------------------------------------------------------------------------------------------
@@ -316,15 +263,8 @@ void VaeDecoder::prepare_encode(int batch, int H, int W) {
                     ": an image whose encoder levels are not all tiled-addressable must be at least 512 x 512 px");
   CFGPP_CHECK_CUDA(cudaSetDevice(device_));
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
-  StreamKScope sk_scope(sk_ws_, sk_flags_);
-  for (void* p : enc_allocs_) cudaFree(p);
-  enc_allocs_.clear();
-  enc_plan_.clear();
-  cur_allocs_ = &enc_allocs_;
-  cur_plan_ = &enc_plan_;
-  cur_flops_ = &enc_flops_;
-  enc_flops_ = 0.0;
-  eB_ = 0;
+  StreamKScope sk_scope(sk_.ws(), sk_.flags());
+  begin_plan(enc_);
   const int NB = batch;
   nb_ = NB;
   size_t max_act = 0;
@@ -344,13 +284,13 @@ void VaeDecoder::prepare_encode(int batch, int H, int W) {
 
   const int C0 = d_.block_out_channels[0];
   const __half* wci = conv_in_w4_;
-  const __half* bci = plain("encoder.conv_in.bias");
+  const __half* bci = weights_.plain("encoder.conv_in.bias");
   __half* x0 = rot_[0];
   add([=](cudaStream_t st) {
     run_vae_image_pad(x_in_, x_is_half_, img4, NB, H, W, st);
     run_conv_in(img4, 1, nullptr, wci, bci, x0, NB, H, W, C0, 1, st);
   });
-  enc_flops_ += 2.0 * NB * H * W * 27.0 * C0;
+  enc_.flops += 2.0 * NB * H * W * 27.0 * C0;
   const __half* x = x0;
   int h = H, w = W, C = C0;
   for (int i = 0; i < L; ++i) {
@@ -362,8 +302,8 @@ void VaeDecoder::prepare_encode(int batch, int H, int W) {
     }
     if (i != L - 1) {
       __half* out = next_out();
-      add_gemm(make_conv3x3_op(x, NB, h, w, C, packed_conv(blk + ".downsamplers.0.conv.weight"), C,
-                               plain(blk + ".downsamplers.0.conv.bias"), nullptr, 0, 1, out, 0, /*stride=*/2, /*pad=*/0));
+      add_gemm(make_conv3x3_op(x, NB, h, w, C, weights_.packed_conv3x3(blk + ".downsamplers.0.conv.weight"), C,
+                               weights_.plain(blk + ".downsamplers.0.conv.bias"), nullptr, 0, 1, out, 0, /*stride=*/2, /*pad=*/0));
       x = out;
       h /= 2;
       w /= 2;
@@ -373,13 +313,13 @@ void VaeDecoder::prepare_encode(int batch, int H, int W) {
   x = build_attention("encoder.mid_block.attentions.0", x, C, h, w);
   x = build_resnet("encoder.mid_block.resnets.1", x, C, C, h, w);
   {
-    const __half *g = plain("encoder.conv_norm_out.weight"), *b = plain("encoder.conv_norm_out.bias");
-    const Tensor& wo = raw("encoder.conv_out.weight");
+    const __half *g = weights_.plain("encoder.conv_norm_out.weight"), *b = weights_.plain("encoder.conv_norm_out.bias");
+    const WeightStore::Weight& wo = weights_.raw("encoder.conv_out.weight");
     CFGPP_REQUIRE(wo.shape.size() == 4 && wo.shape[0] == 8 && wo.shape[1] == C, "encoder.conv_out must produce 8 moments");
-    CFGPP_REQUIRE(raw("quant_conv.weight").numel() == 64 && raw("quant_conv.bias").numel() == 8,
+    CFGPP_REQUIRE(weights_.raw("quant_conv.weight").numel() == 64 && weights_.raw("quant_conv.bias").numel() == 8,
                   "quant_conv must be an 8 -> 8 1x1 convolution");
-    const __half* wco = packed_conv("encoder.conv_out.weight");
-    const __half *bco = plain("encoder.conv_out.bias"), *wq = plain("quant_conv.weight"), *bq = plain("quant_conv.bias");
+    const __half* wco = weights_.packed_conv3x3("encoder.conv_out.weight");
+    const __half *bco = weights_.plain("encoder.conv_out.bias"), *wq = weights_.plain("quant_conv.weight"), *bq = weights_.plain("quant_conv.bias");
     __half* normp = s_norm_;
     float* partial = gn_partial_;
     const __half* xin = x;
@@ -389,9 +329,9 @@ void VaeDecoder::prepare_encode(int batch, int H, int W) {
       run_groupnorm(xin, Cc, nullptr, 0, NB, hc * wc, g, b, 1e-6f, true, partial, normp, st);
       run_vae_moments_sample(normp, wco, bco, wq, bq, noise_in_, scaling, latent_out_, NB, hc, wc, Cc, st);
     });
-    enc_flops_ += 2.0 * NB * hc * wc * 72.0 * Cc;
+    enc_.flops += 2.0 * NB * hc * wc * 72.0 * Cc;
   }
-  eB_ = NB; eH_ = H; eW_ = W;
+  enc_.batch = NB; enc_.h = H; enc_.w = W;
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
 }
 
@@ -399,12 +339,12 @@ void VaeDecoder::encode(const void* image, int x_dtype, int batch, int H, int W,
                         cudaStream_t stream) {
   CFGPP_REQUIRE(x_dtype == CFGPP_F16 || x_dtype == CFGPP_F32, "image dtype must be fp16 or fp32");
   CFGPP_REQUIRE(image != nullptr && latent != nullptr, "null image / latent pointer");
-  if (batch != eB_ || H != eH_ || W != eW_) prepare_encode(batch, H, W);
+  if (batch != enc_.batch || H != enc_.h || W != enc_.w) prepare_encode(batch, H, W);
   x_in_ = image;
   x_is_half_ = (x_dtype == CFGPP_F16) ? 1 : 0;
   noise_in_ = noise;
   latent_out_ = latent;
-  for (auto& fn : enc_plan_) fn(stream);
+  for (auto& fn : enc_.steps) fn(stream);
 }
 
 }  // namespace cfgpp

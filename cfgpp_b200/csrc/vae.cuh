@@ -14,13 +14,12 @@
 #include <vector>
 
 #include "../../include/cfgpp_b200.h"
+#include "executor.cuh"
 #include "gemm.cuh"
 #include "ops.cuh"
 
 namespace cfgpp {
 
-void run_f32_to_f16(const float* in, __half* out, size_t n, cudaStream_t stream);
-void run_pack_conv3x3(const __half* in, __half* out, int Cout, int Cin, cudaStream_t stream);
 // vae_kernels.cu
 void run_vae_latent_prep(const void* z, int z_is_half, float scaling, const __half* w, const __half* bias, __half* out,
                          int B, int HW, cudaStream_t stream);
@@ -35,7 +34,6 @@ void run_vae_moments_sample(const __half* x, const __half* w, const __half* bias
 class VaeDecoder {
  public:
   VaeDecoder(const cfgpp_vae_desc& d, int device);
-  ~VaeDecoder();
   void load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
                    cudaStream_t stream);
   void finalize_weights(cudaStream_t stream);
@@ -46,34 +44,29 @@ class VaeDecoder {
   // fp32 (what the fp16 module returns under the reference's autocast). noise: the caller's `randn(mean.shape)` draw in fp16, or null for the posterior mean.
   void encode(const void* image, int x_dtype, int batch, int H, int W, const __half* noise, float* latent,
               cudaStream_t stream);
-  bool has_encoder() const { return raw_.count("encoder.conv_in.weight") != 0; }
-  double encode_flops() const { return enc_flops_; }
-  double flops() const { return flops_; }
-  size_t workspace_bytes() const { return workspace_bytes_; }
+  bool has_encoder() const { return weights_.has("encoder.conv_in.weight"); }
+  double encode_flops() const { return enc_.flops; }
+  double flops() const { return dec_.flops; }
+  size_t workspace_bytes() const { return dec_.arena.bytes(); }  // one decode of the prepared shape
 
  private:
-  struct Tensor {
-    __half* p = nullptr;
-    std::vector<int64_t> shape;
-    size_t numel() const {
-      size_t n = 1;
-      for (auto d : shape) n *= static_cast<size_t>(d);
-      return n;
-    }
+  // one direction's launch plan for its prepared shape, with the workspace it runs in
+  struct Plan {
+    std::vector<std::function<void(cudaStream_t)>> steps;
+    double flops = 0.0;
+    DeviceArena arena;
+    int batch = 0, h = 0, w = 0;  // batch 0: nothing prepared
   };
-  const Tensor& raw(const std::string& key) const;
-  __half* plain(const std::string& key) const { return raw(key).p; }
-  __half* packed_conv(const std::string& key);  // (Cout,Cin,3,3) -> [Cout][9][Cin]
-  void* alloc_bytes(size_t bytes);
-  __half* alloc_act(size_t numel) { return static_cast<__half*>(alloc_bytes(numel * sizeof(__half))); }
+  void begin_plan(Plan& plan);
+  __half* alloc_act(size_t numel) { return cur_->arena.alloc<__half>(numel); }
   void prepare(int batch, int h_lat, int w_lat);
   void prepare_encode(int batch, int H, int W);
-  void add(std::function<void(cudaStream_t)> fn) { cur_plan_->push_back(std::move(fn)); }
+  void add(std::function<void(cudaStream_t)> fn) { cur_->steps.push_back(std::move(fn)); }
   void add_gemm(const GemmOp& op) {
-    *cur_flops_ += op.flops();
-    cur_plan_->push_back([op](cudaStream_t st) { run_gemm_op(op, st); });
+    cur_->flops += op.flops();
+    cur_->steps.push_back([op](cudaStream_t st) { run_gemm_op(op, st); });
   }
-  void alloc_scratch(size_t max_act, size_t ntok, int Ct);  // the builders' scratch set, into the current allocation list
+  void alloc_scratch(size_t max_act, size_t ntok, int Ct);  // the builders' scratch set, into the current plan's arena
   // builders return the output activation pointer
   __half* build_resnet(const std::string& prefix, const __half* x, int Cin, int Cout, int H, int W);
   __half* build_attention(const std::string& prefix, const __half* x, int C, int H, int W);
@@ -82,22 +75,11 @@ class VaeDecoder {
   cfgpp_vae_desc d_;
   int device_;
   bool finalized_ = false;
-  std::map<std::string, Tensor> raw_;
-  std::map<std::string, __half*> packed_;
-  std::vector<void*> weight_allocs_;
-  std::vector<void*> act_allocs_;   // decode plan
-  std::vector<void*> enc_allocs_;   // encode plan
-  std::vector<void*>* cur_allocs_ = &act_allocs_;
-  size_t workspace_bytes_ = 0;
-  double flops_ = 0.0;
-  // plan for the prepared (batch, h, w)
-  int B_ = 0, H_ = 0, W_ = 0;
-  std::vector<std::function<void(cudaStream_t)>> plan_, enc_plan_;
-  std::vector<std::function<void(cudaStream_t)>>* cur_plan_ = &plan_;
-  double enc_flops_ = 0.0;
-  double* cur_flops_ = &flops_;
+  WeightStore weights_;
+  StreamKWorkspace sk_;
+  Plan dec_, enc_;    // decode (latent shape), encode (image shape)
+  Plan* cur_ = &dec_;  // the plan the builders append to
   int nb_ = 0;                     // batch the builders lay the current plan out for
-  int eB_ = 0, eH_ = 0, eW_ = 0;   // prepared encode shape
   const void* x_in_ = nullptr;     // set per encode() call
   int x_is_half_ = 0;
   const __half* noise_in_ = nullptr;
@@ -112,8 +94,6 @@ class VaeDecoder {
   __half *s_norm_ = nullptr, *s_h1_ = nullptr, *s_sc_ = nullptr, *s_up_ = nullptr, *zq_ = nullptr;
   __half *s_q_ = nullptr, *s_k_ = nullptr, *s_vt_ = nullptr, *s_scores_ = nullptr, *s_o_ = nullptr;
   float* gn_partial_ = nullptr;
-  float* sk_ws_ = nullptr;  // this handle's stream-K workspace (gemm.cuh StreamKScope)
-  unsigned* sk_flags_ = nullptr;
 };
 
 }  // namespace cfgpp

@@ -7,7 +7,7 @@ PyTorch only owns the tensors and the stream. There is no eager / CPU fallback.
 from __future__ import annotations
 
 import ctypes
-from ctypes import POINTER, byref, c_double, c_float, c_int, c_int64, c_size_t, c_void_p
+from ctypes import POINTER, byref, c_double, c_float, c_int, c_size_t
 from typing import Dict, Optional, Sequence
 
 import torch
@@ -17,52 +17,17 @@ from .config import UNetConfig, to_desc
 from .schedule import F16, F32, StepStateC, to_c_array
 
 
-def _dtype_code(t: torch.Tensor) -> int:
-    if t.dtype == torch.float16:
-        return F16
-    if t.dtype == torch.float32:
-        return F32
-    raise TypeError(f"unsupported dtype {t.dtype}")
+class NativeUNet(nv.NativeHandle):
+    _prefix, _what = "", "backend"
 
-
-class NativeUNet:
     def __init__(self, cfg: UNetConfig, state_dict: Dict[str, torch.Tensor], device="cuda:0"):
         self.cfg = cfg
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise nv.NativeError("the cfgpp_b200 backend runs on CUDA (sm_90a) only; use the oracle for CPU runs")
-        self.lib = nv.load()
-        self._h = c_void_p()
-        idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        self.device = torch.device("cuda", idx)
-        desc = to_desc(cfg)
-        with torch.cuda.device(self.device):
-            nv.check(self.lib.cfgpp_create(byref(desc), c_int(idx), byref(self._h)))
-            st = nv.stream_ptr()
-            for key, w in state_dict.items():
-                wd = w.detach().to(self.device).contiguous()
-                shape = (c_int64 * wd.dim())(*wd.shape)
-                nv.check(self.lib.cfgpp_load_weight(self._h, key.encode(), nv.ptr(wd), shape, c_int(wd.dim()),
-                                                    c_int(_dtype_code(wd)), st))
-                del wd
-            torch.cuda.synchronize(self.device)
-            nv.check(self.lib.cfgpp_finalize_weights(self._h, st))
+        self._open(to_desc(cfg), state_dict.items(), device)
         self.batch = 0
         self.latent_hw = (0, 0)
         self._nsteps = 0
         self._state_dtype = torch.float32
         self._bound = None  # strong references to the tensors of the bound prompt (see bind_prompt)
-
-    def close(self):
-        if self._h:
-            self.lib.cfgpp_destroy(self._h)
-            self._h = c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:  # noqa: BLE001
-            pass
 
     # ---- plan ------------------------------------------------------------------------------------------------
     def prepare(self, batch: int, h_lat: int, w_lat: int):
@@ -142,7 +107,7 @@ class NativeUNet:
         eps_uc = torch.empty(z.shape, dtype=torch.float16, device=self.device)
         eps_c = torch.empty_like(eps_uc)
         with torch.cuda.device(self.device):
-            nv.check(self.lib.cfgpp_unet_forward(self._h, nv.ptr(z), c_int(_dtype_code(z)), c_float(float(t)),
+            nv.check(self.lib.cfgpp_unet_forward(self._h, nv.ptr(z), c_int(nv.dtype_code(z)), c_float(float(t)),
                                                  c_float(float(in_scale)), nv.ptr(eps_uc), nv.ptr(eps_c),
                                                  nv.stream_ptr()))
         return eps_uc, eps_c
@@ -157,7 +122,7 @@ class NativeUNet:
         kd = (c_int * max_n)()
         names = ctypes.create_string_buffer(max_n * stride)
         with torch.cuda.device(self.device):
-            nv.check(self.lib.cfgpp_profile_forward(self._h, nv.ptr(z), c_int(_dtype_code(z)), c_float(float(t)),
+            nv.check(self.lib.cfgpp_profile_forward(self._h, nv.ptr(z), c_int(nv.dtype_code(z)), c_float(float(t)),
                                                     c_float(float(in_scale)), c_int(max_n), byref(n), ms, fl, kd, names,
                                                     c_int(stride), nv.stream_ptr()))
         out = []
@@ -192,7 +157,7 @@ class NativeUNet:
     def set_state(self, z: torch.Tensor):
         z = z.to(self.device, self._state_dtype).contiguous()
         with torch.cuda.device(self.device):
-            nv.check(self.lib.cfgpp_set_state(self._h, nv.ptr(z), c_int(_dtype_code(z)), nv.stream_ptr()))
+            nv.check(self.lib.cfgpp_set_state(self._h, nv.ptr(z), c_int(nv.dtype_code(z)), nv.stream_ptr()))
 
     def set_noise(self, noise: torch.Tensor):
         """Ancestral samplers: fp16 noise table (slots, batch, 4, h, w), one slot per step that adds fresh noise."""

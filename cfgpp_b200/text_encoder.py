@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import ctypes
 import math
-from ctypes import byref, c_double, c_float, c_int, c_int64, c_size_t, c_void_p
+from ctypes import byref, c_double, c_float, c_int, c_size_t
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -116,48 +116,25 @@ def synthetic_clip_state_dict(cfg: CLIPTextConfig, seed: int = 777, device="cpu"
     return sd
 
 
-class NativeCLIPTextEncoder:
+class NativeCLIPTextEncoder(nv.NativeHandle):
     """Owner of one `cfgpp_clip_handle`. `encode(ids, skip)` returns (hidden_states[L - skip], last_hidden_state,
     pooled): the three tensors the reference reads from the transformers output object."""
 
+    _prefix, _what = "_clip", "text encoder"
+
     def __init__(self, cfg: CLIPTextConfig, state_dict: Dict[str, torch.Tensor], device="cuda:0"):
         self.cfg = cfg
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise nv.NativeError("the cfgpp_b200 text encoder runs on CUDA (sm_90a) only; use the oracle for CPU runs")
-        idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        self.device = torch.device("cuda", idx)
-        self.lib = nv.load()
-        self._h = c_void_p()
-        desc = to_clip_desc(cfg)
-        with torch.cuda.device(self.device):
-            nv.check(self.lib.cfgpp_clip_create(byref(desc), c_int(idx), byref(self._h)))
-            st = nv.stream_ptr()
+
+        def weights():
             for key, shape, _ in clip_param_specs(cfg):
                 if key not in state_dict:
                     raise KeyError(f"CLIP text state dict lacks '{key}'")
-                w = state_dict[key].detach().to(self.device).contiguous()
+                w = state_dict[key]
                 if tuple(w.shape) != tuple(shape):
                     raise ValueError(f"{key}: shape {tuple(w.shape)} != {tuple(shape)}")
-                if w.dtype not in (torch.float16, torch.float32):
-                    w = w.float()
-                cshape = (c_int64 * w.dim())(*w.shape)
-                nv.check(self.lib.cfgpp_clip_load_weight(self._h, key.encode(), nv.ptr(w), cshape, c_int(w.dim()),
-                                                         c_int(0 if w.dtype == torch.float16 else 1), st))
-                del w
-            torch.cuda.synchronize(self.device)
-            nv.check(self.lib.cfgpp_clip_finalize_weights(self._h, st))
+                yield key, (w if w.dtype in (torch.float16, torch.float32) else w.float())
 
-    def close(self):
-        if self._h:
-            self.lib.cfgpp_clip_destroy(self._h)
-            self._h = c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:  # noqa: BLE001
-            pass
+        self._open(to_clip_desc(cfg), weights(), device)
 
     def pooled_index(self, ids: torch.Tensor) -> torch.Tensor:
         """transformers' pooling row (modeling_clip.CLIPTextTransformer.forward)."""

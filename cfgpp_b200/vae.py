@@ -15,7 +15,7 @@ from __future__ import annotations
 import ctypes
 import math
 import warnings
-from ctypes import byref, c_double, c_float, c_int, c_int64, c_size_t, c_void_p
+from ctypes import byref, c_double, c_float, c_int, c_size_t
 from dataclasses import dataclass
 from typing import Dict, List, Tuple
 
@@ -168,52 +168,29 @@ def synthetic_vae_state_dict(cfg: VAEConfig, seed: int = 4242, device="cpu", dty
     return sd
 
 
-class NativeVAEDecoder:
+class NativeVAEDecoder(nv.NativeHandle):
     """Owner of one `cfgpp_vae_handle`. `decode(zt)` has the contract of the reference's `SDXL.decode` /
     `StableDiffusion.decode`: it takes the SCALED latent and returns `vae.decode(zt / scaling_factor).sample.float()`."""
 
+    _prefix, _what = "_vae", "VAE decoder"
+
     def __init__(self, cfg: VAEConfig, state_dict: Dict[str, torch.Tensor], device="cuda:0"):
         self.cfg = cfg
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise nv.NativeError("the cfgpp_b200 VAE decoder runs on CUDA (sm_90a) only; use the oracle for CPU runs")
-        idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        self.device = torch.device("cuda", idx)
-        self.lib = nv.load()
-        self._h = c_void_p()
-        desc = to_vae_desc(cfg)
-        with torch.cuda.device(self.device):
-            nv.check(self.lib.cfgpp_vae_create(byref(desc), c_int(idx), byref(self._h)))
-            st = nv.stream_ptr()
-            self.has_encoder = "encoder.conv_in.weight" in state_dict
-            specs = vae_decoder_param_specs(cfg) + (vae_encoder_param_specs(cfg) if self.has_encoder else [])
+        self.has_encoder = "encoder.conv_in.weight" in state_dict
+        specs = vae_decoder_param_specs(cfg) + (vae_encoder_param_specs(cfg) if self.has_encoder else [])
+
+        def weights():
             for key, _, _ in specs:
                 if key not in state_dict:
                     raise KeyError(f"VAE state dict lacks '{key}'")
-                w = state_dict[key].detach().to(self.device).contiguous()
-                if w.dtype not in (torch.float16, torch.float32):
-                    w = w.float()
-                shape = (c_int64 * w.dim())(*w.shape)
-                nv.check(self.lib.cfgpp_vae_load_weight(self._h, key.encode(), nv.ptr(w), shape, c_int(w.dim()),
-                                                        c_int(0 if w.dtype == torch.float16 else 1), st))
-                del w
-            torch.cuda.synchronize(self.device)
-            nv.check(self.lib.cfgpp_vae_finalize_weights(self._h, st))
+                w = state_dict[key]
+                yield key, (w if w.dtype in (torch.float16, torch.float32) else w.float())
+
+        self._open(to_vae_desc(cfg), weights(), device)
 
     @property
     def scale_factor(self) -> int:
         return 2 ** (len(self.cfg.block_out_channels) - 1)
-
-    def close(self):
-        if self._h:
-            self.lib.cfgpp_vae_destroy(self._h)
-            self._h = c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:  # noqa: BLE001
-            pass
 
     def decode_fp16(self, zt: torch.Tensor) -> torch.Tensor:
         assert zt.dim() == 4 and zt.shape[1] == 4, "latent must be (B,4,h,w)"
