@@ -1,14 +1,18 @@
 // cfgpp_b200 — persistent, warp-specialised wgmma GEMM / implicit-GEMM conv3x3 kernel for sm_90a.
 // See gemm.cuh for the operator contract. Structure per CTA (384 threads = 3 warpgroups, 1 CTA / SM, persistent over
 // tiles):
-//   warpgroups 0, 1 : MMA + epilogue. Warpgroup g owns rows [64 g, 64 g + 64) of the 128 x BN tile: wgmma m64nBNk16
-//                     from the shared-memory ring into a register accumulator, then bias / addend / GEGLU / LN-fold ->
-//                     fp16 into a swizzled smem staging tile -> TMA store. Warp w of the group owns 16 rows end to end.
-//   warp 8          : TMA producer (A tile 128x64, B tile BNx64 per stage, 128B swizzle, mbarrier complete_tx); the
-//                     rest of warpgroup 2 idles. The producer warpgroup hands registers to the MMA warpgroups
-//                     (setmaxnreg), which hold up to 128 fp32 accumulator registers per thread.
-// Pipeline: smem ring full/empty (TMA <-> MMA); the producer runs ahead into the next tile while the epilogue of the
-// current one runs.
+//   warpgroups 0, 1 : MMA + epilogue arithmetic. Warpgroup g owns rows [64 g, 64 g + 64) of the 128 x BN tile: wgmma
+//                     m64nBNk16 from the shared-memory ring into a register accumulator, then bias / addend / GEGLU /
+//                     LN-fold -> fp16 into a swizzled smem staging tile, from vectors already in shared memory; then
+//                     straight on to the next tile's main loop. Warp w of the group owns 16 rows end to end.
+//   warp 8, lane 0  : TMA producer (A tile 128x64, B tile BNx64 per stage, 128B swizzle, mbarrier complete_tx).
+//   warps 9 .. 11   : epilogue service, off the MMA warps' critical path: they stage the per-tile vectors (bias,
+//                     time-embedding row, LN-fold s_n / t_n and the fold's per-row sums) two tiles ahead from global
+//                     memory, and lanes 0..7 of warp 9 issue the staged tile's TMA stores, wait for their read-out and
+//                     prefetch the next tile's residual into the staging tile.
+// Warpgroup 2 hands registers to the MMA warpgroups (setmaxnreg), which hold up to 128 fp32 accumulator registers per
+// thread. Pipeline: smem ring full/empty (TMA <-> MMA); staging tile staged/free (MMA <-> store lanes); vector buffers
+// vec per parity (service warps -> MMA; the tile's staged arrival hands the buffer back).
 #include <algorithm>
 #include <cstdlib>
 #include <type_traits>
@@ -27,6 +31,8 @@ constexpr int BK = 64;
 constexpr int kThreads = 384;
 constexpr int kEpiWarps = 8;      // warps 0..7: MMA + epilogue (warpgroups 0 and 1)
 constexpr int kProducerWarp = 8;
+constexpr int kSvcWarp0 = 9;      // warps 9..11: epilogue service (vector staging, TMA stores)
+constexpr int kSvcThreads = 3 * 32;
 constexpr int A_BYTES = BM * BK * 2;
 constexpr int kSkMaxCtas = 256;            // stream-K: flags[c] arrivals, flags[kSkDoneOffset + c] consumers
 constexpr int kSkDoneOffset = kSkMaxCtas;
@@ -41,9 +47,10 @@ struct Cfg {
   static constexpr int EPI_SUB_BYTES = BM * 64;
   static constexpr int EPI_BYTES = EPI_SUB * EPI_SUB_BYTES;
   static constexpr int STAGES = GEGLU ? 3 : (BN == 256 ? 3 : (BN == 160 ? 4 : 5));
-  // per-tile vectors staged for the epilogue: bias + time-embedding row (fp16), LayerNorm-fold s_n / t_n (fp32)
-  static constexpr int VEC_ONE = 2 * 256 * 2 + 2 * 256 * 4;
-  static constexpr int VEC_BYTES = 2 * VEC_ONE;  // double-buffered by tile parity
+  // per-tile vectors staged for the epilogue: bias + time-embedding row (fp16), LayerNorm-fold s_n / t_n (fp32), and
+  // the LayerNorm fold's per-row (sum, sum of squares) of the tile's 128 rows (float2)
+  static constexpr int VEC_ONE = 2 * 256 * 2 + 2 * 256 * 4 + BM * 8;
+  static constexpr int VEC_BYTES = 2 * VEC_ONE;  // double-buffered by epilogue-tile parity
   static constexpr int SMEM_BYTES =
       STAGES * STAGE_BYTES + EPI_BYTES + VEC_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB shared memory of an SM");
@@ -62,11 +69,17 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
 
   uint8_t* epi_smem = smem + C::STAGES * C::STAGE_BYTES;
-  uint8_t* vec_smem = epi_smem + C::EPI_BYTES;  // 2 x { bias[256] fp16, temb[256] fp16, ln_s[256] fp32, ln_t[256] fp32 }
+  // 2 x { bias[256] fp16, temb[256] fp16, ln_s[256] fp32, ln_t[256] fp32, ln_sum[128] float2 }
+  uint8_t* vec_smem = epi_smem + C::EPI_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(epi_smem + C::EPI_BYTES + C::VEC_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + C::STAGES;
-  uint64_t* res_bar = bars + 2 * C::STAGES;  // [kEpiWarps]: each epilogue warp loads its own residual sub-blocks
+  uint64_t* res_bar = bars + 2 * C::STAGES;  // [kEpiWarps]: the residual sub-blocks of each epilogue warp's 16 rows
+  // [2] by epilogue-tile parity: every MMA thread has written its part of the staging tile and read the tile's vectors
+  // (two barriers, so a service warp that lags one tile behind can never mistake the next phase for the one it waits on)
+  uint64_t* staged_bar = res_bar + kEpiWarps;
+  uint64_t* free_bar = staged_bar + 2;  // the store lanes have read the staging tile out (and issued the next residual)
+  uint64_t* vec_bar = free_bar + 1;     // [2] by parity: the service warps have staged that buffer's vectors
 
   const int warp_idx = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);  // provably warp-uniform
   const int lane = threadIdx.x & 31;
@@ -87,6 +100,11 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
       mbar_init(&empty_bar[i], kEpiWarps);  // one arrive per consumer warp once its wgmmas on the stage retired
     }
     for (int i = 0; i < kEpiWarps; ++i) mbar_init(&res_bar[i], 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&staged_bar[i], kEpiWarps * 32);
+      mbar_init(&vec_bar[i], kSvcThreads);
+    }
+    mbar_init(free_bar, kEpiWarps);  // one store lane per epilogue warp's slab
     fence_barrier_init();
   }
   __syncthreads();
@@ -181,9 +199,121 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
   // partial accumulator of CTA c: [BN / 4 register pairs][256 consumer threads] float2 (the register fragment order)
   auto sk_ws = [&](int c) { return p.sk_ws + static_cast<size_t>(c) * (static_cast<size_t>(BM) * BN); };
 
+  // ---- epilogue tiles: every item except the stream-K pieces that only park a partial ----------------------------
+  static_assert((2 * C::STAGES + kEpiWarps + 5) * 8 <= 256, "barrier area");
+  auto next_epi_item = [&](int from) {
+    int i = from;
+    while (i < n_items && item_at(i).kind == kItemPart) ++i;
+    return i;
+  };
+  const bool full_res = (p.addend != nullptr) && (p.add_rows_per_group <= 1);
+  // a time-embedding row is staged in shared memory when all of the tile's rows belong to one sample
+  auto temb_staged_for = [&](int m_blk) {
+    const int m_first = m_blk * BM;
+    const int m_last = (m_first + BM - 1 < p.M ? m_first + BM - 1 : p.M - 1);
+    return p.addend != nullptr && !full_res && (m_first < p.M) &&
+           (m_first / p.add_rows_per_group == m_last / p.add_rows_per_group);
+  };
+  auto vec_bias = [&](int parity) { return reinterpret_cast<__half*>(vec_smem + parity * C::VEC_ONE); };  // [256]
+  auto vec_temb = [&](int parity) { return vec_bias(parity) + 256; };                                       // [256]
+  auto vec_lns = [&](int parity) { return reinterpret_cast<float*>(vec_temb(parity) + 256); };             // [256]
+  auto vec_lnt = [&](int parity) { return vec_lns(parity) + 256; };                                        // [256]
+  auto vec_lnsum = [&](int parity) { return reinterpret_cast<float2*>(vec_lnt(parity) + 256); };           // [128]
+  // residual sub-blocks of epilogue warp w's 16 rows, into its slab of the staging tile (one lane)
+  auto issue_residual = [&](int tile, int w) {
+    const int m_blk = tile_m_blk(tile);
+    const int n_blk = tile_n_blk(tile);
+    mbar_arrive_expect_tx(&res_bar[w], C::EPI_SUB * 16 * 64);
+#pragma unroll 1
+    for (int j = 0; j < C::EPI_SUB; ++j)
+      tma_load_2d(epi_smem + w * 16 * 64 + j * C::EPI_SUB_BYTES, &map_res, &res_bar[w], n_blk * C::OUT_N + j * 32,
+                  m_blk * BM + w * 16);
+  };
+
   if (warp_idx >= kEpiWarps) {
     setmaxnreg_dec<40>();
-    if (warp_idx == kProducerWarp && lane == 0) {
+    if (warp_idx >= kSvcWarp0) {
+      // ===================== epilogue service =====================
+      const int st = threadIdx.x - kSvcWarp0 * 32;  // 0 .. kSvcThreads - 1
+      // Stage the vectors of the tile's epilogue into buffer `parity`: bias (and, when all 128 rows belong to one
+      // sample, its time-embedding row), the fold's s_n / t_n, and the rows' (sum, sum of squares) from the producer's
+      // per-N-block partials, summed in a fixed order.
+      auto stage_vectors = [&](int tile, int parity) {
+        const int m_blk = tile_m_blk(tile);
+        const int n_blk = tile_n_blk(tile);
+        __half* s_bias = vec_bias(parity);
+        __half* s_temb = vec_temb(parity);
+        float* s_lns = vec_lns(parity);
+        float* s_lnt = vec_lnt(parity);
+        const bool temb = temb_staged_for(m_blk);
+        const __half* temb_row = p.addend + (temb ? static_cast<size_t>(m_blk * BM / p.add_rows_per_group) * p.ld_add : 0);
+        const int ncols = GEGLU ? BN : C::OUT_N;  // GEGLU stages value + gate biases (packed alike)
+        const int n_base = n_blk * BN;
+        for (int c = st; c < ncols; c += kSvcThreads) {
+          const int n = n_base + c;
+          const bool ok = n < p.N;
+          s_bias[c] = (p.bias && ok) ? p.bias[n] : __float2half(0.f);
+          if (temb) s_temb[c] = ok ? temb_row[n] : __float2half(0.f);
+          if (p.stats_in) {
+            s_lns[c] = ok ? p.ln_s[n] : 0.f;
+            s_lnt[c] = ok ? p.ln_t[n] : 0.f;
+          }
+        }
+        if (p.stats_in) {
+          float2* s_sum = vec_lnsum(parity);
+          for (int r = st; r < BM; r += kSvcThreads) {
+            const int m = m_blk * BM + r;
+            if (m >= p.M) continue;
+            float sx = 0.f, sxx = 0.f;
+            for (int i = 0; i < p.ln_parts; ++i) {
+              const float2 v = *reinterpret_cast<const float2*>(p.stats_in + (static_cast<size_t>(i) * p.M + m) * 2);
+              sx += v.x;
+              sxx += v.y;
+            }
+            s_sum[r] = make_float2(sx, sxx);
+          }
+        }
+        mbar_arrive(&vec_bar[parity]);
+      };
+      const int i0 = next_epi_item(0);
+      const int i1 = i0 < n_items ? next_epi_item(i0 + 1) : n_items;
+      if (full_res && warp_idx == kSvcWarp0 && lane < kEpiWarps && i0 < n_items) issue_residual(item_at(i0).tile, lane);
+      if (i0 < n_items) stage_vectors(item_at(i0).tile, 0);
+      if (i1 < n_items) stage_vectors(item_at(i1).tile, 1);
+      int ahead = i1 < n_items ? next_epi_item(i1 + 1) : n_items;  // the epilogue tile two after the current one
+      int e = 0;                                                    // epilogue tiles done
+      for (int i = i0; i < n_items; ++e) {
+        const int nx = next_epi_item(i + 1);
+        mbar_wait_nocall(&staged_bar[e & 1], (e >> 1) & 1);
+        if (warp_idx == kSvcWarp0 && lane < kEpiWarps) {
+          if (lane == 0) TL(14);
+          // lane w stores epilogue warp w's [16 x OUT_N] slab, then refills it with the next tile's residual
+          const int tile = item_at(i).tile;
+          const int m_blk = tile_m_blk(tile);
+          const int n_blk = tile_n_blk(tile);
+#pragma unroll 1
+          for (int j = 0; j < C::EPI_SUB; ++j)
+            tma_store_2d(&map_out, epi_smem + lane * 16 * 64 + j * C::EPI_SUB_BYTES, n_blk * C::OUT_N + j * 32,
+                         m_blk * BM + lane * 16);
+          tma_store_commit();
+          if (lane == 0) {
+            if (e == 0) TL(8);
+            TL(10);
+          }
+          tma_store_wait_read0();
+          if (full_res && nx < n_items) issue_residual(item_at(nx).tile, lane);
+          mbar_arrive(free_bar);
+          if (lane == 0) TL(15);
+        }
+        if (ahead < n_items) {  // the MMA threads are done with buffer e & 1: refill it for tile e + 2
+          stage_vectors(item_at(ahead).tile, e & 1);
+          ahead = next_epi_item(ahead + 1);
+        }
+        i = nx;
+      }
+      if (warp_idx == kSvcWarp0 && lane < kEpiWarps) tma_store_wait0();
+      if (warp_idx == kSvcWarp0 && lane == 0) TL(11);
+    } else if (lane == 0) {
       // ===================== TMA producer =====================
       int stage = 0;
       uint32_t phase = 0;
@@ -244,30 +374,10 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
     const int cq = 2 * (lane & 3);                // column offset inside an 8-column group
     const int etid = threadIdx.x;                 // 0..255
     const bool leader = (threadIdx.x == 0);
-    const bool full_res = (p.addend != nullptr) && (p.add_rows_per_group <= 1);
-    uint8_t* my_slab = epi_smem + slab_row * 64;  // + j * EPI_SUB_BYTES: this warp's [16 x 64 B] block of sub-tile j
     uint64_t* my_res_bar = &res_bar[warp_idx];
     // byte offset of (tile row r, 8-column group q of a 32-column sub-tile) in the 64B-swizzled staging sub-tile
     auto stage_off = [&](int r, int q) { return r * 64 + ((q ^ ((r >> 1) & 3)) << 4) + (lane & 3) * 4; };
-    auto issue_residual = [&](int tile) {  // one lane
-      const int m_blk = tile_m_blk(tile);
-      const int n_blk = tile_n_blk(tile);
-      mbar_arrive_expect_tx(my_res_bar, C::EPI_SUB * 16 * 64);
-#pragma unroll 1
-      for (int j = 0; j < C::EPI_SUB; ++j)
-        tma_load_2d(my_slab + j * C::EPI_SUB_BYTES, &map_res, my_res_bar, n_blk * C::OUT_N + j * 32,
-                    m_blk * BM + slab_row);
-    };
-    // residual tiles are prefetched one item ahead; stream-K pieces that only park a partial take none
-    auto next_res_item = [&](int from) {
-      int i = from;
-      while (i < n_items && item_at(i).kind == kItemPart) ++i;
-      return i;
-    };
-    if (full_res && lane == 0) {
-      const int i0 = next_res_item(0);
-      if (i0 < n_items) issue_residual(item_at(i0).tile);
-    }
+    int ep = 0;  // epilogue tiles done
     int res_uses = 0;
     int stage = 0;
     uint32_t phase = 0;
@@ -330,6 +440,7 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
     for (int it = 0; it < n_items; ++it) {
       const Item item = item_at(it);
       const int tile = item.tile;
+      if (leader && ep == 1) TL(6);
       // ---- main loop: wgmma over the smem ring, one k-block kept in flight ----
       // a finishing stream-K piece starts from the other pieces' partial sum, every other item from zero (scale-d 0)
       const bool preloaded = item.kind == kItemFin;
@@ -370,51 +481,34 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
       const int m_blk = tile_m_blk(tile);
       const int n_blk = tile_n_blk(tile);
       const int mrow[2] = {m_blk * BM + r0, m_blk * BM + r0 + 8};
-      __half* s_bias = reinterpret_cast<__half*>(vec_smem + (it & 1) * C::VEC_ONE);  // [256]
-      __half* s_temb = s_bias + 256;                                                  // [256]
-      float* s_lns = reinterpret_cast<float*>(s_temb + 256);                          // [256]
-      float* s_lnt = s_lns + 256;                                                     // [256]
-      // Stage this tile's bias (and, when all 128 rows belong to one sample, its time-embedding row) in shared memory.
-      // The buffers alternate with the tile parity, so a warp that runs ahead never overwrites vectors still being read.
+      const int vb = ep & 1;
+      if (leader) {
+        if (ep == 0) TL(5);
+        TL(7);
+      }
+      const __half* s_bias = vec_bias(vb);
+      const __half* s_temb = vec_temb(vb);
+      const float* s_lns = vec_lns(vb);
+      const float* s_lnt = vec_lnt(vb);
       const __half* add_rows[2] = {nullptr, nullptr};  // per-sample row broadcast (ResnetBlock2D time embedding)
-      bool temb_staged = false;
-      if (p.addend != nullptr && !full_res) {
-        const int m_first = m_blk * BM;
-        const int m_last = (m_first + BM - 1 < p.M ? m_first + BM - 1 : p.M - 1);
-        temb_staged = (m_first < p.M) && (m_first / p.add_rows_per_group == m_last / p.add_rows_per_group);
+      const bool temb_staged = temb_staged_for(m_blk);
+      if (p.addend != nullptr && !full_res && !temb_staged) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int mm = mrow[h] < p.M ? mrow[h] : p.M - 1;
           add_rows[h] = p.addend + static_cast<size_t>(mm / p.add_rows_per_group) * p.ld_add;
         }
-        if (temb_staged) add_rows[0] = add_rows[1] = p.addend + static_cast<size_t>(m_first / p.add_rows_per_group) * p.ld_add;
       }
-      {
-        const int ncols = GEGLU ? BN : C::OUT_N;  // GEGLU stages value + gate biases (packed alike)
-        const int n_base = n_blk * BN;
-        for (int c = etid; c < ncols; c += kEpiWarps * 32) {
-          const int n = n_base + c;
-          const bool ok = n < p.N;
-          s_bias[c] = (p.bias && ok) ? p.bias[n] : __float2half(0.f);
-          if (temb_staged) s_temb[c] = ok ? add_rows[0][n] : __float2half(0.f);
-          if (p.stats_in) {
-            s_lns[c] = ok ? p.ln_s[n] : 0.f;
-            s_lnt[c] = ok ? p.ln_t[n] : 0.f;
-          }
-        }
-      }
-      // LayerNorm fold: the rows' mean / rstd from the producer's per-N-block partial sums (fixed order)
+      mbar_wait_nocall(&vec_bar[vb], (ep >> 1) & 1);  // the service warps have staged this tile's vectors
+      // LayerNorm fold: the rows' mean / rstd from their (sum, sum of squares)
       float ln_rstd[2] = {1.f, 1.f}, ln_rm[2] = {0.f, 0.f};
       if (p.stats_in) {
+        const float2* s_sum = vec_lnsum(vb);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           if (mrow[h] >= p.M) continue;
-          float sx = 0.f, sxx = 0.f;
-          for (int i = 0; i < p.ln_parts; ++i) {
-            const float2 v = *reinterpret_cast<const float2*>(p.stats_in + (static_cast<size_t>(i) * p.M + mrow[h]) * 2);
-            sx += v.x;
-            sxx += v.y;
-          }
+          const float2 v = s_sum[r0 + 8 * h];
+          const float sx = v.x, sxx = v.y;
           const float mean = sx * p.ln_inv_c;
           const float var = fmaxf(sxx * p.ln_inv_c - mean * mean, 0.f);
           ln_rstd[h] = rsqrtf(var + p.ln_eps);
@@ -423,9 +517,12 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
       }
       // producer side: partial row statistics [row h][column half] of this thread's columns of the tile
       float ps[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, pss[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
-      named_bar_sync(1, kEpiWarps * 32);  // staged vectors visible to all epilogue threads
-      if (leader) { TL(9); if (tl) tl[12] = it + 1; }
+      if (ep > 0) mbar_wait_nocall(free_bar, (ep - 1) & 1);  // the previous tile has been read out of the staging tile
       if (full_res) mbar_wait_nocall(my_res_bar, (res_uses++) & 1);
+      if (leader) {
+        TL(9);
+        if (tl) tl[12] = it + 1;
+      }
 
       // The arithmetic variant (LayerNorm fold / kind of addend / row statistics) is chosen ONCE per tile and the chunk
       // loop is instantiated per variant, so the unrolled loop carries no per-element branches on them.
@@ -547,20 +644,8 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
           chunks(std::false_type{});
       }
       fence_proxy_async_smem();  // this thread's part of the staging tile -> visible to the TMA engine
-      __syncwarp();
-      if (lane == 0) {
-#pragma unroll 1
-        for (int j = 0; j < C::EPI_SUB; ++j)
-          tma_store_2d(&map_out, my_slab + j * C::EPI_SUB_BYTES, n_blk * C::OUT_N + j * 32, m_blk * BM + slab_row);
-        tma_store_commit();
-        if (leader) { if (it == 0) TL(8); TL(10); }
-        tma_store_wait_read0();  // this warp's staging blocks have been read out: reusable
-        if (full_res) {
-          const int nx = next_res_item(it + 1);
-          if (nx < n_items) issue_residual(item_at(nx).tile);
-        }
-      }
-      __syncwarp();
+      mbar_arrive(&staged_bar[vb]);  // (and this thread is done with the tile's vectors): the store lanes take over
+      if (leader) TL(13);
       if constexpr (!GEGLU) {
         if (p.stats_out) {  // quad reduction (the four lanes of a row), then one float2 per row and column half
 #pragma unroll
@@ -581,9 +666,8 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
           }
         }
       }
+      ++ep;
     }
-    if (lane == 0) tma_store_wait0();
-    if (leader) TL(11);
   }
 #undef TL
 }
