@@ -95,7 +95,7 @@ class NativeHandle:
         self.lib = load()
         self._h = c_void_p()
         with torch.cuda.device(self.device):
-            check(self._entry("create")(ctypes.byref(desc), c_int(idx), ctypes.byref(self._h)))
+            self._create(desc, idx)
             st = stream_ptr()
             for key, w in weights:
                 w = w.detach().to(self.device).contiguous()
@@ -105,6 +105,9 @@ class NativeHandle:
                 del w
             torch.cuda.synchronize(self.device)
             check(self._entry("finalize_weights")(self._h, st))
+
+    def _create(self, desc: ctypes.Structure, idx: int) -> None:
+        check(self._entry("create")(ctypes.byref(desc), c_int(idx), ctypes.byref(self._h)))
 
     def close(self):
         if getattr(self, "_h", None):
@@ -441,6 +444,42 @@ def op_conv_out_step(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, metho
                                      ptr(z), ptr(aux), ptr(z0t), ptr(eps_uc), ptr(eps_c), ptr(noise), ptr(lambdas),
                                      stream_ptr()))
     return eps_uc, eps_c, z0t
+
+
+def op_conv_out_step_v(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, method: int, coef, z: torch.Tensor,
+                       a: float, b: float, in_scale: torch.Tensor | None = None, aux: torch.Tensor | None = None,
+                       want_z0t: bool = True, noise: torch.Tensor | None = None, lambdas: torch.Tensor | None = None):
+    """op_conv_out_step for a v-prediction model: the conv outputs are v (returned as they are) and become
+    eps = fp16(fp32(a v) + fp32(b x_in)) before the step, x_in = z * in_scale (fp32 [1] device scalar, or None) as
+    conv_in forms the UNet input. Returns (v_uc, v_c, z0t or None)."""
+    from ctypes import byref
+    lib = load()
+    B2, H, W, Cin = x.shape
+    B = B2 // 2
+    assert B2 == 2 * B and w.shape == (4, 9, Cin) and method != 0 and z.shape == (B, 4, H, W)
+    assert in_scale is None or (in_scale.dtype == torch.float32 and in_scale.numel() == 1)
+    v_uc = torch.empty((B, 4, H, W), dtype=torch.float16, device=x.device)
+    v_c = torch.empty_like(v_uc)
+    z0t = torch.empty_like(z) if want_z0t else None
+    if lambdas is not None:
+        assert lambdas.dtype == torch.float32 and lambdas.shape == (B,)
+    check(lib.cfgpp_op_conv_out_step_v(ptr(x), ptr(w), ptr(bias), c_int(B), c_int(H), c_int(W), c_int(Cin),
+                                       c_int(method), c_int(dtype_code(z)), byref(coef), ptr(z), ptr(aux), ptr(z0t),
+                                       ptr(v_uc), ptr(v_c), ptr(noise), ptr(lambdas), ptr(in_scale), c_float(a),
+                                       c_float(b), stream_ptr()))
+    return v_uc, v_c, z0t
+
+
+def op_v_to_eps(v: torch.Tensor, z: torch.Tensor, a: float, b: float, in_scale: torch.Tensor | None = None):
+    """eps = fp16(fp32(a v) + fp32(b x_in)), x_in = z * in_scale formed as conv_in forms the UNet input; v fp16, z fp16 /
+    fp32 of v's shape."""
+    lib = load()
+    assert v.dtype == torch.float16 and z.shape == v.shape
+    assert in_scale is None or (in_scale.dtype == torch.float32 and in_scale.numel() == 1)
+    eps = torch.empty_like(v)
+    check(lib.cfgpp_op_v_to_eps(ptr(v), ptr(z), c_int(dtype_code(z)), ptr(in_scale), c_float(a), c_float(b), ptr(eps),
+                                c_int(v.numel()), stream_ptr()))
+    return eps
 
 
 def op_upsample2x(x: torch.Tensor) -> torch.Tensor:

@@ -7,10 +7,15 @@
     <dir>/text_encoder/model[.fp16].safetensors      + <dir>/tokenizer/{vocab.json, merges.txt}
     <dir>/text_encoder_2/model[.fp16].safetensors    + <dir>/tokenizer_2/{vocab.json, merges.txt}     (SDXL only)
 
+SD 2.x (family 'sd20') has the SD v1.5 layout; its text_encoder is OpenCLIP ViT-H. `scheduler/scheduler_config.json`
+(prediction_type) and `unet/config.json` (sample_size) are read when present, so the 768^2 v-prediction checkpoints
+(stable-diffusion-2, -2-1) and the 512^2 epsilon ones (-2-base, -2-1-base) both load with the right UNet config.
+
 `solver_components(dir, family, device)` turns it into the keyword arguments of `get_solver(...)`. Nothing can be
 downloaded here; without a directory every component falls back to seeded synthetic weights."""
 from __future__ import annotations
 
+import json
 from pathlib import Path
 from typing import Dict, Optional
 
@@ -24,7 +29,8 @@ def _weights(folder: Path, stems) -> Optional[Path]:
 
 
 def find_pipeline_files(ckpt_dir, family: str) -> Dict[str, Path]:
-    """family: 'sd15' | 'sdxl'. Raises FileNotFoundError naming every missing piece."""
+    """family: 'sd15' | 'sd20' | 'sdxl'. Raises FileNotFoundError naming every missing piece. For 'sd20' the optional
+    config files are included as 'scheduler_config' / 'unet_config' when they exist."""
     root = Path(ckpt_dir)
     want = {"unet": (root / "unet", ("diffusion_pytorch_model",)), "vae": (root / "vae", ("diffusion_pytorch_model",)),
             "text_encoder": (root / "text_encoder", ("model",))}
@@ -32,7 +38,7 @@ def find_pipeline_files(ckpt_dir, family: str) -> Dict[str, Path]:
     if family == "sdxl":
         want["text_encoder_2"] = (root / "text_encoder_2", ("model",))
         toks.append("tokenizer_2")
-    elif family != "sd15":
+    elif family not in ("sd15", "sd20"):
         raise ValueError(f"unknown model family {family!r}")
     found: Dict[str, Path] = {}
     missing = []
@@ -51,7 +57,24 @@ def find_pipeline_files(ckpt_dir, family: str) -> Dict[str, Path]:
                 missing.append(str(p))
     if missing:
         raise FileNotFoundError("pipeline directory is incomplete, missing: " + ", ".join(missing))
+    if family == "sd20":
+        for key, p in (("scheduler_config", root / "scheduler" / "scheduler_config.json"),
+                       ("unet_config", root / "unet" / "config.json")):
+            if p.is_file():
+                found[key] = p
     return found
+
+
+def sd2_unet_config(files: Dict[str, Path]):
+    """The SD 2 UNet config of a pipeline directory: 768^2 v-prediction unless scheduler_config.json / unet/config.json
+    say otherwise (prediction_type, sample_size)."""
+    from .config import sd2_config
+    pred, size = "v_prediction", 96
+    if "scheduler_config" in files:
+        pred = json.loads(files["scheduler_config"].read_text()).get("prediction_type", "epsilon")
+    if "unet_config" in files:
+        size = int(json.loads(files["unet_config"].read_text()).get("sample_size", size))
+    return sd2_config(sample_size=size, prediction_type=pred)
 
 
 def solver_components(ckpt_dir, family: str, device) -> dict:
@@ -70,6 +93,9 @@ def solver_components(ckpt_dir, family: str, device) -> dict:
                             str(f["tokenizer_2/merges.txt"])))
     else:
         kw["vae"] = get_vae("sd15_vae", device, str(f["vae"]))
-        kw["text_encoder"] = get_conditioner("clip_l", device, "sd15", str(f["text_encoder"]),
-                                             str(f["tokenizer/vocab.json"]), str(f["tokenizer/merges.txt"]))
+        kw["text_encoder"] = get_conditioner("clip_h" if family == "sd20" else "clip_l", device, "sd15",
+                                             str(f["text_encoder"]), str(f["tokenizer/vocab.json"]),
+                                             str(f["tokenizer/merges.txt"]))
+        if family == "sd20":
+            kw["unet_config"] = sd2_unet_config(f)
     return kw

@@ -33,6 +33,7 @@ class UNetConfig:
     projection_class_embeddings_input_dim: int = 2816
     pooled_dim: int = 1280
     vae_scale_factor: int = 8
+    prediction_type: str = "epsilon"  # scheduler_config.json: "epsilon" | "v_prediction" (SD 2.0-v / 2.1 at 768^2)
 
     @property
     def time_embed_dim(self) -> int:
@@ -69,7 +70,29 @@ def tiny_sd15_config(sample_size: int = 32) -> UNetConfig:
                       num_attention_heads=(1, 2, 4, 4), cross_attention_dim=128)
 
 
-CONFIGS = {"sd15": sd15_config, "sdxl": sdxl_config, "tiny_sdxl": tiny_sdxl_config, "tiny_sd15": tiny_sd15_config}
+def sd2_config(sample_size: int = 96, prediction_type: str = "v_prediction") -> UNetConfig:
+    """stabilityai/stable-diffusion-2-1 (and 2.0-v): SD v1.5's 4 levels with linear projections, 64-wide heads
+    (diffusers' `attention_head_dim` (5, 10, 20, 20)), OpenCLIP ViT-H context (1024), v-prediction at 768^2."""
+    return UNetConfig(name="sd2" if prediction_type == "v_prediction" else "sd2_base", sample_size=sample_size,
+                      num_attention_heads=(5, 10, 20, 20), cross_attention_dim=1024, use_linear_projection=True,
+                      prediction_type=prediction_type)
+
+
+def sd2_base_config() -> UNetConfig:
+    """stabilityai/stable-diffusion-2-base (and 2.1-base): the SD 2 UNet at 512^2, epsilon prediction."""
+    return sd2_config(sample_size=64, prediction_type="epsilon")
+
+
+def tiny_sd2_config(sample_size: int = 32, prediction_type: str = "v_prediction") -> UNetConfig:
+    """SD 2 topology (4 levels, linear projections, head_dim 64, v-prediction) at test-sized widths."""
+    return UNetConfig(name="tiny_sd2", sample_size=sample_size, block_out_channels=(64, 128, 256, 256),
+                      num_attention_heads=(1, 2, 4, 4), cross_attention_dim=128, use_linear_projection=True,
+                      prediction_type=prediction_type)
+
+
+CONFIGS = {"sd15": sd15_config, "sdxl": sdxl_config, "tiny_sdxl": tiny_sdxl_config, "tiny_sd15": tiny_sd15_config,
+           "sd2": sd2_config, "sd2_base": sd2_base_config, "tiny_sd2": tiny_sd2_config}
+PREDICTION_TYPES = {"epsilon": 0, "v_prediction": 1}
 
 
 class ModelDescC(ctypes.Structure):
@@ -85,8 +108,15 @@ class ModelDescC(ctypes.Structure):
     ]
 
 
-def to_desc(cfg: UNetConfig) -> ModelDescC:
-    d = ModelDescC()
+class ModelDescExC(ModelDescC):
+    """The full `cfgpp_model_desc` (cfgpp_create_ex): ModelDescC, the layout cfgpp_create reads, + prediction_type."""
+    _fields_ = [("prediction_type", ctypes.c_int)]
+
+
+def to_desc(cfg: UNetConfig) -> ModelDescExC:
+    if cfg.prediction_type not in PREDICTION_TYPES:
+        raise ValueError(f"unsupported prediction_type {cfg.prediction_type!r}")
+    d = ModelDescExC()
     n = len(cfg.block_out_channels)
     d.in_channels, d.out_channels, d.num_levels = cfg.in_channels, cfg.out_channels, n
     for i in range(n):
@@ -103,4 +133,5 @@ def to_desc(cfg: UNetConfig) -> ModelDescC:
     d.addition_time_embed_dim = cfg.addition_time_embed_dim if cfg.addition_embed_type == "text_time" else 0
     d.projection_class_embeddings_input_dim = cfg.projection_class_embeddings_input_dim
     d.pooled_dim = cfg.pooled_dim
+    d.prediction_type = PREDICTION_TYPES[cfg.prediction_type]
     return d

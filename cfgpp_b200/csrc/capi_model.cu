@@ -3,6 +3,7 @@
 #include "unet.cuh"
 
 #include <algorithm>
+#include <cstddef>
 #include <cstring>
 
 using namespace cfgpp;
@@ -14,11 +15,19 @@ struct cfgpp_handle {
 
 extern "C" {
 
-CFGPP_API int cfgpp_create(const cfgpp_model_desc* desc, int device, cfgpp_handle** out) {
+CFGPP_API int cfgpp_create_ex(const cfgpp_model_desc* desc, size_t desc_bytes, int device, cfgpp_handle** out) {
   return guarded([&] {
     CFGPP_REQUIRE(desc && out, "null argument");
-    *out = new cfgpp_handle(*desc, device);
+    constexpr size_t legacy = offsetof(cfgpp_model_desc, prediction_type);
+    CFGPP_REQUIRE(desc_bytes == legacy || desc_bytes == sizeof(cfgpp_model_desc), "unknown cfgpp_model_desc size");
+    cfgpp_model_desc d{};  // fields the caller's layout does not have stay 0 (prediction_type: epsilon)
+    memcpy(&d, desc, desc_bytes);
+    *out = new cfgpp_handle(d, device);
   });
+}
+
+CFGPP_API int cfgpp_create(const cfgpp_model_desc* desc, int device, cfgpp_handle** out) {
+  return cfgpp_create_ex(desc, offsetof(cfgpp_model_desc, prediction_type), device, out);
 }
 
 CFGPP_API int cfgpp_destroy(cfgpp_handle* h) {
@@ -87,6 +96,10 @@ CFGPP_API int cfgpp_set_noise(cfgpp_handle* h, const void* noise_dev, int slots,
 
 CFGPP_API int cfgpp_set_guidance(cfgpp_handle* h, const float* lambda_host, int n, void* stream) {
   return guarded([&] { h->unet.set_guidance(lambda_host, n, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_set_v_coefs(cfgpp_handle* h, const float* ab_host, int nsteps, void* stream) {
+  return guarded([&] { h->unet.set_v_coefs(ab_host, nsteps, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_run_steps(cfgpp_handle* h, int first_step, int nsteps, void* stream) {

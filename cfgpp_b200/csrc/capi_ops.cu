@@ -166,24 +166,28 @@ namespace {
 // Runs one step launch `launch(coef_dev, noise_slot, lambda_slot)` with the coefficients (zeros when coef_host is null)
 // and the two table words (noise, guidance) in a scratch device block, then synchronises and frees the block.
 // lambda_slot is null when there is no guidance table.
+// v_ab (may be null): the (a, b) pair of a v-prediction step, stored behind the table words; the launch receives its
+// device copy (null without it) as a fourth argument.
 template <class Launch>
 void with_step_block(const cfgpp_step_coef* coef_host, const void* noise_dev, const float* lambda_dev,
-                     cudaStream_t stream, Launch&& launch) {
+                     cudaStream_t stream, Launch&& launch, const float* v_ab = nullptr) {
   static_assert(sizeof(cfgpp_step_coef) == sizeof(StepCoef), "ABI struct mismatch");
   static_assert(sizeof(StepCoef) % sizeof(void*) == 0, "the table words are stored right behind the coefficients");
   const StepCoef zero{};
   const void* coef_src = coef_host ? static_cast<const void*>(coef_host) : static_cast<const void*>(&zero);
   StepCoef* coef_dev = nullptr;
-  CFGPP_CHECK_CUDA(cudaMalloc(&coef_dev, sizeof(StepCoef) + 2 * sizeof(void*)));
+  CFGPP_CHECK_CUDA(cudaMalloc(&coef_dev, sizeof(StepCoef) + 2 * sizeof(void*) + sizeof(float2)));
   const __half** slot = reinterpret_cast<const __half**>(coef_dev + 1);
   const float** lslot = reinterpret_cast<const float**>(slot + 1);
+  float2* vslot = reinterpret_cast<float2*>(lslot + 1);
   cudaError_t e = cudaMemcpy(coef_dev, coef_src, sizeof(StepCoef), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(slot, &noise_dev, sizeof(void*), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(lslot, &lambda_dev, sizeof(void*), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && v_ab) e = cudaMemcpy(vslot, v_ab, sizeof(float2), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) {
     try {
       launch(const_cast<const StepCoef*>(coef_dev), const_cast<const __half* const*>(slot),
-             lambda_dev ? const_cast<const float* const*>(lslot) : nullptr);
+             lambda_dev ? const_cast<const float* const*>(lslot) : nullptr, v_ab ? vslot : nullptr);
     } catch (...) {
       cudaFree(coef_dev);
       throw;
@@ -202,7 +206,7 @@ void op_step(const void* eps_uc, const void* eps_c, int n, int method, int state
   CFGPP_REQUIRE(!guided || (batch >= 1 && n % batch == 0), "guidance table: batch must divide n");
   CFGPP_REQUIRE(coef_host != nullptr, "the step needs its coefficients");
   with_step_block(coef_host, noise_dev, lambda_dev, stream,
-                  [&](const StepCoef* coef_dev, const __half* const* slot, const float* const* lslot) {
+                  [&](const StepCoef* coef_dev, const __half* const* slot, const float* const* lslot, const float2*) {
                     run_step_only((const __half*)eps_uc, (const __half*)eps_c, n,
                                   method | (state_dtype == CFGPP_F16 ? 0x100 : 0), coef_dev, z, aux, z0t_out, stream,
                                   slot, lslot, guided ? n / batch : 0);
@@ -269,11 +273,41 @@ CFGPP_API int cfgpp_op_conv_out_step(const void* x, const void* w, const void* b
     CFGPP_REQUIRE(method == CFGPP_STEP_NONE || coef_host != nullptr, "a step method needs its coefficients");
     const cudaStream_t st = (cudaStream_t)stream;
     with_step_block(coef_host, noise_dev, lambda_dev, st,
-                    [&](const StepCoef* coef_dev, const __half* const* slot, const float* const* lslot) {
+                    [&](const StepCoef* coef_dev, const __half* const* slot, const float* const* lslot,
+                        const float2*) {
                       run_conv_out_step((const __half*)x, (const __half*)w, (const __half*)bias, B, H, W, Cin,
                                         method | (state_dtype == CFGPP_F16 ? 0x100 : 0), coef_dev, z, aux, z0t_out,
                                         (__half*)eps_uc, (__half*)eps_c, st, slot, lslot);
                     });
+  });
+}
+
+CFGPP_API int cfgpp_op_conv_out_step_v(const void* x, const void* w, const void* bias, int B, int H, int W, int Cin,
+                                       int method, int state_dtype, const cfgpp_step_coef* coef_host, void* z,
+                                       void* aux, void* z0t_out, void* eps_uc, void* eps_c, const void* noise_dev,
+                                       const float* lambda_dev, const float* in_scale_dev, float a, float b,
+                                       void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(method != CFGPP_STEP_NONE && coef_host != nullptr && z != nullptr,
+                  "the v conversion belongs to a step: method, coefficients and state");
+    const cudaStream_t st = (cudaStream_t)stream;
+    const float ab[2] = {a, b};
+    with_step_block(
+        coef_host, noise_dev, lambda_dev, st,
+        [&](const StepCoef* coef_dev, const __half* const* slot, const float* const* lslot, const float2* vab) {
+          run_conv_out_step((const __half*)x, (const __half*)w, (const __half*)bias, B, H, W, Cin,
+                            method | (state_dtype == CFGPP_F16 ? 0x100 : 0), coef_dev, z, aux, z0t_out,
+                            (__half*)eps_uc, (__half*)eps_c, st, slot, lslot, vab, in_scale_dev);
+        },
+        ab);
+  });
+}
+
+CFGPP_API int cfgpp_op_v_to_eps(const void* v, const void* z, int z_dtype, const float* in_scale_dev, float a, float b,
+                                void* eps, int n, void* stream) {
+  return guarded([&] {
+    run_v_to_eps((const __half*)v, z, z_dtype == CFGPP_F16 ? 1 : 0, in_scale_dev, a, b, (__half*)eps, n,
+                 (cudaStream_t)stream);
   });
 }
 

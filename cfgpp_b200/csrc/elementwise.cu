@@ -103,12 +103,34 @@ __global__ void copy_rows_kernel(const __half* __restrict__ src, int src_rows, i
 // ------------------------------------------------------------------------------------------------------------
 // conv_in: 4 -> Cout, 3x3 pad 1, NCHW latent -> NHWC fp16. thread = (pixel, 8 output channels)
 // ------------------------------------------------------------------------------------------------------------
-__global__ void select_step_kernel(const StepState* __restrict__ table, int* counter, StepState* cur) {
+__global__ void select_step_kernel(const StepState* __restrict__ table, int* counter, StepState* cur,
+                                   const float2* __restrict__ v_table, float2* v_cur) {
   pdl_launch_dependents();
   pdl_wait();
   const int i = *counter;
   *cur = table[i];
+  if (v_table) *v_cur = v_table[i];
   *counter = i + 1;
+}
+
+// The UNet's input value of latent element `off`: z * in_scale as conv_in forms it (fp16 arithmetic for an fp16 state,
+// an fp32 product cast to fp16 for an fp32 one, as under the reference's autocast).
+CFGPP_DEVICE float model_input(const void* __restrict__ z, size_t off, int z_is_half, int use_scale, float in_scale) {
+  if (z_is_half) {
+    __half hv = reinterpret_cast<const __half*>(z)[off];
+    if (use_scale) hv = __float2half_rn(__half2float(hv) * in_scale);  // x * c_in in fp16 arithmetic
+    return __half2float(hv);
+  }
+  float fv = reinterpret_cast<const float*>(z)[off];
+  if (use_scale) fv = fv * in_scale;
+  return __half2float(__float2half_rn(fv));  // autocast: conv input cast to fp16
+}
+
+// v-prediction -> epsilon for a model input x_in at the noise level abar: eps = sqrt(abar) v + sqrt(1 - abar) x_in with
+// a = sqrt(abar), b = sqrt(1 - abar) — two fp32 products and an fp32 sum (no FMA contraction), rounded to fp16 as the
+// model output it replaces.
+CFGPP_DEVICE float v_to_eps(float v, float x_in, float a, float b) {
+  return __half2float(__float2half_rn(__fadd_rn(__fmul_rn(a, v), __fmul_rn(b, x_in))));
 }
 
 __global__ void conv_in_kernel(const void* __restrict__ z, int z_is_half, const float* __restrict__ in_scale_ptr,
@@ -153,18 +175,8 @@ __global__ void conv_in_kernel(const void* __restrict__ z, int z_is_half, const 
         for (int c = 0; c < 6; ++c) {
           const int ww = x0 + c - 1;
           float val = 0.f;
-          if (hh >= 0 && hh < H && ww >= 0 && ww < W) {
-            const size_t off = (static_cast<size_t>(b) * 4 + ci) * HW + hh * W + ww;
-            if (z_is_half) {
-              __half hv = reinterpret_cast<const __half*>(z)[off];
-              if (use_scale) hv = __float2half_rn(__half2float(hv) * in_scale);  // x * c_in in fp16 arithmetic
-              val = __half2float(hv);
-            } else {
-              float fv = reinterpret_cast<const float*>(z)[off];
-              if (use_scale) fv = fv * in_scale;
-              val = __half2float(__float2half_rn(fv));  // autocast: conv input cast to fp16
-            }
-          }
+          if (hh >= 0 && hh < H && ww >= 0 && ww < W)
+            val = model_input(z, (static_cast<size_t>(b) * 4 + ci) * HW + hh * W + ww, z_is_half, use_scale, in_scale);
           v[c] = val;
         }
 #pragma unroll
@@ -314,12 +326,16 @@ CFGPP_DEVICE void apply_step_elem(int mode, int half_state, const StepCoef& k, f
 }
 
 // conv_out (Cin -> 4, 3x3 pad 1) + fused step. One warp per latent pixel of image b, computing both CFG halves.
+// kVPred: the conv output is v; it is converted to eps (v_to_eps with (a, b) = *v_coef and the UNet input rebuilt from
+// the state z and *in_scale_ptr) before the step. eps_uc / eps_c receive the raw output (v) either way.
+template <bool kVPred>
 __global__ void conv_out_step_kernel(const __half* __restrict__ x, const __half* __restrict__ w,
                                      const __half* __restrict__ bias, int B, int H, int W, int Cin, int mode,
                                      int half_state, const StepCoef* __restrict__ coef, void* z, void* aux,
                                      void* z0t_out, __half* __restrict__ eps_uc, __half* __restrict__ eps_c,
                                      const __half* const* __restrict__ noise_slot,
-                                     const float* const* __restrict__ lambda_slot) {
+                                     const float* const* __restrict__ lambda_slot, const float2* __restrict__ v_coef,
+                                     const float* __restrict__ in_scale_ptr) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ __half swh[];  // [4][9][Cin]
@@ -385,10 +401,27 @@ __global__ void conv_out_step_kernel(const __half* __restrict__ x, const __half*
     const size_t i = (static_cast<size_t>(b) * 4 + lane) * HW + r;  // NCHW latent index
     if (eps_uc) eps_uc[i] = __float2half_rn(eu);
     if (eps_c) eps_c[i] = __float2half_rn(ec);
+    if constexpr (kVPred) {
+      const float2 ab = *v_coef;
+      const float x_in = model_input(z, i, half_state, in_scale_ptr != nullptr, in_scale_ptr ? *in_scale_ptr : 1.0f);
+      eu = v_to_eps(eu, x_in, ab.x, ab.y);
+      ec = v_to_eps(ec, x_in, ab.x, ab.y);
+    }
     if (mode != STEP_NONE)
       apply_step_elem(mode, half_state, *coef, eu, ec, z, aux, z0t_out, noise_slot, lambda_slot,
                       static_cast<size_t>(4) * HW, static_cast<size_t>(B) * 4 * HW, i);
   }
+}
+
+__global__ void v_to_eps_kernel(const __half* __restrict__ v, const void* __restrict__ z, int z_is_half,
+                                const float* __restrict__ in_scale_ptr, float a, float b, __half* __restrict__ eps,
+                                int n) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float x_in = model_input(z, i, z_is_half, in_scale_ptr != nullptr, in_scale_ptr ? *in_scale_ptr : 1.0f);
+  eps[i] = __float2half_rn(v_to_eps(__half2float(v[i]), x_in, a, b));
 }
 
 __global__ void step_only_kernel(const __half* __restrict__ eps_uc, const __half* __restrict__ eps_c, int n, int mode,
@@ -446,8 +479,9 @@ void run_copy_rows(const __half* src, int src_rows, int cols, __half* dst, int l
   launch_pdl(copy_rows_kernel, dim3((total + 255) / 256), dim3(256), 0, stream, src, src_rows, cols, dst, ld_dst, col_off, R);
 }
 
-void run_select_step(const StepState* table, int* counter, StepState* cur, cudaStream_t stream) {
-  launch_pdl(select_step_kernel, dim3(1), dim3(1), 0, stream, table, counter, cur);
+void run_select_step(const StepState* table, int* counter, StepState* cur, cudaStream_t stream, const float2* v_table,
+                     float2* v_cur) {
+  launch_pdl(select_step_kernel, dim3(1), dim3(1), 0, stream, table, counter, cur, v_table, v_cur);
 }
 
 void run_conv_in(const void* z, int z_is_half, const float* in_scale, const __half* w, const __half* bias,
@@ -468,7 +502,8 @@ void run_conv_in(const void* z, int z_is_half, const float* in_scale, const __ha
 // The state dtype travels in bit 8 of `mode` (mode | 0x100 = fp16 sampler state).
 void run_conv_out_step(const __half* x, const __half* w, const __half* bias, int B, int H, int W, int Cin, int mode,
                        const StepCoef* coef_dev, void* z, void* aux, void* z0t_out, __half* eps_uc, __half* eps_c,
-                       cudaStream_t stream, const __half* const* noise_slot, const float* const* lambda_slot) {
+                       cudaStream_t stream, const __half* const* noise_slot, const float* const* lambda_slot,
+                       const float2* v_coef, const float* in_scale) {
   CFGPP_REQUIRE(Cin % 8 == 0, "conv_out Cin must be a multiple of 8");
   const int half_state = (mode & 0x100) ? 1 : 0;
   const int m = mode & 0xff;
@@ -476,8 +511,18 @@ void run_conv_out_step(const __half* x, const __half* w, const __half* bias, int
   CFGPP_REQUIRE(smem <= 48 * 1024, "conv_out weights must fit 48 KB of shared memory");
   const int warps = 8;
   const int total = B * H * W;
-  launch_pdl(conv_out_step_kernel, dim3((total + warps - 1) / warps), dim3(warps * 32), smem, stream, 
-      x, w, bias, B, H, W, Cin, m, half_state, coef_dev, z, aux, z0t_out, eps_uc, eps_c, noise_slot, lambda_slot);
+  const dim3 grid((total + warps - 1) / warps), block(warps * 32);
+  if (v_coef != nullptr && m != STEP_NONE)
+    launch_pdl(conv_out_step_kernel<true>, grid, block, smem, stream, x, w, bias, B, H, W, Cin, m, half_state, coef_dev,
+               z, aux, z0t_out, eps_uc, eps_c, noise_slot, lambda_slot, v_coef, in_scale);
+  else
+    launch_pdl(conv_out_step_kernel<false>, grid, block, smem, stream, x, w, bias, B, H, W, Cin, m, half_state,
+               coef_dev, z, aux, z0t_out, eps_uc, eps_c, noise_slot, lambda_slot, nullptr, nullptr);
+}
+
+void run_v_to_eps(const __half* v, const void* z, int z_is_half, const float* in_scale, float a, float b, __half* eps,
+                  int n, cudaStream_t stream) {
+  launch_pdl(v_to_eps_kernel, dim3((n + 255) / 256), dim3(256), 0, stream, v, z, z_is_half, in_scale, a, b, eps, n);
 }
 
 void run_step_only(const __half* eps_uc, const __half* eps_c, int n, int mode, const StepCoef* coef_dev, void* z,

@@ -69,17 +69,28 @@ struct StepState {
   float in_scale;  // c_in (1.0 for DDIM)
   StepCoef coef;
 };
-void run_select_step(const StepState* table, int* counter, StepState* cur, cudaStream_t stream);
+// v_table (may be null): a parallel table of v-prediction coefficients (a, b) per step, selected into *v_cur alongside
+void run_select_step(const StepState* table, int* counter, StepState* cur, cudaStream_t stream,
+                     const float2* v_table = nullptr, float2* v_cur = nullptr);
 
 // conv_out 3x3 (Cin -> 4) on the GroupNorm+SiLU'ed NHWC input x [2B,H,W,Cin] fused with the CFG++ guidance mix and
 // the scheduler update. noise_slot (may be null): device word holding the base of the ancestral noise table
 // [slots][B,4,H,W] fp16. lambda_slot (may be null): device word holding the per-image guidance table [B] fp32 or null;
 // while it holds a table, image b mixes with table[b] instead of coef->lambda. z is the sampler state (NCHW, fp32 for
 // DDIM modes, fp16 for DPM++), updated in place.
+// v_coef (may be null; ignored for STEP_NONE): the model predicts v. Before the step, each conv output becomes
+// eps = fp16(a * v + b * x_in) with (a, b) = *v_coef = (sqrt(abar), sqrt(1 - abar)) and x_in the UNet input rebuilt from
+// z and *in_scale as conv_in forms it (in_scale may be null: 1). eps_uc / eps_c still receive the raw output v.
+// With a null v_coef the kernel is the epsilon-model instantiation, without any of this arithmetic.
 void run_conv_out_step(const __half* x, const __half* w /*[4][9][Cin]*/, const __half* bias, int B, int H, int W,
                        int Cin, int mode, const StepCoef* coef_dev, void* z, void* aux /*old_denoised*/,
                        void* z0t_out, __half* eps_uc, __half* eps_c, cudaStream_t stream,
-                       const __half* const* noise_slot = nullptr, const float* const* lambda_slot = nullptr);
+                       const __half* const* noise_slot = nullptr, const float* const* lambda_slot = nullptr,
+                       const float2* v_coef = nullptr, const float* in_scale = nullptr);
+// eps[i] = fp16(a * v[i] + b * x_in[i]) (the conversion of run_conv_out_step) with x_in from z [n] of z's dtype and
+// *in_scale (may be null) as conv_in forms the UNet input.
+void run_v_to_eps(const __half* v, const void* z, int z_is_half, const float* in_scale, float a, float b, __half* eps,
+                  int n, cudaStream_t stream);
 
 // standalone fused CFG++ update from given eps (used when a per-step callback needs the un-fused seam); with a
 // lambda_slot, element i belongs to image i / sample_elems (sample_elems = 4*H*W)

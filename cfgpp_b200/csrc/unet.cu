@@ -66,6 +66,8 @@ Unet::Unet(const cfgpp_model_desc& d, int device) : d_(d), device_(device), sk_(
   CFGPP_REQUIRE(d.in_channels == 4 && d.out_channels == 4, "latent channels must be 4");
   time_embed_dim_ = d.block_out_channels[0] * 4;
   has_aug_ = d.addition_time_embed_dim > 0;
+  CFGPP_REQUIRE(d.prediction_type == 0 || d.prediction_type == 1, "prediction_type must be 0 (epsilon) or 1 (v)");
+  v_pred_ = d.prediction_type == 1;
   gemm_configure();
   attn_configure();
   CFGPP_CHECK_CUDA(cudaStreamCreateWithFlags(&capture_stream_, cudaStreamNonBlocking));
@@ -447,6 +449,7 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
   // from here on the old plan is gone: a throw below must not leave the handle looking prepared
   prepared_ = false;
   nsteps_ = 0;
+  v_ready_ = false;
   graph_valid_ = false;
   // drop the previous plan / workspace
   act_.clear();
@@ -506,6 +509,10 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
       cur_state_ = act_.alloc<StepState>(1);
       step_counter_ = act_.alloc<int>(1);
       step_table_ = act_.alloc<StepState>(1024);
+      if (v_pred_) {
+        v_table_ = act_.alloc<float2>(1024);
+        v_cur_ = act_.alloc<float2>(1);
+      }
       const size_t lat = static_cast<size_t>(B_) * 4 * H_ * W_;
       z_state_ = act_.alloc<float>(lat);
       aux_state_ = act_.alloc<float>(lat);
@@ -772,6 +779,16 @@ void Unet::set_schedule(int method, int state_dtype, const cfgpp_step_state* ste
   steps_host_.assign(steps, steps + nsteps);
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(step_table_, steps_host_.data(), sizeof(StepState) * nsteps, cudaMemcpyHostToDevice,
                                    stream));
+  v_ready_ = false;
+}
+
+void Unet::set_v_coefs(const float* ab, int nsteps, cudaStream_t stream) {
+  CFGPP_REQUIRE(prepared_ && nsteps_ > 0, "call cfgpp_set_schedule first");
+  CFGPP_REQUIRE(v_pred_, "v coefficients belong to a prediction_type = 1 model");
+  CFGPP_REQUIRE(ab != nullptr && nsteps == nsteps_, "one (a, b) pair per schedule entry");
+  // pageable source: staged before the call returns
+  CFGPP_CHECK_CUDA(cudaMemcpyAsync(v_table_, ab, sizeof(float2) * nsteps, cudaMemcpyHostToDevice, stream));
+  v_ready_ = true;
 }
 
 void Unet::set_state(const void* z, int z_dtype, cudaStream_t stream) {
@@ -818,13 +835,14 @@ void Unet::ensure_graph(cudaStream_t stream) {
   const int mode = method_ | (state_dtype_ == CFGPP_F16 ? 0x100 : 0);
   CFGPP_CHECK_CUDA(cudaStreamBeginCapture(capture_stream_, cudaStreamCaptureModeRelaxed));
   try {
-    run_select_step(step_table_, step_counter_, cur_state_, capture_stream_);
+    run_select_step(step_table_, step_counter_, cur_state_, capture_stream_, v_table_, v_cur_);
     run_plan(prologue_plan_, capture_stream_);
     run_conv_in(z_state_, state_dtype_ == CFGPP_F16 ? 1 : 0, &cur_state_->in_scale, conv_in_w_, conv_in_b_,
                 conv_in_out_, B_, H_, W_, d_.block_out_channels[0], 2, capture_stream_);
     run_body(capture_stream_);
     run_conv_out_step(final_norm_.p, conv_out_w_, conv_out_b_, B_, H_, W_, final_norm_.C, mode, &cur_state_->coef,
-                      z_state_, aux_state_, z0t_state_, nullptr, nullptr, capture_stream_, noise_slot_, lambda_slot_);
+                      z_state_, aux_state_, z0t_state_, nullptr, nullptr, capture_stream_, noise_slot_, lambda_slot_,
+                      v_cur_, &cur_state_->in_scale);
   } catch (...) {
     cudaGraph_t g = nullptr;
     cudaStreamEndCapture(capture_stream_, &g);
@@ -839,6 +857,7 @@ void Unet::ensure_graph(cudaStream_t stream) {
 void Unet::run_steps(int first_step, int nsteps, cudaStream_t stream) {
   CFGPP_REQUIRE(prepared_ && nsteps_ > 0, "call cfgpp_set_schedule first");
   CFGPP_REQUIRE(first_step >= 0 && first_step + nsteps <= nsteps_, "step range outside the schedule");
+  CFGPP_REQUIRE(!v_pred_ || v_ready_, "a v-prediction model needs cfgpp_set_v_coefs for this schedule");
   ensure_graph(stream);
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(step_counter_, &first_step, sizeof(int), cudaMemcpyHostToDevice, stream));
   for (int i = 0; i < nsteps; ++i) CFGPP_CHECK_CUDA(cudaGraphLaunch(graph_exec_, stream));

@@ -48,6 +48,8 @@ class Unet {
   void set_noise(const __half* noise, int slots, cudaStream_t stream);
   // per-image guidance: lambda_host [batch] (host), or n = 0 to return to the schedule's scalar; prepare() clears it
   void set_guidance(const float* lambda_host, int n, cudaStream_t stream);
+  // v-prediction: (a, b) per entry of the current schedule (host [nsteps][2]); see cfgpp_set_v_coefs
+  void set_v_coefs(const float* ab_host, int nsteps, cudaStream_t stream);
   void run_steps(int first_step, int nsteps, cudaStream_t stream);
   void get_state(int which, void* out, cudaStream_t stream);
   void apply_step(int step, const __half* eps_uc, const __half* eps_c, cudaStream_t stream);
@@ -142,6 +144,10 @@ class Unet {
   StepState* step_table_ = nullptr;   // device [nsteps]
   int* step_counter_ = nullptr;       // device
   int nsteps_ = 0, method_ = 0, state_dtype_ = CFGPP_F32;
+  bool v_pred_ = false;               // d_.prediction_type == 1
+  float2* v_table_ = nullptr;         // device [nsteps] (a, b), v-prediction handles only
+  float2* v_cur_ = nullptr;           // device, the current step's (a, b)
+  bool v_ready_ = false;              // set_v_coefs matched the current schedule
   std::vector<cfgpp_step_state> steps_host_;
   void* z_state_ = nullptr;   // (B,4,H,W) fp32-sized buffer (holds fp16 or fp32)
   void* aux_state_ = nullptr;

@@ -14,7 +14,7 @@ import torch
 
 from . import _native as nv
 from .config import UNetConfig, to_desc
-from .schedule import F16, F32, StepStateC, to_c_array
+from .schedule import F16, F32, StepStateC, to_c_array, v_pred_coefs
 
 
 class NativeUNet(nv.NativeHandle):
@@ -22,12 +22,19 @@ class NativeUNet(nv.NativeHandle):
 
     def __init__(self, cfg: UNetConfig, state_dict: Dict[str, torch.Tensor], device="cuda:0"):
         self.cfg = cfg
+        # v-prediction (SD 2.x at 768^2): the fused step converts the UNet's v to eps with per-entry (a, b); the un-fused
+        # seams (predict_noise here, cfgpp_unet_forward) return the raw model output
+        self.v_prediction = cfg.prediction_type == "v_prediction"
+        self.v_coefs = None  # (a, b) per entry of the current schedule (v-prediction only)
         self._open(to_desc(cfg), state_dict.items(), device)
         self.batch = 0
         self.latent_hw = (0, 0)
         self._nsteps = 0
         self._state_dtype = torch.float32
         self._bound = None  # strong references to the tensors of the bound prompt (see bind_prompt)
+
+    def _create(self, desc, idx: int) -> None:
+        nv.check(self.lib.cfgpp_create_ex(byref(desc), c_size_t(ctypes.sizeof(desc)), c_int(idx), byref(self._h)))
 
     # ---- plan ------------------------------------------------------------------------------------------------
     def prepare(self, batch: int, h_lat: int, w_lat: int):
@@ -103,6 +110,7 @@ class NativeUNet(nv.NativeHandle):
 
     # ---- un-fused seam: predict_noise ------------------------------------------------------------------------
     def predict_noise(self, z: torch.Tensor, t: float, in_scale: float = 1.0):
+        """The raw model output of both CFG halves (v for a v-prediction model; the solvers convert)."""
         z = z.to(self.device).contiguous()
         eps_uc = torch.empty(z.shape, dtype=torch.float16, device=self.device)
         eps_c = torch.empty_like(eps_uc)
@@ -140,6 +148,11 @@ class NativeUNet(nv.NativeHandle):
         with torch.cuda.device(self.device):
             nv.check(self.lib.cfgpp_set_schedule(self._h, c_int(method), c_int(code), arr, c_int(len(steps)),
                                                  nv.stream_ptr()))
+            if self.v_prediction:
+                ab = v_pred_coefs(method, list(steps))
+                nv.check(self.lib.cfgpp_set_v_coefs(self._h, ab.ctypes.data_as(POINTER(c_float)), c_int(len(steps)),
+                                                    nv.stream_ptr()))
+                self.v_coefs = ab
         self._nsteps = len(steps)
         self._state_dtype = state_dtype
         self.set_guidance(guidance)

@@ -66,7 +66,14 @@ class KDiffusionMixin:
     def _k_denoise(self, x, sigma, t, cfg_guidance, cond: Sequence):
         """cond = (uc, c) for SD v1.5, (uc, c, add_cond_kwargs) for SDXL. Returns (denoised, uncond_denoised)."""
         xc = self.calculate_input(x, sigma)
-        noise_uc, noise_c = self.predict_noise(xc, t, *cond)
+        if getattr(self, "v_prediction", False):
+            # v -> eps at the level the VE update assigns to x (abar = 1 / (1 + sigma^2)), as the fused step does
+            from . import schedule as S
+            v_uc, v_c = self.model_output(xc, t, *cond)
+            a, b = S.ve_v_coefs(sigma)
+            noise_uc, noise_c = S.v_to_eps(v_uc, xc, a, b), S.v_to_eps(v_c, xc, a, b)
+        else:
+            noise_uc, noise_c = self.predict_noise(xc, t, *cond)
         noise_pred = guidance_mix(noise_uc, noise_c, cfg_guidance)
         return self.calculate_denoised(x, noise_pred, sigma), self.calculate_denoised(x, noise_uc, sigma)
 

@@ -1,4 +1,4 @@
-"""Stable Diffusion v1.5 CFG++ solvers on the Blackwell-native backend.
+"""Stable Diffusion v1.5 and 2.x CFG++ solvers on the Blackwell-native backend.
 
 Mirror of the reference's `latent_diffusion.py` solver API for the hot path: registry (:13-26), `StableDiffusion`
 base (:54-241: `alpha`, `get_text_embed`, `encode`, `decode`, `predict_noise`, `inversion`, `initialize_latent`),
@@ -8,6 +8,9 @@ SURVEY §8 f1 (the rest of the CFG++ `--method` surface): `ddim_edit_cfg++` (:95
 `euler_cfg++` (:682-724), `euler_a_cfg++` (:727-768), `dpm++_2s_a_cfg++` (:771-827), `dpm++_2m_cfg++` (:830-879) as
 fused VE-cast trajectories (kdiffusion.py: the ancestral ones with their noise drawn up front); the op-by-op torch
 form over `predict_noise` runs when a callback is installed.
+
+SD 2.x (`unet_config=sd2_config()` / `sd2_base_config()`) runs on the same solvers: the UNet differs only in its
+config, and a v-prediction model's output is turned into eps inside the fused step (see schedule.v_pred_coefs).
 
 dtype note (reference promotion rules, SURVEY Appendix C.5): `ddim_cfg++` keeps an fp32 latent state (zT is a fp32
 `torch.randn`); `ddim_inversion_cfg++` starts from the fp16 VAE latent, so both its inversion loop and the following
@@ -49,10 +52,13 @@ def get_solver(name: str, **kwargs):
 
 
 def default_text_encoder(cfg: UNetConfig, device):
-    """CLIP-L (hidden 768) for SD v1.5; a proportionally narrow tower for the test-sized configs."""
+    """CLIP-L (hidden 768) for SD v1.5, OpenCLIP ViT-H (hidden 1024) for SD 2.x; a proportionally narrow tower for the
+    test-sized configs."""
     d = cfg.cross_attention_dim
     if d == 768:
         return get_conditioner("clip_l", device, "sd15")
+    if d == 1024:
+        return get_conditioner("clip_h", device, "sd15")
     if d % 64:
         return SyntheticTextEncoder(d, 0)
     small = CLIPTextConfig(name=f"clip_{d}", vocab_size=1024, hidden_size=d, intermediate_size=4 * d, num_hidden_layers=2,
@@ -69,6 +75,9 @@ class StableDiffusion(K.KDiffusionMixin):
         self.device = device
         self.dtype = kwargs.get("pipe_dtype", torch.float16)
         self.cfg: UNetConfig = kwargs.get("unet_config") or sd15_config()
+        # SD 2.0-v / 2.1: the UNet predicts v. The fused steps convert it to eps in the step kernel; predict_noise and
+        # the VE-cast seam (_k_denoise) convert the same way, so every seam still hands eps to the sampler arithmetic.
+        self.v_prediction = self.cfg.prediction_type == "v_prediction"
         self.unet = get_engine(model_key, self.cfg, device, kwargs.get("state_dict"))
         # CLIP-L text tower on the native backend (text_encoder.py; the reference takes pipe.text_encoder,
         # latent_diffusion.py:65-66). Pass `text_encoder=fn`, prompt -> (hidden (1,77,D), None), to override.
@@ -125,12 +134,22 @@ class StableDiffusion(K.KDiffusionMixin):
         self.unet.prepare(b, h, w)
         self.unet.bind_prompt(uc, c, force=force)
 
-    def predict_noise(self, zt: torch.Tensor, t: torch.Tensor, uc: torch.Tensor, c: torch.Tensor):
+    def model_output(self, zt: torch.Tensor, t: torch.Tensor, uc: torch.Tensor, c: torch.Tensor):
+        """The UNet's raw (uncond, cond) output at input zt: eps, or v for a v-prediction model."""
         if uc is None or c is None:
             uc = c if uc is None else uc
             c = uc if c is None else c
         self._prepare(zt, uc, c)
         return self.unet.predict_noise(zt, float(t))
+
+    def predict_noise(self, zt: torch.Tensor, t: torch.Tensor, uc: torch.Tensor, c: torch.Tensor):
+        out_uc, out_c = self.model_output(zt, t, uc, c)
+        if not self.v_prediction:
+            return out_uc, out_c
+        at = self.alpha(t)
+        a, b = at.sqrt(), (1 - at).sqrt()
+        x_in = zt.to(out_uc.device, torch.float16)
+        return S.v_to_eps(out_uc, x_in, a, b), S.v_to_eps(out_c, x_in, a, b)
 
     def _run(self, method, steps, z_init, uc, c, callback_fn=None, cfg_guidance=None):
         """`cfg_guidance`: a per-image sequence goes to the step kernel's guidance table; a float (or None) leaves the
@@ -145,7 +164,11 @@ class StableDiffusion(K.KDiffusionMixin):
             z0t = eng.get_state(1)
         else:
             for i, st in enumerate(steps):
-                eps_uc, eps_c = eng.predict_noise(eng.get_state(0), st.t)
+                z = eng.get_state(0)
+                eps_uc, eps_c = eng.predict_noise(z, st.t)
+                if self.v_prediction:  # the fused step's conversion, with the entry's (a, b)
+                    a, b = eng.v_coefs[i]
+                    eps_uc, eps_c = S.v_to_eps(eps_uc, z.half(), a, b), S.v_to_eps(eps_c, z.half(), a, b)
                 eng.apply_step(i, eps_uc, eps_c)
                 kw = {'z0t': eng.get_state(1).detach(), 'zt': eng.get_state(0).detach(), 'decode': self.decode}
                 kw = callback_fn(i, torch.tensor(int(st.t), device=self.device), kw)

@@ -237,6 +237,38 @@ def kd_ancestral_steps(sigmas: torch.Tensor, timestep_fn, cfg_guidance: float, c
     return out, slot
 
 
+def ve_v_coefs(sigma: torch.Tensor):
+    """(a, b) = (sqrt(abar), sqrt(1 - abar)) of a VE-cast state x at noise level sigma, abar = 1 / (1 + sigma^2): a = c_in
+    (the model-input scale of `kd_steps`, same fp32 CPU ops) and b = sigma * c_in. Then eps = a v + b (c_in x), which is
+    k-diffusion's VDenoiser (c_skip = 1 / (sigma^2 + 1), c_out = -sigma c_in) rewritten as an eps prediction."""
+    c_in = torch.tensor(1.0, dtype=torch.float32) / (sigma ** 2 + 1) ** 0.5
+    return c_in, sigma * c_in
+
+
+def v_pred_coefs(method: int, steps: List[StepStateC]) -> np.ndarray:
+    """Per schedule entry (a, b) = (sqrt(abar), sqrt(1 - abar)) of the noise level the entry's own update assigns to the
+    state the UNet sees, float32 [n, 2]. A v-prediction model's output becomes eps = fp16(fp32(a v) + fp32(b x_in))
+    before the step (see v_to_eps).
+      DDIM family (sampling, inversion, plain CFG): the update's Tweedie divisor c1 = sqrt(abar) and c0 = sqrt(1 - abar)
+        (sampling: abar = alpha(t); inversion: abar = alpha(t - skip), the level the state sits at).
+      VE-cast family: ve_v_coefs(sigma) of the entry's sigma = -c0, i.e. a = in_scale, b = sigma * in_scale — each of
+        the two UNet calls of a DPM-Solver++(2S) step with its own sigma."""
+    out = np.zeros((len(steps), 2), dtype=np.float32)
+    for i, st in enumerate(steps):
+        if method == STEP_DPMPP2M_CFGPP:
+            a = np.float32(st.in_scale)
+            out[i] = (a, np.float32(-st.coef.c0) * a)
+        else:
+            out[i] = (st.coef.c1, st.coef.c0)
+    return out
+
+
+def v_to_eps(v: torch.Tensor, x_in: torch.Tensor, a, b) -> torch.Tensor:
+    """eps = fp16(fp32(a v) + fp32(b x_in)) — the fused step kernel's conversion (two fp32 products, an fp32 sum, no
+    FMA) on fp16 tensors v and x_in (the UNet's fp16 input); a, b fp32 scalars."""
+    return (v.float() * float(a) + x_in.float() * float(b)).half()
+
+
 def to_c_array(steps: List[StepStateC]):
     arr = (StepStateC * len(steps))()
     for i, s in enumerate(steps):

@@ -48,13 +48,21 @@ def clip_bigg_config() -> CLIPTextConfig:
                           num_attention_heads=20, hidden_act="gelu", projection_dim=1280, pad_token_id=0)
 
 
+def clip_h_config() -> CLIPTextConfig:
+    """OpenCLIP ViT-H/14 as SD 2.x's `CLIPTextModel` (text_encoder/config.json): 23 layers (the checkpoint drops the
+    last of OpenCLIP's 24), gelu, conditioning on last_hidden_state; tokenizer pads with "!" (id 0)."""
+    return CLIPTextConfig(name="clip_h", hidden_size=1024, intermediate_size=4096, num_hidden_layers=23,
+                          num_attention_heads=16, hidden_act="gelu", pad_token_id=0)
+
+
 def tiny_clip_config(projection_dim: int = 0, act: str = "quick_gelu") -> CLIPTextConfig:
     return CLIPTextConfig(name="tiny_clip" + ("_proj" if projection_dim else ""), vocab_size=256, hidden_size=128,
                           intermediate_size=256, num_hidden_layers=3, num_attention_heads=2, hidden_act=act,
                           projection_dim=projection_dim, pad_token_id=0 if projection_dim else 255)
 
 
-CLIP_CONFIGS = {"clip_l": clip_l_config, "clip_bigg": clip_bigg_config, "tiny_clip": tiny_clip_config}
+CLIP_CONFIGS = {"clip_l": clip_l_config, "clip_bigg": clip_bigg_config, "clip_h": clip_h_config,
+                "tiny_clip": tiny_clip_config}
 _ACT = {"quick_gelu": 0, "gelu": 1}
 
 

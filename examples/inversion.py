@@ -11,6 +11,7 @@ from types import SimpleNamespace
 import torch
 
 from cfgpp_b200.checkpoints import solver_components
+from examples.text_to_img import build_solver
 from cfgpp_b200.latent_diffusion import get_solver
 from cfgpp_b200.latent_sdxl import get_solver as get_solver_sdxl
 from cfgpp_b200.utils.log_util import create_workdir, set_seed
@@ -33,7 +34,8 @@ def main():
     parser = argparse.ArgumentParser(description="Latent Diffusion")
     parser.add_argument("--workdir", type=Path, default="examples/workdir/inversion")
     parser.add_argument("--img_path", type=Path, default="examples/assets/afhq_1.jpg")
-    parser.add_argument("--img_size", type=int, default=512)
+    parser.add_argument("--img_size", type=int, default=None,
+                        help="square image size (default: the model's native size, 512 / 768 (sd20) / 1024)")
     parser.add_argument("--device", type=str, default="cuda")
     parser.add_argument("--null_prompt", type=str, default="")
     parser.add_argument("--prompt", type=str, default="")
@@ -51,6 +53,8 @@ def main():
     set_seed(args.seed)
     create_workdir(args.workdir)
     solver_config = SimpleNamespace(num_sampling=args.NFE)
+    if args.img_size is None:
+        args.img_size = {"sd15": 512, "sd20": 768, "sdxl": 1024}[args.model]
     img = load_img(args.img_path, size=args.img_size)
     prompts = [args.null_prompt, args.prompt, args.tgt_prompt if args.tgt_prompt is not None else args.prompt]
 
@@ -60,8 +64,7 @@ def main():
         result = solver.sample(prompt1=prompts, prompt2=prompts, src_img=img, cfg_guidance=args.cfg_guidance,
                                target_size=(args.img_size, args.img_size))
     else:
-        extra = solver_components(args.ckpt_dir, "sd15", args.device) if args.ckpt_dir else {}
-        solver = get_solver(args.method, solver_config=solver_config, device=args.device, **extra)
+        solver = build_solver(args.model, args.method, solver_config, args.device, args.ckpt_dir)
         result = solver.sample(prompt=prompts, src_img=img, cfg_guidance=args.cfg_guidance, callback_fn=None)
 
     out = args.workdir.joinpath('result/reconstruct.pt')

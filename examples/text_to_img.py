@@ -10,9 +10,26 @@ import torch
 
 from cfgpp_b200.batching import draw_latents
 from cfgpp_b200.checkpoints import solver_components
+from cfgpp_b200.config import sd2_config
 from cfgpp_b200.latent_diffusion import get_solver
 from cfgpp_b200.latent_sdxl import get_solver as get_solver_sdxl
 from cfgpp_b200.utils.log_util import create_workdir, set_seed
+
+
+def model_family(model: str) -> str:
+    """The checkpoint family of a --model choice: sd15 | sd20 | sdxl (SDXL-Lightning has the SDXL layout)."""
+    return {"sd15": "sd15", "sd20": "sd20", "sdxl": "sdxl", "sdxl_lightning": "sdxl"}[model]
+
+
+def build_solver(model: str, method: str, solver_config, device, ckpt_dir=None):
+    """get_solver for --model: the SDXL registry for sdxl*, the SD registry otherwise — with the SD 2 UNet config
+    (768^2 v-prediction unless the checkpoint directory says otherwise), ViT-H text tower and VAE for sd20."""
+    family = model_family(model)
+    extra = solver_components(ckpt_dir, family, device) if ckpt_dir else {}
+    if family == "sd20":
+        extra.setdefault("unet_config", sd2_config())
+    return (get_solver_sdxl if family == "sdxl" else get_solver)(method, solver_config=solver_config, device=device,
+                                                                 **extra)
 
 
 def main():
@@ -30,8 +47,8 @@ def main():
                         help="diffusers-format pipeline directory (unet/, vae/, text_encoder[_2]/, tokenizer[_2]/); "
                              "default: seeded synthetic weights (nothing can be downloaded here)")
     parser.add_argument("--height", type=int, default=None,
-                        help="image height in pixels (default: the model's native size, 512 for SD v1.5, 1024 for "
-                             "SDXL); a multiple of 8 * 2^(UNet levels - 1), e.g. 1216 x 832 for an SDXL bucket")
+                        help="image height in pixels (default: the model's native size, 512 for SD v1.5, 768 for "
+                             "SD 2.x, 1024 for SDXL); a multiple of 8 * 2^(UNet levels - 1), e.g. 1216 x 832 for an SDXL bucket")
     parser.add_argument("--width", type=int, default=None, help="image width in pixels (default: native size)")
     args = parser.parse_args()
 
@@ -41,9 +58,7 @@ def main():
     callback = None
 
     sdxl = args.model in ("sdxl", "sdxl_lightning")
-    extra = solver_components(args.ckpt_dir, "sdxl" if sdxl else "sd15", args.device) if args.ckpt_dir else {}
-    solver = (get_solver_sdxl if sdxl else get_solver)(args.method, solver_config=solver_config, device=args.device,
-                                                       **extra)
+    solver = build_solver(args.model, args.method, solver_config, args.device, args.ckpt_dir)
     native = solver.cfg.sample_size * 8
     height, width = args.height or native, args.width or native
     if height % 8 or width % 8:

@@ -16,10 +16,11 @@ import torch
 
 from cfgpp_b200 import dist as D
 from cfgpp_b200 import weights as Wt
-from cfgpp_b200.config import sd15_config, sdxl_config
+from cfgpp_b200.config import sd2_config, sd15_config, sdxl_config
 from cfgpp_b200.latent_diffusion import get_solver
 from cfgpp_b200.latent_sdxl import get_solver as get_solver_sdxl
 from cfgpp_b200.utils.log_util import create_workdir, set_seed
+from examples.text_to_img import model_family
 
 
 def read_prompts(path: Path, limit: int = 10000):
@@ -83,13 +84,15 @@ def main():
         create_workdir(args.workdir)
     text_list = read_prompts(args.prompt_dir)
     solver_config = SimpleNamespace(num_sampling=args.NFE)
-    sdxl = args.model in ("sdxl", "sdxl_lightning")
-    cfg = sdxl_config() if sdxl else sd15_config()
+    family = model_family(args.model)
+    sdxl = family == "sdxl"
+    cfg = {"sd15": sd15_config, "sd20": sd2_config, "sdxl": sdxl_config}[family]()
 
-    kw = {}
+    kw = {} if sdxl else {"unet_config": cfg}
     if args.ckpt_dir:  # every rank reads the pipeline directory itself (UNet, VAE, text towers, tokenizers)
         from cfgpp_b200.checkpoints import solver_components
-        kw = solver_components(args.ckpt_dir, "sdxl" if sdxl else "sd15", device)
+        kw.update(solver_components(args.ckpt_dir, family, device))
+        cfg = kw.get("unet_config", cfg)
     elif world > 1:  # one bucketed NCCL broadcast of rank 0's weights; afterwards the ranks never talk again
         sd = Wt.synthetic_state_dict(cfg, seed=1234, device=device) if rank == 0 else None
         kw["state_dict"] = D.broadcast_state_dict(sd, Wt.unet_param_specs(cfg), device, src=0)

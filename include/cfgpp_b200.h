@@ -47,6 +47,9 @@ typedef struct cfgpp_model_desc {
   int addition_time_embed_dim;             /* 0: no add-embedding; 256: SDXL text_time */
   int projection_class_embeddings_input_dim; /* 2816 */
   int pooled_dim;                          /* 1280 */
+  int prediction_type;                     /* 0: the UNet predicts epsilon; 1: v (SD 2.0-v / 2.1 at 768^2). Read by
+                                              cfgpp_create_ex only; cfgpp_create takes the layout that ends at
+                                              pooled_dim and means epsilon. */
 } cfgpp_model_desc;
 
 /* dtype codes */
@@ -91,6 +94,9 @@ const char* cfgpp_last_error(void);
 
 /* ---- model lifetime: replaces pipe.unet obtained at latent_diffusion.py:67 / latent_sdxl.py:50,391 ---------- */
 int cfgpp_create(const cfgpp_model_desc* desc, int device, cfgpp_handle** out);
+/* desc_bytes = sizeof(cfgpp_model_desc), or offsetof(cfgpp_model_desc, prediction_type) for the layout without it (then
+ * identical to cfgpp_create). */
+int cfgpp_create_ex(const cfgpp_model_desc* desc, size_t desc_bytes, int device, cfgpp_handle** out);
 int cfgpp_destroy(cfgpp_handle* h);
 /* One call per state-dict entry under its diffusers key (SURVEY.md A.5), fp16 or fp32 device tensor. */
 int cfgpp_load_weight(cfgpp_handle* h, const char* diffusers_key, const void* data_dev, const int64_t* shape, int ndim,
@@ -120,7 +126,8 @@ int cfgpp_set_prompt(cfgpp_handle* h, const void* ctx_dev, int n_ctx, const void
                      int add_rows, void* stream);
 
 /* ---- un-fused seam == predict_noise ------------------------------------------------------------------------- */
-/* z_dev: (batch,4,h,w) NCHW of z_dtype; model input is z * in_scale; outputs (batch,4,h,w) fp16 each. */
+/* z_dev: (batch,4,h,w) NCHW of z_dtype; model input is z * in_scale; outputs (batch,4,h,w) fp16 each: the raw model
+ * output, i.e. v for a prediction_type = 1 handle (cfgpp_op_v_to_eps converts it). */
 int cfgpp_unet_forward(cfgpp_handle* h, const void* z_dev, int z_dtype, float t, float in_scale, void* eps_uc_dev,
                        void* eps_c_dev, void* stream);
 
@@ -144,12 +151,19 @@ int cfgpp_set_noise(cfgpp_handle* h, const void* noise_dev, int slots, void* str
  * method and second_order bit) uses lambda[b] for image b instead of cfgpp_step_coef.lambda_, with the same rounding.
  * n = 0 clears it; cfgpp_prepare clears it too. Enqueued on `stream`; a captured trajectory graph stays valid. */
 int cfgpp_set_guidance(cfgpp_handle* h, const float* lambda_host, int n, void* stream);
+/* v-prediction handles (prediction_type = 1): ab_host holds nsteps (a, b) pairs, one per entry of the current schedule,
+ * a = sqrt(abar), b = sqrt(1 - abar) of the noise level that entry's update assigns to the state the UNet sees (DDIM
+ * modes: a = c1, b = c0; STEP_DPMPP2M_CFGPP: a = in_scale, b = sigma * in_scale). Each fused step converts the conv
+ * output v to eps = fp16(fp32(a v) + fp32(b x_in)), x_in the UNet input, before the guidance mix. Required after every
+ * cfgpp_set_schedule of such a handle before cfgpp_run_steps; refused by epsilon handles. */
+int cfgpp_set_v_coefs(cfgpp_handle* h, const float* ab_host, int nsteps, void* stream);
 /* Run `nsteps` consecutive steps starting at schedule index `first_step` on the internal state. */
 int cfgpp_run_steps(cfgpp_handle* h, int first_step, int nsteps, void* stream);
 /* which: 0 = state z (same dtype as the state), 1 = z0t of the last executed step. */
 int cfgpp_get_state(cfgpp_handle* h, int which, void* out_dev, void* stream);
 /* Standalone update from caller-provided eps (callback path: the caller may have modified nothing, it just needs
- * z0t / zt materialised between UNet calls). Applies schedule entry `step` to the internal state. */
+ * z0t / zt materialised between UNet calls). Applies schedule entry `step` to the internal state. Takes eps for every
+ * prediction_type (a v model's caller converts first, cfgpp_op_v_to_eps). */
 int cfgpp_apply_step(cfgpp_handle* h, int step, const void* eps_uc_dev, const void* eps_c_dev, void* stream);
 
 /* ---- AutoencoderKL decoder (SURVEY.md section 8 f2): replaces `self.vae.decode(zt / scaling_factor).sample` of
@@ -292,6 +306,17 @@ int cfgpp_op_conv_in(const void* z, int z_dtype, const float* in_scale_dev, cons
 int cfgpp_op_conv_out_step(const void* x, const void* w, const void* bias, int B, int H, int W, int Cin, int method,
                            int state_dtype, const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
                            void* eps_uc, void* eps_c, const void* noise_dev, const float* lambda_dev, void* stream);
+/* cfgpp_op_conv_out_step for a v-prediction model: the conv outputs (written to eps_uc / eps_c as they are) are v and
+ * become eps = fp16(fp32(a v) + fp32(b x_in)) before the step, x_in = the UNet input z * (*in_scale_dev) formed as
+ * cfgpp_op_conv_in forms it (in_scale_dev may be NULL: no scaling). method must not be CFGPP_STEP_NONE. */
+int cfgpp_op_conv_out_step_v(const void* x, const void* w, const void* bias, int B, int H, int W, int Cin, int method,
+                             int state_dtype, const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
+                             void* eps_uc, void* eps_c, const void* noise_dev, const float* lambda_dev,
+                             const float* in_scale_dev, float a, float b, void* stream);
+/* The conversion of cfgpp_op_conv_out_step_v alone: eps[i] = fp16(fp32(a v[i]) + fp32(b x_in[i])), v / eps [n] fp16,
+ * x_in from z [n] of z_dtype and in_scale_dev (may be NULL) as cfgpp_op_conv_in forms the UNet input. */
+int cfgpp_op_v_to_eps(const void* v, const void* z, int z_dtype, const float* in_scale_dev, float a, float b, void* eps,
+                      int n, void* stream);
 /* nearest 2x upsample: x [B,H,W,C] NHWC fp16 (C % 8 == 0) -> out [B,2H,2W,C]. */
 int cfgpp_op_upsample2x(const void* x, void* out, int B, int H, int W, int C, void* stream);
 /* AutoencoderKL decoder front: z [B,4,HW] of z_dtype -> fp16(w . fp16(z / scaling) + bias), w [4][4], out [B,4,HW]. */
