@@ -7,6 +7,8 @@
     <dir>/text_encoder/model[.fp16].safetensors      + <dir>/tokenizer/{vocab.json, merges.txt}
     <dir>/text_encoder_2/model[.fp16].safetensors    + <dir>/tokenizer_2/{vocab.json, merges.txt}     (SDXL only)
 
+The SDXL refiner (family 'sdxl_refiner') has unet/, vae/, text_encoder_2/ and tokenizer_2/ only: no text_encoder/.
+
 SD 2.x (family 'sd20') has the SD v1.5 layout; its text_encoder is OpenCLIP ViT-H. `scheduler/scheduler_config.json`
 (prediction_type) and `unet/config.json` (sample_size) are read when present, so the 768^2 v-prediction checkpoints
 (stable-diffusion-2, -2-1) and the 512^2 epsilon ones (-2-base, -2-1-base) both load with the right UNet config.
@@ -29,15 +31,18 @@ def _weights(folder: Path, stems) -> Optional[Path]:
 
 
 def find_pipeline_files(ckpt_dir, family: str) -> Dict[str, Path]:
-    """family: 'sd15' | 'sd20' | 'sdxl'. Raises FileNotFoundError naming every missing piece. For 'sd20' the optional
-    config files are included as 'scheduler_config' / 'unet_config' when they exist."""
+    """family: 'sd15' | 'sd20' | 'sdxl' | 'sdxl_refiner'. Raises FileNotFoundError naming every missing piece. For 'sd20'
+    the optional config files are included as 'scheduler_config' / 'unet_config' when they exist."""
     root = Path(ckpt_dir)
     want = {"unet": (root / "unet", ("diffusion_pytorch_model",)), "vae": (root / "vae", ("diffusion_pytorch_model",)),
             "text_encoder": (root / "text_encoder", ("model",))}
     toks = ["tokenizer"]
-    if family == "sdxl":
+    if family in ("sdxl", "sdxl_refiner"):
         want["text_encoder_2"] = (root / "text_encoder_2", ("model",))
         toks.append("tokenizer_2")
+        if family == "sdxl_refiner":  # the refiner has one text tower, OpenCLIP bigG
+            del want["text_encoder"]
+            toks.remove("tokenizer")
     elif family not in ("sd15", "sd20"):
         raise ValueError(f"unknown model family {family!r}")
     found: Dict[str, Path] = {}
@@ -99,3 +104,13 @@ def solver_components(ckpt_dir, family: str, device) -> dict:
         if family == "sd20":
             kw["unet_config"] = sd2_unet_config(f)
     return kw
+
+
+def refiner_components(ckpt_dir, device) -> dict:
+    """Keyword arguments for `latent_sdxl.SDXLRefiner` from an SDXL refiner pipeline directory: its UNet and its bigG
+    text tower. Its VAE is the SDXL VAE the base solver already holds, so it is not loaded again."""
+    from .text_encoder import get_conditioner
+    f = find_pipeline_files(ckpt_dir, "sdxl_refiner")
+    return {"model_key": str(f["unet"]),
+            "text_encoder": get_conditioner("clip_bigg", device, "sdxl", str(f["text_encoder_2"]),
+                                            str(f["tokenizer_2/vocab.json"]), str(f["tokenizer_2/merges.txt"]))}

@@ -39,6 +39,14 @@ class UNetConfig:
     def time_embed_dim(self) -> int:
         return self.block_out_channels[0] * 4
 
+    @property
+    def num_time_ids(self) -> int:
+        """Time ids of the text_time add-embedding (6 for the SDXL base, 5 for the refiner), 0 without one. The native
+        handle derives the same count from the same three fields and refuses one that does not divide."""
+        if self.addition_embed_type != "text_time":
+            return 0
+        return (self.projection_class_embeddings_input_dim - self.pooled_dim) // self.addition_time_embed_dim
+
 
 def sd15_config() -> UNetConfig:
     return UNetConfig(name="sd15", sample_size=64)
@@ -62,6 +70,30 @@ def tiny_sdxl_config(sample_size: int = 32) -> UNetConfig:
         transformer_layers_per_block=(1, 1, 2), num_attention_heads=(1, 2, 4), cross_attention_dim=128,
         use_linear_projection=True, addition_embed_type="text_time", addition_time_embed_dim=32,
         projection_class_embeddings_input_dim=6 * 32 + 64, pooled_dim=64)
+
+
+def sdxl_refiner_config() -> UNetConfig:
+    """stabilityai/stable-diffusion-xl-refiner-1.0: 4 levels (384, 768, 1536, 1536) with attention on the middle two
+    (4 transformer layers each and in the mid block, 64-wide heads), OpenCLIP bigG penultimate context only (1280), and
+    a text_time add-embedding of 5 time ids: original size, crop top-left and an aesthetic score (2560 = 1280 + 5*256)."""
+    return UNetConfig(
+        name="sdxl_refiner", sample_size=128, block_out_channels=(384, 768, 1536, 1536),
+        down_block_types=("DownBlock2D", "CrossAttnDownBlock2D", "CrossAttnDownBlock2D", "DownBlock2D"),
+        up_block_types=("UpBlock2D", "CrossAttnUpBlock2D", "CrossAttnUpBlock2D", "UpBlock2D"),
+        transformer_layers_per_block=(4, 4, 4, 4), num_attention_heads=(6, 12, 24, 24), cross_attention_dim=1280,
+        use_linear_projection=True, addition_embed_type="text_time", projection_class_embeddings_input_dim=2560)
+
+
+def tiny_sdxl_refiner_config(sample_size: int = 32) -> UNetConfig:
+    """SDXL refiner topology (4 levels, attention on the middle two only, 5 time ids, head_dim 64) at test-sized
+    widths. Its context is the hidden state of tiny_sdxl's second text tower (64 wide), as the refiner's is bigG's."""
+    return UNetConfig(
+        name="tiny_sdxl_refiner", sample_size=sample_size, block_out_channels=(64, 128, 256, 256),
+        down_block_types=("DownBlock2D", "CrossAttnDownBlock2D", "CrossAttnDownBlock2D", "DownBlock2D"),
+        up_block_types=("UpBlock2D", "CrossAttnUpBlock2D", "CrossAttnUpBlock2D", "UpBlock2D"),
+        transformer_layers_per_block=(1, 1, 2, 2), num_attention_heads=(1, 2, 4, 4), cross_attention_dim=64,
+        use_linear_projection=True, addition_embed_type="text_time", addition_time_embed_dim=32,
+        projection_class_embeddings_input_dim=5 * 32 + 64, pooled_dim=64)
 
 
 def tiny_sd15_config(sample_size: int = 32) -> UNetConfig:
@@ -91,7 +123,8 @@ def tiny_sd2_config(sample_size: int = 32, prediction_type: str = "v_prediction"
 
 
 CONFIGS = {"sd15": sd15_config, "sdxl": sdxl_config, "tiny_sdxl": tiny_sdxl_config, "tiny_sd15": tiny_sd15_config,
-           "sd2": sd2_config, "sd2_base": sd2_base_config, "tiny_sd2": tiny_sd2_config}
+           "sd2": sd2_config, "sd2_base": sd2_base_config, "tiny_sd2": tiny_sd2_config,
+           "sdxl_refiner": sdxl_refiner_config, "tiny_sdxl_refiner": tiny_sdxl_refiner_config}
 PREDICTION_TYPES = {"epsilon": 0, "v_prediction": 1}
 
 

@@ -66,6 +66,15 @@ Unet::Unet(const cfgpp_model_desc& d, int device) : d_(d), device_(device), sk_(
   CFGPP_REQUIRE(d.in_channels == 4 && d.out_channels == 4, "latent channels must be 4");
   time_embed_dim_ = d.block_out_channels[0] * 4;
   has_aug_ = d.addition_time_embed_dim > 0;
+  if (has_aug_) {
+    // text_time: pooled text embeds followed by one sinusoid per time id (SDXL base 6, SDXL refiner 5)
+    const int ids_dim = d.projection_class_embeddings_input_dim - d.pooled_dim;
+    CFGPP_REQUIRE(ids_dim > 0 && ids_dim % d.addition_time_embed_dim == 0,
+                  "projection_class_embeddings_input_dim - pooled_dim must be a whole multiple of "
+                  "addition_time_embed_dim");
+    n_time_ids_ = ids_dim / d.addition_time_embed_dim;
+    CFGPP_REQUIRE(n_time_ids_ >= 1 && n_time_ids_ <= 8, "the add-embedding must take 1..8 time ids");
+  }
   CFGPP_REQUIRE(d.prediction_type == 0 || d.prediction_type == 1, "prediction_type must be 0 (epsilon) or 1 (v)");
   v_pred_ = d.prediction_type == 1;
   gemm_configure();
@@ -504,7 +513,7 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
         add_h1_ = alloc_act(static_cast<size_t>(NB_) * TE);
         aug_emb_ = alloc_act(static_cast<size_t>(NB_) * TE);
         pooled_copy_ = alloc_act(static_cast<size_t>(NB_) * d_.pooled_dim);
-        time_ids_copy_ = act_.alloc<float>(static_cast<size_t>(NB_) * 6);
+        time_ids_copy_ = act_.alloc<float>(static_cast<size_t>(NB_) * n_time_ids_);
       }
       cur_state_ = act_.alloc<StepState>(1);
       step_counter_ = act_.alloc<int>(1);
@@ -560,15 +569,15 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
     if (!sizing_ && has_aug_) {
       const int NB = NB_;
       const int ATE = d_.addition_time_embed_dim, PD = d_.pooled_dim, AIN = d_.projection_class_embeddings_input_dim;
-      CFGPP_REQUIRE(AIN == PD + 6 * ATE, "projection_class_embeddings_input_dim != pooled_dim + 6*addition_time_embed_dim");
+      const int NT = n_time_ids_;
       const __half *w1 = weights_.plain("add_embedding.linear_1.weight"), *b1 = weights_.plain("add_embedding.linear_1.bias");
       const __half *w2 = weights_.plain("add_embedding.linear_2.weight"), *b2 = weights_.plain("add_embedding.linear_2.bias");
       __half *add_in = add_in_, *add_h1 = add_h1_, *aug = aug_emb_, *pooled = pooled_copy_;
       float* tids = time_ids_copy_;
       add_step("add_embedding.assemble", [=](cudaStream_t st) {
         run_copy_rows(pooled, NB, PD, add_in, AIN, 0, NB, st);
-        for (int j = 0; j < 6; ++j) run_sincos_embed(tids + j, 6, NB, ATE, add_in, AIN, PD + j * ATE, st);
-      }, 7);
+        for (int j = 0; j < NT; ++j) run_sincos_embed(tids + j, NT, NB, ATE, add_in, AIN, PD + j * ATE, st);
+      }, 1 + NT);
       add_step("add_embedding.linear_1+silu", [=](cudaStream_t st) {
         run_small_linear(add_in, AIN, w1, b1, nullptr, 0, add_h1, TE, nullptr, NB, TE, AIN, true, st);
       });
@@ -695,9 +704,9 @@ void Unet::set_prompt(const __half* ctx, int n_ctx, const __half* pooled, const 
       CFGPP_CHECK_CUDA(cudaMemcpyAsync(pooled_copy_ + static_cast<size_t>(r0) * d_.pooled_dim, pooled,
                                        static_cast<size_t>(add_rows) * d_.pooled_dim * 2, cudaMemcpyDeviceToDevice,
                                        stream));
-      CFGPP_CHECK_CUDA(cudaMemcpyAsync(time_ids_copy_ + static_cast<size_t>(r0) * 6, time_ids,
-                                       static_cast<size_t>(add_rows) * 6 * sizeof(float), cudaMemcpyDeviceToDevice,
-                                       stream));
+      CFGPP_CHECK_CUDA(cudaMemcpyAsync(time_ids_copy_ + static_cast<size_t>(r0) * n_time_ids_, time_ids,
+                                       static_cast<size_t>(add_rows) * n_time_ids_ * sizeof(float),
+                                       cudaMemcpyDeviceToDevice, stream));
     }
   }
   run_plan(prompt_plan_, stream);

@@ -136,8 +136,9 @@ class Unet {
   __half* add_h1_ = nullptr;
   __half* aug_emb_ = nullptr;   // [NB][time_embed_dim]
   __half* pooled_copy_ = nullptr;
-  float* time_ids_copy_ = nullptr;
+  float* time_ids_copy_ = nullptr;  // [NB][n_time_ids_]
   bool has_aug_ = false;
+  int n_time_ids_ = 0;  // (projection_class_embeddings_input_dim - pooled_dim) / addition_time_embed_dim
   __half *t_sin_ = nullptr, *t_h1_ = nullptr, *emb_ = nullptr, *semb_ = nullptr, *temb_all_ = nullptr;
   float* gn_partial_ = nullptr;
   StepState* cur_state_ = nullptr;    // device

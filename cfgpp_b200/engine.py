@@ -75,8 +75,8 @@ class NativeUNet(nv.NativeHandle):
     # ---- conditioning ----------------------------------------------------------------------------------------
     def set_prompt(self, ctx: torch.Tensor, pooled: Optional[torch.Tensor] = None,
                    time_ids: Optional[torch.Tensor] = None):
-        """ctx = cat([uc, c]) (2*batch, n_ctx, D); pooled (rows, pooled_dim), time_ids (rows, 6), rows in
-        {batch, 2*batch} (latent_sdxl.py:249-257)."""
+        """ctx = cat([uc, c]) (2*batch, n_ctx, D); pooled (rows, pooled_dim), time_ids (rows, cfg.num_time_ids), rows
+        in {batch, 2*batch} (latent_sdxl.py:249-257)."""
         nb = 2 * self.batch
         assert ctx.shape[0] == nb, f"ctx must have 2*batch={nb} rows"
         ctx = ctx.to(self.device, torch.float16).contiguous()
@@ -85,7 +85,7 @@ class NativeUNet(nv.NativeHandle):
             pooled = pooled.to(self.device, torch.float16).contiguous()
             time_ids = time_ids.to(self.device, torch.float32).contiguous()
             add_rows = pooled.shape[0]
-            assert time_ids.shape == (add_rows, 6)
+            assert time_ids.shape == (add_rows, self.cfg.num_time_ids)
         with torch.cuda.device(self.device):
             nv.check(self.lib.cfgpp_set_prompt(self._h, nv.ptr(ctx), c_int(ctx.shape[1]), nv.ptr(pooled),
                                                ctypes.cast(nv.ptr(time_ids), POINTER(c_float)), c_int(add_rows),

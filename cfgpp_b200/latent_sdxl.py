@@ -29,7 +29,7 @@ from .batching import (draw_latents, encode_prompts, guidance_table, guidance_va
                        sdxl_added_conditions)
 from .conditioning import SyntheticTextEncoder
 from .text_encoder import CLIPTextConfig, ClipConditioner, get_conditioner
-from .config import UNetConfig, sdxl_config
+from .config import UNetConfig, sdxl_config, sdxl_refiner_config
 from .engine import NativeUNet
 from .weights import load_safetensors_state_dict, synthetic_state_dict
 
@@ -127,9 +127,38 @@ def default_text_encoders(cfg: UNetConfig, device):
             get_conditioner("", device, "sdxl", cfg=small(f"clip_{d2}_proj", d2, cfg.pooled_dim, "gelu", 0)))
 
 
+def _prepare_engine(eng: NativeUNet, zt, uc, c, added_cond_kwargs, force: bool = False):
+    b, _, h, w = zt.shape
+    eng.prepare(b, h, w)
+    if eng.cfg.addition_embed_type == "text_time":
+        eng.bind_prompt(uc, c, added_cond_kwargs['text_embeds'], added_cond_kwargs['time_ids'], force=force)
+    else:
+        eng.bind_prompt(uc, c, force=force)
+
+
+REFINER_SOLVERS = ("ddim", "ddim_cfg++", "dpm++_2m_cfgpp")
+
+
+class SDXLRefiner:
+    """The second expert of SDXL 1.0 (stabilityai/stable-diffusion-xl-refiner-1.0): a UNet that takes over a base
+    trajectory for its last, low-noise steps ("ensemble of experts"; diffusers' `denoising_end` on the base pipeline,
+    `denoising_start` on the refiner's). Pass it to `sample(refiner=...)` of one of REFINER_SOLVERS.
+
+    It holds only its UNet engine (cached next to the base's in the engine cache, keyed by the config name) and,
+    optionally, its text tower: None uses the base solver's second tower (OpenCLIP bigG), the refiner's only one, so no
+    second copy is loaded. The base solver's VAE decodes the refined latent."""
+
+    def __init__(self, model_key: str = "stabilityai/stable-diffusion-xl-refiner-1.0", device='cuda',
+                 unet_config: Optional[UNetConfig] = None, state_dict=None, text_encoder=None):
+        self.cfg = unet_config or sdxl_refiner_config()
+        self.unet = get_engine(model_key, self.cfg, device, state_dict)
+        self.text_enc = text_encoder
+
+
 class SDXL(K.KDiffusionMixin):
     schedule_kind = "ddim"
     quantize = True
+    supports_refiner = False  # the fused DDIM / DPM++ trajectories of REFINER_SOLVERS hand over to a refiner
 
     def __init__(self,
                  solver_config,
@@ -208,12 +237,7 @@ class SDXL(K.KDiffusionMixin):
 
     # ---- the seam: batched (uncond + cond) UNet forward on the native backend -----------------------------------
     def _prepare(self, zt, uc, c, added_cond_kwargs, force: bool = False):
-        b, _, h, w = zt.shape
-        self.unet.prepare(b, h, w)
-        if self.cfg.addition_embed_type == "text_time":
-            self.unet.bind_prompt(uc, c, added_cond_kwargs['text_embeds'], added_cond_kwargs['time_ids'], force=force)
-        else:
-            self.unet.bind_prompt(uc, c, force=force)
+        _prepare_engine(self.unet, zt, uc, c, added_cond_kwargs, force)
 
     def predict_noise(self, zt, t, uc, c, added_cond_kwargs, in_scale: float = 1.0):
         if uc is None or c is None:
@@ -223,10 +247,18 @@ class SDXL(K.KDiffusionMixin):
         self._prepare(zt, uc, c, added_cond_kwargs)
         return self.unet.predict_noise(zt, float(t), in_scale)
 
-    def _get_add_time_ids(self, original_size, crops_coords_top_left, target_size, dtype, text_encoder_projection_dim):
-        add_time_ids = list(original_size + crops_coords_top_left + target_size)
-        passed_add_embed_dim = self.cfg.addition_time_embed_dim * len(add_time_ids) + text_encoder_projection_dim
-        expected_add_embed_dim = self.cfg.projection_class_embeddings_input_dim
+    def _get_add_time_ids(self, original_size, crops_coords_top_left, target_size, dtype, text_encoder_projection_dim,
+                          aesthetic_score: Optional[float] = None, cfg: Optional[UNetConfig] = None):
+        """`cfg` (default: this solver's UNet) decides the form, as diffusers' `requires_aesthetics_score` does: a UNet
+        of 5 time ids (the SDXL refiner) takes (original size, crop top-left, aesthetic score) in place of the
+        base's (original size, crop top-left, target size)."""
+        cfg = cfg or self.cfg
+        if cfg.num_time_ids == 5:
+            add_time_ids = list(original_size + crops_coords_top_left + (aesthetic_score,))
+        else:
+            add_time_ids = list(original_size + crops_coords_top_left + target_size)
+        passed_add_embed_dim = cfg.addition_time_embed_dim * len(add_time_ids) + text_encoder_projection_dim
+        expected_add_embed_dim = cfg.projection_class_embeddings_input_dim
         assert expected_add_embed_dim == passed_add_embed_dim, (
             f"Model expects an added time embedding vector of length {expected_add_embed_dim}, but a vector of "
             f"{passed_add_embed_dim} was created. The model has an incorrect config.")
@@ -243,11 +275,22 @@ class SDXL(K.KDiffusionMixin):
                negative_crops_coords_top_left: Tuple[int, int] = (0, 0),
                negative_target_size: Optional[Tuple[int, int]] = None,
                clip_skip: Optional[int] = None,
+               refiner: Optional[SDXLRefiner] = None,
+               denoising_end: float = 0.8,
+               aesthetic_score: float = 6.0,
+               negative_aesthetic_score: float = 2.5,
                **kwargs):
         """Batched: `prompt1[1]` / `prompt2[1]` one string or B strings, the null prompts one string (broadcast) or B
         strings, `cfg_guidance` a float or B floats (one per image, applied in the fused step kernel), `zT` None or
         (B,4,h,w); without zT the B latents are drawn one image at a time, so image i does not depend on B. Mismatched
-        lengths raise ValueError. Returns (B, 3, H, W)."""
+        lengths raise ValueError. Returns (B, 3, H, W).
+
+        `refiner`: an SDXLRefiner that runs the steps after `denoising_end` (a fraction of the schedule, see
+        schedule.expert_split) in the same trajectory; the image is decoded once, after it. The refiner is conditioned
+        as diffusers' refiner pipeline conditions it: `prompt1` through its text tower, time ids (original size, crop
+        top-left, `aesthetic_score`) and, for the uncond row, `negative_aesthetic_score`."""
+        if refiner is not None:
+            self._check_refiner()
         height = self.default_sample_size * self.vae_scale_factor
         width = self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)
@@ -275,12 +318,52 @@ class SDXL(K.KDiffusionMixin):
 
         add_cond_kwargs = {'text_embeds': add_text_embeds.to(self.device), 'time_ids': add_time_ids.to(self.device)}
 
+        if refiner is not None:
+            kwargs.update(refiner=refiner, denoising_end=denoising_end, refiner_cond=self.refiner_conditions(
+                refiner, p["prompt1[0]"], p["prompt1[1]"], cfg_guidance, original_size, crops_coords_top_left,
+                negative_original_size or original_size, negative_crops_coords_top_left, aesthetic_score,
+                negative_aesthetic_score, clip_skip, B))
         zt = self.reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, target_size,
                                   **kwargs)
         with torch.no_grad():
             img = self.decode(zt)
         img = (img / 2 + 0.5).clamp(0, 1)
         return img.detach().cpu()
+
+    @torch.no_grad()
+    def refiner_conditions(self, refiner: SDXLRefiner, null_prompt, prompt, cfg_guidance, original_size,
+                           crops_coords_top_left, negative_original_size, negative_crops_coords_top_left,
+                           aesthetic_score, negative_aesthetic_score, clip_skip=None, batch: int = 1):
+        """(uc, c, added_cond_kwargs) of the refiner, following diffusers' StableDiffusionXLImg2ImgPipeline (stated
+        here: diffusers is not a dependency): its encode_prompt zips [prompt, prompt_2] with its single tokenizer, so
+        only the `prompt1` pair reaches the one text tower (bigG), whose penultimate hidden state is the context and
+        whose text_embeds are the pooled embedding; the time ids take the aesthetic form; the rows are assembled per
+        image by the same lambda rule as the base's."""
+        enc = refiner.text_enc or self.text_enc_2
+        uc, pool_null = self._text_embed(null_prompt, enc, clip_skip, batch)
+        c, pool = self._text_embed(prompt, enc, clip_skip, batch)
+        proj = int(pool.shape[-1])
+        time_ids = self._get_add_time_ids(original_size, crops_coords_top_left, None, c.dtype, proj,
+                                          aesthetic_score, refiner.cfg)
+        negative_time_ids = self._get_add_time_ids(negative_original_size, negative_crops_coords_top_left, None,
+                                                   c.dtype, proj, negative_aesthetic_score, refiner.cfg)
+        text_embeds, time_ids = sdxl_added_conditions(pool_null, pool, negative_time_ids, time_ids, cfg_guidance,
+                                                      batch)
+        return uc, c, {'text_embeds': text_embeds.to(self.device), 'time_ids': time_ids.to(self.device)}
+
+    def _check_refiner(self):
+        if not self.supports_refiner or self.schedule_kind == "lightning":
+            raise ValueError(f"an SDXL refiner runs with the solvers {', '.join(REFINER_SOLVERS)} only, not with "
+                             f"{type(self).__name__}")
+
+    def _hand_off(self, kwargs, nsteps: int):
+        """(refiner, its (uc, c, added_cond_kwargs), k) of a reverse_process call given `refiner=`, else None."""
+        refiner = kwargs.get('refiner')
+        if refiner is None:
+            return None
+        self._check_refiner()
+        k = S.expert_split(self._sch.timesteps, kwargs.get('denoising_end', 0.8), nsteps)
+        return refiner, kwargs['refiner_cond'], k
 
     def initialize_latent(self, method: str = 'random', src_img: Optional[torch.Tensor] = None,
                           add_cond_kwargs: Optional[dict] = None, **kwargs):
@@ -324,17 +407,35 @@ class SDXL(K.KDiffusionMixin):
 
     # ---- shared trajectory driver -------------------------------------------------------------------------------
     def _run_trajectory(self, method, state_dtype, steps, z_init, uc, c, add_cond_kwargs, callback_fn, result,
-                        cfg_guidance=None):
+                        cfg_guidance=None, hand_off=None):
         """`result`: 'z0t' (DDIM family returns the Tweedie estimate of the last step) or 'zt' (DPM++ returns x).
-        `cfg_guidance`: a per-image sequence goes to the step kernel's guidance table."""
-        self._prepare(z_init, uc, c, add_cond_kwargs, force=True)  # every trajectory re-binds its prompt
+        `cfg_guidance`: a per-image sequence goes to the step kernel's guidance table.
+        `hand_off` (see _hand_off): steps [k, n) of the same table run on the refiner's engine, which continues from
+        the base's state in the sampler's own parameterization; both engines are set up before the first step, so
+        the hand-off is a device-to-device copy with no host synchronisation. The step index a callback sees runs
+        0..n-1 across both."""
+        table = None if cfg_guidance is None else guidance_table(cfg_guidance)
+        experts = [(self.unet, (uc, c, add_cond_kwargs))]
+        k = len(steps)
+        if hand_off is not None:
+            refiner, refiner_cond, k = hand_off
+            experts.append((refiner.unet, refiner_cond))
+        for e, cond in experts:
+            _prepare_engine(e, z_init, *cond, force=True)  # every trajectory re-binds its prompt
+            e.set_schedule(method, state_dtype, steps, table)
         eng = self.unet
-        eng.set_schedule(method, state_dtype, steps, None if cfg_guidance is None else guidance_table(cfg_guidance))
         eng.set_state(z_init)
         if callback_fn is None:
-            eng.run_steps(0, len(steps))
+            eng.run_steps(0, k)
+            if hand_off is not None:
+                eng, base = experts[1][0], eng
+                eng.set_state(base.get_state(0))
+                eng.run_steps(k, len(steps) - k)
         else:
             for i, st in enumerate(steps):
+                if i == k:
+                    eng, base = experts[1][0], eng
+                    eng.set_state(base.get_state(0))
                 zt = eng.get_state(0)
                 eps_uc, eps_c = eng.predict_noise(zt, st.t, st.in_scale)
                 eng.apply_step(i, eps_uc, eps_c)
@@ -372,9 +473,12 @@ class SDXLLightning(SDXL):
 class BaseDDIM(SDXL):
     """latent_sdxl.py:425-467: fp32 state, fused trajectory, renoise with the guided eps."""
     step_mode = S.STEP_DDIM_CFG
+    supports_refiner = True
 
     def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
                         callback_fn=None, **kwargs):
+        """`refiner=`, `refiner_cond=` (uc, c, added_cond_kwargs), `denoising_end=`: hand the trajectory to an SDXL
+        refiner (sample() builds the conditioning)."""
         b = null_prompt_embeds.shape[0]
         zt = kwargs.get('zT')
         if zt is None:
@@ -382,7 +486,8 @@ class BaseDDIM(SDXL):
         steps = S.ddim_cfgpp_steps(self._sch, cfg_guidance, sdxl_indexing=True,
                                    tables_on_device=(self.schedule_kind == "lightning"))
         return self._run_trajectory(self.step_mode, torch.float32, steps, zt.float(), null_prompt_embeds,
-                                    prompt_embeds, add_cond_kwargs, callback_fn, 'z0t', cfg_guidance)
+                                    prompt_embeds, add_cond_kwargs, callback_fn, 'z0t', cfg_guidance,
+                                    self._hand_off(kwargs, len(steps)))
 
 
 @register_solver('euler')
@@ -439,6 +544,8 @@ class EulerLight(Euler, SDXLLightning):
 
 @register_solver("ddim_cfg++")
 class BaseDDIMCFGpp(SDXL):
+    supports_refiner = True
+
     def reverse_process(self,
                         null_prompt_embeds,
                         prompt_embeds,
@@ -455,7 +562,8 @@ class BaseDDIMCFGpp(SDXL):
                                    tables_on_device=(self.schedule_kind == "lightning"))
         # fp32 state: zt comes from torch.randn (fp32) and promotes every update (latent_sdxl.py:289, 741-744)
         return self._run_trajectory(S.STEP_DDIM_CFGPP, torch.float32, steps, zt.float(), null_prompt_embeds,
-                                    prompt_embeds, add_cond_kwargs, callback_fn, 'z0t', cfg_guidance)
+                                    prompt_embeds, add_cond_kwargs, callback_fn, 'z0t', cfg_guidance,
+                                    self._hand_off(kwargs, len(steps)))
 
 
 @register_solver('ddim_cfg++_lightning')
@@ -479,6 +587,7 @@ class BaseDDIMCFGppLight(BaseDDIMCFGpp, SDXLLightning):
 @register_solver('dpm++_2m_cfgpp')
 class DPMpp2mCFGppSolver(SDXL):
     quantize = True
+    supports_refiner = True
 
     def reverse_process(self,
                         null_prompt_embeds,
@@ -489,7 +598,10 @@ class DPMpp2mCFGppSolver(SDXL):
                         callback_fn=None,
                         **kwargs):
         b = null_prompt_embeds.shape[0]
-        steps, sigma0 = S.dpmpp_2m_cfgpp_steps(self._sch, cfg_guidance)
+        # a refiner starts with no multistep history: its first step takes the first-order update
+        hand_off = self._hand_off(kwargs, len(self._sch.timesteps) - 1)
+        steps, sigma0 = S.dpmpp_2m_cfgpp_steps(self._sch, cfg_guidance,
+                                               restart_at=None if hand_off is None else hand_off[2])
         x = kwargs.get('zT')
         if x is None:
             x = self.initialize_latent(method='random', size=(b, 4, shape[1] // self.vae_scale_factor,
@@ -497,7 +609,7 @@ class DPMpp2mCFGppSolver(SDXL):
         x = x.to(torch.float16)
         x = x * sigma0  # fp16 tensor x 0-dim fp32 -> fp16 (latent_sdxl.py:882-884)
         return self._run_trajectory(S.STEP_DPMPP2M_CFGPP, torch.float16, steps, x, null_prompt_embeds, prompt_embeds,
-                                    add_cond_kwargs, callback_fn, 'zt', cfg_guidance)
+                                    add_cond_kwargs, callback_fn, 'zt', cfg_guidance, hand_off)
 
 
 @register_solver('dpm++_2m_cfgpp_lightning')
@@ -577,6 +689,8 @@ class EditWardSwapDDIM(SDXL):
                negative_target_size: Optional[Tuple[int, int]] = None,
                clip_skip: Optional[int] = None,
                **kwargs):
+        if kwargs.get('refiner') is not None:
+            self._check_refiner()
         height = self.default_sample_size * self.vae_scale_factor
         width = self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)

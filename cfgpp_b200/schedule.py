@@ -14,7 +14,7 @@ from __future__ import annotations
 
 import ctypes
 from dataclasses import dataclass
-from typing import List
+from typing import List, Optional
 
 import numpy as np
 import torch
@@ -133,8 +133,24 @@ def sigma_to_t(sch: Schedule, sigma: torch.Tensor, quantize: bool = True) -> tor
     return t.view(sigma.shape)
 
 
-def dpmpp_2m_cfgpp_steps(sch: Schedule, cfg_guidance: float):
-    """DPMpp2mCFGppSolver.reverse_process scalars (latent_sdxl.py:877-918). Returns (steps, sigma0)."""
+def expert_split(timesteps: torch.Tensor, denoising_end: float, nsteps: int) -> int:
+    """Index k of the first step the second expert (the SDXL refiner) runs: the base runs steps [0, k), the refiner
+    [k, nsteps). k = #{t in timesteps : t >= round(1000 * (1 - denoising_end))}, diffusers' rule for both the base
+    pipeline's `denoising_end` and the refiner pipeline's `denoising_start`. Both experts must run at least one step."""
+    if not 0.0 < denoising_end < 1.0:
+        raise ValueError(f"denoising_end must lie strictly between 0 and 1, got {denoising_end}")
+    cutoff = int(round(NUM_TRAIN_TIMESTEPS * (1.0 - denoising_end)))
+    k = int((timesteps >= cutoff).sum())
+    if not 1 <= k <= nsteps - 1:
+        raise ValueError(f"denoising_end={denoising_end} leaves {k} of {nsteps} steps to the base model; each expert "
+                         f"needs at least one step")
+    return k
+
+
+def dpmpp_2m_cfgpp_steps(sch: Schedule, cfg_guidance: float, restart_at: Optional[int] = None):
+    """DPMpp2mCFGppSolver.reverse_process scalars (latent_sdxl.py:877-918). Returns (steps, sigma0).
+    restart_at=k: entry k takes the first-order update, as the first step of a new call does — the hand-off to the
+    SDXL refiner, which starts with no multistep history. Every other entry is unchanged."""
     alphas = sch.alphas_cumprod[sch.timesteps.int()]
     sigmas = (1 - alphas).sqrt() / alphas.sqrt()
     t_fn = lambda s: s.log().neg()  # noqa: E731
@@ -147,7 +163,7 @@ def dpmpp_2m_cfgpp_steps(sch: Schedule, cfg_guidance: float):
         t, t_next = t_fn(sigmas[i]), t_fn(sigmas[i + 1])
         h = t_next - t
         inv_sigma = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(sigmas[i].item(), dtype=torch.float32)
-        if i == 0 or sigmas[i + 1] == 0:
+        if i == 0 or i == restart_at or sigmas[i + 1] == 0:
             out.append(_state(float(new_t), c_in, cfg_guidance, c=(c_out, inv_sigma, sigmas[i + 1], 0.0)))
         else:
             h_last = t - t_fn(sigmas[i - 1])

@@ -3,16 +3,17 @@
 Runs on the Hopper-native (sm_90a) backend. Without checkpoints (offline) the UNet weights are seeded synthetic and the
 text encoder / VAE are stand-ins (cfgpp_b200/conditioning.py), so the PNG is only a plumbing check."""
 import argparse
+import warnings
 from pathlib import Path
 from types import SimpleNamespace
 
 import torch
 
 from cfgpp_b200.batching import draw_latents
-from cfgpp_b200.checkpoints import solver_components
+from cfgpp_b200.checkpoints import refiner_components, solver_components
 from cfgpp_b200.config import sd2_config
 from cfgpp_b200.latent_diffusion import get_solver
-from cfgpp_b200.latent_sdxl import get_solver as get_solver_sdxl
+from cfgpp_b200.latent_sdxl import SDXLRefiner, get_solver as get_solver_sdxl
 from cfgpp_b200.utils.log_util import create_workdir, set_seed
 
 
@@ -30,6 +31,14 @@ def build_solver(model: str, method: str, solver_config, device, ckpt_dir=None):
         extra.setdefault("unet_config", sd2_config())
     return (get_solver_sdxl if family == "sdxl" else get_solver)(method, solver_config=solver_config, device=device,
                                                                  **extra)
+
+
+def build_refiner(device, ckpt_dir=None) -> SDXLRefiner:
+    """The SDXL refiner from its pipeline directory, or on seeded synthetic weights (with a warning) without one."""
+    if ckpt_dir:
+        return SDXLRefiner(device=device, **refiner_components(ckpt_dir, device))
+    warnings.warn("no --refiner_ckpt_dir given; the SDXL refiner runs on seeded synthetic UNet weights")
+    return SDXLRefiner(model_key="synthetic:8765", device=device)
 
 
 def main():
@@ -50,7 +59,15 @@ def main():
                         help="image height in pixels (default: the model's native size, 512 for SD v1.5, 768 for "
                              "SD 2.x, 1024 for SDXL); a multiple of 8 * 2^(UNet levels - 1), e.g. 1216 x 832 for an SDXL bucket")
     parser.add_argument("--width", type=int, default=None, help="image width in pixels (default: native size)")
+    parser.add_argument("--denoising_end", type=float, default=None,
+                        help="--model sdxl: hand the last (1 - F) of the schedule to the SDXL refiner (e.g. 0.8; "
+                             "methods ddim, ddim_cfg++, dpm++_2m_cfgpp); default: the base model alone")
+    parser.add_argument("--refiner_ckpt_dir", type=Path, default=None,
+                        help="SDXL refiner pipeline directory (unet/, vae/, text_encoder_2/, tokenizer_2/); default: "
+                             "seeded synthetic refiner weights")
     args = parser.parse_args()
+    if args.denoising_end is not None and args.model != "sdxl":
+        raise SystemExit("--denoising_end needs --model sdxl")
 
     set_seed(args.seed)
     create_workdir(args.workdir)
@@ -65,9 +82,13 @@ def main():
         raise SystemExit(f"--height / --width must be multiples of 8 (got {height} x {width})")
     zT = draw_latents((1, 4, height // 8, width // 8))  # N(0, 1) start latent from the seeded CPU generator
     if sdxl:
+        refiner = {}
+        if args.denoising_end is not None:
+            refiner = {"refiner": build_refiner(args.device, args.refiner_ckpt_dir),
+                       "denoising_end": args.denoising_end}
         result = solver.sample(prompt1=[args.null_prompt, args.prompt], prompt2=[args.null_prompt, args.prompt],
                                cfg_guidance=args.cfg_guidance, original_size=(height, width),
-                               target_size=(height, width), callback_fn=callback, zT=zT)
+                               target_size=(height, width), callback_fn=callback, zT=zT, **refiner)
     else:
         result = solver.sample(prompt=[args.null_prompt, args.prompt], cfg_guidance=args.cfg_guidance,
                                callback_fn=callback, zT=zT)

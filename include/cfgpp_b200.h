@@ -45,7 +45,7 @@ typedef struct cfgpp_model_desc {
   int norm_num_groups;                     /* 32 */
   float norm_eps;                          /* 1e-5 (Transformer2DModel's GroupNorm uses 1e-6) */
   int addition_time_embed_dim;             /* 0: no add-embedding; 256: SDXL text_time */
-  int projection_class_embeddings_input_dim; /* 2816 */
+  int projection_class_embeddings_input_dim; /* 2816 (SDXL base: 6 time ids), 2560 (SDXL refiner: 5) */
   int pooled_dim;                          /* 1280 */
   int prediction_type;                     /* 0: the UNet predicts epsilon; 1: v (SD 2.0-v / 2.1 at 768^2). Read by
                                               cfgpp_create_ex only; cfgpp_create takes the layout that ends at
@@ -119,7 +119,8 @@ int cfgpp_plan_stats(cfgpp_handle* h, double* step_flops, double* prompt_flops, 
 
 /* ---- per-prompt conditioning: the tensors predict_noise concatenates (latent_sdxl.py:178-182, 249-257) ------ */
 /* ctx_dev: (2*batch, 77, cross_dim) fp16 = cat([uc, c]); pooled_dev: (add_rows, pooled_dim) fp16;
- * time_ids_dev: (add_rows, 6) fp32; add_rows is 2*batch, or batch when the reference does not duplicate the added
+ * time_ids_dev: (add_rows, n_time_ids) fp32, n_time_ids = (projection_class_embeddings_input_dim - pooled_dim) /
+ * addition_time_embed_dim (6 for the SDXL base, 5 for the SDXL refiner; 1..8, checked at create); add_rows is 2*batch, or batch when the reference does not duplicate the added
  * conditions (cfg_guidance in {0,1}: latent_sdxl.py:249-252 — rows then broadcast over both halves).
  * pooled/time_ids are ignored (may be NULL) for models without add-embedding. n_ctx = tokens per row (77). */
 int cfgpp_set_prompt(cfgpp_handle* h, const void* ctx_dev, int n_ctx, const void* pooled_dev, const float* time_ids_dev,
