@@ -248,6 +248,23 @@ def op_fold_ln(w: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, bias: t
     return wf, s, t
 
 
+def op_lora_merge(base: torch.Tensor, downs, ups, coefs, out: torch.Tensor | None = None) -> torch.Tensor:
+    """The LoRA merge kernel: fp16(fp32(base) + sum_a coefs[a] * ups[a] @ downs[a]) with fp32 accumulation and one
+    rounding; base [N,K] fp16, downs[a] [r_a,K], ups[a] [N,r_a] fp16, up to 4 adapters of rank 1..128."""
+    lib = load()
+    N, K = base.shape
+    n = len(downs)
+    assert len(ups) == n and len(coefs) == n and base.dtype == torch.float16
+    for d, u in zip(downs, ups):
+        assert d.dtype == u.dtype == torch.float16 and d.shape == (u.shape[1], K) and u.shape[0] == N
+    out = torch.empty_like(base) if out is None else out
+    check(lib.cfgpp_op_lora_merge(ptr(base), (c_void_p * n)(*[d.data_ptr() for d in downs]),
+                                  (c_void_p * n)(*[u.data_ptr() for u in ups]),
+                                  (c_int * n)(*[d.shape[0] for d in downs]), (c_float * n)(*[float(c) for c in coefs]),
+                                  c_int(n), c_int(N), c_int(K), ptr(out), stream_ptr()))
+    return out
+
+
 def op_conv3x3(x_nhwc: torch.Tensor, w_packed: torch.Tensor, bias=None, addend=None,
                add_rows_per_group: int = 1, force_bn: int = 0) -> torch.Tensor:
     """x [B,H,W,Cin] fp16 NHWC, w_packed [Cout, 9*Cin] (tap-major), returns [B,H,W,Cout]."""

@@ -43,6 +43,27 @@ CFGPP_API int cfgpp_finalize_weights(cfgpp_handle* h, void* stream) {
   return guarded([&] { h->unet.finalize_weights((cudaStream_t)stream); });
 }
 
+CFGPP_API int cfgpp_lora_add(cfgpp_handle* h, int adapter, const char* key, const void* down, const void* up, int rank,
+                             float alpha, int dtype, void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(key, "null key");
+    h->unet.lora_add(adapter, key, down, up, rank, alpha, dtype, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_lora_set_scales(cfgpp_handle* h, const float* scales_host, int n_adapters, void* stream) {
+  return guarded([&] { h->unet.lora_set_scales(scales_host, n_adapters, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_lora_clear(cfgpp_handle* h, void* stream) {
+  return guarded([&] { h->unet.lora_clear((cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_lora_stats(cfgpp_handle* h, int* n_adapters, int* n_targets, size_t* backup_bytes,
+                               size_t* bytes_moved) {
+  return guarded([&] { h->unet.lora_stats(n_adapters, n_targets, backup_bytes, bytes_moved); });
+}
+
 CFGPP_API int cfgpp_prepare(cfgpp_handle* h, int batch, int h_lat, int w_lat) {
   return guarded([&] { h->unet.prepare(batch, h_lat, w_lat); });
 }

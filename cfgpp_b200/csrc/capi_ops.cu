@@ -3,6 +3,7 @@
 // status (0 = OK) and records a message retrievable with cfgpp_last_error().
 #include "capi_util.h"
 #include "attention.cuh"
+#include "executor.cuh"
 #include "gemm.cuh"
 #include "ops.cuh"
 #include "../../include/cfgpp_b200.h"
@@ -52,6 +53,22 @@ CFGPP_API int cfgpp_op_fold_ln(const void* w, const void* gamma, const void* bet
   return guarded([&] {
     run_fold_ln((const __half*)w, (const __half*)gamma, (const __half*)beta, (const __half*)bias, (__half*)wf, s, t, N,
                 K, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_lora_merge(const void* base, const void* const* downs, const void* const* ups, const int* ranks,
+                                  const float* coefs_host, int n_adapters, int N, int K, void* out, void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(n_adapters >= 0 && n_adapters <= kMaxLoraPerTarget, "at most 4 adapters merge into one weight");
+    LoraMergeArgs a{};
+    a.n = n_adapters;
+    for (int i = 0; i < n_adapters; ++i) {
+      a.down[i] = (const __half*)downs[i];
+      a.up[i] = (const __half*)ups[i];
+      a.rank[i] = ranks[i];
+      a.coef[i] = coefs_host[i];
+    }
+    run_lora_merge((const __half*)base, a, N, K, (__half*)out, (cudaStream_t)stream);
   });
 }
 

@@ -94,12 +94,112 @@ __half* WeightStore::packed_conv3x3(const std::string& key) {
   if (it != conv3x3_.end()) return it->second;
   const Weight& t = raw(key);
   CFGPP_REQUIRE(t.shape.size() == 4 && t.shape[2] == 3 && t.shape[3] == 3, "expected (Cout,Cin,3,3): " + key);
-  const int Cout = static_cast<int>(t.shape[0]), Cin = static_cast<int>(t.shape[1]);
-  __half* out = alloc(t.numel());
-  pack_conv3x3_kernel<<<grid_for(t.numel()), 256>>>(t.p(), out, Cout, Cin);
+  conv3x3_[key] = alloc(t.numel());
+  refresh_conv3x3(key, nullptr);
+  return conv3x3_[key];
+}
+
+size_t WeightStore::refresh_conv3x3(const std::string& key, cudaStream_t stream) {
+  auto it = conv3x3_.find(key);
+  if (it == conv3x3_.end()) return 0;
+  const Weight& t = raw(key);
+  pack_conv3x3_kernel<<<grid_for(t.numel()), 256, 0, stream>>>(t.p(), it->second, static_cast<int>(t.shape[0]),
+                                                               static_cast<int>(t.shape[1]));
   CFGPP_CHECK_CUDA(cudaGetLastError());
-  conv3x3_[key] = out;
-  return out;
+  return 2 * t.numel() * sizeof(__half);
+}
+
+// ---- LoRA ----------------------------------------------------------------------------------------------------
+namespace {
+
+WeightStore::Weight::Ptr device_halves(size_t n) {
+  __half* p = nullptr;
+  CFGPP_CHECK_CUDA(cudaMalloc(&p, std::max<size_t>(n, 8) * sizeof(__half)));
+  return WeightStore::Weight::Ptr(p);
+}
+
+}  // namespace
+
+void WeightStore::lora_add(int adapter, const std::string& key, const void* down, const void* up, int rank, float alpha,
+                           int dtype, cudaStream_t stream) {
+  CFGPP_REQUIRE(dtype == CFGPP_F16 || dtype == CFGPP_F32, "LoRA factor dtype must be fp16 or fp32");
+  CFGPP_REQUIRE(adapter >= 0 && adapter < 64, "adapter id must be 0..63");
+  CFGPP_REQUIRE(down && up, "null LoRA factor for " + key);
+  const Weight& w = raw(key);
+  CFGPP_REQUIRE(w.shape.size() >= 2, "a LoRA targets a weight of 2 or more dimensions: " + key);
+  CFGPP_REQUIRE(rank >= 1 && rank <= kMaxLoraRank, "LoRA rank must be 1..128: " + key);
+  auto it = lora_.find(key);
+  if (it != lora_.end()) {
+    for (const LoraFactor& f : it->second.factors)
+      if (f.adapter == adapter) throw Error(-12, "adapter " + std::to_string(adapter) + " already targets " + key);
+    if (static_cast<int>(it->second.factors.size()) >= kMaxLoraPerTarget)
+      throw Error(-12, "too many LoRA adapters on " + key + " (at most 4 per weight)");
+  }
+  const size_t N = static_cast<size_t>(w.shape[0]), K = w.numel() / N;
+  auto ingest = [&](const void* src, size_t n) {
+    Weight::Ptr dst = device_halves(n);
+    if (dtype == CFGPP_F16) {
+      CFGPP_CHECK_CUDA(cudaMemcpyAsync(dst.get(), src, n * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
+    } else {
+      f32_to_f16_kernel<<<grid_for(n), 256, 0, stream>>>(static_cast<const float*>(src), dst.get(), n);
+      CFGPP_CHECK_CUDA(cudaGetLastError());
+    }
+    return dst;
+  };
+  LoraFactor f{adapter, rank, alpha, ingest(down, rank * K), ingest(up, N * rank)};
+  if (it == lora_.end()) {  // first adapter on this key: raw storage still holds the base weight
+    LoraTarget t;
+    t.backup = device_halves(w.numel());
+    CFGPP_CHECK_CUDA(cudaMemcpyAsync(t.backup.get(), w.p(), w.numel() * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
+    it = lora_.emplace(key, std::move(t)).first;
+  }
+  it->second.factors.push_back(std::move(f));
+  lora_adapters_ = std::max(lora_adapters_, adapter + 1);
+}
+
+std::set<std::string> WeightStore::lora_apply(const float* scales, int n, cudaStream_t stream, size_t* bytes) {
+  CFGPP_REQUIRE(n == lora_adapters_ && (n == 0 || scales), "one scale per adapter id (" + std::to_string(lora_adapters_) + ")");
+  std::set<std::string> touched;
+  for (auto& kv : lora_) {
+    const Weight& w = raw(kv.first);
+    const int N = static_cast<int>(w.shape[0]), K = static_cast<int>(w.numel() / N);
+    LoraMergeArgs a{};
+    for (const LoraFactor& f : kv.second.factors) {
+      a.down[a.n] = f.down.get();
+      a.up[a.n] = f.up.get();
+      a.rank[a.n] = f.rank;
+      a.coef[a.n] = scales[f.adapter] * f.alpha / static_cast<float>(f.rank);
+      *bytes += (static_cast<size_t>(N) + K) * f.rank * sizeof(__half);
+      ++a.n;
+    }
+    run_lora_merge(kv.second.backup.get(), a, N, K, w.p(), stream);
+    *bytes += 2 * w.numel() * sizeof(__half);
+    touched.insert(kv.first);
+  }
+  return touched;
+}
+
+std::set<std::string> WeightStore::lora_restore(cudaStream_t stream, size_t* bytes) {
+  std::set<std::string> touched;
+  for (auto& kv : lora_) {
+    const Weight& w = raw(kv.first);
+    CFGPP_CHECK_CUDA(cudaMemcpyAsync(w.p(), kv.second.backup.get(), w.numel() * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
+    *bytes += 2 * w.numel() * sizeof(__half);
+    touched.insert(kv.first);
+  }
+  return touched;
+}
+
+void WeightStore::lora_free(cudaStream_t stream) {
+  CFGPP_CHECK_CUDA(cudaStreamSynchronize(stream));  // the restore and the repacks still read what is freed here
+  lora_.clear();
+  lora_adapters_ = 0;
+}
+
+size_t WeightStore::lora_backup_bytes() const {
+  size_t b = 0;
+  for (auto& kv : lora_) b += raw(kv.first).numel() * sizeof(__half);
+  return b;
 }
 
 // ---- StreamKWorkspace -----------------------------------------------------------------------------------------------

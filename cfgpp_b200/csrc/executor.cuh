@@ -3,6 +3,7 @@
 #pragma once
 #include <map>
 #include <memory>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -35,6 +36,21 @@ class DeviceArena {
   size_t bytes_ = 0;
 };
 
+// ---- lora.cu ---------------------------------------------------------------------------------------------------
+constexpr int kMaxLoraPerTarget = 4;
+constexpr int kMaxLoraRank = 128;
+// The adapters merged into one weight: down_a [rank_a][K], up_a [N][rank_a] fp16 (device), coef_a fp32.
+struct LoraMergeArgs {
+  const __half* down[kMaxLoraPerTarget];
+  const __half* up[kMaxLoraPerTarget];
+  int rank[kMaxLoraPerTarget];
+  float coef[kMaxLoraPerTarget];
+  int n;
+};
+// out[n,k] = fp16(fp32(base[n,k]) + sum_a coef_a * sum_r up_a[n,r] * down_a[r,k]): fp32 accumulation on the tensor
+// cores, one rounding. Any N, K; ranks 1..128. out may be base.
+void run_lora_merge(const __half* base, const LoraMergeArgs& a, int N, int K, __half* out, cudaStream_t stream);
+
 // The raw fp16 weights of one model by key, plus the arena its repacked weights are allocated from.
 class WeightStore {
  public:
@@ -42,7 +58,8 @@ class WeightStore {
     struct Free {
       void operator()(__half* p) const { cudaFree(p); }
     };
-    std::unique_ptr<__half, Free> data;
+    using Ptr = std::unique_ptr<__half, Free>;
+    Ptr data;
     std::vector<int64_t> shape;
     __half* p() const { return data.get(); }
     size_t numel() const;
@@ -55,14 +72,45 @@ class WeightStore {
   __half* plain(const std::string& key) const { return raw(key).p(); }
   __half* plain(const std::string& key, size_t expect_numel) const;  // Error -11 on a size mismatch
   __half* packed_conv3x3(const std::string& key);                    // (Cout,Cin,3,3) -> [Cout][tap][Cin], cached
+  // packs `key` again into the buffer packed_conv3x3 returned, on `stream`; bytes read + written (0: never packed)
+  size_t refresh_conv3x3(const std::string& key, cudaStream_t stream);
+
+  // ---- LoRA adapters: W_eff = fp16(fp32(W) + sum_a c_a up_a down_a), c_a = scale_a * alpha_a / rank_a, always merged
+  // from a pristine copy of W into the raw tensor's own storage (pointers handed out by plain() stay valid) ----
+  // Adds adapter `adapter`'s factors for `key`: down [rank][K], up [N][rank] (device, fp16 or fp32 rounded to fp16),
+  // N = shape[0] and K = numel / N of raw(key). The key's first adapter takes its pristine backup. Nothing is merged
+  // until lora_apply.
+  void lora_add(int adapter, const std::string& key, const void* down, const void* up, int rank, float alpha, int dtype,
+                cudaStream_t stream);
+  // Merges every target at `scales` (one per adapter id 0..n-1) on `stream`; returns the keys written and adds the
+  // bytes read + written to *bytes.
+  std::set<std::string> lora_apply(const float* scales, int n, cudaStream_t stream, size_t* bytes);
+  // Copies every backup over its raw tensor on `stream` (the base bits) and returns those keys; lora_free then
+  // synchronises `stream` and releases factors and backups.
+  std::set<std::string> lora_restore(cudaStream_t stream, size_t* bytes);
+  void lora_free(cudaStream_t stream);
+  int lora_adapters() const { return lora_adapters_; }
+  int lora_targets() const { return static_cast<int>(lora_.size()); }
+  size_t lora_backup_bytes() const;
   template <typename T = __half>
   T* alloc(size_t n) {
     return packed_.alloc<T>(n);
   }
 
  private:
+  struct LoraFactor {
+    int adapter, rank;
+    float alpha;
+    Weight::Ptr down, up;
+  };
+  struct LoraTarget {
+    Weight::Ptr backup;
+    std::vector<LoraFactor> factors;
+  };
   std::map<std::string, Weight> raw_;
   std::map<std::string, __half*> conv3x3_;
+  std::map<std::string, LoraTarget> lora_;
+  int lora_adapters_ = 0;  // highest adapter id added + 1
   DeviceArena packed_;
 };
 

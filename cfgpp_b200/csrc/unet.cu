@@ -24,9 +24,13 @@ __global__ void pack_geglu_kernel(const __half* __restrict__ in, __half* __restr
   }
 }
 
+struct HeadMats {
+  const __half* p[3];
+};
+
 // rows of `nmat` stacked (heads*hd, K) matrices -> [(mat, head, hdp)][K], rows hd..hdp-1 of every head zero
-__global__ void pack_heads_rows_kernel(const __half* const* __restrict__ mats, __half* __restrict__ out, int nmat,
-                                       int heads, int hd, int hdp, int K) {
+__global__ void pack_heads_rows_kernel(HeadMats mats, __half* __restrict__ out, int nmat, int heads, int hd, int hdp,
+                                       int K) {
   const size_t n = static_cast<size_t>(nmat) * heads * hdp * K;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<size_t>(gridDim.x) * blockDim.x) {
@@ -36,7 +40,7 @@ __global__ void pack_heads_rows_kernel(const __half* const* __restrict__ mats, _
     t /= hdp;
     const int h = t % heads;
     const int m = t / heads;
-    out[i] = (r < hd) ? mats[m][(static_cast<size_t>(h) * hd + r) * K + k] : __float2half(0.f);
+    out[i] = (r < hd) ? mats.p[m][(static_cast<size_t>(h) * hd + r) * K + k] : __float2half(0.f);
   }
 }
 
@@ -98,91 +102,158 @@ void Unet::load_weight(const std::string& key, const void* data, const int64_t* 
   weights_.load(key, data, shape, ndim, dtype, stream);
 }
 
+__half* Unet::packed(const std::string& name, Pack recipe, size_t numel) {
+  auto it = packed_cache_.find(name);
+  if (it != packed_cache_.end()) return it->second.out;
+  recipe.out = weights_.alloc(numel);
+  run_pack(recipe, nullptr);
+  packed_cache_[name] = recipe;
+  return recipe.out;
+}
+
+size_t Unet::run_pack(const Pack& p, cudaStream_t stream) {
+  size_t total = 0;
+  switch (p.kind) {
+    case Pack::kCatRows:
+      for (auto& k : p.keys) {
+        const WeightStore::Weight& t = weights_.raw(k);
+        CFGPP_CHECK_CUDA(cudaMemcpyAsync(p.out + total, t.p(), t.numel() * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
+        total += t.numel();
+      }
+      break;
+    case Pack::kGeglu: {
+      const WeightStore::Weight& t = weights_.raw(p.keys[0]);
+      const int rows = static_cast<int>(t.shape[0]);
+      total = t.numel();
+      pack_geglu_kernel<<<grid_for(total), 256, 0, stream>>>(t.p(), p.out, rows / 2, p.is_bias ? 1 : static_cast<int>(t.shape[1]));
+      break;
+    }
+    case Pack::kHeadsRows: {
+      HeadMats mats{};
+      for (size_t i = 0; i < p.keys.size(); ++i) mats.p[i] = weights_.plain(p.keys[i]);
+      const int K = static_cast<int>(weights_.raw(p.keys[0]).shape[1]);
+      total = p.keys.size() * static_cast<size_t>(p.heads) * p.hdp * K;
+      pack_heads_rows_kernel<<<grid_for(total), 256, 0, stream>>>(mats, p.out, static_cast<int>(p.keys.size()), p.heads, p.hd, p.hdp, K);
+      break;
+    }
+    case Pack::kHeadsCols: {
+      const WeightStore::Weight& t = weights_.raw(p.keys[0]);
+      const int N = static_cast<int>(t.shape[0]);
+      total = static_cast<size_t>(N) * p.heads * p.hdp;
+      pack_heads_cols_kernel<<<grid_for(total), 256, 0, stream>>>(t.p(), p.out, N, p.heads, p.hd, p.hdp);
+      break;
+    }
+  }
+  CFGPP_CHECK_CUDA(cudaGetLastError());
+  return 2 * total * sizeof(__half);
+}
+
 __half* Unet::packed_cat_rows(const std::vector<std::string>& keys) {
   std::string name = "cat:";
-  for (auto& k : keys) name += k + "|";
-  auto it = packed_cache_.find(name);
-  if (it != packed_cache_.end()) return it->second;
   size_t total = 0;
-  for (auto& k : keys) total += weights_.raw(k).numel();
-  __half* out = weights_.alloc(total);
-  size_t off = 0;
   for (auto& k : keys) {
-    const WeightStore::Weight& t = weights_.raw(k);
-    CFGPP_CHECK_CUDA(cudaMemcpy(out + off, t.p(), t.numel() * sizeof(__half), cudaMemcpyDeviceToDevice));
-    off += t.numel();
+    name += k + "|";
+    total += weights_.raw(k).numel();
   }
-  packed_cache_[name] = out;
-  return out;
+  return packed(name, Pack{Pack::kCatRows, keys}, total);
 }
 
 __half* Unet::packed_geglu(const std::string& key, bool is_bias) {
-  auto it = packed_cache_.find("geglu:" + key);
-  if (it != packed_cache_.end()) return it->second;
   const WeightStore::Weight& t = weights_.raw(key);
-  const int rows = static_cast<int>(t.shape[0]);
-  const int K = is_bias ? 1 : static_cast<int>(t.shape[1]);
-  CFGPP_REQUIRE(rows % 256 == 0, "GEGLU width must be a multiple of 256: " + key);
-  __half* out = weights_.alloc(t.numel());
-  pack_geglu_kernel<<<grid_for(t.numel()), 256>>>(t.p(), out, rows / 2, K);
-  CFGPP_CHECK_CUDA(cudaGetLastError());
-  packed_cache_["geglu:" + key] = out;
-  return out;
+  CFGPP_REQUIRE(t.shape[0] % 256 == 0, "GEGLU width must be a multiple of 256: " + key);
+  Pack p{Pack::kGeglu, {key}};
+  p.is_bias = is_bias;
+  return packed("geglu:" + key, p, t.numel());
 }
 
 __half* Unet::packed_heads_rows(const std::vector<std::string>& keys, int heads, int hd, int hdp) {
   if (hd == hdp) return keys.size() == 1 ? weights_.plain(keys[0]) : packed_cat_rows(keys);
   std::string name = "heads_rows:";
   for (auto& k : keys) name += k + "|";
-  auto it = packed_cache_.find(name);
-  if (it != packed_cache_.end()) return it->second;
+  CFGPP_REQUIRE(keys.size() <= 3, "at most three stacked projections");
   const int K = static_cast<int>(weights_.raw(keys[0]).shape[1]);
-  std::vector<const __half*> ptrs;
   for (auto& k : keys) {
     const WeightStore::Weight& t = weights_.raw(k);
     CFGPP_REQUIRE(t.shape.size() >= 2 && t.shape[0] == heads * hd && t.shape[1] == K, "unexpected projection shape: " + k);
-    ptrs.push_back(t.p());
   }
-  const __half** dptrs = nullptr;
-  CFGPP_CHECK_CUDA(cudaMalloc(&dptrs, ptrs.size() * sizeof(__half*)));
-  CFGPP_CHECK_CUDA(cudaMemcpy(dptrs, ptrs.data(), ptrs.size() * sizeof(__half*), cudaMemcpyHostToDevice));
-  const size_t total = keys.size() * static_cast<size_t>(heads) * hdp * K;
-  __half* out = weights_.alloc(total);
-  pack_heads_rows_kernel<<<grid_for(total), 256>>>(dptrs, out, static_cast<int>(keys.size()), heads, hd, hdp, K);
-  CFGPP_CHECK_CUDA(cudaGetLastError());
-  CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
-  cudaFree(dptrs);
-  packed_cache_[name] = out;
-  return out;
+  Pack p{Pack::kHeadsRows, keys, heads, hd, hdp};
+  return packed(name, p, keys.size() * static_cast<size_t>(heads) * hdp * K);
 }
 
 __half* Unet::packed_heads_cols(const std::string& key, int heads, int hd, int hdp) {
   if (hd == hdp) return weights_.plain(key);
-  auto it = packed_cache_.find("heads_cols:" + key);
-  if (it != packed_cache_.end()) return it->second;
   const WeightStore::Weight& t = weights_.raw(key);
-  const int N = static_cast<int>(t.shape[0]);
   CFGPP_REQUIRE(t.shape[1] == heads * hd, "unexpected to_out shape: " + key);
-  const size_t total = static_cast<size_t>(N) * heads * hdp;
-  __half* out = weights_.alloc(total);
-  pack_heads_cols_kernel<<<grid_for(total), 256>>>(t.p(), out, N, heads, hd, hdp);
-  CFGPP_CHECK_CUDA(cudaGetLastError());
-  packed_cache_["heads_cols:" + key] = out;
-  return out;
+  Pack p{Pack::kHeadsCols, {key}, heads, hd, hdp};
+  return packed("heads_cols:" + key, p, static_cast<size_t>(t.shape[0]) * heads * hdp);
 }
 
-Unet::FoldedLN Unet::folded_ln(const std::string& cache_key, const __half* w_packed, int N, int K,
-                               const std::string& norm_prefix, const __half* bias_packed) {
+Unet::FoldedLN Unet::folded_ln(const std::string& cache_key, const std::vector<std::string>& keys, const __half* w_packed,
+                               int N, int K, const std::string& norm_prefix, const __half* bias_packed) {
   auto it = fold_cache_.find(cache_key);
-  if (it != fold_cache_.end()) return it->second;
-  FoldedLN f;
-  f.w = weights_.alloc(static_cast<size_t>(N) * K);
-  f.s = weights_.alloc<float>(N);
-  f.t = weights_.alloc<float>(N);
-  run_fold_ln(w_packed, weights_.plain(norm_prefix + ".weight"), weights_.plain(norm_prefix + ".bias"), bias_packed,
-              f.w, f.s, f.t, N, K, nullptr);
+  if (it != fold_cache_.end()) return it->second.f;
+  Fold f{{}, keys, w_packed, N, K, norm_prefix, bias_packed};
+  f.f.w = weights_.alloc(static_cast<size_t>(N) * K);
+  f.f.s = weights_.alloc<float>(N);
+  f.f.t = weights_.alloc<float>(N);
+  run_fold(f, nullptr);
   fold_cache_[cache_key] = f;
-  return f;
+  return f.f;
+}
+
+size_t Unet::run_fold(const Fold& f, cudaStream_t stream) {
+  run_fold_ln(f.w_packed, weights_.plain(f.norm_prefix + ".weight"), weights_.plain(f.norm_prefix + ".bias"),
+              f.bias_packed, f.f.w, f.f.s, f.f.t, f.N, f.K, stream);
+  return 2 * static_cast<size_t>(f.N) * f.K * sizeof(__half) + 2 * static_cast<size_t>(f.N) * sizeof(float);
+}
+
+size_t Unet::refresh_packed(const std::set<std::string>& keys, cudaStream_t stream) {
+  auto reads = [&](const std::vector<std::string>& src) {
+    return std::any_of(src.begin(), src.end(), [&](const std::string& k) { return keys.count(k) != 0; });
+  };
+  size_t bytes = 0;
+  for (auto& k : keys) bytes += weights_.refresh_conv3x3(k, stream);
+  for (auto& kv : packed_cache_)
+    if (reads(kv.second.keys)) bytes += run_pack(kv.second, stream);
+  for (auto& kv : fold_cache_)  // after the packers: a fold reads the packed matrix
+    if (reads(kv.second.keys)) bytes += run_fold(kv.second, stream);
+  return bytes;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// LoRA adapters
+// ------------------------------------------------------------------------------------------------------------
+void Unet::lora_add(int adapter, const std::string& key, const void* down, const void* up, int rank, float alpha,
+                    int dtype, cudaStream_t stream) {
+  CFGPP_REQUIRE(finalized_, "call cfgpp_finalize_weights first");
+  weights_.lora_add(adapter, key, down, up, rank, alpha, dtype, stream);
+}
+
+void Unet::lora_set_scales(const float* scales, int n, cudaStream_t stream) {
+  size_t bytes = 0;
+  const std::set<std::string> touched = weights_.lora_apply(scales, n, stream, &bytes);
+  prompt_stale_ = true;
+  lora_bytes_moved_ = bytes + refresh_packed(touched, stream);
+}
+
+void Unet::lora_clear(cudaStream_t stream) {
+  size_t bytes = 0;
+  const std::set<std::string> touched = weights_.lora_restore(stream, &bytes);
+  prompt_stale_ = true;
+  lora_bytes_moved_ = bytes + refresh_packed(touched, stream);
+  weights_.lora_free(stream);
+}
+
+void Unet::lora_stats(int* n_adapters, int* n_targets, size_t* backup_bytes, size_t* bytes_moved) const {
+  if (n_adapters) *n_adapters = weights_.lora_adapters();
+  if (n_targets) *n_targets = weights_.lora_targets();
+  if (backup_bytes) *backup_bytes = weights_.lora_backup_bytes();
+  if (bytes_moved) *bytes_moved = lora_bytes_moved_;
+}
+
+void Unet::require_fresh_prompt() const {
+  CFGPP_REQUIRE(!prompt_stale_, "LoRA weights changed since cfgpp_set_prompt: call cfgpp_set_prompt again (the "
+                                "cross-attention K/V and the add-embedding were computed from the previous weights)");
 }
 
 void Unet::finalize_weights(cudaStream_t stream) {
@@ -355,7 +426,7 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
     // --- self-attention ---
     __half* wqkv = packed_heads_rows({b + ".attn1.to_q.weight", b + ".attn1.to_k.weight", b + ".attn1.to_v.weight"},
                                      heads, hd, hdp);
-    const FoldedLN f1 = folded_ln(b + ".attn1.qkv", wqkv, 3 * Cp, C, b + ".norm1", nullptr);
+    const FoldedLN f1 = folded_ln(b + ".attn1.qkv", {b + ".attn1.to_q.weight", b + ".attn1.to_k.weight", b + ".attn1.to_v.weight"}, wqkv, 3 * Cp, C, b + ".norm1", nullptr);
     add_gemm(b + ".attn1.to_qkv(+norm1)",
              consumer(make_linear_op(tok, C, nullptr, 0, 0, f1.w, Mi, 3 * Cp, C, nullptr, nullptr, 0, 1, qkv, 3 * Cp, false),
                       f1, 0),
@@ -370,7 +441,7 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
              2.0 * Mi * static_cast<double>(C) * C);
     // --- cross-attention (K/V projected once per prompt by the prompt plan) ---
     __half* wq2 = packed_heads_rows({b + ".attn2.to_q.weight"}, heads, hd, hdp);
-    const FoldedLN f2 = folded_ln(b + ".attn2.q", wq2, Cp, C, b + ".norm2", nullptr);
+    const FoldedLN f2 = folded_ln(b + ".attn2.q", {b + ".attn2.to_q.weight"}, wq2, Cp, C, b + ".norm2", nullptr);
     add_gemm(b + ".attn2.to_q(+norm2)",
              consumer(make_linear_op(tok, C, nullptr, 0, 0, f2.w, Mi, Cp, C, nullptr, nullptr, 0, 1, qb, Cp, false), f2, 1),
              2.0 * Mi * static_cast<double>(C) * C);
@@ -394,7 +465,7 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
     // --- GEGLU feed-forward ---
     __half* wg = packed_geglu(b + ".ff.net.0.proj.weight", false);
     __half* bg = packed_geglu(b + ".ff.net.0.proj.bias", true);
-    const FoldedLN f3 = folded_ln(b + ".ff.geglu", wg, 8 * C, C, b + ".norm3", bg);
+    const FoldedLN f3 = folded_ln(b + ".ff.geglu", {b + ".ff.net.0.proj.weight"}, wg, 8 * C, C, b + ".norm3", bg);
     add_gemm(b + ".ff.geglu(+norm3)",
              consumer(make_linear_op(tok, C, nullptr, 0, 0, f3.w, Mi, 8 * C, C, nullptr, nullptr, 0, 1, ff, 4 * C, true), f3, 2));
     add_gemm(b + ".ff.out", producer([&](int bn) {
@@ -710,6 +781,7 @@ void Unet::set_prompt(const __half* ctx, int n_ctx, const __half* pooled, const 
     }
   }
   run_plan(prompt_plan_, stream);
+  prompt_stale_ = false;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -718,6 +790,7 @@ void Unet::set_prompt(const __half* ctx, int n_ctx, const __half* pooled, const 
 void Unet::unet_forward(const void* z, int z_dtype, float t, float in_scale, __half* eps_uc, __half* eps_c,
                         cudaStream_t stream) {
   CFGPP_REQUIRE(prepared_, "call cfgpp_prepare first");
+  require_fresh_prompt();
   StepState s{};
   s.t = t;
   s.in_scale = in_scale;
@@ -867,6 +940,7 @@ void Unet::run_steps(int first_step, int nsteps, cudaStream_t stream) {
   CFGPP_REQUIRE(prepared_ && nsteps_ > 0, "call cfgpp_set_schedule first");
   CFGPP_REQUIRE(first_step >= 0 && first_step + nsteps <= nsteps_, "step range outside the schedule");
   CFGPP_REQUIRE(!v_pred_ || v_ready_, "a v-prediction model needs cfgpp_set_v_coefs for this schedule");
+  require_fresh_prompt();
   ensure_graph(stream);
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(step_counter_, &first_step, sizeof(int), cudaMemcpyHostToDevice, stream));
   for (int i = 0; i < nsteps; ++i) CFGPP_CHECK_CUDA(cudaGraphLaunch(graph_exec_, stream));

@@ -31,6 +31,14 @@ class Unet {
   void load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
                    cudaStream_t stream);
   void finalize_weights(cudaStream_t stream);
+  // LoRA adapters (WeightStore::lora_*): factors are added per diffusers weight key after finalize; set_scales merges
+  // every target from its pristine backup into the raw weight and re-runs the packers that read it, on `stream`. No
+  // plan or graph pointer changes. The bound prompt goes stale (its K/V and add-embedding came from the old weights).
+  void lora_add(int adapter, const std::string& key, const void* down, const void* up, int rank, float alpha, int dtype,
+                cudaStream_t stream);
+  void lora_set_scales(const float* scales_host, int n, cudaStream_t stream);
+  void lora_clear(cudaStream_t stream);
+  void lora_stats(int* n_adapters, int* n_targets, size_t* backup_bytes, size_t* bytes_moved) const;
   void prepare(int batch, int h_lat, int w_lat);
   size_t workspace_bytes() const { return act_.bytes(); }
   double forward_flops() const { return forward_flops_; }
@@ -64,6 +72,16 @@ class Unet {
 
  private:
   // ---- weights ----
+  // A packed copy of raw weights and how it is produced, so that it can be produced again into the same buffer.
+  struct Pack {
+    enum Kind { kCatRows, kGeglu, kHeadsRows, kHeadsCols } kind;
+    std::vector<std::string> keys;  // the raw weights it reads
+    int heads = 0, hd = 0, hdp = 0;
+    bool is_bias = false;
+    __half* out = nullptr;
+  };
+  __half* packed(const std::string& name, Pack recipe, size_t numel);  // cached by name; packs on first use
+  size_t run_pack(const Pack& p, cudaStream_t stream);                  // returns bytes read + written
   __half* packed_cat_rows(const std::vector<std::string>& keys);
   __half* packed_geglu(const std::string& key, bool is_bias);
   __half* packed_heads_rows(const std::vector<std::string>& keys, int heads, int hd, int hdp);
@@ -73,9 +91,23 @@ class Unet {
     float* s;
     float* t;
   };
-  FoldedLN folded_ln(const std::string& cache_key, const __half* w_packed, int N, int K, const std::string& norm_prefix,
-                     const __half* bias_packed);
-  std::map<std::string, FoldedLN> fold_cache_;
+  struct Fold {
+    FoldedLN f;
+    std::vector<std::string> keys;  // the raw weights w_packed was packed from
+    const __half* w_packed;
+    int N, K;
+    std::string norm_prefix;
+    const __half* bias_packed;
+  };
+  FoldedLN folded_ln(const std::string& cache_key, const std::vector<std::string>& keys, const __half* w_packed, int N,
+                     int K, const std::string& norm_prefix, const __half* bias_packed);
+  size_t run_fold(const Fold& f, cudaStream_t stream);
+  // re-runs, on `stream`, every packer and LayerNorm fold that reads one of `keys`; returns bytes read + written
+  size_t refresh_packed(const std::set<std::string>& keys, cudaStream_t stream);
+  std::map<std::string, Fold> fold_cache_;
+  size_t lora_bytes_moved_ = 0;  // of the last lora_set_scales / lora_clear
+  bool prompt_stale_ = false;    // weights changed under the bound prompt: set_prompt must run again
+  void require_fresh_prompt() const;
 
   // ---- workspace ----
   __half* alloc_act(size_t numel) { return act_.alloc<__half>(numel); }
@@ -107,7 +139,7 @@ class Unet {
   StreamKWorkspace sk_;
 
   // packed weights: resolved lazily during plan building (finalize just validates + packs what is shape-independent)
-  std::map<std::string, __half*> packed_cache_;
+  std::map<std::string, Pack> packed_cache_;
   __half* temb_w_all_ = nullptr;  // [sumCout][time_embed_dim]
   __half* temb_b_all_ = nullptr;
   int temb_total_ = 0;

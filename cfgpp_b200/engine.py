@@ -32,6 +32,8 @@ class NativeUNet(nv.NativeHandle):
         self._nsteps = 0
         self._state_dtype = torch.float32
         self._bound = None  # strong references to the tensors of the bound prompt (see bind_prompt)
+        self._loras = {}  # name -> [adapter id, scale]
+        self._lora_per_key = {}  # weight key -> adapters targeting it
 
     def _create(self, desc, idx: int) -> None:
         nv.check(self.lib.cfgpp_create_ex(byref(desc), c_size_t(ctypes.sizeof(desc)), c_int(idx), byref(self._h)))
@@ -195,3 +197,64 @@ class NativeUNet(nv.NativeHandle):
         with torch.cuda.device(self.device):
             nv.check(self.lib.cfgpp_apply_step(self._h, c_int(step), nv.ptr(eps_uc.contiguous()),
                                                nv.ptr(eps_c.contiguous()), nv.stream_ptr()))
+
+    # ---- LoRA adapters ----------------------------------------------------------------------------------------
+    MAX_LORAS_PER_WEIGHT = 4
+
+    def add_lora(self, adapter, scale: float = 1.0, name: Optional[str] = None) -> str:
+        """Upload the factors of a `lora.LoraAdapter` and merge it at `scale` next to the adapters already loaded.
+        Returns its name (`name`, or lora<id>). The bound prompt is dropped: its K/V came from the old weights."""
+        idx = len(self._loras)
+        name = name or f"lora{idx}"
+        if name in self._loras:
+            raise ValueError(f"a LoRA named '{name}' is already loaded")
+        for key in adapter.targets:
+            if self._lora_per_key.get(key, 0) >= self.MAX_LORAS_PER_WEIGHT:
+                raise ValueError(f"{key} already carries {self.MAX_LORAS_PER_WEIGHT} LoRA adapters")
+        with torch.cuda.device(self.device):
+            for key, (down, up, alpha) in adapter.targets.items():
+                down = down.to(self.device, torch.float16).contiguous()
+                up = up.to(self.device, torch.float16).contiguous()
+                nv.check(self.lib.cfgpp_lora_add(self._h, c_int(idx), key.encode(), nv.ptr(down), nv.ptr(up),
+                                                 c_int(down.shape[0]), c_float(float(alpha)), c_int(F16),
+                                                 nv.stream_ptr()))
+                self._lora_per_key[key] = self._lora_per_key.get(key, 0) + 1
+        self._loras[name] = [idx, float(scale)]
+        self._apply_lora_scales()
+        return name
+
+    def set_lora_scales(self, scales: Dict[str, float]) -> None:
+        """Re-merge with new scales for the named adapters (the others keep theirs). Always from the pristine weights:
+        the result is the one a fresh engine loaded at these scales would hold, bit for bit."""
+        for name in scales:
+            if name not in self._loras:
+                raise KeyError(f"no LoRA named '{name}' (loaded: {sorted(self._loras)})")
+        for name, s in scales.items():
+            self._loras[name][1] = float(s)
+        self._apply_lora_scales()
+
+    def _apply_lora_scales(self) -> None:
+        by_id = sorted(self._loras.values())
+        arr = (c_float * len(by_id))(*[s for _, s in by_id])
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_lora_set_scales(self._h, arr, c_int(len(by_id)), nv.stream_ptr()))
+        self._bound = None
+
+    def clear_lora(self) -> None:
+        """Restore the base weights bit for bit and free factors and backups."""
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_lora_clear(self._h, nv.stream_ptr()))
+        self._loras, self._lora_per_key, self._bound = {}, {}, None
+
+    @property
+    def loras(self) -> Dict[str, float]:
+        """name -> scale of the loaded adapters."""
+        return {name: s for name, (_, s) in self._loras.items()}
+
+    @property
+    def lora_stats(self) -> dict:
+        """{'adapters', 'targets', 'backup_bytes': device memory of the pristine copies, 'bytes_moved': bytes the last
+        merge / clear read and wrote (merge and every refreshed packed layout), from shapes}."""
+        na, nt, bb, bm = c_int(), c_int(), c_size_t(), c_size_t()
+        nv.check(self.lib.cfgpp_lora_stats(self._h, byref(na), byref(nt), byref(bb), byref(bm)))
+        return {"adapters": na.value, "targets": nt.value, "backup_bytes": bb.value, "bytes_moved": bm.value}

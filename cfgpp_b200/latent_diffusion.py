@@ -29,6 +29,7 @@ from .conditioning import SyntheticTextEncoder
 from .text_encoder import CLIPTextConfig, get_conditioner
 from .config import UNetConfig, sd15_config
 from .latent_sdxl import _Scheduler, get_engine
+from .lora import LoraMixin
 
 ####### Factory #######
 __SOLVER__ = {}
@@ -66,7 +67,7 @@ def default_text_encoder(cfg: UNetConfig, device):
     return get_conditioner("", device, "sd15", cfg=small)
 
 
-class StableDiffusion(K.KDiffusionMixin):
+class StableDiffusion(K.KDiffusionMixin, LoraMixin):
     def __init__(self,
                  solver_config,
                  model_key: str = "runwayml/stable-diffusion-v1-5",

@@ -31,6 +31,7 @@ from .conditioning import SyntheticTextEncoder
 from .text_encoder import CLIPTextConfig, ClipConditioner, get_conditioner
 from .config import UNetConfig, sdxl_config, sdxl_refiner_config
 from .engine import NativeUNet
+from .lora import LoraMixin, is_lora_file, read_lora
 from .weights import load_safetensors_state_dict, synthetic_state_dict
 
 ####### Factory #######
@@ -71,13 +72,16 @@ def resolve_state_dict(model_key: str, cfg: UNetConfig, device):
     return synthetic_state_dict(cfg, seed=seed, device=device)
 
 
-def get_engine(model_key: str, cfg: UNetConfig, device, state_dict=None) -> NativeUNet:
+def get_engine(model_key: str, cfg: UNetConfig, device, state_dict=None, lora: Optional[str] = None) -> NativeUNet:
+    """The engine of (model_key, config, device), built once and shared. `lora`: a LoRA file that belongs to the
+    model's identity (SDXL-Lightning distributed as a LoRA): such an engine is cached apart from the plain base model's
+    and carries the adapter at scale 1."""
     dev = torch.device(device)
     if dev.type != "cuda":
         raise RuntimeError("cfgpp_b200 solvers run on CUDA (sm_90a) only — there is no CPU fallback on the product "
                            "path; the CPU eager baseline lives in oracle/ and bench.py")
     idx = dev.index if dev.index is not None else torch.cuda.current_device()
-    key = (model_key, cfg.name, idx)
+    key = (model_key if lora is None else f"{model_key}+lora:{lora}", cfg.name, idx)
     ent = _ENGINES.get(key)
     # an explicit state_dict is part of the identity: the entry keeps a strong reference to it and compares with `is`
     # (an id() of a dead dict can be recycled by a different one)
@@ -87,6 +91,8 @@ def get_engine(model_key: str, cfg: UNetConfig, device, state_dict=None) -> Nati
     # as soon as the last solver holding it goes away
     sd = state_dict if state_dict is not None else resolve_state_dict(model_key, cfg, torch.device("cuda", idx))
     eng = NativeUNet(cfg, sd, torch.device("cuda", idx))
+    if lora is not None:
+        eng.add_lora(read_lora(lora, cfg), 1.0)
     _ENGINES[key] = (eng, state_dict)
     return eng
 
@@ -139,7 +145,7 @@ def _prepare_engine(eng: NativeUNet, zt, uc, c, added_cond_kwargs, force: bool =
 REFINER_SOLVERS = ("ddim", "ddim_cfg++", "dpm++_2m_cfgpp")
 
 
-class SDXLRefiner:
+class SDXLRefiner(LoraMixin):
     """The second expert of SDXL 1.0 (stabilityai/stable-diffusion-xl-refiner-1.0): a UNet that takes over a base
     trajectory for its last, low-noise steps ("ensemble of experts"; diffusers' `denoising_end` on the base pipeline,
     `denoising_start` on the refiner's). Pass it to `sample(refiner=...)` of one of REFINER_SOLVERS.
@@ -155,7 +161,7 @@ class SDXLRefiner:
         self.text_enc = text_encoder
 
 
-class SDXL(K.KDiffusionMixin):
+class SDXL(K.KDiffusionMixin, LoraMixin):
     schedule_kind = "ddim"
     quantize = True
     supports_refiner = False  # the fused DDIM / DPM++ trajectories of REFINER_SOLVERS hand over to a refiner
@@ -168,11 +174,12 @@ class SDXL(K.KDiffusionMixin):
                  unet_config: Optional[UNetConfig] = None,
                  state_dict=None,
                  text_encoders=None,
-                 vae=None):
+                 vae=None,
+                 lora: Optional[str] = None):
         self.device = device
         self.dtype = dtype
         self.cfg = unet_config or sdxl_config()
-        self.unet = get_engine(model_key, self.cfg, device, state_dict)
+        self.unet = get_engine(model_key, self.cfg, device, state_dict, lora)
 
         # CLIP text towers on the native backend (text_encoder.py; the reference takes pipe.text_encoder /
         # pipe.text_encoder_2, latent_sdxl.py:46-49). Pass `text_encoders=(fn1, fn2)`, prompt -> (hidden, pooled), to override.
@@ -459,6 +466,11 @@ class SDXLLightning(SDXL):
                  device='cuda',
                  **kwargs):
         import os
+        if os.path.exists(light_model_ckpt) and is_lora_file(light_model_ckpt):
+            # the LoRA distribution (sdxl_lightning_*step_lora.safetensors): the base UNet with the file as an adapter
+            SDXL.__init__(self, solver_config, model_key=base_model_key, dtype=dtype, device=device,
+                          lora=light_model_ckpt, **kwargs)
+            return
         key = light_model_ckpt if os.path.exists(light_model_ckpt) else "synthetic:4321"
         if key.startswith("synthetic"):
             warnings.warn(f"Lightning checkpoint '{light_model_ckpt}' not found; using seeded synthetic UNet weights")

@@ -65,6 +65,9 @@ def main():
     parser.add_argument("--refiner_ckpt_dir", type=Path, default=None,
                         help="SDXL refiner pipeline directory (unet/, vae/, text_encoder_2/, tokenizer_2/); default: "
                              "seeded synthetic refiner weights")
+    parser.add_argument("--lora", action="append", default=[], metavar="PATH[:SCALE]",
+                        help="a UNet LoRA *.safetensors (diffusers / peft or kohya naming) merged at SCALE (default 1.0); "
+                             "repeatable, up to 4 adapters per weight")
     args = parser.parse_args()
     if args.denoising_end is not None and args.model != "sdxl":
         raise SystemExit("--denoising_end needs --model sdxl")
@@ -76,6 +79,9 @@ def main():
 
     sdxl = args.model in ("sdxl", "sdxl_lightning")
     solver = build_solver(args.model, args.method, solver_config, args.device, args.ckpt_dir)
+    for spec in args.lora:
+        path, _, scale = spec.partition(":")
+        solver.load_lora(path, float(scale) if scale else 1.0)
     native = solver.cfg.sample_size * 8
     height, width = args.height or native, args.width or native
     if height % 8 or width % 8:

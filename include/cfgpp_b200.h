@@ -117,6 +117,29 @@ int cfgpp_launches_per_step(cfgpp_handle* h, int* n);
  * algorithmic figure (diffusers recomputes the K/V projections every step). */
 int cfgpp_plan_stats(cfgpp_handle* h, double* step_flops, double* prompt_flops, int* prompt_launches);
 
+/* ---- LoRA adapters: replaces diffusers' load_lora_weights + fuse_lora. For a weight W viewed as [N, K] (K = every
+ * dimension after the first, a 3x3 conv in its (Cout,Cin,3,3) order) and adapters a with down_a [rank_a, K],
+ * up_a [N, rank_a], alpha_a and a user scale s_a:
+ *     W_eff = fp16( fp32(W) + sum_a c_a * sum_r up_a[n,r] down_a[r,k] ),   c_a = s_a * alpha_a / rank_a   (fp32)
+ * with fp16 factors, fp32 accumulation and ONE rounding. W_eff is always formed from a pristine copy of W, written into
+ * W's own device storage, and every kernel-native repack that reads W (conv layout, fused q|k|v and k|v, head padding,
+ * GEGLU interleave, concatenated time_emb_proj, LayerNorm fold) is re-run into the buffer it already occupies: the
+ * prepared plan and its captured graph stay as they are. ---------------------------------------------------------- */
+/* After cfgpp_finalize_weights. adapter: id 0..63; down_dev / up_dev: device tensors of `dtype` (fp32 is rounded to fp16
+ * once), copied; rank 1..128; at most 4 adapters per weight. The first adapter on a key takes that key's pristine
+ * backup. Fails naming the key when it is missing, 1-D, or already targeted by this adapter. Merges nothing yet. */
+int cfgpp_lora_add(cfgpp_handle* h, int adapter, const char* diffusers_weight_key, const void* down_dev,
+                   const void* up_dev, int rank, float alpha, int dtype, void* stream);
+/* Merges every targeted weight at scales_host[adapter id] (n_adapters = highest id + 1) and refreshes the packed copies,
+ * all enqueued on `stream`. Afterwards cfgpp_run_steps / cfgpp_unet_forward fail until cfgpp_set_prompt is called again:
+ * the cross-attention K/V and the add-embedding of the bound prompt came from the previous weights. */
+int cfgpp_lora_set_scales(cfgpp_handle* h, const float* scales_host, int n_adapters, void* stream);
+/* The base weights bit for bit; factors and backups are freed (synchronises `stream`). The prompt goes stale as above. */
+int cfgpp_lora_clear(cfgpp_handle* h, void* stream);
+/* backup_bytes: device memory held by pristine copies; bytes_moved: bytes the last set_scales / clear read and wrote
+ * (merge and every refreshed packer), computed from shapes. Any pointer may be NULL. */
+int cfgpp_lora_stats(cfgpp_handle* h, int* n_adapters, int* n_targets, size_t* backup_bytes, size_t* bytes_moved);
+
 /* ---- per-prompt conditioning: the tensors predict_noise concatenates (latent_sdxl.py:178-182, 249-257) ------ */
 /* ctx_dev: (2*batch, 77, cross_dim) fp16 = cat([uc, c]); pooled_dev: (add_rows, pooled_dim) fp16;
  * time_ids_dev: (add_rows, n_time_ids) fp32, n_time_ids = (projection_class_embeddings_input_dim - pooled_dim) /
@@ -253,6 +276,11 @@ int cfgpp_op_linear_lnfold(const void* a, const void* w, int M, int N, int K, co
  * [N,K] fp16, s[n] = sum_k wf[n,k], t[n] = sum_k beta[k] w[n,k] + bias[n] (fp32). */
 int cfgpp_op_fold_ln(const void* w, const void* gamma, const void* beta, const void* bias, void* wf, float* s, float* t,
                      int N, int K, void* stream);
+/* The LoRA merge kernel on its own: out [N,K] fp16 = fp16(fp32(base) + sum_a coefs_host[a] * up_a down_a), downs[a]
+ * [ranks[a], K] and ups[a] [N, ranks[a]] fp16 device tensors (host arrays of device pointers), ranks 1..128,
+ * n_adapters 0..4, any N and K. out may be base. */
+int cfgpp_op_lora_merge(const void* base, const void* const* downs, const void* const* ups, const int* ranks,
+                        const float* coefs_host, int n_adapters, int N, int K, void* out, void* stream);
 int cfgpp_op_conv3x3(const void* x, int B, int H, int W, int Cin, const void* w, int Cout, const void* bias,
                      const void* addend, int ld_add, int add_rows_per_group, void* out, int force_bn, void* stream);
 /* Downsample2D: 3x3, stride 2 on NHWC x [B,H,W,Cin] (even H, W) -> [B,H/2,W/2,Cout]; the A tile is fetched by TMA with
