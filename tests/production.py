@@ -1,0 +1,62 @@
+"""The production sizes every per-element kernel pin derives its cases from, and the attention launches of a UNet.
+
+`test_gpu_gemm.py`, `test_gpu_norms.py` and `test_gpu_attention.py` walk these tables through their derivation
+functions; `test_production_lists_cpu.py` asserts that every full-size model and text tower is listed, so a model added
+to `config.CONFIGS` without sizes fails on any machine."""
+
+# latent (h, w) per full-size UNet config of `config.CONFIGS`: the native resolution first, then the non-square sizes
+# whose levels are not multiples of 64 tokens (1216x832: 76x52 = 3952 tokens at level 1, 19x13 at level 3;
+# 1344x768: 21x12 at level 3)
+UNET_SIZES = {
+    "sdxl": ((128, 128), (152, 104)),
+    "sd15": ((64, 64),),
+    "sd2": ((96, 96), (96, 64)),
+    "sd2_base": ((64, 64),),
+    "sdxl_refiner": ((128, 128), (152, 104), (168, 96)),
+}
+
+# AutoencoderKL image (H, W): SDXL 1024² and the 1216x832 bucket, SD 2 768² and 768x512, SD v1.5 / SD 2-base 512²
+VAE_SIZES = ((1024, 1024), (1216, 832), (768, 768), (768, 512), (512, 512))
+
+# text towers of `text_encoder.CLIP_CONFIGS` and the prompt batches they run at (M = 77·B)
+TEXT_TOWERS = {"clip_l": (1, 2, 8), "clip_bigg": (1, 2, 8), "clip_h": (1, 2, 8)}
+
+N_CTX = 77
+
+
+def unet_sizes():
+    """(model, h, w) over the table, in table order."""
+    return [(m, h, w) for m, sizes in UNET_SIZES.items() for h, w in sizes]
+
+
+def size_tag(model, h, w):
+    """The case-id prefix of one (model, latent size): model and image width x height."""
+    return f"{model}-{8 * w}x{8 * h}"
+
+
+def unet_attn_launches(cfg, h, w, NB=4):
+    """Every flash-attention launch of a UNet's body on an h x w latent at UNet batch NB, in `Unet::prepare` order:
+    per transformer block the self-attention (heads, HW, HW, head_dim) and the cross-attention against the 77-token
+    prompt (heads, HW, 77, head_dim), with the plan name and the algorithmic FLOPs 4·NB·heads·Nq·Nkv·head_dim."""
+    ch, L, lpb = cfg.block_out_channels, len(cfg.block_out_channels), cfg.layers_per_block
+    tl, nh = cfg.transformer_layers_per_block, cfg.num_attention_heads
+    out = []
+
+    def transformer(p, level):
+        C, heads, H, W = ch[level], nh[level], h >> level, w >> level
+        hd = C // heads
+        for k in range(tl[level]):
+            for attn, nkv in (("attn1", H * W), ("attn2", N_CTX)):
+                out.append(dict(name=f"{p}.transformer_blocks.{k}.{attn}.sdpa", heads=heads, Nq=H * W, Nkv=nkv,
+                                hd=hd, flops=4.0 * NB * heads * H * W * nkv * hd))
+
+    for i in range(L):
+        if cfg.down_block_types[i].startswith("CrossAttn"):
+            for j in range(lpb):
+                transformer(f"down_blocks.{i}.attentions.{j}", i)
+    transformer("mid_block.attentions.0", L - 1)
+    for i in range(L):
+        if cfg.up_block_types[i].startswith("CrossAttn"):
+            for j in range(lpb + 1):
+                transformer(f"up_blocks.{i}.attentions.{j}", L - 1 - i)
+    return out

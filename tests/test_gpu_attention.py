@@ -183,22 +183,43 @@ def test_tile_boundary_sweep(name, hd):
                 check(f"{name} hd{hd} B{B} {Nq}x{Nkv}", heads(q, hdp), k, v, H, hd)
 
 
-PRODUCTION = [  # (heads, Nq, Nkv, head_dim): every attention shape of the UNets' transformer blocks
-    # SDXL 1024²: 64×64 latent tokens at 640 channels, 32×32 at 1280
-    (10, 4096, 4096, 64), (10, 4096, 77, 64), (20, 1024, 1024, 64), (20, 1024, 77, 64),
-    # SDXL landscape bucket 1024×768 (latent 96×128)
-    (10, 3072, 3072, 64), (10, 3072, 77, 64), (20, 768, 768, 64), (20, 768, 77, 64),
-    # SD v1.5 512²: eight heads of 40 / 80 / 160 at 64×64 ... 8×8 latent tokens (the mid block at 8×8)
-    (8, 4096, 4096, 40), (8, 4096, 77, 40), (8, 1024, 1024, 80), (8, 1024, 77, 80),
-    (8, 256, 256, 160), (8, 256, 77, 160), (8, 64, 64, 160), (8, 64, 77, 160)]
+def production_lists():
+    """{(model, (h, w)): [(case id, (heads, Nq, Nkv, head_dim))]}: the distinct attention shapes of every UNet at every
+    latent size of `production.py` (self-attention and cross-attention per attention level and the mid block)."""
+    import production as P
+    from cfgpp_b200 import config as C
+    out = {}
+    for m, h, w in P.unet_sizes():
+        shapes = []
+        for l in P.unet_attn_launches(C.CONFIGS[m](), h, w):
+            s = (l["heads"], l["Nq"], l["Nkv"], l["hd"])
+            if s not in shapes:
+                shapes.append(s)
+        out[(m, (h, w))] = [(f"{P.size_tag(m, h, w)}-{'self' if s[1] == s[2] else 'cross'}-H{s[0]}-{s[1]}x{s[2]}"
+                             f"-hd{s[3]}", s) for s in shapes]
+    return out
+
+
+def _production_cases():
+    """One case per shape over all models and sizes, under the id of the first (model, size) that has it."""
+    seen, cases = set(), []
+    for shapes in production_lists().values():
+        for cid, s in shapes:
+            if s not in seen:
+                seen.add(s)
+                cases.append(pytest.param(*s, id=cid))
+    return cases
 
 
 @pytest.mark.parametrize("name", ["flat", "peaked"])
-@pytest.mark.parametrize("H,Nq,Nkv,hd", PRODUCTION)
+@pytest.mark.parametrize("H,Nq,Nkv,hd", _production_cases())
 @pytest.mark.parametrize("NB", [4, 16])
 def test_production_shapes(NB, H, Nq, Nkv, hd, name):
-    """UNet batch NB = 4 / 16 (B = 2 / 8 images with CFG), in the layouts the UNet launches: self-attention reads q / k
-    / v as column slices of the fused [NB, N, 3·H·hdp] QKV buffer, cross-attention reads K / V as slices of the prompt's
+    """Every attention shape of the UNets' transformer blocks at every production size (`production.py`: SDXL and
+    the refiner at 1024² and 1216x832, whose 76x52 = 3952-token level ends in a 48-column KV tile after 61 full ones;
+    the refiner at 1344x768; SD 2 at 768² (9216 tokens) and 768x512; SD v1.5 and SD 2-base at 512²), at UNet batch
+    NB = 4 / 16 (B = 2 / 8 images with CFG), in the layouts the UNet launches: self-attention reads q / k / v as column
+    slices of the fused [NB, N, 3·H·hdp] QKV buffer, cross-attention reads K / V as slices of the prompt's
     [NB, 77, 2·H·hdp] KV buffer and q from its own [NB, N, H·hdp] buffer."""
     hdp = padded(hd)
     g = gen(NB * 100003 + Nq * 1009 + Nkv * 7 + hd + (name == "peaked"))

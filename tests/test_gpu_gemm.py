@@ -42,11 +42,12 @@ dynamic range (row scales 2^-8..2^8, column scales 2^-8..2^0), bias cancellation
 accumulator) and softmax rows (non-negative fp16 rows summing to 1, flat and peaked, against V at mean 10σ: the VAE's
 P·V at K = 16384). Every case asserts a finite output (except the overflow cases) and prints max |err|/E and rel-L2.
 
-The production launches are derived from the model configs (SDXL at 1024² and 1216x832, SD v1.5 at 512², UNet batch
-4; the VAE decoder and encoder at 1024² and 1216x832; CLIP-L and CLIP-bigG at M = B·77) and run in their production
-layouts; `test_unet_launch_list_matches_profile` checks the derived UNet list against the launches the native UNet
-reports. The LayerNorm-fold consumers run their shapes as plain linears here (the fold arithmetic has its own relative
-gate in `test_gpu_gemm_epilogues.py`)."""
+The production launches are derived from the model configs at the sizes of `production.py` (every full-size UNet at
+each of its latent sizes, UNet batch 4; the VAE decoder and encoder at each image size; every text tower at
+M = B·77), run once per distinct launch signature in their production layouts; `test_unet_launch_list_matches_profile`
+checks the derived UNet GEMM and attention lists against the launches the native UNet reports. The LayerNorm-fold
+consumers run their shapes as plain linears here (the fold arithmetic has its own relative gate in
+`test_gpu_gemm_epilogues.py`)."""
 import zlib
 
 import pytest
@@ -879,21 +880,36 @@ def unique_launches(launches):
     return out
 
 
-def _production_cases():
+def production_lists():
+    """{(model, size): [(case id, launch)]} over `production.py`: each UNet at each latent size, the VAE at each image
+    size, each text tower at each prompt batch. Launches are unique within a list, not across lists."""
+    import production as P
     from cfgpp_b200 import config as C
-    from cfgpp_b200.text_encoder import clip_bigg_config, clip_l_config
+    from cfgpp_b200.text_encoder import CLIP_CONFIGS
     from cfgpp_b200.vae import VAEConfig
-    cases = []
-    for model, h, w in [("sdxl", 128, 128), ("sdxl", 152, 104), ("sd15", 64, 64)]:
-        for i, l in enumerate(unique_launches(unet_gemm_launches(C.CONFIGS[model](), h, w))):
-            cases.append(pytest.param(l, id=f"{model}-{8 * w}x{8 * h}-{i}-{l['name']}"))
-    for H, W in [(1024, 1024), (1216, 832)]:
-        for i, l in enumerate(unique_launches(vae_gemm_launches(VAEConfig(), H, W))):
-            cases.append(pytest.param(l, id=f"vae-{W}x{H}-{i}-{l['name']}"))
-    for cfg in (clip_l_config(), clip_bigg_config()):
-        for B in (1, 2, 8):
-            for l in clip_gemm_launches(cfg, B):
-                cases.append(pytest.param(l, id=f"B{B}-{l['name']}"))
+    out = {}
+    for m, h, w in P.unet_sizes():
+        tag = P.size_tag(m, h, w)
+        out[(m, (h, w))] = [(f"{tag}-{i}-{l['name']}", l)
+                            for i, l in enumerate(unique_launches(unet_gemm_launches(C.CONFIGS[m](), h, w)))]
+    for H, W in P.VAE_SIZES:
+        out[("vae", (H, W))] = [(f"vae-{W}x{H}-{i}-{l['name']}", l)
+                                for i, l in enumerate(unique_launches(vae_gemm_launches(VAEConfig(), H, W)))]
+    for tower, batches in P.TEXT_TOWERS.items():
+        for B in batches:
+            out[(tower, B)] = [(f"B{B}-{l['name']}", l) for l in clip_gemm_launches(CLIP_CONFIGS[tower](), B)]
+    return out
+
+
+def _production_cases():
+    """One case per launch signature over all production lists: a shape shared by two models or sizes (SD v1.5 and
+    SD 2-base, the VAE at two sizes) runs once, under the id of the first list that has it."""
+    seen, cases = set(), []
+    for launches in production_lists().values():
+        for cid, l in launches:
+            if signature(l) not in seen:
+                seen.add(signature(l))
+                cases.append(pytest.param(l, id=cid))
     return cases
 
 
@@ -955,10 +971,10 @@ def test_production_launch(launch):
 
 
 def test_vae_pv_softmax_families():
-    """The VAE mid-block's P·V0 + b_v at K = 16384 (1024²) and 15808 (1216x832): flat and peaked softmax rows of P
-    against V0 at mean 10σ, the deepest accumulation of the project."""
+    """The VAE mid-block's P·V0 + b_v at K = 16384 (1024²), 15808 (1216x832), 9216 (768²) and 6144 (768x512): flat
+    and peaked softmax rows of P against V0 at mean 10σ, the deepest accumulation of the project."""
     g = gen(77)
-    for n, C in [(16384, 512), (15808, 512)]:
+    for n, C in [(16384, 512), (15808, 512), (9216, 512), (6144, 512)]:
         w = (torch.randn(C, n, generator=g, device=dev) + 10).half()
         b = torch.randn(C, generator=g, device=dev).half()
         for peaked in (False, True):
@@ -966,33 +982,62 @@ def test_vae_pv_softmax_families():
                        w, bias=b, family="softmax")
 
 
-@pytest.mark.parametrize("model,hw", [("tiny_sdxl", 32), ("tiny_sd15", 32), ("sdxl", 128)])
-def test_unet_launch_list_matches_profile(model, hw):
-    """The derived UNet launch list (name, kind, algorithmic FLOPs) equals the GEMM entries the native UNet's
-    profile_forward reports for its body and tail plans, so the production list cannot silently miss a launch."""
+def check_launch_lists_against_profile(model, h, w):
+    """Build the native UNet (synthetic weights) at batch 2 on an h x w latent, profile one forward and compare its
+    GEMM entries (kinds 0 / 1) with `unet_gemm_launches` and its attention entries (kind 2) with
+    `production.unet_attn_launches`: the same names, kinds and algorithmic FLOPs."""
+    import production as P
     from cfgpp_b200 import config as C, weights as Wt
     from cfgpp_b200.engine import NativeUNet
     cfg = C.CONFIGS[model]()
     sd = Wt.synthetic_state_dict(cfg, seed=3, device=dev)
     net = NativeUNet(cfg, sd, dev)
     try:
-        net.prepare(2, hw, hw)
+        net.prepare(2, h, w)
         g = torch.Generator().manual_seed(0)
         ctx = torch.randn(4, 77, cfg.cross_attention_dim, generator=g).half().to(dev)
         if cfg.addition_embed_type == "text_time":
+            # original size, crop top-left, then the target size (base) or the aesthetic score (refiner)
+            ids = [h * 8.0, w * 8, 0, 0, h * 8, w * 8][:cfg.num_time_ids]
+            if cfg.num_time_ids == 5:
+                ids[4] = 6.0
             net.set_prompt(ctx, torch.randn(4, cfg.pooled_dim, generator=g).half().to(dev),
-                           torch.tensor([[hw * 8.0, hw * 8, 0, 0, hw * 8, hw * 8]] * 4).to(dev))
+                           torch.tensor([ids] * 4).to(dev))
         else:
             net.set_prompt(ctx)
-        prof = net.profile_forward(torch.randn(2, 4, hw, hw, generator=g).to(dev), 500.0)
+        prof = net.profile_forward(torch.randn(2, 4, h, w, generator=g).to(dev), 500.0)
     finally:
         net.close()
+        del sd
+        torch.cuda.empty_cache()
     got = sorted((n, "conv" if k == 1 else "linear", f) for n, k, f, _ in prof if k in (0, 1))
-    want = sorted((l["name"], l["kind"], l["flops"]) for l in unet_gemm_launches(cfg, hw, hw)
+    want = sorted((l["name"], l["kind"], l["flops"]) for l in unet_gemm_launches(cfg, h, w)
                   if l.get("plan") != "prompt")
     assert len(got) == len(want), f"{len(got)} GEMM launches reported, {len(want)} derived"
     for x, y in zip(got, want):
         assert x[:2] == y[:2] and abs(x[2] - y[2]) <= 1e-9 * y[2], f"reported {x}, derived {y}"
+    got = sorted((n, f) for n, k, f, _ in prof if k == 2)
+    want = sorted((l["name"], l["flops"]) for l in P.unet_attn_launches(cfg, h, w))
+    assert len(got) == len(want), f"{len(got)} attention launches reported, {len(want)} derived"
+    for x, y in zip(got, want):
+        assert x[0] == y[0] and abs(x[1] - y[1]) <= 1e-9 * y[1], f"reported {x}, derived {y}"
+    print(f"[gemm] {model} {8 * w}x{8 * h}: {len(prof)} profiled launches, GEMM and attention lists match")
+
+
+@pytest.mark.parametrize("model,hw", [("tiny_sdxl", 32), ("tiny_sd15", 32), ("sdxl", 128)])
+def test_unet_launch_list_matches_profile(model, hw):
+    """The derived UNet launch lists (GEMM: name, kind, algorithmic FLOPs; attention: name, FLOPs) equal the entries
+    the native UNet's profile_forward reports for its body and tail plans, so the production lists cannot silently miss
+    a launch."""
+    check_launch_lists_against_profile(model, hw, hw)
+
+
+@pytest.mark.parametrize("model,h,w", [("sd2", 96, 96), ("sd2", 96, 64), ("sdxl_refiner", 128, 128),
+                                       ("sdxl_refiner", 152, 104)])
+def test_unet_launch_list_matches_profile_rect(model, h, w):
+    """The same cross-check for SD 2 at 768² and 768x512 and the SDXL refiner (5 time ids, 4 levels of 384..1536
+    channels, about 4.5 GB of weights) at 1024² and 1216x832."""
+    check_launch_lists_against_profile(model, h, w)
 
 
 # ================================================================================================= coverage (last)

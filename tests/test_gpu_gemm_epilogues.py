@@ -239,14 +239,47 @@ def test_lnfold_consumer_rejects_bias():
     assert st != 0 and b"bias" in lib.cfgpp_last_error()
 
 
+def producer_bn(nv, attn, wo, bo, tok):
+    """The tile width the UNet's LayerNorm-fold producer takes (`producer` in unet.cu): the launch's own schedule, or
+    when that width does not divide C the first of 160, 128, 64 that does."""
+    C = wo.shape[0]
+    bn = nv.linear_schedule(attn, wo, bo, tok, out=tok)["bn"]
+    return bn if C % bn == 0 else next(b for b in (160, 128, 64) if C % b == 0)
+
+
+UNET_CHAINS = [  # (M, C) at UNet batch 4 on the production latents: every transformer level
+    pytest.param(4 * 64 * 64, 768, id="sdxl_refiner-1024x1024-C768"),
+    pytest.param(4 * 32 * 32, 1536, id="sdxl_refiner-1024x1024-C1536"),
+    pytest.param(4 * 16 * 16, 1536, id="sdxl_refiner-1024x1024-mid-C1536"),
+    pytest.param(4 * 76 * 52, 768, id="sdxl_refiner-832x1216-C768"),
+    pytest.param(4 * 38 * 26, 1536, id="sdxl_refiner-832x1216-C1536"),
+    pytest.param(4 * 96 * 96, 320, id="sd2-768x768-C320"),
+    pytest.param(4 * 48 * 48, 640, id="sd2-768x768-C640"),
+    pytest.param(4 * 24 * 24, 1280, id="sd2-768x768-C1280"),
+    pytest.param(4 * 12 * 12, 1280, id="sd2-768x768-mid-C1280"),
+]
+
+
+@pytest.mark.parametrize("M,C", UNET_CHAINS)
+def test_lnfold_chain_production(M, C):
+    """The chain of `test_lnfold_chain_as_unet` at the SDXL refiner's and SD 2's widths and production M (head dim 64:
+    Cp = C), with the producer at the tile width the UNet picks, so the consumers see the real count of partial
+    statistics (2·C / BN: up to 24 at C = 1536)."""
+    lnfold_chain(M, C, C, None, seed=M + C + 1, reps=3)
+
+
 @pytest.mark.parametrize("M,C,Cp,bn", [(16384, 640, 640, 128), (4096, 1280, 1280, 256), (8192, 320, 512, 160),
                                        (2048, 1280, 1536, 64)])
 def test_lnfold_chain_as_unet(M, C, Cp, bn):
     """The transformer block's wiring: to_out writes `tok` in place (+ residual) and its statistics, then
     to_qkv(+norm1) and ff.geglu(+norm3) read `tok` with the same statistics buffer. SDXL (C = 640 / 1280, head dim 64)
     and SD v1.5 (padded heads Cp) shapes. Twelve repetitions are bit-identical."""
+    lnfold_chain(M, C, Cp, bn, seed=M + C, reps=12)
+
+
+def lnfold_chain(M, C, Cp, bn, seed, reps):
     from cfgpp_b200 import _native as nv
-    g = torch.Generator().manual_seed(M + C)
+    g = torch.Generator().manual_seed(seed)
     attn, wo, bo = rnd(g, M, Cp), rnd(g, C, Cp, scale=Cp ** -0.5), rnd(g, C)
     tok0 = rnd(g, M, C, shift=0.5)
     gamma, beta = rnd(g, C, scale=0.2, shift=1.0), rnd(g, C, scale=0.2)
@@ -264,8 +297,10 @@ def test_lnfold_chain_as_unet(M, C, Cp, bn):
         hff = nv.op_linear_lnfold(tok, *ff, stats, geglu=True)
         return tok.clone(), stats, qkv, hff
 
+    if bn is None:
+        bn = producer_bn(nv, attn, wo, bo, tok)
     first = run()
-    what = f"chain {M}x{C} Cp{Cp} BN{bn}"
+    what = f"chain {M}x{C} Cp{Cp} BN{bn} ({2 * -(-C // bn)} statistics parts)"
     gate_linear(what + " to_out", first[0], attn, wo, bo, tok0, 1, bn)
     check_stats(first[0], first[1], bn, what)
     for name, got, w, b, geglu in (("to_qkv", first[2], wqkv, None, False), ("ff.geglu", first[3], wff, bff, True)):
@@ -275,7 +310,7 @@ def test_lnfold_chain_as_unet(M, C, Cp, bn):
         ef, eu = rel_l2_64(got, ref), rel_l2_64(unfused, ref)
         print(f"[epilogue] {what} {name}(+norm): fused rel-L2 {ef:.3e}, unfused {eu:.3e}")
         assert ef <= 1.5 * eu + FOLD_FLOOR
-    for _ in range(12):
+    for _ in range(reps):
         again = run()
         assert all(torch.equal(x, y) for x, y in zip(again, first))
 

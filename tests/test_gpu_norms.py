@@ -312,12 +312,28 @@ def vae_gn_launches(cfg, H, W):
     return sorted(enc), sorted(dec)
 
 
-UNET_SIZES = [("sdxl", 128, 128), ("sdxl", 152, 104), ("sd15", 64, 64)]  # 1024², the 1216x832 bucket, 512²
+def production_lists():
+    """{(model, (h, w)): [(C1, C2, HW, silu, eps)]} of every UNet at every latent size of `production.py`, and
+    {("vae", (H, W)): [(part, C, HW, silu)]} of the AutoencoderKL at every image size."""
+    import production as P
+    from cfgpp_b200 import config as C
+    from cfgpp_b200.vae import VAEConfig
+    out = {(m, (h, w)): unet_gn_launches(C.CONFIGS[m](), h, w) for m, h, w in P.unet_sizes()}
+    for H, W in P.VAE_SIZES:
+        enc, dec = vae_gn_launches(VAEConfig(), H, W)
+        out[("vae", (H, W))] = [("decoder", *l) for l in dec] + [("encoder", *l) for l in enc]
+    return out
 
 
 def _unet_cases():
-    from cfgpp_b200 import config as C
-    return [(m, h, w, *l) for m, h, w in UNET_SIZES for l in unet_gn_launches(C.CONFIGS[m](), h, w)]
+    """One case per launch over all UNets and sizes: SD 2-base repeats SD v1.5's list, which runs once."""
+    seen, cases = set(), []
+    for (m, (h, w)), launches in production_lists().items():
+        for l in launches:
+            if m != "vae" and l not in seen:
+                seen.add(l)
+                cases.append((m, h, w, *l))
+    return cases
 
 
 def test_unet_launch_list():
@@ -332,8 +348,9 @@ def test_unet_launch_list():
 
 @pytest.mark.parametrize("model,h,w,C1,C2,HW,silu,eps", _unet_cases())
 def test_groupnorm_unet_launches(model, h, w, C1, C2, HW, silu, eps):
-    """Every GroupNorm launch of the SDXL UNet at 1024² and at the 1216x832 bucket and of SD v1.5 at 512², at UNet
-    batch 4, with per-image and per-group means and scales."""
+    """Every GroupNorm launch of every UNet at every latent size of `production.py`, at UNet batch 4, with per-image
+    and per-group means and scales. The SDXL refiner brings 12..96 channels per group (384..3072 channels) and concat
+    groups that straddle the source boundary (1536 + 768, 768 + 384); SD 2 at 768² puts 9216 pixels in a level."""
     g = gen(C1 * 3 + C2 + HW)
     x, gamma, beta = gn_inputs("per_group", g, 4, HW, C1 + C2, mu_max=30.0)
     x = (x.float() * torch.exp2(torch.rand(4, 1, 1, generator=g, device=dev) * 4 - 2)).half()
@@ -342,18 +359,20 @@ def test_groupnorm_unet_launches(model, h, w, C1, C2, HW, silu, eps):
 
 
 def _vae_cases():
-    from cfgpp_b200.vae import VAEConfig
-    out = []
-    for H, W in [(1024, 1024), (1216, 832)]:
-        enc, dec = vae_gn_launches(VAEConfig(), H, W)
-        out += [("decoder", H, W, *l) for l in dec] + [("encoder", H, W, *l) for l in enc]
-    return out
+    """One case per (part, launch) over all VAE sizes."""
+    seen, cases = set(), []
+    for (m, (H, W)), launches in production_lists().items():
+        for part, *l in launches:
+            if m == "vae" and (part, *l) not in seen:
+                seen.add((part, *l))
+                cases.append((part, H, W, *l))
+    return cases
 
 
 @pytest.mark.parametrize("part,H,W,C,HW,silu", _vae_cases())
 def test_groupnorm_vae_launches(part, H, W, C, HW, silu):
-    """Every GroupNorm launch of the AutoencoderKL encoder and decoder at 1024² and at 1216x832 (up to 4 M elements
-    per group), per-group means and scales."""
+    """Every GroupNorm launch of the AutoencoderKL encoder and decoder at every image size of `production.py` (up to
+    4 M elements per group at 1024²), per-group means and scales."""
     g = gen(C + HW)
     x, gamma, beta = gn_inputs("per_group", g, 1, HW, C, mu_max=30.0)
     gn_check(f"VAE {part} {H}x{W} HW{HW} C{C} silu={silu}", x, gamma, beta, 1e-6, silu)

@@ -14,6 +14,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from cfgpp_b200.config import sdxl_refiner_config
 from helpers import coef_variants, rel_l2
 
 pytestmark = pytest.mark.gpu
@@ -77,7 +78,7 @@ def _check_sincos(what, got, vals, dim):
     assert worst <= 1.0, f"{what}: error {worst:.3f}x the bound"
 
 
-@pytest.mark.parametrize("dim", [320, 256, 1280])
+@pytest.mark.parametrize("dim", [320, 256, 1280, 384])
 def test_timestep_embedding_one_row_per_value(dim):
     from cfgpp_b200 import _native as nv
     ts = [0.0, 1.0, 517.37, 83.125, 999.0, 1024.0, 2048.0]
@@ -90,28 +91,43 @@ def test_timestep_embedding_one_row_per_value(dim):
     _check_sincos(f"sincos dim {dim} {len(ts)} rows", out, vals, dim)
 
 
-def test_timestep_embedding_sdxl_add_layout():
-    """The SDXL add-embedding input [pooled (PD) | 6 time ids x 256]: one launch per id, val_stride 6,
+def _check_add_layout(what, tids, seed):
+    """The text_time add-embedding input [pooled (PD) | NT time ids x 256]: one launch per id, val_stride NT,
     col_off = PD + j 256; columns outside each slice keep what was there."""
     from cfgpp_b200 import _native as nv
     PD, ATE = 1280, 256
-    tids = torch.tensor([[1024., 1024, 0, 0, 1024, 1024], [768, 1344, 64, 32, 1024, 1024],
-                         [517.37, 999, 1, 2048, 896, 1152], [2048, 2048, 0, 0, 2048, 2048]], device=dev)
-    n = tids.shape[0]
-    g = torch.Generator().manual_seed(3)
-    before = rnd(g, n, PD + 6 * ATE)
+    n, NT = tids.shape
+    g = torch.Generator().manual_seed(seed)
+    before = rnd(g, n, PD + NT * ATE)
     out = before.clone()
     flat = tids.reshape(-1).contiguous()
-    for j in range(6):
-        nv.op_timestep_embedding(flat[j:], n, ATE, out=out, val_stride=6, col_off=PD + j * ATE)
+    for j in range(NT):
+        nv.op_timestep_embedding(flat[j:], n, ATE, out=out, val_stride=NT, col_off=PD + j * ATE)
     torch.cuda.synchronize()
     assert torch.equal(bits(out[:, :PD]), bits(before[:, :PD])), "columns before the time-id slices were written"
-    for j in range(6):
-        _check_sincos(f"sincos SDXL time id {j}", out[:, PD + j * ATE:PD + (j + 1) * ATE], tids[:, j].contiguous(), ATE)
+    for j in range(NT):
+        _check_sincos(f"sincos {what} time id {j}", out[:, PD + j * ATE:PD + (j + 1) * ATE], tids[:, j].contiguous(),
+                      ATE)
     narrow = before.clone()[:, :PD + 2 * ATE].contiguous()
     mark = narrow.clone()
-    nv.op_timestep_embedding(flat, n, ATE, out=narrow, val_stride=6, col_off=PD)
+    nv.op_timestep_embedding(flat, n, ATE, out=narrow, val_stride=NT, col_off=PD)
     assert torch.equal(bits(narrow[:, PD + ATE:]), bits(mark[:, PD + ATE:])), "columns after the slice were written"
+
+
+def test_timestep_embedding_sdxl_add_layout():
+    """The SDXL base's 6 time ids: original size, crop top-left, target size."""
+    tids = torch.tensor([[1024., 1024, 0, 0, 1024, 1024], [768, 1344, 64, 32, 1024, 1024],
+                         [517.37, 999, 1, 2048, 896, 1152], [2048, 2048, 0, 0, 2048, 2048]], device=dev)
+    _check_add_layout("SDXL", tids, 3)
+
+
+def test_timestep_embedding_refiner_add_layout():
+    """The SDXL refiner's 5 time ids (2560 = 1280 + 5 x 256 input columns): original size, crop top-left and the
+    aesthetic score (6 for the positive prompt, 2.5 for the negative, and others)."""
+    tids = torch.tensor([[1024., 1024, 0, 0, 6], [1216, 832, 0, 0, 2.5], [1344, 768, 64, 32, 7.25],
+                         [517.37, 999, 1, 2048, 0], [2048, 2048, 0, 0, 10]], device=dev)
+    assert tids.shape[1] == sdxl_refiner_config().num_time_ids
+    _check_add_layout("SDXL refiner", tids, 5)
 
 
 # ---- small_linear -----------------------------------------------------------------------------------------------
@@ -128,8 +144,19 @@ def _linear_ref(x, w, b, addend=None, out_silu=False):
 SDXL_TEMB_TOTAL = 2 * 320 + 2 * 640 + 2 * 1280 + 2 * 1280 + 3 * 1280 + 3 * 640 + 3 * 320  # every resnet's time_emb_proj
 
 
+def temb_total(cfg):
+    """Rows of the concatenated time_emb_proj of every resnet (down, mid, up) of a UNet config."""
+    ch, lpb = cfg.block_out_channels, cfg.layers_per_block
+    return lpb * sum(ch) + 2 * ch[-1] + (lpb + 1) * sum(ch)
+
+
+REFINER_TEMB_TOTAL = temb_total(sdxl_refiner_config())
+
+
 @pytest.mark.parametrize("R", [1, 2, 7, 16])
-@pytest.mark.parametrize("K,N", [(320, 1000), (1280, 1280), (2816, 1000), (1280, SDXL_TEMB_TOTAL)])
+@pytest.mark.parametrize("K,N", [(320, 1000), (1280, 1280), (2816, 1000), (1280, SDXL_TEMB_TOTAL),
+                                 # the SDXL refiner: time_embedding.linear_1 / _2, add_embedding.linear_1, time_emb_proj
+                                 (384, 1536), (1536, 1536), (2560, 1536), (1536, REFINER_TEMB_TOTAL)])
 def test_small_linear(R, K, N):
     from cfgpp_b200 import _native as nv
     g = torch.Generator().manual_seed(R * 131 + K + N)
@@ -201,7 +228,9 @@ def _conv_in_input(z, scale):
 
 
 @pytest.mark.parametrize("Cout,B,H,W", [(320, 8, 8, 8), (320, 2, 64, 64), (320, 1, 96, 128), (128, 1, 152, 104),
-                                        (128, 3, 12, 4), (512, 1, 64, 64), (512, 8, 8, 4), (512, 1, 152, 104)])
+                                        (128, 3, 12, 4), (512, 1, 64, 64), (512, 8, 8, 4), (512, 1, 152, 104),
+                                        # the SDXL refiner: 37·384 fp32 of weights and bias, over 48 KB of shared memory
+                                        (384, 2, 128, 128), (384, 1, 152, 104), (384, 3, 12, 4)])
 def test_conv_in(Cout, B, H, W):
     from cfgpp_b200 import _native as nv
     g = torch.Generator().manual_seed(Cout + B * H + W)
@@ -226,9 +255,18 @@ def test_conv_in(Cout, B, H, W):
 
 @pytest.mark.parametrize("B,H,W", [(1, 17, 12), (3, 13, 20), (8, 9, 14)])
 def test_conv_out_step(B, H, W):
+    _conv_out_step_case(B, H, W, 320, B * 100 + H + W)
+
+
+@pytest.mark.parametrize("B,H,W", [(1, 17, 12), (3, 13, 20), (2, 128, 128)])
+def test_conv_out_step_refiner(B, H, W):
+    """The SDXL refiner's conv_out (Cin 384: 27 KB of weights in shared memory), the last at its 1024² latent."""
+    _conv_out_step_case(B, H, W, 384, B * 100 + H + W + 384)
+
+
+def _conv_out_step_case(B, H, W, Cin, seed):
     from cfgpp_b200 import _native as nv
-    Cin = 320
-    g = torch.Generator().manual_seed(B * 100 + H + W)
+    g = torch.Generator().manual_seed(seed)
     x = (rnd(g, 2 * B, H, W, Cin).float().abs() * 0.7 - 0.2).half()  # roughly GroupNorm + SiLU output
     w, b = rnd(g, 4, Cin, 3, 3, scale=(9 * Cin) ** -0.5), rnd(g, 4, scale=0.2)
     wp = w.permute(0, 2, 3, 1).reshape(4, 9, Cin).contiguous()
@@ -308,7 +346,7 @@ def _softmax_rows(n, g):
     return rows
 
 
-@pytest.mark.parametrize("n", [64, 4096, 16384])
+@pytest.mark.parametrize("n", [64, 4096, 16384, 9216, 6144])
 def test_vae_row_softmax(n):
     """p = softmax(s / sqrt(512)) per row, against the fp64 softmax of the fp16 scores. The kernel normalises in fp32
     and rounds P once; the gate per element is 1 fp16 ulp of p, or 2^-25 (half the subnormal spacing) below the normal
@@ -414,7 +452,8 @@ def test_clip_embed_and_gather_rows():
     assert torch.equal(bits(got), bits(x[torch.arange(B, device=dev) * T + index.long()])), "clip_gather_rows"
 
 
-@pytest.mark.parametrize("B,T,heads", [(1, 1, 12), (2, 2, 12), (16, 77, 12), (4, 77, 20), (2, 128, 20)])
+@pytest.mark.parametrize("B,T,heads", [(1, 1, 12), (2, 2, 12), (16, 77, 12), (4, 77, 20), (2, 128, 20),
+                                       (1, 77, 16), (8, 77, 16), (3, 128, 16)])  # 16 heads: ViT-H
 def test_clip_attention(B, T, heads):
     from cfgpp_b200 import _native as nv
     D = 64 * heads

@@ -1,0 +1,110 @@
+"""The production size table (`production.py`) and the per-element case lists derived from it, checked without a GPU:
+every full-size UNet config and every text tower has sizes, and the GEMM / conv, attention and GroupNorm case lists
+cover every (model, size). A model added to `config.CONFIGS` or `text_encoder.CLIP_CONFIGS` without sizes fails here,
+on any machine, before its kernels go unpinned."""
+import pytest
+
+import production as P
+import test_gpu_attention as TA
+import test_gpu_gemm as TG
+import test_gpu_norms as TN
+from cfgpp_b200 import config as C
+from cfgpp_b200.text_encoder import CLIP_CONFIGS
+
+# the sizes the pins must keep: each model's native resolution and the non-square sizes whose levels end in partial
+# tiles (removing one of these from the table fails here)
+REQUIRED_UNET = {"sdxl": {(128, 128), (152, 104)}, "sd15": {(64, 64)}, "sd2": {(96, 96), (96, 64)},
+                 "sd2_base": {(64, 64)}, "sdxl_refiner": {(128, 128), (152, 104), (168, 96)}}
+REQUIRED_VAE = {(1024, 1024), (1216, 832), (768, 768), (768, 512), (512, 512)}
+
+
+def full_size(names):
+    return sorted(n for n in names if not n.startswith("tiny"))
+
+
+def test_every_unet_config_has_sizes():
+    missing = [m for m in full_size(C.CONFIGS) if not P.UNET_SIZES.get(m)]
+    assert not missing, f"full-size UNet configs without production sizes: {missing}"
+    for m, sizes in P.UNET_SIZES.items():
+        cfg = C.CONFIGS[m]()
+        assert (cfg.sample_size, cfg.sample_size) in sizes, f"{m}: its native {cfg.sample_size}² latent is not listed"
+        down = 1 << (len(cfg.block_out_channels) - 1)
+        for h, w in sizes:
+            assert h % down == 0 and w % down == 0, f"{m}: latent {h}x{w} is not a multiple of {down}"
+
+
+def test_required_sizes_listed():
+    for m, sizes in REQUIRED_UNET.items():
+        assert sizes <= set(P.UNET_SIZES.get(m, ())), f"{m}: {sorted(sizes - set(P.UNET_SIZES.get(m, ())))} removed"
+    assert REQUIRED_VAE <= set(P.VAE_SIZES), f"VAE sizes removed: {sorted(REQUIRED_VAE - set(P.VAE_SIZES))}"
+
+
+def test_every_text_tower_listed():
+    missing = [t for t in full_size(CLIP_CONFIGS) if not P.TEXT_TOWERS.get(t)]
+    assert not missing, f"text towers without prompt batches: {missing}"
+
+
+def expected_keys(vae=True, towers=True):
+    keys = {(m, (h, w)) for m, h, w in P.unet_sizes()}
+    if vae:
+        keys |= {("vae", hw) for hw in P.VAE_SIZES}
+    if towers:
+        keys |= {(t, B) for t, batches in P.TEXT_TOWERS.items() for B in batches}
+    return keys
+
+
+def assert_covered(what, lists, run, key_of):
+    """Every list is non-empty and every entry of it runs (possibly under another model's id, when shared)."""
+    for k, entries in lists.items():
+        assert entries, f"{what}: no cases derived for {k}"
+        lost = [e for e in entries if key_of(e) not in run]
+        assert not lost, f"{what}: {len(lost)} launches of {k} do not run, first {lost[0]}"
+
+
+def test_gemm_cases_cover_every_model_and_size():
+    lists = TG.production_lists()
+    assert set(lists) == expected_keys()
+    run = {TG.signature(p.values[0]) for p in TG._production_cases()}
+    assert_covered("GEMM", lists, run, lambda e: TG.signature(e[1]))
+
+
+def test_attention_cases_cover_every_model_and_size():
+    lists = TA.production_lists()
+    assert set(lists) == expected_keys(vae=False, towers=False)
+    for k, shapes in lists.items():  # self- and cross-attention at every size
+        assert {s[1] == s[2] for _, s in shapes} == {True, False}, f"attention {k}: {shapes}"
+    run = {tuple(p.values) for p in TA._production_cases()}
+    assert_covered("attention", lists, run, lambda e: e[1])
+
+
+def test_groupnorm_cases_cover_every_model_and_size():
+    lists = TN.production_lists()
+    assert set(lists) == expected_keys(towers=False)
+    unet = {tuple(c[3:]) for c in TN._unet_cases()}
+    vae = {(c[0], *c[3:]) for c in TN._vae_cases()}
+    assert_covered("GroupNorm", {k: v for k, v in lists.items() if k[0] != "vae"}, unet, tuple)
+    assert_covered("GroupNorm", {k: v for k, v in lists.items() if k[0] == "vae"}, vae, tuple)
+
+
+@pytest.mark.parametrize("model", sorted(REQUIRED_UNET))
+def test_new_levels_reach_the_lists(model):
+    """Spot checks of what each model brings: SD 2's 9216-token level at 768², the refiner's 12..96 channels per
+    group with concat groups across the source boundary and its 3072-channel conv (K = 27648), SDXL's 3952-token
+    level at 1216x832."""
+    cfg = C.CONFIGS[model]()
+    native = (model, (cfg.sample_size, cfg.sample_size))
+    gemm = [l for _, l in TG.production_lists()[native]]
+    attn = [s for _, s in TA.production_lists()[native]]
+    gn = TN.production_lists()[native]
+    ch = cfg.block_out_channels
+    assert max(l.get("Cin", 0) for l in gemm) == 2 * ch[-1]
+    assert (cfg.num_attention_heads[-1], 77) in {(s[0], s[2]) for s in attn}
+    assert {(c1 + c2) // 32 for c1, c2, *_ in gn} >= {c // 32 for c in ch}
+    if model == "sdxl_refiner":
+        assert {(c1 + c2) // 32 for c1, c2, *_ in gn} >= {12, 24, 36, 48, 72, 96}
+        assert (1536, 768) in {(c1, c2) for c1, c2, *_ in gn} and (768, 384) in {(c1, c2) for c1, c2, *_ in gn}
+    if model == "sd2":
+        assert (5, 9216, 9216, 64) in attn
+    if model in ("sdxl", "sdxl_refiner"):
+        tall = [s for _, s in TA.production_lists()[(model, (152, 104))]]
+        assert any(s[1] == 3952 for s in tall)
