@@ -14,7 +14,7 @@ import torch
 
 from . import _native as nv
 from .config import UNetConfig, to_desc
-from .schedule import F16, F32, StepStateC, to_c_array, v_pred_coefs
+from .schedule import F16, F32, StepStateC, to_c_array, v_pred_coefs, v_to_eps
 
 
 class NativeUNet(nv.NativeHandle):
@@ -197,6 +197,29 @@ class NativeUNet(nv.NativeHandle):
         with torch.cuda.device(self.device):
             nv.check(self.lib.cfgpp_apply_step(self._h, c_int(step), nv.ptr(eps_uc.contiguous()),
                                                nv.ptr(eps_c.contiguous()), nv.stream_ptr()))
+
+    def run_trajectory(self, method: int, state_dtype: torch.dtype, steps: Sequence[StepStateC], z: torch.Tensor,
+                       guidance: Optional[Sequence[float]] = None, noise: Optional[torch.Tensor] = None):
+        """A whole trajectory from state `z` on the prepared, prompt-bound handle: NFE replays of the step graph with no
+        host synchronisation in between. `noise`: the ancestral samplers' table (set_noise). Returns (z0t, zt)."""
+        self.set_schedule(method, state_dtype, steps, guidance)
+        self.set_state(z)
+        if noise is not None:
+            self.set_noise(noise)
+        self.run_steps(0, len(steps))
+        return self.get_state(1), self.get_state(0)
+
+    def callback_step(self, i: int, step: StepStateC):
+        """Entry i of the current schedule un-fused, so that a callback can see and replace the state: the UNet through
+        predict_noise, a v-prediction output turned into eps with the entry's own (a, b) as the fused step does, then
+        the step kernel's update. Returns (z0t, zt)."""
+        z = self.get_state(0)
+        eps_uc, eps_c = self.predict_noise(z, step.t, step.in_scale)
+        if self.v_prediction:
+            a, b = self.v_coefs[i]
+            eps_uc, eps_c = v_to_eps(eps_uc, z.half(), a, b), v_to_eps(eps_c, z.half(), a, b)
+        self.apply_step(i, eps_uc, eps_c)
+        return self.get_state(1), self.get_state(0)
 
     # ---- LoRA adapters ----------------------------------------------------------------------------------------
     MAX_LORAS_PER_WEIGHT = 4

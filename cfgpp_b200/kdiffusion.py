@@ -18,6 +18,7 @@ from typing import Callable, Optional, Sequence
 
 import torch
 
+from . import schedule as S
 from .batching import guidance_mix, guidance_table
 
 
@@ -68,7 +69,6 @@ class KDiffusionMixin:
         xc = self.calculate_input(x, sigma)
         if getattr(self, "v_prediction", False):
             # v -> eps at the level the VE update assigns to x (abar = 1 / (1 + sigma^2)), as the fused step does
-            from . import schedule as S
             v_uc, v_c = self.model_output(xc, t, *cond)
             a, b = S.ve_v_coefs(sigma)
             noise_uc, noise_c = S.v_to_eps(v_uc, xc, a, b), S.v_to_eps(v_c, xc, a, b)
@@ -84,34 +84,18 @@ class KDiffusionMixin:
         return self._k_denoise(x, sigma, t, cfg_guidance, (uc, c, add_cond_kwargs))
 
 
-def _fused_trajectory(solver, x, steps, cond, cfg_guidance):
+def _fused_trajectory(solver, x, steps, cond, cfg_guidance, noise_slots: int = 0):
     """Whole VE-cast trajectory on the fused step kernel (UNet + CFG / CFG++ mix + Euler / DPM++2M update in the conv_out
-    epilogue, one CUDA-graph replay per step, no elementwise launch or host sync in between). Returns (last denoised, x)."""
-    from . import schedule as S
+    epilogue, one CUDA-graph replay per step, no elementwise launch or host sync in between). Returns (last denoised, x).
+    Ancestral loops (`noise_slots` > 0, see schedule.kd_ancestral_steps): the fresh noise of every step is drawn up
+    front, in loop order, with the calls the op-by-op loop would make (`torch.randn_like(x)`, same generator state =>
+    same values), and travels as a table the step kernel indexes; dpm++_2s_a replays the graph twice per step
+    (midpoint, final)."""
     solver._prepare(x, *cond, force=True)
-    eng = solver.unet
-    eng.set_schedule(S.STEP_DPMPP2M_CFGPP, torch.float16, steps, guidance_table(cfg_guidance))
-    eng.set_state(x)
-    eng.run_steps(0, len(steps))
-    return eng.get_state(1), eng.get_state(0)
-
-
-def _fused_ancestral_trajectory(solver, x, sigmas, cfg_guidance, cond, cfgpp: bool, two_s: bool):
-    """Ancestral loops on the fused step kernel: the fresh noise of every step is drawn up front, in loop order, with
-    the calls the op-by-op loop would make (`torch.randn_like(x)`, same generator state => same values), and travels
-    as a table the step kernel indexes; dpm++_2s_a replays the graph twice per step (midpoint, final)."""
-    from . import schedule as S
-    steps, slots = S.kd_ancestral_steps(sigmas, solver.timestep, cfg_guidance, cfgpp, two_s)
-    solver._prepare(x, *cond, force=True)
-    eng = solver.unet
-    state0 = x.to(eng.device, torch.float16)
-    noise = torch.stack([torch.randn_like(state0) for _ in range(slots)]) if slots else None
-    eng.set_schedule(S.STEP_DPMPP2M_CFGPP, torch.float16, steps, guidance_table(cfg_guidance))
-    eng.set_state(state0)
-    if noise is not None:
-        eng.set_noise(noise)
-    eng.run_steps(0, len(steps))
-    return eng.get_state(1), eng.get_state(0)
+    x = x.to(solver.unet.device, torch.float16)
+    noise = torch.stack([torch.randn_like(x) for _ in range(noise_slots)]) if noise_slots else None
+    return solver.unet.run_trajectory(S.STEP_DPMPP2M_CFGPP, torch.float16, steps, x, guidance_table(cfg_guidance),
+                                      noise)
 
 
 def _fusable(solver, callback_fn) -> bool:
@@ -137,8 +121,8 @@ def euler_cfgpp_loop(solver: KDiffusionMixin, x, sigmas, cfg_guidance, cond, cal
     returns (:757-762). `cfgpp=False`: plain CFG, the derivative uses the guided estimate (:326-330, :372-379)."""
     if _fusable(solver, callback_fn):
         if ancestral:
-            return _fused_ancestral_trajectory(solver, x, sigmas, cfg_guidance, cond, cfgpp, two_s=False)
-        from . import schedule as S
+            steps, slots = S.kd_ancestral_steps(sigmas, solver.timestep, cfg_guidance, cfgpp)
+            return _fused_trajectory(solver, x, steps, cond, cfg_guidance, slots)
         return _fused_trajectory(solver, x, S.kd_steps(sigmas, solver.timestep, cfg_guidance, cfgpp), cond,
                                  cfg_guidance)
     denoised = None
@@ -167,7 +151,8 @@ def dpmpp_2s_a_cfgpp_loop(solver: KDiffusionMixin, x, sigmas, cfg_guidance, cond
     Tweedie estimate — latent_diffusion.py:782-825 (two UNet calls per step). `cfgpp=False`: the plain-CFG original
     (:408-437), guided estimate everywhere and the standard final update."""
     if _fusable(solver, callback_fn):
-        return _fused_ancestral_trajectory(solver, x, sigmas, cfg_guidance, cond, cfgpp, two_s=True)
+        steps, slots = S.kd_ancestral_steps(sigmas, solver.timestep, cfg_guidance, cfgpp, two_s=True)
+        return _fused_trajectory(solver, x, steps, cond, cfg_guidance, slots)
     t_fn = lambda s: s.log().neg()      # noqa: E731
     sigma_fn = lambda t: t.neg().exp()  # noqa: E731
     denoised = None
@@ -206,7 +191,6 @@ def dpmpp_2m_cfgpp_karras_loop(solver: KDiffusionMixin, x, sigmas, cfg_guidance,
     unconditional one (latent_sdxl.py:916; that one runs on the fused step kernel). `cfgpp=False`: plain `dpm++_2m`
     (:470-487), guided estimate everywhere."""
     if _fusable(solver, callback_fn):
-        from . import schedule as S
         return _fused_trajectory(solver, x, S.kd_steps(sigmas, solver.timestep, cfg_guidance, cfgpp, second_order=True,
                                                        diff_guided=True), cond, cfg_guidance)
     t_fn = lambda s: s.log().neg()  # noqa: E731

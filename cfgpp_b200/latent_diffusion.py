@@ -1,13 +1,15 @@
 """Stable Diffusion v1.5 and 2.x CFG++ solvers on the Blackwell-native backend.
 
 Mirror of the reference's `latent_diffusion.py` solver API for the hot path: registry (:13-26), `StableDiffusion`
-base (:54-241: `alpha`, `get_text_embed`, `encode`, `decode`, `predict_noise`, `inversion`, `initialize_latent`),
+base (:54-241: `alpha`, `get_text_embed`, `predict_noise`, `inversion`, `initialize_latent`; `encode` / `decode` and
+the registry factory are shared with the SDXL family in solver_base.py),
 `ddim_cfg++` (:621-679) and `ddim_inversion_cfg++` (:882-957). Same names, argument meaning and errors; the UNet
 forward, CFG++ mix and DDIM update run in hand-written sm_90a CUDA behind include/cfgpp_b200.h.
 SURVEY §8 f1 (the rest of the CFG++ `--method` surface): `ddim_edit_cfg++` (:959-1010) on the same fused step modes;
 `euler_cfg++` (:682-724), `euler_a_cfg++` (:727-768), `dpm++_2s_a_cfg++` (:771-827), `dpm++_2m_cfg++` (:830-879) as
 fused VE-cast trajectories (kdiffusion.py: the ancestral ones with their noise drawn up front); the op-by-op torch
-form over `predict_noise` runs when a callback is installed.
+form over `predict_noise` runs when a callback is installed. A plain-CFG DDIM solver and its CFG++ twin share one body
+and differ in the class attributes `step_mode` / `inversion_mode` (the fused step kernel's modes).
 
 SD 2.x (`unet_config=sd2_config()` / `sd2_base_config()`) runs on the same solvers: the UNet differs only in its
 config, and a v-prediction model's output is turned into eps inside the fused step (see schedule.v_pred_coefs).
@@ -28,28 +30,10 @@ from .batching import draw_latents, encode_prompts, guidance_table, normalize_ba
 from .conditioning import SyntheticTextEncoder
 from .text_encoder import CLIPTextConfig, get_conditioner
 from .config import UNetConfig, sd15_config
-from .latent_sdxl import _Scheduler, get_engine
-from .lora import LoraMixin
+from .latent_sdxl import get_engine
+from .solver_base import SolverBase, registry
 
-####### Factory #######
-__SOLVER__ = {}
-
-
-def register_solver(name: str):
-    def wrapper(cls):
-        if __SOLVER__.get(name, None) is not None:
-            raise ValueError(f"Solver {name} already registered.")
-        __SOLVER__[name] = cls
-        return cls
-    return wrapper
-
-
-def get_solver(name: str, **kwargs):
-    if name not in __SOLVER__:
-        raise ValueError(f"Solver {name} does not exist.")
-    return __SOLVER__[name](**kwargs)
-
-########################
+__SOLVER__, register_solver, get_solver = registry()
 
 
 def default_text_encoder(cfg: UNetConfig, device):
@@ -67,7 +51,10 @@ def default_text_encoder(cfg: UNetConfig, device):
     return get_conditioner("", device, "sd15", cfg=small)
 
 
-class StableDiffusion(K.KDiffusionMixin, LoraMixin):
+class StableDiffusion(SolverBase):
+    step_mode = S.STEP_DDIM_CFG       # fused step mode of the sampling loop
+    inversion_mode = S.STEP_DDIM_CFG  # ... and of the inversion loop
+
     def __init__(self,
                  solver_config,
                  model_key: str = "runwayml/stable-diffusion-v1-5",
@@ -88,17 +75,7 @@ class StableDiffusion(K.KDiffusionMixin, LoraMixin):
             # AutoencoderKL decoder on the native backend (vae.py; the reference uses pipe.vae, latent_diffusion.py:64)
             from .vae import get_vae
             self.vae = get_vae("sd15_vae", device)
-
-        self._sch = S.Schedule.make(solver_config.num_sampling, "ddim")
-        self.total_alphas = self._sch.total_alphas
-        self.sigmas = self._sch.sigmas
-        self.log_sigmas = self._sch.log_sigmas
-        self.skip = self._sch.skip
-        self.final_alpha_cumprod = self._sch.final_alpha_cumprod
-        self.scheduler = _Scheduler(self._sch, device)
-
-    def __call__(self, *args: Any, **kwargs: Any) -> Any:
-        self.sample(*args, **kwargs)
+        self._init_schedule(solver_config.num_sampling, "ddim", device)
 
     def sample(self, *args: Any, **kwargs: Any) -> Any:
         raise NotImplementedError("Solver must implement sample() method.")
@@ -124,12 +101,6 @@ class StableDiffusion(K.KDiffusionMixin, LoraMixin):
         uc, c = self.get_text_embed(null_prompt=p["prompt[0]"], prompt=p["prompt[1]"], batch=B)
         return uc, c, cfg_guidance, zT
 
-    def encode(self, x):
-        return self.vae.encode(x, self.dtype)
-
-    def decode(self, zt):
-        return self.vae.decode(zt).float()
-
     def _prepare(self, zt, uc, c, force: bool = False):
         b, _, h, w = zt.shape
         self.unet.prepare(b, h, w)
@@ -153,36 +124,28 @@ class StableDiffusion(K.KDiffusionMixin, LoraMixin):
         return S.v_to_eps(out_uc, x_in, a, b), S.v_to_eps(out_c, x_in, a, b)
 
     def _run(self, method, steps, z_init, uc, c, callback_fn=None, cfg_guidance=None):
-        """`cfg_guidance`: a per-image sequence goes to the step kernel's guidance table; a float (or None) leaves the
-        steps' scalar in charge."""
+        """(z0t, zt) of a DDIM-family trajectory. `cfg_guidance`: a per-image sequence goes to the step kernel's
+        guidance table; a float (or None) leaves the steps' scalar in charge."""
         self._prepare(z_init, uc, c, force=True)  # every trajectory re-binds its prompt
-        eng = self.unet
-        eng.set_schedule(method, z_init.dtype, steps, None if cfg_guidance is None else guidance_table(cfg_guidance))
-        eng.set_state(z_init)
-        z0t = None
+        eng, table = self.unet, guidance_table(cfg_guidance)
         if callback_fn is None:
-            eng.run_steps(0, len(steps))
-            z0t = eng.get_state(1)
-        else:
-            for i, st in enumerate(steps):
-                z = eng.get_state(0)
-                eps_uc, eps_c = eng.predict_noise(z, st.t)
-                if self.v_prediction:  # the fused step's conversion, with the entry's (a, b)
-                    a, b = eng.v_coefs[i]
-                    eps_uc, eps_c = S.v_to_eps(eps_uc, z.half(), a, b), S.v_to_eps(eps_c, z.half(), a, b)
-                eng.apply_step(i, eps_uc, eps_c)
-                kw = {'z0t': eng.get_state(1).detach(), 'zt': eng.get_state(0).detach(), 'decode': self.decode}
-                kw = callback_fn(i, torch.tensor(int(st.t), device=self.device), kw)
-                z0t = kw['z0t']
-                eng.set_state(kw['zt'])
+            return eng.run_trajectory(method, z_init.dtype, steps, z_init, table)
+        eng.set_schedule(method, z_init.dtype, steps, table)
+        eng.set_state(z_init)
+        for i, st in enumerate(steps):
+            z0t, zt = eng.callback_step(i, st)
+            kw = {'z0t': z0t.detach(), 'zt': zt.detach(), 'decode': self.decode}
+            kw = callback_fn(i, torch.tensor(int(st.t), device=self.device), kw)
+            z0t = kw['z0t']
+            eng.set_state(kw['zt'])
         return z0t, eng.get_state(0)
 
     @torch.no_grad()
     def inversion(self, z0: torch.Tensor, uc: torch.Tensor, c: torch.Tensor, cfg_guidance: float = 1.0):
-        """Plain-CFG DDIM inversion (latent_diffusion.py:160-182): Tweedie and renoise both with the guided eps. Same
-        scalars as the CFG++ inversion; the fused step kernel's STEP_DDIM_CFG mode picks the eps."""
+        """DDIM inversion (latent_diffusion.py:160-182) on the fused `inversion_mode`: plain CFG takes Tweedie and
+        renoise both with the guided eps; CFG++ (:897-908) takes Tweedie with eps_uc. Same scalars for both."""
         steps = S.ddim_inversion_cfgpp_steps(self._sch, cfg_guidance)
-        _, zt = self._run(S.STEP_DDIM_CFG, steps, z0.clone().to(self.device), uc, c)
+        _, zt = self._run(self.inversion_mode, steps, z0.clone().to(self.device), uc, c)
         return zt
 
     def initialize_latent(self, method: str = 'random', src_img: Optional[torch.Tensor] = None, **kwargs):
@@ -206,7 +169,7 @@ class StableDiffusion(K.KDiffusionMixin, LoraMixin):
 
 
 ###########################################
-# Base version (plain CFG — the baselines the paper compares against, SURVEY §8 f4)
+# DDIM: plain CFG (the baselines the paper compares against, SURVEY §8 f4) and CFG++
 ###########################################
 
 @register_solver("ddim")
@@ -215,7 +178,7 @@ class BaseDDIM(StableDiffusion):
 
     def reverse_process(self, uc, c, cfg_guidance, zt, callback_fn=None):
         steps = S.ddim_cfgpp_steps(self._sch, cfg_guidance, sdxl_indexing=False)
-        z0t, _ = self._run(S.STEP_DDIM_CFG, steps, zt, uc, c, callback_fn, cfg_guidance)
+        z0t, _ = self._run(self.step_mode, steps, zt, uc, c, callback_fn, cfg_guidance)
         return z0t
 
     def sample(self, cfg_guidance=7.5, prompt=["", ""], callback_fn=None, **kwargs):
@@ -223,23 +186,17 @@ class BaseDDIM(StableDiffusion):
         uc, c, cfg_guidance, zt = self.batch_inputs(prompt, cfg_guidance, kwargs.get('zT'))
         if zt is None:
             zt = self.initialize_latent(latent_dim=(uc.shape[0], 4, self.cfg.sample_size, self.cfg.sample_size))
-        z0t = self.reverse_process(uc, c, cfg_guidance, zt, callback_fn)
-        img = self.decode(z0t)
-        img = (img / 2 + 0.5).clamp(0, 1)
-        return img.detach().cpu()
+        return self.to_image(self.reverse_process(uc, c, cfg_guidance, zt, callback_fn))
 
 
 @register_solver("ddim_inversion")
 class InversionDDIM(BaseDDIM):
     """Reconstruction / editing after plain-CFG inversion (latent_diffusion.py:506-558)."""
 
-    def sample(self, src_img, cfg_guidance=7.5, prompt=["", "", ""], callback_fn=None, **kwargs):
+    def sample(self, src_img, cfg_guidance=7.5, prompt=["", ""], callback_fn=None, **kwargs):
         uc, c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[1])
         zt = self.initialize_latent(method='ddim', src_img=src_img, uc=uc, c=c, cfg_guidance=cfg_guidance)
-        z0t = self.reverse_process(uc, c, cfg_guidance, zt, callback_fn)
-        img = self.decode(z0t)
-        img = (img / 2 + 0.5).clamp(0, 1)
-        return img.detach().cpu()
+        return self.to_image(self.reverse_process(uc, c, cfg_guidance, zt, callback_fn))
 
 
 @register_solver("ddim_edit")
@@ -250,68 +207,26 @@ class EditWordSwapDDIM(InversionDDIM):
         uc, src_c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[1])
         _, tgt_c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[2])
         zt = self.initialize_latent(method='ddim', src_img=src_img, uc=uc, c=src_c, cfg_guidance=cfg_guidance)
-        z0t = self.reverse_process(uc, tgt_c, cfg_guidance, zt, callback_fn)
-        img = self.decode(z0t)
-        img = (img / 2 + 0.5).clamp(0, 1)
-        return img.detach().cpu()
+        return self.to_image(self.reverse_process(uc, tgt_c, cfg_guidance, zt, callback_fn))
 
-
-###########################################
-# CFG++ version
-###########################################
 
 @register_solver("ddim_cfg++")
-class BaseDDIMCFGpp(StableDiffusion):
+class BaseDDIMCFGpp(BaseDDIM):
     """DDIM solver for SD with CFG++ (text-to-image)."""
-
-    def reverse_process(self, uc, c, cfg_guidance, zt, callback_fn=None):
-        steps = S.ddim_cfgpp_steps(self._sch, cfg_guidance, sdxl_indexing=False)
-        z0t, _ = self._run(S.STEP_DDIM_CFGPP, steps, zt, uc, c, callback_fn, cfg_guidance)
-        return z0t
-
-    def sample(self, cfg_guidance=7.5, prompt=["", ""], callback_fn=None, **kwargs):
-        """Batched: see StableDiffusion.batch_inputs. Returns (B, 3, H, W)."""
-        uc, c, cfg_guidance, zt = self.batch_inputs(prompt, cfg_guidance, kwargs.get('zT'))
-        if zt is None:
-            zt = self.initialize_latent(latent_dim=(uc.shape[0], 4, self.cfg.sample_size, self.cfg.sample_size))
-        z0t = self.reverse_process(uc, c, cfg_guidance, zt, callback_fn)
-        img = self.decode(z0t)
-        img = (img / 2 + 0.5).clamp(0, 1)
-        return img.detach().cpu()
+    step_mode = S.STEP_DDIM_CFGPP
 
 
 @register_solver("ddim_inversion_cfg++")
-class InversionDDIMCFGpp(BaseDDIMCFGpp):
-    """Editing via WordSwap after inversion (CFG++ inversion: Tweedie with eps_uc, renoise with the guided eps)."""
-
-    @torch.no_grad()
-    def inversion(self, z0: torch.Tensor, uc: torch.Tensor, c: torch.Tensor, cfg_guidance: float = 1.0):
-        steps = S.ddim_inversion_cfgpp_steps(self._sch, cfg_guidance)
-        _, zt = self._run(S.STEP_DDIM_INV_CFGPP, steps, z0.clone().to(self.device), uc, c)
-        return zt
-
-    def sample(self, src_img, cfg_guidance=7.5, prompt=["", ""], callback_fn=None, **kwargs):
-        uc, c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[1])
-        zt = self.initialize_latent(method='ddim', src_img=src_img, uc=uc, c=c, cfg_guidance=cfg_guidance)
-        z0t = self.reverse_process(uc, c, cfg_guidance, zt, callback_fn)
-        img = self.decode(z0t)
-        img = (img / 2 + 0.5).clamp(0, 1)
-        return img.detach().cpu()
+class InversionDDIMCFGpp(InversionDDIM):
+    """Reconstruction after CFG++ inversion (Tweedie with eps_uc, renoise with the guided eps) and CFG++ sampling."""
+    step_mode, inversion_mode = S.STEP_DDIM_CFGPP, S.STEP_DDIM_INV_CFGPP
 
 
 @register_solver("ddim_edit_cfg++")
-class EditWordSwapDDIMCFGpp(InversionDDIMCFGpp):
+class EditWordSwapDDIMCFGpp(EditWordSwapDDIM):
     """Editing via WordSwap after inversion: CFG++ inversion under the source prompt, CFG++ sampling under the target
     prompt (latent_diffusion.py:959-1010). Both loops run as fused trajectories with an fp16 state."""
-
-    def sample(self, src_img, cfg_guidance=7.5, prompt=["", "", ""], callback_fn=None, **kwargs):
-        uc, src_c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[1])
-        _, tgt_c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[2])
-        zt = self.initialize_latent(method='ddim', src_img=src_img, uc=uc, c=src_c, cfg_guidance=cfg_guidance)
-        z0t = self.reverse_process(uc, tgt_c, cfg_guidance, zt, callback_fn)
-        img = self.decode(z0t)
-        img = (img / 2 + 0.5).clamp(0, 1)
-        return img.detach().cpu()
+    step_mode, inversion_mode = S.STEP_DDIM_CFGPP, S.STEP_DDIM_INV_CFGPP
 
 
 class _KarrasCFGpp(StableDiffusion):
@@ -343,9 +258,7 @@ class _KarrasCFGpp(StableDiffusion):
         the whole batch, as the reference's loop would on a batched x: their images are not the serial runs' images."""
         uc, c, cfg_guidance, zt = self.batch_inputs(prompt, cfg_guidance, kwargs.get('zT'))
         denoised, x = self.reverse_process(uc, c, cfg_guidance, kwargs.get('xT'), callback_fn, zt)
-        img = self.decode(x if self.decode_state else denoised)
-        img = (img / 2 + 0.5).clamp(0, 1)
-        return img.detach().cpu()
+        return self.to_image(x if self.decode_state else denoised)
 
 
 @register_solver("euler_cfg++")

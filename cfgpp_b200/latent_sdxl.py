@@ -7,19 +7,23 @@ Mirror of the reference's `latent_sdxl.py` solver API for the hot path named by 
 AssertionError for Lightning with cfg_guidance != 1, NotImplementedError for unknown init methods) — but the UNet
 forward, the CFG++ guidance mix and the scheduler update run in hand-written sm_90a CUDA behind the C ABI
 (include/cfgpp_b200.h). With `callback_fn=None` a whole trajectory is enqueued as NFE replays of one CUDA graph with
-no host synchronisation; with a callback the un-fused seam (`predict_noise` + `apply_step`) is used so that `z0t` /
-`zt` are materialised and may be replaced by the callback, exactly like the reference loop.
+no host synchronisation (`NativeUNet.run_trajectory`); with a callback the un-fused seam (`NativeUNet.callback_step`:
+`predict_noise` + `apply_step`) is used so that `z0t` / `zt` are materialised and may be replaced by the callback,
+exactly like the reference loop.
 
 Registered here: ddim_cfg++, ddim_cfg++_lightning, dpm++_2m_cfgpp (the solvers of SURVEY.md §8a) and, from §8 f1,
 dpm++_2m_cfgpp_lightning (:932-952), ddim_edit_cfg++ (:954-1025, both loops on the fused step modes), euler_cfg++ and
 euler_cfg++_lightning (:757-836: fused VE-cast trajectories, kdiffusion.py; the op-by-op torch form only with a callback).
+A plain-CFG solver and its CFG++ twin share one body: the DDIM ones differ in the class attributes `step_mode` /
+`inversion_mode`, the Euler ones in their sigma table and `cfgpp`. A Lightning solver lists SDXLLightning first in its
+bases, for its checkpoint, its schedule and its guidance check.
 The VAE (decode and encode, vae.py, SURVEY §8 f2) and the two CLIP text towers (text_encoder.py, §8 f3) run on the
 native backend too; `text_encoders=` / `vae=` accept replacements.
 """
 from __future__ import annotations
 
 import warnings
-from typing import Any, Optional, Tuple
+from typing import Optional, Tuple
 
 import torch
 
@@ -32,27 +36,10 @@ from .text_encoder import CLIPTextConfig, ClipConditioner, get_conditioner
 from .config import UNetConfig, sdxl_config, sdxl_refiner_config
 from .engine import NativeUNet
 from .lora import LoraMixin, is_lora_file, read_lora
+from .solver_base import SolverBase, registry
 from .weights import load_safetensors_state_dict, synthetic_state_dict
 
-####### Factory #######
-__SOLVER__ = {}
-
-
-def register_solver(name: str):
-    def wrapper(cls):
-        if __SOLVER__.get(name, None) is not None:
-            raise ValueError(f"Solver {name} already registered.")
-        __SOLVER__[name] = cls
-        return cls
-    return wrapper
-
-
-def get_solver(name: str, **kwargs):
-    if name not in __SOLVER__:
-        raise ValueError(f"Solver {name} does not exist.")
-    return __SOLVER__[name](**kwargs)
-
-########################
+__SOLVER__, register_solver, get_solver = registry()
 
 _ENGINES = {}
 
@@ -104,14 +91,6 @@ def release_engines():
     _ENGINES.clear()
 
 
-class _Scheduler:
-    """The two attributes of the diffusers scheduler object the reference touches."""
-    def __init__(self, sch: S.Schedule, device):
-        self.timesteps = sch.timesteps.to(device)
-        self.alphas_cumprod = sch.alphas_cumprod
-        self.final_alpha_cumprod = sch.final_alpha_cumprod
-
-
 def default_text_encoders(cfg: UNetConfig, device):
     """(text_enc_1, text_enc_2) for a UNet config: CLIP-L + OpenCLIP bigG for the real SDXL widths (768 + 1280 = 2048,
     pooled 1280), proportionally narrow towers for the test-sized configs; widths that are not multiples of the 64-wide
@@ -161,10 +140,12 @@ class SDXLRefiner(LoraMixin):
         self.text_enc = text_encoder
 
 
-class SDXL(K.KDiffusionMixin, LoraMixin):
+class SDXL(SolverBase):
     schedule_kind = "ddim"
     quantize = True
     supports_refiner = False  # the fused DDIM / DPM++ trajectories of REFINER_SOLVERS hand over to a refiner
+    step_mode = S.STEP_DDIM_CFG       # fused step mode of the DDIM sampling loop
+    inversion_mode = S.STEP_DDIM_CFG  # ... and of the inversion loop
 
     def __init__(self,
                  solver_config,
@@ -192,22 +173,10 @@ class SDXL(K.KDiffusionMixin, LoraMixin):
         self.vae = vae
         self.vae_scale_factor = self.cfg.vae_scale_factor
         self.default_sample_size = self.cfg.sample_size
-
-        # sampling parameters (latent_sdxl.py:56-67 / :407-418)
-        self._sch = S.Schedule.make(solver_config.num_sampling, self.schedule_kind)
-        self.total_alphas = self._sch.total_alphas
-        self.sigmas = self._sch.sigmas
-        self.log_sigmas = self._sch.log_sigmas
-        self.skip = self._sch.skip
-        self.final_alpha_cumprod = self._sch.final_alpha_cumprod
-        self.scheduler = _Scheduler(self._sch, device)
-
-    def __call__(self, *args: Any, **kwargs: Any) -> Any:
-        self.sample(*args, **kwargs)
+        self._init_schedule(solver_config.num_sampling, self.schedule_kind, device)
 
     def alpha(self, t):
-        at = self.scheduler.alphas_cumprod[t] if t >= 0 else self.final_alpha_cumprod
-        return at
+        return self.scheduler.alphas_cumprod[t] if t >= 0 else self.final_alpha_cumprod
 
     @torch.no_grad()
     def _text_embed(self, prompt, text_enc, clip_skip, batch: int = 1):
@@ -234,13 +203,6 @@ class SDXL(K.KDiffusionMixin, LoraMixin):
         null_prompt_embeds = torch.concat(null_embed, dim=-1)
         prompt_embeds = torch.concat(prompt_embed, dim=-1)
         return null_prompt_embeds, prompt_embeds, pool_null_embed, pool_prompt_embed
-
-    @torch.no_grad()
-    def encode(self, x):
-        return self.vae.encode(x, self.dtype)
-
-    def decode(self, zt):
-        return self.vae.decode(zt).float()
 
     # ---- the seam: batched (uncond + cond) UNet forward on the native backend -----------------------------------
     def _prepare(self, zt, uc, c, added_cond_kwargs, force: bool = False):
@@ -271,6 +233,17 @@ class SDXL(K.KDiffusionMixin, LoraMixin):
             f"{passed_add_embed_dim} was created. The model has an incorrect config.")
         return torch.tensor([add_time_ids], dtype=dtype)
 
+    def _time_id_pair(self, dtype, pool, original_size, crops_coords_top_left, target_size, negative_original_size,
+                      negative_crops_coords_top_left, negative_target_size):
+        """(negative, positive) time ids of a sample() call; the negative ones are the positive ones unless both
+        negative sizes are given."""
+        kw = dict(dtype=dtype, text_encoder_projection_dim=int(pool.shape[-1]))
+        add_time_ids = self._get_add_time_ids(original_size, crops_coords_top_left, target_size, **kw)
+        if negative_original_size is None or negative_target_size is None:
+            return add_time_ids, add_time_ids
+        return self._get_add_time_ids(negative_original_size, negative_crops_coords_top_left, negative_target_size,
+                                      **kw), add_time_ids
+
     def sample(self,
                prompt1=["", ""],
                prompt2=["", ""],
@@ -298,26 +271,17 @@ class SDXL(K.KDiffusionMixin, LoraMixin):
         top-left, `aesthetic_score`) and, for the uncond row, `negative_aesthetic_score`."""
         if refiner is not None:
             self._check_refiner()
-        height = self.default_sample_size * self.vae_scale_factor
-        width = self.default_sample_size * self.vae_scale_factor
-        original_size = original_size or (height, width)
-        target_size = target_size or (height, width)
+        size = self.default_sample_size * self.vae_scale_factor
+        original_size, target_size = original_size or (size, size), target_size or (size, size)
 
         B, p, cfg_guidance = normalize_batch({"prompt1[0]": prompt1[0], "prompt1[1]": prompt1[1],
                                               "prompt2[0]": prompt2[0], "prompt2[1]": prompt2[1]},
                                              cfg_guidance, kwargs.get('zT'))
         (null_prompt_embeds, prompt_embeds, pool_null_embed, pool_prompt_embed) = self.get_text_embed(
             p["prompt1[0]"], p["prompt1[1]"], p["prompt2[0]"], p["prompt2[1]"], clip_skip, batch=B)
-
-        add_time_ids = self._get_add_time_ids(original_size, crops_coords_top_left, target_size,
-                                              dtype=prompt_embeds.dtype,
-                                              text_encoder_projection_dim=int(pool_prompt_embed.shape[-1]))
-        if negative_original_size is not None and negative_target_size is not None:
-            negative_add_time_ids = self._get_add_time_ids(negative_original_size, negative_crops_coords_top_left,
-                                                           negative_target_size, dtype=prompt_embeds.dtype,
-                                                           text_encoder_projection_dim=int(pool_prompt_embed.shape[-1]))
-        else:
-            negative_add_time_ids = add_time_ids
+        negative_add_time_ids, add_time_ids = self._time_id_pair(
+            prompt_embeds.dtype, pool_prompt_embed, original_size, crops_coords_top_left, target_size,
+            negative_original_size, negative_crops_coords_top_left, negative_target_size)
 
         # per image: the uncond row takes the negative pooled embedding / time ids unless its lambda is 0 or 1
         add_text_embeds, add_time_ids = sdxl_added_conditions(pool_null_embed, pool_prompt_embed, negative_add_time_ids,
@@ -330,12 +294,8 @@ class SDXL(K.KDiffusionMixin, LoraMixin):
                 refiner, p["prompt1[0]"], p["prompt1[1]"], cfg_guidance, original_size, crops_coords_top_left,
                 negative_original_size or original_size, negative_crops_coords_top_left, aesthetic_score,
                 negative_aesthetic_score, clip_skip, B))
-        zt = self.reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, target_size,
-                                  **kwargs)
-        with torch.no_grad():
-            img = self.decode(zt)
-        img = (img / 2 + 0.5).clamp(0, 1)
-        return img.detach().cpu()
+        return self.to_image(self.reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs,
+                                                  target_size, **kwargs))
 
     @torch.no_grad()
     def refiner_conditions(self, refiner: SDXLRefiner, null_prompt, prompt, cfg_guidance, original_size,
@@ -399,63 +359,66 @@ class SDXL(K.KDiffusionMixin, LoraMixin):
 
     @torch.no_grad()
     def inversion(self, z0, uc, c, cfg_guidance, add_cond_kwargs):
-        """Plain-CFG DDIM inversion (latent_sdxl.py:301-324): Tweedie and renoise both with the guided eps; fused
-        trajectory on the STEP_DDIM_CFG mode with the fp16 VAE latent as state."""
+        """DDIM inversion (latent_sdxl.py:301-324) on the fused `inversion_mode` with the fp16 VAE latent as state:
+        plain CFG takes Tweedie and renoise both with the guided eps, CFG++ (:955-1025) Tweedie with eps_uc."""
         if cfg_guidance == 0.0 or cfg_guidance == 1.0:
             add_cond_kwargs['text_embeds'] = add_cond_kwargs['text_embeds'][-1].unsqueeze(0)
             add_cond_kwargs['time_ids'] = add_cond_kwargs['time_ids'][-1].unsqueeze(0)
         steps = S.ddim_inversion_cfgpp_steps(self._sch, cfg_guidance)
         z0 = z0.clone().to(self.device)
-        return self._run_trajectory(S.STEP_DDIM_CFG, z0.dtype, steps, z0, uc, c, add_cond_kwargs, None, 'zt')
+        _, zt = self._run_trajectory(self.inversion_mode, z0.dtype, steps, z0, (uc, c, add_cond_kwargs))
+        return zt
 
     def sigma_to_t(self, sigma, quantize=None):
         quantize = self.quantize if quantize is None else quantize
         return S.sigma_to_t(self._sch, sigma, quantize)
 
-    # ---- shared trajectory driver -------------------------------------------------------------------------------
-    def _run_trajectory(self, method, state_dtype, steps, z_init, uc, c, add_cond_kwargs, callback_fn, result,
-                        cfg_guidance=None, hand_off=None):
-        """`result`: 'z0t' (DDIM family returns the Tweedie estimate of the last step) or 'zt' (DPM++ returns x).
-        `cfg_guidance`: a per-image sequence goes to the step kernel's guidance table.
+    # ---- trajectory: fused, or step by step under a callback; optionally handed to a refiner ----------------------
+    def _run_trajectory(self, method, state_dtype, steps, z_init, cond, callback_fn=None, cfg_guidance=None,
+                        hand_off=None):
+        """(z0t, zt) after the last step from `z_init` under `cond` = (uc, c, added_cond_kwargs): the DDIM family returns
+        the Tweedie estimate z0t, DPM++ the state zt. `cfg_guidance`: a per-image sequence goes to the step kernel's
+        guidance table.
         `hand_off` (see _hand_off): steps [k, n) of the same table run on the refiner's engine, which continues from
         the base's state in the sampler's own parameterization; both engines are set up before the first step, so
         the hand-off is a device-to-device copy with no host synchronisation. The step index a callback sees runs
         0..n-1 across both."""
-        table = None if cfg_guidance is None else guidance_table(cfg_guidance)
-        experts = [(self.unet, (uc, c, add_cond_kwargs))]
+        table = guidance_table(cfg_guidance)
+        if hand_off is None and callback_fn is None:
+            _prepare_engine(self.unet, z_init, *cond, force=True)  # every trajectory re-binds its prompt
+            return self.unet.run_trajectory(method, state_dtype, steps, z_init, table)
+        experts = [(self.unet, cond)]
         k = len(steps)
         if hand_off is not None:
             refiner, refiner_cond, k = hand_off
             experts.append((refiner.unet, refiner_cond))
-        for e, cond in experts:
-            _prepare_engine(e, z_init, *cond, force=True)  # every trajectory re-binds its prompt
+        for e, e_cond in experts:
+            _prepare_engine(e, z_init, *e_cond, force=True)
             e.set_schedule(method, state_dtype, steps, table)
         eng = self.unet
         eng.set_state(z_init)
         if callback_fn is None:
             eng.run_steps(0, k)
-            if hand_off is not None:
+            eng, base = experts[1][0], eng
+            eng.set_state(base.get_state(0))
+            eng.run_steps(k, len(steps) - k)
+            return eng.get_state(1), eng.get_state(0)
+        for i, st in enumerate(steps):
+            if i == k:
                 eng, base = experts[1][0], eng
                 eng.set_state(base.get_state(0))
-                eng.run_steps(k, len(steps) - k)
-        else:
-            for i, st in enumerate(steps):
-                if i == k:
-                    eng, base = experts[1][0], eng
-                    eng.set_state(base.get_state(0))
-                zt = eng.get_state(0)
-                eps_uc, eps_c = eng.predict_noise(zt, st.t, st.in_scale)
-                eng.apply_step(i, eps_uc, eps_c)
-                kw = {'z0t': eng.get_state(1).detach(), 'zt': eng.get_state(0).detach(), 'decode': self.decode}
-                kw = callback_fn(i, torch.tensor(int(st.t), device=self.device), kw)
-                eng.set_state(kw['zt'])
-                self._cb_z0t = kw['z0t']
-            if result == 'z0t':
-                return self._cb_z0t
-        return eng.get_state(1 if result == 'z0t' else 0)
+            z0t, zt = eng.callback_step(i, st)
+            kw = {'z0t': z0t.detach(), 'zt': zt.detach(), 'decode': self.decode}
+            kw = callback_fn(i, torch.tensor(int(st.t), device=self.device), kw)
+            eng.set_state(kw['zt'])
+            z0t = kw['z0t']
+        return z0t, eng.get_state(0)
 
 
 class SDXLLightning(SDXL):
+    """SDXL-Lightning: the distilled UNet (or its LoRA on the base UNet) on the trailing schedule, guidance off. A
+    Lightning solver lists this class first in its bases, so that this __init__ and the guidance check run in place of
+    the plain sampler's."""
     schedule_kind = "lightning"
 
     def __init__(self,
@@ -476,15 +439,21 @@ class SDXLLightning(SDXL):
             warnings.warn(f"Lightning checkpoint '{light_model_ckpt}' not found; using seeded synthetic UNet weights")
         SDXL.__init__(self, solver_config, model_key=key, dtype=dtype, device=device, **kwargs)
 
+    def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
+                        callback_fn=None, **kwargs):
+        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
+        return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
+                                       callback_fn, **kwargs)
+
 
 ###########################################
-# Base version (plain CFG — the baselines the paper compares against, SURVEY §8 f4)
+# Samplers: plain CFG (the baselines the paper compares against, SURVEY §8 f4) and CFG++
 ###########################################
+
 
 @register_solver('ddim')
 class BaseDDIM(SDXL):
     """latent_sdxl.py:425-467: fp32 state, fused trajectory, renoise with the guided eps."""
-    step_mode = S.STEP_DDIM_CFG
     supports_refiner = True
 
     def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
@@ -497,21 +466,41 @@ class BaseDDIM(SDXL):
             zt = self.initialize_latent(size=(b, 4, shape[1] // self.vae_scale_factor, shape[0] // self.vae_scale_factor))
         steps = S.ddim_cfgpp_steps(self._sch, cfg_guidance, sdxl_indexing=True,
                                    tables_on_device=(self.schedule_kind == "lightning"))
-        return self._run_trajectory(self.step_mode, torch.float32, steps, zt.float(), null_prompt_embeds,
-                                    prompt_embeds, add_cond_kwargs, callback_fn, 'z0t', cfg_guidance,
-                                    self._hand_off(kwargs, len(steps)))
+        # fp32 state: zt comes from torch.randn (fp32) and promotes every update (latent_sdxl.py:289, 741-744)
+        z0t, _ = self._run_trajectory(self.step_mode, torch.float32, steps, zt.float(),
+                                      (null_prompt_embeds, prompt_embeds, add_cond_kwargs), callback_fn, cfg_guidance,
+                                      self._hand_off(kwargs, len(steps)))
+        return z0t
+
+
+@register_solver("ddim_cfg++")
+class BaseDDIMCFGpp(BaseDDIM):
+    step_mode = S.STEP_DDIM_CFGPP
+
+
+@register_solver('ddim_lightning')
+class BaseDDIMLight(SDXLLightning, BaseDDIM):
+    pass
+
+
+@register_solver('ddim_cfg++_lightning')
+class BaseDDIMCFGppLight(SDXLLightning, BaseDDIMCFGpp):
+    pass
 
 
 @register_solver('euler')
 class Euler(SDXL):
     """Karras Euler (VE casted), plain CFG, Karras sigmas (latent_sdxl.py:469-517)."""
-    quantize = True
+    cfgpp = False
+
+    def euler_sigmas(self):
+        ts = self.total_sigmas()
+        return K.get_sigmas_karras(len(self.scheduler.timesteps), ts.min(), ts.max(), rho=7.)
 
     @torch.no_grad()
     def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
                         callback_fn=None, **kwargs):
-        ts = self.total_sigmas()
-        sigmas = K.get_sigmas_karras(len(self.scheduler.timesteps), ts.min(), ts.max(), rho=7.)
+        sigmas = self.euler_sigmas()
         zt = kwargs.get('xT')
         if zt is None and kwargs.get('zT') is not None:  # an N(0,1) draw, as every other solver accepts it
             zt = kwargs['zT'].to(self.device) * (sigmas[0] ** 2 + 1) ** 0.5
@@ -520,95 +509,37 @@ class Euler(SDXL):
                       shape[0] // self.vae_scale_factor)
             zt = self.initialize_latent(method="random_kdiffusion", latent_dim=zt_dim, sigmas=sigmas)
         z0t, _ = K.euler_cfgpp_loop(self, zt.to(torch.float16), sigmas, cfg_guidance,
-                                    (null_prompt_embeds, prompt_embeds, add_cond_kwargs), callback_fn, cfgpp=False)
+                                    (null_prompt_embeds, prompt_embeds, add_cond_kwargs), callback_fn, cfgpp=self.cfgpp)
         return z0t
 
 
-@register_solver('ddim_lightning')
-class BaseDDIMLight(BaseDDIM, SDXLLightning):
-    def __init__(self, **kwargs):
-        SDXLLightning.__init__(self, **kwargs)
+@register_solver('euler_cfg++')
+class EulerCFGpp(Euler):
+    """Karras Euler (VE casted) with CFG++ on the sampling timesteps' own sigmas (latent_sdxl.py:757-808): the native
+    UNet behind `predict_noise`, the Euler update in torch (kdiffusion.py)."""
+    cfgpp = True
 
-    def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
-                        callback_fn=None, **kwargs):
-        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
-        return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
-                                       callback_fn, **kwargs)
+    def euler_sigmas(self):
+        sigmas = self.total_sigmas()[torch.round(self.scheduler.timesteps.cpu()).int()]
+        return torch.cat([sigmas, torch.tensor([0.0])])
 
 
 @register_solver('euler_lightning')
-class EulerLight(Euler, SDXLLightning):
-    quantize = True
-
-    def __init__(self, **kwargs):
-        SDXLLightning.__init__(self, **kwargs)
-
-    def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
-                        callback_fn=None, **kwargs):
-        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
-        return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
-                                       callback_fn, **kwargs)
+class EulerLight(SDXLLightning, Euler):
+    pass
 
 
-###########################################
-# CFG++ version
-###########################################
-
-@register_solver("ddim_cfg++")
-class BaseDDIMCFGpp(SDXL):
-    supports_refiner = True
-
-    def reverse_process(self,
-                        null_prompt_embeds,
-                        prompt_embeds,
-                        cfg_guidance,
-                        add_cond_kwargs,
-                        shape=(1024, 1024),
-                        callback_fn=None,
-                        **kwargs):
-        b = null_prompt_embeds.shape[0]
-        zt = kwargs.get('zT')
-        if zt is None:
-            zt = self.initialize_latent(size=(b, 4, shape[1] // self.vae_scale_factor, shape[0] // self.vae_scale_factor))
-        steps = S.ddim_cfgpp_steps(self._sch, cfg_guidance, sdxl_indexing=True,
-                                   tables_on_device=(self.schedule_kind == "lightning"))
-        # fp32 state: zt comes from torch.randn (fp32) and promotes every update (latent_sdxl.py:289, 741-744)
-        return self._run_trajectory(S.STEP_DDIM_CFGPP, torch.float32, steps, zt.float(), null_prompt_embeds,
-                                    prompt_embeds, add_cond_kwargs, callback_fn, 'z0t', cfg_guidance,
-                                    self._hand_off(kwargs, len(steps)))
-
-
-@register_solver('ddim_cfg++_lightning')
-class BaseDDIMCFGppLight(BaseDDIMCFGpp, SDXLLightning):
-    def __init__(self, **kwargs):
-        SDXLLightning.__init__(self, **kwargs)
-
-    def reverse_process(self,
-                        null_prompt_embeds,
-                        prompt_embeds,
-                        cfg_guidance,
-                        add_cond_kwargs,
-                        shape=(1024, 1024),
-                        callback_fn=None,
-                        **kwargs):
-        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
-        return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
-                                       callback_fn, **kwargs)
+@register_solver('euler_cfg++_lightning')
+class EulerCFGppLight(SDXLLightning, EulerCFGpp):
+    pass
 
 
 @register_solver('dpm++_2m_cfgpp')
 class DPMpp2mCFGppSolver(SDXL):
-    quantize = True
     supports_refiner = True
 
-    def reverse_process(self,
-                        null_prompt_embeds,
-                        prompt_embeds,
-                        cfg_guidance,
-                        add_cond_kwargs,
-                        shape=(1024, 1024),
-                        callback_fn=None,
-                        **kwargs):
+    def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
+                        callback_fn=None, **kwargs):
         b = null_prompt_embeds.shape[0]
         # a refiner starts with no multistep history: its first step takes the first-order update
         hand_off = self._hand_off(kwargs, len(self._sch.timesteps) - 1)
@@ -620,58 +551,15 @@ class DPMpp2mCFGppSolver(SDXL):
                                                               shape[0] // self.vae_scale_factor))
         x = x.to(torch.float16)
         x = x * sigma0  # fp16 tensor x 0-dim fp32 -> fp16 (latent_sdxl.py:882-884)
-        return self._run_trajectory(S.STEP_DPMPP2M_CFGPP, torch.float16, steps, x, null_prompt_embeds, prompt_embeds,
-                                    add_cond_kwargs, callback_fn, 'zt', cfg_guidance, hand_off)
+        _, x = self._run_trajectory(S.STEP_DPMPP2M_CFGPP, torch.float16, steps, x,
+                                    (null_prompt_embeds, prompt_embeds, add_cond_kwargs), callback_fn, cfg_guidance,
+                                    hand_off)
+        return x
 
 
 @register_solver('dpm++_2m_cfgpp_lightning')
-class DPMpp2mCFGppLightningSolver(DPMpp2mCFGppSolver, SDXLLightning):
-    def __init__(self, **kwargs):
-        SDXLLightning.__init__(self, **kwargs)
-
-    def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
-                        callback_fn=None, **kwargs):
-        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
-        return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
-                                       callback_fn, **kwargs)
-
-
-@register_solver('euler_cfg++')
-class EulerCFGpp(SDXL):
-    """Karras Euler (VE casted) with CFG++ on the sampling timesteps' own sigmas (latent_sdxl.py:757-808): the native
-    UNet behind `predict_noise`, the Euler update in torch (kdiffusion.py)."""
-    quantize = True
-
-    @torch.no_grad()
-    def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
-                        callback_fn=None, **kwargs):
-        total_sigmas = self.total_sigmas()
-        sigmas = total_sigmas[torch.round(self.scheduler.timesteps.cpu()).int()]
-        sigmas = torch.cat([sigmas, torch.tensor([0.0])])
-        zt = kwargs.get('xT')
-        if zt is None and kwargs.get('zT') is not None:  # an N(0,1) draw, as every other solver accepts it
-            zt = kwargs['zT'].to(self.device) * (sigmas[0] ** 2 + 1) ** 0.5
-        if zt is None:
-            zt_dim = (null_prompt_embeds.shape[0], 4, shape[1] // self.vae_scale_factor,
-                      shape[0] // self.vae_scale_factor)
-            zt = self.initialize_latent(method="random_kdiffusion", latent_dim=zt_dim, sigmas=sigmas)
-        z0t, _ = K.euler_cfgpp_loop(self, zt.to(torch.float16), sigmas, cfg_guidance,
-                                    (null_prompt_embeds, prompt_embeds, add_cond_kwargs), callback_fn)
-        return z0t
-
-
-@register_solver('euler_cfg++_lightning')
-class EulerCFGppLight(EulerCFGpp, SDXLLightning):
-    quantize = True
-
-    def __init__(self, **kwargs):
-        SDXLLightning.__init__(self, **kwargs)
-
-    def reverse_process(self, null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape=(1024, 1024),
-                        callback_fn=None, **kwargs):
-        assert all(g == 1.0 for g in guidance_values(cfg_guidance)), "CFG should be turned off in the lightning version"
-        return super().reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, shape,
-                                       callback_fn, **kwargs)
+class DPMpp2mCFGppLightningSolver(SDXLLightning, DPMpp2mCFGppSolver):
+    pass
 
 
 @register_solver("ddim_edit")
@@ -686,8 +574,9 @@ class EditWardSwapDDIM(SDXL):
                                     c=src_prompt_embeds, cfg_guidance=cfg_guidance,
                                     add_cond_kwargs=add_src_cond_kwargs)
         steps = S.ddim_cfgpp_steps(self._sch, cfg_guidance, sdxl_indexing=False)
-        return self._run_trajectory(S.STEP_DDIM_CFG, zt.dtype, steps, zt, null_prompt_embeds, tgt_prompt_embed,
-                                    add_tgt_cond_kwargs, callback_fn, 'z0t')
+        z0t, _ = self._run_trajectory(self.step_mode, zt.dtype, steps, zt,
+                                      (null_prompt_embeds, tgt_prompt_embed, add_tgt_cond_kwargs), callback_fn)
+        return z0t
 
     def sample(self,
                prompt1=["", "", ""],
@@ -703,24 +592,17 @@ class EditWardSwapDDIM(SDXL):
                **kwargs):
         if kwargs.get('refiner') is not None:
             self._check_refiner()
-        height = self.default_sample_size * self.vae_scale_factor
-        width = self.default_sample_size * self.vae_scale_factor
-        original_size = original_size or (height, width)
-        target_size = target_size or (height, width)
+        size = self.default_sample_size * self.vae_scale_factor
+        original_size, target_size = original_size or (size, size), target_size or (size, size)
 
         (null_prompt_embeds, src_prompt_embeds, pool_null_embed, pool_src) = self.get_text_embed(
             prompt1[0], prompt1[1], prompt2[0], prompt2[1], clip_skip)
         (_, tgt_prompt_embeds, _, pool_tgt) = self.get_text_embed(prompt1[0], prompt1[2], prompt2[0], prompt2[2],
                                                                   clip_skip)
-        proj_dim = int(pool_src.shape[-1])
-        add_time_ids = self._get_add_time_ids(original_size, crops_coords_top_left, target_size,
-                                              dtype=src_prompt_embeds.dtype, text_encoder_projection_dim=proj_dim)
-        if negative_original_size is not None and negative_target_size is not None:
-            negative_add_time_ids = self._get_add_time_ids(negative_original_size, negative_crops_coords_top_left,
-                                                           negative_target_size, dtype=src_prompt_embeds.dtype,
-                                                           text_encoder_projection_dim=proj_dim)
-        else:
-            negative_add_time_ids = add_time_ids
+        negative_add_time_ids, add_time_ids = self._time_id_pair(
+            src_prompt_embeds.dtype, pool_src, original_size, crops_coords_top_left, target_size,
+            negative_original_size, negative_crops_coords_top_left, negative_target_size)
+        # one image: the reference's lambda in {0, 1} rule on the scalar guidance (latent_sdxl.py:249-257)
         add_src, add_tgt = pool_src, pool_tgt
         if cfg_guidance != 0.0 and cfg_guidance != 1.0:
             add_src = torch.cat([pool_null_embed, add_src], dim=0)
@@ -729,12 +611,8 @@ class EditWardSwapDDIM(SDXL):
         add_src_cond_kwargs = {'text_embeds': add_src.to(self.device), 'time_ids': add_time_ids.to(self.device)}
         add_tgt_cond_kwargs = {'text_embeds': add_tgt.to(self.device), 'time_ids': add_time_ids.to(self.device)}
 
-        zt = self.reverse_process(null_prompt_embeds, src_prompt_embeds, tgt_prompt_embeds, cfg_guidance,
-                                  add_src_cond_kwargs, add_tgt_cond_kwargs, **kwargs)
-        with torch.no_grad():
-            img = self.decode(zt)
-        img = (img / 2 + 0.5).clamp(0, 1)
-        return img.detach().cpu()
+        return self.to_image(self.reverse_process(null_prompt_embeds, src_prompt_embeds, tgt_prompt_embeds,
+                                                  cfg_guidance, add_src_cond_kwargs, add_tgt_cond_kwargs, **kwargs))
 
 
 @register_solver("ddim_edit_cfg++")
@@ -743,24 +621,7 @@ class EditWardSwapDDIMCFGpp(EditWardSwapDDIM):
     sampling under the target prompt — latent_sdxl.py:955-1025. Both loops index the schedule through `alpha()`
     (negative t -> final_alpha_cumprod) and carry the fp16 VAE latent, so they run as the two fused step modes the
     SD v1.5 `ddim_inversion_cfg++` uses."""
-
-    @torch.no_grad()
-    def inversion(self, z0, uc, c, cfg_guidance, add_cond_kwargs):
-        if cfg_guidance == 0.0 or cfg_guidance == 1.0:
-            add_cond_kwargs['text_embeds'] = add_cond_kwargs['text_embeds'][-1].unsqueeze(0)
-            add_cond_kwargs['time_ids'] = add_cond_kwargs['time_ids'][-1].unsqueeze(0)
-        steps = S.ddim_inversion_cfgpp_steps(self._sch, cfg_guidance)
-        z0 = z0.clone().to(self.device)
-        return self._run_trajectory(S.STEP_DDIM_INV_CFGPP, z0.dtype, steps, z0, uc, c, add_cond_kwargs, None, 'zt')
-
-    def reverse_process(self, null_prompt_embeds, src_prompt_embeds, tgt_prompt_embed, cfg_guidance,
-                        add_src_cond_kwargs, add_tgt_cond_kwargs, callback_fn=None, **kwargs):
-        zt = self.initialize_latent(method='ddim', src_img=kwargs.get('src_img', None), uc=null_prompt_embeds,
-                                    c=src_prompt_embeds, cfg_guidance=cfg_guidance,
-                                    add_cond_kwargs=add_src_cond_kwargs)
-        steps = S.ddim_cfgpp_steps(self._sch, cfg_guidance, sdxl_indexing=False)
-        return self._run_trajectory(S.STEP_DDIM_CFGPP, zt.dtype, steps, zt, null_prompt_embeds, tgt_prompt_embed,
-                                    add_tgt_cond_kwargs, callback_fn, 'z0t')
+    step_mode, inversion_mode = S.STEP_DDIM_CFGPP, S.STEP_DDIM_INV_CFGPP
 
 
 if __name__ == "__main__":

@@ -1,0 +1,68 @@
+"""What the SD (latent_diffusion.py) and SDXL (latent_sdxl.py) solver families share: the registry factory, the
+schedule attributes the reference keeps on `self`, and the VAE front and back end."""
+from __future__ import annotations
+
+from typing import Any
+
+import torch
+
+from . import kdiffusion as K
+from . import schedule as S
+from .lora import LoraMixin
+
+
+def registry():
+    """(__SOLVER__, register_solver, get_solver) of one solver family (latent_diffusion.py:13-26)."""
+    solvers = {}
+
+    def register_solver(name: str):
+        def wrapper(cls):
+            if solvers.get(name, None) is not None:
+                raise ValueError(f"Solver {name} already registered.")
+            solvers[name] = cls
+            return cls
+        return wrapper
+
+    def get_solver(name: str, **kwargs):
+        if name not in solvers:
+            raise ValueError(f"Solver {name} does not exist.")
+        return solvers[name](**kwargs)
+
+    return solvers, register_solver, get_solver
+
+
+class _Scheduler:
+    """The two attributes of the diffusers scheduler object the reference touches."""
+    def __init__(self, sch: S.Schedule, device):
+        self.timesteps = sch.timesteps.to(device)
+        self.alphas_cumprod = sch.alphas_cumprod
+        self.final_alpha_cumprod = sch.final_alpha_cumprod
+
+
+class SolverBase(K.KDiffusionMixin, LoraMixin):
+    """The host class provides `vae`, `dtype` and `sample`."""
+
+    def _init_schedule(self, num_sampling: int, kind: str, device):
+        """Sampling parameters (latent_diffusion.py:69-80, latent_sdxl.py:56-67 / :407-418)."""
+        self._sch = S.Schedule.make(num_sampling, kind)
+        self.total_alphas = self._sch.total_alphas
+        self.sigmas = self._sch.sigmas
+        self.log_sigmas = self._sch.log_sigmas
+        self.skip = self._sch.skip
+        self.final_alpha_cumprod = self._sch.final_alpha_cumprod
+        self.scheduler = _Scheduler(self._sch, device)
+
+    def __call__(self, *args: Any, **kwargs: Any) -> Any:
+        self.sample(*args, **kwargs)
+
+    @torch.no_grad()
+    def encode(self, x):
+        return self.vae.encode(x, self.dtype)
+
+    def decode(self, zt):
+        return self.vae.decode(zt).float()
+
+    @torch.no_grad()
+    def to_image(self, zt):
+        """The decoded latent as images in [0, 1] on the host, (B, 3, H, W)."""
+        return (self.decode(zt) / 2 + 0.5).clamp(0, 1).detach().cpu()
