@@ -235,6 +235,21 @@ def op_linear_lnfold(h: torch.Tensor, wf: torch.Tensor, s: torch.Tensor, t: torc
     return out
 
 
+def op_linear_scaled_residual(a: torch.Tensor, w: torch.Tensor, addend: torch.Tensor, scale: torch.Tensor | None,
+                              bias=None, out: torch.Tensor | None = None, force_bn: int = 0) -> torch.Tensor:
+    """The ControlNet zero-conv epilogue: fp16(addend + fp16(fp16(a @ w.T + bias) * s)), s = scale (fp32 [1] device
+    tensor; None: the plain residual epilogue). `out` may be `addend` itself (in place)."""
+    lib = load()
+    M, K = a.shape
+    N = w.shape[0]
+    assert a.is_contiguous() and w.shape[1] == K and addend.shape == (M, N) and addend.is_contiguous()
+    assert scale is None or (scale.dtype == torch.float32 and scale.numel() == 1)
+    out = _linear_out(out, M, N, a.device)
+    check(lib.cfgpp_op_linear_scaled_residual(ptr(a), ptr(w), c_int(M), c_int(N), c_int(K), ptr(bias), ptr(addend),
+                                              ptr(scale), ptr(out), c_int(force_bn), stream_ptr()))
+    return out
+
+
 def op_fold_ln(w: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, bias: torch.Tensor | None = None):
     """The LayerNorm fold of w [N,K] (the production weight preparation): (wf = fp16(w * gamma), s [N] fp32 =
     sum_k wf, t [N] fp32 = w @ beta + bias)."""
@@ -432,6 +447,19 @@ def op_conv_in(z: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, in_scale: t
     out = torch.empty((reps * B, H, W, Cout), dtype=torch.float16, device=z.device)
     check(lib.cfgpp_op_conv_in(ptr(z), c_int(dtype_code(z)), ptr(in_scale), ptr(w), ptr(bias), ptr(out), c_int(B),
                                c_int(H), c_int(W), c_int(Cout), c_int(reps), stream_ptr()))
+    return out
+
+
+def op_conv_in_add(z: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, addend: torch.Tensor,
+                   in_scale: torch.Tensor | None = None, reps: int = 1) -> torch.Tensor:
+    """op_conv_in followed by fp16(out + addend), addend [B,H,W,Cout] NHWC fp16 shared by the `reps` repetitions."""
+    lib = load()
+    B, Cin, H, W = z.shape
+    Cout = w.shape[0]
+    assert Cin == 4 and w.shape == (Cout, 36) and addend.shape == (B, H, W, Cout) and addend.dtype == torch.float16
+    out = torch.empty((reps * B, H, W, Cout), dtype=torch.float16, device=z.device)
+    check(lib.cfgpp_op_conv_in_add(ptr(z), c_int(dtype_code(z)), ptr(in_scale), ptr(w), ptr(bias), ptr(addend),
+                                   ptr(out), c_int(B), c_int(H), c_int(W), c_int(Cout), c_int(reps), stream_ptr()))
     return out
 
 

@@ -114,3 +114,23 @@ def refiner_components(ckpt_dir, device) -> dict:
     return {"model_key": str(f["unet"]),
             "text_encoder": get_conditioner("clip_bigg", device, "sdxl", str(f["text_encoder_2"]),
                                             str(f["tokenizer_2/vocab.json"]), str(f["tokenizer_2/merges.txt"]))}
+
+
+def find_controlnet_files(ckpt_dir) -> Dict[str, Path]:
+    """A diffusers ControlNetModel directory: {'config': <dir>/config.json, 'weights':
+    <dir>/diffusion_pytorch_model[.fp16].safetensors}. Raises FileNotFoundError naming every missing file."""
+    root = Path(ckpt_dir)
+    found: Dict[str, Path] = {}
+    missing = []
+    if (root / "config.json").is_file():
+        found["config"] = root / "config.json"
+    else:
+        missing.append(f"{root}/config.json")
+    w = _weights(root, ("diffusion_pytorch_model",))
+    if w is None:
+        missing.append(f"{root}/diffusion_pytorch_model[.fp16].safetensors")
+    else:
+        found["weights"] = w
+    if missing:
+        raise FileNotFoundError("ControlNet directory is missing: " + ", ".join(missing))
+    return found

@@ -10,8 +10,20 @@ using namespace cfgpp;
 
 struct cfgpp_handle {
   Unet unet;
-  cfgpp_handle(const cfgpp_model_desc& d, int device) : unet(d, device) {}
+  cfgpp_handle(const cfgpp_model_desc& d, int device, const cfgpp_controlnet_desc* cn = nullptr)
+      : unet(d, device, cn) {}
 };
+
+namespace {
+// The entry points that run, schedule or configure a UNet: a ControlNet handle runs only through the UNet it is
+// attached to, so these refuse it with an error status instead of touching buffers it does not own.
+Unet& unet_of(cfgpp_handle* h) {
+  CFGPP_REQUIRE(h != nullptr, "null handle");
+  CFGPP_REQUIRE(!h->unet.is_controlnet(), "this is a ControlNet handle: it runs through the UNet handle it is attached "
+                                          "to (cfgpp_attach_controlnet)");
+  return h->unet;
+}
+}  // namespace
 
 extern "C" {
 
@@ -47,16 +59,16 @@ CFGPP_API int cfgpp_lora_add(cfgpp_handle* h, int adapter, const char* key, cons
                              float alpha, int dtype, void* stream) {
   return guarded([&] {
     CFGPP_REQUIRE(key, "null key");
-    h->unet.lora_add(adapter, key, down, up, rank, alpha, dtype, (cudaStream_t)stream);
+    unet_of(h).lora_add(adapter, key, down, up, rank, alpha, dtype, (cudaStream_t)stream);
   });
 }
 
 CFGPP_API int cfgpp_lora_set_scales(cfgpp_handle* h, const float* scales_host, int n_adapters, void* stream) {
-  return guarded([&] { h->unet.lora_set_scales(scales_host, n_adapters, (cudaStream_t)stream); });
+  return guarded([&] { unet_of(h).lora_set_scales(scales_host, n_adapters, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_lora_clear(cfgpp_handle* h, void* stream) {
-  return guarded([&] { h->unet.lora_clear((cudaStream_t)stream); });
+  return guarded([&] { unet_of(h).lora_clear((cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_lora_stats(cfgpp_handle* h, int* n_adapters, int* n_targets, size_t* backup_bytes,
@@ -65,7 +77,7 @@ CFGPP_API int cfgpp_lora_stats(cfgpp_handle* h, int* n_adapters, int* n_targets,
 }
 
 CFGPP_API int cfgpp_prepare(cfgpp_handle* h, int batch, int h_lat, int w_lat) {
-  return guarded([&] { h->unet.prepare(batch, h_lat, w_lat); });
+  return guarded([&] { unet_of(h).prepare(batch, h_lat, w_lat); });
 }
 
 CFGPP_API int cfgpp_workspace_bytes(cfgpp_handle* h, size_t* bytes) {
@@ -91,55 +103,55 @@ CFGPP_API int cfgpp_plan_stats(cfgpp_handle* h, double* step_flops, double* prom
 CFGPP_API int cfgpp_set_prompt(cfgpp_handle* h, const void* ctx, int n_ctx, const void* pooled, const float* time_ids,
                                int add_rows, void* stream) {
   return guarded([&] {
-    h->unet.set_prompt((const __half*)ctx, n_ctx, (const __half*)pooled, time_ids, add_rows, (cudaStream_t)stream);
+    unet_of(h).set_prompt((const __half*)ctx, n_ctx, (const __half*)pooled, time_ids, add_rows, (cudaStream_t)stream);
   });
 }
 
 CFGPP_API int cfgpp_unet_forward(cfgpp_handle* h, const void* z, int z_dtype, float t, float in_scale, void* eps_uc,
                                  void* eps_c, void* stream) {
   return guarded([&] {
-    h->unet.unet_forward(z, z_dtype, t, in_scale, (__half*)eps_uc, (__half*)eps_c, (cudaStream_t)stream);
+    unet_of(h).unet_forward(z, z_dtype, t, in_scale, (__half*)eps_uc, (__half*)eps_c, (cudaStream_t)stream);
   });
 }
 
 CFGPP_API int cfgpp_set_schedule(cfgpp_handle* h, int method, int state_dtype, const cfgpp_step_state* steps,
                                  int nsteps, void* stream) {
-  return guarded([&] { h->unet.set_schedule(method, state_dtype, steps, nsteps, (cudaStream_t)stream); });
+  return guarded([&] { unet_of(h).set_schedule(method, state_dtype, steps, nsteps, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_set_state(cfgpp_handle* h, const void* z, int z_dtype, void* stream) {
-  return guarded([&] { h->unet.set_state(z, z_dtype, (cudaStream_t)stream); });
+  return guarded([&] { unet_of(h).set_state(z, z_dtype, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_set_noise(cfgpp_handle* h, const void* noise_dev, int slots, void* stream) {
-  return guarded([&] { h->unet.set_noise((const __half*)noise_dev, slots, (cudaStream_t)stream); });
+  return guarded([&] { unet_of(h).set_noise((const __half*)noise_dev, slots, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_set_guidance(cfgpp_handle* h, const float* lambda_host, int n, void* stream) {
-  return guarded([&] { h->unet.set_guidance(lambda_host, n, (cudaStream_t)stream); });
+  return guarded([&] { unet_of(h).set_guidance(lambda_host, n, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_set_v_coefs(cfgpp_handle* h, const float* ab_host, int nsteps, void* stream) {
-  return guarded([&] { h->unet.set_v_coefs(ab_host, nsteps, (cudaStream_t)stream); });
+  return guarded([&] { unet_of(h).set_v_coefs(ab_host, nsteps, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_run_steps(cfgpp_handle* h, int first_step, int nsteps, void* stream) {
-  return guarded([&] { h->unet.run_steps(first_step, nsteps, (cudaStream_t)stream); });
+  return guarded([&] { unet_of(h).run_steps(first_step, nsteps, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_get_state(cfgpp_handle* h, int which, void* out, void* stream) {
-  return guarded([&] { h->unet.get_state(which, out, (cudaStream_t)stream); });
+  return guarded([&] { unet_of(h).get_state(which, out, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_apply_step(cfgpp_handle* h, int step, const void* eps_uc, const void* eps_c, void* stream) {
-  return guarded([&] { h->unet.apply_step(step, (const __half*)eps_uc, (const __half*)eps_c, (cudaStream_t)stream); });
+  return guarded([&] { unet_of(h).apply_step(step, (const __half*)eps_uc, (const __half*)eps_c, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_profile_forward(cfgpp_handle* h, const void* z, int z_dtype, float t, float in_scale, int max_n,
                                     int* n_out, float* ms_out, double* flops_out, int* kind_out, char* names_out,
                                     int name_stride, void* stream) {
   return guarded([&] {
-    auto prof = h->unet.profile_forward(z, z_dtype, t, in_scale, (cudaStream_t)stream);
+    auto prof = unet_of(h).profile_forward(z, z_dtype, t, in_scale, (cudaStream_t)stream);
     const int n = static_cast<int>(prof.size()) < max_n ? static_cast<int>(prof.size()) : max_n;
     *n_out = n;
     for (int i = 0; i < n; ++i) {
@@ -152,6 +164,37 @@ CFGPP_API int cfgpp_profile_forward(cfgpp_handle* h, const void* z, int z_dtype,
         names_out[static_cast<size_t>(i) * name_stride + len] = 0;
       }
     }
+  });
+}
+
+CFGPP_API int cfgpp_controlnet_create(const cfgpp_controlnet_desc* desc, int device, cfgpp_handle** out) {
+  return guarded([&] {
+    CFGPP_REQUIRE(desc && out, "null argument");
+    *out = new cfgpp_handle(desc->model, device, desc);
+  });
+}
+
+CFGPP_API int cfgpp_attach_controlnet(cfgpp_handle* h, cfgpp_handle* cn) {
+  return guarded([&] { unet_of(h).attach_controlnet(cn ? &cn->unet : nullptr); });
+}
+
+CFGPP_API int cfgpp_set_control_image(cfgpp_handle* h, const void* image, int dtype, void* stream) {
+  return guarded([&] { unet_of(h).set_control_image(image, dtype, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_set_control_scale(cfgpp_handle* h, float scale, void* stream) {
+  return guarded([&] { unet_of(h).set_control_scale(scale, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_set_control_scales(cfgpp_handle* h, const float* scales_host, int nsteps, void* stream) {
+  return guarded([&] { unet_of(h).set_control_scales(scales_host, nsteps, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_controlnet_embed(cfgpp_handle* cn, const void* image, int dtype, int batch, int height, int width,
+                                     void* out, void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(dtype == CFGPP_F16 || dtype == CFGPP_F32, "control image: fp16 or fp32 tensor");
+    cn->unet.cond_embed(image, dtype == CFGPP_F16, batch, height, width, (__half*)out, (cudaStream_t)stream);
   });
 }
 

@@ -48,6 +48,18 @@ CFGPP_API int cfgpp_op_linear_lnfold(const void* a, const void* w, int M, int N,
   });
 }
 
+CFGPP_API int cfgpp_op_linear_scaled_residual(const void* a, const void* w, int M, int N, int K, const void* bias,
+                                              const void* addend, const float* scale_dev, void* out, int force_bn,
+                                              void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(addend != nullptr, "the scaled residual epilogue needs an addend");
+    GemmOp op = make_linear_op((const __half*)a, K, nullptr, 0, 0, (const __half*)w, M, N, K, (const __half*)bias,
+                               (const __half*)addend, N, 1, (__half*)out, N, false, force_bn);
+    op.p.res_scale = scale_dev;
+    run_gemm_op(op, (cudaStream_t)stream);
+  });
+}
+
 CFGPP_API int cfgpp_op_fold_ln(const void* w, const void* gamma, const void* beta, const void* bias, void* wf,
                                float* s, float* t, int N, int K, void* stream) {
   return guarded([&] {
@@ -279,6 +291,16 @@ CFGPP_API int cfgpp_op_conv_in(const void* z, int z_dtype, const float* in_scale
   return guarded([&] {
     run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, in_scale_dev, (const __half*)w, (const __half*)bias, (__half*)out, B,
                 H, W, Cout, reps, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_conv_in_add(const void* z, int z_dtype, const float* in_scale_dev, const void* w,
+                                   const void* bias, const void* addend, void* out, int B, int H, int W, int Cout,
+                                   int reps, void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(addend != nullptr, "null addend");
+    run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, in_scale_dev, (const __half*)w, (const __half*)bias, (__half*)out, B,
+                H, W, Cout, reps, (cudaStream_t)stream, (const __half*)addend);
   });
 }
 

@@ -3,6 +3,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "executor.cuh"
 #include "ops.cuh"
 
 namespace cfgpp {
@@ -104,12 +105,14 @@ __global__ void copy_rows_kernel(const __half* __restrict__ src, int src_rows, i
 // conv_in: 4 -> Cout, 3x3 pad 1, NCHW latent -> NHWC fp16. thread = (pixel, 8 output channels)
 // ------------------------------------------------------------------------------------------------------------
 __global__ void select_step_kernel(const StepState* __restrict__ table, int* counter, StepState* cur,
-                                   const float2* __restrict__ v_table, float2* v_cur) {
+                                   const float2* __restrict__ v_table, float2* v_cur, const float* __restrict__ s_table,
+                                   float* s_cur) {
   pdl_launch_dependents();
   pdl_wait();
   const int i = *counter;
   *cur = table[i];
   if (v_table) *v_cur = v_table[i];
+  if (s_table) *s_cur = s_table[i];
   *counter = i + 1;
 }
 
@@ -135,7 +138,8 @@ CFGPP_DEVICE float v_to_eps(float v, float x_in, float a, float b) {
 
 __global__ void conv_in_kernel(const void* __restrict__ z, int z_is_half, const float* __restrict__ in_scale_ptr,
                                const __half* __restrict__ w, const __half* __restrict__ bias, __half* __restrict__ out,
-                               int B, int H, int W, int Cout, int reps, int px_per_block) {
+                               int B, int H, int W, int Cout, int reps, int px_per_block,
+                               const __half* __restrict__ addend) {
   pdl_launch_dependents();
   pdl_wait();
   // thread = (group of 4 horizontally adjacent pixels, 8 output channels): the 4 x 3 x 6 input patch is loaded once
@@ -200,6 +204,14 @@ __global__ void conv_in_kernel(const void* __restrict__ z, int z_is_half, const 
       o.z = pack_half2(acc[px][4], acc[px][5]);
       o.w = pack_half2(acc[px][6], acc[px][7]);
       const size_t pix = static_cast<size_t>(b) * HW + h * W + x0 + px;
+      if (addend) {  // fp16(fp16(conv) + addend), the addend's B images shared by every repetition
+        const uint4 a = *reinterpret_cast<const uint4*>(addend + pix * Cout + ocg * 8);
+        const __half2* ah = reinterpret_cast<const __half2*>(&a);
+        __half2* oh = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          oh[i] = __floats2half2_rn(__low2float(oh[i]) + __low2float(ah[i]), __high2float(oh[i]) + __high2float(ah[i]));
+      }
       for (int rep = 0; rep < reps; ++rep)
         *reinterpret_cast<uint4*>(out + (static_cast<size_t>(rep) * total + pix) * Cout + ocg * 8) = o;
     }
@@ -480,12 +492,12 @@ void run_copy_rows(const __half* src, int src_rows, int cols, __half* dst, int l
 }
 
 void run_select_step(const StepState* table, int* counter, StepState* cur, cudaStream_t stream, const float2* v_table,
-                     float2* v_cur) {
-  launch_pdl(select_step_kernel, dim3(1), dim3(1), 0, stream, table, counter, cur, v_table, v_cur);
+                     float2* v_cur, const float* s_table, float* s_cur) {
+  launch_pdl(select_step_kernel, dim3(1), dim3(1), 0, stream, table, counter, cur, v_table, v_cur, s_table, s_cur);
 }
 
 void run_conv_in(const void* z, int z_is_half, const float* in_scale, const __half* w, const __half* bias,
-                 __half* out, int B, int H, int W, int Cout, int reps, cudaStream_t stream) {
+                 __half* out, int B, int H, int W, int Cout, int reps, cudaStream_t stream, const __half* addend) {
   CFGPP_REQUIRE(Cout % 8 == 0 && W % 4 == 0, "conv_in needs Cout % 8 == 0 and W % 4 == 0");
   const int ppb = 128;
   const size_t smem = (36 * Cout + Cout) * sizeof(float);
@@ -496,7 +508,69 @@ void run_conv_in(const void* z, int z_is_half, const float* in_scale, const __ha
   }
   const int total = B * H * W;
   launch_pdl(conv_in_kernel, dim3((total + ppb - 1) / ppb), dim3(320), smem, stream, z, z_is_half, in_scale, w, bias, out, B, H, W, Cout,
-                                                                 reps, ppb);
+                                                                 reps, ppb, addend);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// ControlNet conditioning embedding: the image in, a SiLU pass, and its 3x3 convolutions' weights zero-padded to
+// channel counts the implicit-GEMM convolution takes (exact: padded channels are zero in and zero out)
+// ------------------------------------------------------------------------------------------------------------
+__global__ void image_to_nhwc_kernel(const void* __restrict__ x, int x_is_half, __half* __restrict__ out, int B, int C,
+                                     int HW, int Cp) {
+  const size_t n = static_cast<size_t>(B) * HW * Cp;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int c = i % Cp;
+    const size_t pix = i / Cp;
+    const size_t b = pix / HW, p = pix % HW;
+    __half v = __float2half(0.f);
+    if (c < C) {
+      const size_t src = (b * C + c) * HW + p;
+      v = x_is_half ? reinterpret_cast<const __half*>(x)[src] : __float2half_rn(reinterpret_cast<const float*>(x)[src]);
+    }
+    out[i] = v;
+  }
+}
+
+__global__ void silu_kernel(__half* __restrict__ x, size_t n) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const float v = __half2float(x[i]);
+    x[i] = __float2half_rn(v / (1.0f + expf(-v)));
+  }
+}
+
+__global__ void pack_conv3x3_padded_kernel(const __half* __restrict__ w, const __half* __restrict__ bias,
+                                           __half* __restrict__ wp, __half* __restrict__ bp, int Cout, int Cin,
+                                           int Cout_p, int Cin_p) {
+  const size_t n = static_cast<size_t>(Cout_p) * 9 * Cin_p;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int c = i % Cin_p;
+    const int tap = (i / Cin_p) % 9;
+    const int o = i / (static_cast<size_t>(9) * Cin_p);
+    wp[i] = (o < Cout && c < Cin) ? w[(static_cast<size_t>(o) * Cin + c) * 9 + tap] : __float2half(0.f);
+    if (tap == 0 && c == 0) bp[o] = o < Cout ? bias[o] : __float2half(0.f);
+  }
+}
+
+void run_image_to_nhwc(const void* x, int x_is_half, __half* out, int B, int C, int H, int W, int Cp,
+                       cudaStream_t stream) {
+  const size_t n = static_cast<size_t>(B) * H * W * Cp;
+  image_to_nhwc_kernel<<<grid_for(n), 256, 0, stream>>>(x, x_is_half, out, B, C, H * W, Cp);
+  CFGPP_CHECK_CUDA(cudaGetLastError());
+}
+
+void run_silu(__half* x, size_t n, cudaStream_t stream) {
+  silu_kernel<<<grid_for(n), 256, 0, stream>>>(x, n);
+  CFGPP_CHECK_CUDA(cudaGetLastError());
+}
+
+void run_pack_conv3x3_padded(const __half* w, const __half* bias, __half* wp, __half* bp, int Cout, int Cin, int Cout_p,
+                             int Cin_p, cudaStream_t stream) {
+  const size_t n = static_cast<size_t>(Cout_p) * 9 * Cin_p;
+  pack_conv3x3_padded_kernel<<<grid_for(n), 256, 0, stream>>>(w, bias, wp, bp, Cout, Cin, Cout_p, Cin_p);
+  CFGPP_CHECK_CUDA(cudaGetLastError());
 }
 
 // The state dtype travels in bit 8 of `mode` (mode | 0x100 = fp16 sampler state).

@@ -57,7 +57,9 @@ struct Cfg {
   static constexpr int ACC = BN / 2;  // fp32 accumulator registers per thread (m64 x BN over 128 threads)
 };
 
-template <int BN, bool GEGLU>
+// SCALED: the scaled-residual epilogue (GemmParams::res_scale), a kernel of its own so that the production epilogues
+// compile exactly as they would without it
+template <int BN, bool GEGLU, bool SCALED = false>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_a2,
             const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_out,
@@ -529,8 +531,11 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
       if constexpr (!GEGLU) {
         auto chunks = [&](auto ln_c, auto add_c, auto st_c) {
           constexpr bool LN = decltype(ln_c)::value;
-          constexpr int ADD = decltype(add_c)::value;  // 0 none, 1 full residual tile, 2 staged row, 3 per-row global
+          // 0 none, 1 full residual tile, 2 staged row, 3 per-row global, 4 full residual tile + scaled result
+          constexpr int ADD = decltype(add_c)::value;
           constexpr bool ST = decltype(st_c)::value;
+          float res_s = 1.f;
+          if constexpr (ADD == 4) res_s = *p.res_scale;
 #pragma unroll
           for (int i = 0; i < BN / 8; ++i) {  // 8-column group i: sub-tile i / 4, 16-byte piece i % 4
             const int col = i * 8 + cq;
@@ -557,7 +562,11 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
               }
               __half2 t = __floats2half2_rn(x0, x1);
               __half2* sp = reinterpret_cast<__half2*>(sub + stage_off(r, i & 3));
-              if constexpr (ADD == 1 || ADD == 2) {
+              if constexpr (ADD == 4) {  // fp16(addend + fp16(t * s)): the ControlNet residual at its step's scale
+                const __half2 rh = *sp;
+                const __half2 ts = __floats2half2_rn(__low2float(t) * res_s, __high2float(t) * res_s);
+                t = __floats2half2_rn(__low2float(rh) + __low2float(ts), __high2float(rh) + __high2float(ts));
+              } else if constexpr (ADD == 1 || ADD == 2) {
                 const __half2 rh = ADD == 1 ? *sp : *reinterpret_cast<const __half2*>(s_temb + col);
                 t = __floats2half2_rn(__low2float(t) + __low2float(rh), __high2float(t) + __high2float(rh));
               } else if constexpr (ADD == 3) {  // tile spans several samples (tiny latents): per-row global loads
@@ -580,7 +589,9 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
         using T = std::true_type;
         using F = std::false_type;
         const int add_mode = full_res ? 1 : (p.addend == nullptr ? 0 : (temb_staged ? 2 : 3));
-        if (p.stats_in) {  // LayerNorm-fold consumer: bias is inside t_n; no addend, no statistics (host-checked)
+        if constexpr (SCALED) {  // full residual, no fold, no statistics (host-checked)
+          chunks(F{}, std::integral_constant<int, 4>{}, F{});
+        } else if (p.stats_in) {  // LayerNorm-fold consumer: bias is inside t_n; no addend, no statistics (host-checked)
           chunks(T{}, std::integral_constant<int, 0>{}, F{});
         } else if (p.stats_out) {
           switch (add_mode) {
@@ -672,17 +683,17 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap map_a, const
 #undef TL
 }
 
-template <int BN, bool GEGLU>
+template <int BN, bool GEGLU, bool SCALED = false>
 void configure_one() {
-  CFGPP_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, GEGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  CFGPP_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, GEGLU, SCALED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         Cfg<BN, GEGLU>::SMEM_BYTES));
 }
 
-template <int BN, bool GEGLU>
+template <int BN, bool GEGLU, bool SCALED = false>
 void launch(const GemmOp& op, cudaStream_t stream) {
   gemm_configure();
-  launch_pdl(gemm_kernel<BN, GEGLU>, dim3(op.grid), dim3(kThreads), Cfg<BN, GEGLU>::SMEM_BYTES, stream, op.p, op.map_a,
-             op.map_a2, op.map_b, op.map_out, op.map_res);
+  launch_pdl(gemm_kernel<BN, GEGLU, SCALED>, dim3(op.grid), dim3(kThreads), Cfg<BN, GEGLU>::SMEM_BYTES, stream, op.p,
+             op.map_a, op.map_a2, op.map_b, op.map_out, op.map_res);
 }
 
 constexpr double kSkMinSaved = 4.0;  // k-blocks of main loop the split must save per CTA
@@ -819,6 +830,10 @@ void gemm_configure() {
   configure_one<160, false>();
   configure_one<256, false>();
   configure_one<256, true>();
+  configure_one<64, false, true>();
+  configure_one<128, false, true>();
+  configure_one<160, false, true>();
+  configure_one<256, false, true>();
   done = true;
 }
 
@@ -921,7 +936,19 @@ void run_gemm_op(const GemmOp& op, cudaStream_t stream) {
   CFGPP_REQUIRE(!(op.p.stats_in && op.p.bias),
                 "a LayerNorm-fold consumer GEMM takes its bias inside t_n (run_fold_ln), not as a bias vector");
   CFGPP_REQUIRE(!(op.p.geglu && (op.p.addend || op.p.stats_out)), "the GEGLU epilogue takes no addend / statistics");
+  CFGPP_REQUIRE(!op.p.res_scale || (op.p.addend && op.p.add_rows_per_group <= 1 && !op.p.stats_out && !op.p.stats_in &&
+                                    !op.p.geglu),
+                "a scaled residual needs a full residual addend and no LayerNorm fold, statistics or GEGLU");
   if (op.p.geglu) return launch<256, true>(op, stream);
+  if (op.p.res_scale) {
+    switch (op.bn) {
+      case 64: return launch<64, false, true>(op, stream);
+      case 128: return launch<128, false, true>(op, stream);
+      case 160: return launch<160, false, true>(op, stream);
+      case 256: return launch<256, false, true>(op, stream);
+      default: throw Error(-1, "bad BN");
+    }
+  }
   switch (op.bn) {
     case 64: return launch<64, false>(op, stream);
     case 128: return launch<128, false>(op, stream);

@@ -18,6 +18,9 @@
 //   t = fp16(acc + bias[n]);  out = addend ? fp16(float(t) + float(addend)) : t
 //   addend is either a full residual [M, ld_add] or a per-sample row broadcast [M / add_rows_per_group][ld_add]
 //   (the ResnetBlock2D time-embedding add).
+//   Scaled residual (res_scale set, full residual only — a ControlNet zero conv adding into a UNet skip tensor):
+//   out = fp16(float(addend) + float(fp16(float(t) * s))), s = *res_scale read on the device (a kernel instantiation of
+//   its own: the other epilogues compile as they would without it).
 //   GEGLU variant: weight rows interleaved per 256-wide tile as 128 'value' rows + 128 'gate' rows;
 //   out[m, j] = fp16( fp16(a) * fp16(gelu_erf(fp16(g))) ), N_out = N / 2.
 #pragma once
@@ -41,6 +44,7 @@ struct GemmParams {
   const __half* addend;
   int ld_add;
   int add_rows_per_group;  // 1: full residual; >1: row m uses addend row (m / add_rows_per_group)
+  const float* res_scale;  // full residual only: scale the tile's fp16 result by *res_scale before the add, or null
   __half* out;
   int ldc;
   int geglu;

@@ -36,8 +36,19 @@ void run_copy_rows(const __half* src, int src_rows, int cols, __half* dst, int l
 // conv_in 3x3 pad 1, Cin = 4: z [B,4,H,W] (fp32 or fp16 NCHW, optionally scaled by in_scale in fp16 arithmetic)
 // -> NHWC fp16 [reps*B, H, W, Cout]; the same result is written `reps` times (uncond and cond halves share z).
 // in_scale (device pointer, may be null): model input is z * (*in_scale) — the DPM++ `x * c_in` (latent_sdxl.py:901).
+// addend (may be null): [B, H, W, Cout] NHWC fp16, added to every repetition as fp16(fp16(conv) + addend) — the
+// ControlNet's `sample + cond`.
 void run_conv_in(const void* z, int z_is_half, const float* in_scale, const __half* w /*[Cout][36]*/,
-                 const __half* bias, __half* out, int B, int H, int W, int Cout, int reps, cudaStream_t stream);
+                 const __half* bias, __half* out, int B, int H, int W, int Cout, int reps, cudaStream_t stream,
+                 const __half* addend = nullptr);
+// ControlNet conditioning embedding helpers: image [B,C,H,W] NCHW (fp16 or fp32) -> fp16 NHWC [B,H,W,Cp] with zero
+// channels C..Cp-1; in-place fp16(SiLU(x)) over n values; a (Cout,Cin,3,3) weight and its bias -> [Cout_p][9][Cin_p]
+// and [Cout_p], zero beyond Cout / Cin.
+void run_image_to_nhwc(const void* x, int x_is_half, __half* out, int B, int C, int H, int W, int Cp,
+                       cudaStream_t stream);
+void run_silu(__half* x, size_t n, cudaStream_t stream);
+void run_pack_conv3x3_padded(const __half* w, const __half* bias, __half* wp, __half* bp, int Cout, int Cin, int Cout_p,
+                             int Cin_p, cudaStream_t stream);
 
 enum StepMode : int {
   STEP_NONE = 0,        // only emit eps_uc / eps_c (the predict_noise seam)
@@ -70,8 +81,10 @@ struct StepState {
   StepCoef coef;
 };
 // v_table (may be null): a parallel table of v-prediction coefficients (a, b) per step, selected into *v_cur alongside
+// s_table (may be null): the ControlNet conditioning scale per step, selected into *s_cur alongside
 void run_select_step(const StepState* table, int* counter, StepState* cur, cudaStream_t stream,
-                     const float2* v_table = nullptr, float2* v_cur = nullptr);
+                     const float2* v_table = nullptr, float2* v_cur = nullptr, const float* s_table = nullptr,
+                     float* s_cur = nullptr);
 
 // conv_out 3x3 (Cin -> 4) on the GroupNorm+SiLU'ed NHWC input x [2B,H,W,Cin] fused with the CFG++ guidance mix and
 // the scheduler update. noise_slot (may be null): device word holding the base of the ancestral noise table

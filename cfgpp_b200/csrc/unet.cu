@@ -63,8 +63,20 @@ __global__ void pack_heads_cols_kernel(const __half* __restrict__ in, __half* __
 void gemm_configure();
 void attn_configure();
 
-Unet::Unet(const cfgpp_model_desc& d, int device) : d_(d), device_(device), sk_(device) {
+Unet::Unet(const cfgpp_model_desc& d, int device, const cfgpp_controlnet_desc* cn)
+    : d_(d), device_(device), sk_(device) {
   CFGPP_CHECK_CUDA(cudaSetDevice(device));
+  if (cn) {
+    is_cn_ = true;
+    cn_desc_ = *cn;
+    CFGPP_REQUIRE(cn->conditioning_channels >= 1 && cn->conditioning_channels <= 64,
+                  "conditioning_channels must be 1..64");
+    CFGPP_REQUIRE(cn->num_embedding_levels == 4,
+                  "the conditioning embedding must take 4 channel counts (it downsamples the image by 8 to the latent)");
+    for (int i = 0; i < cn->num_embedding_levels; ++i)
+      CFGPP_REQUIRE(cn->embedding_channels[i] >= 1, "conditioning embedding channels must be positive");
+    CFGPP_REQUIRE(d.block_out_channels[0] % 8 == 0, "block_out_channels[0] must be a multiple of 8");
+  }
   CFGPP_REQUIRE(d.num_levels >= 2 && d.num_levels <= CFGPP_MAX_LEVELS, "num_levels must be 2..4");
   CFGPP_REQUIRE(d.norm_num_groups == 32, "only GroupNorm(32) is implemented");
   CFGPP_REQUIRE(d.in_channels == 4 && d.out_channels == 4, "latent channels must be 4");
@@ -87,6 +99,12 @@ Unet::Unet(const cfgpp_model_desc& d, int device) : d_(d), device_(device), sk_(
 }
 
 Unet::~Unet() {
+  if (owner_) {  // the UNet's plan reads this handle's buffers: it must be built again
+    owner_->cn_ = nullptr;
+    owner_->prepared_ = false;
+    owner_->graph_valid_ = false;
+  }
+  if (cn_) cn_->owner_ = nullptr;
   if (graph_exec_) cudaGraphExecDestroy(graph_exec_);
   if (graph_) cudaGraphDestroy(graph_);
   if (capture_stream_) cudaStreamDestroy(capture_stream_);
@@ -263,7 +281,42 @@ void Unet::finalize_weights(cudaStream_t stream) {
   try {
     // the smallest latent for which every level keeps a spatial extent (H, W >= 1 at the deepest level)
     const int s = 1 << (d_.num_levels - 1);
-    prepare(1, std::max(8, s * 8), std::max(8, s * 8));
+    if (is_cn_) {
+      // the conditioning embedding's convolutions, zero-padded to whole 64-channel K blocks, and the zero convs
+      auto pad64 = [](int c) { return (c + 63) / 64 * 64; };
+      const int n = cn_desc_.num_embedding_levels;
+      const int* ch = cn_desc_.embedding_channels;
+      auto pack = [&](const std::string& name, int cin, int cout, int cout_p) {
+        const std::string k = "controlnet_cond_embedding." + name;
+        const WeightStore::Weight& w = weights_.raw(k + ".weight");
+        CFGPP_REQUIRE(w.shape.size() == 4 && w.shape[0] == cout && w.shape[1] == cin && w.shape[2] == 3 &&
+                          w.shape[3] == 3,
+                      "unexpected shape of " + k + ".weight");
+        EmbedConv c{weights_.alloc(static_cast<size_t>(cout_p) * 9 * pad64(cin)), weights_.alloc(cout_p), cout_p,
+                    pad64(cin)};
+        run_pack_conv3x3_padded(w.p(), weights_.plain(k + ".bias", cout), c.w, c.b, cout, cin, cout_p, c.cin_p, stream);
+        embed_convs_[name] = c;
+      };
+      pack("conv_in", cn_desc_.conditioning_channels, ch[0], pad64(ch[0]));
+      for (int i = 0; i + 1 < n; ++i) {
+        pack("blocks." + std::to_string(2 * i), ch[i], ch[i], pad64(ch[i]));
+        pack("blocks." + std::to_string(2 * i + 1), ch[i], ch[i + 1], pad64(ch[i + 1]));
+      }
+      pack("conv_out", ch[n - 1], d_.block_out_channels[0], d_.block_out_channels[0]);
+      CFGPP_CHECK_CUDA(cudaStreamSynchronize(stream));
+      CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
+      StreamKScope sk_scope(sk_.ws(), sk_.flags());
+      build(1, std::max(8, s * 8), std::max(8, s * 8), nullptr);
+      const std::vector<std::string> keys = zero_conv_keys();
+      for (size_t k = 0; k < keys.size(); ++k) {
+        const size_t C = res_[k].C;
+        weights_.plain(keys[k] + ".weight", C * C);
+        weights_.plain(keys[k] + ".bias", C);
+      }
+      CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
+    } else {
+      prepare(1, std::max(8, s * 8), std::max(8, s * 8));
+    }
     prepared_ = false;
   } catch (...) {
     finalized_ = false;
@@ -506,6 +559,7 @@ Unet::Act Unet::build_upsample(const std::string& prefix, Act x, int H, int W) {
 }
 
 void Unet::prepare(int batch, int h_lat, int w_lat) {
+  CFGPP_REQUIRE(!is_cn_, "a ControlNet handle is prepared through the UNet handle it is attached to");
   CFGPP_REQUIRE(finalized_, "call cfgpp_finalize_weights first");
   // validate BEFORE anything is freed: a rejected shape must leave the previous plan usable
   CFGPP_REQUIRE(batch >= 1 && 2 * batch <= 16, "batch must be 1..8 (UNet batch 2*batch <= 16)");
@@ -526,6 +580,24 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
   CFGPP_CHECK_CUDA(cudaSetDevice(device_));
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
   StreamKScope sk_scope(sk_.ws(), sk_.flags());  // every GEMM op built below parks its stream-K partials in OUR workspace
+  cn_image_ready_ = false;
+  build(batch, h_lat, w_lat, nullptr);
+  if (cn_) {
+    // the ControlNet's ops are built under this handle's stream-K scope: they run on this handle's stream
+    cn_->build(batch, h_lat, w_lat, cur_state_);
+    cn_->account();
+    cn_scale_table_ = act_.alloc<float>(1024);
+    cn_scale_cur_ = act_.alloc<float>(1);
+    fill_control_table(nullptr);
+    CFGPP_CHECK_CUDA(cudaMemcpy(cn_scale_cur_, &cn_scale_, sizeof(float), cudaMemcpyHostToDevice));
+    build_control_plan();
+  }
+  account();
+  CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
+  prepared_ = true;
+}
+
+void Unet::build(int batch, int h_lat, int w_lat, StepState* shared_state) {
   // from here on the old plan is gone: a throw below must not leave the handle looking prepared
   prepared_ = false;
   nsteps_ = 0;
@@ -536,8 +608,12 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
   scratch_.clear();
   prologue_plan_.clear();
   body_plan_.clear();
+  control_plan_.clear();
+  up_plan_.clear();
   tail_plan_.clear();
   prompt_plan_.clear();
+  res_.clear();
+  res_hw_.clear();
   B_ = batch; NB_ = 2 * batch; H_ = h_lat; W_ = w_lat;
   const int L = d_.num_levels;
   const int C0 = d_.block_out_channels[0];
@@ -558,7 +634,7 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
       reg_resnet("down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), d_.block_out_channels[i]);
   reg_resnet("mid_block.resnets.0", d_.block_out_channels[L - 1]);
   reg_resnet("mid_block.resnets.1", d_.block_out_channels[L - 1]);
-  for (int i = 0; i < L; ++i)
+  for (int i = 0; i < (is_cn_ ? 0 : L); ++i)  // a ControlNet has no up path
     for (int j = 0; j < d_.layers_per_block + 1; ++j)
       reg_resnet("up_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), d_.block_out_channels[L - 1 - i]);
   auto temb_off = [&](const std::string& prefix) {
@@ -586,30 +662,36 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
         pooled_copy_ = alloc_act(static_cast<size_t>(NB_) * d_.pooled_dim);
         time_ids_copy_ = act_.alloc<float>(static_cast<size_t>(NB_) * n_time_ids_);
       }
-      cur_state_ = act_.alloc<StepState>(1);
-      step_counter_ = act_.alloc<int>(1);
-      step_table_ = act_.alloc<StepState>(1024);
-      if (v_pred_) {
-        v_table_ = act_.alloc<float2>(1024);
-        v_cur_ = act_.alloc<float2>(1);
+      cur_state_ = shared_state ? shared_state : act_.alloc<StepState>(1);
+      if (!is_cn_) {  // the sampler state and tables: a ControlNet runs inside its UNet's step
+        step_counter_ = act_.alloc<int>(1);
+        step_table_ = act_.alloc<StepState>(1024);
+        if (v_pred_) {
+          v_table_ = act_.alloc<float2>(1024);
+          v_cur_ = act_.alloc<float2>(1);
+        }
+        const size_t lat = static_cast<size_t>(B_) * 4 * H_ * W_;
+        z_state_ = act_.alloc<float>(lat);
+        aux_state_ = act_.alloc<float>(lat);
+        z0t_state_ = act_.alloc<float>(lat);
+        noise_slot_ = act_.alloc<const __half*>(1);
+        CFGPP_CHECK_CUDA(cudaMemcpy(noise_slot_, &noise_buf_, sizeof(__half*), cudaMemcpyHostToDevice));
+        lambda_buf_ = act_.alloc<float>(B_);
+        lambda_slot_ = act_.alloc<const float*>(1);
+        CFGPP_CHECK_CUDA(cudaMemset(lambda_slot_, 0, sizeof(float*)));  // no table: the schedule's scalar lambda
+        fwd_eps_uc_ = alloc_act(lat);
+        fwd_eps_c_ = alloc_act(lat);
+      } else {
+        cond_ = alloc_act(static_cast<size_t>(B_) * H_ * W_ * C0);
       }
-      const size_t lat = static_cast<size_t>(B_) * 4 * H_ * W_;
-      z_state_ = act_.alloc<float>(lat);
-      aux_state_ = act_.alloc<float>(lat);
-      z0t_state_ = act_.alloc<float>(lat);
-      noise_slot_ = act_.alloc<const __half*>(1);
-      CFGPP_CHECK_CUDA(cudaMemcpy(noise_slot_, &noise_buf_, sizeof(__half*), cudaMemcpyHostToDevice));
-      lambda_buf_ = act_.alloc<float>(B_);
-      lambda_slot_ = act_.alloc<const float*>(1);
-      CFGPP_CHECK_CUDA(cudaMemset(lambda_slot_, 0, sizeof(float*)));  // no table: the schedule's scalar lambda
-      fwd_eps_uc_ = alloc_act(lat);
-      fwd_eps_c_ = alloc_act(lat);
       temb_w_all_ = packed_cat_rows(temb_w_keys);
       temb_b_all_ = packed_cat_rows(temb_b_keys);
       conv_in_w_ = weights_.plain("conv_in.weight");
       conv_in_b_ = weights_.plain("conv_in.bias");
-      conv_out_w_ = weights_.packed_conv3x3("conv_out.weight");
-      conv_out_b_ = weights_.plain("conv_out.bias");
+      if (!is_cn_) {
+        conv_out_w_ = weights_.packed_conv3x3("conv_out.weight");
+        conv_out_b_ = weights_.plain("conv_out.bias");
+      }
     }
 
     // ---- prologue: timestep embedding -> per-resnet time_emb_proj (SURVEY A.2 step 1, ResnetBlock2D temb) ----
@@ -687,6 +769,17 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
       h = build_transformer("mid_block.attentions.0", h, H, W, d_.transformer_layers[L - 1], d_.num_heads[L - 1]);
       h = build_resnet("mid_block.resnets.1", h, nullptr, Cm, H, W, temb_off("mid_block.resnets.1"));
     }
+    if (!sizing_) {
+      conv_in_out_ = h0.p;
+      res_ = skips;
+      res_.push_back(h);
+      for (int i = 0, hh = H_, ww = W_; i < L; ++i, hh /= 2, ww /= 2)
+        for (int j = 0; j < d_.layers_per_block + (i == 0 ? 1 : 0) + (i != L - 1 ? 1 : 0); ++j)
+          res_hw_.push_back(j == d_.layers_per_block + (i == 0 ? 1 : 0) && i != L - 1 ? (hh / 2) * (ww / 2) : hh * ww);
+      res_hw_.push_back(H * W);
+    }
+    if (is_cn_) continue;  // a ControlNet's plan ends with its mid block
+    cur_plan_ = &up_plan_;
     for (int i = 0; i < L; ++i) {
       const std::string blk = "up_blocks." + std::to_string(i);
       const int rev = L - 1 - i;
@@ -720,14 +813,18 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
         run_groupnorm(hp, C0, nullptr, 0, NB, HW, g, b, eps, true, partial, normp, st);
       }, 2);
       final_norm_ = Act{normp, C0};
-      conv_in_out_ = h0.p;
     }
   }
+  if (is_cn_ && shared_state) prepared_ = true;  // built for its UNet: set_prompt may run
+}
 
+void Unet::account() {
   // FLOP / launch accounting (the reference executes the K/V projections every step: count them per forward)
+  const int C0 = d_.block_out_channels[0];
+  const int TE = time_embed_dim_;
   forward_flops_ = 0.0;
-  launches_per_step_ = 3;  // select_step + conv_in + conv_out_step
-  for (auto* pl : {&body_plan_, &tail_plan_})
+  launches_per_step_ = is_cn_ ? 1 : 3;  // (select_step +) conv_in (+ conv_out_step)
+  for (auto* pl : {&body_plan_, &control_plan_, &up_plan_, &tail_plan_})
     for (auto& s : *pl) { forward_flops_ += s.flops; launches_per_step_ += s.launches; }
   for (auto& s : prologue_plan_) launches_per_step_ += s.launches;
   prompt_flops_ = 0.0;
@@ -735,7 +832,7 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
   for (auto& s : prompt_plan_) { prompt_flops_ += s.flops; prompt_launches_ += s.launches; }
   forward_flops_ += prompt_flops_;
   const double px = static_cast<double>(NB_) * H_ * W_;
-  forward_flops_ += 2.0 * px * (36.0 * C0 + 36.0 * C0);  // conv_in + conv_out
+  forward_flops_ += 2.0 * px * (36.0 * C0 + (is_cn_ ? 0.0 : 36.0 * C0));  // conv_in + conv_out
   forward_flops_ += 2.0 * NB_ * (static_cast<double>(C0) * TE + static_cast<double>(TE) * TE +
                                  static_cast<double>(temb_total_) * TE);
   if (has_aug_) {  // the add-embedding MLP runs in the prompt plan
@@ -744,8 +841,37 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
     forward_flops_ += f;
     prompt_flops_ += f;
   }
-  CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
-  prepared_ = true;
+  if (cn_) {
+    forward_flops_ += cn_->forward_flops_;
+    launches_per_step_ += cn_->launches_per_step_;
+    prompt_flops_ += cn_->prompt_flops_;
+    prompt_launches_ += cn_->prompt_launches_;
+  }
+}
+
+std::vector<std::string> Unet::zero_conv_keys() const {
+  std::vector<std::string> keys;
+  for (size_t k = 0; k + 1 < res_.size(); ++k) keys.push_back("controlnet_down_blocks." + std::to_string(k));
+  keys.push_back("controlnet_mid_block");
+  return keys;
+}
+
+void Unet::build_control_plan() {
+  // zero conv k: a 1x1 convolution of the ControlNet's k-th residual, scaled and added in place into the UNet's k-th
+  // skip tensor (the last: the mid-block output). The UNet's down path and mid block have consumed these tensors by
+  // the time this plan runs, so only the up path sees the sums.
+  CFGPP_REQUIRE(cn_->res_.size() == res_.size(), "internal: ControlNet residual count differs from the UNet's");
+  cur_plan_ = &control_plan_;
+  const std::vector<std::string> keys = cn_->zero_conv_keys();
+  for (size_t k = 0; k < res_.size(); ++k) {
+    const int C = res_[k].C;
+    CFGPP_REQUIRE(cn_->res_[k].C == C && cn_->res_hw_[k] == res_hw_[k], "internal: ControlNet residual shape mismatch");
+    const int M = NB_ * res_hw_[k];
+    GemmOp op = make_linear_op(cn_->res_[k].p, C, nullptr, 0, 0, cn_->weights_.plain(keys[k] + ".weight", size_t(C) * C),
+                               M, C, C, cn_->weights_.plain(keys[k] + ".bias", C), res_[k].p, C, 1, res_[k].p, C, false);
+    op.p.res_scale = cn_scale_cur_;
+    add_gemm(keys[k], op);
+  }
 }
 
 void Unet::run_plan(const std::vector<PlanStep>& plan, cudaStream_t stream) {
@@ -754,8 +880,32 @@ void Unet::run_plan(const std::vector<PlanStep>& plan, cudaStream_t stream) {
 
 // Body of the forward: conv_in output .. conv_norm_out, on the caller's stream.
 void Unet::run_body(cudaStream_t stream) {
+  if (cn_) run_plan(cn_->body_plan_, stream);
   run_plan(body_plan_, stream);
+  run_plan(control_plan_, stream);
+  run_plan(up_plan_, stream);
   run_plan(tail_plan_, stream);
+}
+
+// Prologue: the timestep embeddings; then conv_in (and the ControlNet's conv_in + conditioning embedding) on z.
+void Unet::run_inputs(const void* z, int z_is_half, cudaStream_t stream) {
+  run_plan(prologue_plan_, stream);
+  if (cn_) run_plan(cn_->prologue_plan_, stream);
+  const int C0 = d_.block_out_channels[0];
+  run_conv_in(z, z_is_half, &cur_state_->in_scale, conv_in_w_, conv_in_b_, conv_in_out_, B_, H_, W_, C0, 2, stream);
+  if (cn_)
+    run_conv_in(z, z_is_half, &cur_state_->in_scale, cn_->conv_in_w_, cn_->conv_in_b_, cn_->conv_in_out_, B_, H_, W_,
+                C0, 2, stream, cn_->cond_);
+}
+
+void Unet::require_control_ready() const {
+  CFGPP_REQUIRE(!cn_ || cn_image_ready_, "a ControlNet is attached: call cfgpp_set_control_image for the prepared shape");
+}
+
+void Unet::fill_control_table(cudaStream_t stream) {
+  cn_fill_.assign(1024, cn_scale_);
+  CFGPP_CHECK_CUDA(cudaMemcpyAsync(cn_scale_table_, cn_fill_.data(), 1024 * sizeof(float), cudaMemcpyHostToDevice,
+                                   stream));
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -781,6 +931,7 @@ void Unet::set_prompt(const __half* ctx, int n_ctx, const __half* pooled, const 
     }
   }
   run_plan(prompt_plan_, stream);
+  if (cn_) cn_->set_prompt(ctx, n_ctx, pooled, time_ids, add_rows, stream);
   prompt_stale_ = false;
 }
 
@@ -791,14 +942,14 @@ void Unet::unet_forward(const void* z, int z_dtype, float t, float in_scale, __h
                         cudaStream_t stream) {
   CFGPP_REQUIRE(prepared_, "call cfgpp_prepare first");
   require_fresh_prompt();
+  require_control_ready();
   StepState s{};
   s.t = t;
   s.in_scale = in_scale;
   // cudaMemcpyAsync from pageable memory stages the 48 bytes before returning: `s` may go out of scope
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(cur_state_, &s, sizeof(s), cudaMemcpyHostToDevice, stream));
-  run_plan(prologue_plan_, stream);
-  run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, &cur_state_->in_scale, conv_in_w_, conv_in_b_, conv_in_out_, B_, H_, W_,
-              d_.block_out_channels[0], 2, stream);
+  if (cn_) CFGPP_CHECK_CUDA(cudaMemcpyAsync(cn_scale_cur_, &cn_scale_, sizeof(float), cudaMemcpyHostToDevice, stream));
+  run_inputs(z, z_dtype == CFGPP_F16 ? 1 : 0, stream);
   run_body(stream);
   run_conv_out_step(final_norm_.p, conv_out_w_, conv_out_b_, B_, H_, W_, final_norm_.C, STEP_NONE, nullptr, nullptr,
                     nullptr, nullptr, eps_uc, eps_c, stream);
@@ -818,23 +969,34 @@ std::vector<Unet::ProfEntry> Unet::profile_forward(const void* z, int z_dtype, f
   StepState s{};
   s.t = t;
   s.in_scale = in_scale;
+  require_control_ready();
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(cur_state_, &s, sizeof(s), cudaMemcpyHostToDevice, stream));
+  if (cn_) CFGPP_CHECK_CUDA(cudaMemcpyAsync(cn_scale_cur_, &cn_scale_, sizeof(float), cudaMemcpyHostToDevice, stream));
   mark();
-  for (const auto& st : prologue_plan_) {
-    st.fn(stream);
-    mark();
-    out.push_back({st.name, st.kind, st.flops, 0.f});
-  }
-  run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, &cur_state_->in_scale, conv_in_w_, conv_in_b_, conv_in_out_, B_, H_, W_,
-              d_.block_out_channels[0], 2, stream);
-  mark();
-  out.push_back({"conv_in", 3, 2.0 * NB_ * H_ * W_ * 36.0 * d_.block_out_channels[0], 0.f});
-  for (auto* pl : {&body_plan_, &tail_plan_})
-    for (const auto& st : *pl) {
+  auto run = [&](const std::vector<PlanStep>& plan, const std::string& prefix) {
+    for (const auto& st : plan) {
       st.fn(stream);
       mark();
-      out.push_back({st.name, st.kind, st.flops, 0.f});
+      out.push_back({prefix + st.name, st.kind, st.flops, 0.f});
     }
+  };
+  const std::string cnp = "controlnet:";
+  run(prologue_plan_, "");
+  if (cn_) run(cn_->prologue_plan_, cnp);
+  const int C0 = d_.block_out_channels[0];
+  const double conv_in_flops = 2.0 * NB_ * H_ * W_ * 36.0 * C0;
+  run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, &cur_state_->in_scale, conv_in_w_, conv_in_b_, conv_in_out_, B_, H_, W_,
+              C0, 2, stream);
+  mark();
+  out.push_back({"conv_in", 3, conv_in_flops, 0.f});
+  if (cn_) {
+    run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, &cur_state_->in_scale, cn_->conv_in_w_, cn_->conv_in_b_,
+                cn_->conv_in_out_, B_, H_, W_, C0, 2, stream, cn_->cond_);
+    mark();
+    out.push_back({cnp + "conv_in(+cond)", 3, conv_in_flops, 0.f});
+    run(cn_->body_plan_, cnp);
+  }
+  for (auto* pl : {&body_plan_, &control_plan_, &up_plan_, &tail_plan_}) run(*pl, "");
   run_conv_out_step(final_norm_.p, conv_out_w_, conv_out_b_, B_, H_, W_, final_norm_.C, STEP_NONE, nullptr, nullptr,
                     nullptr, nullptr, fwd_eps_uc_, fwd_eps_c_, stream);
   mark();
@@ -862,6 +1024,7 @@ void Unet::set_schedule(int method, int state_dtype, const cfgpp_step_state* ste
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(step_table_, steps_host_.data(), sizeof(StepState) * nsteps, cudaMemcpyHostToDevice,
                                    stream));
   v_ready_ = false;
+  if (cn_) fill_control_table(stream);  // a per-entry scale table belongs to the schedule it was set for
 }
 
 void Unet::set_v_coefs(const float* ab, int nsteps, cudaStream_t stream) {
@@ -917,10 +1080,9 @@ void Unet::ensure_graph(cudaStream_t stream) {
   const int mode = method_ | (state_dtype_ == CFGPP_F16 ? 0x100 : 0);
   CFGPP_CHECK_CUDA(cudaStreamBeginCapture(capture_stream_, cudaStreamCaptureModeRelaxed));
   try {
-    run_select_step(step_table_, step_counter_, cur_state_, capture_stream_, v_table_, v_cur_);
-    run_plan(prologue_plan_, capture_stream_);
-    run_conv_in(z_state_, state_dtype_ == CFGPP_F16 ? 1 : 0, &cur_state_->in_scale, conv_in_w_, conv_in_b_,
-                conv_in_out_, B_, H_, W_, d_.block_out_channels[0], 2, capture_stream_);
+    run_select_step(step_table_, step_counter_, cur_state_, capture_stream_, v_table_, v_cur_,
+                    cn_ ? cn_scale_table_ : nullptr, cn_scale_cur_);
+    run_inputs(z_state_, state_dtype_ == CFGPP_F16 ? 1 : 0, capture_stream_);
     run_body(capture_stream_);
     run_conv_out_step(final_norm_.p, conv_out_w_, conv_out_b_, B_, H_, W_, final_norm_.C, mode, &cur_state_->coef,
                       z_state_, aux_state_, z0t_state_, nullptr, nullptr, capture_stream_, noise_slot_, lambda_slot_,
@@ -941,6 +1103,7 @@ void Unet::run_steps(int first_step, int nsteps, cudaStream_t stream) {
   CFGPP_REQUIRE(first_step >= 0 && first_step + nsteps <= nsteps_, "step range outside the schedule");
   CFGPP_REQUIRE(!v_pred_ || v_ready_, "a v-prediction model needs cfgpp_set_v_coefs for this schedule");
   require_fresh_prompt();
+  require_control_ready();
   ensure_graph(stream);
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(step_counter_, &first_step, sizeof(int), cudaMemcpyHostToDevice, stream));
   for (int i = 0; i < nsteps; ++i) CFGPP_CHECK_CUDA(cudaGraphLaunch(graph_exec_, stream));
@@ -960,6 +1123,107 @@ void Unet::apply_step(int step, const __half* eps_uc, const __half* eps_c, cudaS
   const int n = B_ * 4 * H_ * W_;
   run_step_only(eps_uc, eps_c, n, mode, &step_table_[step].coef, z_state_, aux_state_, z0t_state_, stream, noise_slot_,
                 lambda_slot_, 4 * H_ * W_);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// ControlNet
+// ------------------------------------------------------------------------------------------------------------
+void Unet::attach_controlnet(Unet* cn) {
+  CFGPP_REQUIRE(!is_cn_, "a ControlNet attaches to a UNet handle, not to another ControlNet");
+  if (cn) {
+    CFGPP_REQUIRE(cn->is_cn_, "the handle to attach is not a ControlNet handle (cfgpp_controlnet_create)");
+    CFGPP_REQUIRE(cn->finalized_, "call cfgpp_finalize_weights on the ControlNet first");
+    CFGPP_REQUIRE(cn->device_ == device_, "the ControlNet lives on another device");
+    CFGPP_REQUIRE(cn->owner_ == nullptr || cn->owner_ == this, "the ControlNet is attached to another UNet handle");
+    const cfgpp_model_desc& c = cn->d_;
+    auto same = [](bool ok, const char* field) {
+      CFGPP_REQUIRE(ok, std::string("ControlNet ") + field + " differs from the UNet's");
+    };
+    same(c.num_levels == d_.num_levels, "num_levels");
+    for (int i = 0; i < d_.num_levels; ++i) same(c.block_out_channels[i] == d_.block_out_channels[i], "block_out_channels");
+    same(c.layers_per_block == d_.layers_per_block, "layers_per_block");
+    same(c.cross_attention_dim == d_.cross_attention_dim, "cross_attention_dim");
+    same(c.addition_time_embed_dim == d_.addition_time_embed_dim, "addition_time_embed_dim");
+    if (has_aug_) {
+      same(c.projection_class_embeddings_input_dim == d_.projection_class_embeddings_input_dim,
+           "projection_class_embeddings_input_dim");
+      same(c.pooled_dim == d_.pooled_dim, "pooled_dim");
+    }
+  }
+  if (cn_ && cn_ != cn) cn_->owner_ = nullptr;
+  cn_ = cn;
+  if (cn) cn->owner_ = this;
+  // the plan changes shape: the next cfgpp_prepare builds it
+  prepared_ = false;
+  graph_valid_ = false;
+  nsteps_ = 0;
+  cn_image_ready_ = false;
+}
+
+void Unet::set_control_image(const void* image, int dtype, cudaStream_t stream) {
+  CFGPP_REQUIRE(cn_ != nullptr, "no ControlNet attached");
+  CFGPP_REQUIRE(prepared_, "call cfgpp_prepare first");
+  CFGPP_REQUIRE(image != nullptr && (dtype == CFGPP_F16 || dtype == CFGPP_F32), "control image: fp16 or fp32 tensor");
+  StreamKScope sk_scope(sk_.ws(), sk_.flags());
+  cn_->cond_embed(image, dtype == CFGPP_F16, B_, 8 * H_, 8 * W_, cn_->cond_, stream);
+  cn_image_ready_ = true;
+}
+
+void Unet::set_control_scale(float scale, cudaStream_t stream) {
+  CFGPP_REQUIRE(!is_cn_, "the conditioning scale is set on the UNet handle");
+  cn_scale_ = scale;
+  if (cn_ && prepared_) fill_control_table(stream);
+}
+
+void Unet::set_control_scales(const float* scales, int n, cudaStream_t stream) {
+  CFGPP_REQUIRE(cn_ != nullptr && prepared_, "attach a ControlNet and call cfgpp_prepare first");
+  CFGPP_REQUIRE(nsteps_ > 0 && scales != nullptr && n == nsteps_, "one conditioning scale per schedule entry");
+  // pageable source: staged before the call returns; the stream orders it after a replay still reading the table
+  CFGPP_CHECK_CUDA(cudaMemcpyAsync(cn_scale_table_, scales, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
+}
+
+void Unet::cond_embed(const void* image, int is_half, int B, int Hi, int Wi, __half* out, cudaStream_t stream) {
+  CFGPP_REQUIRE(is_cn_ && finalized_, "the conditioning embedding runs on a finalized ControlNet handle");
+  CFGPP_REQUIRE(image != nullptr && out != nullptr, "null argument");
+  const int n = cn_desc_.num_embedding_levels;
+  const int f = 1 << (n - 1);
+  CFGPP_REQUIRE(B >= 1 && B <= 8 && Hi >= f && Wi >= f && Hi % f == 0 && Wi % f == 0,
+                "control image: batch 1..8, height and width multiples of 8");
+  // every intermediate is NHWC with its channels zero-padded to the convolution's 64-wide K blocks; two ping-pong
+  // buffers sized for the largest, allocated for this call only (the embedding runs once per image, not per step)
+  const EmbedConv& in = embed_convs_.at("conv_in");
+  size_t need = static_cast<size_t>(B) * Hi * Wi * std::max(in.cin_p, in.cout_p);
+  for (int i = 0; i + 1 < n; ++i) {
+    const EmbedConv& s2 = embed_convs_.at("blocks." + std::to_string(2 * i + 1));
+    need = std::max(need, static_cast<size_t>(B) * (Hi >> i) * (Wi >> i) * s2.cin_p);
+    need = std::max(need, static_cast<size_t>(B) * (Hi >> (i + 1)) * (Wi >> (i + 1)) * s2.cout_p);
+  }
+  __half *a = nullptr, *b = nullptr;
+  CFGPP_CHECK_CUDA(cudaMallocAsync(&a, need * sizeof(__half), stream));
+  CFGPP_CHECK_CUDA(cudaMallocAsync(&b, need * sizeof(__half), stream));
+  try {
+    run_image_to_nhwc(image, is_half, a, B, cn_desc_.conditioning_channels, Hi, Wi, in.cin_p, stream);
+    int h = Hi, w = Wi;
+    auto conv = [&](const std::string& name, const __half* x, __half* y, int stride, bool silu) {
+      const EmbedConv& c = embed_convs_.at(name);
+      run_gemm_op(make_conv3x3_op(x, B, h, w, c.cin_p, c.w, c.cout_p, c.b, nullptr, 0, 1, y, 0, stride), stream);
+      h /= stride;
+      w /= stride;
+      if (silu) run_silu(y, static_cast<size_t>(B) * h * w * c.cout_p, stream);
+    };
+    conv("conv_in", a, b, 1, true);
+    for (int i = 0; i + 1 < n; ++i) {
+      conv("blocks." + std::to_string(2 * i), b, a, 1, true);
+      conv("blocks." + std::to_string(2 * i + 1), a, b, 2, true);
+    }
+    conv("conv_out", b, out, 1, false);
+  } catch (...) {
+    cudaFreeAsync(a, stream);
+    cudaFreeAsync(b, stream);
+    throw;
+  }
+  CFGPP_CHECK_CUDA(cudaFreeAsync(a, stream));
+  CFGPP_CHECK_CUDA(cudaFreeAsync(b, stream));
 }
 
 }  // namespace cfgpp

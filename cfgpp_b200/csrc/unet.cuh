@@ -25,7 +25,9 @@ struct PlanStep {
 
 class Unet {
  public:
-  Unet(const cfgpp_model_desc& d, int device);
+  // cn != null makes a ControlNet handle (diffusers ControlNetModel): the down / mid half of this class's plan on its
+  // own weights, plus the conditioning embedding and the zero convs, run through the UNet handle it is attached to
+  Unet(const cfgpp_model_desc& d, int device, const cfgpp_controlnet_desc* cn = nullptr);
   ~Unet();
 
   void load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
@@ -40,7 +42,9 @@ class Unet {
   void lora_clear(cudaStream_t stream);
   void lora_stats(int* n_adapters, int* n_targets, size_t* backup_bytes, size_t* bytes_moved) const;
   void prepare(int batch, int h_lat, int w_lat);
-  size_t workspace_bytes() const { return act_.bytes(); }
+  // the prepared plan's workspace, the attached ControlNet's included
+  size_t workspace_bytes() const { return act_.bytes() + (cn_ ? cn_->act_.bytes() : 0); }
+  bool is_controlnet() const { return is_cn_; }
   double forward_flops() const { return forward_flops_; }
   int launches_per_step() const { return launches_per_step_; }
   double prompt_flops() const { return prompt_flops_; }
@@ -60,6 +64,13 @@ class Unet {
   void set_v_coefs(const float* ab_host, int nsteps, cudaStream_t stream);
   void run_steps(int first_step, int nsteps, cudaStream_t stream);
   void get_state(int which, void* out, cudaStream_t stream);
+  // ---- ControlNet (see cfgpp_attach_controlnet) ----
+  void attach_controlnet(Unet* cn);  // UNet handles; null detaches
+  void set_control_image(const void* image, int dtype, cudaStream_t stream);
+  void set_control_scale(float scale, cudaStream_t stream);
+  void set_control_scales(const float* scales_host, int n, cudaStream_t stream);
+  // ControlNet handles: the conditioning embedding of image [B,3,Hi,Wi] -> out [B,Hi/8,Wi/8,C0] NHWC fp16
+  void cond_embed(const void* image, int is_half, int B, int Hi, int Wi, __half* out, cudaStream_t stream);
   void apply_step(int step, const __half* eps_uc, const __half* eps_c, cudaStream_t stream);
   // Eager un-fused forward with a CUDA-event pair around every plan entry (profiling aid for bench.py).
   struct ProfEntry {
@@ -129,6 +140,16 @@ class Unet {
   void add_step(const std::string& name, std::function<void(cudaStream_t)> fn, int launches = 1);
   void run_plan(const std::vector<PlanStep>& plan, cudaStream_t stream);
   void run_body(cudaStream_t stream);
+  // the structure walk of prepare() (both passes) for this handle alone; `shared_state` (ControlNet handles built for
+  // a UNet): the UNet's current-step word, whose timestep and input scale the ControlNet reads
+  void build(int batch, int h_lat, int w_lat, StepState* shared_state);
+  void build_control_plan();  // UNet handles with a ControlNet: the zero convs into the skip tensors and mid output
+  void account();             // FLOP / launch totals of the built plan (+ the attached ControlNet's)
+  std::vector<std::string> zero_conv_keys() const;  // ControlNet handles: one per entry of res_
+  // prologue(s) and conv_in(s) of one forward on input z
+  void run_inputs(const void* z, int z_is_half, cudaStream_t stream);
+  void require_control_ready() const;
+  void fill_control_table(cudaStream_t stream);  // every entry of the scale table = cn_scale_
   void ensure_graph(cudaStream_t stream);
 
   cfgpp_model_desc d_;
@@ -151,7 +172,9 @@ class Unet {
   bool sizing_ = false;  // prepare()'s first pass: records scratch sizes, allocates and pushes nothing
   std::vector<PlanStep>* cur_plan_ = nullptr;
   std::vector<PlanStep> prologue_plan_;  // timestep embedding -> temb for all resnets
-  std::vector<PlanStep> body_plan_;      // conv_in output .. last up block
+  std::vector<PlanStep> body_plan_;      // conv_in output .. mid block
+  std::vector<PlanStep> control_plan_;   // the attached ControlNet's zero convs, added into res_ in place
+  std::vector<PlanStep> up_plan_;        // up blocks
   std::vector<PlanStep> tail_plan_;      // conv_norm_out + SiLU
   std::vector<PlanStep> prompt_plan_;    // cross-attention K/V projections + add-embedding
   double forward_flops_ = 0.0, prompt_flops_ = 0.0;
@@ -194,6 +217,25 @@ class Unet {
   Act final_norm_{nullptr, 0};
   __half* conv_in_out_ = nullptr;
   __half *conv_in_w_ = nullptr, *conv_in_b_ = nullptr, *conv_out_w_ = nullptr, *conv_out_b_ = nullptr;
+
+  // ControlNet
+  bool is_cn_ = false;
+  cfgpp_controlnet_desc cn_desc_{};
+  Unet* cn_ = nullptr;     // UNet handles: the attached ControlNet
+  Unet* owner_ = nullptr;  // ControlNet handles: the UNet it is attached to
+  std::vector<Act> res_;   // the down path's skip tensors, then the mid-block output (recorded by build)
+  std::vector<int> res_hw_;
+  __half* cond_ = nullptr;  // ControlNet handles: the conditioning embedding [B,H,W,C0] of the prepared shape
+  struct EmbedConv {
+    __half *w, *b;  // [Cout_p][9][Cin_p], [Cout_p], zero-padded
+    int cout_p, cin_p;
+  };
+  std::map<std::string, EmbedConv> embed_convs_;
+  float* cn_scale_table_ = nullptr;  // UNet handles with a ControlNet: device [1024], one scale per schedule entry
+  float* cn_scale_cur_ = nullptr;    // device word the zero convs read
+  float cn_scale_ = 1.0f;
+  std::vector<float> cn_fill_;       // host staging of fill_control_table
+  bool cn_image_ready_ = false;
 
   cudaGraph_t graph_ = nullptr;
   cudaGraphExec_t graph_exec_ = nullptr;

@@ -34,6 +34,8 @@ class NativeUNet(nv.NativeHandle):
         self._bound = None  # strong references to the tensors of the bound prompt (see bind_prompt)
         self._loras = {}  # name -> [adapter id, scale]
         self._lora_per_key = {}  # weight key -> adapters targeting it
+        self.controlnet = None  # the attached NativeControlNet (its plan is part of ours)
+        self._control_image = None  # the control image embedded for the prepared shape
 
     def _create(self, desc, idx: int) -> None:
         nv.check(self.lib.cfgpp_create_ex(byref(desc), c_size_t(ctypes.sizeof(desc)), c_int(idx), byref(self._h)))
@@ -45,6 +47,7 @@ class NativeUNet(nv.NativeHandle):
         # a failing native prepare() leaves the handle unprepared: forget the old shape and the bound prompt first so
         # that the next call re-plans instead of running on freed buffers
         self.batch, self.latent_hw, self._nsteps, self._bound = 0, (0, 0), 0, None
+        self._control_image = None
         with torch.cuda.device(self.device):
             nv.check(self.lib.cfgpp_prepare(self._h, c_int(batch), c_int(h_lat), c_int(w_lat)))
         self.batch, self.latent_hw = batch, (h_lat, w_lat)
@@ -143,8 +146,9 @@ class NativeUNet(nv.NativeHandle):
 
     # ---- fused trajectory ------------------------------------------------------------------------------------
     def set_schedule(self, method: int, state_dtype: torch.dtype, steps: Sequence[StepStateC],
-                     guidance: Optional[Sequence[float]] = None):
-        """`guidance`: per-image guidance scales (set_guidance); None leaves the steps' scalar lambda in charge."""
+                     guidance: Optional[Sequence[float]] = None, control_scales: Optional[Sequence[float]] = None):
+        """`guidance`: per-image guidance scales (set_guidance); None leaves the steps' scalar lambda in charge.
+        `control_scales`: one ControlNet conditioning scale per entry (set_control_scales); None leaves the scalar."""
         arr = to_c_array(list(steps))
         code = F16 if state_dtype == torch.float16 else F32
         with torch.cuda.device(self.device):
@@ -158,6 +162,8 @@ class NativeUNet(nv.NativeHandle):
         self._nsteps = len(steps)
         self._state_dtype = state_dtype
         self.set_guidance(guidance)
+        if control_scales is not None:
+            self.set_control_scales(control_scales)
 
     def set_guidance(self, guidance: Optional[Sequence[float]] = None):
         """One guidance scale per image of the prepared batch, rounded to fp32, used by every following step (fused
@@ -199,10 +205,12 @@ class NativeUNet(nv.NativeHandle):
                                                nv.ptr(eps_c.contiguous()), nv.stream_ptr()))
 
     def run_trajectory(self, method: int, state_dtype: torch.dtype, steps: Sequence[StepStateC], z: torch.Tensor,
-                       guidance: Optional[Sequence[float]] = None, noise: Optional[torch.Tensor] = None):
+                       guidance: Optional[Sequence[float]] = None, noise: Optional[torch.Tensor] = None,
+                       control_scales: Optional[Sequence[float]] = None):
         """A whole trajectory from state `z` on the prepared, prompt-bound handle: NFE replays of the step graph with no
-        host synchronisation in between. `noise`: the ancestral samplers' table (set_noise). Returns (z0t, zt)."""
-        self.set_schedule(method, state_dtype, steps, guidance)
+        host synchronisation in between. `noise`: the ancestral samplers' table (set_noise); `control_scales`: the
+        attached ControlNet's scale per entry. Returns (z0t, zt)."""
+        self.set_schedule(method, state_dtype, steps, guidance, control_scales)
         self.set_state(z)
         if noise is not None:
             self.set_noise(noise)
@@ -220,6 +228,67 @@ class NativeUNet(nv.NativeHandle):
             eps_uc, eps_c = v_to_eps(eps_uc, z.half(), a, b), v_to_eps(eps_c, z.half(), a, b)
         self.apply_step(i, eps_uc, eps_c)
         return self.get_state(1), self.get_state(0)
+
+    def close(self):
+        if getattr(self, "controlnet", None) is not None:  # the native handle detaches itself; keep both sides in step
+            self.controlnet.attached_to = None
+            self.controlnet = None
+        super().close()
+
+    def bind_control(self, request, zt: torch.Tensor, uc, c, pooled=None, time_ids=None, force: bool = False):
+        """Attach (or, with request None, detach) the request's ControlNet, prepare for zt's shape, bind the prompt and
+        embed the control image: the engine set-up of one controlled or uncontrolled call. Engines are shared between
+        solvers, so an uncontrolled call detaches whatever an earlier call left attached."""
+        b, _, h, w = zt.shape
+        self.attach_controlnet(None if request is None else request.engine)
+        self.prepare(b, h, w)
+        self.bind_prompt(uc, c, pooled, time_ids, force=force)
+        if request is not None:
+            self.set_control_image(request.image)
+
+    # ---- ControlNet ----------------------------------------------------------------------------------------------
+    def attach_controlnet(self, cn) -> None:
+        """Attach a NativeControlNet (None detaches). A change drops the plan: the next prepare() builds the plan with
+        (or without) the ControlNet, so attaching the one already attached costs nothing."""
+        if cn is self.controlnet:
+            return
+        if cn is not None and cn.attached_to is not None:
+            cn.attached_to.attach_controlnet(None)
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_attach_controlnet(self._h, cn._h if cn is not None else None))
+        if self.controlnet is not None:
+            self.controlnet.attached_to = None
+        self.controlnet = cn
+        if cn is not None:
+            cn.attached_to = self
+        self.batch, self.latent_hw, self._nsteps, self._bound, self._control_image = 0, (0, 0), 0, None, None
+
+    def set_control_image(self, image: torch.Tensor, force: bool = False) -> None:
+        """(batch, 3, 8h, 8w) RGB in [0, 1] for the prepared shape; its conditioning embedding runs once, here. The
+        same tensor object (same in-place version) is not embedded again unless `force`."""
+        h, w = self.latent_hw
+        assert tuple(image.shape) == (self.batch, 3, 8 * h, 8 * w), "control image shape"
+        key = (image, image._version)
+        if not force and self._control_image is not None and self._control_image[0] is image \
+                and self._control_image[1] == key[1]:
+            return
+        img = image.to(self.device).contiguous()
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_set_control_image(self._h, nv.ptr(img), c_int(nv.dtype_code(img)),
+                                                      nv.stream_ptr()))
+        self._control_image = key
+
+    def set_control_scale(self, scale: float) -> None:
+        """The conditioning scale of predict_noise and of every step; clears a per-entry table."""
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_set_control_scale(self._h, c_float(float(scale)), nv.stream_ptr()))
+
+    def set_control_scales(self, scales: Sequence[float]) -> None:
+        """One conditioning scale per entry of the current schedule (controlnet.control_scales), read on the device:
+        changing it never recaptures the step graph. set_schedule clears it."""
+        arr = (c_float * len(scales))(*[float(s) for s in scales])
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_set_control_scales(self._h, arr, c_int(len(scales)), nv.stream_ptr()))
 
     # ---- LoRA adapters ----------------------------------------------------------------------------------------
     MAX_LORAS_PER_WEIGHT = 4

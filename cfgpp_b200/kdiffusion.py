@@ -95,7 +95,14 @@ def _fused_trajectory(solver, x, steps, cond, cfg_guidance, noise_slots: int = 0
     x = x.to(solver.unet.device, torch.float16)
     noise = torch.stack([torch.randn_like(x) for _ in range(noise_slots)]) if noise_slots else None
     return solver.unet.run_trajectory(S.STEP_DPMPP2M_CFGPP, torch.float16, steps, x, guidance_table(cfg_guidance),
-                                      noise)
+                                      noise, solver._control_entries(steps))
+
+
+def _control_step(solver, i: int, n: int) -> None:
+    """The ControlNet scale of step i of n before its UNet call(s) (solvers without one have no hook)."""
+    hook = getattr(solver, "_control_step", None)
+    if hook is not None:
+        hook(i, n)
 
 
 def _fusable(solver, callback_fn) -> bool:
@@ -129,6 +136,7 @@ def euler_cfgpp_loop(solver: KDiffusionMixin, x, sigmas, cfg_guidance, cond, cal
     for i in range(len(sigmas) - 1):
         sigma = sigmas[i]
         t = solver.timestep(sigma).to(solver.device)
+        _control_step(solver, i, len(sigmas) - 1)
         denoised, uncond_denoised = solver._k_denoise(x, sigma, t, cfg_guidance, cond)
         d = solver.to_d(x, sigma, uncond_denoised if cfgpp else denoised)
         if ancestral:
@@ -159,6 +167,7 @@ def dpmpp_2s_a_cfgpp_loop(solver: KDiffusionMixin, x, sigmas, cfg_guidance, cond
     for i in range(len(sigmas) - 1):
         sigma = sigmas[i]
         new_t = solver.timestep(sigma).to(solver.device)
+        _control_step(solver, i, len(sigmas) - 1)  # both UNet calls of the step take its scale
         denoised, uncond_denoised = solver._k_denoise(x, sigma, new_t, cfg_guidance, cond)
         sigma_down, sigma_up = get_ancestral_step(sigmas[i], sigmas[i + 1])
         extrap = uncond_denoised if cfgpp else denoised
@@ -199,6 +208,7 @@ def dpmpp_2m_cfgpp_karras_loop(solver: KDiffusionMixin, x, sigmas, cfg_guidance,
     for i in range(len(sigmas) - 1):
         sigma = sigmas[i]
         new_t = solver.timestep(sigma).to(solver.device)
+        _control_step(solver, i, len(sigmas) - 1)
         denoised, uncond_denoised = solver._k_denoise(x, sigma, new_t, cfg_guidance, cond)
         t, t_next = t_fn(sigmas[i]), t_fn(sigmas[i + 1])
         h = t_next - t

@@ -31,7 +31,7 @@ from .conditioning import SyntheticTextEncoder
 from .text_encoder import CLIPTextConfig, get_conditioner
 from .config import UNetConfig, sd15_config
 from .latent_sdxl import get_engine
-from .solver_base import SolverBase, registry
+from .solver_base import SolverBase, refuse_control, registry
 
 __SOLVER__, register_solver, get_solver = registry()
 
@@ -102,9 +102,7 @@ class StableDiffusion(SolverBase):
         return uc, c, cfg_guidance, zT
 
     def _prepare(self, zt, uc, c, force: bool = False):
-        b, _, h, w = zt.shape
-        self.unet.prepare(b, h, w)
-        self.unet.bind_prompt(uc, c, force=force)
+        self.unet.bind_control(self._control, zt, uc, c, force=force)
 
     def model_output(self, zt: torch.Tensor, t: torch.Tensor, uc: torch.Tensor, c: torch.Tensor):
         """The UNet's raw (uncond, cond) output at input zt: eps, or v for a v-prediction model."""
@@ -127,12 +125,14 @@ class StableDiffusion(SolverBase):
         """(z0t, zt) of a DDIM-family trajectory. `cfg_guidance`: a per-image sequence goes to the step kernel's
         guidance table; a float (or None) leaves the steps' scalar in charge."""
         self._prepare(z_init, uc, c, force=True)  # every trajectory re-binds its prompt
-        eng, table = self.unet, guidance_table(cfg_guidance)
+        eng, table, scales = self.unet, guidance_table(cfg_guidance), self._control_entries(steps)
         if callback_fn is None:
-            return eng.run_trajectory(method, z_init.dtype, steps, z_init, table)
+            return eng.run_trajectory(method, z_init.dtype, steps, z_init, table, control_scales=scales)
         eng.set_schedule(method, z_init.dtype, steps, table)
         eng.set_state(z_init)
         for i, st in enumerate(steps):
+            if scales is not None:
+                eng.set_control_scale(scales[i])
             z0t, zt = eng.callback_step(i, st)
             kw = {'z0t': z0t.detach(), 'zt': zt.detach(), 'decode': self.decode}
             kw = callback_fn(i, torch.tensor(int(st.t), device=self.device), kw)
@@ -182,11 +182,14 @@ class BaseDDIM(StableDiffusion):
         return z0t
 
     def sample(self, cfg_guidance=7.5, prompt=["", ""], callback_fn=None, **kwargs):
-        """Batched: see StableDiffusion.batch_inputs. Returns (B, 3, H, W)."""
+        """Batched: see StableDiffusion.batch_inputs. Returns (B, 3, H, W). ControlNet: `controlnet=` (a
+        controlnet.ControlNet), `control_image=` (B or 1, 3, H, W) in [0, 1] at the output size,
+        `controlnet_conditioning_scale=`, `control_guidance_start=` / `control_guidance_end=` (diffusers' meaning)."""
         uc, c, cfg_guidance, zt = self.batch_inputs(prompt, cfg_guidance, kwargs.get('zT'))
         if zt is None:
             zt = self.initialize_latent(latent_dim=(uc.shape[0], 4, self.cfg.sample_size, self.cfg.sample_size))
-        return self.to_image(self.reverse_process(uc, c, cfg_guidance, zt, callback_fn))
+        return self.to_image(self._controlled(kwargs, uc.shape[0], zt.shape[2], zt.shape[3],
+                                              lambda: self.reverse_process(uc, c, cfg_guidance, zt, callback_fn)))
 
 
 @register_solver("ddim_inversion")
@@ -194,6 +197,7 @@ class InversionDDIM(BaseDDIM):
     """Reconstruction / editing after plain-CFG inversion (latent_diffusion.py:506-558)."""
 
     def sample(self, src_img, cfg_guidance=7.5, prompt=["", ""], callback_fn=None, **kwargs):
+        refuse_control(kwargs, "ddim_inversion")
         uc, c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[1])
         zt = self.initialize_latent(method='ddim', src_img=src_img, uc=uc, c=c, cfg_guidance=cfg_guidance)
         return self.to_image(self.reverse_process(uc, c, cfg_guidance, zt, callback_fn))
@@ -204,6 +208,7 @@ class EditWordSwapDDIM(InversionDDIM):
     """Editing via WordSwap after plain-CFG inversion (latent_diffusion.py:561-612)."""
 
     def sample(self, src_img, cfg_guidance=7.5, prompt=["", "", ""], callback_fn=None, **kwargs):
+        refuse_control(kwargs, "ddim_edit")
         uc, src_c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[1])
         _, tgt_c = self.get_text_embed(null_prompt=prompt[0], prompt=prompt[2])
         zt = self.initialize_latent(method='ddim', src_img=src_img, uc=uc, c=src_c, cfg_guidance=cfg_guidance)
@@ -257,7 +262,10 @@ class _KarrasCFGpp(StableDiffusion):
         """Batched: see StableDiffusion.batch_inputs. Ancestral methods draw each step's noise with `randn_like` over
         the whole batch, as the reference's loop would on a batched x: their images are not the serial runs' images."""
         uc, c, cfg_guidance, zt = self.batch_inputs(prompt, cfg_guidance, kwargs.get('zT'))
-        denoised, x = self.reverse_process(uc, c, cfg_guidance, kwargs.get('xT'), callback_fn, zt)
+        ref = kwargs.get('xT') if kwargs.get('xT') is not None else zt
+        h, w = (ref.shape[2], ref.shape[3]) if ref is not None else (self.cfg.sample_size,) * 2
+        denoised, x = self._controlled(kwargs, uc.shape[0], h, w, lambda: self.reverse_process(
+            uc, c, cfg_guidance, kwargs.get('xT'), callback_fn, zt))
         return self.to_image(x if self.decode_state else denoised)
 
 

@@ -36,7 +36,7 @@ from .text_encoder import CLIPTextConfig, ClipConditioner, get_conditioner
 from .config import UNetConfig, sdxl_config, sdxl_refiner_config
 from .engine import NativeUNet
 from .lora import LoraMixin, is_lora_file, read_lora
-from .solver_base import SolverBase, registry
+from .solver_base import SolverBase, refuse_control, registry
 from .weights import load_safetensors_state_dict, synthetic_state_dict
 
 __SOLVER__, register_solver, get_solver = registry()
@@ -112,13 +112,13 @@ def default_text_encoders(cfg: UNetConfig, device):
             get_conditioner("", device, "sdxl", cfg=small(f"clip_{d2}_proj", d2, cfg.pooled_dim, "gelu", 0)))
 
 
-def _prepare_engine(eng: NativeUNet, zt, uc, c, added_cond_kwargs, force: bool = False):
-    b, _, h, w = zt.shape
-    eng.prepare(b, h, w)
+def _prepare_engine(eng: NativeUNet, zt, uc, c, added_cond_kwargs, force: bool = False, control=None):
+    """Prepare `eng` for zt's shape and bind the prompt, with `control`'s ControlNet attached (None: detached)."""
     if eng.cfg.addition_embed_type == "text_time":
-        eng.bind_prompt(uc, c, added_cond_kwargs['text_embeds'], added_cond_kwargs['time_ids'], force=force)
+        eng.bind_control(control, zt, uc, c, added_cond_kwargs['text_embeds'], added_cond_kwargs['time_ids'],
+                         force=force)
     else:
-        eng.bind_prompt(uc, c, force=force)
+        eng.bind_control(control, zt, uc, c, force=force)
 
 
 REFINER_SOLVERS = ("ddim", "ddim_cfg++", "dpm++_2m_cfgpp")
@@ -206,7 +206,7 @@ class SDXL(SolverBase):
 
     # ---- the seam: batched (uncond + cond) UNet forward on the native backend -----------------------------------
     def _prepare(self, zt, uc, c, added_cond_kwargs, force: bool = False):
-        _prepare_engine(self.unet, zt, uc, c, added_cond_kwargs, force)
+        _prepare_engine(self.unet, zt, uc, c, added_cond_kwargs, force, self._control)
 
     def predict_noise(self, zt, t, uc, c, added_cond_kwargs, in_scale: float = 1.0):
         if uc is None or c is None:
@@ -268,7 +268,11 @@ class SDXL(SolverBase):
         `refiner`: an SDXLRefiner that runs the steps after `denoising_end` (a fraction of the schedule, see
         schedule.expert_split) in the same trajectory; the image is decoded once, after it. The refiner is conditioned
         as diffusers' refiner pipeline conditions it: `prompt1` through its text tower, time ids (original size, crop
-        top-left, `aesthetic_score`) and, for the uncond row, `negative_aesthetic_score`."""
+        top-left, `aesthetic_score`) and, for the uncond row, `negative_aesthetic_score`.
+
+        ControlNet: `controlnet=` (a controlnet.ControlNet), `control_image=` (B or 1, 3, H, W) in [0, 1] at the output
+        size, `controlnet_conditioning_scale=`, `control_guidance_start=` / `control_guidance_end=` (diffusers' meaning,
+        over the whole schedule); a refiner runs uncontrolled."""
         if refiner is not None:
             self._check_refiner()
         size = self.default_sample_size * self.vae_scale_factor
@@ -294,8 +298,11 @@ class SDXL(SolverBase):
                 refiner, p["prompt1[0]"], p["prompt1[1]"], cfg_guidance, original_size, crops_coords_top_left,
                 negative_original_size or original_size, negative_crops_coords_top_left, aesthetic_score,
                 negative_aesthetic_score, clip_skip, B))
-        return self.to_image(self.reverse_process(null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs,
-                                                  target_size, **kwargs))
+        zT = kwargs.get('zT')
+        lat = (zT.shape[2], zT.shape[3]) if zT is not None else (target_size[1] // self.vae_scale_factor,
+                                                                 target_size[0] // self.vae_scale_factor)
+        return self.to_image(self._controlled(kwargs, B, *lat, lambda: self.reverse_process(
+            null_prompt_embeds, prompt_embeds, cfg_guidance, add_cond_kwargs, target_size, **kwargs)))
 
     @torch.no_grad()
     def refiner_conditions(self, refiner: SDXLRefiner, null_prompt, prompt, cfg_guidance, original_size,
@@ -383,18 +390,18 @@ class SDXL(SolverBase):
         the base's state in the sampler's own parameterization; both engines are set up before the first step, so
         the hand-off is a device-to-device copy with no host synchronisation. The step index a callback sees runs
         0..n-1 across both."""
-        table = guidance_table(cfg_guidance)
+        table, scales = guidance_table(cfg_guidance), self._control_entries(steps)
         if hand_off is None and callback_fn is None:
-            _prepare_engine(self.unet, z_init, *cond, force=True)  # every trajectory re-binds its prompt
-            return self.unet.run_trajectory(method, state_dtype, steps, z_init, table)
-        experts = [(self.unet, cond)]
+            _prepare_engine(self.unet, z_init, *cond, force=True, control=self._control)  # re-binds its prompt
+            return self.unet.run_trajectory(method, state_dtype, steps, z_init, table, control_scales=scales)
+        experts = [(self.unet, cond, self._control, scales)]
         k = len(steps)
         if hand_off is not None:
             refiner, refiner_cond, k = hand_off
-            experts.append((refiner.unet, refiner_cond))
-        for e, e_cond in experts:
-            _prepare_engine(e, z_init, *e_cond, force=True)
-            e.set_schedule(method, state_dtype, steps, table)
+            experts.append((refiner.unet, refiner_cond, None, None))  # the refiner runs uncontrolled
+        for e, e_cond, e_control, e_scales in experts:
+            _prepare_engine(e, z_init, *e_cond, force=True, control=e_control)
+            e.set_schedule(method, state_dtype, steps, table, e_scales)
         eng = self.unet
         eng.set_state(z_init)
         if callback_fn is None:
@@ -407,6 +414,8 @@ class SDXL(SolverBase):
             if i == k:
                 eng, base = experts[1][0], eng
                 eng.set_state(base.get_state(0))
+            if scales is not None and i < k:
+                eng.set_control_scale(scales[i])
             z0t, zt = eng.callback_step(i, st)
             kw = {'z0t': z0t.detach(), 'zt': zt.detach(), 'decode': self.decode}
             kw = callback_fn(i, torch.tensor(int(st.t), device=self.device), kw)
@@ -590,6 +599,7 @@ class EditWardSwapDDIM(SDXL):
                negative_target_size: Optional[Tuple[int, int]] = None,
                clip_skip: Optional[int] = None,
                **kwargs):
+        refuse_control(kwargs, "ddim_edit")
         if kwargs.get('refiner') is not None:
             self._check_refiner()
         size = self.default_sample_size * self.vae_scale_factor

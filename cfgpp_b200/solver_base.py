@@ -39,8 +39,37 @@ class _Scheduler:
         self.final_alpha_cumprod = sch.final_alpha_cumprod
 
 
+CONTROL_KWARGS = ("controlnet", "control_image", "controlnet_conditioning_scale", "control_guidance_start",
+                  "control_guidance_end")
+
+
+def refuse_control(kwargs: dict, what: str) -> None:
+    """The inversion / editing solvers take no ControlNet."""
+    if kwargs.get("controlnet") is not None or kwargs.get("control_image") is not None:
+        raise ValueError(f"{what} does not take a ControlNet (text-to-image solvers only)")
+
+
 class SolverBase(K.KDiffusionMixin, LoraMixin):
     """The host class provides `vae`, `dtype` and `sample`."""
+    _control = None  # the ControlRequest of the running sample() call (controlnet.control_request), else None
+
+    def _controlled(self, kwargs: dict, batch: int, lat_h: int, lat_w: int, run):
+        """run() under the ControlNet that sample()'s keyword arguments ask for (none: the engine is detached)."""
+        from .controlnet import control_request
+        self._control = control_request(kwargs, batch, 8 * lat_h, 8 * lat_w, self.device)
+        try:
+            return run()
+        finally:
+            self._control = None
+
+    def _control_entries(self, steps):
+        """The conditioning scale of every entry of `steps`, or None when uncontrolled."""
+        return None if self._control is None else self._control.entry_scales(steps)
+
+    def _control_step(self, i: int, n: int) -> None:
+        """Sampler step i of n runs un-fused next: its UNet calls take that step's conditioning scale."""
+        if self._control is not None:
+            self.unet.set_control_scale(self._control.step_scale(i, n))
 
     def _init_schedule(self, num_sampling: int, kind: str, device):
         """Sampling parameters (latent_diffusion.py:69-80, latent_sdxl.py:56-67 / :407-418)."""

@@ -121,9 +121,15 @@ def synthetic_state_dict(cfg: UNetConfig, seed: int = 1234, device="cpu", dtype=
     """Seeded synthetic weights with activation-preserving scales (unit-gain matrices, attention logits of O(1),
     damped residual branches) so that every kernel sees realistic dynamic range. Values are generated in fp32 on
     `device` and stored as `dtype`; the fp16 values ARE the model (the fp32 oracle upcasts the same fp16 numbers)."""
+    return synthetic_from_specs(unet_param_specs(cfg), seed, device, dtype)
+
+
+def synthetic_from_specs(specs: List[Spec], seed: int = 1234, device="cpu",
+                         dtype=torch.float16) -> Dict[str, torch.Tensor]:
+    """The seeded weights of synthetic_state_dict for any list of (key, shape, kind) specs, drawn in list order."""
     g = torch.Generator(device=device).manual_seed(seed)
     sd: Dict[str, torch.Tensor] = {}
-    for key, shape, kind in unet_param_specs(cfg):
+    for key, shape, kind in specs:
         if kind == "norm_w":
             t = 1.0 + 0.1 * torch.randn(shape, generator=g, device=device)
         elif kind in ("norm_b", "b"):

@@ -68,7 +68,17 @@ def main():
     parser.add_argument("--lora", action="append", default=[], metavar="PATH[:SCALE]",
                         help="a UNet LoRA *.safetensors (diffusers / peft or kohya naming) merged at SCALE (default 1.0); "
                              "repeatable, up to 4 adapters per weight")
+    parser.add_argument("--controlnet", type=str, default=None, metavar="DIR",
+                        help="a diffusers ControlNetModel directory (config.json + diffusion_pytorch_model"
+                             "[.fp16].safetensors), or a name for seeded synthetic weights")
+    parser.add_argument("--control_image", type=Path, default=None,
+                        help="the control map (canny, depth, ...) as an image file at exactly the output size")
+    parser.add_argument("--controlnet_scale", type=float, default=1.0)
+    parser.add_argument("--control_guidance_start", type=float, default=0.0)
+    parser.add_argument("--control_guidance_end", type=float, default=1.0)
     args = parser.parse_args()
+    if (args.controlnet is None) != (args.control_image is None):
+        raise SystemExit("--controlnet and --control_image go together")
     if args.denoising_end is not None and args.model != "sdxl":
         raise SystemExit("--denoising_end needs --model sdxl")
 
@@ -87,6 +97,14 @@ def main():
     if height % 8 or width % 8:
         raise SystemExit(f"--height / --width must be multiples of 8 (got {height} x {width})")
     zT = draw_latents((1, 4, height // 8, width // 8))  # N(0, 1) start latent from the seeded CPU generator
+    control = {}
+    if args.controlnet is not None:
+        from cfgpp_b200.controlnet import ControlNet
+        control = {"controlnet": ControlNet(args.controlnet, args.device, base_cfg=solver.cfg),
+                   "control_image": load_control_image(args.control_image, height, width),
+                   "controlnet_conditioning_scale": args.controlnet_scale,
+                   "control_guidance_start": args.control_guidance_start,
+                   "control_guidance_end": args.control_guidance_end}
     if sdxl:
         refiner = {}
         if args.denoising_end is not None:
@@ -94,10 +112,10 @@ def main():
                        "denoising_end": args.denoising_end}
         result = solver.sample(prompt1=[args.null_prompt, args.prompt], prompt2=[args.null_prompt, args.prompt],
                                cfg_guidance=args.cfg_guidance, original_size=(height, width),
-                               target_size=(height, width), callback_fn=callback, zT=zT, **refiner)
+                               target_size=(height, width), callback_fn=callback, zT=zT, **refiner, **control)
     else:
         result = solver.sample(prompt=[args.null_prompt, args.prompt], cfg_guidance=args.cfg_guidance,
-                               callback_fn=callback, zT=zT)
+                               callback_fn=callback, zT=zT, **control)
 
     out = args.workdir.joinpath('result/generated.pt')
     torch.save(result, out)
@@ -107,6 +125,16 @@ def main():
     except Exception:  # torchvision is optional here
         pass
     print(f"saved {out}")
+
+
+def load_control_image(path: Path, height: int, width: int) -> torch.Tensor:
+    """(1, 3, H, W) RGB in [0, 1]. The image must already have the output size: it is not resized."""
+    import numpy as np
+    from PIL import Image
+    img = Image.open(path).convert("RGB")
+    if img.size != (width, height):
+        raise SystemExit(f"--control_image is {img.size[0]} x {img.size[1]}, the output is {width} x {height}")
+    return torch.from_numpy(np.asarray(img).copy()).permute(2, 0, 1)[None].float() / 255.0
 
 
 if __name__ == "__main__":

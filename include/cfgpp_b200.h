@@ -190,6 +190,52 @@ int cfgpp_get_state(cfgpp_handle* h, int which, void* out_dev, void* stream);
  * prediction_type (a v model's caller converts first, cfgpp_op_v_to_eps). */
 int cfgpp_apply_step(cfgpp_handle* h, int step, const void* eps_uc_dev, const void* eps_c_dev, void* stream);
 
+/* ---- ControlNet (diffusers ControlNetModel, guess_mode off): spatial conditioning of a UNet handle ---------------
+ * A ControlNet handle holds its own weights under the ControlNetModel keys (`conv_in.*`, `time_embedding.*`,
+ * `add_embedding.*`, `down_blocks.*`, `mid_block.*`, `controlnet_cond_embedding.*`, `controlnet_down_blocks.{k}.*`,
+ * `controlnet_mid_block.*`), loaded with cfgpp_load_weight / cfgpp_finalize_weights and destroyed with cfgpp_destroy.
+ * It is run through the UNet handle it is attached to. Per UNet call, on the full 2*batch rows:
+ *   sample  = fp16(fp16(conv_in(z * in_scale)) + cond),  cond = controlnet_cond_embedding(fp16(image)) (batch rows,
+ *             shared by both CFG halves), then the ControlNet's own time / add-embedding, down blocks and mid block
+ *             on the UNet's timestep, context and added conditions;
+ *   r_k     = fp16(zero_conv_k(res_k) + bias_k) for every down-path skip tensor k and the mid-block output;
+ *   skip_k' = fp16(float(skip_k) + float(fp16(float(r_k) * s))), the same for the UNet's mid-block output, with s the
+ *             conditioning scale of the step. The UNet's down path and mid block see the un-added tensors; only the up
+ *             path sees the sums. */
+typedef struct cfgpp_controlnet_desc {
+  cfgpp_model_desc model;       /* down / mid geometry of the ControlNet (up_* fields ignored; out_channels 4) */
+  int conditioning_channels;    /* 3 (RGB) */
+  int num_embedding_levels;     /* len(conditioning_embedding_out_channels): 4 (the embedding downsamples by 8) */
+  int embedding_channels[CFGPP_MAX_LEVELS]; /* (16, 32, 96, 256) */
+} cfgpp_controlnet_desc;
+int cfgpp_controlnet_create(const cfgpp_controlnet_desc* desc, int device, cfgpp_handle** out);
+/* On a ControlNet handle, every entry point that prepares, conditions, runs or schedules a UNet (cfgpp_prepare,
+ * cfgpp_set_prompt, cfgpp_unet_forward, cfgpp_profile_forward, cfgpp_set_schedule .. cfgpp_apply_step, cfgpp_lora_*,
+ * cfgpp_attach_controlnet's first argument, cfgpp_set_control_*) fails with an error status. cfgpp_workspace_bytes of a
+ * UNet handle counts the attached ControlNet's workspace too. */
+/* Attach a finalized ControlNet handle to a UNet handle (cn = NULL detaches). num_levels, block_out_channels,
+ * layers_per_block, cross_attention_dim and the add-embedding dims must equal the UNet's (the error names the first
+ * field that differs). Attaching or detaching drops the prepared plan: the next cfgpp_prepare builds one plan of
+ * ControlNet prologue, ControlNet down + mid, UNet down + mid, zero convs (in place into the UNet's skip tensors and
+ * mid output), UNet up path; cfgpp_run_steps, cfgpp_unet_forward and cfgpp_profile_forward all run it.
+ * cfgpp_set_prompt also projects the ControlNet's cross-attention K/V and its add-embedding. A ControlNet is attached
+ * to at most one UNet at a time and must outlive the attachment (destroying either end detaches). */
+int cfgpp_attach_controlnet(cfgpp_handle* h, cfgpp_handle* cn);
+/* image_dev: (batch, 3, 8*h_lat, 8*w_lat) NCHW RGB in [0, 1] of `dtype`, for the prepared shape. Runs the conditioning
+ * embedding once into the plan's buffer; cfgpp_run_steps / cfgpp_unet_forward of an attached handle fail until it has
+ * been called after the last cfgpp_prepare. */
+int cfgpp_set_control_image(cfgpp_handle* h, const void* image_dev, int dtype, void* stream);
+/* The conditioning scale s of cfgpp_unet_forward and of every step (1.0 after create); clears the per-entry table
+ * (enqueued on `stream`). */
+int cfgpp_set_control_scale(cfgpp_handle* h, float scale, void* stream);
+/* One scale per entry of the current schedule (host [nsteps], copied), read on the device by the step selection:
+ * changing it never recaptures the step graph. cfgpp_set_schedule and cfgpp_set_control_scale clear it. */
+int cfgpp_set_control_scales(cfgpp_handle* h, const float* scales_host, int nsteps, void* stream);
+/* The conditioning embedding on its own, on a ControlNet handle: image (batch, 3, height, width) as above ->
+ * out_dev (batch, height/8, width/8, C0) NHWC fp16. */
+int cfgpp_controlnet_embed(cfgpp_handle* cn, const void* image_dev, int dtype, int batch, int height, int width,
+                           void* out_dev, void* stream);
+
 /* ---- AutoencoderKL decoder (SURVEY.md section 8 f2): replaces `self.vae.decode(zt / scaling_factor).sample` of
  * latent_sdxl.py:155-164 (VAE madebyollin/sdxl-vae-fp16-fix, :44) and latent_diffusion.py:123-129 on the same conv /
  * GEMM / GroupNorm kernels. Weights under the diffusers AutoencoderKL keys (`post_quant_conv.*`, `decoder.*`). ----- */
@@ -295,6 +341,15 @@ int cfgpp_op_conv3x3_s2(const void* x, int B, int H, int W, int Cin, const void*
 int cfgpp_op_conv3x3_ex(const void* x, int B, int H, int W, int Cin, const void* w, int Cout, const void* bias,
                         const void* addend, int ld_add, int add_rows_per_group, void* out, int force_bn, int stride,
                         int pad, int force_im2col, void* stream);
+/* The ControlNet zero-conv epilogue: out [M,N] = fp16(float(addend) + float(fp16(float(fp16(a w^T + bias)) * s))),
+ * a [M,K], w [N,K], addend [M,N] fp16 (ld = N), s = *scale_dev (fp32, device). out may be addend (in place).
+ * scale_dev = NULL is the plain residual epilogue of cfgpp_op_linear. */
+int cfgpp_op_linear_scaled_residual(const void* a, const void* w, int M, int N, int K, const void* bias,
+                                    const void* addend, const float* scale_dev, void* out, int force_bn, void* stream);
+/* cfgpp_op_conv_in with an addend [B,H,W,Cout] NHWC fp16 shared by the `reps` repetitions:
+ * out = fp16(fp16(conv_in(z)) + addend). */
+int cfgpp_op_conv_in_add(const void* z, int z_dtype, const float* in_scale_dev, const void* w, const void* bias,
+                         const void* addend, void* out, int B, int H, int W, int Cout, int reps, void* stream);
 /* head h of q / k / v / out occupies columns [h*P, h*P + head_dim) with P = head_dim rounded up to a multiple of 64
  * (columns head_dim..P-1 must be zero in q / k / v and come back zero in out). */
 int cfgpp_op_attention(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out, int ldo, int B,
