@@ -361,32 +361,20 @@ def op_layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: 
 
 
 def op_cfgpp_step(eps_uc: torch.Tensor, eps_c: torch.Tensor, method: int, coef, z: torch.Tensor,
-                  aux: torch.Tensor | None = None, want_z0t: bool = True, noise: torch.Tensor | None = None):
+                  aux: torch.Tensor | None = None, want_z0t: bool = True, noise: torch.Tensor | None = None,
+                  lambdas: torch.Tensor | None = None):
     """In-place CFG++ update of z (fp32 or fp16 state) from given eps; returns z0t (or None). `noise`: fp16 table
-    [slots, *z.shape] of the ancestral samplers (slot = coef.c3)."""
-    from ctypes import byref
-    lib = load()
-    z0t = torch.empty_like(z) if want_z0t else None
-    code = 0 if z.dtype == torch.float16 else 1
-    check(lib.cfgpp_op_cfgpp_step(ptr(eps_uc), ptr(eps_c), c_int(z.numel()), c_int(method), c_int(code), byref(coef),
-                                  ptr(z), ptr(aux), ptr(z0t), ptr(noise), stream_ptr()))
-    return z0t
-
-
-def op_cfgpp_step_guided(eps_uc: torch.Tensor, eps_c: torch.Tensor, method: int, coef, z: torch.Tensor,
-                         lambdas: torch.Tensor | None, aux: torch.Tensor | None = None, want_z0t: bool = True,
-                         noise: torch.Tensor | None = None):
-    """op_cfgpp_step with a per-image guidance table: lambdas fp32 [z.shape[0]] on the device, row b of z mixing
-    with lambdas[b]; None falls back to coef.lambda_."""
+    [slots, *z.shape] of the ancestral samplers (slot = coef.c3). `lambdas`: a per-image guidance table, fp32
+    [z.shape[0]] on the device, row b of z mixing with lambdas[b]; None uses coef.lambda_."""
     from ctypes import byref
     lib = load()
     z0t = torch.empty_like(z) if want_z0t else None
     code = 0 if z.dtype == torch.float16 else 1
     if lambdas is not None:
         assert lambdas.dtype == torch.float32 and lambdas.shape == (z.shape[0],)
-    check(lib.cfgpp_op_cfgpp_step_guided(ptr(eps_uc), ptr(eps_c), c_int(z.numel()), c_int(method), c_int(code),
-                                         byref(coef), ptr(z), ptr(aux), ptr(z0t), ptr(noise), ptr(lambdas),
-                                         c_int(z.shape[0]), stream_ptr()))
+    check(lib.cfgpp_op_cfgpp_step(ptr(eps_uc), ptr(eps_c), c_int(z.numel()), c_int(method), c_int(code), byref(coef),
+                                  ptr(z), ptr(aux), ptr(z0t), ptr(noise), ptr(lambdas), c_int(z.shape[0]),
+                                  stream_ptr()))
     return z0t
 
 
@@ -465,10 +453,13 @@ def op_conv_in_add(z: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, addend:
 
 def op_conv_out_step(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, method: int = 0, coef=None,
                      z: torch.Tensor | None = None, aux: torch.Tensor | None = None, want_z0t: bool = True,
-                     noise: torch.Tensor | None = None, lambdas: torch.Tensor | None = None):
+                     noise: torch.Tensor | None = None, lambdas: torch.Tensor | None = None, v_ab=None,
+                     in_scale: torch.Tensor | None = None):
     """conv_out 3x3 (Cin -> 4) on x [2B,H,W,Cin] NHWC fp16, w [4, 9, Cin] (`w.permute(0, 2, 3, 1)`), fused with the
     step `method` on the state z [B,4,H,W] (in place). Returns (eps_uc, eps_c, z0t or None); method 0 (STEP_NONE) only
-    writes the eps. noise / lambdas as in op_cfgpp_step_guided."""
+    writes the eps. noise / lambdas as in op_cfgpp_step. `v_ab` = (a, b) of a v-prediction model: the conv outputs are
+    v (returned as they are) and become eps = fp16(fp32(a v) + fp32(b x_in)) before the step, x_in = z * in_scale
+    (fp32 [1] device scalar, or None) as conv_in forms the UNet input."""
     from ctypes import byref
     lib = load()
     B2, H, W, Cin = x.shape
@@ -484,35 +475,13 @@ def op_conv_out_step(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, metho
         code = dtype_code(z)
     if lambdas is not None:
         assert lambdas.dtype == torch.float32 and lambdas.shape == (B,)
+    assert in_scale is None or (in_scale.dtype == torch.float32 and in_scale.numel() == 1)
+    ab = (c_float * 2)(*v_ab) if v_ab is not None else None
     check(lib.cfgpp_op_conv_out_step(ptr(x), ptr(w), ptr(bias), c_int(B), c_int(H), c_int(W), c_int(Cin),
                                      c_int(method), c_int(code), byref(coef) if coef is not None else c_void_p(0),
                                      ptr(z), ptr(aux), ptr(z0t), ptr(eps_uc), ptr(eps_c), ptr(noise), ptr(lambdas),
-                                     stream_ptr()))
+                                     ab, ptr(in_scale), stream_ptr()))
     return eps_uc, eps_c, z0t
-
-
-def op_conv_out_step_v(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, method: int, coef, z: torch.Tensor,
-                       a: float, b: float, in_scale: torch.Tensor | None = None, aux: torch.Tensor | None = None,
-                       want_z0t: bool = True, noise: torch.Tensor | None = None, lambdas: torch.Tensor | None = None):
-    """op_conv_out_step for a v-prediction model: the conv outputs are v (returned as they are) and become
-    eps = fp16(fp32(a v) + fp32(b x_in)) before the step, x_in = z * in_scale (fp32 [1] device scalar, or None) as
-    conv_in forms the UNet input. Returns (v_uc, v_c, z0t or None)."""
-    from ctypes import byref
-    lib = load()
-    B2, H, W, Cin = x.shape
-    B = B2 // 2
-    assert B2 == 2 * B and w.shape == (4, 9, Cin) and method != 0 and z.shape == (B, 4, H, W)
-    assert in_scale is None or (in_scale.dtype == torch.float32 and in_scale.numel() == 1)
-    v_uc = torch.empty((B, 4, H, W), dtype=torch.float16, device=x.device)
-    v_c = torch.empty_like(v_uc)
-    z0t = torch.empty_like(z) if want_z0t else None
-    if lambdas is not None:
-        assert lambdas.dtype == torch.float32 and lambdas.shape == (B,)
-    check(lib.cfgpp_op_conv_out_step_v(ptr(x), ptr(w), ptr(bias), c_int(B), c_int(H), c_int(W), c_int(Cin),
-                                       c_int(method), c_int(dtype_code(z)), byref(coef), ptr(z), ptr(aux), ptr(z0t),
-                                       ptr(v_uc), ptr(v_c), ptr(noise), ptr(lambdas), ptr(in_scale), c_float(a),
-                                       c_float(b), stream_ptr()))
-    return v_uc, v_c, z0t
 
 
 def op_v_to_eps(v: torch.Tensor, z: torch.Tensor, a: float, b: float, in_scale: torch.Tensor | None = None):

@@ -1,6 +1,8 @@
 // cfgpp_b200 — C ABI, operator-level entry points (one call = one kernel launch on the caller's stream).
 // Declared in include/cfgpp_b200.h. No C++ exception crosses the boundary: every entry point returns an int
 // status (0 = OK) and records a message retrievable with cfgpp_last_error().
+#include <cstring>
+
 #include "capi_util.h"
 #include "attention.cuh"
 #include "executor.cuh"
@@ -192,54 +194,37 @@ CFGPP_API int cfgpp_op_layernorm(const void* x, int M, int C, const void* gamma,
 }  // extern "C"
 
 namespace {
-// Runs one step launch `launch(coef_dev, noise_slot, lambda_slot)` with the coefficients (zeros when coef_host is null)
-// and the two table words (noise, guidance) in a scratch device block, then synchronises and frees the block.
-// lambda_slot is null when there is no guidance table.
-// v_ab (may be null): the (a, b) pair of a v-prediction step, stored behind the table words; the launch receives its
-// device copy (null without it) as a fourth argument.
+// Runs one step launch `launch(args_dev)` on a scratch device copy of `args`, then synchronises and frees it.
+// in_scale_dev (may be null: 1.0, which leaves the model input exact): the entry's input scale, copied on the device.
 template <class Launch>
-void with_step_block(const cfgpp_step_coef* coef_host, const void* noise_dev, const float* lambda_dev,
-                     cudaStream_t stream, Launch&& launch, const float* v_ab = nullptr) {
-  static_assert(sizeof(cfgpp_step_coef) == sizeof(StepCoef), "ABI struct mismatch");
-  static_assert(sizeof(StepCoef) % sizeof(void*) == 0, "the table words are stored right behind the coefficients");
-  const StepCoef zero{};
-  const void* coef_src = coef_host ? static_cast<const void*>(coef_host) : static_cast<const void*>(&zero);
-  StepCoef* coef_dev = nullptr;
-  CFGPP_CHECK_CUDA(cudaMalloc(&coef_dev, sizeof(StepCoef) + 2 * sizeof(void*) + sizeof(float2)));
-  const __half** slot = reinterpret_cast<const __half**>(coef_dev + 1);
-  const float** lslot = reinterpret_cast<const float**>(slot + 1);
-  float2* vslot = reinterpret_cast<float2*>(lslot + 1);
-  cudaError_t e = cudaMemcpy(coef_dev, coef_src, sizeof(StepCoef), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(slot, &noise_dev, sizeof(void*), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(lslot, &lambda_dev, sizeof(void*), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && v_ab) e = cudaMemcpy(vslot, v_ab, sizeof(float2), cudaMemcpyHostToDevice);
+void with_step_block(const StepArgs& args, const float* in_scale_dev, cudaStream_t stream, Launch&& launch) {
+  StepArgs* dev = nullptr;
+  CFGPP_CHECK_CUDA(cudaMalloc(&dev, sizeof(StepArgs)));
+  cudaError_t e = cudaMemcpyAsync(dev, &args, sizeof(StepArgs), cudaMemcpyHostToDevice, stream);
+  if (e == cudaSuccess && in_scale_dev)
+    e = cudaMemcpyAsync(&dev->cur.s.in_scale, in_scale_dev, sizeof(float), cudaMemcpyDeviceToDevice, stream);
   if (e == cudaSuccess) {
     try {
-      launch(const_cast<const StepCoef*>(coef_dev), const_cast<const __half* const*>(slot),
-             lambda_dev ? const_cast<const float* const*>(lslot) : nullptr, v_ab ? vslot : nullptr);
+      launch(const_cast<const StepArgs*>(dev));
     } catch (...) {
-      cudaFree(coef_dev);
+      cudaFree(dev);
       throw;
     }
     e = cudaStreamSynchronize(stream);  // test-only entry point: scratch freed below
   }
-  cudaFree(coef_dev);
+  cudaFree(dev);
   CFGPP_CHECK_CUDA(e);
 }
 
-// One step-only launch from given eps.
-void op_step(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype, const cfgpp_step_coef* coef_host,
-             void* z, void* aux, void* z0t_out, const void* noise_dev, const float* lambda_dev, int batch,
-             cudaStream_t stream) {
-  const bool guided = lambda_dev != nullptr;
-  CFGPP_REQUIRE(!guided || (batch >= 1 && n % batch == 0), "guidance table: batch must divide n");
-  CFGPP_REQUIRE(coef_host != nullptr, "the step needs its coefficients");
-  with_step_block(coef_host, noise_dev, lambda_dev, stream,
-                  [&](const StepCoef* coef_dev, const __half* const* slot, const float* const* lslot, const float2*) {
-                    run_step_only((const __half*)eps_uc, (const __half*)eps_c, n,
-                                  method | (state_dtype == CFGPP_F16 ? 0x100 : 0), coef_dev, z, aux, z0t_out, stream,
-                                  slot, lslot, guided ? n / batch : 0);
-                  });
+// The record of one op-level step: coefficients (zeros when coef_host is null), in_scale 1, the two tables.
+StepArgs step_args(const cfgpp_step_coef* coef_host, const void* noise_dev, const float* lambda_dev) {
+  static_assert(sizeof(cfgpp_step_coef) == sizeof(StepCoef), "ABI struct mismatch");
+  StepArgs a{};
+  if (coef_host) std::memcpy(&a.cur.s.coef, coef_host, sizeof(StepCoef));
+  a.cur.s.in_scale = 1.0f;
+  a.noise = static_cast<const __half*>(noise_dev);
+  a.lambda = lambda_dev;
+  return a;
 }
 }  // namespace
 
@@ -247,19 +232,15 @@ extern "C" {
 
 CFGPP_API int cfgpp_op_cfgpp_step(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype,
                                   const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
-                                  const void* noise_dev, void* stream) {
+                                  const void* noise_dev, const float* lambda_dev, int batch, void* stream) {
   return guarded([&] {
-    op_step(eps_uc, eps_c, n, method, state_dtype, coef_host, z, aux, z0t_out, noise_dev, nullptr, 0,
-            (cudaStream_t)stream);
-  });
-}
-
-CFGPP_API int cfgpp_op_cfgpp_step_guided(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype,
-                                         const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
-                                         const void* noise_dev, const float* lambda_dev, int batch, void* stream) {
-  return guarded([&] {
-    op_step(eps_uc, eps_c, n, method, state_dtype, coef_host, z, aux, z0t_out, noise_dev, lambda_dev, batch,
-            (cudaStream_t)stream);
+    CFGPP_REQUIRE(!lambda_dev || (batch >= 1 && n % batch == 0), "guidance table: batch must divide n");
+    CFGPP_REQUIRE(coef_host != nullptr, "the step needs its coefficients");
+    const cudaStream_t st = (cudaStream_t)stream;
+    with_step_block(step_args(coef_host, noise_dev, lambda_dev), nullptr, st, [&](const StepArgs* args) {
+      run_step_only((const __half*)eps_uc, (const __half*)eps_c, n, method | (state_dtype == CFGPP_F16 ? 0x100 : 0),
+                    args, z, aux, z0t_out, lambda_dev ? n / batch : n, st);
+    });
   });
 }
 
@@ -307,38 +288,20 @@ CFGPP_API int cfgpp_op_conv_in_add(const void* z, int z_dtype, const float* in_s
 CFGPP_API int cfgpp_op_conv_out_step(const void* x, const void* w, const void* bias, int B, int H, int W, int Cin,
                                      int method, int state_dtype, const cfgpp_step_coef* coef_host, void* z, void* aux,
                                      void* z0t_out, void* eps_uc, void* eps_c, const void* noise_dev,
-                                     const float* lambda_dev, void* stream) {
+                                     const float* lambda_dev, const float* v_ab_host, const float* in_scale_dev,
+                                     void* stream) {
   return guarded([&] {
     CFGPP_REQUIRE(method == CFGPP_STEP_NONE || coef_host != nullptr, "a step method needs its coefficients");
-    const cudaStream_t st = (cudaStream_t)stream;
-    with_step_block(coef_host, noise_dev, lambda_dev, st,
-                    [&](const StepCoef* coef_dev, const __half* const* slot, const float* const* lslot,
-                        const float2*) {
-                      run_conv_out_step((const __half*)x, (const __half*)w, (const __half*)bias, B, H, W, Cin,
-                                        method | (state_dtype == CFGPP_F16 ? 0x100 : 0), coef_dev, z, aux, z0t_out,
-                                        (__half*)eps_uc, (__half*)eps_c, st, slot, lslot);
-                    });
-  });
-}
-
-CFGPP_API int cfgpp_op_conv_out_step_v(const void* x, const void* w, const void* bias, int B, int H, int W, int Cin,
-                                       int method, int state_dtype, const cfgpp_step_coef* coef_host, void* z,
-                                       void* aux, void* z0t_out, void* eps_uc, void* eps_c, const void* noise_dev,
-                                       const float* lambda_dev, const float* in_scale_dev, float a, float b,
-                                       void* stream) {
-  return guarded([&] {
-    CFGPP_REQUIRE(method != CFGPP_STEP_NONE && coef_host != nullptr && z != nullptr,
+    CFGPP_REQUIRE(!v_ab_host || (method != CFGPP_STEP_NONE && z != nullptr),
                   "the v conversion belongs to a step: method, coefficients and state");
+    StepArgs a = step_args(coef_host, noise_dev, lambda_dev);
+    if (v_ab_host) a.cur.v_ab = make_float2(v_ab_host[0], v_ab_host[1]);
     const cudaStream_t st = (cudaStream_t)stream;
-    const float ab[2] = {a, b};
-    with_step_block(
-        coef_host, noise_dev, lambda_dev, st,
-        [&](const StepCoef* coef_dev, const __half* const* slot, const float* const* lslot, const float2* vab) {
-          run_conv_out_step((const __half*)x, (const __half*)w, (const __half*)bias, B, H, W, Cin,
-                            method | (state_dtype == CFGPP_F16 ? 0x100 : 0), coef_dev, z, aux, z0t_out,
-                            (__half*)eps_uc, (__half*)eps_c, st, slot, lslot, vab, in_scale_dev);
-        },
-        ab);
+    with_step_block(a, in_scale_dev, st, [&](const StepArgs* args) {
+      run_conv_out_step((const __half*)x, (const __half*)w, (const __half*)bias, B, H, W, Cin,
+                        method | (state_dtype == CFGPP_F16 ? 0x100 : 0), args, z, aux, z0t_out, (__half*)eps_uc,
+                        (__half*)eps_c, st, v_ab_host != nullptr);
+    });
   });
 }
 

@@ -104,15 +104,11 @@ __global__ void copy_rows_kernel(const __half* __restrict__ src, int src_rows, i
 // ------------------------------------------------------------------------------------------------------------
 // conv_in: 4 -> Cout, 3x3 pad 1, NCHW latent -> NHWC fp16. thread = (pixel, 8 output channels)
 // ------------------------------------------------------------------------------------------------------------
-__global__ void select_step_kernel(const StepState* __restrict__ table, int* counter, StepState* cur,
-                                   const float2* __restrict__ v_table, float2* v_cur, const float* __restrict__ s_table,
-                                   float* s_cur) {
+__global__ void select_step_kernel(const StepEntry* __restrict__ table, int* counter, StepArgs* args) {
   pdl_launch_dependents();
   pdl_wait();
   const int i = *counter;
-  *cur = table[i];
-  if (v_table) *v_cur = v_table[i];
-  if (s_table) *s_cur = s_table[i];
+  args->cur = table[i];
   *counter = i + 1;
 }
 
@@ -306,26 +302,20 @@ CFGPP_DEVICE void store_state(void* p, size_t i, bool is_half, float v) {
     reinterpret_cast<float*>(p)[i] = v;
 }
 
-CFGPP_DEVICE void apply_step_elem(int mode, int half_state, const StepCoef& k, float eu, float ec, void* z, void* aux,
-                                  void* z0t_out, const __half* const* noise_slot, const float* const* lambda_slot,
-                                  size_t sample_elems, size_t n, size_t i) {
+CFGPP_DEVICE void apply_step_elem(int mode, int half_state, const StepArgs* args, float eu, float ec, void* z,
+                                  void* aux, void* z0t_out, size_t sample_elems, size_t n, size_t i) {
+  const StepCoef& k = args->cur.s.coef;
+  const float* table = args->lambda;  // per-image guidance [batch]; null: the schedule's scalar
+  const float lambda = table ? table[i / sample_elems] : k.lambda;
   const bool hs = half_state != 0;
   const float zv = load_state(z, i, hs);
   const bool kd = mode == STEP_DPMPP2M_CFGPP;
   const float old_d = (kd && (k.second_order & (1 | 32))) ? load_state(aux, i, hs) : 0.f;
   float noise = 0.f;
-  if (kd && (k.second_order & 8) && noise_slot) {
-    // slot index travels in c3 (exact for any realistic step count); the base pointer lives in device memory so the
-    // captured graph survives a re-allocation of the noise table
-    const __half* base = *noise_slot;
+  if (kd && (k.second_order & 8)) {
+    // slot index travels in c3 (exact for any realistic step count)
+    const __half* base = args->noise;
     if (base) noise = __half2float(base[static_cast<size_t>(k.c3) * n + i]);
-  }
-  float lambda = k.lambda;
-  if (lambda_slot) {
-    // per-image guidance table [batch]: read through a device word like the noise table, so the captured graph
-    // survives setting and clearing it; a null table means the schedule's scalar
-    const float* table = *lambda_slot;
-    if (table) lambda = table[i / sample_elems];
   }
   float zn, z0, no;
   if (hs)
@@ -338,16 +328,14 @@ CFGPP_DEVICE void apply_step_elem(int mode, int half_state, const StepCoef& k, f
 }
 
 // conv_out (Cin -> 4, 3x3 pad 1) + fused step. One warp per latent pixel of image b, computing both CFG halves.
-// kVPred: the conv output is v; it is converted to eps (v_to_eps with (a, b) = *v_coef and the UNet input rebuilt from
-// the state z and *in_scale_ptr) before the step. eps_uc / eps_c receive the raw output (v) either way.
+// kVPred: the conv output is v; it is converted to eps (v_to_eps with (a, b) = args->cur.v_ab and the UNet input
+// rebuilt from the state z and args->cur.s.in_scale) before the step. eps_uc / eps_c receive the raw output (v) either
+// way.
 template <bool kVPred>
 __global__ void conv_out_step_kernel(const __half* __restrict__ x, const __half* __restrict__ w,
                                      const __half* __restrict__ bias, int B, int H, int W, int Cin, int mode,
-                                     int half_state, const StepCoef* __restrict__ coef, void* z, void* aux,
-                                     void* z0t_out, __half* __restrict__ eps_uc, __half* __restrict__ eps_c,
-                                     const __half* const* __restrict__ noise_slot,
-                                     const float* const* __restrict__ lambda_slot, const float2* __restrict__ v_coef,
-                                     const float* __restrict__ in_scale_ptr) {
+                                     int half_state, const StepArgs* __restrict__ args, void* z, void* aux,
+                                     void* z0t_out, __half* __restrict__ eps_uc, __half* __restrict__ eps_c) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ __half swh[];  // [4][9][Cin]
@@ -414,14 +402,14 @@ __global__ void conv_out_step_kernel(const __half* __restrict__ x, const __half*
     if (eps_uc) eps_uc[i] = __float2half_rn(eu);
     if (eps_c) eps_c[i] = __float2half_rn(ec);
     if constexpr (kVPred) {
-      const float2 ab = *v_coef;
-      const float x_in = model_input(z, i, half_state, in_scale_ptr != nullptr, in_scale_ptr ? *in_scale_ptr : 1.0f);
+      const float2 ab = args->cur.v_ab;
+      const float x_in = model_input(z, i, half_state, 1, args->cur.s.in_scale);
       eu = v_to_eps(eu, x_in, ab.x, ab.y);
       ec = v_to_eps(ec, x_in, ab.x, ab.y);
     }
     if (mode != STEP_NONE)
-      apply_step_elem(mode, half_state, *coef, eu, ec, z, aux, z0t_out, noise_slot, lambda_slot,
-                      static_cast<size_t>(4) * HW, static_cast<size_t>(B) * 4 * HW, i);
+      apply_step_elem(mode, half_state, args, eu, ec, z, aux, z0t_out, static_cast<size_t>(4) * HW,
+                      static_cast<size_t>(B) * 4 * HW, i);
   }
 }
 
@@ -437,15 +425,14 @@ __global__ void v_to_eps_kernel(const __half* __restrict__ v, const void* __rest
 }
 
 __global__ void step_only_kernel(const __half* __restrict__ eps_uc, const __half* __restrict__ eps_c, int n, int mode,
-                                 int half_state, const StepCoef* __restrict__ coef, void* z, void* aux, void* z0t_out,
-                                 const __half* const* __restrict__ noise_slot,
-                                 const float* const* __restrict__ lambda_slot, int sample_elems) {
+                                 int half_state, const StepArgs* __restrict__ args, void* z, void* aux, void* z0t_out,
+                                 int sample_elems) {
   pdl_launch_dependents();
   pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  apply_step_elem(mode, half_state, *coef, __half2float(eps_uc[i]), __half2float(eps_c[i]), z, aux, z0t_out, noise_slot,
-                  lambda_slot, sample_elems, n, i);
+  apply_step_elem(mode, half_state, args, __half2float(eps_uc[i]), __half2float(eps_c[i]), z, aux, z0t_out,
+                  sample_elems, n, i);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -491,9 +478,8 @@ void run_copy_rows(const __half* src, int src_rows, int cols, __half* dst, int l
   launch_pdl(copy_rows_kernel, dim3((total + 255) / 256), dim3(256), 0, stream, src, src_rows, cols, dst, ld_dst, col_off, R);
 }
 
-void run_select_step(const StepState* table, int* counter, StepState* cur, cudaStream_t stream, const float2* v_table,
-                     float2* v_cur, const float* s_table, float* s_cur) {
-  launch_pdl(select_step_kernel, dim3(1), dim3(1), 0, stream, table, counter, cur, v_table, v_cur, s_table, s_cur);
+void run_select_step(const StepEntry* table, int* counter, StepArgs* args, cudaStream_t stream) {
+  launch_pdl(select_step_kernel, dim3(1), dim3(1), 0, stream, table, counter, args);
 }
 
 void run_conv_in(const void* z, int z_is_half, const float* in_scale, const __half* w, const __half* bias,
@@ -575,9 +561,8 @@ void run_pack_conv3x3_padded(const __half* w, const __half* bias, __half* wp, __
 
 // The state dtype travels in bit 8 of `mode` (mode | 0x100 = fp16 sampler state).
 void run_conv_out_step(const __half* x, const __half* w, const __half* bias, int B, int H, int W, int Cin, int mode,
-                       const StepCoef* coef_dev, void* z, void* aux, void* z0t_out, __half* eps_uc, __half* eps_c,
-                       cudaStream_t stream, const __half* const* noise_slot, const float* const* lambda_slot,
-                       const float2* v_coef, const float* in_scale) {
+                       const StepArgs* args, void* z, void* aux, void* z0t_out, __half* eps_uc, __half* eps_c,
+                       cudaStream_t stream, bool v_pred) {
   CFGPP_REQUIRE(Cin % 8 == 0, "conv_out Cin must be a multiple of 8");
   const int half_state = (mode & 0x100) ? 1 : 0;
   const int m = mode & 0xff;
@@ -586,12 +571,12 @@ void run_conv_out_step(const __half* x, const __half* w, const __half* bias, int
   const int warps = 8;
   const int total = B * H * W;
   const dim3 grid((total + warps - 1) / warps), block(warps * 32);
-  if (v_coef != nullptr && m != STEP_NONE)
-    launch_pdl(conv_out_step_kernel<true>, grid, block, smem, stream, x, w, bias, B, H, W, Cin, m, half_state, coef_dev,
-               z, aux, z0t_out, eps_uc, eps_c, noise_slot, lambda_slot, v_coef, in_scale);
+  if (v_pred && m != STEP_NONE)
+    launch_pdl(conv_out_step_kernel<true>, grid, block, smem, stream, x, w, bias, B, H, W, Cin, m, half_state, args, z,
+               aux, z0t_out, eps_uc, eps_c);
   else
-    launch_pdl(conv_out_step_kernel<false>, grid, block, smem, stream, x, w, bias, B, H, W, Cin, m, half_state,
-               coef_dev, z, aux, z0t_out, eps_uc, eps_c, noise_slot, lambda_slot, nullptr, nullptr);
+    launch_pdl(conv_out_step_kernel<false>, grid, block, smem, stream, x, w, bias, B, H, W, Cin, m, half_state, args,
+               z, aux, z0t_out, eps_uc, eps_c);
 }
 
 void run_v_to_eps(const __half* v, const void* z, int z_is_half, const float* in_scale, float a, float b, __half* eps,
@@ -599,14 +584,13 @@ void run_v_to_eps(const __half* v, const void* z, int z_is_half, const float* in
   launch_pdl(v_to_eps_kernel, dim3((n + 255) / 256), dim3(256), 0, stream, v, z, z_is_half, in_scale, a, b, eps, n);
 }
 
-void run_step_only(const __half* eps_uc, const __half* eps_c, int n, int mode, const StepCoef* coef_dev, void* z,
-                   void* aux, void* z0t_out, cudaStream_t stream, const __half* const* noise_slot,
-                   const float* const* lambda_slot, int sample_elems) {
-  CFGPP_REQUIRE(!lambda_slot || (sample_elems > 0 && n % sample_elems == 0),
-                "a guidance table needs the per-image element count (a divisor of n)");
+void run_step_only(const __half* eps_uc, const __half* eps_c, int n, int mode, const StepArgs* args, void* z,
+                   void* aux, void* z0t_out, int sample_elems, cudaStream_t stream) {
+  CFGPP_REQUIRE(sample_elems > 0 && n % sample_elems == 0,
+                "the step needs the per-image element count (a divisor of n) for a guidance table");
   const int half_state = (mode & 0x100) ? 1 : 0;
-  launch_pdl(step_only_kernel, dim3((n + 255) / 256), dim3(256), 0, stream, eps_uc, eps_c, n, mode & 0xff, half_state, coef_dev, z, aux,
-                                                        z0t_out, noise_slot, lambda_slot, sample_elems);
+  launch_pdl(step_only_kernel, dim3((n + 255) / 256), dim3(256), 0, stream, eps_uc, eps_c, n, mode & 0xff, half_state,
+             args, z, aux, z0t_out, sample_elems);
 }
 
 void run_upsample2x(const __half* x, __half* out, int B, int H, int W, int C, cudaStream_t stream) {

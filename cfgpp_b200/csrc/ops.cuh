@@ -73,43 +73,51 @@ struct StepCoef {  // per-step scalars, computed on the host in fp32 exactly as 
                          // d1 = sigma_down / sigma_t, d2 = expm1(-h))
 };
 
-// One sampler step's device-resident scalars; a table of these lives in HBM and a 1-thread kernel selects the
-// current entry, so a single CUDA graph replays for every step without host involvement.
+// One sampler step's scalars, the layout of cfgpp_step_state.
 struct StepState {
   float t;         // timestep fed to the UNet
   float in_scale;  // c_in (1.0 for DDIM)
   StepCoef coef;
 };
-// v_table (may be null): a parallel table of v-prediction coefficients (a, b) per step, selected into *v_cur alongside
-// s_table (may be null): the ControlNet conditioning scale per step, selected into *s_cur alongside
-void run_select_step(const StepState* table, int* counter, StepState* cur, cudaStream_t stream,
-                     const float2* v_table = nullptr, float2* v_cur = nullptr, const float* s_table = nullptr,
-                     float* s_cur = nullptr);
+// One schedule entry: everything a step reads that changes from step to step. A table of these lives in HBM and a
+// 1-thread kernel copies the current entry into the StepArgs record, so a single CUDA graph replays for every step
+// without host involvement.
+struct StepEntry {
+  StepState s;
+  float2 v_ab;          // v-prediction (a, b) = (sqrt(abar), sqrt(1 - abar)); unused by epsilon models
+  float control_scale;  // ControlNet conditioning scale
+};
+// The one device record every step consumer reads (timestep embedding, conv_in, zero convs, the step kernels).
+// noise: base of the ancestral noise table [slots][B,4,H,W] fp16, or null. lambda: the per-image guidance table [B]
+// fp32, or null for the entry's scalar cur.s.coef.lambda. Both are read from the record, so a captured graph survives
+// re-allocating, setting and clearing the tables.
+struct StepArgs {
+  StepEntry cur;
+  const __half* noise;
+  const float* lambda;
+};
+// args->cur = table[*counter]; ++*counter
+void run_select_step(const StepEntry* table, int* counter, StepArgs* args, cudaStream_t stream);
 
 // conv_out 3x3 (Cin -> 4) on the GroupNorm+SiLU'ed NHWC input x [2B,H,W,Cin] fused with the CFG++ guidance mix and
-// the scheduler update. noise_slot (may be null): device word holding the base of the ancestral noise table
-// [slots][B,4,H,W] fp16. lambda_slot (may be null): device word holding the per-image guidance table [B] fp32 or null;
-// while it holds a table, image b mixes with table[b] instead of coef->lambda. z is the sampler state (NCHW, fp32 for
-// DDIM modes, fp16 for DPM++), updated in place.
-// v_coef (may be null; ignored for STEP_NONE): the model predicts v. Before the step, each conv output becomes
-// eps = fp16(a * v + b * x_in) with (a, b) = *v_coef = (sqrt(abar), sqrt(1 - abar)) and x_in the UNet input rebuilt from
-// z and *in_scale as conv_in forms it (in_scale may be null: 1). eps_uc / eps_c still receive the raw output v.
-// With a null v_coef the kernel is the epsilon-model instantiation, without any of this arithmetic.
+// the scheduler update of args->cur (args may be null for STEP_NONE). z is the sampler state (NCHW, fp32 for DDIM
+// modes, fp16 for DPM++), updated in place; image b of a guidance table mixes with args->lambda[b].
+// v_pred (ignored for STEP_NONE): the model predicts v. Before the step, each conv output becomes
+// eps = fp16(a * v + b * x_in) with (a, b) = args->cur.v_ab and x_in the UNet input rebuilt from z and
+// args->cur.s.in_scale as conv_in forms it. eps_uc / eps_c still receive the raw output v. Without v_pred the kernel is
+// the epsilon-model instantiation, without any of this arithmetic.
 void run_conv_out_step(const __half* x, const __half* w /*[4][9][Cin]*/, const __half* bias, int B, int H, int W,
-                       int Cin, int mode, const StepCoef* coef_dev, void* z, void* aux /*old_denoised*/,
-                       void* z0t_out, __half* eps_uc, __half* eps_c, cudaStream_t stream,
-                       const __half* const* noise_slot = nullptr, const float* const* lambda_slot = nullptr,
-                       const float2* v_coef = nullptr, const float* in_scale = nullptr);
+                       int Cin, int mode, const StepArgs* args, void* z, void* aux /*old_denoised*/, void* z0t_out,
+                       __half* eps_uc, __half* eps_c, cudaStream_t stream, bool v_pred = false);
 // eps[i] = fp16(a * v[i] + b * x_in[i]) (the conversion of run_conv_out_step) with x_in from z [n] of z's dtype and
 // *in_scale (may be null) as conv_in forms the UNet input.
 void run_v_to_eps(const __half* v, const void* z, int z_is_half, const float* in_scale, float a, float b, __half* eps,
                   int n, cudaStream_t stream);
 
-// standalone fused CFG++ update from given eps (used when a per-step callback needs the un-fused seam); with a
-// lambda_slot, element i belongs to image i / sample_elems (sample_elems = 4*H*W)
-void run_step_only(const __half* eps_uc, const __half* eps_c, int n, int mode, const StepCoef* coef_dev, void* z,
-                   void* aux, void* z0t_out, cudaStream_t stream, const __half* const* noise_slot = nullptr,
-                   const float* const* lambda_slot = nullptr, int sample_elems = 0);
+// standalone fused CFG++ update of args->cur from given eps (used when a per-step callback needs the un-fused seam);
+// element i belongs to image i / sample_elems (sample_elems = 4*H*W) for args->lambda
+void run_step_only(const __half* eps_uc, const __half* eps_c, int n, int mode, const StepArgs* args, void* z,
+                   void* aux, void* z0t_out, int sample_elems, cudaStream_t stream);
 
 void run_upsample2x(const __half* x, __half* out, int B, int H, int W, int C, cudaStream_t stream);
 

@@ -584,12 +584,8 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
   build(batch, h_lat, w_lat, nullptr);
   if (cn_) {
     // the ControlNet's ops are built under this handle's stream-K scope: they run on this handle's stream
-    cn_->build(batch, h_lat, w_lat, cur_state_);
+    cn_->build(batch, h_lat, w_lat, args_);
     cn_->account();
-    cn_scale_table_ = act_.alloc<float>(1024);
-    cn_scale_cur_ = act_.alloc<float>(1);
-    fill_control_table(nullptr);
-    CFGPP_CHECK_CUDA(cudaMemcpy(cn_scale_cur_, &cn_scale_, sizeof(float), cudaMemcpyHostToDevice));
     build_control_plan();
   }
   account();
@@ -597,10 +593,11 @@ void Unet::prepare(int batch, int h_lat, int w_lat) {
   prepared_ = true;
 }
 
-void Unet::build(int batch, int h_lat, int w_lat, StepState* shared_state) {
+void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
   // from here on the old plan is gone: a throw below must not leave the handle looking prepared
   prepared_ = false;
   nsteps_ = 0;
+  entries_.clear();
   v_ready_ = false;
   graph_valid_ = false;
   // drop the previous plan / workspace
@@ -662,23 +659,17 @@ void Unet::build(int batch, int h_lat, int w_lat, StepState* shared_state) {
         pooled_copy_ = alloc_act(static_cast<size_t>(NB_) * d_.pooled_dim);
         time_ids_copy_ = act_.alloc<float>(static_cast<size_t>(NB_) * n_time_ids_);
       }
-      cur_state_ = shared_state ? shared_state : act_.alloc<StepState>(1);
+      args_ = shared_args ? shared_args : act_.alloc<StepArgs>(1);
       if (!is_cn_) {  // the sampler state and tables: a ControlNet runs inside its UNet's step
         step_counter_ = act_.alloc<int>(1);
-        step_table_ = act_.alloc<StepState>(1024);
-        if (v_pred_) {
-          v_table_ = act_.alloc<float2>(1024);
-          v_cur_ = act_.alloc<float2>(1);
-        }
+        step_table_ = act_.alloc<StepEntry>(1024);
         const size_t lat = static_cast<size_t>(B_) * 4 * H_ * W_;
         z_state_ = act_.alloc<float>(lat);
         aux_state_ = act_.alloc<float>(lat);
         z0t_state_ = act_.alloc<float>(lat);
-        noise_slot_ = act_.alloc<const __half*>(1);
-        CFGPP_CHECK_CUDA(cudaMemcpy(noise_slot_, &noise_buf_, sizeof(__half*), cudaMemcpyHostToDevice));
         lambda_buf_ = act_.alloc<float>(B_);
-        lambda_slot_ = act_.alloc<const float*>(1);
-        CFGPP_CHECK_CUDA(cudaMemset(lambda_slot_, 0, sizeof(float*)));  // no table: the schedule's scalar lambda
+        const StepArgs a{{}, noise_buf_, nullptr};  // no guidance table: the schedule's scalar lambda
+        CFGPP_CHECK_CUDA(cudaMemcpy(args_, &a, sizeof(a), cudaMemcpyHostToDevice));
         fwd_eps_uc_ = alloc_act(lat);
         fwd_eps_c_ = alloc_act(lat);
       } else {
@@ -702,10 +693,10 @@ void Unet::build(int batch, int h_lat, int w_lat, StepState* shared_state) {
       const __half *w2 = weights_.plain("time_embedding.linear_2.weight"), *b2 = weights_.plain("time_embedding.linear_2.bias");
       __half *t_sin = t_sin_, *t_h1 = t_h1_, *emb = emb_, *semb = semb_, *temb_all = temb_all_;
       const __half* aug = has_aug_ ? aug_emb_ : nullptr;
-      const StepState* cur = cur_state_;
+      const StepArgs* args = args_;
       const __half *wa = temb_w_all_, *ba = temb_b_all_;
       const int ttot = temb_total_;
-      add_step("time_proj", [=](cudaStream_t st) { run_sincos_embed(&cur->t, 1, 1, C0, t_sin, C0, 0, st); });
+      add_step("time_proj", [=](cudaStream_t st) { run_sincos_embed(&args->cur.s.t, 1, 1, C0, t_sin, C0, 0, st); });
       add_step("time_embedding.linear_1+silu", [=](cudaStream_t st) {
         run_small_linear(t_sin, C0, w1, b1, nullptr, 0, t_h1, TE, nullptr, 1, TE, C0, true, st);
       });
@@ -815,7 +806,7 @@ void Unet::build(int batch, int h_lat, int w_lat, StepState* shared_state) {
       final_norm_ = Act{normp, C0};
     }
   }
-  if (is_cn_ && shared_state) prepared_ = true;  // built for its UNet: set_prompt may run
+  if (is_cn_ && shared_args) prepared_ = true;  // built for its UNet: set_prompt may run
 }
 
 void Unet::account() {
@@ -869,7 +860,7 @@ void Unet::build_control_plan() {
     const int M = NB_ * res_hw_[k];
     GemmOp op = make_linear_op(cn_->res_[k].p, C, nullptr, 0, 0, cn_->weights_.plain(keys[k] + ".weight", size_t(C) * C),
                                M, C, C, cn_->weights_.plain(keys[k] + ".bias", C), res_[k].p, C, 1, res_[k].p, C, false);
-    op.p.res_scale = cn_scale_cur_;
+    op.p.res_scale = &args_->cur.control_scale;
     add_gemm(keys[k], op);
   }
 }
@@ -892,20 +883,30 @@ void Unet::run_inputs(const void* z, int z_is_half, cudaStream_t stream) {
   run_plan(prologue_plan_, stream);
   if (cn_) run_plan(cn_->prologue_plan_, stream);
   const int C0 = d_.block_out_channels[0];
-  run_conv_in(z, z_is_half, &cur_state_->in_scale, conv_in_w_, conv_in_b_, conv_in_out_, B_, H_, W_, C0, 2, stream);
+  const float* in_scale = &args_->cur.s.in_scale;
+  run_conv_in(z, z_is_half, in_scale, conv_in_w_, conv_in_b_, conv_in_out_, B_, H_, W_, C0, 2, stream);
   if (cn_)
-    run_conv_in(z, z_is_half, &cur_state_->in_scale, cn_->conv_in_w_, cn_->conv_in_b_, cn_->conv_in_out_, B_, H_, W_,
-                C0, 2, stream, cn_->cond_);
+    run_conv_in(z, z_is_half, in_scale, cn_->conv_in_w_, cn_->conv_in_b_, cn_->conv_in_out_, B_, H_, W_, C0, 2, stream,
+                cn_->cond_);
 }
 
 void Unet::require_control_ready() const {
   CFGPP_REQUIRE(!cn_ || cn_image_ready_, "a ControlNet is attached: call cfgpp_set_control_image for the prepared shape");
 }
 
-void Unet::fill_control_table(cudaStream_t stream) {
-  cn_fill_.assign(1024, cn_scale_);
-  CFGPP_CHECK_CUDA(cudaMemcpyAsync(cn_scale_table_, cn_fill_.data(), 1024 * sizeof(float), cudaMemcpyHostToDevice,
+void Unet::upload_entries(cudaStream_t stream) {
+  // pageable source: staged before the call returns; the stream orders it after a replay still reading the table
+  CFGPP_CHECK_CUDA(cudaMemcpyAsync(step_table_, entries_.data(), sizeof(StepEntry) * nsteps_, cudaMemcpyHostToDevice,
                                    stream));
+}
+
+void Unet::stage_entry(float t, float in_scale, cudaStream_t stream) {
+  StepEntry e{};
+  e.s.t = t;
+  e.s.in_scale = in_scale;
+  e.control_scale = cn_scale_;
+  // cudaMemcpyAsync from pageable memory stages the 64 bytes before returning: `e` may go out of scope
+  CFGPP_CHECK_CUDA(cudaMemcpyAsync(&args_->cur, &e, sizeof(e), cudaMemcpyHostToDevice, stream));
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -943,12 +944,7 @@ void Unet::unet_forward(const void* z, int z_dtype, float t, float in_scale, __h
   CFGPP_REQUIRE(prepared_, "call cfgpp_prepare first");
   require_fresh_prompt();
   require_control_ready();
-  StepState s{};
-  s.t = t;
-  s.in_scale = in_scale;
-  // cudaMemcpyAsync from pageable memory stages the 48 bytes before returning: `s` may go out of scope
-  CFGPP_CHECK_CUDA(cudaMemcpyAsync(cur_state_, &s, sizeof(s), cudaMemcpyHostToDevice, stream));
-  if (cn_) CFGPP_CHECK_CUDA(cudaMemcpyAsync(cn_scale_cur_, &cn_scale_, sizeof(float), cudaMemcpyHostToDevice, stream));
+  stage_entry(t, in_scale, stream);
   run_inputs(z, z_dtype == CFGPP_F16 ? 1 : 0, stream);
   run_body(stream);
   run_conv_out_step(final_norm_.p, conv_out_w_, conv_out_b_, B_, H_, W_, final_norm_.C, STEP_NONE, nullptr, nullptr,
@@ -966,12 +962,8 @@ std::vector<Unet::ProfEntry> Unet::profile_forward(const void* z, int z_dtype, f
     CFGPP_CHECK_CUDA(cudaEventRecord(e, stream));
     evs.push_back(e);
   };
-  StepState s{};
-  s.t = t;
-  s.in_scale = in_scale;
   require_control_ready();
-  CFGPP_CHECK_CUDA(cudaMemcpyAsync(cur_state_, &s, sizeof(s), cudaMemcpyHostToDevice, stream));
-  if (cn_) CFGPP_CHECK_CUDA(cudaMemcpyAsync(cn_scale_cur_, &cn_scale_, sizeof(float), cudaMemcpyHostToDevice, stream));
+  stage_entry(t, in_scale, stream);
   mark();
   auto run = [&](const std::vector<PlanStep>& plan, const std::string& prefix) {
     for (const auto& st : plan) {
@@ -985,12 +977,12 @@ std::vector<Unet::ProfEntry> Unet::profile_forward(const void* z, int z_dtype, f
   if (cn_) run(cn_->prologue_plan_, cnp);
   const int C0 = d_.block_out_channels[0];
   const double conv_in_flops = 2.0 * NB_ * H_ * W_ * 36.0 * C0;
-  run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, &cur_state_->in_scale, conv_in_w_, conv_in_b_, conv_in_out_, B_, H_, W_,
-              C0, 2, stream);
+  run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, &args_->cur.s.in_scale, conv_in_w_, conv_in_b_, conv_in_out_, B_, H_,
+              W_, C0, 2, stream);
   mark();
   out.push_back({"conv_in", 3, conv_in_flops, 0.f});
   if (cn_) {
-    run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, &cur_state_->in_scale, cn_->conv_in_w_, cn_->conv_in_b_,
+    run_conv_in(z, z_dtype == CFGPP_F16 ? 1 : 0, &args_->cur.s.in_scale, cn_->conv_in_w_, cn_->conv_in_b_,
                 cn_->conv_in_out_, B_, H_, W_, C0, 2, stream, cn_->cond_);
     mark();
     out.push_back({cnp + "conv_in(+cond)", 3, conv_in_flops, 0.f});
@@ -1020,19 +1012,22 @@ void Unet::set_schedule(int method, int state_dtype, const cfgpp_step_state* ste
   method_ = method;
   state_dtype_ = state_dtype;
   nsteps_ = nsteps;
-  steps_host_.assign(steps, steps + nsteps);
-  CFGPP_CHECK_CUDA(cudaMemcpyAsync(step_table_, steps_host_.data(), sizeof(StepState) * nsteps, cudaMemcpyHostToDevice,
-                                   stream));
+  // v coefficients and per-entry conditioning scales belong to the schedule they were set for
+  entries_.assign(nsteps, StepEntry{});
+  for (int i = 0; i < nsteps; ++i) {
+    std::memcpy(&entries_[i].s, &steps[i], sizeof(StepState));
+    entries_[i].control_scale = cn_scale_;
+  }
   v_ready_ = false;
-  if (cn_) fill_control_table(stream);  // a per-entry scale table belongs to the schedule it was set for
+  upload_entries(stream);
 }
 
 void Unet::set_v_coefs(const float* ab, int nsteps, cudaStream_t stream) {
   CFGPP_REQUIRE(prepared_ && nsteps_ > 0, "call cfgpp_set_schedule first");
   CFGPP_REQUIRE(v_pred_, "v coefficients belong to a prediction_type = 1 model");
   CFGPP_REQUIRE(ab != nullptr && nsteps == nsteps_, "one (a, b) pair per schedule entry");
-  // pageable source: staged before the call returns
-  CFGPP_CHECK_CUDA(cudaMemcpyAsync(v_table_, ab, sizeof(float2) * nsteps, cudaMemcpyHostToDevice, stream));
+  for (int i = 0; i < nsteps; ++i) entries_[i].v_ab = make_float2(ab[2 * i], ab[2 * i + 1]);
+  upload_entries(stream);
   v_ready_ = true;
 }
 
@@ -1055,7 +1050,7 @@ void Unet::set_noise(const __half* noise, int slots, cudaStream_t stream) {
     noise_cap_ = 0;
     CFGPP_CHECK_CUDA(cudaMalloc(&noise_buf_, n * sizeof(__half)));
     noise_cap_ = n;
-    CFGPP_CHECK_CUDA(cudaMemcpyAsync(noise_slot_, &noise_buf_, sizeof(__half*), cudaMemcpyHostToDevice, stream));
+    CFGPP_CHECK_CUDA(cudaMemcpyAsync(&args_->noise, &noise_buf_, sizeof(__half*), cudaMemcpyHostToDevice, stream));
     CFGPP_CHECK_CUDA(cudaStreamSynchronize(stream));  // &noise_buf_ is host memory of this object: do not let it race
   }
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(noise_buf_, noise, n * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
@@ -1070,7 +1065,7 @@ void Unet::set_guidance(const float* lambda, int n, cudaStream_t stream) {
     CFGPP_CHECK_CUDA(cudaMemcpyAsync(lambda_buf_, lambda, static_cast<size_t>(n) * sizeof(float),
                                      cudaMemcpyHostToDevice, stream));
   const float* table = n > 0 ? lambda_buf_ : nullptr;
-  CFGPP_CHECK_CUDA(cudaMemcpyAsync(lambda_slot_, &table, sizeof(table), cudaMemcpyHostToDevice, stream));
+  CFGPP_CHECK_CUDA(cudaMemcpyAsync(&args_->lambda, &table, sizeof(table), cudaMemcpyHostToDevice, stream));
 }
 
 void Unet::ensure_graph(cudaStream_t stream) {
@@ -1080,13 +1075,11 @@ void Unet::ensure_graph(cudaStream_t stream) {
   const int mode = method_ | (state_dtype_ == CFGPP_F16 ? 0x100 : 0);
   CFGPP_CHECK_CUDA(cudaStreamBeginCapture(capture_stream_, cudaStreamCaptureModeRelaxed));
   try {
-    run_select_step(step_table_, step_counter_, cur_state_, capture_stream_, v_table_, v_cur_,
-                    cn_ ? cn_scale_table_ : nullptr, cn_scale_cur_);
+    run_select_step(step_table_, step_counter_, args_, capture_stream_);
     run_inputs(z_state_, state_dtype_ == CFGPP_F16 ? 1 : 0, capture_stream_);
     run_body(capture_stream_);
-    run_conv_out_step(final_norm_.p, conv_out_w_, conv_out_b_, B_, H_, W_, final_norm_.C, mode, &cur_state_->coef,
-                      z_state_, aux_state_, z0t_state_, nullptr, nullptr, capture_stream_, noise_slot_, lambda_slot_,
-                      v_cur_, &cur_state_->in_scale);
+    run_conv_out_step(final_norm_.p, conv_out_w_, conv_out_b_, B_, H_, W_, final_norm_.C, mode, args_, z_state_,
+                      aux_state_, z0t_state_, nullptr, nullptr, capture_stream_, v_pred_);
   } catch (...) {
     cudaGraph_t g = nullptr;
     cudaStreamEndCapture(capture_stream_, &g);
@@ -1121,8 +1114,9 @@ void Unet::apply_step(int step, const __half* eps_uc, const __half* eps_c, cudaS
   CFGPP_REQUIRE(prepared_ && step >= 0 && step < nsteps_, "step outside the schedule");
   const int mode = method_ | (state_dtype_ == CFGPP_F16 ? 0x100 : 0);
   const int n = B_ * 4 * H_ * W_;
-  run_step_only(eps_uc, eps_c, n, mode, &step_table_[step].coef, z_state_, aux_state_, z0t_state_, stream, noise_slot_,
-                lambda_slot_, 4 * H_ * W_);
+  CFGPP_CHECK_CUDA(cudaMemcpyAsync(&args_->cur, step_table_ + step, sizeof(StepEntry), cudaMemcpyDeviceToDevice,
+                                   stream));
+  run_step_only(eps_uc, eps_c, n, mode, args_, z_state_, aux_state_, z0t_state_, 4 * H_ * W_, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1172,14 +1166,15 @@ void Unet::set_control_image(const void* image, int dtype, cudaStream_t stream) 
 void Unet::set_control_scale(float scale, cudaStream_t stream) {
   CFGPP_REQUIRE(!is_cn_, "the conditioning scale is set on the UNet handle");
   cn_scale_ = scale;
-  if (cn_ && prepared_) fill_control_table(stream);
+  for (StepEntry& e : entries_) e.control_scale = scale;
+  if (cn_ && prepared_) upload_entries(stream);
 }
 
 void Unet::set_control_scales(const float* scales, int n, cudaStream_t stream) {
   CFGPP_REQUIRE(cn_ != nullptr && prepared_, "attach a ControlNet and call cfgpp_prepare first");
   CFGPP_REQUIRE(nsteps_ > 0 && scales != nullptr && n == nsteps_, "one conditioning scale per schedule entry");
-  // pageable source: staged before the call returns; the stream orders it after a replay still reading the table
-  CFGPP_CHECK_CUDA(cudaMemcpyAsync(cn_scale_table_, scales, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
+  for (int i = 0; i < n; ++i) entries_[i].control_scale = scales[i];
+  upload_entries(stream);
 }
 
 void Unet::cond_embed(const void* image, int is_half, int B, int Hi, int Wi, __half* out, cudaStream_t stream) {

@@ -140,16 +140,18 @@ class Unet {
   void add_step(const std::string& name, std::function<void(cudaStream_t)> fn, int launches = 1);
   void run_plan(const std::vector<PlanStep>& plan, cudaStream_t stream);
   void run_body(cudaStream_t stream);
-  // the structure walk of prepare() (both passes) for this handle alone; `shared_state` (ControlNet handles built for
-  // a UNet): the UNet's current-step word, whose timestep and input scale the ControlNet reads
-  void build(int batch, int h_lat, int w_lat, StepState* shared_state);
+  // the structure walk of prepare() (both passes) for this handle alone; `shared_args` (ControlNet handles built for
+  // a UNet): the UNet's step record, whose timestep and input scale the ControlNet reads
+  void build(int batch, int h_lat, int w_lat, StepArgs* shared_args);
   void build_control_plan();  // UNet handles with a ControlNet: the zero convs into the skip tensors and mid output
   void account();             // FLOP / launch totals of the built plan (+ the attached ControlNet's)
   std::vector<std::string> zero_conv_keys() const;  // ControlNet handles: one per entry of res_
   // prologue(s) and conv_in(s) of one forward on input z
   void run_inputs(const void* z, int z_is_half, cudaStream_t stream);
   void require_control_ready() const;
-  void fill_control_table(cudaStream_t stream);  // every entry of the scale table = cn_scale_
+  void upload_entries(cudaStream_t stream);  // entries_ -> step_table_
+  // the un-fused forward's current entry: timestep and input scale, no step, the scalar conditioning scale
+  void stage_entry(float t, float in_scale, cudaStream_t stream);
   void ensure_graph(cudaStream_t stream);
 
   cfgpp_model_desc d_;
@@ -196,22 +198,18 @@ class Unet {
   int n_time_ids_ = 0;  // (projection_class_embeddings_input_dim - pooled_dim) / addition_time_embed_dim
   __half *t_sin_ = nullptr, *t_h1_ = nullptr, *emb_ = nullptr, *semb_ = nullptr, *temb_all_ = nullptr;
   float* gn_partial_ = nullptr;
-  StepState* cur_state_ = nullptr;    // device
-  StepState* step_table_ = nullptr;   // device [nsteps]
+  StepArgs* args_ = nullptr;          // device; a ControlNet handle's is its UNet's
+  StepEntry* step_table_ = nullptr;   // device [1024]
   int* step_counter_ = nullptr;       // device
   int nsteps_ = 0, method_ = 0, state_dtype_ = CFGPP_F32;
+  std::vector<StepEntry> entries_;    // host mirror of the current schedule's nsteps_ entries
   bool v_pred_ = false;               // d_.prediction_type == 1
-  float2* v_table_ = nullptr;         // device [nsteps] (a, b), v-prediction handles only
-  float2* v_cur_ = nullptr;           // device, the current step's (a, b)
   bool v_ready_ = false;              // set_v_coefs matched the current schedule
-  std::vector<cfgpp_step_state> steps_host_;
   void* z_state_ = nullptr;   // (B,4,H,W) fp32-sized buffer (holds fp16 or fp32)
   void* aux_state_ = nullptr;
   void* z0t_state_ = nullptr;
-  const __half** noise_slot_ = nullptr;  // device word holding noise_buf_ (read by the step kernel: graph-stable)
   __half* noise_buf_ = nullptr;          // owned, survives prepare(); re-allocated when a larger table arrives
   size_t noise_cap_ = 0;                 // elements
-  const float** lambda_slot_ = nullptr;  // device word holding lambda_buf_ or null (read by the step kernel)
   float* lambda_buf_ = nullptr;          // [B] per-image guidance, workspace of the prepared plan
   __half *fwd_eps_uc_ = nullptr, *fwd_eps_c_ = nullptr;
   Act final_norm_{nullptr, 0};
@@ -231,10 +229,7 @@ class Unet {
     int cout_p, cin_p;
   };
   std::map<std::string, EmbedConv> embed_convs_;
-  float* cn_scale_table_ = nullptr;  // UNet handles with a ControlNet: device [1024], one scale per schedule entry
-  float* cn_scale_cur_ = nullptr;    // device word the zero convs read
   float cn_scale_ = 1.0f;
-  std::vector<float> cn_fill_;       // host staging of fill_control_table
   bool cn_image_ready_ = false;
 
   cudaGraph_t graph_ = nullptr;

@@ -358,15 +358,12 @@ int cfgpp_op_groupnorm(const void* x1, int C1, const void* x2, int C2, int B, in
                        const void* beta, float eps, int silu, void* out, void* stream);
 int cfgpp_op_layernorm(const void* x, int M, int C, const void* gamma, const void* beta, float eps, void* out,
                        void* stream);
-/* noise_dev (may be null): fp16 ancestral-noise table [slots][n]; the slot is coef_host->c3 (second_order bit 8). */
+/* noise_dev (may be null): fp16 ancestral-noise table [slots][n]; the slot is coef_host->c3 (second_order bit 8).
+ * lambda_dev (may be null): a per-image guidance table fp32 [batch] (device); element i of the n belongs to image
+ * i / (n / batch) and mixes with lambda_dev[image]. NULL uses coef_host->lambda_ (batch is then ignored). */
 int cfgpp_op_cfgpp_step(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype,
                         const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out, const void* noise_dev,
-                        void* stream);
-/* cfgpp_op_cfgpp_step with a per-image guidance table: lambda_dev fp32 [batch] (device), element i of the n belongs to
- * image i / (n / batch) and mixes with lambda_dev[image]; lambda_dev = NULL uses coef_host->lambda_. */
-int cfgpp_op_cfgpp_step_guided(const void* eps_uc, const void* eps_c, int n, int method, int state_dtype,
-                               const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
-                               const void* noise_dev, const float* lambda_dev, int batch, void* stream);
+                        const float* lambda_dev, int batch, void* stream);
 /* Sinusoidal embedding (diffusers get_timestep_embedding, flip_sin_to_cos): value i = vals_dev[i * val_stride] (fp32)
  * -> out[i * ld + col_off + (0 .. dim/2)] = cos, [.. + dim/2 .. dim) = sin, fp16; other columns are not written. */
 int cfgpp_op_timestep_embedding(const float* vals_dev, int val_stride, int n, int dim, void* out, int ld, int col_off,
@@ -386,18 +383,16 @@ int cfgpp_op_conv_in(const void* z, int z_dtype, const float* in_scale_dev, cons
 /* conv_out 3x3 pad 1, Cin -> 4 on x [2B,H,W,Cin] NHWC fp16 (rows [0, B) uncond, [B, 2B) cond), w [4][9][Cin] fp16,
  * fused with the step `method` (CFGPP_STEP_NONE: no update; coef_host may then be null) on the state z [B,4,H,W] of
  * state_dtype. eps_uc / eps_c (may be null): the conv outputs [B,4,H,W] fp16. noise_dev / lambda_dev as in
- * cfgpp_op_cfgpp_step_guided (lambda_dev has B entries). Synchronises the stream. */
+ * cfgpp_op_cfgpp_step (lambda_dev has B entries).
+ * v_ab_host (may be null: an epsilon model): (a, b) of a v-prediction model. The conv outputs (written to eps_uc / eps_c
+ * as they are) are then v and become eps = fp16(fp32(a v) + fp32(b x_in)) before the step, x_in = the UNet input
+ * z * (*in_scale_dev) formed as cfgpp_op_conv_in forms it (in_scale_dev may be NULL: no scaling); method must not be
+ * CFGPP_STEP_NONE. Synchronises the stream. */
 int cfgpp_op_conv_out_step(const void* x, const void* w, const void* bias, int B, int H, int W, int Cin, int method,
                            int state_dtype, const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
-                           void* eps_uc, void* eps_c, const void* noise_dev, const float* lambda_dev, void* stream);
-/* cfgpp_op_conv_out_step for a v-prediction model: the conv outputs (written to eps_uc / eps_c as they are) are v and
- * become eps = fp16(fp32(a v) + fp32(b x_in)) before the step, x_in = the UNet input z * (*in_scale_dev) formed as
- * cfgpp_op_conv_in forms it (in_scale_dev may be NULL: no scaling). method must not be CFGPP_STEP_NONE. */
-int cfgpp_op_conv_out_step_v(const void* x, const void* w, const void* bias, int B, int H, int W, int Cin, int method,
-                             int state_dtype, const cfgpp_step_coef* coef_host, void* z, void* aux, void* z0t_out,
-                             void* eps_uc, void* eps_c, const void* noise_dev, const float* lambda_dev,
-                             const float* in_scale_dev, float a, float b, void* stream);
-/* The conversion of cfgpp_op_conv_out_step_v alone: eps[i] = fp16(fp32(a v[i]) + fp32(b x_in[i])), v / eps [n] fp16,
+                           void* eps_uc, void* eps_c, const void* noise_dev, const float* lambda_dev,
+                           const float* v_ab_host, const float* in_scale_dev, void* stream);
+/* The v conversion of cfgpp_op_conv_out_step alone: eps[i] = fp16(fp32(a v[i]) + fp32(b x_in[i])), v / eps [n] fp16,
  * x_in from z [n] of z_dtype and in_scale_dev (may be NULL) as cfgpp_op_conv_in forms the UNet input. */
 int cfgpp_op_v_to_eps(const void* v, const void* z, int z_dtype, const float* in_scale_dev, float a, float b, void* eps,
                       int n, void* stream);

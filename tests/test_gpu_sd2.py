@@ -90,13 +90,13 @@ def test_conv_out_step_v_equals_convert_then_step(B, H, W):
         noise = torch.randn(max(slots, 1), B, 4, H, W, generator=g).half().to(dev) if slots else None
         for lam in (None, lams):
             z, aux = z0.clone(), (aux0.clone() if uses_aux else None)
-            v_uc, v_c, zt = nv.op_conv_out_step_v(x, w, b, method, coef, z, a, bb, in_scale=sdev, aux=aux, noise=noise,
-                                                  lambdas=lam)
+            v_uc, v_c, zt = nv.op_conv_out_step(x, w, b, method, coef, z, aux=aux, noise=noise, lambdas=lam,
+                                                v_ab=(a, bb), in_scale=sdev)
             assert torch.equal(v_uc, v_none) and torch.equal(v_c, vc_none), "the v launch must write the raw output"
             e_uc, e_c = nv.op_v_to_eps(v_uc, z0, a, bb, sdev), nv.op_v_to_eps(v_c, z0, a, bb, sdev)
             assert torch.equal(e_uc, _v_to_eps_ref(v_uc, z0, a, bb, scale))
             zs, auxs = z0.clone(), (aux0.clone() if uses_aux else None)
-            zts = nv.op_cfgpp_step_guided(e_uc, e_c, method, coef, zs, lam, aux=auxs, noise=noise)
+            zts = nv.op_cfgpp_step(e_uc, e_c, method, coef, zs, aux=auxs, noise=noise, lambdas=lam)
             tag = f"v step {B}x{H}x{W} variant {k} (method {method}, {dt}, bits {coef.second_order}, " \
                   f"{'table' if lam is not None else 'scalar'})"
             assert torch.equal(z, zs) and torch.equal(zt, zts), tag

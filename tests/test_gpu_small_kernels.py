@@ -289,7 +289,7 @@ def _conv_out_step_case(B, H, W, Cin, seed):
             e_uc, e_c, zt = nv.op_conv_out_step(x, wp, b, method, coef, z, aux=aux, noise=noise, lambdas=lam)
             assert torch.equal(e_uc, eu) and torch.equal(e_c, ec), "the eps of a fused launch differ from STEP_NONE's"
             zs, auxs = z0.clone(), (aux0.clone() if uses_aux else None)
-            zts = nv.op_cfgpp_step_guided(e_uc, e_c, method, coef, zs, lam, aux=auxs, noise=noise)
+            zts = nv.op_cfgpp_step(e_uc, e_c, method, coef, zs, aux=auxs, noise=noise, lambdas=lam)
             tag = f"conv_out_step {B}x{H}x{W} variant {k} (method {method}, {dt}, bits {coef.second_order}, " \
                   f"{'table' if lam is not None else 'scalar'})"
             assert torch.equal(z, zs) and torch.equal(zt, zts), tag

@@ -5,11 +5,14 @@ solver layer (latent_diffusion.py, latent_sdxl.py, kdiffusion.py, engine.py) com
     python tools/solver_outputs.py --compare OLD.pt NEW.pt     # every tensor torch.equal, same keys, same errors
 
 To compare against an earlier commit, export its package (`git archive <commit> cfgpp_b200 | tar -x -C old`) and run
-both trees on one native library (`CFGPP_B200_LIB=cfgpp_b200/lib/libcfgpp_b200.so`). Covered: both registries on
-the tiny SD v1.5 and SDXL configs, three SD solvers on the tiny v-prediction SD 2 config, and the SDXL solvers that take
-a refiner with a tiny refiner. Per solver: `sample()` (B = 2 prompts, per-image guidance [0.6, 1.0] where the solver
+both trees on one native library (`CFGPP_B200_LIB=cfgpp_b200/lib/libcfgpp_b200.so`), or each on its own build when
+the change is to the library. Covered: both registries on the tiny SD v1.5 and SDXL configs, three SD solvers on the
+tiny v-prediction SD 2 config, and the SDXL solvers that take a refiner with a tiny refiner. Per solver: `sample()` (B = 2 prompts, per-image guidance [0.6, 1.0] where the solver
 takes it; Lightning at 1.0), `reverse_process()` fused, `reverse_process()` under an identity callback with every
-(t, z0t, zt) it saw, and `inversion()`; every call after `torch.manual_seed(0)`. Needs a CUDA device."""
+(t, z0t, zt) it saw, and `inversion()`; every call after `torch.manual_seed(0)`. ControlNet: `sample()` with a
+synthetic ControlNet whose scale differs between schedule entries, fused and under the identity callback, for a
+deterministic and an ancestral SD v1.5 and SD 2 method and two SDXL methods (SDXL has no ancestral one). Needs a CUDA
+device."""
 from __future__ import annotations
 
 import argparse
@@ -20,6 +23,8 @@ import torch
 
 SD2_SOLVERS = ("ddim_cfg++", "ddim_inversion_cfg++", "dpm++_2s_a_cfg++")
 HW, B, LAM = 32, 2, [0.6, 1.0]
+# 5 steps from 0.2 to 0.8: the first and last entries run unconditioned, the others at 0.7
+CONTROL = dict(controlnet_conditioning_scale=0.7, control_guidance_start=0.2, control_guidance_end=0.8)
 
 
 class Recorder:
@@ -106,6 +111,29 @@ def sdxl_outputs(out: Outputs, dev):
             out.call(f"{key}/refiner_cb", ref)
 
 
+def controlnet_outputs(out: Outputs, dev):
+    from cfgpp_b200 import config as C, controlnet as CN, latent_diffusion as LD, latent_sdxl as LX
+    jobs = [(LD, C.tiny_sd15_config(), ("ddim_cfg++", "euler_a_cfg++")),
+            (LD, C.tiny_sd2_config(), ("ddim_cfg++", "dpm++_2s_a_cfg++")),
+            (LX, C.tiny_sdxl_config(), ("ddim_cfg++", "dpm++_2m_cfgpp"))]
+    for family, cfg, names in jobs:
+        cn = CN.ControlNet("synthetic-controlnet", dev, base_cfg=cfg)  # controlnet.synthetic_controlnet_state_dict
+        image = torch.rand(1, 3, 8 * HW, 8 * HW, generator=torch.Generator().manual_seed(3))
+        ctl = dict(controlnet=cn, control_image=image, **CONTROL)
+        p = ["", ["a cat", "a dog"]]
+        for name in names:
+            s = family.get_solver(name, solver_config=SimpleNamespace(num_sampling=5), device=dev, unet_config=cfg,
+                                  model_key="synthetic:14")
+            if family is LD:
+                run = lambda cb: s.sample(cfg_guidance=LAM, prompt=p, callback_fn=cb, **ctl)  # noqa: E731
+            else:
+                run = lambda cb: s.sample(p, p, cfg_guidance=LAM, callback_fn=cb, **ctl)  # noqa: E731
+            key = f"{cfg.name}/controlnet/{name}"
+            out.call(f"{key}/sample", lambda cb: run(None))
+            out.call(f"{key}/sample_cb", run)
+        cn.engine.close()
+
+
 def compare(a_path: str, b_path: str) -> int:
     a, b = torch.load(a_path), torch.load(b_path)
     bad = sorted(set(a) ^ set(b))
@@ -134,6 +162,7 @@ def main():
     with torch.no_grad():
         sd_outputs(out, dev)
         sdxl_outputs(out, dev)
+        controlnet_outputs(out, dev)
     torch.save(dict(out), args.out)
     print(f"{len(out) - ('errors' in out)} tensors -> {args.out}; errors: {out.get('errors', {})}")
 
