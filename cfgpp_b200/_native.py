@@ -339,6 +339,26 @@ def op_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, 
     return out
 
 
+def op_attention_ip(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k2: torch.Tensor, v2: torch.Tensor,
+                    scale: torch.Tensor, heads: int, head_dim: int = 64) -> torch.Tensor:
+    """Decoupled cross-attention: op_attention over (k, v) plus s times a softmax attention over the image tokens
+    k2 / v2 [B,Nkv2,H*P] (Nkv2 <= 64), summed in fp32 and rounded once; s = scale[0], an fp32 device tensor the kernel
+    reads (a view into a larger tensor is fine)."""
+    lib = load()
+    B, Nq, C = q.shape
+    Nkv, Nkv2 = k.shape[1], k2.shape[1]
+    out = torch.empty((B, Nq, C), dtype=torch.float16, device=q.device)
+    for t in (q, k, v, k2, v2):
+        assert t.is_cuda and t.stride(2) == 1 and t.stride(0) == t.shape[1] * t.stride(1)
+    assert scale.is_cuda and scale.dtype == torch.float32
+    check(lib.cfgpp_op_attention_ip(c_void_p(q.data_ptr()), c_int(q.stride(1)), c_void_p(k.data_ptr()),
+                                    c_int(k.stride(1)), c_void_p(v.data_ptr()), c_int(v.stride(1)),
+                                    c_void_p(k2.data_ptr()), c_int(k2.stride(1)), c_void_p(v2.data_ptr()),
+                                    c_int(v2.stride(1)), c_int(Nkv2), c_void_p(scale.data_ptr()), ptr(out), c_int(C),
+                                    c_int(B), c_int(heads), c_int(Nq), c_int(Nkv), c_int(head_dim), stream_ptr()))
+    return out
+
+
 def op_groupnorm(x1: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float, silu: bool,
                  x2: torch.Tensor | None = None) -> torch.Tensor:
     """x1 [B,HW,C1] (+ x2 [B,HW,C2]) NHWC fp16 -> GroupNorm(32) over the channel concat, optional SiLU."""

@@ -37,10 +37,12 @@ CFGPP_DEVICE uint32_t tile_off(int row, int chunk) {
   return (chunk >> 3) * ATOM_BYTES + row * 128 + (((chunk & 7) ^ (row & 7)) << 4);
 }
 
-template <int HD>
-__global__ void __launch_bounds__(kThreads)
-attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-            const __grid_constant__ CUtensorMap map_v) {
+// IP: the decoupled cross-attention of attn_ip_kernel. After the text tiles, one more ring fill brings the image
+// tokens' K / V (a 64-row tile of which the first p.Nkv2 rows are valid); their softmax has its own max and sum, and
+// the output is O1 / l1 + s * O2 / l2 rounded once. s = 0 skips the image tile: the plain kernel's arithmetic exactly.
+template <int HD, bool IP>
+CFGPP_DEVICE void attn_body(const AttnParams& p, const CUtensorMap* map_q, const CUtensorMap* map_k,
+                            const CUtensorMap* map_v, const CUtensorMap* map_k2, const CUtensorMap* map_v2) {
   using A = ACfg<HD>;
   constexpr int NA = A::NA;
   constexpr int TILE_BYTES = A::TILE_BYTES;
@@ -62,9 +64,9 @@ attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const
   const int n_tiles = (p.Nkv + BKV - 1) / BKV;
 
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&map_q);
-    tma_prefetch_desc(&map_k);
-    tma_prefetch_desc(&map_v);
+    tma_prefetch_desc(map_q);
+    tma_prefetch_desc(map_k);
+    tma_prefetch_desc(map_v);
     mbar_init(q_full, 1);
     mbar_init(&kv_full[0], 1);
     mbar_init(&kv_full[1], 1);
@@ -73,22 +75,33 @@ attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const
   __syncthreads();
   pdl_launch_dependents();
   pdl_wait();
+  const float ip_scale = IP ? *p.ip_scale : 0.f;
+  const bool ip = IP && ip_scale != 0.f;   // uniform over the CTA
+  const int n_fills = n_tiles + (ip ? 1 : 0);  // ring fills: the text tiles, then the image tile
 
   auto load_kv = [&](int j) {  // thread 0
     const int s = j & 1;
+    const bool image = IP && j == n_tiles;
+    const CUtensorMap* mk = image ? map_k2 : map_k;
+    const CUtensorMap* mv = image ? map_v2 : map_v;
+    const int row = image ? 0 : j * BKV;
     mbar_arrive_expect_tx(&kv_full[s], 2 * TILE_BYTES);
 #pragma unroll
     for (int a = 0; a < NA; ++a) {
-      tma_load_3d(sK + s * TILE_BYTES + a * ATOM_BYTES, &map_k, &kv_full[s], head * HD + a * 64, j * BKV, batch);
-      tma_load_3d(sV + s * TILE_BYTES + a * ATOM_BYTES, &map_v, &kv_full[s], head * HD + a * 64, j * BKV, batch);
+      tma_load_3d(sK + s * TILE_BYTES + a * ATOM_BYTES, mk, &kv_full[s], head * HD + a * 64, row, batch);
+      tma_load_3d(sV + s * TILE_BYTES + a * ATOM_BYTES, mv, &kv_full[s], head * HD + a * 64, row, batch);
     }
   };
   if (threadIdx.x == 0) {
+    if (IP) {
+      tma_prefetch_desc(map_k2);
+      tma_prefetch_desc(map_v2);
+    }
     mbar_arrive_expect_tx(q_full, TILE_BYTES);
 #pragma unroll
-    for (int a = 0; a < NA; ++a) tma_load_3d(sQ + a * ATOM_BYTES, &map_q, q_full, head * HD + a * 64, q0, batch);
+    for (int a = 0; a < NA; ++a) tma_load_3d(sQ + a * ATOM_BYTES, map_q, q_full, head * HD + a * 64, q0, batch);
     load_kv(0);
-    if (n_tiles > 1) load_kv(1);
+    if (n_fills > 1) load_kv(1);
   }
 
   const float c = p.scale_log2e;
@@ -99,15 +112,8 @@ attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   const uint32_t q_base = smem_u32(sQ);
   const int qrow_ld = warp * 16 + (lane & 15);  // ldmatrix row of this lane for the A operand (Q)
-  mbar_wait(q_full, 0);
-
-  for (int j = 0; j < n_tiles; ++j) {
-    const int s = j & 1;
-    mbar_wait(&kv_full[s], (j >> 1) & 1);
-    const uint32_t k_base = smem_u32(sK + s * TILE_BYTES);
-    const uint32_t v_base = smem_u32(sV + s * TILE_BYTES);
-    // ---- S = Q K^T: 16 rows x 64 kv columns per warp ----
-    float sc[BKV / 8][4];
+  // S = Q K^T of one KV tile: 16 rows x 64 kv columns per warp; columns >= valid are set to -inf
+  auto scores = [&](uint32_t k_base, int valid, float (&sc)[BKV / 8][4]) {
 #pragma unroll
     for (int n = 0; n < BKV / 8; ++n) sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
 #pragma unroll
@@ -123,8 +129,6 @@ attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const
         mma_16816(sc[2 * n2 + 1], a, b2, b3);
       }
     }
-    // ---- online softmax (rows lane / 4 and lane / 4 + 8; the four lanes of a quad share a row) ----
-    const int valid = p.Nkv - j * BKV;  // columns >= valid are padding (last tile only)
     if (valid < BKV) {
 #pragma unroll
       for (int n = 0; n < BKV / 8; ++n) {
@@ -133,6 +137,17 @@ attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const
         if (col + 1 >= valid) sc[n][1] = sc[n][3] = -INFINITY;
       }
     }
+  };
+  mbar_wait(q_full, 0);
+
+  for (int j = 0; j < n_tiles; ++j) {
+    const int s = j & 1;
+    mbar_wait(&kv_full[s], (j >> 1) & 1);
+    const uint32_t k_base = smem_u32(sK + s * TILE_BYTES);
+    const uint32_t v_base = smem_u32(sV + s * TILE_BYTES);
+    float sc[BKV / 8][4];
+    scores(k_base, p.Nkv - j * BKV, sc);  // columns past Nkv are padding (last tile only)
+    // ---- online softmax (rows lane / 4 and lane / 4 + 8; the four lanes of a quad share a row) ----
     float alpha[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -181,7 +196,7 @@ attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const
       }
     }
     __syncthreads();  // every warp is done with stage s
-    if (threadIdx.x == 0 && j + 2 < n_tiles) load_kv(j + 2);
+    if (threadIdx.x == 0 && j + 2 < n_fills) load_kv(j + 2);
   }
 
   float inv_l[2];
@@ -192,6 +207,66 @@ attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     inv_l[h] = 1.0f / l;
   }
+  if (ip) {
+    // ---- the image tile: one KV tile, so its max and sum are final before PV; a softmax of its own ----
+    const int s = n_tiles & 1;
+    mbar_wait(&kv_full[s], (n_tiles >> 1) & 1);
+    const uint32_t v_base = smem_u32(sV + s * TILE_BYTES);
+    float sc[BKV / 8][4];
+    scores(smem_u32(sK + s * TILE_BYTES), p.Nkv2, sc);
+    float mc[2], inv_l2[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int n = 0; n < BKV / 8; ++n) mx = fmaxf(mx, fmaxf(sc[n][2 * h], sc[n][2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      mc[h] = mx * c;  // finite: Nkv2 >= 1
+    }
+    float rs[2] = {0.f, 0.f};
+    uint32_t pa[BKV / 8][2];
+#pragma unroll
+    for (int n = 0; n < BKV / 8; ++n) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float p0 = fast_exp2(sc[n][2 * h] * c - mc[h]);
+        const float p1 = fast_exp2(sc[n][2 * h + 1] * c - mc[h]);
+        rs[h] += p0 + p1;
+        pa[n][h] = pack_half2(p0, p1);
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float l = rs[h];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      inv_l2[h] = 1.0f / l;
+    }
+    // O2 = P V2 two d tiles at a time, over the k steps that hold valid image tokens (P and V2 are zero past Nkv2),
+    // folded straight into o: o = O1 / l1 + s * O2 / l2
+    const int k_steps = (p.Nkv2 + 15) / 16;
+#pragma unroll
+    for (int d2 = 0; d2 < HD / 16; ++d2) {
+      float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+#pragma unroll
+      for (int t = 0; t < BKV / 16; ++t) {
+        if (t >= k_steps) break;
+        const uint32_t a[4] = {pa[2 * t][0], pa[2 * t][1], pa[2 * t + 1][0], pa[2 * t + 1][1]};
+        const int vrow = t * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
+        uint32_t b0, b1, b2, b3;
+        ldmatrix_x4_trans(v_base + tile_off(vrow, 2 * d2 + (lane >> 4)), b0, b1, b2, b3);
+        mma_16816(acc[0], a, b0, b1);
+        mma_16816(acc[1], a, b2, b3);
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          o[2 * d2 + i][e] = o[2 * d2 + i][e] * inv_l[e >> 1] + ip_scale * (acc[i][e] * inv_l2[e >> 1]);
+    }
+    inv_l[0] = inv_l[1] = 1.0f;  // o holds the output
+  }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int qrow = q0 + warp * 16 + (lane >> 2) + 8 * h;
@@ -201,6 +276,21 @@ attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const
     for (int n = 0; n < HD / 8; ++n)
       *reinterpret_cast<uint32_t*>(dst + n * 8) = pack_half2(o[n][2 * h] * inv_l[h], o[n][2 * h + 1] * inv_l[h]);
   }
+}
+
+template <int HD>
+__global__ void __launch_bounds__(kThreads)
+attn_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+            const __grid_constant__ CUtensorMap map_v) {
+  attn_body<HD, false>(p, &map_q, &map_k, &map_v, nullptr, nullptr);
+}
+
+template <int HD>
+__global__ void __launch_bounds__(kThreads)
+attn_ip_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+               const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_k2,
+               const __grid_constant__ CUtensorMap map_v2) {
+  attn_body<HD, true>(p, &map_q, &map_k, &map_v, &map_k2, &map_v2);
 }
 
 CUtensorMap make_head_map(const __half* base, int ld, int B, int N, int cols) {
@@ -214,12 +304,19 @@ template <int HD>
 void configure_one() {
   CFGPP_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         ACfg<HD>::SMEM_BYTES));
+  CFGPP_CHECK_CUDA(cudaFuncSetAttribute(attn_ip_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        ACfg<HD>::SMEM_BYTES));
 }
 
 template <int HD>
 void launch(const AttnOp& op, cudaStream_t stream) {
   dim3 grid((op.p.Nq + BQ - 1) / BQ, op.p.H, op.p.B);
-  launch_pdl(attn_kernel<HD>, grid, dim3(kThreads), ACfg<HD>::SMEM_BYTES, stream, op.p, op.map_q, op.map_k, op.map_v);
+  if (op.p.ip_scale)
+    launch_pdl(attn_ip_kernel<HD>, grid, dim3(kThreads), ACfg<HD>::SMEM_BYTES, stream, op.p, op.map_q, op.map_k,
+               op.map_v, op.map_k2, op.map_v2);
+  else
+    launch_pdl(attn_kernel<HD>, grid, dim3(kThreads), ACfg<HD>::SMEM_BYTES, stream, op.p, op.map_q, op.map_k,
+               op.map_v);
 }
 
 }  // namespace
@@ -240,6 +337,19 @@ AttnOp make_attn_op(const __half* q, int ldq, const __half* k, int ldk, const __
   op.map_q = make_head_map(q, ldq, B, Nq, H * hdp);
   op.map_k = make_head_map(k, ldk, B, Nkv, H * hdp);
   op.map_v = make_head_map(v, ldv, B, Nkv, H * hdp);
+  return op;
+}
+
+AttnOp make_attn_ip_op(const __half* q, int ldq, const __half* k, int ldk, const __half* v, int ldv, const __half* k2,
+                       int ldk2, const __half* v2, int ldv2, int Nkv2, const float* ip_scale, __half* out, int ldo,
+                       int B, int H, int Nq, int Nkv, int head_dim) {
+  CFGPP_REQUIRE(Nkv2 >= 1 && Nkv2 <= 64, "the image segment holds 1..64 tokens");
+  CFGPP_REQUIRE(ip_scale != nullptr, "the image segment needs its scale word");
+  AttnOp op = make_attn_op(q, ldq, k, ldk, v, ldv, out, ldo, B, H, Nq, Nkv, head_dim);
+  op.p.Nkv2 = Nkv2;
+  op.p.ip_scale = ip_scale;
+  op.map_k2 = make_head_map(k2, ldk2, B, Nkv2, H * op.hd_pad);
+  op.map_v2 = make_head_map(v2, ldv2, B, Nkv2, H * op.hd_pad);
   return op;
 }
 

@@ -190,6 +190,38 @@ CFGPP_API int cfgpp_set_control_scales(cfgpp_handle* h, const float* scales_host
   return guarded([&] { unet_of(h).set_control_scales(scales_host, nsteps, (cudaStream_t)stream); });
 }
 
+CFGPP_API int cfgpp_ip_adapter_load_weight(cfgpp_handle* h, const char* key, const void* data, const int64_t* shape,
+                                           int ndim, int dtype, void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(key && data && shape, "null argument");
+    unet_of(h).ip_load_weight(key, data, shape, ndim, dtype, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_ip_adapter_attach(cfgpp_handle* h, int n_tokens, int image_embed_dim) {
+  return guarded([&] {
+    CFGPP_REQUIRE(n_tokens >= 1, "an IP-Adapter has at least one image token (cfgpp_ip_adapter_clear detaches)");
+    unet_of(h).ip_attach(n_tokens, image_embed_dim);
+  });
+}
+
+CFGPP_API int cfgpp_ip_adapter_clear(cfgpp_handle* h) {
+  return guarded([&] { unet_of(h).ip_attach(0, 0); });
+}
+
+CFGPP_API int cfgpp_set_ip_image_embeds(cfgpp_handle* h, const void* embeds_dev, void* stream) {
+  return guarded([&] { unet_of(h).set_ip_image_embeds((const __half*)embeds_dev, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_set_ip_adapter_scale(cfgpp_handle* h, float scale, void* stream) {
+  return guarded([&] { unet_of(h).set_ip_scale(scale, (cudaStream_t)stream); });
+}
+
+// Debug aid (not in the public header): how many step graphs the handle has captured.
+CFGPP_API int cfgpp_dbg_graph_captures(cfgpp_handle* h, int* n) {
+  return guarded([&] { *n = unet_of(h).graph_captures(); });
+}
+
 CFGPP_API int cfgpp_controlnet_embed(cfgpp_handle* cn, const void* image, int dtype, int batch, int height, int width,
                                      void* out, void* stream) {
   return guarded([&] {

@@ -166,6 +166,18 @@ CFGPP_API int cfgpp_op_attention(const void* q, int ldq, const void* k, int ldk,
   });
 }
 
+CFGPP_API int cfgpp_op_attention_ip(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv,
+                                    const void* k2, int ldk2, const void* v2, int ldv2, int Nkv2,
+                                    const float* ip_scale_dev, void* out, int ldo, int B, int H, int Nq, int Nkv,
+                                    int head_dim, void* stream) {
+  return guarded([&] {
+    AttnOp op = make_attn_ip_op((const __half*)q, ldq, (const __half*)k, ldk, (const __half*)v, ldv, (const __half*)k2,
+                                ldk2, (const __half*)v2, ldv2, Nkv2, ip_scale_dev, (__half*)out, ldo, B, H, Nq, Nkv,
+                                head_dim);
+    run_attn_op(op, (cudaStream_t)stream);
+  });
+}
+
 CFGPP_API int cfgpp_op_groupnorm(const void* x1, int C1, const void* x2, int C2, int B, int HW, const void* gamma,
                                  const void* beta, float eps, int silu, void* out, void* stream) {
   return guarded([&] {

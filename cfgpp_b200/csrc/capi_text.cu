@@ -47,6 +47,46 @@ CFGPP_API int cfgpp_clip_stats(cfgpp_clip_handle* h, double* flops, size_t* work
   });
 }
 
+struct cfgpp_clip_vision_handle {
+  ClipVisionEncoder enc;
+  cfgpp_clip_vision_handle(const cfgpp_clip_vision_desc& d, int device) : enc(d, device) {}
+};
+
+CFGPP_API int cfgpp_clip_vision_create(const cfgpp_clip_vision_desc* desc, int device, cfgpp_clip_vision_handle** out) {
+  return guarded([&] {
+    CFGPP_REQUIRE(desc && out, "null argument");
+    *out = new cfgpp_clip_vision_handle(*desc, device);
+  });
+}
+
+CFGPP_API int cfgpp_clip_vision_destroy(cfgpp_clip_vision_handle* h) {
+  return guarded([&] { delete h; });
+}
+
+CFGPP_API int cfgpp_clip_vision_load_weight(cfgpp_clip_vision_handle* h, const char* key, const void* data,
+                                            const int64_t* shape, int ndim, int dtype, void* stream) {
+  return guarded([&] { h->enc.load_weight(key, data, shape, ndim, dtype, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_clip_vision_finalize_weights(cfgpp_clip_vision_handle* h, void* stream) {
+  return guarded([&] { h->enc.finalize_weights((cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_clip_vision_encode(cfgpp_clip_vision_handle* h, const void* pixels, int dtype, int batch,
+                                       void* embeds_out, void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(dtype == CFGPP_F16 || dtype == CFGPP_F32, "pixel values: fp16 or fp32");
+    h->enc.encode(pixels, dtype == CFGPP_F16, batch, (__half*)embeds_out, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_clip_vision_stats(cfgpp_clip_vision_handle* h, double* flops, size_t* workspace_bytes) {
+  return guarded([&] {
+    if (flops) *flops = h->enc.flops();
+    if (workspace_bytes) *workspace_bytes = h->enc.workspace_bytes();
+  });
+}
+
 // ---- operator-level entry points (one kernel launch each, on the caller's stream) ----
 CFGPP_API int cfgpp_op_clip_embed(const int32_t* ids, const void* tok, const void* pos, void* out, int M, int T, int D,
                                   int vocab, void* stream) {

@@ -90,11 +90,13 @@ struct StepEntry {
 // The one device record every step consumer reads (timestep embedding, conv_in, zero convs, the step kernels).
 // noise: base of the ancestral noise table [slots][B,4,H,W] fp16, or null. lambda: the per-image guidance table [B]
 // fp32, or null for the entry's scalar cur.s.coef.lambda. Both are read from the record, so a captured graph survives
-// re-allocating, setting and clearing the tables.
+// re-allocating, setting and clearing the tables. ip_scale: the IP-Adapter scale s every decoupled cross-attention
+// launch reads (cfgpp_set_ip_adapter_scale writes it; the captured graph follows).
 struct StepArgs {
   StepEntry cur;
   const __half* noise;
   const float* lambda;
+  float ip_scale;
 };
 // args->cur = table[*counter]; ++*counter
 void run_select_step(const StepEntry* table, int* counter, StepArgs* args, cudaStream_t stream);

@@ -4,9 +4,49 @@
 #include <algorithm>
 #include <cmath>
 
+#include "attention.cuh"
+
 namespace cfgpp {
 
 void gemm_configure();
+void attn_configure();
+
+std::vector<std::vector<ClipStep>> build_clip_layers(const ClipLayerArgs& a, double* flops) {
+  const int D = a.D, I = a.I, M = a.M, act_mode = a.act_mode;
+  const size_t sD = D, sI = I;
+  const float eps = a.eps;
+  __half *x0 = a.x0, *x1 = a.x1, *ln = a.ln, *qkv = a.qkv, *att = a.att, *mlp = a.mlp;
+  const WeightStore& w = *a.weights;
+  std::vector<std::vector<ClipStep>> plan;
+  for (int l = 0; l < a.layers; ++l) {
+    const std::string p = a.prefix + std::to_string(l) + ".";
+    std::vector<ClipStep> steps;
+    auto add_gemm = [&](const GemmOp& op) {
+      *flops += op.flops();
+      steps.push_back([op](cudaStream_t st) { run_gemm_op(op, st); });
+    };
+    const __half *g1 = w.plain(p + "layer_norm1.weight", sD), *b1 = w.plain(p + "layer_norm1.bias", sD);
+    const __half *g2 = w.plain(p + "layer_norm2.weight", sD), *b2 = w.plain(p + "layer_norm2.bias", sD);
+    // x1 = x0 + out_proj(attention(q, k, v of LN1(x0)))
+    steps.push_back([=](cudaStream_t st) { run_layernorm(x0, M, D, g1, b1, eps, ln, st); });
+    add_gemm(make_linear_op(ln, D, nullptr, 0, 0, a.qkv_w[l], M, a.qkv_n, D, a.qkv_b[l], nullptr, 0, 1, qkv, a.qkv_n,
+                            false));
+    const auto attention = a.attention;
+    steps.push_back([=](cudaStream_t st) { attention(qkv, att, st); });
+    *flops += a.attention_flops;
+    add_gemm(make_linear_op(att, a.att_c, nullptr, 0, 0, a.out_w[l], M, D, a.att_c,
+                            w.plain(p + "self_attn.out_proj.bias", sD), x0, D, 1, x1, D, false));
+    // x0 = x1 + fc2(act(fc1(LN2(x1))))
+    steps.push_back([=](cudaStream_t st) { run_layernorm(x1, M, D, g2, b2, eps, ln, st); });
+    add_gemm(make_linear_op(ln, D, nullptr, 0, 0, w.plain(p + "mlp.fc1.weight", sI * sD), M, I, D,
+                            w.plain(p + "mlp.fc1.bias", sI), nullptr, 0, 1, mlp, I, false));
+    steps.push_back([=](cudaStream_t st) { run_clip_activation(mlp, static_cast<size_t>(M) * I, act_mode, st); });
+    add_gemm(make_linear_op(mlp, I, nullptr, 0, 0, w.plain(p + "mlp.fc2.weight", sD * sI), M, D, I,
+                            w.plain(p + "mlp.fc2.bias", sD), x1, D, 1, x0, D, false));
+    plan.push_back(std::move(steps));
+  }
+  return plan;
+}
 
 ClipTextEncoder::ClipTextEncoder(const cfgpp_clip_desc& d, int device) : d_(d), device_(device), sk_(device) {
   CFGPP_CHECK_CUDA(cudaSetDevice(device));
@@ -83,34 +123,14 @@ void ClipTextEncoder::prepare(int batch, int tokens) {
   weights_.plain(tm + "final_layer_norm.weight", sD);
   weights_.plain(tm + "final_layer_norm.bias", sD);
   if (d_.projection_dim > 0) weights_.plain("text_projection.weight", static_cast<size_t>(d_.projection_dim) * sD);
-  const float eps = d_.layer_norm_eps;
-  const int heads = d_.num_heads, act_mode = d_.hidden_act;
-  __half *x0 = x0_, *x1 = x1_, *ln = ln_, *qkv = qkv_, *att = att_, *mlp = mlp_;
-  for (int l = 0; l < d_.num_layers; ++l) {
-    const std::string p = tm + "encoder.layers." + std::to_string(l) + ".";
-    std::vector<Step> steps;
-    auto add_gemm = [&](const GemmOp& op) {
-      flops_ += op.flops();
-      steps.push_back([op](cudaStream_t st) { run_gemm_op(op, st); });
-    };
-    const __half *g1 = weights_.plain(p + "layer_norm1.weight", sD), *b1 = weights_.plain(p + "layer_norm1.bias", sD);
-    const __half *g2 = weights_.plain(p + "layer_norm2.weight", sD), *b2 = weights_.plain(p + "layer_norm2.bias", sD);
-    // x1 = x0 + out_proj(attention(q, k, v of LN1(x0)))
-    steps.push_back([=](cudaStream_t st) { run_layernorm(x0, M, D, g1, b1, eps, ln, st); });
-    add_gemm(make_linear_op(ln, D, nullptr, 0, 0, qkv_w_[l], M, 3 * D, D, qkv_b_[l], nullptr, 0, 1, qkv, 3 * D, false));
-    steps.push_back([=](cudaStream_t st) { run_clip_attention(qkv, att, NB, T, heads, D, st); });
-    flops_ += 2.0 * NB * heads * static_cast<double>(T) * T * 64.0;  // causal: half of 2 * (QK^T + PV)
-    add_gemm(make_linear_op(att, D, nullptr, 0, 0, weights_.plain(p + "self_attn.out_proj.weight", sD * sD), M, D, D,
-                            weights_.plain(p + "self_attn.out_proj.bias", sD), x0, D, 1, x1, D, false));
-    // x0 = x1 + fc2(act(fc1(LN2(x1))))
-    steps.push_back([=](cudaStream_t st) { run_layernorm(x1, M, D, g2, b2, eps, ln, st); });
-    add_gemm(make_linear_op(ln, D, nullptr, 0, 0, weights_.plain(p + "mlp.fc1.weight", sI * sD), M, I, D,
-                            weights_.plain(p + "mlp.fc1.bias", sI), nullptr, 0, 1, mlp, I, false));
-    steps.push_back([=](cudaStream_t st) { run_clip_activation(mlp, static_cast<size_t>(M) * I, act_mode, st); });
-    add_gemm(make_linear_op(mlp, I, nullptr, 0, 0, weights_.plain(p + "mlp.fc2.weight", sD * sI), M, D, I,
-                            weights_.plain(p + "mlp.fc2.bias", sD), x1, D, 1, x0, D, false));
-    layer_plan_.push_back(std::move(steps));
-  }
+  const int heads = d_.num_heads;
+  ClipLayerArgs a{&weights_, tm + "encoder.layers.", d_.num_layers, D, I, M, d_.hidden_act, d_.layer_norm_eps, 3 * D, D,
+                  qkv_w_, qkv_b_, {}, nullptr, 2.0 * NB * heads * static_cast<double>(T) * T * 64.0,  // causal: half
+                  x0_, x1_, ln_, qkv_, att_, mlp_};
+  for (int l = 0; l < d_.num_layers; ++l)
+    a.out_w.push_back(weights_.plain(tm + "encoder.layers." + std::to_string(l) + ".self_attn.out_proj.weight", sD * sD));
+  a.attention = [=](const __half* qkv, __half* att, cudaStream_t st) { run_clip_attention(qkv, att, NB, T, heads, D, st); };
+  layer_plan_ = build_clip_layers(a, &flops_);
   B_ = NB;
   T_ = T;
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
@@ -150,6 +170,151 @@ void ClipTextEncoder::encode(const int* ids, const int* pooled_index, int batch,
       run_clip_gather_rows(last, pooled_index, pooled_out, batch, tokens, D, stream);
     }
   }
+}
+
+
+// ------------------------------------------------------------------------------------------------------------
+// vision tower
+// ------------------------------------------------------------------------------------------------------------
+ClipVisionEncoder::ClipVisionEncoder(const cfgpp_clip_vision_desc& d, int device) : d_(d), device_(device), sk_(device) {
+  CFGPP_CHECK_CUDA(cudaSetDevice(device));
+  CFGPP_REQUIRE(d.num_layers >= 1 && d.num_layers <= 64, "num_layers must be 1..64");
+  CFGPP_REQUIRE(d.num_heads >= 1 && d.hidden_size % d.num_heads == 0 && d.hidden_size / d.num_heads <= 192 &&
+                    d.hidden_size % 64 == 0,
+                "hidden_size must be num_heads * head_dim with head_dim <= 192, a multiple of 64");
+  CFGPP_REQUIRE(d.intermediate_size % 64 == 0 && d.intermediate_size > 0, "intermediate_size must be a multiple of 64");
+  CFGPP_REQUIRE(d.patch_size >= 1 && d.image_size % d.patch_size == 0, "image_size must be a multiple of patch_size");
+  CFGPP_REQUIRE(d.hidden_act == 0 || d.hidden_act == 1, "hidden_act: 0 quick_gelu, 1 gelu");
+  CFGPP_REQUIRE(d.projection_dim > 0 && d.projection_dim % 8 == 0, "projection_dim must be a positive multiple of 8");
+  CFGPP_REQUIRE(d.layer_norm_eps > 0.f, "layer_norm_eps must be positive");
+  np_ = (d.image_size / d.patch_size) * (d.image_size / d.patch_size);
+  T_ = np_ + 1;
+  Kp_ = (3 * d.patch_size * d.patch_size + 63) / 64 * 64;
+  hdp_ = attn_padded_head_dim(d.hidden_size / d.num_heads);
+  Cp_ = d.num_heads * hdp_;
+  gemm_configure();
+  attn_configure();
+}
+
+void ClipVisionEncoder::load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
+                                    cudaStream_t stream) {
+  CFGPP_REQUIRE(!finalized_, "weights already finalized");
+  weights_.load(key, data, shape, ndim, dtype, stream);
+}
+
+void ClipVisionEncoder::finalize_weights(cudaStream_t stream) {
+  CFGPP_REQUIRE(!finalized_, "weights already finalized");
+  const size_t D = d_.hidden_size, H = d_.num_heads, hd = D / H, hdp = hdp_, K = 3 * d_.patch_size * d_.patch_size;
+  const std::string vm = "vision_model.";
+  // the patch conv as [D][Kp], K zero-padded to whole 64-wide k blocks
+  patch_w_ = weights_.alloc(D * Kp_);
+  CFGPP_CHECK_CUDA(cudaMemsetAsync(patch_w_, 0, D * Kp_ * sizeof(__half), stream));
+  CFGPP_CHECK_CUDA(cudaMemcpy2DAsync(patch_w_, Kp_ * sizeof(__half), weights_.plain(vm + "embeddings.patch_embedding.weight", D * K),
+                                     K * sizeof(__half), K * sizeof(__half), D, cudaMemcpyDeviceToDevice, stream));
+  // q | k | v with every head zero-padded to hdp rows (the flash kernel's layout), out_proj with hdp-wide head columns
+  for (int l = 0; l < d_.num_layers; ++l) {
+    const std::string a = vm + "encoder.layers." + std::to_string(l) + ".self_attn.";
+    __half* w = weights_.alloc(3 * H * hdp * D);
+    __half* b = weights_.alloc(3 * H * hdp);
+    __half* o = weights_.alloc(D * H * hdp);
+    CFGPP_CHECK_CUDA(cudaMemsetAsync(w, 0, 3 * H * hdp * D * sizeof(__half), stream));
+    CFGPP_CHECK_CUDA(cudaMemsetAsync(b, 0, 3 * H * hdp * sizeof(__half), stream));
+    CFGPP_CHECK_CUDA(cudaMemsetAsync(o, 0, D * H * hdp * sizeof(__half), stream));
+    const char* names[3] = {"q_proj", "k_proj", "v_proj"};
+    for (int i = 0; i < 3; ++i) {
+      const __half* sw = weights_.plain(a + names[i] + ".weight", D * D);
+      const __half* sb = weights_.plain(a + names[i] + ".bias", D);
+      for (size_t h = 0; h < H; ++h) {
+        CFGPP_CHECK_CUDA(cudaMemcpyAsync(w + ((i * H + h) * hdp) * D, sw + h * hd * D, hd * D * sizeof(__half),
+                                         cudaMemcpyDeviceToDevice, stream));
+        CFGPP_CHECK_CUDA(cudaMemcpyAsync(b + (i * H + h) * hdp, sb + h * hd, hd * sizeof(__half),
+                                         cudaMemcpyDeviceToDevice, stream));
+      }
+    }
+    CFGPP_CHECK_CUDA(cudaMemcpy2DAsync(o, hdp * sizeof(__half), weights_.plain(a + "out_proj.weight", D * D),
+                                       hd * sizeof(__half), hd * sizeof(__half), D * H, cudaMemcpyDeviceToDevice,
+                                       stream));
+    qkv_w_.push_back(w);
+    qkv_b_.push_back(b);
+    out_w_.push_back(o);
+  }
+  CFGPP_CHECK_CUDA(cudaStreamSynchronize(stream));
+  finalized_ = true;
+  try {
+    prepare(1);
+  } catch (...) {
+    finalized_ = false;
+    throw;
+  }
+}
+
+void ClipVisionEncoder::prepare(int batch) {
+  CFGPP_REQUIRE(finalized_, "call cfgpp_clip_vision_finalize_weights first");
+  CFGPP_REQUIRE(batch >= 1 && batch <= 16, "encode batch must be 1..16 images");
+  CFGPP_CHECK_CUDA(cudaSetDevice(device_));
+  CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
+  StreamKScope sk_scope(sk_.ws(), sk_.flags());
+  act_.clear();
+  layer_plan_.clear();
+  flops_ = 0.0;
+  B_ = 0;
+  const int D = d_.hidden_size, I = d_.intermediate_size, T = T_, NB = batch, M = NB * T, H = d_.num_heads;
+  const int hd = D / H, Cp = Cp_;
+  const size_t sD = D;
+  auto act = [&](size_t numel) { return act_.alloc<__half>(numel); };
+  patches_ = act(static_cast<size_t>(NB) * np_ * Kp_);
+  pe_ = act(static_cast<size_t>(NB) * np_ * sD);
+  emb_ = act(M * sD);
+  x0_ = act(M * sD);
+  x1_ = act(M * sD);
+  ln_ = act(M * sD);
+  qkv_ = act(static_cast<size_t>(M) * 3 * Cp);
+  att_ = act(static_cast<size_t>(M) * Cp);
+  mlp_ = act(static_cast<size_t>(M) * I);
+  cls_ = act(NB * sD);
+  cls_ln_ = act(NB * sD);
+  const std::string vm = "vision_model.";
+  weights_.plain(vm + "embeddings.class_embedding", sD);
+  weights_.plain(vm + "embeddings.position_embedding.weight", static_cast<size_t>(T) * sD);
+  for (const char* n : {"pre_layrnorm", "post_layernorm"}) {
+    weights_.plain(vm + n + ".weight", sD);
+    weights_.plain(vm + n + ".bias", sD);
+  }
+  weights_.plain("visual_projection.weight", static_cast<size_t>(d_.projection_dim) * sD);
+  flops_ += 2.0 * NB * np_ * static_cast<double>(D) * 3 * d_.patch_size * d_.patch_size;
+  ClipLayerArgs a{&weights_, vm + "encoder.layers.", d_.num_layers, D, I, M, d_.hidden_act, d_.layer_norm_eps, 3 * Cp,
+                  Cp, qkv_w_, qkv_b_, out_w_, nullptr, 4.0 * NB * H * static_cast<double>(T) * T * hd,
+                  x0_, x1_, ln_, qkv_, att_, mlp_};
+  const AttnOp op = make_attn_op(qkv_, 3 * Cp, qkv_ + Cp, 3 * Cp, qkv_ + 2 * Cp, 3 * Cp, att_, Cp, NB, H, T, T, hd);
+  a.attention = [op](const __half*, __half*, cudaStream_t st) { run_attn_op(op, st); };
+  layer_plan_ = build_clip_layers(a, &flops_);
+  flops_ += 2.0 * NB * static_cast<double>(d_.projection_dim) * D;
+  B_ = NB;
+  CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
+}
+
+void ClipVisionEncoder::encode(const void* image, int is_half, int batch, __half* embeds_out, cudaStream_t stream) {
+  CFGPP_REQUIRE(image != nullptr && embeds_out != nullptr, "null argument");
+  if (batch != B_) prepare(batch);
+  StreamKScope sk_scope(sk_.ws(), sk_.flags());
+  const int D = d_.hidden_size, M = batch * T_;
+  const std::string vm = "vision_model.";
+  run_clip_patchify(image, is_half, patches_, batch, d_.image_size, d_.patch_size, Kp_, stream);
+  run_gemm_op(make_linear_op(patches_, Kp_, nullptr, 0, 0, patch_w_, batch * np_, D, Kp_, nullptr, nullptr, 0, 1, pe_, D,
+                             false),
+              stream);
+  run_clip_vision_embed(pe_, weights_.plain(vm + "embeddings.class_embedding"),
+                        weights_.plain(vm + "embeddings.position_embedding.weight"), emb_, batch, np_, D, stream);
+  run_layernorm(emb_, M, D, weights_.plain(vm + "pre_layrnorm.weight"), weights_.plain(vm + "pre_layrnorm.bias"),
+                d_.layer_norm_eps, x0_, stream);
+  for (auto& layer : layer_plan_)
+    for (auto& fn : layer) fn(stream);
+  CFGPP_CHECK_CUDA(cudaMemcpy2DAsync(cls_, D * sizeof(__half), x0_, static_cast<size_t>(T_) * D * sizeof(__half),
+                                     D * sizeof(__half), batch, cudaMemcpyDeviceToDevice, stream));
+  run_layernorm(cls_, batch, D, weights_.plain(vm + "post_layernorm.weight"), weights_.plain(vm + "post_layernorm.bias"),
+                d_.layer_norm_eps, cls_ln_, stream);
+  run_small_linear(cls_ln_, D, weights_.plain("visual_projection.weight"), nullptr, nullptr, 0, embeds_out,
+                   d_.projection_dim, nullptr, batch, d_.projection_dim, D, false, stream);
 }
 
 }  // namespace cfgpp

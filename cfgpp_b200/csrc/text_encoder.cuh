@@ -26,6 +26,31 @@ void run_clip_attention(const __half* qkv, __half* out, int B, int T, int heads,
 void run_clip_activation(__half* x, size_t n, int mode, cudaStream_t stream);
 void run_clip_gather_rows(const __half* x, const int* index, __half* out, int B, int T, int D, cudaStream_t stream);
 
+// CLIP vision front end (text_kernels.cu): image [B,3,S,S] NCHW (fp16 or fp32) -> patch rows [B*(S/P)^2][Kp] fp16,
+// row-major (channel, ky, kx) as conv2d's weight, columns 3*P*P..Kp-1 zero; and the embedding assembly
+// x[b,0] = fp16(cls + pos[0]), x[b,1+p] = fp16(pe[b*np + p] + pos[1+p]).
+void run_clip_patchify(const void* image, int is_half, __half* out, int B, int S, int P, int Kp, cudaStream_t stream);
+void run_clip_vision_embed(const __half* pe, const __half* cls, const __half* pos, __half* out, int B, int np, int D,
+                           cudaStream_t stream);
+
+using ClipStep = std::function<void(cudaStream_t)>;
+// The pre-LN encoder layer loop both CLIP towers share: per layer LN1 -> q|k|v GEMM -> attention -> out_proj (+ the
+// residual, epilogue) -> LN2 -> fc1 -> activation -> fc2 (+ the residual). The towers differ only in the attention
+// step (`attention`: qkv [M][qkv_n] -> att [M][att_c]) and in how q|k|v and out_proj are packed (`qkv_w` / `qkv_b` /
+// `out_w` per layer; the text tower's are the plain concatenation and weight).
+struct ClipLayerArgs {
+  const WeightStore* weights;
+  std::string prefix;  // "<tower>.encoder.layers."
+  int layers, D, I, M, act_mode;
+  float eps;
+  int qkv_n, att_c;
+  std::vector<__half*> qkv_w, qkv_b, out_w;
+  std::function<void(const __half* qkv, __half* att, cudaStream_t)> attention;
+  double attention_flops;  // per layer
+  __half *x0, *x1, *ln, *qkv, *att, *mlp;
+};
+std::vector<std::vector<ClipStep>> build_clip_layers(const ClipLayerArgs& a, double* flops);
+
 class ClipTextEncoder {
  public:
   ClipTextEncoder(const cfgpp_clip_desc& d, int device);
@@ -52,11 +77,43 @@ class ClipTextEncoder {
   std::vector<__half*> qkv_w_, qkv_b_;  // per layer: [3D][D], [3D]
   double flops_ = 0.0;
   int B_ = 0, T_ = 0;
-  using Step = std::function<void(cudaStream_t)>;
-  std::vector<std::vector<Step>> layer_plan_;  // one group of launches per encoder layer
+  std::vector<std::vector<ClipStep>> layer_plan_;  // one group of launches per encoder layer
   const int* ids_in_ = nullptr;                 // set per encode() call
   __half *x0_ = nullptr, *x1_ = nullptr, *ln_ = nullptr, *qkv_ = nullptr, *att_ = nullptr, *mlp_ = nullptr;
   __half *last_ = nullptr, *pool_ = nullptr;
+};
+
+// transformers CLIPVisionModelWithProjection: patch embedding (a bias-free PxP stride-P conv, as an unfold and a
+// GEMM), class token and position embedding, pre_layrnorm, the shared layer loop with non-causal attention on the flash
+// kernel (heads zero-padded to a multiple of 64 columns), post_layernorm of the CLS row, visual_projection.
+class ClipVisionEncoder {
+ public:
+  ClipVisionEncoder(const cfgpp_clip_vision_desc& d, int device);
+  void load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
+                   cudaStream_t stream);
+  void finalize_weights(cudaStream_t stream);
+  // image [batch][3][S][S] (fp16 or fp32, normalised pixel values) -> image_embeds [batch][projection_dim] fp16
+  void encode(const void* image, int is_half, int batch, __half* embeds_out, cudaStream_t stream);
+  double flops() const { return flops_; }
+  size_t workspace_bytes() const { return act_.bytes(); }
+
+ private:
+  void prepare(int batch);
+
+  cfgpp_clip_vision_desc d_;
+  int device_;
+  bool finalized_ = false;
+  int T_ = 0, np_ = 0, Kp_ = 0, hdp_ = 0, Cp_ = 0;
+  WeightStore weights_;
+  DeviceArena act_;
+  StreamKWorkspace sk_;
+  __half* patch_w_ = nullptr;  // [D][Kp]
+  std::vector<__half*> qkv_w_, qkv_b_, out_w_;
+  double flops_ = 0.0;
+  int B_ = 0;
+  std::vector<std::vector<ClipStep>> layer_plan_;
+  __half *patches_ = nullptr, *pe_ = nullptr, *emb_ = nullptr, *x0_ = nullptr, *x1_ = nullptr, *ln_ = nullptr,
+         *qkv_ = nullptr, *att_ = nullptr, *mlp_ = nullptr, *cls_ = nullptr, *cls_ln_ = nullptr;
 };
 
 }  // namespace cfgpp

@@ -9,6 +9,43 @@ namespace cfgpp {
 
 namespace {
 
+// patch rows of an NCHW image: out[(b * g + py) * g + px][(c * P + ky) * P + kx] = fp16(x[b, c, py P + ky, px P + kx]),
+// columns 3 P P .. Kp - 1 zero (g = S / P)
+__global__ void clip_patchify_kernel(const void* __restrict__ x, int is_half, __half* __restrict__ out, int B, int S,
+                                     int P, int Kp) {
+  const int g = S / P, K = 3 * P * P;
+  const size_t n = static_cast<size_t>(B) * g * g * Kp;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int k = static_cast<int>(i % Kp);
+    const size_t row = i / Kp;
+    __half v = __float2half(0.f);
+    if (k < K) {
+      const int px = static_cast<int>(row % g), py = static_cast<int>((row / g) % g), b = static_cast<int>(row / g / g);
+      const int c = k / (P * P), ky = (k / P) % P, kx = k % P;
+      const size_t src = ((static_cast<size_t>(b) * 3 + c) * S + py * P + ky) * S + px * P + kx;
+      v = is_half ? static_cast<const __half*>(x)[src] : __float2half_rn(static_cast<const float*>(x)[src]);
+    }
+    out[i] = v;
+  }
+}
+
+// x[b, 0, :] = fp16(cls + pos[0]), x[b, 1 + p, :] = fp16(pe[b np + p] + pos[1 + p])
+__global__ void clip_vision_embed_kernel(const __half* __restrict__ pe, const __half* __restrict__ cls,
+                                         const __half* __restrict__ pos, __half* __restrict__ out, int B, int np,
+                                         int D) {
+  const int T = np + 1;
+  const size_t n = static_cast<size_t>(B) * T * D;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int d = static_cast<int>(i % D);
+    const int t = static_cast<int>((i / D) % T);
+    const int b = static_cast<int>(i / D / T);
+    const __half a = t == 0 ? cls[d] : pe[(static_cast<size_t>(b) * np + t - 1) * D + d];
+    out[i] = __float2half_rn(__half2float(a) + __half2float(pos[static_cast<size_t>(t) * D + d]));
+  }
+}
+
 // out[r, :] = fp16(tok[ids[r], :] + pos[r % T, :])   (one rounding, as the fp16 module's `inputs_embeds + position_embeddings`)
 __global__ void clip_embed_kernel(const int* __restrict__ ids, const uint4* __restrict__ tok, const uint4* __restrict__ pos,
                                   uint4* __restrict__ out, int M, int T, int Dv, int vocab) {
@@ -183,6 +220,21 @@ void run_clip_gather_rows(const __half* x, const int* index, __half* out, int B,
   const int total = B * (D / 8);
   launch_pdl(clip_gather_rows_kernel, dim3((total + 127) / 128), dim3(128), 0, stream, reinterpret_cast<const uint4*>(x),
              index, reinterpret_cast<uint4*>(out), B, T, D / 8);
+}
+
+void run_clip_patchify(const void* image, int is_half, __half* out, int B, int S, int P, int Kp, cudaStream_t stream) {
+  const size_t n = static_cast<size_t>(B) * (S / P) * (S / P) * Kp;
+  clip_patchify_kernel<<<static_cast<int>(std::min<size_t>((n + 255) / 256, 8192)), 256, 0, stream>>>(image, is_half, out,
+                                                                                                       B, S, P, Kp);
+  CFGPP_CHECK_CUDA(cudaGetLastError());
+}
+
+void run_clip_vision_embed(const __half* pe, const __half* cls, const __half* pos, __half* out, int B, int np, int D,
+                           cudaStream_t stream) {
+  const size_t n = static_cast<size_t>(B) * (np + 1) * D;
+  clip_vision_embed_kernel<<<static_cast<int>(std::min<size_t>((n + 255) / 256, 8192)), 256, 0, stream>>>(pe, cls, pos,
+                                                                                                           out, B, np, D);
+  CFGPP_CHECK_CUDA(cudaGetLastError());
 }
 
 }  // namespace cfgpp

@@ -508,7 +508,25 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
                2.0 * Mkv * 2.0 * C * D);
       cur_plan_ = save;
     }
-    add_attn(b + ".attn2.sdpa", make_attn_op(qb, Cp, kv, 2 * Cp, kv + Cp, 2 * Cp, attn, Cp, NB_, heads, HW, n_ctx_, hd));
+    if (ip_ntok_ > 0 && !is_cn_) {  // IP-Adapter: the image tokens' K‖V once per image, attended to in the same kernel
+      const int Mip = NB_ * ip_ntok_;
+      __half* kv_ip = alloc_act(static_cast<size_t>(Mip) * 2 * Cp);
+      const std::string pk = b + ".attn2.processor.to_k_ip.0.weight", pv = b + ".attn2.processor.to_v_ip.0.weight";
+      weights_.plain(pk, static_cast<size_t>(C) * D);
+      weights_.plain(pv, static_cast<size_t>(C) * D);
+      __half* wkv = packed_heads_rows({pk, pv}, heads, hd, hdp);
+      std::vector<PlanStep>* save = cur_plan_;
+      cur_plan_ = &ip_plan_;
+      add_gemm(b + ".attn2.to_kv_ip",
+               make_linear_op(ip_tokens_, D, nullptr, 0, 0, wkv, Mip, 2 * Cp, D, nullptr, nullptr, 0, 1, kv_ip, 2 * Cp,
+                              false),
+               2.0 * Mip * 2.0 * C * D);
+      cur_plan_ = save;
+      add_attn(b + ".attn2.sdpa", make_attn_ip_op(qb, Cp, kv, 2 * Cp, kv + Cp, 2 * Cp, kv_ip, 2 * Cp, kv_ip + Cp, 2 * Cp,
+                                                  ip_ntok_, &args_->ip_scale, attn, Cp, NB_, heads, HW, n_ctx_, hd));
+    } else {
+      add_attn(b + ".attn2.sdpa", make_attn_op(qb, Cp, kv, 2 * Cp, kv + Cp, 2 * Cp, attn, Cp, NB_, heads, HW, n_ctx_, hd));
+    }
     add_gemm(b + ".attn2.to_out", producer([&](int bn) {
                return make_linear_op(attn, Cp, nullptr, 0, 0,
                                      packed_heads_cols(b + ".attn2.to_out.0.weight", heads, hd, hdp), Mi, C, Cp,
@@ -609,6 +627,8 @@ void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
   up_plan_.clear();
   tail_plan_.clear();
   prompt_plan_.clear();
+  ip_plan_.clear();
+  ip_ready_ = false;
   res_.clear();
   res_hw_.clear();
   B_ = batch; NB_ = 2 * batch; H_ = h_lat; W_ = w_lat;
@@ -660,6 +680,11 @@ void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
         time_ids_copy_ = act_.alloc<float>(static_cast<size_t>(NB_) * n_time_ids_);
       }
       args_ = shared_args ? shared_args : act_.alloc<StepArgs>(1);
+      if (ip_ntok_ > 0 && !is_cn_) {
+        ip_embeds_ = alloc_act(static_cast<size_t>(NB_) * ip_embed_dim_);
+        ip_proj_ = alloc_act(static_cast<size_t>(NB_) * ip_ntok_ * d_.cross_attention_dim);
+        ip_tokens_ = alloc_act(static_cast<size_t>(NB_) * ip_ntok_ * d_.cross_attention_dim);
+      }
       if (!is_cn_) {  // the sampler state and tables: a ControlNet runs inside its UNet's step
         step_counter_ = act_.alloc<int>(1);
         step_table_ = act_.alloc<StepEntry>(1024);
@@ -668,7 +693,7 @@ void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
         aux_state_ = act_.alloc<float>(lat);
         z0t_state_ = act_.alloc<float>(lat);
         lambda_buf_ = act_.alloc<float>(B_);
-        const StepArgs a{{}, noise_buf_, nullptr};  // no guidance table: the schedule's scalar lambda
+        const StepArgs a{{}, noise_buf_, nullptr, ip_scale_};  // no guidance table: the schedule's scalar lambda
         CFGPP_CHECK_CUDA(cudaMemcpy(args_, &a, sizeof(a), cudaMemcpyHostToDevice));
         fwd_eps_uc_ = alloc_act(lat);
         fwd_eps_c_ = alloc_act(lat);
@@ -728,6 +753,19 @@ void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
       add_step("add_embedding.linear_2", [=](cudaStream_t st) {
         run_small_linear(add_h1, TE, w2, b2, nullptr, 0, aug, TE, nullptr, NB, TE, TE, false, st);
       });
+    }
+
+    // ---- IP-Adapter image projection (diffusers ImageProjection): LayerNorm(D) of the rows of Linear(E -> ntok * D) ----
+    cur_plan_ = &ip_plan_;
+    if (!sizing_ && ip_ntok_ > 0 && !is_cn_) {
+      const int NB = NB_, D = d_.cross_attention_dim, E = ip_embed_dim_, T = ip_ntok_;
+      add_gemm("image_proj.proj",
+               make_linear_op(ip_embeds_, E, nullptr, 0, 0, weights_.plain("image_proj.proj.weight", size_t(T) * D * E),
+                              NB, T * D, E, weights_.plain("image_proj.proj.bias", size_t(T) * D), nullptr, 0, 1,
+                              ip_proj_, T * D, false));
+      const __half *g = weights_.plain("image_proj.norm.weight", D), *bt = weights_.plain("image_proj.norm.bias", D);
+      __half *in = ip_proj_, *out = ip_tokens_;
+      add_step("image_proj.norm", [=](cudaStream_t st) { run_layernorm(in, NB * T, D, g, bt, 1e-5f, out, st); });
     }
 
     // ---- body (SURVEY A.2 steps 2-6) ----
@@ -820,7 +858,8 @@ void Unet::account() {
   for (auto& s : prologue_plan_) launches_per_step_ += s.launches;
   prompt_flops_ = 0.0;
   prompt_launches_ = 0;
-  for (auto& s : prompt_plan_) { prompt_flops_ += s.flops; prompt_launches_ += s.launches; }
+  for (auto* pl : {&prompt_plan_, &ip_plan_})
+    for (auto& s : *pl) { prompt_flops_ += s.flops; prompt_launches_ += s.launches; }
   forward_flops_ += prompt_flops_;
   const double px = static_cast<double>(NB_) * H_ * W_;
   forward_flops_ += 2.0 * px * (36.0 * C0 + (is_cn_ ? 0.0 : 36.0 * C0));  // conv_in + conv_out
@@ -890,6 +929,11 @@ void Unet::run_inputs(const void* z, int z_is_half, cudaStream_t stream) {
                 cn_->cond_);
 }
 
+void Unet::require_ip_ready() const {
+  CFGPP_REQUIRE(ip_ntok_ == 0 || ip_ready_, "an IP-Adapter is attached: call cfgpp_set_ip_image_embeds for the prepared "
+                                            "plan and the loaded adapter");
+}
+
 void Unet::require_control_ready() const {
   CFGPP_REQUIRE(!cn_ || cn_image_ready_, "a ControlNet is attached: call cfgpp_set_control_image for the prepared shape");
 }
@@ -944,6 +988,7 @@ void Unet::unet_forward(const void* z, int z_dtype, float t, float in_scale, __h
   CFGPP_REQUIRE(prepared_, "call cfgpp_prepare first");
   require_fresh_prompt();
   require_control_ready();
+  require_ip_ready();
   stage_entry(t, in_scale, stream);
   run_inputs(z, z_dtype == CFGPP_F16 ? 1 : 0, stream);
   run_body(stream);
@@ -963,6 +1008,7 @@ std::vector<Unet::ProfEntry> Unet::profile_forward(const void* z, int z_dtype, f
     evs.push_back(e);
   };
   require_control_ready();
+  require_ip_ready();
   stage_entry(t, in_scale, stream);
   mark();
   auto run = [&](const std::vector<PlanStep>& plan, const std::string& prefix) {
@@ -1089,6 +1135,7 @@ void Unet::ensure_graph(cudaStream_t stream) {
   CFGPP_CHECK_CUDA(cudaStreamEndCapture(capture_stream_, &graph_));
   CFGPP_CHECK_CUDA(cudaGraphInstantiate(&graph_exec_, graph_, 0));
   graph_valid_ = true;
+  ++graph_captures_;
 }
 
 void Unet::run_steps(int first_step, int nsteps, cudaStream_t stream) {
@@ -1097,6 +1144,7 @@ void Unet::run_steps(int first_step, int nsteps, cudaStream_t stream) {
   CFGPP_REQUIRE(!v_pred_ || v_ready_, "a v-prediction model needs cfgpp_set_v_coefs for this schedule");
   require_fresh_prompt();
   require_control_ready();
+  require_ip_ready();
   ensure_graph(stream);
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(step_counter_, &first_step, sizeof(int), cudaMemcpyHostToDevice, stream));
   for (int i = 0; i < nsteps; ++i) CFGPP_CHECK_CUDA(cudaGraphLaunch(graph_exec_, stream));
@@ -1175,6 +1223,73 @@ void Unet::set_control_scales(const float* scales, int n, cudaStream_t stream) {
   CFGPP_REQUIRE(nsteps_ > 0 && scales != nullptr && n == nsteps_, "one conditioning scale per schedule entry");
   for (int i = 0; i < n; ++i) entries_[i].control_scale = scales[i];
   upload_entries(stream);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// IP-Adapter
+// ------------------------------------------------------------------------------------------------------------
+void Unet::ip_load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
+                          cudaStream_t stream) {
+  CFGPP_REQUIRE(!is_cn_, "an IP-Adapter loads into a UNet handle, not a ControlNet");
+  CFGPP_REQUIRE(finalized_, "call cfgpp_finalize_weights first");
+  const bool proj = key.rfind("image_proj.", 0) == 0;
+  const bool kv = key.find(".attn2.processor.to_k_ip.0.weight") != std::string::npos ||
+                  key.find(".attn2.processor.to_v_ip.0.weight") != std::string::npos;
+  CFGPP_REQUIRE(proj || kv, "not an IP-Adapter weight key: " + key);
+  if (kv) {  // [C, D] like the block's own to_k
+    const std::string base = key.substr(0, key.find(".attn2.processor."));
+    CFGPP_REQUIRE(weights_.has(base + ".attn2.to_k.weight"), "no cross-attention at " + base + " for " + key);
+    const std::vector<int64_t>& want = weights_.raw(base + ".attn2.to_k.weight").shape;
+    CFGPP_REQUIRE(static_cast<size_t>(ndim) == want.size() && std::equal(want.begin(), want.end(), shape),
+                  "shape of " + key + " differs from the block's to_k");
+  }
+  // a key loaded again gets a new buffer: the plan, which holds raw pointers, is dropped (the next cfgpp_prepare
+  // builds it), and the packed K‖V copies that read the key are re-packed in place
+  const bool reload = weights_.has(key);
+  if (reload) CFGPP_CHECK_CUDA(cudaDeviceSynchronize());  // a replay may still read the old tensor
+  weights_.load(key, data, shape, ndim, dtype, stream);
+  if (reload) {
+    refresh_packed({key}, stream);
+    prepared_ = false;
+    graph_valid_ = false;
+    nsteps_ = 0;
+  }
+  ip_ready_ = false;
+}
+
+void Unet::ip_attach(int n_tokens, int embed_dim) {
+  CFGPP_REQUIRE(!is_cn_, "an IP-Adapter attaches to a UNet handle, not a ControlNet");
+  CFGPP_REQUIRE(finalized_, "call cfgpp_finalize_weights first");
+  if (n_tokens != 0) {
+    CFGPP_REQUIRE(n_tokens >= 1 && n_tokens <= 64, "an IP-Adapter has 1..64 image tokens");
+    CFGPP_REQUIRE(embed_dim >= 8 && embed_dim % 8 == 0, "the image embedding width must be a positive multiple of 8");
+  }
+  ip_ntok_ = n_tokens;
+  ip_embed_dim_ = n_tokens ? embed_dim : 0;
+  // the plan changes shape: the next cfgpp_prepare builds it
+  prepared_ = false;
+  graph_valid_ = false;
+  nsteps_ = 0;
+  ip_ready_ = false;
+}
+
+void Unet::set_ip_image_embeds(const __half* embeds, cudaStream_t stream) {
+  CFGPP_REQUIRE(ip_ntok_ > 0, "no IP-Adapter attached");
+  CFGPP_REQUIRE(prepared_, "call cfgpp_prepare first");
+  CFGPP_REQUIRE(embeds != nullptr, "null image embeds");
+  CFGPP_CHECK_CUDA(cudaMemcpyAsync(ip_embeds_, embeds, static_cast<size_t>(NB_) * ip_embed_dim_ * sizeof(__half),
+                                   cudaMemcpyDeviceToDevice, stream));
+  StreamKScope sk_scope(sk_.ws(), sk_.flags());
+  run_plan(ip_plan_, stream);
+  ip_ready_ = true;
+}
+
+void Unet::set_ip_scale(float scale, cudaStream_t stream) {
+  CFGPP_REQUIRE(!is_cn_, "the IP-Adapter scale is set on the UNet handle");
+  ip_scale_ = scale;
+  // pageable source: staged before the call returns; the stream orders it after a replay still reading the word
+  if (prepared_)
+    CFGPP_CHECK_CUDA(cudaMemcpyAsync(&args_->ip_scale, &ip_scale_, sizeof(float), cudaMemcpyHostToDevice, stream));
 }
 
 void Unet::cond_embed(const void* image, int is_half, int B, int Hi, int Wi, __half* out, cudaStream_t stream) {

@@ -49,6 +49,7 @@ class Unet {
   int launches_per_step() const { return launches_per_step_; }
   double prompt_flops() const { return prompt_flops_; }
   int prompt_launches() const { return prompt_launches_; }
+  int graph_captures() const { return graph_captures_; }  // step graphs captured over the handle's life
 
   void set_prompt(const __half* ctx, int n_ctx, const __half* pooled, const float* time_ids, int add_rows,
                   cudaStream_t stream);
@@ -72,6 +73,12 @@ class Unet {
   // ControlNet handles: the conditioning embedding of image [B,3,Hi,Wi] -> out [B,Hi/8,Wi/8,C0] NHWC fp16
   void cond_embed(const void* image, int is_half, int B, int Hi, int Wi, __half* out, cudaStream_t stream);
   void apply_step(int step, const __half* eps_uc, const __half* eps_c, cudaStream_t stream);
+  // ---- IP-Adapter (see cfgpp_ip_adapter_attach) ----
+  void ip_load_weight(const std::string& key, const void* data, const int64_t* shape, int ndim, int dtype,
+                      cudaStream_t stream);
+  void ip_attach(int n_tokens, int embed_dim);  // n_tokens = 0 detaches
+  void set_ip_image_embeds(const __half* embeds, cudaStream_t stream);
+  void set_ip_scale(float scale, cudaStream_t stream);
   // Eager un-fused forward with a CUDA-event pair around every plan entry (profiling aid for bench.py).
   struct ProfEntry {
     std::string name;
@@ -149,6 +156,7 @@ class Unet {
   // prologue(s) and conv_in(s) of one forward on input z
   void run_inputs(const void* z, int z_is_half, cudaStream_t stream);
   void require_control_ready() const;
+  void require_ip_ready() const;
   void upload_entries(cudaStream_t stream);  // entries_ -> step_table_
   // the un-fused forward's current entry: timestep and input scale, no step, the scalar conditioning scale
   void stage_entry(float t, float in_scale, cudaStream_t stream);
@@ -232,9 +240,18 @@ class Unet {
   float cn_scale_ = 1.0f;
   bool cn_image_ready_ = false;
 
+  // IP-Adapter: the image tokens image_proj(embeds) [NB * ip_ntok_][D] and, per attn2, their K‖V, projected by
+  // ip_plan_ once per set_ip_image_embeds; every attn2 of the body runs the decoupled cross-attention kernel
+  int ip_ntok_ = 0, ip_embed_dim_ = 0;  // ip_ntok_ = 0: no adapter attached
+  float ip_scale_ = 1.0f;
+  bool ip_ready_ = false;               // image embeds projected for the current plan and weights
+  __half *ip_embeds_ = nullptr, *ip_proj_ = nullptr, *ip_tokens_ = nullptr;
+  std::vector<PlanStep> ip_plan_;
+
   cudaGraph_t graph_ = nullptr;
   cudaGraphExec_t graph_exec_ = nullptr;
   bool graph_valid_ = false;
+  int graph_captures_ = 0;
   cudaStream_t capture_stream_ = nullptr;
 };
 

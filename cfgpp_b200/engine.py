@@ -36,6 +36,9 @@ class NativeUNet(nv.NativeHandle):
         self._lora_per_key = {}  # weight key -> adapters targeting it
         self.controlnet = None  # the attached NativeControlNet (its plan is part of ours)
         self._control_image = None  # the control image embedded for the prepared shape
+        self.ip_adapter = None  # the attached ip_adapter.IPAdapter
+        self.ip_request = None  # the IPRequest of the running sample() call (bind_control applies it), else None
+        self._ip_embeds = None  # the image embeds projected for the prepared plan
 
     def _create(self, desc, idx: int) -> None:
         nv.check(self.lib.cfgpp_create_ex(byref(desc), c_size_t(ctypes.sizeof(desc)), c_int(idx), byref(self._h)))
@@ -47,7 +50,7 @@ class NativeUNet(nv.NativeHandle):
         # a failing native prepare() leaves the handle unprepared: forget the old shape and the bound prompt first so
         # that the next call re-plans instead of running on freed buffers
         self.batch, self.latent_hw, self._nsteps, self._bound = 0, (0, 0), 0, None
-        self._control_image = None
+        self._control_image = self._ip_embeds = None
         with torch.cuda.device(self.device):
             nv.check(self.lib.cfgpp_prepare(self._h, c_int(batch), c_int(h_lat), c_int(w_lat)))
         self.batch, self.latent_hw = batch, (h_lat, w_lat)
@@ -241,10 +244,15 @@ class NativeUNet(nv.NativeHandle):
         solvers, so an uncontrolled call detaches whatever an earlier call left attached."""
         b, _, h, w = zt.shape
         self.attach_controlnet(None if request is None else request.engine)
+        ip = self.ip_request
+        self.attach_ip_adapter(None if ip is None else ip.adapter)
         self.prepare(b, h, w)
         self.bind_prompt(uc, c, pooled, time_ids, force=force)
         if request is not None:
             self.set_control_image(request.image)
+        if ip is not None:
+            self.set_ip_image_embeds(ip.embeds, force=force)
+            self.set_ip_adapter_scale(ip.scale)
 
     # ---- ControlNet ----------------------------------------------------------------------------------------------
     def attach_controlnet(self, cn) -> None:
@@ -289,6 +297,50 @@ class NativeUNet(nv.NativeHandle):
         arr = (c_float * len(scales))(*[float(s) for s in scales])
         with torch.cuda.device(self.device):
             nv.check(self.lib.cfgpp_set_control_scales(self._h, arr, c_int(len(scales)), nv.stream_ptr()))
+
+    # ---- IP-Adapter -------------------------------------------------------------------------------------------
+    def attach_ip_adapter(self, adapter) -> None:
+        """Load an `ip_adapter.IPAdapter` into this live handle and attach it (None detaches; the UNet's own weights are
+        untouched either way). A change drops the plan: the next prepare() builds every attn2 with (or without) the
+        image segment, and set_ip_image_embeds must run after it."""
+        if adapter is self.ip_adapter:
+            return
+        with torch.cuda.device(self.device):
+            if adapter is None:
+                nv.check(self.lib.cfgpp_ip_adapter_clear(self._h))
+            else:
+                st = nv.stream_ptr()
+                for key, w in adapter.weights.items():
+                    w = w.detach().to(self.device).contiguous()
+                    shape = (ctypes.c_int64 * w.dim())(*w.shape)
+                    nv.check(self.lib.cfgpp_ip_adapter_load_weight(self._h, key.encode(), nv.ptr(w), shape,
+                                                                   c_int(w.dim()), c_int(nv.dtype_code(w)), st))
+                torch.cuda.synchronize(self.device)
+                nv.check(self.lib.cfgpp_ip_adapter_attach(self._h, c_int(adapter.n_tokens), c_int(adapter.embed_dim)))
+        self.ip_adapter = adapter
+        self._ip_embeds = None
+        self.batch, self.latent_hw, self._nsteps, self._bound, self._control_image = 0, (0, 0), 0, None, None
+
+    def set_ip_image_embeds(self, embeds: torch.Tensor, force: bool = True) -> None:
+        """embeds [batch, E]: one image embedding per image of the prepared batch. The unconditional half gets zeros,
+        as diffusers' negative image embeds; the image projection and every block's K / V projection run here. With
+        force False, the same tensor object (same in-place version) already projected for this plan is not projected
+        again; any other tensor is (a new reference image with the same prompt)."""
+        assert embeds.dim() == 2 and embeds.shape[0] == self.batch, "one image embedding per image of the batch"
+        key = (embeds, embeds._version)
+        if not force and self._ip_embeds is not None and self._ip_embeds[0] is embeds \
+                and self._ip_embeds[1] == key[1]:
+            return
+        e = embeds.to(self.device, torch.float16)
+        rows = torch.cat([torch.zeros_like(e), e]).contiguous()
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_set_ip_image_embeds(self._h, nv.ptr(rows), nv.stream_ptr()))
+        self._ip_embeds = key
+
+    def set_ip_adapter_scale(self, scale: float) -> None:
+        """The scale s of every decoupled cross-attention: a device word, so the step graph is never recaptured."""
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_set_ip_adapter_scale(self._h, c_float(float(scale)), nv.stream_ptr()))
 
     # ---- LoRA adapters ----------------------------------------------------------------------------------------
     MAX_LORAS_PER_WEIGHT = 4

@@ -184,7 +184,9 @@ class BaseDDIM(StableDiffusion):
     def sample(self, cfg_guidance=7.5, prompt=["", ""], callback_fn=None, **kwargs):
         """Batched: see StableDiffusion.batch_inputs. Returns (B, 3, H, W). ControlNet: `controlnet=` (a
         controlnet.ControlNet), `control_image=` (B or 1, 3, H, W) in [0, 1] at the output size,
-        `controlnet_conditioning_scale=`, `control_guidance_start=` / `control_guidance_end=` (diffusers' meaning)."""
+        `controlnet_conditioning_scale=`, `control_guidance_start=` / `control_guidance_end=` (diffusers' meaning).
+        IP-Adapter: `ip_adapter=` (an ip_adapter.IPAdapter for this UNet), `ip_adapter_image=` (one image, broadcast,
+        or one per prompt), `ip_adapter_scale=` (1.0)."""
         uc, c, cfg_guidance, zt = self.batch_inputs(prompt, cfg_guidance, kwargs.get('zT'))
         if zt is None:
             zt = self.initialize_latent(latent_dim=(uc.shape[0], 4, self.cfg.sample_size, self.cfg.sample_size))

@@ -36,7 +36,7 @@ from .text_encoder import CLIPTextConfig, ClipConditioner, get_conditioner
 from .config import UNetConfig, sdxl_config, sdxl_refiner_config
 from .engine import NativeUNet
 from .lora import LoraMixin, is_lora_file, read_lora
-from .solver_base import SolverBase, refuse_control, registry
+from .solver_base import SolverBase, refuse_control, refuse_ip_adapter, registry
 from .weights import load_safetensors_state_dict, synthetic_state_dict
 
 __SOLVER__, register_solver, get_solver = registry()
@@ -272,9 +272,13 @@ class SDXL(SolverBase):
 
         ControlNet: `controlnet=` (a controlnet.ControlNet), `control_image=` (B or 1, 3, H, W) in [0, 1] at the output
         size, `controlnet_conditioning_scale=`, `control_guidance_start=` / `control_guidance_end=` (diffusers' meaning,
-        over the whole schedule); a refiner runs uncontrolled."""
+        over the whole schedule); a refiner runs uncontrolled.
+
+        IP-Adapter: `ip_adapter=` (an ip_adapter.IPAdapter for this UNet), `ip_adapter_image=` (one image, broadcast,
+        or one per prompt), `ip_adapter_scale=` (1.0); not with `refiner=`."""
         if refiner is not None:
             self._check_refiner()
+            refuse_ip_adapter(kwargs, "sample(refiner=...)")
         size = self.default_sample_size * self.vae_scale_factor
         original_size, target_size = original_size or (size, size), target_size or (size, size)
 

@@ -44,9 +44,34 @@ CONTROL_KWARGS = ("controlnet", "control_image", "controlnet_conditioning_scale"
 
 
 def refuse_control(kwargs: dict, what: str) -> None:
-    """The inversion / editing solvers take no ControlNet."""
+    """The inversion / editing solvers take no ControlNet and no IP-Adapter."""
     if kwargs.get("controlnet") is not None or kwargs.get("control_image") is not None:
         raise ValueError(f"{what} does not take a ControlNet (text-to-image solvers only)")
+    refuse_ip_adapter(kwargs, what)
+
+
+def refuse_ip_adapter(kwargs: dict, what: str) -> None:
+    if kwargs.get("ip_adapter") is not None or kwargs.get("ip_adapter_image") is not None:
+        raise ValueError(f"{what} does not take an IP-Adapter (SD v1.5 / SDXL text-to-image solvers only)")
+
+
+class IPRequest:
+    """The IP-Adapter of one sample() call: the adapter, the image embeds of its batch (one per prompt) and the
+    scale."""
+
+    def __init__(self, adapter, embeds: torch.Tensor, scale: float):
+        self.adapter, self.embeds, self.scale = adapter, embeds, float(scale)
+
+
+def ip_request(kwargs: dict, batch: int):
+    """The IPRequest that sample()'s `ip_adapter=`, `ip_adapter_image=` (one image, broadcast, or one per prompt) and
+    `ip_adapter_scale=` ask for, or None."""
+    ad, image = kwargs.get("ip_adapter"), kwargs.get("ip_adapter_image")
+    if ad is None and image is None:
+        return None
+    if ad is None or image is None:
+        raise ValueError("ip_adapter and ip_adapter_image go together")
+    return IPRequest(ad, ad.image_embeds(image, batch), kwargs.get("ip_adapter_scale", 1.0))
 
 
 class SolverBase(K.KDiffusionMixin, LoraMixin):
@@ -56,11 +81,19 @@ class SolverBase(K.KDiffusionMixin, LoraMixin):
     def _controlled(self, kwargs: dict, batch: int, lat_h: int, lat_w: int, run):
         """run() under the ControlNet that sample()'s keyword arguments ask for (none: the engine is detached)."""
         from .controlnet import control_request
+        ip = ip_request(kwargs, batch)
+        if ip is not None and ip.adapter.base_cfg != self.unet.cfg:
+            raise ValueError(f"ip_adapter was built for {ip.adapter.base_cfg.name}, this solver runs "
+                             f"{self.unet.cfg.name} (IP-Adapter: SD v1.5 and SDXL)")
         self._control = control_request(kwargs, batch, 8 * lat_h, 8 * lat_w, self.device)
+        if ip is not None:  # the engine's set-up (bind_control) attaches it; without one it detaches any adapter
+            self.unet.ip_request = ip
         try:
             return run()
         finally:
             self._control = None
+            if ip is not None:
+                self.unet.ip_request = None
 
     def _control_entries(self, steps):
         """The conditioning scale of every entry of `steps`, or None when uncontrolled."""

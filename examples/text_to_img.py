@@ -76,9 +76,17 @@ def main():
     parser.add_argument("--controlnet_scale", type=float, default=1.0)
     parser.add_argument("--control_guidance_start", type=float, default=0.0)
     parser.add_argument("--control_guidance_end", type=float, default=1.0)
+    parser.add_argument("--ip_adapter", type=str, default=None, metavar="PATH",
+                        help="IP-Adapter checkpoint (.bin / .safetensors); any other name: seeded synthetic weights")
+    parser.add_argument("--ip_adapter_image", type=Path, default=None, help="the reference image of --ip_adapter")
+    parser.add_argument("--ip_adapter_scale", type=float, default=1.0)
+    parser.add_argument("--image_encoder", type=Path, default=None, metavar="DIR",
+                        help="the adapter's CLIP image encoder (config.json + model.safetensors); default: synthetic")
     args = parser.parse_args()
     if (args.controlnet is None) != (args.control_image is None):
         raise SystemExit("--controlnet and --control_image go together")
+    if (args.ip_adapter is None) != (args.ip_adapter_image is None):
+        raise SystemExit("--ip_adapter and --ip_adapter_image go together")
     if args.denoising_end is not None and args.model != "sdxl":
         raise SystemExit("--denoising_end needs --model sdxl")
 
@@ -105,6 +113,12 @@ def main():
                    "controlnet_conditioning_scale": args.controlnet_scale,
                    "control_guidance_start": args.control_guidance_start,
                    "control_guidance_end": args.control_guidance_end}
+    if args.ip_adapter is not None:
+        from PIL import Image
+        from cfgpp_b200.ip_adapter import IPAdapter
+        control.update(ip_adapter=IPAdapter(args.ip_adapter, args.device, solver.cfg,
+                                            image_encoder=str(args.image_encoder) if args.image_encoder else None),
+                       ip_adapter_image=Image.open(args.ip_adapter_image), ip_adapter_scale=args.ip_adapter_scale)
     if sdxl:
         refiner = {}
         if args.denoising_end is not None:

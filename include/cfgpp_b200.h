@@ -236,6 +236,39 @@ int cfgpp_set_control_scales(cfgpp_handle* h, const float* scales_host, int nste
 int cfgpp_controlnet_embed(cfgpp_handle* cn, const void* image_dev, int dtype, int batch, int height, int width,
                            void* out_dev, void* stream);
 
+/* ---- IP-Adapter (Ye et al. 2023; diffusers ImageProjection + IPAdapterAttnProcessor2_0): a reference image as a
+ * prompt, on a UNet handle. Weights, under diffusers' UNet-side keys:
+ *   image_proj.proj.{weight,bias}  [n_tokens * D, E], [n_tokens * D]   (D = cross_attention_dim, E = image embed width)
+ *   image_proj.norm.{weight,bias}  [D]
+ *   {block}.attn2.processor.to_k_ip.0.weight, {block}.attn2.processor.to_v_ip.0.weight  [C, D] for every cross-attention
+ *   block of the UNet ({block} = e.g. down_blocks.1.attentions.0.transformer_blocks.0; the original checkpoints'
+ *   `ip_adapter.{i}` index maps to it in diffusers' attn_processors order, cfgpp_b200/ip_adapter.py).
+ * Per UNet call, with tokens = LayerNorm_D(rows of fp16(embeds W_proj^T + b_proj)) [2*batch * n_tokens, D] projected
+ * once per image (K2 = tokens W_k_ip^T, V2 = tokens W_v_ip^T, fp16), every attn2 computes
+ *   out = fp16(O_txt / l_txt + s * O_ip / l_ip)
+ * in one kernel: the text softmax attention and the image softmax attention (each with its own max and sum) summed in
+ * fp32 and rounded once (diffusers rounds each term to fp16 first), then to_out as before. s = 0 gives the plain
+ * cross-attention bit for bit. An attached ControlNet sees the text context only. -------------------------------- */
+/* After cfgpp_finalize_weights, any number of times (a key loaded again replaces its tensor); fails naming a key that
+ * is not one of the above, has no cross-attention block, or whose shape differs from the block's to_k. Loading drops
+ * the image projection (call cfgpp_set_ip_image_embeds again); loading a key a second time also drops the prepared
+ * plan. The UNet's own weights are untouched. */
+int cfgpp_ip_adapter_load_weight(cfgpp_handle* h, const char* key, const void* data_dev, const int64_t* shape, int ndim,
+                                 int dtype, void* stream);
+/* Attach the loaded adapter (n_tokens 1..64, image_embed_dim E a multiple of 8) or detach it (cfgpp_ip_adapter_clear;
+ * its weights stay loaded). Either drops the prepared plan: the next cfgpp_prepare builds every attn2 with or without
+ * the image segment; without an adapter the plan is exactly the one built before any adapter was attached. */
+int cfgpp_ip_adapter_attach(cfgpp_handle* h, int n_tokens, int image_embed_dim);
+int cfgpp_ip_adapter_clear(cfgpp_handle* h);
+/* embeds_dev: (2*batch, E) fp16 device tensor, rows in cfgpp_set_prompt's order (the unconditional half: zeros, as
+ * diffusers' negative image embeds). Runs the image projection and every block's K2 / V2 projection now, into the
+ * plan's buffers; cfgpp_run_steps / cfgpp_unet_forward of a handle with an adapter fail until it has been called after
+ * the last cfgpp_prepare or weight load. */
+int cfgpp_set_ip_image_embeds(cfgpp_handle* h, const void* embeds_dev, void* stream);
+/* The scale s (1.0 after create): one fp32 device word every decoupled cross-attention launch reads, written on
+ * `stream`; never recaptures the step graph. */
+int cfgpp_set_ip_adapter_scale(cfgpp_handle* h, float scale, void* stream);
+
 /* ---- AutoencoderKL decoder (SURVEY.md section 8 f2): replaces `self.vae.decode(zt / scaling_factor).sample` of
  * latent_sdxl.py:155-164 (VAE madebyollin/sdxl-vae-fp16-fix, :44) and latent_diffusion.py:123-129 on the same conv /
  * GEMM / GroupNorm kernels. Weights under the diffusers AutoencoderKL keys (`post_quant_conv.*`, `decoder.*`). ----- */
@@ -301,6 +334,33 @@ int cfgpp_clip_encode(cfgpp_clip_handle* h, const int32_t* input_ids_dev, const 
                       int n_tokens, int skip, void* hidden_out, void* last_hidden_out, void* pooled_out, void* stream);
 int cfgpp_clip_stats(cfgpp_clip_handle* h, double* flops, size_t* workspace_bytes);
 
+/* ---- CLIP vision tower: transformers CLIPVisionModelWithProjection (IP-Adapter's image encoder: ViT-H/14 for SD v1.5,
+ * ViT-bigG/14 for SDXL). Weights under its keys (`vision_model.*`, `visual_projection.weight`). The patch conv runs as
+ * an unfold and a GEMM, the layers are the text towers' pre-LN loop with non-causal flash attention (heads zero-padded
+ * to a multiple of 64 columns), then post_layernorm of the CLS row and visual_projection. ----- */
+typedef struct cfgpp_clip_vision_desc {
+  int hidden_size;       /* 1280 (ViT-H) / 1664 (bigG) */
+  int intermediate_size; /* 5120 / 8192 */
+  int num_layers;        /* 32 / 48 */
+  int num_heads;         /* 16 (heads of 80 / 104) */
+  int image_size;        /* 224 */
+  int patch_size;        /* 14 */
+  int hidden_act;        /* 0 = quick_gelu, 1 = gelu */
+  int projection_dim;    /* 1024 / 1280 */
+  float layer_norm_eps;  /* 1e-5 */
+} cfgpp_clip_vision_desc;
+typedef struct cfgpp_clip_vision_handle cfgpp_clip_vision_handle;
+int cfgpp_clip_vision_create(const cfgpp_clip_vision_desc* desc, int device, cfgpp_clip_vision_handle** out);
+int cfgpp_clip_vision_destroy(cfgpp_clip_vision_handle* h);
+int cfgpp_clip_vision_load_weight(cfgpp_clip_vision_handle* h, const char* transformers_key, const void* data_dev,
+                                  const int64_t* shape, int ndim, int dtype, void* stream);
+int cfgpp_clip_vision_finalize_weights(cfgpp_clip_vision_handle* h, void* stream);
+/* pixel_values_dev: (batch 1..16, 3, image_size, image_size) NCHW of `dtype`, CLIPImageProcessor's output (rounded to
+ * fp16 as the fp16 model's conv input); image_embeds_out: (batch, projection_dim) fp16. */
+int cfgpp_clip_vision_encode(cfgpp_clip_vision_handle* h, const void* pixel_values_dev, int dtype, int batch,
+                             void* image_embeds_out, void* stream);
+int cfgpp_clip_vision_stats(cfgpp_clip_vision_handle* h, double* flops, size_t* workspace_bytes);
+
 /* ---- operator-level entry points (one kernel each; used by the kernel parity tests and micro-benchmarks) ----- */
 /* force_streamk (also in cfgpp_op_linear_lnfold): take the stream-K remainder split whenever its pieces are at least 2
  * k-blocks deep. The linear layers never take it otherwise; this lets tests reach the split's fix-up path. */
@@ -354,6 +414,14 @@ int cfgpp_op_conv_in_add(const void* z, int z_dtype, const float* in_scale_dev, 
  * (columns head_dim..P-1 must be zero in q / k / v and come back zero in out). */
 int cfgpp_op_attention(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out, int ldo, int B,
                        int H, int Nq, int Nkv, int head_dim, void* stream);
+/* Decoupled cross-attention (IP-Adapter): cfgpp_op_attention over (k, v) plus a second segment of Nkv2 = 1..64 image
+ * tokens k2 / v2 [B, Nkv2, H*P] (row strides ldk2 / ldv2) with a softmax of its own:
+ *   out = fp16(O1 / l1 + s * O2 / l2),  s = *ip_scale_dev (fp32, device, read by the kernel),
+ * summed in fp32 and rounded once, where diffusers rounds each term to fp16 first. s = 0 returns cfgpp_op_attention's
+ * output bit for bit. */
+int cfgpp_op_attention_ip(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, const void* k2,
+                          int ldk2, const void* v2, int ldv2, int Nkv2, const float* ip_scale_dev, void* out, int ldo,
+                          int B, int H, int Nq, int Nkv, int head_dim, void* stream);
 int cfgpp_op_groupnorm(const void* x1, int C1, const void* x2, int C2, int B, int HW, const void* gamma,
                        const void* beta, float eps, int silu, void* out, void* stream);
 int cfgpp_op_layernorm(const void* x, int M, int C, const void* gamma, const void* beta, float eps, void* out,
