@@ -525,6 +525,24 @@ def op_upsample2x(x: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def op_image_to_nhwc(x: torch.Tensor, Cp: int) -> torch.Tensor:
+    """The ControlNet conditioning image in: x [B,C,H,W] fp16 / fp32 -> [B,H,W,Cp] NHWC fp16, channels C..Cp-1 +0."""
+    lib = load()
+    B, C, H, W = x.shape
+    out = torch.empty((B, H, W, Cp), dtype=torch.float16, device=x.device)
+    check(lib.cfgpp_op_image_to_nhwc(ptr(x), c_int(dtype_code(x)), ptr(out), c_int(B), c_int(C), c_int(H), c_int(W),
+                                     c_int(Cp), stream_ptr()))
+    return out
+
+
+def op_silu(x: torch.Tensor) -> torch.Tensor:
+    """In place on fp16 x: fp16(x / (1 + expf(-x))), the SiLU of the ControlNet conditioning embedding."""
+    lib = load()
+    assert x.dtype == torch.float16
+    check(lib.cfgpp_op_silu(ptr(x), ctypes.c_size_t(x.numel()), stream_ptr()))
+    return x
+
+
 def op_vae_latent_prep(z: torch.Tensor, scaling: float, w: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
     """fp16(w @ fp16(z / scaling) + bias) per pixel: z [B,4,H,W] fp16 / fp32, w [4, 4] fp16 -> [B,4,H,W] fp16."""
     lib = load()
@@ -619,4 +637,28 @@ def op_clip_gather_rows(x: torch.Tensor, index: torch.Tensor, T: int) -> torch.T
     assert index.dtype == torch.int32 and BT == B * T
     out = torch.empty((B, D), dtype=torch.float16, device=x.device)
     check(lib.cfgpp_op_clip_gather_rows(ptr(x), ptr(index), ptr(out), c_int(B), c_int(T), c_int(D), stream_ptr()))
+    return out
+
+
+def op_clip_patchify(image: torch.Tensor, patch: int, Kp: int) -> torch.Tensor:
+    """CLIP vision patch rows: image [B,3,S,S] fp16 / fp32 -> [B*(S/patch)^2, Kp] fp16, column (c*P + ky)*P + kx,
+    columns 3*P*P..Kp-1 +0."""
+    lib = load()
+    B, C, S, S2 = image.shape
+    assert C == 3 and S == S2 and S % patch == 0
+    out = torch.empty((B * (S // patch) ** 2, Kp), dtype=torch.float16, device=image.device)
+    check(lib.cfgpp_op_clip_patchify(ptr(image), c_int(dtype_code(image)), ptr(out), c_int(B), c_int(S), c_int(patch),
+                                     c_int(Kp), stream_ptr()))
+    return out
+
+
+def op_clip_vision_embed(pe: torch.Tensor, cls: torch.Tensor, pos: torch.Tensor, B: int) -> torch.Tensor:
+    """CLIP vision embeddings: pe [B*np, D], cls [D], pos [np + 1, D] fp16 -> [B*(np + 1), D] fp16, row (b, 0) =
+    fp16(cls + pos[0]), row (b, 1 + p) = fp16(pe[b*np + p] + pos[1 + p])."""
+    lib = load()
+    T, D = pos.shape
+    assert pe.shape == (B * (T - 1), D) and cls.shape == (D,)
+    out = torch.empty((B * T, D), dtype=torch.float16, device=pe.device)
+    check(lib.cfgpp_op_clip_vision_embed(ptr(pe), ptr(cls), ptr(pos), ptr(out), c_int(B), c_int(T - 1), c_int(D),
+                                         stream_ptr()))
     return out

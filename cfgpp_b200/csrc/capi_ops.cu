@@ -329,4 +329,17 @@ CFGPP_API int cfgpp_op_upsample2x(const void* x, void* out, int B, int H, int W,
   return guarded([&] { run_upsample2x((const __half*)x, (__half*)out, B, H, W, C, (cudaStream_t)stream); });
 }
 
+CFGPP_API int cfgpp_op_image_to_nhwc(const void* x, int dtype, void* out, int B, int C, int H, int W, int Cp,
+                                     void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(dtype == CFGPP_F16 || dtype == CFGPP_F32, "image: fp16 or fp32");
+    CFGPP_REQUIRE(C >= 1 && Cp >= C, "the padded channel count must hold the image's channels");
+    run_image_to_nhwc(x, dtype == CFGPP_F16, (__half*)out, B, C, H, W, Cp, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_silu(void* x, size_t n, void* stream) {
+  return guarded([&] { run_silu((__half*)x, n, (cudaStream_t)stream); });
+}
+
 }  // extern "C"

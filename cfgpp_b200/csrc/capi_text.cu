@@ -110,4 +110,21 @@ CFGPP_API int cfgpp_op_clip_gather_rows(const void* x, const int32_t* index, voi
   });
 }
 
+CFGPP_API int cfgpp_op_clip_patchify(const void* image, int dtype, void* out, int B, int S, int P, int Kp,
+                                     void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(dtype == CFGPP_F16 || dtype == CFGPP_F32, "image: fp16 or fp32");
+    CFGPP_REQUIRE(P >= 1 && S % P == 0 && Kp >= 3 * P * P, "image size a multiple of the patch, Kp >= 3 P P");
+    run_clip_patchify(image, dtype == CFGPP_F16, (__half*)out, B, S, P, Kp, (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_op_clip_vision_embed(const void* pe, const void* cls, const void* pos, void* out, int B, int np,
+                                         int D, void* stream) {
+  return guarded([&] {
+    run_clip_vision_embed((const __half*)pe, (const __half*)cls, (const __half*)pos, (__half*)out, B, np, D,
+                          (cudaStream_t)stream);
+  });
+}
+
 }  // extern "C"

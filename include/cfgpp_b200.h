@@ -466,6 +466,11 @@ int cfgpp_op_v_to_eps(const void* v, const void* z, int z_dtype, const float* in
                       int n, void* stream);
 /* nearest 2x upsample: x [B,H,W,C] NHWC fp16 (C % 8 == 0) -> out [B,2H,2W,C]. */
 int cfgpp_op_upsample2x(const void* x, void* out, int B, int H, int W, int C, void* stream);
+/* ControlNet conditioning image in: x [B,C,H,W] fp16 / fp32 (dtype) -> out [B,H,W,Cp] NHWC fp16, channels C..Cp-1
+ * +0. */
+int cfgpp_op_image_to_nhwc(const void* x, int dtype, void* out, int B, int C, int H, int W, int Cp, void* stream);
+/* In-place SiLU on n fp16 values: x = fp16(x / (1 + expf(-x))) in fp32. */
+int cfgpp_op_silu(void* x, size_t n, void* stream);
 /* AutoencoderKL decoder front: z [B,4,HW] of z_dtype -> fp16(w . fp16(z / scaling) + bias), w [4][4], out [B,4,HW]. */
 int cfgpp_op_vae_latent_prep(const void* z, int z_dtype, float scaling, const void* w, const void* bias, void* out,
                              int B, int HW, void* stream);
@@ -490,6 +495,13 @@ int cfgpp_op_clip_attention(const void* qkv, void* out, int B, int T, int heads,
 int cfgpp_op_clip_activation(void* x, size_t n, int mode, void* stream);
 /* out[b] = x[b * T + index[b]], x [B*T, D] fp16, out [B, D]. */
 int cfgpp_op_clip_gather_rows(const void* x, const int32_t* index, void* out, int B, int T, int D, void* stream);
+/* CLIP vision patch rows: image [B,3,S,S] fp16 / fp32 (dtype) -> out [B*(S/P)^2, Kp] fp16, row (b, py, px), column
+ * (c*P + ky)*P + kx, columns 3*P*P..Kp-1 +0. */
+int cfgpp_op_clip_patchify(const void* image, int dtype, void* out, int B, int S, int P, int Kp, void* stream);
+/* CLIP vision embeddings: out[b, 0] = fp16(cls + pos[0]), out[b, 1 + p] = fp16(pe[b*np + p] + pos[1 + p]); pe [B*np, D],
+ * cls [D], pos [np + 1, D], out [B*(np + 1), D], all fp16. */
+int cfgpp_op_clip_vision_embed(const void* pe, const void* cls, const void* pos, void* out, int B, int np, int D,
+                               void* stream);
 
 #ifdef __cplusplus
 }

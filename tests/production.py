@@ -1,8 +1,8 @@
 """The production sizes every per-element kernel pin derives its cases from, and the attention launches of a UNet.
 
 `test_gpu_gemm.py`, `test_gpu_norms.py` and `test_gpu_attention.py` walk these tables through their derivation
-functions; `test_production_lists_cpu.py` asserts that every full-size model and text tower is listed, so a model added
-to `config.CONFIGS` without sizes fails on any machine."""
+functions; `test_production_lists_cpu.py` asserts that every full-size model, text tower, vision tower, ControlNet-capable
+UNet and IP-Adapter is listed, so a model added without sizes fails on any machine."""
 
 # latent (h, w) per full-size UNet config of `config.CONFIGS`: the native resolution first, then the non-square sizes
 # whose levels are not multiples of 64 tokens (1216x832: 76x52 = 3952 tokens at level 1, 19x13 at level 3;
@@ -20,6 +20,24 @@ VAE_SIZES = ((1024, 1024), (1216, 832), (768, 768), (768, 512), (512, 512))
 
 # text towers of `text_encoder.CLIP_CONFIGS` and the prompt batches they run at (M = 77·B)
 TEXT_TOWERS = {"clip_l": (1, 2, 8), "clip_bigg": (1, 2, 8), "clip_h": (1, 2, 8)}
+
+# the UNets that take a ControlNet (every UNET_SIZES entry but the SDXL refiner, which refuses one) at the same latent
+# sizes; the conditioning embedding runs at the image size (8x the latent) for 1 image and the engine's maximum of 8
+CONTROLNET_SIZES = {
+    "sdxl": ((128, 128), (152, 104)),
+    "sd15": ((64, 64),),
+    "sd2": ((96, 96), (96, 64)),
+    "sd2_base": ((64, 64),),
+}
+CONTROL_IMAGE_BATCHES = (1, 8)
+
+# IP-Adapters: (base UNet, image-embedding width E): SD v1.5 with ViT-H (1024), SDXL with the default ViT-bigG tower
+# (1280) and the ViT-H adapters for SDXL (1024); each projects one image embedding to IP_TOKENS image tokens
+IP_ADAPTERS = (("sd15", 1024), ("sdxl", 1280), ("sdxl", 1024))
+IP_TOKENS = 4
+
+# CLIP vision towers of `vision_encoder` (`<name>_config`) and the image batches they encode
+VISION_TOWERS = {"vit_h": (1, 2, 8), "vit_bigg": (1, 2, 8)}
 
 N_CTX = 77
 
@@ -60,3 +78,13 @@ def unet_attn_launches(cfg, h, w, NB=4):
             for j in range(lpb + 1):
                 transformer(f"up_blocks.{i}.attentions.{j}", L - 1 - i)
     return out
+
+
+def controlnet_sizes():
+    """(model, h, w) over CONTROLNET_SIZES, in table order."""
+    return [(m, h, w) for m, sizes in CONTROLNET_SIZES.items() for h, w in sizes]
+
+
+def vision_config(tower):
+    from cfgpp_b200 import vision_encoder as V
+    return getattr(V, f"{tower}_config")()

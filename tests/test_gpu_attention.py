@@ -231,6 +231,42 @@ def test_production_shapes(NB, H, Nq, Nkv, hd, name):
     check(f"{name} NB{NB} H{H} {Nq}x{Nkv} hd{hd}", q, k, v, H, hd)
 
 
+def vision_production_lists():
+    """{(tower, B): [(case id, (B, heads, T, head_dim))]}: the non-causal self-attention of every CLIP vision tower of
+    `production.VISION_TOWERS` (T = (image_size / patch_size)² + 1 tokens) at each image batch."""
+    import production as P
+    out = {}
+    for tower, batches in P.VISION_TOWERS.items():
+        v = P.vision_config(tower)
+        H, T = v.num_attention_heads, v.num_positions
+        for B in batches:
+            s = (B, H, T, v.hidden_size // H)
+            out[(tower, B)] = [(f"{tower}-B{B}-H{H}-{T}x{T}-hd{s[3]}", s)]
+    return out
+
+
+def _vision_cases():
+    seen, cases = set(), []
+    for shapes in vision_production_lists().values():
+        for cid, s in shapes:
+            if s not in seen:
+                seen.add(s)
+                cases.append(pytest.param(*s, id=cid))
+    return cases
+
+
+@pytest.mark.parametrize("name", ["flat", "peaked"])
+@pytest.mark.parametrize("B,H,T,hd", _vision_cases())
+def test_vision_tower_shapes(B, H, T, hd, name):
+    """The CLIP vision towers' self-attention (ViT-H: heads of 80, ViT-bigG: heads of 104, both padded to 128 columns)
+    over 257 tokens (four full KV tiles and one of a single key), reading q / k / v as column slices of the fused
+    [B·257, 3·Cp] buffer the qkv GEMM writes."""
+    hdp = padded(hd)
+    g = gen(B * 100003 + T * 1009 + hd + (name == "peaked"))
+    q, k, v = fused(*(heads(t, hdp) for t in family(name, g, B, T, T, H, hd)))
+    check(f"vision {name} B{B} H{H} {T}x{T} hd{hd}", q, k, v, H, hd)
+
+
 # ---- cases of the earlier rel-L2 tests, under the per-element gate -----------------------------------------------
 
 def rnd(g, *s, scale=1.0):
@@ -280,7 +316,7 @@ def attention(q, k, v, H, hd):
     return nv.op_attention(q, k, v, H, head_dim=hd)
 
 
-@pytest.mark.parametrize("hd", HEAD_DIMS)
+@pytest.mark.parametrize("hd", HEAD_DIMS + (104,))
 def test_known_answer_uniform_keys(hd):
     """Every key row is the same and every value row is the same row v0: all scores of a query row are equal, every p
     is 1 and the output is v0 bit for bit. The logits are small (std ≈ 0.3) and of both signs, so one padding key of
@@ -297,7 +333,7 @@ def test_known_answer_uniform_keys(hd):
             assert torch.equal(out, v0.expand(B, Nq, H * hdp)), f"hd{hd} {Nq}x{Nkv}: output != v0"
 
 
-@pytest.mark.parametrize("hd", HEAD_DIMS)
+@pytest.mark.parametrize("hd", HEAD_DIMS + (104,))
 def test_known_answer_one_hot(hd):
     """One key ≈ 70 nats above every other (≥ 47 above the 'warm' keys, ≈ 68 above the rest): every other p is below
     e^-40 and rounds to 0 in fp16, so the output is that key's value row bit for bit. The hot key sits at column 0, in

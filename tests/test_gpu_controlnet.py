@@ -57,12 +57,25 @@ def test_scaled_residual_epilogue_bit_exact(M, C, s):
 # ---------------------------------------------------------------------------------------------------------------
 # conv_in + addend
 # ---------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("B,H,W,C", [(1, 64, 64, 320), (2, 16, 24, 64)])
+def _conv_in_cases():
+    """The earlier shapes, then every latent size of `production.CONTROLNET_SIZES` at C0 = 320 for 2 images."""
+    import production as P
+    cases = [(1, 64, 64, 320), (2, 16, 24, 64)]
+    for _, h, w in P.controlnet_sizes():
+        if (2, h, w, 320) not in cases:
+            cases.append((2, h, w, 320))
+    return cases
+
+
+@pytest.mark.parametrize("B,H,W,C", _conv_in_cases())
 def test_conv_in_with_addend(B, H, W, C):
-    """fp16(fp16(conv_in(z)) + addend) on every repetition: against fp64 with the stated rounding, and bit for bit
-    against today's conv_in followed by the fp16 add."""
+    """fp16(fp16(conv_in(z)) + addend) on every repetition, per element against fp64: the fp32 sum of 36 products and
+    the bias (37 roundings in a fixed order, E_acc = 38·u·(Σ|w·x| + |b|)), ½ ulp for the conv's fp16 rounding, then
+    the add (u·|ref| and its ½ ulp); and bit for bit against conv_in followed by the fp16 add."""
     from cfgpp_b200 import _native as nv
-    g = torch.Generator().manual_seed(11)
+    from test_gpu_norms import Gate, ulp16
+    u = 2.0 ** -24
+    g = torch.Generator().manual_seed(11 + B * H + W)
     z = torch.randn(B, 4, H, W, generator=g).to(dev)
     w = (torch.randn(C, 4, 3, 3, generator=g) * 0.3).half().to(dev)
     bias = (torch.randn(C, generator=g) * 0.1).half().to(dev)
@@ -71,11 +84,16 @@ def test_conv_in_with_addend(B, H, W, C):
     plain = nv.op_conv_in(z, w.reshape(C, 36), bias, reps=2)
     want = (plain.float() + torch.cat([addend] * 2).float()).half()
     assert torch.equal(got, want)
-    conv64 = torch.nn.functional.conv2d(z.half().double(), w.double(), bias.double(), padding=1).permute(0, 2, 3, 1)
-    ref = (conv64.half().double() + addend.double()).half()
-    # fp32 accumulation vs fp64: the conv may round to the neighbouring fp16 value before the add
-    err = (got[:B].double() - ref.double()).abs()
-    assert (err <= 2 * torch.finfo(torch.float16).eps * ref.double().abs().clamp(min=1.0)).all()
+    assert torch.equal(got[:B], got[B:]), "the two repetitions differ"
+    zh = z.half().double()
+    conv64 = torch.nn.functional.conv2d(zh, w.double(), bias.double(), padding=1).permute(0, 2, 3, 1)
+    mag = torch.nn.functional.conv2d(zh.abs(), w.double().abs(), bias.double().abs(), padding=1).permute(0, 2, 3, 1)
+    e_t = 38 * u * mag
+    e_t = e_t + 0.5 * ulp16(conv64.abs() + e_t)
+    ref = conv64 + addend.double()
+    gate = Gate(f"conv_in+addend {B}x{H}x{W} C{C}")
+    gate.add(got[:B].double(), ref, e_t + u * ref.abs())
+    gate.done("controlnet")
 
 
 # ---------------------------------------------------------------------------------------------------------------

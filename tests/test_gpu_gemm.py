@@ -182,8 +182,11 @@ def geglu_cols(N):
 
 # ------------------------------------------------------------------------------------------------ the two gates
 
-def check_bound(what, out, blocks, w, M, bias=None, addend=None, rpg=1, sched=None, geglu=False, signed=False):
-    """Family B: every element of out [M, n_out] within E of fp64 (module docstring). Returns the worst |err|/E."""
+def check_bound(what, out, blocks, w, M, bias=None, addend=None, rpg=1, sched=None, geglu=False, signed=False,
+                scale=None):
+    """Family B: every element of out [M, n_out] within E of fp64 (module docstring). Returns the worst |err|/E. With
+    `scale` s (the scaled-residual epilogue, fp16(addend + fp16(fp16(t)·s))) the addend terms follow
+      E_s = |s|·E_t + u·|s·ref_t| + ½·ulp16(|s·ref_t| + |s|·E_t),   ref = s·ref_t + addend."""
     assert torch.isfinite(out).all(), f"{what}: non-finite output"
     sk = bool(sched and sched["streamk"])
     gate = Gate(what)
@@ -202,6 +205,9 @@ def check_bound(what, out, blocks, w, M, bias=None, addend=None, rpg=1, sched=No
             bound = ea * (G.abs() + e_ge) + a.abs() * e_ge + U * (a.abs() + ea) * (G.abs() + e_ge)
         elif addend is not None:
             e_t = e_t + 0.5 * ulp16(pre.abs() + e_t)
+            if scale is not None:
+                pre = scale * pre
+                e_t = abs(scale) * e_t + U * pre.abs() + 0.5 * ulp16(pre.abs() + abs(scale) * e_t)
             ref = pre + addend_rows(addend, rpg, r0, r1).double()
             bound = e_t + U * ref.abs()
         else:
@@ -215,8 +221,10 @@ def check_bound(what, out, blocks, w, M, bias=None, addend=None, rpg=1, sched=No
     return worst
 
 
-def check_exact(what, out, blocks, w, M, bias=None, addend=None, rpg=1, geglu=False, limit=2048.0, finite=True):
-    """Family A: out [M, n_out] bit-identical to the fp16 rounding chain of the exact (fp64) integer result."""
+def check_exact(what, out, blocks, w, M, bias=None, addend=None, rpg=1, geglu=False, limit=2048.0, finite=True,
+                scale=None):
+    """Family A: out [M, n_out] bit-identical to the fp16 rounding chain of the exact (fp64) integer result (with
+    `scale` s: fp16(addend + fp16(fp32(fp16(exact + bias))·s)))."""
     if finite:
         assert torch.isfinite(out).all(), f"{what}: non-finite output"
     bad, mx = 0, 0.0
@@ -227,6 +235,8 @@ def check_exact(what, out, blocks, w, M, bias=None, addend=None, rpg=1, geglu=Fa
             vi, gi = geglu_cols(w.shape[0])
             t = (t[:, vi].float() * t[:, gi].float()).half()
         elif addend is not None:
+            if scale is not None:
+                t = (t.float() * torch.tensor(scale, dtype=torch.float32, device=dev)).half()
             t = (t.float() + addend_rows(addend, rpg, r0, r1).float()).half()
         o = out[r0:r1]
         neq = ~((o == t) | (torch.isnan(o) & torch.isnan(t)))
@@ -340,6 +350,23 @@ def run_conv(what, x, w, *, bias=None, addend=None, rpg=1, stride=1, pad=1, forc
     else:
         check_bound(f"{tag} [{family}]", out, blocks, w, M, bias, addend, rpg, sched)
     return out, sched
+
+
+def run_scaled_residual(what, a, w, bias, addend, s, family=None):
+    """Launch op_linear_scaled_residual in place into `addend` with s an fp32 device word, read its schedule, gate it."""
+    from cfgpp_b200 import _native as nv
+    M = a.shape[0]
+    s32 = torch.tensor([s], dtype=torch.float32, device=dev)
+    add0 = addend.clone()
+    sched = nv.linear_schedule(a, w, bias, addend)
+    nv.op_linear_scaled_residual(a, w, addend, s32, bias, out=addend)
+    record(sched, {"scaled_residual"})
+    tag = f"{what} s {s} BN{sched['bn']} grid {sched['grid']} tiles {sched['tiles']} scaled_residual in place"
+    if family is None:
+        check_exact(tag, addend, linear_kblocks(a), w, M, bias, add0, scale=s32.item())
+    else:
+        check_bound(f"{tag} [{family}]", addend, linear_kblocks(a), w, M, bias, add0, sched=sched, scale=s32.item())
+    return addend
 
 
 def assert_gelu_identity(values):
@@ -864,10 +891,115 @@ def clip_gemm_launches(cfg, B):
             dict(name=f"{cfg.name} fc2", kind="linear", M=M, N=D, K=I, addend="residual")]
 
 
+# layout keys of the ControlNet and vision-tower launches: the real channel counts of a zero-padded convolution, the
+# real K of the patch GEMM, the (heads, head_dim) of head-padded q|k|v rows or out_proj columns
+EXTRA_KEYS = ("cin_real", "cout_real", "k_real", "vit_heads", "ip_heads")
+
+
+def pad64(c):
+    return -(-c // 64) * 64
+
+
+def controlnet_body_launches(cfg, h, w, NB=4):
+    """The GEMM / conv launches of a ControlNet's body (its down blocks and mid block, the UNet's shapes) on an h x w
+    latent: `unet_gemm_launches` without the up path, the tail and the prompt plan, and with the time-embedding rows of
+    the ControlNet's own resnets (down and mid only), so the temb row stride is the ControlNet's."""
+    ch, L, lpb = cfg.block_out_channels, len(cfg.block_out_channels), cfg.layers_per_block
+    order = [f"down_blocks.{i}.resnets.{j}" for i in range(L) for j in range(lpb)]
+    order += ["mid_block.resnets.0", "mid_block.resnets.1"]
+    widths = [ch[i] for i in range(L) for _ in range(lpb)] + [ch[-1], ch[-1]]
+    off, tot = {}, 0
+    for n, c in zip(order, widths):
+        off[n] = tot
+        tot += c
+    out = []
+    for l in unet_gemm_launches(cfg, h, w, NB):
+        if l.get("plan") == "prompt" or not l["name"].startswith(("down_blocks.", "mid_block.")):
+            continue
+        l = dict(l)
+        if l.get("addend") == "temb":
+            l.update(ld_add=tot, temb_off=off[l["name"].rsplit(".", 1)[0]])
+        out.append(l)
+    return out
+
+
+def controlnet_embed_launches(cn_cfg, h, w, B):
+    """The conditioning embedding's convolutions on B images of 8h x 8w, as `Unet::cond_embed` issues them: NHWC
+    activations and weights with the channels zero-padded to whole 64-wide K blocks (`pack_conv3x3_padded`), stride 2
+    with pad 1 on blocks.1 / 3 / 5, conv_out to the unpadded C0."""
+    ch, C0 = cn_cfg.conditioning_embedding_out_channels, cn_cfg.unet.block_out_channels[0]
+    H, W, out = 8 * h, 8 * w, []
+
+    def conv(name, cin, cout, cout_p, stride):
+        nonlocal H, W
+        out.append(dict(name=f"controlnet_cond_embedding.{name}", kind="conv", B=B, H=H, W=W, Cin=pad64(cin),
+                        Cout=cout_p, stride=stride, pad=1, cin_real=cin, cout_real=cout,
+                        flops=2.0 * B * (H // stride) * (W // stride) * cout * 9 * cin))
+        H, W = H // stride, W // stride
+
+    conv("conv_in", cn_cfg.conditioning_channels, ch[0], pad64(ch[0]), 1)
+    for i in range(len(ch) - 1):
+        conv(f"blocks.{2 * i}", ch[i], ch[i], pad64(ch[i]), 1)
+        conv(f"blocks.{2 * i + 1}", ch[i], ch[i + 1], pad64(ch[i + 1]), 2)
+    conv("conv_out", ch[-1], C0, C0, 1)
+    assert (H, W) == (h, w)
+    return out
+
+
+def zero_conv_launches(cn_cfg, h, w, NB=4):
+    """The zero convs of `Unet::build_control_plan`: per ControlNet residual k (`residual_channels` order, the last one
+    the mid block's) a 1x1 convolution as a linear over the residual's NB·HW rows, N = K = C, with the scaled-residual
+    epilogue in place into the UNet's skip tensor."""
+    ch, L, lpb = cn_cfg.unet.block_out_channels, len(cn_cfg.unet.block_out_channels), cn_cfg.unet.layers_per_block
+    H, W, hw = h, w, [h * w]
+    for i in range(L):
+        hw += [H * W] * lpb
+        if i != L - 1:
+            H, W = H // 2, W // 2
+            hw.append(H * W)
+    hw.append(H * W)
+    res = cn_cfg.residual_channels
+    assert len(res) == len(hw)
+    names = [f"controlnet_down_blocks.{k}" for k in range(len(res) - 1)] + ["controlnet_mid_block"]
+    return [dict(name=n, kind="linear", M=NB * p, N=C, K=C, addend="scaled_residual", flops=2.0 * NB * p * C * C)
+            for n, C, p in zip(names, res, hw)]
+
+
+def vision_gemm_launches(vcfg, tower, B):
+    """The vision tower's GEMMs at B images, as `ClipVisionEncoder::encode` and `build_clip_layers` issue them: the
+    patch GEMM (K = 3·P² zero-padded to whole k blocks, no bias), q|k|v into heads zero-padded to 64-multiples
+    (N = 3·Cp, bias), out_proj over the padded head columns (K = Cp, residual), fc1, fc2 (residual)."""
+    D, I, H, P = vcfg.hidden_size, vcfg.intermediate_size, vcfg.num_attention_heads, vcfg.patch_size
+    hd = D // H
+    Cp, K = H * pad64(hd), 3 * P * P
+    npch = (vcfg.image_size // P) ** 2
+    M = B * (npch + 1)
+    return [dict(name=f"{tower} patch_embedding", kind="linear", M=B * npch, N=D, K=pad64(K), bias=False, k_real=K),
+            dict(name=f"{tower} qkv", kind="linear", M=M, N=3 * Cp, K=D, vit_heads=(H, hd)),
+            dict(name=f"{tower} out_proj", kind="linear", M=M, N=D, K=Cp, addend="residual", vit_heads=(H, hd)),
+            dict(name=f"{tower} fc1", kind="linear", M=M, N=I, K=D),
+            dict(name=f"{tower} fc2", kind="linear", M=M, N=D, K=I, addend="residual")]
+
+
+def ip_adapter_gemm_launches(cfg, E, n_tokens, NB=4):
+    """An IP-Adapter's GEMMs in the UNet's image plan at UNet batch NB: image_proj.proj (M = NB, N = n_tokens·D, K = E,
+    bias), then per transformer block attn2.to_kv_ip (M = NB·n_tokens, N = 2·Cp over heads zero-padded to 64-multiples,
+    K = D, no bias)."""
+    import production as P
+    D = cfg.cross_attention_dim
+    out = [dict(name="image_proj.proj", kind="linear", M=NB, N=n_tokens * D, K=E)]
+    for l in P.unet_attn_launches(cfg, 8, 8):  # the block list does not depend on the latent size
+        if l["name"].endswith(".attn2.sdpa"):
+            H, hd = l["heads"], l["hd"]
+            out.append(dict(name=l["name"][:-len(".sdpa")] + ".to_kv_ip", kind="linear", M=NB * n_tokens,
+                            N=2 * H * pad64(hd), K=D, bias=False, ip_heads=(H, hd)))
+    return out
+
+
 def signature(l):
     keys = ("kind", "B", "H", "W", "Cin", "Cout", "stride", "pad", "M", "N", "K", "addend", "k_split", "geglu",
             "bias", "softmax", "ld_add")
-    return tuple(l.get(k) for k in keys)
+    return tuple(l.get(k) for k in keys) + tuple((k, l[k]) for k in EXTRA_KEYS if k in l)
 
 
 def unique_launches(launches):
@@ -898,6 +1030,30 @@ def production_lists():
     for tower, batches in P.TEXT_TOWERS.items():
         for B in batches:
             out[(tower, B)] = [(f"B{B}-{l['name']}", l) for l in clip_gemm_launches(CLIP_CONFIGS[tower](), B)]
+    out.update(controlnet_production_lists())
+    for tower, batches in P.VISION_TOWERS.items():
+        for B in batches:
+            out[(tower, B)] = [(f"B{B}-{l['name']}", l) for l in vision_gemm_launches(P.vision_config(tower), tower, B)]
+    for m, E in P.IP_ADAPTERS:
+        out[("ip_adapter", m, E)] = [(f"ip-{m}-E{E}-{i}-{l['name']}", l) for i, l in
+                                     enumerate(unique_launches(ip_adapter_gemm_launches(C.CONFIGS[m](), E, P.IP_TOKENS)))]
+    return out
+
+
+def controlnet_production_lists():
+    """{("controlnet", model, size): [(case id, launch)]}: per controlled model and latent size, the ControlNet body,
+    the zero convs and the conditioning embedding at every image batch of CONTROL_IMAGE_BATCHES."""
+    import production as P
+    from cfgpp_b200 import config as C, controlnet as CN
+    out = {}
+    for m, h, w in P.controlnet_sizes():
+        cfg = C.CONFIGS[m]()
+        cn_cfg = CN.controlnet_config(cfg)
+        launches = controlnet_body_launches(cfg, h, w) + zero_conv_launches(cn_cfg, h, w)
+        for B in P.CONTROL_IMAGE_BATCHES:
+            launches += [dict(l, name=f"B{B} {l['name']}") for l in controlnet_embed_launches(cn_cfg, h, w, B)]
+        out[("controlnet", m, (h, w))] = [(f"cn-{P.size_tag(m, h, w)}-{i}-{l['name']}", l)
+                                         for i, l in enumerate(unique_launches(launches))]
     return out
 
 
@@ -928,6 +1084,14 @@ def run_production(l, family):
             x = torch.randn(B, H, W, Cin, generator=g, device=dev).half()
             w = (torch.randn(Cout, 9 * Cin, generator=g, device=dev) * (9 * Cin) ** -0.5).half()
             b = torch.randn(Cout, generator=g, device=dev).half()
+        if "cin_real" in l:  # zero-padded channels: +0 inputs, zero weight rows / columns and bias entries
+            ci, co = l["cin_real"], l["cout_real"]
+            x[..., ci:] = 0
+            w = w.reshape(Cout, 9, Cin)
+            w[:, :, ci:] = 0
+            w[co:] = 0
+            w = w.reshape(Cout, 9 * Cin)
+            b[co:] = 0
         addend, rpg = None, 1
         mk = (lambda *s: int_vec(g, *s)) if exact else (lambda *s: torch.randn(*s, generator=g, device=dev).half())
         if l.get("addend") == "temb":  # the resnet's column slice of the time-embedding rows of all resnets
@@ -935,7 +1099,9 @@ def run_production(l, family):
             addend, rpg = temb_all[:, l["temb_off"]:l["temb_off"] + Cout], (H // s) * (W // s)
         elif l.get("addend") == "residual":
             addend = mk(Mo, Cout)
-        run_conv(name, x, w, bias=b, addend=addend, rpg=rpg, stride=s, pad=l["pad"], family=family)
+        out, _ = run_conv(name, x, w, bias=b, addend=addend, rpg=rpg, stride=s, pad=l["pad"], family=family)
+        if "cout_real" in l:
+            assert (out[:, l["cout_real"]:].view(torch.int16) == 0).all(), f"{name}: padded channels are not +0"
         return
     M, N, K = l["M"], l["N"], l["K"]
     geglu = bool(l.get("geglu"))
@@ -953,7 +1119,25 @@ def run_production(l, family):
             w, b = pack_geglu(w, b)
         if not l.get("bias", True):
             b = None
+    if "k_real" in l:  # the patch GEMM: columns K_real..K-1 of A and W zero
+        a[:, l["k_real"]:] = 0
+        w[:, l["k_real"]:] = 0
+    for key in ("vit_heads", "ip_heads"):
+        if key in l:  # rows (q|k|v, K‖V) or columns (out_proj) of every head's padding zero
+            H, hd = l[key]
+            if K == H * pad64(hd):
+                a[:, (torch.arange(K, device=dev) % pad64(hd)) >= hd] = 0
+                w[:, (torch.arange(K, device=dev) % pad64(hd)) >= hd] = 0
+            else:
+                pad_rows = (torch.arange(N, device=dev) % pad64(hd)) >= hd
+                w[pad_rows] = 0
+                if b is not None:
+                    b[pad_rows] = 0
     mk = (lambda *s: int_vec(g, *s)) if exact else (lambda *s: torch.randn(*s, generator=g, device=dev).half())
+    if l.get("addend") == "scaled_residual":  # a ControlNet zero conv, at two conditioning scales
+        for sc in (0.37, 2.0):
+            run_scaled_residual(name, a, w, b, mk(M, N), sc, family=family)
+        return
     a2 = None
     if l.get("k_split"):  # the dual-source shortcut: h and the skip connection, two buffers
         a, a2 = a[:, :l["k_split"]].contiguous(), a[:, l["k_split"]:].contiguous()
@@ -982,18 +1166,27 @@ def test_vae_pv_softmax_families():
                        w, bias=b, family="softmax")
 
 
-def check_launch_lists_against_profile(model, h, w):
+def check_launch_lists_against_profile(model, h, w, controlnet=False):
     """Build the native UNet (synthetic weights) at batch 2 on an h x w latent, profile one forward and compare its
     GEMM entries (kinds 0 / 1) with `unet_gemm_launches` and its attention entries (kind 2) with
-    `production.unet_attn_launches`: the same names, kinds and algorithmic FLOPs."""
+    `production.unet_attn_launches`: the same names, kinds and algorithmic FLOPs. With `controlnet`, a ControlNet is
+    attached: its `controlnet:` entries must equal `controlnet_body_launches` and the zero convs `zero_conv_launches`."""
     import production as P
-    from cfgpp_b200 import config as C, weights as Wt
+    from cfgpp_b200 import config as C, controlnet as CN, weights as Wt
     from cfgpp_b200.engine import NativeUNet
     cfg = C.CONFIGS[model]()
     sd = Wt.synthetic_state_dict(cfg, seed=3, device=dev)
     net = NativeUNet(cfg, sd, dev)
+    cn = None
+    if controlnet:
+        cn_cfg = CN.controlnet_config(cfg)
+        cn = CN.NativeControlNet(cn_cfg, CN.synthetic_controlnet_state_dict(cn_cfg, seed=4, device=dev), dev)
     try:
+        if cn is not None:
+            net.attach_controlnet(cn)
         net.prepare(2, h, w)
+        if cn is not None:
+            net.set_control_image(torch.rand(2, 3, 8 * h, 8 * w, generator=torch.Generator().manual_seed(1)).to(dev))
         g = torch.Generator().manual_seed(0)
         ctx = torch.randn(4, 77, cfg.cross_attention_dim, generator=g).half().to(dev)
         if cfg.addition_embed_type == "text_time":
@@ -1007,9 +1200,27 @@ def check_launch_lists_against_profile(model, h, w):
             net.set_prompt(ctx)
         prof = net.profile_forward(torch.randn(2, 4, h, w, generator=g).to(dev), 500.0)
     finally:
+        if cn is not None:
+            cn.close()
         net.close()
         del sd
         torch.cuda.empty_cache()
+    cnp = "controlnet:"
+    if controlnet:
+        got = sorted((n[len(cnp):], "conv" if k == 1 else "linear", f) for n, k, f, _ in prof
+                     if k in (0, 1) and n.startswith(cnp))
+        want = sorted((l["name"], l["kind"], l["flops"]) for l in controlnet_body_launches(cfg, h, w))
+        assert len(got) == len(want), f"{len(got)} ControlNet GEMM launches reported, {len(want)} derived"
+        for x, y in zip(got, want):
+            assert x[:2] == y[:2] and abs(x[2] - y[2]) <= 1e-9 * y[2], f"ControlNet: reported {x}, derived {y}"
+        zc = zero_conv_launches(cn_cfg, h, w)
+        got = sorted((n, "conv" if k == 1 else "linear", f) for n, k, f, _ in prof
+                     if k in (0, 1) and n.startswith("controlnet_"))
+        want = sorted((l["name"], l["kind"], l["flops"]) for l in zc)
+        assert len(got) == len(want), f"{len(got)} zero convs reported, {len(want)} derived"
+        for x, y in zip(got, want):
+            assert x[:2] == y[:2] and abs(x[2] - y[2]) <= 1e-9 * y[2], f"zero conv: reported {x}, derived {y}"
+        prof = [e for e in prof if not e[0].startswith((cnp, "controlnet_"))]
     got = sorted((n, "conv" if k == 1 else "linear", f) for n, k, f, _ in prof if k in (0, 1))
     want = sorted((l["name"], l["kind"], l["flops"]) for l in unet_gemm_launches(cfg, h, w)
                   if l.get("plan") != "prompt")
@@ -1021,7 +1232,8 @@ def check_launch_lists_against_profile(model, h, w):
     assert len(got) == len(want), f"{len(got)} attention launches reported, {len(want)} derived"
     for x, y in zip(got, want):
         assert x[0] == y[0] and abs(x[1] - y[1]) <= 1e-9 * y[1], f"reported {x}, derived {y}"
-    print(f"[gemm] {model} {8 * w}x{8 * h}: {len(prof)} profiled launches, GEMM and attention lists match")
+    print(f"[gemm] {model} {8 * w}x{8 * h}{' + ControlNet' if controlnet else ''}: {len(prof)} profiled launches, "
+          f"GEMM and attention lists match")
 
 
 @pytest.mark.parametrize("model,hw", [("tiny_sdxl", 32), ("tiny_sd15", 32), ("sdxl", 128)])
@@ -1040,11 +1252,18 @@ def test_unet_launch_list_matches_profile_rect(model, h, w):
     check_launch_lists_against_profile(model, h, w)
 
 
+@pytest.mark.parametrize("model,hw", [("tiny_sd15", 32), ("tiny_sdxl", 32), ("sdxl", 128)])
+def test_controlnet_launch_list_matches_profile(model, hw):
+    """With a ControlNet attached: its body's `controlnet:` entries equal `controlnet_body_launches`, the zero convs
+    equal `zero_conv_launches` (name, kind, FLOPs), and the UNet's own entries still equal its derived lists."""
+    check_launch_lists_against_profile(model, hw, hw, controlnet=True)
+
+
 # ================================================================================================= coverage (last)
 
 def test_zz_coverage():
     """Over the module: every tile width, both conv A-tile modes, natural and forced stream-K, tiles of >= 3 pieces and
-    every addend mode ran under the per-element gates."""
+    every addend mode (the ControlNet zero convs' scaled residual included) ran under the per-element gates."""
     if SEEN["cases"] < 500:
         pytest.skip(f"only {SEEN['cases']} gated launches ran: coverage is asserted over the whole module")
     print(f"[gemm coverage] {SEEN['cases']} gated launches: BN {sorted(SEEN['bn'])}, A tile {sorted(SEEN['a_mode'])}, "
@@ -1054,4 +1273,4 @@ def test_zz_coverage():
     assert SEEN["a_mode"] >= {"linear", "tiled", "im2col"}
     assert SEEN["streamk"] >= {None, "natural", "forced"}
     assert SEEN["pieces3"] > 0
-    assert SEEN["addend"] >= {"none", "residual", "temb_staged", "temb_rows"}
+    assert SEEN["addend"] >= {"none", "residual", "temb_staged", "temb_rows", "scaled_residual"}

@@ -534,3 +534,50 @@ def test_layernorm(M, Cc):
 def test_layernorm_mean_offset():
     """Rows whose mean is 100 times their std (the kernel is two-pass: no cancellation in the variance)."""
     check_layernorm(4096, 1280, 100)
+
+
+# ------------------------------------------------------------------------------------------------ LayerNorm launches
+
+def layernorm_production_lists():
+    """{key: [(case id, (M, C))]}: every LayerNorm launch of the text towers (layer_norm1 / 2 and final_layer_norm
+    at M = 77·B), the vision towers (pre_layrnorm and the layers' norms at M = 257·B, post_layernorm over the B class
+    rows) and an IP-Adapter's image_proj.norm (M = NB·tokens rows of width D at UNet batch NB = 4)."""
+    import production as P
+    from cfgpp_b200 import config as C
+    from cfgpp_b200.text_encoder import CLIP_CONFIGS
+    out = {}
+    for tower, batches in P.TEXT_TOWERS.items():
+        D = CLIP_CONFIGS[tower]().hidden_size
+        for B in batches:
+            out[(tower, B)] = [(f"{tower}-B{B}-layer_norm", (P.N_CTX * B, D))]
+    for tower, batches in P.VISION_TOWERS.items():
+        v = P.vision_config(tower)
+        for B in batches:
+            out[(tower, B)] = [(f"{tower}-B{B}-layer_norm", (v.num_positions * B, v.hidden_size)),
+                               (f"{tower}-B{B}-post_layernorm", (B, v.hidden_size))]
+    for m, E in P.IP_ADAPTERS:
+        D = C.CONFIGS[m]().cross_attention_dim
+        out[("ip_adapter", m, E)] = [(f"ip-{m}-image_proj.norm", (4 * P.IP_TOKENS, D))]
+    return out
+
+
+def _layernorm_cases():
+    seen, cases = set(), []
+    for launches in layernorm_production_lists().values():
+        for cid, s in launches:
+            if s not in seen:
+                seen.add(s)
+                cases.append(pytest.param(*s, id=cid))
+    return cases
+
+
+@pytest.mark.parametrize("M,C", _layernorm_cases())
+def test_layernorm_production_launches(M, C):
+    """Every LayerNorm launch of the text and vision towers and the IP-Adapter projection, per element against fp64:
+    rows with their own mean (up to 30σ) and scale; from 14 rows on every 7th row constant (exactly fp16(β))."""
+    g = gen(M * 7 + C)
+    every = 7 if M >= 14 else 0
+    x, gamma, beta = ln_inputs(g, M, C, 30, const_every=every)
+    out = ln_check(f"production M{M} C{C}", x, gamma, beta)
+    if every:
+        assert torch.equal(out[::7], beta.expand_as(out[::7])), "constant row: not exactly β"

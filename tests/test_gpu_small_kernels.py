@@ -156,7 +156,9 @@ REFINER_TEMB_TOTAL = temb_total(sdxl_refiner_config())
 @pytest.mark.parametrize("R", [1, 2, 7, 16])
 @pytest.mark.parametrize("K,N", [(320, 1000), (1280, 1280), (2816, 1000), (1280, SDXL_TEMB_TOTAL),
                                  # the SDXL refiner: time_embedding.linear_1 / _2, add_embedding.linear_1, time_emb_proj
-                                 (384, 1536), (1536, 1536), (2560, 1536), (1536, REFINER_TEMB_TOTAL)])
+                                 (384, 1536), (1536, 1536), (2560, 1536), (1536, REFINER_TEMB_TOTAL),
+                                 # the CLIP vision towers' visual_projection: ViT-H 1280 -> 1024, ViT-bigG 1664 -> 1280
+                                 (1280, 1024), (1664, 1280)])
 def test_small_linear(R, K, N):
     from cfgpp_b200 import _native as nv
     g = torch.Generator().manual_seed(R * 131 + K + N)

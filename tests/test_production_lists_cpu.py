@@ -1,6 +1,6 @@
 """The production size table (`production.py`) and the per-element case lists derived from it, checked without a GPU:
-every full-size UNet config and every text tower has sizes, and the GEMM / conv, attention and GroupNorm case lists
-cover every (model, size). A model added to `config.CONFIGS` or `text_encoder.CLIP_CONFIGS` without sizes fails here,
+every full-size UNet config, text tower, vision tower, ControlNet-capable UNet and IP-Adapter has sizes, and the GEMM /
+conv, attention, GroupNorm and LayerNorm case lists cover every (model, size). A model added to `config.CONFIGS` or `text_encoder.CLIP_CONFIGS` without sizes fails here,
 on any machine, before its kernels go unpinned."""
 import pytest
 
@@ -63,6 +63,7 @@ def assert_covered(what, lists, run, key_of):
 
 def test_gemm_cases_cover_every_model_and_size():
     lists = TG.production_lists()
+    lists = {k: v for k, v in lists.items() if k[0] not in ("controlnet", "ip_adapter") and k[0] not in P.VISION_TOWERS}
     assert set(lists) == expected_keys()
     run = {TG.signature(p.values[0]) for p in TG._production_cases()}
     assert_covered("GEMM", lists, run, lambda e: TG.signature(e[1]))
@@ -108,3 +109,106 @@ def test_new_levels_reach_the_lists(model):
     if model in ("sdxl", "sdxl_refiner"):
         tall = [s for _, s in TA.production_lists()[(model, (152, 104))]]
         assert any(s[1] == 3952 for s in tall)
+
+
+# ------------------------------------------------------------------------------------------------ ControlNet, IP-Adapter, vision towers
+
+REQUIRED_CONTROL_BATCHES = {1, 8}
+REQUIRED_IP = {("sd15", 1024), ("sdxl", 1280), ("sdxl", 1024)}
+NO_CONTROLNET = {"sdxl_refiner"}  # the refiner refuses a ControlNet
+
+
+def test_every_vision_tower_listed():
+    from cfgpp_b200 import vision_encoder as V
+    towers = {n[:-len("_config")] for n in dir(V) if n.endswith("_config") and callable(getattr(V, n))}
+    missing = [t for t in full_size(towers) if not P.VISION_TOWERS.get(t)]
+    assert not missing, f"vision towers without image batches: {missing}"
+    for t, batches in P.VISION_TOWERS.items():
+        assert {1, 2, 8} <= set(batches), f"{t}: image batches {batches}"
+
+
+def test_every_controlnet_unet_has_sizes():
+    capable = [m for m in full_size(C.CONFIGS) if m not in NO_CONTROLNET]
+    for m in capable:
+        assert set(P.CONTROLNET_SIZES.get(m, ())) == set(P.UNET_SIZES[m]), f"{m}: ControlNet sizes differ from its sizes"
+    assert not NO_CONTROLNET & set(P.CONTROLNET_SIZES), "the refiner takes no ControlNet"
+    assert set(P.CONTROLNET_SIZES) == set(capable)
+    assert REQUIRED_CONTROL_BATCHES <= set(P.CONTROL_IMAGE_BATCHES)
+
+
+def test_every_ip_adapter_listed():
+    assert REQUIRED_IP <= set(P.IP_ADAPTERS) and P.IP_TOKENS == 4
+
+
+def test_controlnet_and_vision_gemm_lists_run():
+    lists = TG.production_lists()
+    want = {("controlnet", m, (h, w)) for m, h, w in P.controlnet_sizes()}
+    want |= {(t, B) for t, batches in P.VISION_TOWERS.items() for B in batches}
+    want |= {("ip_adapter", m, E) for m, E in P.IP_ADAPTERS}
+    assert want <= set(lists)
+    run = {TG.signature(p.values[0]) for p in TG._production_cases()}
+    assert_covered("GEMM", {k: lists[k] for k in want}, run, lambda e: TG.signature(e[1]))
+    kinds = {l.get("addend") for k in want if k[0] == "controlnet" for _, l in lists[k]}
+    assert "scaled_residual" in kinds
+
+
+@pytest.mark.parametrize("model", sorted(P.CONTROLNET_SIZES))
+def test_conditioning_embedding_launches_match_param_specs(model):
+    """One padded conv per `controlnet_cond_embedding.*` weight, with its Cin, Cout and stride (2 on blocks.1 / 3 / 5)."""
+    from cfgpp_b200 import controlnet as CN
+    cn_cfg = CN.controlnet_config(C.CONFIGS[model]())
+    specs = {k[:-len(".weight")]: shape for k, shape, _ in CN.controlnet_param_specs(cn_cfg)
+             if k.startswith("controlnet_cond_embedding.") and k.endswith(".weight")}
+    for h, w in P.CONTROLNET_SIZES[model]:
+        for B in P.CONTROL_IMAGE_BATCHES:
+            got = {l["name"]: l for l in TG.controlnet_embed_launches(cn_cfg, h, w, B)}
+            assert set(got) == set(specs)
+            for name, (cout, cin, kh, kw) in specs.items():
+                l = got[name]
+                assert (l["cin_real"], l["cout_real"], kh, kw) == (cin, cout, 3, 3), name
+                assert l["Cin"] == TG.pad64(cin) and l["Cout"] >= cout and l["Cout"] % 64 == 0 and l["B"] == B
+                assert l["stride"] == (2 if name.endswith(("blocks.1", "blocks.3", "blocks.5")) else 1), name
+            assert got["controlnet_cond_embedding.conv_in"]["H"] == 8 * h
+        zc = TG.zero_conv_launches(cn_cfg, h, w)
+        zspec = {k[:-len(".weight")]: s for k, s, _ in CN.controlnet_param_specs(cn_cfg)
+                 if k.startswith(("controlnet_down_blocks.", "controlnet_mid_block")) and k.endswith(".weight")}
+        assert {l["name"]: (l["N"], l["K"]) for l in zc} == {k: s[:2] for k, s in zspec.items()}
+
+
+@pytest.mark.parametrize("model,E", sorted(REQUIRED_IP))
+def test_to_kv_ip_launches_match_adapter_keys(model, E):
+    """The derived to_kv_ip launches are one per cross-attention block, with K = D and N = 2·Cp for the block's width C
+    (the rows of its to_k_ip weight); image_proj.proj takes the E-wide embedding to IP_TOKENS tokens."""
+    from cfgpp_b200 import ip_adapter as IP
+    cfg = C.CONFIGS[model]()
+    sd = IP.synthetic_ip_adapter(cfg, E, P.IP_TOKENS)
+    blocks = IP.processor_blocks(cfg)
+    launches = TG.ip_adapter_gemm_launches(cfg, E, P.IP_TOKENS)
+    proj, kv = launches[0], launches[1:]
+    assert (proj["name"], proj["N"], proj["K"]) == ("image_proj.proj", tuple(sd["image_proj.proj.weight"].shape)[0], E)
+    want = {blocks[i]: sd[f"ip_adapter.{i}.to_k_ip.weight"].shape for i in blocks}
+    got = {l["name"][:-len(".attn2.to_kv_ip")]: l for l in kv}
+    assert set(got) == set(want)
+    for b, (Cb, D) in want.items():
+        H, hd = got[b]["ip_heads"]
+        assert H * hd == Cb and got[b]["K"] == D == cfg.cross_attention_dim and got[b]["N"] == 2 * H * TG.pad64(hd)
+
+
+def test_layernorm_cases_cover_every_tower_and_adapter():
+    lists = TN.layernorm_production_lists()
+    want = {(t, B) for t, batches in P.TEXT_TOWERS.items() for B in batches}
+    want |= {(t, B) for t, batches in P.VISION_TOWERS.items() for B in batches}
+    want |= {("ip_adapter", m, E) for m, E in P.IP_ADAPTERS}
+    assert set(lists) == want
+    run = {tuple(c.values[:2]) for c in TN._layernorm_cases()}
+    assert_covered("LayerNorm", lists, run, lambda e: e[1])
+    widths = {c for v in lists.values() for _, (M, c) in v}
+    assert {768, 1280, 1024, 1664, 2048} <= widths
+
+
+def test_vision_attention_cases_listed():
+    lists = TA.vision_production_lists()
+    assert set(lists) == {(t, B) for t, batches in P.VISION_TOWERS.items() for B in batches}
+    run = {tuple(p.values) for p in TA._vision_cases()}
+    assert_covered("vision attention", lists, run, lambda e: e[1])
+    assert {s[3] for v in lists.values() for _, s in v} == {80, 104}
