@@ -1,4 +1,6 @@
-// cfgpp_b200 — flash-style attention forward on sm_90a tensor cores (mma.sync m16n8k16). See attention.cuh.
+// cfgpp_b200 — flash-style attention forward on sm_90a tensor cores. See attention.cuh.
+// Padded head dim 64 runs on the warp-specialised wgmma kernel attn64_kernel further down; head dims 128 and 192 on
+// attn_kernel<HD> (mma.sync m16n8k16):
 //
 // One CTA = one 64-row query tile of one (batch, head), 4 warps of 16 query rows each, looping over 64-row KV tiles:
 //   thread 0 : TMA producer (Q once; K / V into a 2-deep ring, 128B swizzle, mbarrier complete_tx)
@@ -9,6 +11,7 @@
 // zero-filled by the TMA and its columns are masked to -inf. Head dims of 40 / 80 / 160 arrive zero-padded to 64 / 128
 // / 192 columns; the padding columns of V are zero, so those of the output are too.
 #include <cmath>
+#include <type_traits>
 
 #include "attention.cuh"
 #include "common.cuh"
@@ -293,6 +296,294 @@ attn_ip_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, co
   attn_body<HD, true>(p, &map_q, &map_k, &map_v, &map_k2, &map_v2);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Head dim 64 (padded): warp-specialised wgmma kernel. One CTA = one 128-row query tile of one (batch, head), 384
+// threads, 1 CTA / SM:
+//   warpgroups 0, 1 : consumers; warpgroup g owns query rows [64 g, 64 g + 64). S = Q K^T is wgmma m64n128k16 with
+//                     both operands in shared memory (K-major, 128B swizzle); the online softmax runs on the fp32
+//                     accumulator, whose per-warp layout is the m16n8 fragment of the mma.sync kernel above (same
+//                     rounding points); P rounded to fp16 is the register A operand of O += P V (wgmma m64n64k16,
+//                     V an MN-major B operand).
+//   warpgroup 2     : one thread issues TMA: Q once, then K / V as 128-row tiles into a W_STAGES-deep ring
+//                     (full / empty mbarriers, no CTA-wide barrier in the loop).
+// Each consumer issues S_j together with P_{j-1} V_{j-1} as one wgmma group, then runs the softmax of S_j. Two named
+// barriers hand the tensor pipe back and forth between the warpgroups, so one warpgroup's softmax runs under the
+// other's GEMMs. Every wgmma group is retired before the softmax: none stays in flight across the loop.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int W_BQ = 128;
+constexpr int W_BKV = 128;
+constexpr int W_STAGES = 4;
+constexpr int W_THREADS = 384;
+constexpr int W_KV_BYTES = 2 * ATOM_BYTES;  // one 128-row K or V tile: two 64-row TMA boxes
+constexpr int W_SMEM_BYTES = 2 * ATOM_BYTES + W_STAGES * 2 * W_KV_BYTES + 1024 + 256;
+static_assert(W_SMEM_BYTES <= 232448, "shared memory overflow");
+constexpr int kTurnBar = 1;  // named barriers kTurnBar + g: warpgroup g may issue its wgmma group
+
+// IP: the image tokens' K / V arrive as one more ring fill (64-row boxes, p.Nkv2 valid rows, TMA zero fill past
+// them; the slot's rows 64..127 are left from an earlier fill or never written). S over that slot reads them but the
+// mask replaces those columns, and PV runs over rows 0..63 only, which the fill wrote (zeros past Nkv2).
+template <bool IP>
+CFGPP_DEVICE void attn64_body(const AttnParams& p, const CUtensorMap* map_q, const CUtensorMap* map_k,
+                              const CUtensorMap* map_v, const CUtensorMap* map_k2, const CUtensorMap* map_v2) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+  uint8_t* sQ = smem;                            // [128 rows x 64]: warpgroup g reads atom g
+  uint8_t* sK = sQ + 2 * ATOM_BYTES;             // W_STAGES x [128 rows x 64]
+  uint8_t* sV = sK + W_STAGES * W_KV_BYTES;      // W_STAGES x [128 rows x 64]
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(sV + W_STAGES * W_KV_BYTES);
+  uint64_t* full = q_full + 1;                   // [W_STAGES]
+  uint64_t* empty = full + W_STAGES;             // [W_STAGES]: one arrive per consumer warp
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int q0 = blockIdx.x * W_BQ;
+  const int head = blockIdx.y;
+  const int batch = blockIdx.z;
+  const int n_tiles = (p.Nkv + W_BKV - 1) / W_BKV;
+
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int s = 0; s < W_STAGES; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_launch_dependents();
+  pdl_wait();
+  const float ip_scale = IP ? *p.ip_scale : 0.f;
+  const bool ip = IP && ip_scale != 0.f;  // uniform over the CTA
+
+  if (warp >= 8) {
+    // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 256) {
+      tma_prefetch_desc(map_q);
+      tma_prefetch_desc(map_k);
+      tma_prefetch_desc(map_v);
+      if (IP) {
+        tma_prefetch_desc(map_k2);
+        tma_prefetch_desc(map_v2);
+      }
+      mbar_arrive_expect_tx(q_full, 2 * ATOM_BYTES);
+      tma_load_3d(sQ, map_q, q_full, head * 64, q0, batch);
+      tma_load_3d(sQ + ATOM_BYTES, map_q, q_full, head * 64, q0 + 64, batch);
+      for (int f = 0; f < n_tiles + (IP ? 1 : 0); ++f) {
+        const int s = f % W_STAGES;
+        mbar_wait_nocall(&empty[s], ((f / W_STAGES) & 1) ^ 1);
+        uint8_t* k_dst = sK + s * W_KV_BYTES;
+        uint8_t* v_dst = sV + s * W_KV_BYTES;
+        if (IP && f == n_tiles) {
+          mbar_arrive_expect_tx(&full[s], 2 * ATOM_BYTES);
+          tma_load_3d(k_dst, map_k2, &full[s], head * 64, 0, batch);
+          tma_load_3d(v_dst, map_v2, &full[s], head * 64, 0, batch);
+        } else {
+          mbar_arrive_expect_tx(&full[s], 4 * ATOM_BYTES);
+          for (int h = 0; h < 2; ++h) {
+            tma_load_3d(k_dst + h * ATOM_BYTES, map_k, &full[s], head * 64, f * W_BKV + h * 64, batch);
+            tma_load_3d(v_dst + h * ATOM_BYTES, map_v, &full[s], head * 64, f * W_BKV + h * 64, batch);
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== consumers (warpgroups 0 and 1) =====================
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2;
+  const float c = p.scale_log2e;
+  // accumulator fragments: sc[8 n + e] / o[4 n + e] hold (row r, column 8 n + 2 (lane % 4) + e) for e < 2 and
+  // (row r + 8, same column) for e >= 2, r = 16 (warp % 4) + lane / 4 of the warpgroup's 64 rows
+  float sc[W_BKV / 2];
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  uint32_t pa[W_BKV / 4];  // P rounded to fp16: pa[2 n + h] packs sc[4 n + 2 h], sc[4 n + 2 h + 1]
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const uint64_t q_desc = make_wgmma_desc_sw128(smem_u32(sQ + wg * ATOM_BYTES));
+
+  auto issue_s = [&](int s) {
+    const uint64_t k_desc = make_wgmma_desc_sw128(smem_u32(sK + s * W_KV_BYTES));
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_f16<W_BKV>(sc, q_desc + 2 * k, k_desc + 2 * k, k != 0 ? 1u : 0u);
+  };
+  // acc += P V over the first ROWS rows of slot s
+  auto issue_pv = [&](float (&acc)[32], int s, auto rows) {
+    const uint64_t v_desc = make_wgmma_desc_sw128_mn(smem_u32(sV + s * W_KV_BYTES));
+#pragma unroll
+    for (int t = 0; t < decltype(rows)::value / 16; ++t) {
+      const uint32_t a[4] = {pa[4 * t], pa[4 * t + 1], pa[4 * t + 2], pa[4 * t + 3]};
+      wgmma_f16_rs_tb64(acc, a, v_desc + 128 * t, 1u);
+    }
+  };
+  // online softmax of sc (columns >= valid set to -inf) against the running (m, l); rescales acc, writes pa
+  auto softmax = [&](int valid, float (&m)[2], float (&l)[2], float (&acc)[32]) {
+    if (valid < W_BKV) {
+#pragma unroll
+      for (int n = 0; n < W_BKV / 8; ++n) {
+        const int col = n * 8 + 2 * (lane & 3);
+        if (col >= valid) sc[4 * n] = sc[4 * n + 2] = -INFINITY;
+        if (col + 1 >= valid) sc[4 * n + 1] = sc[4 * n + 3] = -INFINITY;
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int n = 0; n < W_BKV / 8; ++n) mx = fmaxf(mx, fmaxf(sc[4 * n + 2 * h], sc[4 * n + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m[h], mx);  // finite: every tile holds at least one valid column
+      alpha[h] = fast_exp2((m[h] - m_new) * c);
+      m[h] = m_new;
+    }
+    float rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int n = 0; n < W_BKV / 8; ++n) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float mc = m[h] * c;
+        const float p0 = fast_exp2(sc[4 * n + 2 * h] * c - mc);
+        const float p1 = fast_exp2(sc[4 * n + 2 * h + 1] * c - mc);
+        rs[h] += p0 + p1;
+        pa[2 * n + h] = pack_half2(p0, p1);
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l[h] = l[h] * alpha[h] + rs[h];  // per-lane partial; quad-reduced at the end
+#pragma unroll
+    for (int n = 0; n < 8; ++n) {
+      acc[4 * n] *= alpha[0];
+      acc[4 * n + 1] *= alpha[0];
+      acc[4 * n + 2] *= alpha[1];
+      acc[4 * n + 3] *= alpha[1];
+    }
+  };
+
+  mbar_wait_nocall(q_full, 0);
+  if (wg == 1) named_bar_arrive(kTurnBar, 256);  // warpgroup 0 issues first
+  // Step 0 issues S_0; step j in [1, n_tiles) issues S_j and P_{j-1} V_{j-1} as one group; the last step P V of the
+  // last tile. A warpgroup issues a step once the other has issued its previous one. No wgmma sits on a branch (a
+  // wgmma under a condition ptxas cannot prove uniform makes it serialise every wgmma of the kernel).
+  constexpr std::integral_constant<int, W_BKV> kAllRows{};
+  mbar_wait_nocall(&full[0], 0);
+  named_bar_sync(kTurnBar + wg, 256);
+  wgmma_fence();
+  issue_s(0);
+  wgmma_commit();
+  named_bar_arrive(kTurnBar + (wg ^ 1), 256);
+  wgmma_wait<0>();
+  fence_acc(sc);
+  softmax(p.Nkv, m_run, l_run, o);  // columns past Nkv: padding (last tile only)
+  for (int j = 1; j < n_tiles; ++j) {
+    const int s = j % W_STAGES;
+    const int sp = (j - 1) % W_STAGES;
+    mbar_wait_nocall(&full[s], (j / W_STAGES) & 1);
+    named_bar_sync(kTurnBar + wg, 256);
+    wgmma_fence();
+    issue_s(s);
+    issue_pv(o, sp, kAllRows);
+    wgmma_commit();
+    named_bar_arrive(kTurnBar + (wg ^ 1), 256);
+    wgmma_wait<0>();
+    fence_acc(sc);
+    fence_acc(o);
+    fence_acc(pa);
+    if (lane == 0) mbar_arrive(&empty[sp]);
+    softmax(p.Nkv - j * W_BKV, m_run, l_run, o);
+  }
+  const int s_last = (n_tiles - 1) % W_STAGES;
+  named_bar_sync(kTurnBar + wg, 256);
+  wgmma_fence();
+  issue_pv(o, s_last, kAllRows);
+  wgmma_commit();
+  if (wg == 0) named_bar_arrive(kTurnBar + 1, 256);  // warpgroup 1's last sync; its own first arrive balances ours
+  wgmma_wait<0>();
+  fence_acc(o);
+  fence_acc(pa);
+  if (lane == 0) mbar_arrive(&empty[s_last]);
+
+  float inv_l[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    inv_l[h] = 1.0f / l;
+  }
+  if constexpr (IP) {
+    // ---- the image tile: one ring fill, a softmax of its own (max and sum final before PV). It is computed at
+    // s = 0 as well (a branch around it would serialise the wgmmas) and dropped by the select below. ----
+    const int s = n_tiles % W_STAGES;
+    mbar_wait_nocall(&full[s], (n_tiles / W_STAGES) & 1);
+    wgmma_fence();
+    issue_s(s);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(sc);
+    float m2[2] = {-INFINITY, -INFINITY}, l2[2] = {0.f, 0.f};
+    float o2[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o2[i] = 0.f;
+    softmax(p.Nkv2, m2, l2, o2);
+    wgmma_fence();
+    issue_pv(o2, s, std::integral_constant<int, 64>{});  // the rows this fill wrote; P and V2 are zero past Nkv2
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(o2);
+    fence_acc(pa);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float l = l2[h];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      l2[h] = 1.0f / l;
+    }
+    // o = O1 / l1 + s * O2 / l2, rounded once below; s = 0 keeps the plain kernel's o / l1
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const float fold = o[i] * inv_l[(i >> 1) & 1] + ip_scale * (o2[i] * l2[(i >> 1) & 1]);
+      o[i] = ip ? fold : o[i];
+    }
+    if (ip) inv_l[0] = inv_l[1] = 1.0f;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int qrow = q0 + warp * 16 + (lane >> 2) + 8 * h;  // warp = 4 wg + warp % 4
+    if (qrow >= p.Nq) continue;
+    __half* dst = p.out + (static_cast<size_t>(batch) * p.Nq + qrow) * p.ldo + head * 64 + 2 * (lane & 3);
+#pragma unroll
+    for (int n = 0; n < 8; ++n)
+      *reinterpret_cast<uint32_t*>(dst + n * 8) = pack_half2(o[4 * n + 2 * h] * inv_l[h], o[4 * n + 2 * h + 1] * inv_l[h]);
+  }
+}
+
+__global__ void __launch_bounds__(W_THREADS, 1)
+attn64_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+              const __grid_constant__ CUtensorMap map_v) {
+  attn64_body<false>(p, &map_q, &map_k, &map_v, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(W_THREADS, 1)
+attn64_ip_kernel(const AttnParams p, const __grid_constant__ CUtensorMap map_q,
+                 const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+                 const __grid_constant__ CUtensorMap map_k2, const __grid_constant__ CUtensorMap map_v2) {
+  attn64_body<true>(p, &map_q, &map_k, &map_v, &map_k2, &map_v2);
+}
+
+void launch64(const AttnOp& op, cudaStream_t stream) {
+  dim3 grid((op.p.Nq + W_BQ - 1) / W_BQ, op.p.H, op.p.B);
+  if (op.p.ip_scale)
+    launch_pdl(attn64_ip_kernel, grid, dim3(W_THREADS), W_SMEM_BYTES, stream, op.p, op.map_q, op.map_k, op.map_v,
+               op.map_k2, op.map_v2);
+  else
+    launch_pdl(attn64_kernel, grid, dim3(W_THREADS), W_SMEM_BYTES, stream, op.p, op.map_q, op.map_k, op.map_v);
+}
+
 CUtensorMap make_head_map(const __half* base, int ld, int B, int N, int cols) {
   uint64_t dims[3] = {(uint64_t)cols, (uint64_t)N, (uint64_t)B};
   uint64_t strides[2] = {(uint64_t)ld * 2, (uint64_t)N * ld * 2};
@@ -356,7 +647,8 @@ AttnOp make_attn_ip_op(const __half* q, int ldq, const __half* k, int ldk, const
 void attn_configure() {
   static bool done = false;
   if (done) return;
-  configure_one<64>();
+  CFGPP_CHECK_CUDA(cudaFuncSetAttribute(attn64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W_SMEM_BYTES));
+  CFGPP_CHECK_CUDA(cudaFuncSetAttribute(attn64_ip_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W_SMEM_BYTES));
   configure_one<128>();
   configure_one<192>();
   done = true;
@@ -365,7 +657,7 @@ void attn_configure() {
 void run_attn_op(const AttnOp& op, cudaStream_t stream) {
   attn_configure();
   switch (op.hd_pad) {
-    case 64: return launch<64>(op, stream);
+    case 64: return launch64(op, stream);
     case 128: return launch<128>(op, stream);
     case 192: return launch<192>(op, stream);
     default: throw Error(-1, "unsupported padded head dim");

@@ -11,8 +11,9 @@
 //   out[b, i, h*P + :] = fp16( O1 / l1 + s * O2 / l2 ),   O / l = the unnormalised PV and the sum of each segment,
 // s = *ip_scale, an fp32 device word read by every launch (a captured graph follows it). The text half is the plain
 // kernel's arithmetic; the sum is formed in fp32 and rounded once. diffusers (IPAdapterAttnProcessor2_0) rounds each
-// term first: fp16(fp16(O_txt) + fp16(s * fp16(O_ip))); the two differ by at most an ulp or so of each term. s = 0 skips
-// the image tile (it is never loaded): the output is then the plain kernel's, bit for bit.
+// term first: fp16(fp16(O_txt) + fp16(s * fp16(O_ip))); the two differ by at most an ulp or so of each term. At s = 0
+// the output is the plain kernel's, bit for bit (head dims 128 / 192 skip the image tile; head dim 64 computes it and
+// drops it by a select).
 #pragma once
 #include "host.h"
 

@@ -151,6 +151,9 @@ CFGPP_DEVICE void tma_store_wait0() { asm volatile("cp.async.bulk.wait_group 0;"
 CFGPP_DEVICE void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+CFGPP_DEVICE void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // generic-proxy smem writes -> visible to the async proxy (wgmma / TMA reads)
 CFGPP_DEVICE void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -177,6 +180,12 @@ template <int N>
 CFGPP_DEVICE void fence_acc(float (&d)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// the same for A fragments a register-A wgmma reads: they stay live (unreused) until the wait that retires it
+template <int N>
+CFGPP_DEVICE void fence_acc(uint32_t (&a)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(a[i])::"memory");
 }
 
 // Shared-memory matrix descriptor (sm_90 wgmma), 128B swizzle, K-major operand whose K extent per tile row is exactly
@@ -244,6 +253,32 @@ CFGPP_DEVICE void wgmma_f16<256>(float (&d)[128], uint64_t a_desc, uint64_t b_de
                "}, %128, %129, p, 1, 1, 0, 0;\n}\n"
                : CFGPP_D8(0), CFGPP_D8(8), CFGPP_D8(16), CFGPP_D8(24), CFGPP_D8(32), CFGPP_D8(40), CFGPP_D8(48), CFGPP_D8(56), CFGPP_D8(64), CFGPP_D8(72), CFGPP_D8(80), CFGPP_D8(88), CFGPP_D8(96), CFGPP_D8(104), CFGPP_D8(112), CFGPP_D8(120)
                : "l"(a_desc), "l"(b_desc), "r"(scale_d)
+               : "memory");
+}
+
+// MN-major 128B-swizzle descriptor: the operand's rows run along K, each row holding 64 fp16 of N contiguously (a
+// [K rows x 64] tile as TMA writes it with SWIZZLE_128B, e.g. V for O += P V). 8-row K groups are 1024 B apart. The N
+// extent of one row is the whole swizzle atom, so the stride between atoms along N is never applied; both offset fields
+// carry the 1024 B group stride. Advancing 16 rows along K (2048 B) is +128 in the start-address field.
+CFGPP_DEVICE uint64_t make_wgmma_desc_sw128_mn(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
+  d |= static_cast<uint64_t>(1024 >> 4) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
+}
+
+// D[64 x 64] += A[64 x 16] * B[16 x 64], A from registers (the m16n8k16 A fragment of each warp's 16 rows: a[0] / a[1]
+// rows r / r + 8 at columns 2 (lane % 4) + {0, 1}, a[2] / a[3] the same rows 8 columns on), B an MN-major smem
+// descriptor (imm-trans-b = 1).
+CFGPP_DEVICE void wgmma_f16_rs_tb64(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\nwgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+               "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,"
+               "%27,%28,%29,%30,%31"
+               "}, {%32,%33,%34,%35}, %36, p, 1, 1, 1;\n}\n"
+               : CFGPP_D8(0), CFGPP_D8(8), CFGPP_D8(16), CFGPP_D8(24)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d)
                : "memory");
 }
 #undef CFGPP_D8
