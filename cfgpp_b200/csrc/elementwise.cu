@@ -498,8 +498,8 @@ void run_conv_in(const void* z, int z_is_half, const float* in_scale, const __ha
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// ControlNet conditioning embedding: the image in, a SiLU pass, and its 3x3 convolutions' weights zero-padded to
-// channel counts the implicit-GEMM convolution takes (exact: padded channels are zero in and zero out)
+// ControlNet conditioning embedding: the image in, with its channels zero-padded to the count the implicit-GEMM
+// convolution takes (exact: padded channels are zero in and zero out), and a SiLU pass
 // ------------------------------------------------------------------------------------------------------------
 __global__ void image_to_nhwc_kernel(const void* __restrict__ x, int x_is_half, __half* __restrict__ out, int B, int C,
                                      int HW, int Cp) {
@@ -526,20 +526,6 @@ __global__ void silu_kernel(__half* __restrict__ x, size_t n) {
   }
 }
 
-__global__ void pack_conv3x3_padded_kernel(const __half* __restrict__ w, const __half* __restrict__ bias,
-                                           __half* __restrict__ wp, __half* __restrict__ bp, int Cout, int Cin,
-                                           int Cout_p, int Cin_p) {
-  const size_t n = static_cast<size_t>(Cout_p) * 9 * Cin_p;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int c = i % Cin_p;
-    const int tap = (i / Cin_p) % 9;
-    const int o = i / (static_cast<size_t>(9) * Cin_p);
-    wp[i] = (o < Cout && c < Cin) ? w[(static_cast<size_t>(o) * Cin + c) * 9 + tap] : __float2half(0.f);
-    if (tap == 0 && c == 0) bp[o] = o < Cout ? bias[o] : __float2half(0.f);
-  }
-}
-
 void run_image_to_nhwc(const void* x, int x_is_half, __half* out, int B, int C, int H, int W, int Cp,
                        cudaStream_t stream) {
   const size_t n = static_cast<size_t>(B) * H * W * Cp;
@@ -549,13 +535,6 @@ void run_image_to_nhwc(const void* x, int x_is_half, __half* out, int B, int C, 
 
 void run_silu(__half* x, size_t n, cudaStream_t stream) {
   silu_kernel<<<grid_for(n), 256, 0, stream>>>(x, n);
-  CFGPP_CHECK_CUDA(cudaGetLastError());
-}
-
-void run_pack_conv3x3_padded(const __half* w, const __half* bias, __half* wp, __half* bp, int Cout, int Cin, int Cout_p,
-                             int Cin_p, cudaStream_t stream) {
-  const size_t n = static_cast<size_t>(Cout_p) * 9 * Cin_p;
-  pack_conv3x3_padded_kernel<<<grid_for(n), 256, 0, stream>>>(w, bias, wp, bp, Cout, Cin, Cout_p, Cin_p);
   CFGPP_CHECK_CUDA(cudaGetLastError());
 }
 

@@ -42,13 +42,11 @@ void run_conv_in(const void* z, int z_is_half, const float* in_scale, const __ha
                  const __half* bias, __half* out, int B, int H, int W, int Cout, int reps, cudaStream_t stream,
                  const __half* addend = nullptr);
 // ControlNet conditioning embedding helpers: image [B,C,H,W] NCHW (fp16 or fp32) -> fp16 NHWC [B,H,W,Cp] with zero
-// channels C..Cp-1; in-place fp16(SiLU(x)) over n values; a (Cout,Cin,3,3) weight and its bias -> [Cout_p][9][Cin_p]
-// and [Cout_p], zero beyond Cout / Cin.
+// channels C..Cp-1; in-place fp16(SiLU(x)) over n values. Its convolutions' weights and biases are zero-padded to
+// [Cout_p][9][Cin_p] and [Cout_p] by the weight store (WeightStore::packed_conv3x3 and packed_heads_rows).
 void run_image_to_nhwc(const void* x, int x_is_half, __half* out, int B, int C, int H, int W, int Cp,
                        cudaStream_t stream);
 void run_silu(__half* x, size_t n, cudaStream_t stream);
-void run_pack_conv3x3_padded(const __half* w, const __half* bias, __half* wp, __half* bp, int Cout, int Cin, int Cout_p,
-                             int Cin_p, cudaStream_t stream);
 
 enum StepMode : int {
   STEP_NONE = 0,        // only emit eps_uc / eps_c (the predict_noise seam)

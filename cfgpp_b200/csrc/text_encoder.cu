@@ -16,10 +16,23 @@ std::vector<std::vector<ClipStep>> build_clip_layers(const ClipLayerArgs& a, dou
   const size_t sD = D, sI = I;
   const float eps = a.eps;
   __half *x0 = a.x0, *x1 = a.x1, *ln = a.ln, *qkv = a.qkv, *att = a.att, *mlp = a.mlp;
-  const WeightStore& w = *a.weights;
+  const int hd = D / a.heads, qkv_n = 3 * a.heads * a.hdp, att_c = a.heads * a.hdp;
+  WeightStore& w = *a.weights;
   std::vector<std::vector<ClipStep>> plan;
   for (int l = 0; l < a.layers; ++l) {
     const std::string p = a.prefix + std::to_string(l) + ".";
+    const std::string q = p + "self_attn.q_proj", k = p + "self_attn.k_proj", v = p + "self_attn.v_proj",
+                      o = p + "self_attn.out_proj.weight";
+    for (const std::string& n : {q, k, v}) {  // sizes are checked before anything is packed from them
+      w.plain(n + ".weight", sD * sD);
+      w.plain(n + ".bias", sD);
+    }
+    w.plain(o, sD * sD);
+    // q | k | v as one operand (one GEMM instead of three) with every head zero-padded to hdp rows, and out_proj with
+    // hdp-wide head columns
+    const __half* qkv_w = w.packed_heads_rows({q + ".weight", k + ".weight", v + ".weight"}, a.heads, hd, a.hdp);
+    const __half* qkv_b = w.packed_heads_rows({q + ".bias", k + ".bias", v + ".bias"}, a.heads, hd, a.hdp);
+    const __half* out_w = w.packed_heads_cols(o, a.heads, hd, a.hdp);
     std::vector<ClipStep> steps;
     auto add_gemm = [&](const GemmOp& op) {
       *flops += op.flops();
@@ -29,12 +42,11 @@ std::vector<std::vector<ClipStep>> build_clip_layers(const ClipLayerArgs& a, dou
     const __half *g2 = w.plain(p + "layer_norm2.weight", sD), *b2 = w.plain(p + "layer_norm2.bias", sD);
     // x1 = x0 + out_proj(attention(q, k, v of LN1(x0)))
     steps.push_back([=](cudaStream_t st) { run_layernorm(x0, M, D, g1, b1, eps, ln, st); });
-    add_gemm(make_linear_op(ln, D, nullptr, 0, 0, a.qkv_w[l], M, a.qkv_n, D, a.qkv_b[l], nullptr, 0, 1, qkv, a.qkv_n,
-                            false));
+    add_gemm(make_linear_op(ln, D, nullptr, 0, 0, qkv_w, M, qkv_n, D, qkv_b, nullptr, 0, 1, qkv, qkv_n, false));
     const auto attention = a.attention;
     steps.push_back([=](cudaStream_t st) { attention(qkv, att, st); });
     *flops += a.attention_flops;
-    add_gemm(make_linear_op(att, a.att_c, nullptr, 0, 0, a.out_w[l], M, D, a.att_c,
+    add_gemm(make_linear_op(att, att_c, nullptr, 0, 0, out_w, M, D, att_c,
                             w.plain(p + "self_attn.out_proj.bias", sD), x0, D, 1, x1, D, false));
     // x0 = x1 + fc2(act(fc1(LN2(x1))))
     steps.push_back([=](cudaStream_t st) { run_layernorm(x1, M, D, g2, b2, eps, ln, st); });
@@ -68,26 +80,9 @@ void ClipTextEncoder::load_weight(const std::string& key, const void* data, cons
 
 void ClipTextEncoder::finalize_weights(cudaStream_t stream) {
   CFGPP_REQUIRE(!finalized_, "weights already finalized");
-  const size_t D = d_.hidden_size;
-  const std::string tm = "text_model.";
-  // q | k | v projections of a layer as one [3D][D] operand (one GEMM instead of three)
-  for (int l = 0; l < d_.num_layers; ++l) {
-    const std::string a = tm + "encoder.layers." + std::to_string(l) + ".self_attn.";
-    __half* w = weights_.alloc(3 * D * D);
-    __half* b = weights_.alloc(3 * D);
-    const char* names[3] = {"q_proj", "k_proj", "v_proj"};
-    for (int i = 0; i < 3; ++i) {
-      CFGPP_CHECK_CUDA(cudaMemcpyAsync(w + i * D * D, weights_.plain(a + names[i] + ".weight", D * D), D * D * sizeof(__half),
-                                       cudaMemcpyDeviceToDevice, stream));
-      CFGPP_CHECK_CUDA(cudaMemcpyAsync(b + i * D, weights_.plain(a + names[i] + ".bias", D), D * sizeof(__half),
-                                       cudaMemcpyDeviceToDevice, stream));
-    }
-    qkv_w_.push_back(w);
-    qkv_b_.push_back(b);
-  }
   CFGPP_CHECK_CUDA(cudaStreamSynchronize(stream));
   finalized_ = true;
-  try {  // structural validation: building a plan touches (and size-checks) every weight
+  try {  // structural validation: building a plan touches (size-checks and packs) every weight
     prepare(1, d_.max_positions);
   } catch (...) {
     finalized_ = false;
@@ -124,11 +119,9 @@ void ClipTextEncoder::prepare(int batch, int tokens) {
   weights_.plain(tm + "final_layer_norm.bias", sD);
   if (d_.projection_dim > 0) weights_.plain("text_projection.weight", static_cast<size_t>(d_.projection_dim) * sD);
   const int heads = d_.num_heads;
-  ClipLayerArgs a{&weights_, tm + "encoder.layers.", d_.num_layers, D, I, M, d_.hidden_act, d_.layer_norm_eps, 3 * D, D,
-                  qkv_w_, qkv_b_, {}, nullptr, 2.0 * NB * heads * static_cast<double>(T) * T * 64.0,  // causal: half
+  ClipLayerArgs a{&weights_, tm + "encoder.layers.", d_.num_layers, D, I, M, d_.hidden_act, d_.layer_norm_eps, heads, 64,
+                  nullptr, 2.0 * NB * heads * static_cast<double>(T) * T * 64.0,  // causal: half
                   x0_, x1_, ln_, qkv_, att_, mlp_};
-  for (int l = 0; l < d_.num_layers; ++l)
-    a.out_w.push_back(weights_.plain(tm + "encoder.layers." + std::to_string(l) + ".self_attn.out_proj.weight", sD * sD));
   a.attention = [=](const __half* qkv, __half* att, cudaStream_t st) { run_clip_attention(qkv, att, NB, T, heads, D, st); };
   layer_plan_ = build_clip_layers(a, &flops_);
   B_ = NB;
@@ -204,41 +197,12 @@ void ClipVisionEncoder::load_weight(const std::string& key, const void* data, co
 
 void ClipVisionEncoder::finalize_weights(cudaStream_t stream) {
   CFGPP_REQUIRE(!finalized_, "weights already finalized");
-  const size_t D = d_.hidden_size, H = d_.num_heads, hd = D / H, hdp = hdp_, K = 3 * d_.patch_size * d_.patch_size;
-  const std::string vm = "vision_model.";
-  // the patch conv as [D][Kp], K zero-padded to whole 64-wide k blocks
-  patch_w_ = weights_.alloc(D * Kp_);
-  CFGPP_CHECK_CUDA(cudaMemsetAsync(patch_w_, 0, D * Kp_ * sizeof(__half), stream));
-  CFGPP_CHECK_CUDA(cudaMemcpy2DAsync(patch_w_, Kp_ * sizeof(__half), weights_.plain(vm + "embeddings.patch_embedding.weight", D * K),
-                                     K * sizeof(__half), K * sizeof(__half), D, cudaMemcpyDeviceToDevice, stream));
-  // q | k | v with every head zero-padded to hdp rows (the flash kernel's layout), out_proj with hdp-wide head columns
-  for (int l = 0; l < d_.num_layers; ++l) {
-    const std::string a = vm + "encoder.layers." + std::to_string(l) + ".self_attn.";
-    __half* w = weights_.alloc(3 * H * hdp * D);
-    __half* b = weights_.alloc(3 * H * hdp);
-    __half* o = weights_.alloc(D * H * hdp);
-    CFGPP_CHECK_CUDA(cudaMemsetAsync(w, 0, 3 * H * hdp * D * sizeof(__half), stream));
-    CFGPP_CHECK_CUDA(cudaMemsetAsync(b, 0, 3 * H * hdp * sizeof(__half), stream));
-    CFGPP_CHECK_CUDA(cudaMemsetAsync(o, 0, D * H * hdp * sizeof(__half), stream));
-    const char* names[3] = {"q_proj", "k_proj", "v_proj"};
-    for (int i = 0; i < 3; ++i) {
-      const __half* sw = weights_.plain(a + names[i] + ".weight", D * D);
-      const __half* sb = weights_.plain(a + names[i] + ".bias", D);
-      for (size_t h = 0; h < H; ++h) {
-        CFGPP_CHECK_CUDA(cudaMemcpyAsync(w + ((i * H + h) * hdp) * D, sw + h * hd * D, hd * D * sizeof(__half),
-                                         cudaMemcpyDeviceToDevice, stream));
-        CFGPP_CHECK_CUDA(cudaMemcpyAsync(b + (i * H + h) * hdp, sb + h * hd, hd * sizeof(__half),
-                                         cudaMemcpyDeviceToDevice, stream));
-      }
-    }
-    CFGPP_CHECK_CUDA(cudaMemcpy2DAsync(o, hdp * sizeof(__half), weights_.plain(a + "out_proj.weight", D * D),
-                                       hd * sizeof(__half), hd * sizeof(__half), D * H, cudaMemcpyDeviceToDevice,
-                                       stream));
-    qkv_w_.push_back(w);
-    qkv_b_.push_back(b);
-    out_w_.push_back(o);
-  }
   CFGPP_CHECK_CUDA(cudaStreamSynchronize(stream));
+  // the patch conv as [D][Kp], K zero-padded to whole 64-wide k blocks
+  const int K = 3 * d_.patch_size * d_.patch_size;
+  const std::string patch = "vision_model.embeddings.patch_embedding.weight";
+  weights_.plain(patch, static_cast<size_t>(d_.hidden_size) * K);
+  patch_w_ = weights_.packed_heads_cols(patch, 1, K, Kp_);
   finalized_ = true;
   try {
     prepare(1);
@@ -282,9 +246,8 @@ void ClipVisionEncoder::prepare(int batch) {
   }
   weights_.plain("visual_projection.weight", static_cast<size_t>(d_.projection_dim) * sD);
   flops_ += 2.0 * NB * np_ * static_cast<double>(D) * 3 * d_.patch_size * d_.patch_size;
-  ClipLayerArgs a{&weights_, vm + "encoder.layers.", d_.num_layers, D, I, M, d_.hidden_act, d_.layer_norm_eps, 3 * Cp,
-                  Cp, qkv_w_, qkv_b_, out_w_, nullptr, 4.0 * NB * H * static_cast<double>(T) * T * hd,
-                  x0_, x1_, ln_, qkv_, att_, mlp_};
+  ClipLayerArgs a{&weights_, vm + "encoder.layers.", d_.num_layers, D, I, M, d_.hidden_act, d_.layer_norm_eps, H, hdp_,
+                  nullptr, 4.0 * NB * H * static_cast<double>(T) * T * hd, x0_, x1_, ln_, qkv_, att_, mlp_};
   const AttnOp op = make_attn_op(qkv_, 3 * Cp, qkv_ + Cp, 3 * Cp, qkv_ + 2 * Cp, 3 * Cp, att_, Cp, NB, H, T, T, hd);
   a.attention = [op](const __half*, __half*, cudaStream_t st) { run_attn_op(op, st); };
   layer_plan_ = build_clip_layers(a, &flops_);

@@ -36,15 +36,14 @@ void run_clip_vision_embed(const __half* pe, const __half* cls, const __half* po
 using ClipStep = std::function<void(cudaStream_t)>;
 // The pre-LN encoder layer loop both CLIP towers share: per layer LN1 -> q|k|v GEMM -> attention -> out_proj (+ the
 // residual, epilogue) -> LN2 -> fc1 -> activation -> fc2 (+ the residual). The towers differ only in the attention
-// step (`attention`: qkv [M][qkv_n] -> att [M][att_c]) and in how q|k|v and out_proj are packed (`qkv_w` / `qkv_b` /
-// `out_w` per layer; the text tower's are the plain concatenation and weight).
+// step (`attention`: qkv [M][3 * heads * hdp] -> att [M][heads * hdp]) and in the padded head width hdp the q|k|v and
+// out_proj operands are packed with (the text tower's 64 is the plain concatenation and weight).
 struct ClipLayerArgs {
-  const WeightStore* weights;
+  WeightStore* weights;
   std::string prefix;  // "<tower>.encoder.layers."
   int layers, D, I, M, act_mode;
   float eps;
-  int qkv_n, att_c;
-  std::vector<__half*> qkv_w, qkv_b, out_w;
+  int heads, hdp;
   std::function<void(const __half* qkv, __half* att, cudaStream_t)> attention;
   double attention_flops;  // per layer
   __half *x0, *x1, *ln, *qkv, *att, *mlp;
@@ -74,7 +73,6 @@ class ClipTextEncoder {
   WeightStore weights_;
   DeviceArena act_;  // workspace of the prepared plan
   StreamKWorkspace sk_;
-  std::vector<__half*> qkv_w_, qkv_b_;  // per layer: [3D][D], [3D]
   double flops_ = 0.0;
   int B_ = 0, T_ = 0;
   std::vector<std::vector<ClipStep>> layer_plan_;  // one group of launches per encoder layer
@@ -108,7 +106,6 @@ class ClipVisionEncoder {
   DeviceArena act_;
   StreamKWorkspace sk_;
   __half* patch_w_ = nullptr;  // [D][Kp]
-  std::vector<__half*> qkv_w_, qkv_b_, out_w_;
   double flops_ = 0.0;
   int B_ = 0;
   std::vector<std::vector<ClipStep>> layer_plan_;

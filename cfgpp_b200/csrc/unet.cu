@@ -9,57 +9,6 @@
 
 namespace cfgpp {
 
-namespace {
-
-// GEGLU proj rows (2*inner, K): per 128 rows interleave value / gate halves into 256-row tiles
-__global__ void pack_geglu_kernel(const __half* __restrict__ in, __half* __restrict__ out, int inner, int K) {
-  const size_t n = static_cast<size_t>(2) * inner * K;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int k = i % K;
-    const int r = i / K;  // packed row
-    const int tile = r / 256, w = r % 256;
-    const int src_row = (w < 128) ? (tile * 128 + w) : (inner + tile * 128 + (w - 128));
-    out[i] = in[static_cast<size_t>(src_row) * K + k];
-  }
-}
-
-struct HeadMats {
-  const __half* p[3];
-};
-
-// rows of `nmat` stacked (heads*hd, K) matrices -> [(mat, head, hdp)][K], rows hd..hdp-1 of every head zero
-__global__ void pack_heads_rows_kernel(HeadMats mats, __half* __restrict__ out, int nmat, int heads, int hd, int hdp,
-                                       int K) {
-  const size_t n = static_cast<size_t>(nmat) * heads * hdp * K;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int k = i % K;
-    size_t t = i / K;
-    const int r = t % hdp;
-    t /= hdp;
-    const int h = t % heads;
-    const int m = t / heads;
-    out[i] = (r < hd) ? mats.p[m][(static_cast<size_t>(h) * hd + r) * K + k] : __float2half(0.f);
-  }
-}
-
-// (N, heads*hd) -> (N, heads*hdp) with zero columns hd..hdp-1 per head
-__global__ void pack_heads_cols_kernel(const __half* __restrict__ in, __half* __restrict__ out, int N, int heads, int hd,
-                                       int hdp) {
-  const size_t n = static_cast<size_t>(N) * heads * hdp;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int c = i % hdp;
-    size_t t = i / hdp;
-    const int h = t % heads;
-    const int row = t / heads;
-    out[i] = (c < hd) ? in[(static_cast<size_t>(row) * heads + h) * hd + c] : __float2half(0.f);
-  }
-}
-
-}  // namespace
-
 void gemm_configure();
 void attn_configure();
 
@@ -120,124 +69,6 @@ void Unet::load_weight(const std::string& key, const void* data, const int64_t* 
   weights_.load(key, data, shape, ndim, dtype, stream);
 }
 
-__half* Unet::packed(const std::string& name, Pack recipe, size_t numel) {
-  auto it = packed_cache_.find(name);
-  if (it != packed_cache_.end()) return it->second.out;
-  recipe.out = weights_.alloc(numel);
-  run_pack(recipe, nullptr);
-  packed_cache_[name] = recipe;
-  return recipe.out;
-}
-
-size_t Unet::run_pack(const Pack& p, cudaStream_t stream) {
-  size_t total = 0;
-  switch (p.kind) {
-    case Pack::kCatRows:
-      for (auto& k : p.keys) {
-        const WeightStore::Weight& t = weights_.raw(k);
-        CFGPP_CHECK_CUDA(cudaMemcpyAsync(p.out + total, t.p(), t.numel() * sizeof(__half), cudaMemcpyDeviceToDevice, stream));
-        total += t.numel();
-      }
-      break;
-    case Pack::kGeglu: {
-      const WeightStore::Weight& t = weights_.raw(p.keys[0]);
-      const int rows = static_cast<int>(t.shape[0]);
-      total = t.numel();
-      pack_geglu_kernel<<<grid_for(total), 256, 0, stream>>>(t.p(), p.out, rows / 2, p.is_bias ? 1 : static_cast<int>(t.shape[1]));
-      break;
-    }
-    case Pack::kHeadsRows: {
-      HeadMats mats{};
-      for (size_t i = 0; i < p.keys.size(); ++i) mats.p[i] = weights_.plain(p.keys[i]);
-      const int K = static_cast<int>(weights_.raw(p.keys[0]).shape[1]);
-      total = p.keys.size() * static_cast<size_t>(p.heads) * p.hdp * K;
-      pack_heads_rows_kernel<<<grid_for(total), 256, 0, stream>>>(mats, p.out, static_cast<int>(p.keys.size()), p.heads, p.hd, p.hdp, K);
-      break;
-    }
-    case Pack::kHeadsCols: {
-      const WeightStore::Weight& t = weights_.raw(p.keys[0]);
-      const int N = static_cast<int>(t.shape[0]);
-      total = static_cast<size_t>(N) * p.heads * p.hdp;
-      pack_heads_cols_kernel<<<grid_for(total), 256, 0, stream>>>(t.p(), p.out, N, p.heads, p.hd, p.hdp);
-      break;
-    }
-  }
-  CFGPP_CHECK_CUDA(cudaGetLastError());
-  return 2 * total * sizeof(__half);
-}
-
-__half* Unet::packed_cat_rows(const std::vector<std::string>& keys) {
-  std::string name = "cat:";
-  size_t total = 0;
-  for (auto& k : keys) {
-    name += k + "|";
-    total += weights_.raw(k).numel();
-  }
-  return packed(name, Pack{Pack::kCatRows, keys}, total);
-}
-
-__half* Unet::packed_geglu(const std::string& key, bool is_bias) {
-  const WeightStore::Weight& t = weights_.raw(key);
-  CFGPP_REQUIRE(t.shape[0] % 256 == 0, "GEGLU width must be a multiple of 256: " + key);
-  Pack p{Pack::kGeglu, {key}};
-  p.is_bias = is_bias;
-  return packed("geglu:" + key, p, t.numel());
-}
-
-__half* Unet::packed_heads_rows(const std::vector<std::string>& keys, int heads, int hd, int hdp) {
-  if (hd == hdp) return keys.size() == 1 ? weights_.plain(keys[0]) : packed_cat_rows(keys);
-  std::string name = "heads_rows:";
-  for (auto& k : keys) name += k + "|";
-  CFGPP_REQUIRE(keys.size() <= 3, "at most three stacked projections");
-  const int K = static_cast<int>(weights_.raw(keys[0]).shape[1]);
-  for (auto& k : keys) {
-    const WeightStore::Weight& t = weights_.raw(k);
-    CFGPP_REQUIRE(t.shape.size() >= 2 && t.shape[0] == heads * hd && t.shape[1] == K, "unexpected projection shape: " + k);
-  }
-  Pack p{Pack::kHeadsRows, keys, heads, hd, hdp};
-  return packed(name, p, keys.size() * static_cast<size_t>(heads) * hdp * K);
-}
-
-__half* Unet::packed_heads_cols(const std::string& key, int heads, int hd, int hdp) {
-  if (hd == hdp) return weights_.plain(key);
-  const WeightStore::Weight& t = weights_.raw(key);
-  CFGPP_REQUIRE(t.shape[1] == heads * hd, "unexpected to_out shape: " + key);
-  Pack p{Pack::kHeadsCols, {key}, heads, hd, hdp};
-  return packed("heads_cols:" + key, p, static_cast<size_t>(t.shape[0]) * heads * hdp);
-}
-
-Unet::FoldedLN Unet::folded_ln(const std::string& cache_key, const std::vector<std::string>& keys, const __half* w_packed,
-                               int N, int K, const std::string& norm_prefix, const __half* bias_packed) {
-  auto it = fold_cache_.find(cache_key);
-  if (it != fold_cache_.end()) return it->second.f;
-  Fold f{{}, keys, w_packed, N, K, norm_prefix, bias_packed};
-  f.f.w = weights_.alloc(static_cast<size_t>(N) * K);
-  f.f.s = weights_.alloc<float>(N);
-  f.f.t = weights_.alloc<float>(N);
-  run_fold(f, nullptr);
-  fold_cache_[cache_key] = f;
-  return f.f;
-}
-
-size_t Unet::run_fold(const Fold& f, cudaStream_t stream) {
-  run_fold_ln(f.w_packed, weights_.plain(f.norm_prefix + ".weight"), weights_.plain(f.norm_prefix + ".bias"),
-              f.bias_packed, f.f.w, f.f.s, f.f.t, f.N, f.K, stream);
-  return 2 * static_cast<size_t>(f.N) * f.K * sizeof(__half) + 2 * static_cast<size_t>(f.N) * sizeof(float);
-}
-
-size_t Unet::refresh_packed(const std::set<std::string>& keys, cudaStream_t stream) {
-  auto reads = [&](const std::vector<std::string>& src) {
-    return std::any_of(src.begin(), src.end(), [&](const std::string& k) { return keys.count(k) != 0; });
-  };
-  size_t bytes = 0;
-  for (auto& k : keys) bytes += weights_.refresh_conv3x3(k, stream);
-  for (auto& kv : packed_cache_)
-    if (reads(kv.second.keys)) bytes += run_pack(kv.second, stream);
-  for (auto& kv : fold_cache_)  // after the packers: a fold reads the packed matrix
-    if (reads(kv.second.keys)) bytes += run_fold(kv.second, stream);
-  return bytes;
-}
-
 // ------------------------------------------------------------------------------------------------------------
 // LoRA adapters
 // ------------------------------------------------------------------------------------------------------------
@@ -251,14 +82,14 @@ void Unet::lora_set_scales(const float* scales, int n, cudaStream_t stream) {
   size_t bytes = 0;
   const std::set<std::string> touched = weights_.lora_apply(scales, n, stream, &bytes);
   prompt_stale_ = true;
-  lora_bytes_moved_ = bytes + refresh_packed(touched, stream);
+  lora_bytes_moved_ = bytes + weights_.refresh(touched, stream);
 }
 
 void Unet::lora_clear(cudaStream_t stream) {
   size_t bytes = 0;
   const std::set<std::string> touched = weights_.lora_restore(stream, &bytes);
   prompt_stale_ = true;
-  lora_bytes_moved_ = bytes + refresh_packed(touched, stream);
+  lora_bytes_moved_ = bytes + weights_.refresh(touched, stream);
   weights_.lora_free(stream);
 }
 
@@ -292,10 +123,9 @@ void Unet::finalize_weights(cudaStream_t stream) {
         CFGPP_REQUIRE(w.shape.size() == 4 && w.shape[0] == cout && w.shape[1] == cin && w.shape[2] == 3 &&
                           w.shape[3] == 3,
                       "unexpected shape of " + k + ".weight");
-        EmbedConv c{weights_.alloc(static_cast<size_t>(cout_p) * 9 * pad64(cin)), weights_.alloc(cout_p), cout_p,
-                    pad64(cin)};
-        run_pack_conv3x3_padded(w.p(), weights_.plain(k + ".bias", cout), c.w, c.b, cout, cin, cout_p, c.cin_p, stream);
-        embed_convs_[name] = c;
+        weights_.plain(k + ".bias", cout);
+        embed_convs_[name] = EmbedConv{weights_.packed_conv3x3(k + ".weight", pad64(cin), cout_p),
+                                       weights_.packed_heads_rows({k + ".bias"}, 1, cout, cout_p), cout_p, pad64(cin)};
       };
       pack("conv_in", cn_desc_.conditioning_channels, ch[0], pad64(ch[0]));
       for (int i = 0; i + 1 < n; ++i) {
@@ -303,7 +133,6 @@ void Unet::finalize_weights(cudaStream_t stream) {
         pack("blocks." + std::to_string(2 * i + 1), ch[i], ch[i + 1], pad64(ch[i + 1]));
       }
       pack("conv_out", ch[n - 1], d_.block_out_channels[0], d_.block_out_channels[0]);
-      CFGPP_CHECK_CUDA(cudaStreamSynchronize(stream));
       CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
       StreamKScope sk_scope(sk_.ws(), sk_.flags());
       build(1, std::max(8, s * 8), std::max(8, s * 8), nullptr);
@@ -477,9 +306,9 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
   for (int k = 0; k < layers; ++k) {
     const std::string b = prefix + ".transformer_blocks." + std::to_string(k);
     // --- self-attention ---
-    __half* wqkv = packed_heads_rows({b + ".attn1.to_q.weight", b + ".attn1.to_k.weight", b + ".attn1.to_v.weight"},
+    __half* wqkv = weights_.packed_heads_rows({b + ".attn1.to_q.weight", b + ".attn1.to_k.weight", b + ".attn1.to_v.weight"},
                                      heads, hd, hdp);
-    const FoldedLN f1 = folded_ln(b + ".attn1.qkv", {b + ".attn1.to_q.weight", b + ".attn1.to_k.weight", b + ".attn1.to_v.weight"}, wqkv, 3 * Cp, C, b + ".norm1", nullptr);
+    const FoldedLN f1 = weights_.folded_ln(b + ".attn1.qkv", {b + ".attn1.to_q.weight", b + ".attn1.to_k.weight", b + ".attn1.to_v.weight"}, wqkv, 3 * Cp, C, b + ".norm1", nullptr);
     add_gemm(b + ".attn1.to_qkv(+norm1)",
              consumer(make_linear_op(tok, C, nullptr, 0, 0, f1.w, Mi, 3 * Cp, C, nullptr, nullptr, 0, 1, qkv, 3 * Cp, false),
                       f1, 0),
@@ -488,19 +317,19 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
              make_attn_op(qkv, 3 * Cp, qkv + Cp, 3 * Cp, qkv + 2 * Cp, 3 * Cp, attn, Cp, NB_, heads, HW, HW, hd));
     add_gemm(b + ".attn1.to_out", producer([&](int bn) {
                return make_linear_op(attn, Cp, nullptr, 0, 0,
-                                     packed_heads_cols(b + ".attn1.to_out.0.weight", heads, hd, hdp), Mi, C, Cp,
+                                     weights_.packed_heads_cols(b + ".attn1.to_out.0.weight", heads, hd, hdp), Mi, C, Cp,
                                      weights_.plain(b + ".attn1.to_out.0.bias"), tok, C, 1, tok, C, false, bn);
              }, 1),
              2.0 * Mi * static_cast<double>(C) * C);
     // --- cross-attention (K/V projected once per prompt by the prompt plan) ---
-    __half* wq2 = packed_heads_rows({b + ".attn2.to_q.weight"}, heads, hd, hdp);
-    const FoldedLN f2 = folded_ln(b + ".attn2.q", {b + ".attn2.to_q.weight"}, wq2, Cp, C, b + ".norm2", nullptr);
+    __half* wq2 = weights_.packed_heads_rows({b + ".attn2.to_q.weight"}, heads, hd, hdp);
+    const FoldedLN f2 = weights_.folded_ln(b + ".attn2.q", {b + ".attn2.to_q.weight"}, wq2, Cp, C, b + ".norm2", nullptr);
     add_gemm(b + ".attn2.to_q(+norm2)",
              consumer(make_linear_op(tok, C, nullptr, 0, 0, f2.w, Mi, Cp, C, nullptr, nullptr, 0, 1, qb, Cp, false), f2, 1),
              2.0 * Mi * static_cast<double>(C) * C);
     __half* kv = alloc_act(static_cast<size_t>(Mkv) * 2 * Cp);
     {
-      __half* wkv = packed_heads_rows({b + ".attn2.to_k.weight", b + ".attn2.to_v.weight"}, heads, hd, hdp);
+      __half* wkv = weights_.packed_heads_rows({b + ".attn2.to_k.weight", b + ".attn2.to_v.weight"}, heads, hd, hdp);
       std::vector<PlanStep>* save = cur_plan_;
       cur_plan_ = &prompt_plan_;
       add_gemm(b + ".attn2.to_kv",
@@ -514,7 +343,7 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
       const std::string pk = b + ".attn2.processor.to_k_ip.0.weight", pv = b + ".attn2.processor.to_v_ip.0.weight";
       weights_.plain(pk, static_cast<size_t>(C) * D);
       weights_.plain(pv, static_cast<size_t>(C) * D);
-      __half* wkv = packed_heads_rows({pk, pv}, heads, hd, hdp);
+      __half* wkv = weights_.packed_heads_rows({pk, pv}, heads, hd, hdp);
       std::vector<PlanStep>* save = cur_plan_;
       cur_plan_ = &ip_plan_;
       add_gemm(b + ".attn2.to_kv_ip",
@@ -529,14 +358,14 @@ Unet::Act Unet::build_transformer(const std::string& prefix, Act x, int H, int W
     }
     add_gemm(b + ".attn2.to_out", producer([&](int bn) {
                return make_linear_op(attn, Cp, nullptr, 0, 0,
-                                     packed_heads_cols(b + ".attn2.to_out.0.weight", heads, hd, hdp), Mi, C, Cp,
+                                     weights_.packed_heads_cols(b + ".attn2.to_out.0.weight", heads, hd, hdp), Mi, C, Cp,
                                      weights_.plain(b + ".attn2.to_out.0.bias"), tok, C, 1, tok, C, false, bn);
              }, 2),
              2.0 * Mi * static_cast<double>(C) * C);
     // --- GEGLU feed-forward ---
-    __half* wg = packed_geglu(b + ".ff.net.0.proj.weight", false);
-    __half* bg = packed_geglu(b + ".ff.net.0.proj.bias", true);
-    const FoldedLN f3 = folded_ln(b + ".ff.geglu", {b + ".ff.net.0.proj.weight"}, wg, 8 * C, C, b + ".norm3", bg);
+    __half* wg = weights_.packed_geglu(b + ".ff.net.0.proj.weight", false);
+    __half* bg = weights_.packed_geglu(b + ".ff.net.0.proj.bias", true);
+    const FoldedLN f3 = weights_.folded_ln(b + ".ff.geglu", {b + ".ff.net.0.proj.weight"}, wg, 8 * C, C, b + ".norm3", bg);
     add_gemm(b + ".ff.geglu(+norm3)",
              consumer(make_linear_op(tok, C, nullptr, 0, 0, f3.w, Mi, 8 * C, C, nullptr, nullptr, 0, 1, ff, 4 * C, true), f3, 2));
     add_gemm(b + ".ff.out", producer([&](int bn) {
@@ -700,8 +529,8 @@ void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
       } else {
         cond_ = alloc_act(static_cast<size_t>(B_) * H_ * W_ * C0);
       }
-      temb_w_all_ = packed_cat_rows(temb_w_keys);
-      temb_b_all_ = packed_cat_rows(temb_b_keys);
+      temb_w_all_ = weights_.packed_cat_rows(temb_w_keys);
+      temb_b_all_ = weights_.packed_cat_rows(temb_b_keys);
       conv_in_w_ = weights_.plain("conv_in.weight");
       conv_in_b_ = weights_.plain("conv_in.bias");
       if (!is_cn_) {
@@ -1249,7 +1078,7 @@ void Unet::ip_load_weight(const std::string& key, const void* data, const int64_
   if (reload) CFGPP_CHECK_CUDA(cudaDeviceSynchronize());  // a replay may still read the old tensor
   weights_.load(key, data, shape, ndim, dtype, stream);
   if (reload) {
-    refresh_packed({key}, stream);
+    weights_.refresh({key}, stream);
     prepared_ = false;
     graph_valid_ = false;
     nsteps_ = 0;

@@ -1,4 +1,4 @@
-// cfgpp_b200 — UNet2DConditionModel executor: weight registry + repacking, static launch plan over the hand-written
+// cfgpp_b200 — UNet2DConditionModel executor: weights in a WeightStore, static launch plan over the hand-written
 // kernels, CUDA-graph replay of one fused sampler step. Structure follows SURVEY.md Appendix A (diffusers 0.27.1).
 #pragma once
 #include <functional>
@@ -90,39 +90,6 @@ class Unet {
 
  private:
   // ---- weights ----
-  // A packed copy of raw weights and how it is produced, so that it can be produced again into the same buffer.
-  struct Pack {
-    enum Kind { kCatRows, kGeglu, kHeadsRows, kHeadsCols } kind;
-    std::vector<std::string> keys;  // the raw weights it reads
-    int heads = 0, hd = 0, hdp = 0;
-    bool is_bias = false;
-    __half* out = nullptr;
-  };
-  __half* packed(const std::string& name, Pack recipe, size_t numel);  // cached by name; packs on first use
-  size_t run_pack(const Pack& p, cudaStream_t stream);                  // returns bytes read + written
-  __half* packed_cat_rows(const std::vector<std::string>& keys);
-  __half* packed_geglu(const std::string& key, bool is_bias);
-  __half* packed_heads_rows(const std::vector<std::string>& keys, int heads, int hd, int hdp);
-  __half* packed_heads_cols(const std::string& key, int heads, int hd, int hdp);
-  struct FoldedLN {
-    __half* w;
-    float* s;
-    float* t;
-  };
-  struct Fold {
-    FoldedLN f;
-    std::vector<std::string> keys;  // the raw weights w_packed was packed from
-    const __half* w_packed;
-    int N, K;
-    std::string norm_prefix;
-    const __half* bias_packed;
-  };
-  FoldedLN folded_ln(const std::string& cache_key, const std::vector<std::string>& keys, const __half* w_packed, int N,
-                     int K, const std::string& norm_prefix, const __half* bias_packed);
-  size_t run_fold(const Fold& f, cudaStream_t stream);
-  // re-runs, on `stream`, every packer and LayerNorm fold that reads one of `keys`; returns bytes read + written
-  size_t refresh_packed(const std::set<std::string>& keys, cudaStream_t stream);
-  std::map<std::string, Fold> fold_cache_;
   size_t lora_bytes_moved_ = 0;  // of the last lora_set_scales / lora_clear
   bool prompt_stale_ = false;    // weights changed under the bound prompt: set_prompt must run again
   void require_fresh_prompt() const;
@@ -170,7 +137,6 @@ class Unet {
   StreamKWorkspace sk_;
 
   // packed weights: resolved lazily during plan building (finalize just validates + packs what is shape-independent)
-  std::map<std::string, Pack> packed_cache_;
   __half* temb_w_all_ = nullptr;  // [sumCout][time_embed_dim]
   __half* temb_b_all_ = nullptr;
   int temb_total_ = 0;

@@ -35,12 +35,7 @@ void VaeDecoder::finalize_weights(cudaStream_t stream) {
       CFGPP_REQUIRE(ci.shape.size() == 4 && ci.shape[1] == 3 && ci.shape[2] == 3 && ci.shape[3] == 3 &&
                         ci.shape[0] == d_.block_out_channels[0],
                     "encoder.conv_in.weight must be (C0,3,3,3)");
-      const size_t c0 = static_cast<size_t>(ci.shape[0]);
-      __half* p4 = weights_.alloc(c0 * 36);
-      CFGPP_CHECK_CUDA(cudaMemset(p4, 0, c0 * 36 * sizeof(__half)));
-      CFGPP_CHECK_CUDA(cudaMemcpy2D(p4, 36 * sizeof(__half), ci.p(), 27 * sizeof(__half), 27 * sizeof(__half), c0,
-                                    cudaMemcpyDeviceToDevice));
-      conv_in_w4_ = p4;
+      conv_in_w4_ = weights_.packed_heads_cols("encoder.conv_in.weight", 1, 27, 36);
       prepare_encode(1, 128, 128);
     }
   } catch (...) {

@@ -6,7 +6,7 @@ SiLU (away from rounding ties).
 
 Then the two executors against chains of their per-element pinned ops, bit for bit: `NativeControlNet.embed` equals
 image_to_nhwc → (conv3x3 → SiLU)* → conv_out with the weights zero-padded in torch to the packed layout (pinning
-`pack_conv3x3_padded`, the strides, the padded widths and where SiLU runs), and `NativeCLIPVisionEncoder.encode` equals
+`packed_conv3x3`, the strides, the padded widths and where SiLU runs), and `NativeCLIPVisionEncoder.encode` equals
 patchify → patch GEMM → vision_embed → pre-LN → per layer (LN, qkv over heads padded in torch, attention, out_proj +
 residual, LN, fc1, activation, fc2 + residual) → class row → post-LN → projection."""
 import pytest
@@ -148,7 +148,7 @@ def test_silu_every_fp16_input():
 # ---- composition: the ControlNet conditioning embedding -------------------------------------------------------------
 
 def embed_chain(cn_cfg, sd, image):
-    """The conditioning embedding from the pinned ops, weights zero-padded in torch as `pack_conv3x3_padded` lays them
+    """The conditioning embedding from the pinned ops, weights zero-padded in torch as `packed_conv3x3` lays them
     out ([Cout_p][tap][Cin_p], bias padded with zeros)."""
     from cfgpp_b200 import _native as nv
     ch = cn_cfg.conditioning_embedding_out_channels

@@ -925,7 +925,7 @@ def controlnet_body_launches(cfg, h, w, NB=4):
 
 def controlnet_embed_launches(cn_cfg, h, w, B):
     """The conditioning embedding's convolutions on B images of 8h x 8w, as `Unet::cond_embed` issues them: NHWC
-    activations and weights with the channels zero-padded to whole 64-wide K blocks (`pack_conv3x3_padded`), stride 2
+    activations and weights with the channels zero-padded to whole 64-wide K blocks (`packed_conv3x3`), stride 2
     with pad 1 on blocks.1 / 3 / 5, conv_out to the unpadded C0."""
     ch, C0 = cn_cfg.conditioning_embedding_out_channels, cn_cfg.unet.block_out_channels[0]
     H, W, out = 8 * h, 8 * w, []

@@ -327,6 +327,31 @@ def test_new_image_same_prompt_reprojects_and_batching():
     net.close()
 
 
+@pytest.mark.parametrize("name,hw", [("tiny_sd15", 32), ("tiny_sdxl", 32), ("sd15", 64)])
+def test_second_adapter_on_a_live_handle(name, hw):
+    """Attaching adapter B to a handle that already packed adapter A loads B's keys over A's and re-packs every image
+    K‖V operand that reads them in place (a plain concatenation at head_dim 64, head-padded at SD v1.5's 40 / 80 /
+    160): the forward equals a fresh handle's with B bit for bit."""
+    cfg, sd, net = _net(name)
+    a, b = _adapter(cfg, "ip-a"), _adapter(cfg, "ip-b")
+    B, h, w = 1, hw, hw
+    z, uc, c, add, embeds = _inputs(cfg, B, h, w, a.embed_dim)
+    net.attach_ip_adapter(a)
+    _bind(net, B, h, w, uc, c, add, embeds)
+    with_a = _native(net, z, 501)
+    net.attach_ip_adapter(b)
+    _bind(net, B, h, w, uc, c, add, embeds)
+    got = _native(net, z, 501)
+    net.close()
+    _, _, fresh = _net(name)
+    fresh.attach_ip_adapter(b)
+    _bind(fresh, B, h, w, uc, c, add, embeds)
+    want = _native(fresh, z, 501)
+    fresh.close()
+    assert not torch.equal(got, with_a), "adapter B's forward equals adapter A's"
+    assert torch.equal(got, want), "B loaded over A differs from B on a fresh handle"
+
+
 def test_controlnet_handle_refuses_adapter_and_sees_text_only():
     """A ControlNet handle refuses an adapter; with both attached the forward matches the oracle ControlNet (text
     context only) feeding the oracle UNet with the adapter."""
