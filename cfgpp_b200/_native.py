@@ -380,6 +380,21 @@ def op_layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: 
     return out
 
 
+def op_ip_ln_concat(x: torch.Tensor, lat: torch.Tensor, g0: torch.Tensor, b0: torch.Tensor, g1: torch.Tensor,
+                    b1: torch.Tensor, eps: float = 1e-5):
+    """The two LayerNorms of a Resampler layer in one launch: x [NB, T, C], lat [NB, Q, C] fp16 ->
+    (kv [NB, T + Q, C] = cat(LN0(x), LN1(lat)), q [NB, Q, C] = LN1(lat))."""
+    lib = load()
+    NB, T, C = x.shape
+    Q = lat.shape[1]
+    assert tuple(lat.shape) == (NB, Q, C)
+    kv = torch.empty((NB, T + Q, C), dtype=torch.float16, device=x.device)
+    q = torch.empty_like(lat)
+    check(lib.cfgpp_op_ip_ln_concat(ptr(x), ptr(lat), c_int(NB), c_int(T), c_int(Q), c_int(C), ptr(g0), ptr(b0),
+                                    ptr(g1), ptr(b1), c_float(eps), ptr(kv), ptr(q), stream_ptr()))
+    return kv, q
+
+
 def op_cfgpp_step(eps_uc: torch.Tensor, eps_c: torch.Tensor, method: int, coef, z: torch.Tensor,
                   aux: torch.Tensor | None = None, want_z0t: bool = True, noise: torch.Tensor | None = None,
                   lambdas: torch.Tensor | None = None):

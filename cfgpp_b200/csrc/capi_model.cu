@@ -213,6 +213,17 @@ CFGPP_API int cfgpp_set_ip_image_embeds(cfgpp_handle* h, const void* embeds_dev,
   return guarded([&] { unet_of(h).set_ip_image_embeds((const __half*)embeds_dev, (cudaStream_t)stream); });
 }
 
+CFGPP_API int cfgpp_ip_adapter_attach_resampler(cfgpp_handle* h, const cfgpp_ip_resampler_desc* desc) {
+  return guarded([&] {
+    CFGPP_REQUIRE(desc != nullptr, "null argument");
+    unet_of(h).ip_attach_resampler(*desc);
+  });
+}
+
+CFGPP_API int cfgpp_set_ip_image_hidden_states(cfgpp_handle* h, const void* hidden_dev, void* stream) {
+  return guarded([&] { unet_of(h).set_ip_image_hidden_states((const __half*)hidden_dev, (cudaStream_t)stream); });
+}
+
 CFGPP_API int cfgpp_set_ip_adapter_scale(cfgpp_handle* h, float scale, void* stream) {
   return guarded([&] { unet_of(h).set_ip_scale(scale, (cudaStream_t)stream); });
 }
@@ -220,6 +231,13 @@ CFGPP_API int cfgpp_set_ip_adapter_scale(cfgpp_handle* h, float scale, void* str
 // Debug aid (not in the public header): how many step graphs the handle has captured.
 CFGPP_API int cfgpp_dbg_graph_captures(cfgpp_handle* h, int* n) {
   return guarded([&] { *n = unet_of(h).graph_captures(); });
+}
+
+// Test and measurement aid (not in the public header): the IP-Adapter image projection alone, on the rows the last
+// cfgpp_set_ip_image_embeds / cfgpp_set_ip_image_hidden_states set, and its tokens [2*batch * n_tokens, D] fp16
+// copied into tokens_out_dev (may be null).
+CFGPP_API int cfgpp_dbg_ip_image_proj(cfgpp_handle* h, void* tokens_out_dev, void* stream) {
+  return guarded([&] { unet_of(h).run_image_proj((__half*)tokens_out_dev, (cudaStream_t)stream); });
 }
 
 CFGPP_API int cfgpp_controlnet_embed(cfgpp_handle* cn, const void* image, int dtype, int batch, int height, int width,

@@ -203,6 +203,15 @@ CFGPP_API int cfgpp_op_layernorm(const void* x, int M, int C, const void* gamma,
   });
 }
 
+CFGPP_API int cfgpp_op_ip_ln_concat(const void* x, const void* lat, int NB, int T, int Q, int C, const void* g0,
+                                    const void* b0, const void* g1, const void* b1, float eps, void* kv, void* q,
+                                    void* stream) {
+  return guarded([&] {
+    run_ln_concat((const __half*)x, (const __half*)lat, NB, T, Q, C, (const __half*)g0, (const __half*)b0,
+                  (const __half*)g1, (const __half*)b1, eps, (__half*)kv, (__half*)q, (cudaStream_t)stream);
+  });
+}
+
 }  // extern "C"
 
 namespace {

@@ -80,6 +80,14 @@ CFGPP_API int cfgpp_clip_vision_encode(cfgpp_clip_vision_handle* h, const void* 
   });
 }
 
+CFGPP_API int cfgpp_clip_vision_encode_hidden(cfgpp_clip_vision_handle* h, const void* pixels, int dtype, int batch,
+                                              int skip, void* hidden_out, void* stream) {
+  return guarded([&] {
+    CFGPP_REQUIRE(dtype == CFGPP_F16 || dtype == CFGPP_F32, "pixel values: fp16 or fp32");
+    h->enc.encode_hidden(pixels, dtype == CFGPP_F16, batch, skip, (__half*)hidden_out, (cudaStream_t)stream);
+  });
+}
+
 CFGPP_API int cfgpp_clip_vision_stats(cfgpp_clip_vision_handle* h, double* flops, size_t* workspace_bytes) {
   return guarded([&] {
     if (flops) *flops = h->enc.flops();

@@ -239,14 +239,12 @@ __global__ void gn_apply_kernel(GnSrc src, int HW, int C, int px_per_block, cons
   for (; pp < pend; pp += pstep) emit(load_vec(src, base + pp, c0), base + pp);
 }
 
-// one warp per row; C % 8 == 0, C <= 2048
-__global__ void layernorm_kernel(const __half* __restrict__ x, int M, int C, const __half* __restrict__ gamma,
-                                 const __half* __restrict__ beta, float eps, __half* __restrict__ out) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (row >= M) return;
+// LayerNorm of one row xr [C] by one warp (C % 8 == 0, C <= 2048): fp32 statistics and affine transform, one fp16
+// rounding; store(vi, o) writes the 8 outputs of columns [8 vi, 8 vi + 8). Every LayerNorm kernel runs this body, so a
+// row normalised by any of them has the same bits.
+template <typename Store>
+CFGPP_DEVICE void layernorm_row(const __half* __restrict__ xr, int C, const __half* __restrict__ gamma,
+                                const __half* __restrict__ beta, float eps, int lane, Store store) {
   const int nvec = C >> 3;
   constexpr int MAXV = 8;
   uint4 v[MAXV];
@@ -255,7 +253,7 @@ __global__ void layernorm_kernel(const __half* __restrict__ x, int M, int C, con
   for (int i = 0; i < MAXV; ++i) {
     const int vi = lane + i * 32;
     if (vi < nvec) {
-      v[i] = *reinterpret_cast<const uint4*>(x + static_cast<size_t>(row) * C + vi * 8);
+      v[i] = *reinterpret_cast<const uint4*>(xr + vi * 8);
       const __half2* h = reinterpret_cast<const __half2*>(&v[i]);
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
@@ -301,8 +299,48 @@ __global__ void layernorm_kernel(const __half* __restrict__ x, int M, int C, con
       o.y = pack_half2(y[2], y[3]);
       o.z = pack_half2(y[4], y[5]);
       o.w = pack_half2(y[6], y[7]);
-      *reinterpret_cast<uint4*>(out + static_cast<size_t>(row) * C + vi * 8) = o;
+      store(vi, o);
     }
+  }
+}
+
+// one warp per row; C % 8 == 0, C <= 2048
+__global__ void layernorm_kernel(const __half* __restrict__ x, int M, int C, const __half* __restrict__ gamma,
+                                 const __half* __restrict__ beta, float eps, __half* __restrict__ out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= M) return;
+  __half* orow = out + static_cast<size_t>(row) * C;
+  layernorm_row(x + static_cast<size_t>(row) * C, C, gamma, beta, eps, lane,
+                [=](int vi, const uint4& o) { *reinterpret_cast<uint4*>(orow + vi * 8) = o; });
+}
+
+// The two LayerNorms of a Resampler layer in one launch, one warp per row of kv [NB][T + Q][C]: row (b, j < T) is
+// LN0(x[b, j]), row (b, T + i) is LN1(lat[b, i]), which also goes to q [NB][Q][C] (the query operand).
+__global__ void ln_concat_kernel(const __half* __restrict__ x, const __half* __restrict__ lat, int NB, int T, int Q,
+                                 int C, const __half* __restrict__ g0, const __half* __restrict__ b0,
+                                 const __half* __restrict__ g1, const __half* __restrict__ b1, float eps,
+                                 __half* __restrict__ kv, __half* __restrict__ q) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  const int S = T + Q;
+  if (row >= NB * S) return;
+  const int b = row / S, j = row - b * S;
+  __half* kvrow = kv + static_cast<size_t>(row) * C;
+  if (j < T) {
+    layernorm_row(x + (static_cast<size_t>(b) * T + j) * C, C, g0, b0, eps, lane,
+                  [=](int vi, const uint4& o) { *reinterpret_cast<uint4*>(kvrow + vi * 8) = o; });
+  } else {
+    const size_t r = static_cast<size_t>(b) * Q + (j - T);
+    __half* qrow = q + r * C;
+    layernorm_row(lat + r * C, C, g1, b1, eps, lane, [=](int vi, const uint4& o) {
+      *reinterpret_cast<uint4*>(kvrow + vi * 8) = o;
+      *reinterpret_cast<uint4*>(qrow + vi * 8) = o;
+    });
   }
 }
 
@@ -370,6 +408,15 @@ void run_layernorm(const __half* x, int M, int C, const __half* gamma, const __h
   CFGPP_REQUIRE(C % 8 == 0 && C <= 2048, "LayerNorm needs C % 8 == 0 and C <= 2048");
   const int warps = 8;
   launch_pdl(layernorm_kernel, dim3((M + warps - 1) / warps), dim3(warps * 32), 0, stream, x, M, C, gamma, beta, eps, out);
+}
+
+void run_ln_concat(const __half* x, const __half* lat, int NB, int T, int Q, int C, const __half* g0, const __half* b0,
+                   const __half* g1, const __half* b1, float eps, __half* kv, __half* q, cudaStream_t stream) {
+  CFGPP_REQUIRE(C % 8 == 0 && C <= 2048, "LayerNorm needs C % 8 == 0 and C <= 2048");
+  CFGPP_REQUIRE(NB >= 1 && T >= 1 && Q >= 1, "empty LayerNorm concatenation");
+  const int warps = 8, rows = NB * (T + Q);
+  launch_pdl(ln_concat_kernel, dim3((rows + warps - 1) / warps), dim3(warps * 32), 0, stream, x, lat, NB, T, Q, C, g0, b0,
+             g1, b1, eps, kv, q);
 }
 
 void run_fold_ln(const __half* w, const __half* gamma, const __half* beta, const __half* bias, __half* wf, float* s,

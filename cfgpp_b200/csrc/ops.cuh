@@ -14,6 +14,11 @@ void run_groupnorm(const __half* x1, int C1, const __half* x2, int C2, int B, in
                    const __half* beta, float eps, bool silu, float* partial, __half* out, cudaStream_t stream);
 void run_layernorm(const __half* x, int M, int C, const __half* gamma, const __half* beta, float eps, __half* out,
                    cudaStream_t stream);
+// The two LayerNorms of one IP-Adapter Plus Resampler layer: kv [NB][T + Q][C] holds LN0(x[b]) (x [NB][T][C]) in its
+// first T rows per image and LN1(lat[b]) (lat [NB][Q][C]) in the last Q, and q [NB][Q][C] gets LN1(lat) again. Every
+// row is bit-identical to run_layernorm's output for it.
+void run_ln_concat(const __half* x, const __half* lat, int NB, int T, int Q, int C, const __half* g0, const __half* b0,
+                   const __half* g1, const __half* b1, float eps, __half* kv, __half* q, cudaStream_t stream);
 // LayerNorm fold of a weight w [N][K] (see GemmParams): wf = fp16(w * gamma), s[n] = sum_k wf[n,k],
 // t[n] = sum_k beta[k] w[n,k] + bias[n] (bias may be null); s, t fp32.
 void run_fold_ln(const __half* w, const __half* gamma, const __half* beta, const __half* bias, __half* wf, float* s,

@@ -256,10 +256,9 @@ void ClipVisionEncoder::prepare(int batch) {
   CFGPP_CHECK_CUDA(cudaDeviceSynchronize());
 }
 
-void ClipVisionEncoder::encode(const void* image, int is_half, int batch, __half* embeds_out, cudaStream_t stream) {
-  CFGPP_REQUIRE(image != nullptr && embeds_out != nullptr, "null argument");
+void ClipVisionEncoder::embed(const void* image, int is_half, int batch, cudaStream_t stream) {
+  CFGPP_REQUIRE(image != nullptr, "null argument");
   if (batch != B_) prepare(batch);
-  StreamKScope sk_scope(sk_.ws(), sk_.flags());
   const int D = d_.hidden_size, M = batch * T_;
   const std::string vm = "vision_model.";
   run_clip_patchify(image, is_half, patches_, batch, d_.image_size, d_.patch_size, Kp_, stream);
@@ -270,6 +269,14 @@ void ClipVisionEncoder::encode(const void* image, int is_half, int batch, __half
                         weights_.plain(vm + "embeddings.position_embedding.weight"), emb_, batch, np_, D, stream);
   run_layernorm(emb_, M, D, weights_.plain(vm + "pre_layrnorm.weight"), weights_.plain(vm + "pre_layrnorm.bias"),
                 d_.layer_norm_eps, x0_, stream);
+}
+
+void ClipVisionEncoder::encode(const void* image, int is_half, int batch, __half* embeds_out, cudaStream_t stream) {
+  CFGPP_REQUIRE(embeds_out != nullptr, "null argument");
+  StreamKScope sk_scope(sk_.ws(), sk_.flags());
+  embed(image, is_half, batch, stream);
+  const int D = d_.hidden_size;
+  const std::string vm = "vision_model.";
   for (auto& layer : layer_plan_)
     for (auto& fn : layer) fn(stream);
   CFGPP_CHECK_CUDA(cudaMemcpy2DAsync(cls_, D * sizeof(__half), x0_, static_cast<size_t>(T_) * D * sizeof(__half),
@@ -278,6 +285,20 @@ void ClipVisionEncoder::encode(const void* image, int is_half, int batch, __half
                 d_.layer_norm_eps, cls_ln_, stream);
   run_small_linear(cls_ln_, D, weights_.plain("visual_projection.weight"), nullptr, nullptr, 0, embeds_out,
                    d_.projection_dim, nullptr, batch, d_.projection_dim, D, false, stream);
+}
+
+void ClipVisionEncoder::encode_hidden(const void* image, int is_half, int batch, int skip, __half* hidden_out,
+                                      cudaStream_t stream) {
+  CFGPP_REQUIRE(hidden_out != nullptr, "null argument");
+  CFGPP_REQUIRE(skip >= 0 && skip <= d_.num_layers, "skip must be 0..num_layers (hidden_states[num_layers - skip])");
+  StreamKScope sk_scope(sk_.ws(), sk_.flags());
+  embed(image, is_half, batch, stream);
+  // hidden_states[0] is pre_layrnorm's output; layer l writes hidden_states[l + 1]. The layers after the wanted one
+  // do not run.
+  for (int l = 0; l < d_.num_layers - skip; ++l)
+    for (auto& fn : layer_plan_[l]) fn(stream);
+  CFGPP_CHECK_CUDA(cudaMemcpyAsync(hidden_out, x0_, static_cast<size_t>(batch) * T_ * d_.hidden_size * sizeof(__half),
+                                   cudaMemcpyDeviceToDevice, stream));
 }
 
 }  // namespace cfgpp

@@ -92,11 +92,15 @@ class ClipVisionEncoder {
   void finalize_weights(cudaStream_t stream);
   // image [batch][3][S][S] (fp16 or fp32, normalised pixel values) -> image_embeds [batch][projection_dim] fp16
   void encode(const void* image, int is_half, int batch, __half* embeds_out, cudaStream_t stream);
+  // the same image -> hidden_states[num_layers - skip] [batch][T][hidden_size] fp16 (no post_layernorm; skip = 1 is
+  // the penultimate layer IP-Adapter Plus reads); only the layers up to that one run
+  void encode_hidden(const void* image, int is_half, int batch, int skip, __half* hidden_out, cudaStream_t stream);
   double flops() const { return flops_; }
   size_t workspace_bytes() const { return act_.bytes(); }
 
  private:
   void prepare(int batch);
+  void embed(const void* image, int is_half, int batch, cudaStream_t stream);  // image -> hidden_states[0] in x0_
 
   cfgpp_clip_vision_desc d_;
   int device_;

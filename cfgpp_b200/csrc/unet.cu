@@ -510,8 +510,10 @@ void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
       }
       args_ = shared_args ? shared_args : act_.alloc<StepArgs>(1);
       if (ip_ntok_ > 0 && !is_cn_) {
-        ip_embeds_ = alloc_act(static_cast<size_t>(NB_) * ip_embed_dim_);
-        ip_proj_ = alloc_act(static_cast<size_t>(NB_) * ip_ntok_ * d_.cross_attention_dim);
+        if (ip_rs_.num_queries == 0) {  // the Resampler allocates its own buffers (build_ip_resampler)
+          ip_embeds_ = alloc_act(static_cast<size_t>(NB_) * ip_embed_dim_);
+          ip_proj_ = alloc_act(static_cast<size_t>(NB_) * ip_ntok_ * d_.cross_attention_dim);
+        }
         ip_tokens_ = alloc_act(static_cast<size_t>(NB_) * ip_ntok_ * d_.cross_attention_dim);
       }
       if (!is_cn_) {  // the sampler state and tables: a ControlNet runs inside its UNet's step
@@ -586,7 +588,9 @@ void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
 
     // ---- IP-Adapter image projection (diffusers ImageProjection): LayerNorm(D) of the rows of Linear(E -> ntok * D) ----
     cur_plan_ = &ip_plan_;
-    if (!sizing_ && ip_ntok_ > 0 && !is_cn_) {
+    if (!sizing_ && ip_ntok_ > 0 && !is_cn_ && ip_rs_.num_queries > 0) {
+      build_ip_resampler();  // IP-Adapter Plus
+    } else if (!sizing_ && ip_ntok_ > 0 && !is_cn_) {
       const int NB = NB_, D = d_.cross_attention_dim, E = ip_embed_dim_, T = ip_ntok_;
       add_gemm("image_proj.proj",
                make_linear_op(ip_embeds_, E, nullptr, 0, 0, weights_.plain("image_proj.proj.weight", size_t(T) * D * E),
@@ -759,8 +763,10 @@ void Unet::run_inputs(const void* z, int z_is_half, cudaStream_t stream) {
 }
 
 void Unet::require_ip_ready() const {
-  CFGPP_REQUIRE(ip_ntok_ == 0 || ip_ready_, "an IP-Adapter is attached: call cfgpp_set_ip_image_embeds for the prepared "
-                                            "plan and the loaded adapter");
+  CFGPP_REQUIRE(ip_ntok_ == 0 || ip_ready_, std::string("an IP-Adapter is attached: call ") +
+                                                (ip_rs_.num_queries ? "cfgpp_set_ip_image_hidden_states"
+                                                                    : "cfgpp_set_ip_image_embeds") +
+                                                " for the prepared plan and the loaded adapter");
 }
 
 void Unet::require_control_ready() const {
@@ -1095,6 +1101,7 @@ void Unet::ip_attach(int n_tokens, int embed_dim) {
   }
   ip_ntok_ = n_tokens;
   ip_embed_dim_ = n_tokens ? embed_dim : 0;
+  ip_rs_ = cfgpp_ip_resampler_desc{};  // ip_attach_resampler sets it after this call
   // the plan changes shape: the next cfgpp_prepare builds it
   prepared_ = false;
   graph_valid_ = false;
@@ -1104,6 +1111,8 @@ void Unet::ip_attach(int n_tokens, int embed_dim) {
 
 void Unet::set_ip_image_embeds(const __half* embeds, cudaStream_t stream) {
   CFGPP_REQUIRE(ip_ntok_ > 0, "no IP-Adapter attached");
+  CFGPP_REQUIRE(ip_rs_.num_queries == 0, "the attached IP-Adapter Plus takes the image encoder's hidden states "
+                                         "(cfgpp_set_ip_image_hidden_states), not image embeds");
   CFGPP_REQUIRE(prepared_, "call cfgpp_prepare first");
   CFGPP_REQUIRE(embeds != nullptr, "null image embeds");
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(ip_embeds_, embeds, static_cast<size_t>(NB_) * ip_embed_dim_ * sizeof(__half),

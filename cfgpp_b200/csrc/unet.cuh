@@ -78,6 +78,12 @@ class Unet {
                       cudaStream_t stream);
   void ip_attach(int n_tokens, int embed_dim);  // n_tokens = 0 detaches
   void set_ip_image_embeds(const __half* embeds, cudaStream_t stream);
+  // IP-Adapter Plus (ip_resampler.cu): the Resampler image projection over hidden states [2*batch][seq_len][E]
+  void ip_attach_resampler(const cfgpp_ip_resampler_desc& r);
+  void set_ip_image_hidden_states(const __half* hidden, cudaStream_t stream);
+  // Test and measurement aid: the image projection alone (the `image_proj.*` entries of the plan, on the image rows
+  // already set), and a copy of its tokens [2*batch * n_tokens][D] into tokens_out (may be null)
+  void run_image_proj(__half* tokens_out, cudaStream_t stream);
   void set_ip_scale(float scale, cudaStream_t stream);
   // Eager un-fused forward with a CUDA-event pair around every plan entry (profiling aid for bench.py).
   struct ProfEntry {
@@ -124,6 +130,8 @@ class Unet {
   void run_inputs(const void* z, int z_is_half, cudaStream_t stream);
   void require_control_ready() const;
   void require_ip_ready() const;
+  void build_ip_resampler();  // ip_plan_ of an attached Resampler (ip_resampler.cu)
+  void require_resampler_weights(const cfgpp_ip_resampler_desc& r) const;
   void upload_entries(cudaStream_t stream);  // entries_ -> step_table_
   // the un-fused forward's current entry: timestep and input scale, no step, the scalar conditioning scale
   void stage_entry(float t, float in_scale, cudaStream_t stream);
@@ -213,6 +221,9 @@ class Unet {
   bool ip_ready_ = false;               // image embeds projected for the current plan and weights
   __half *ip_embeds_ = nullptr, *ip_proj_ = nullptr, *ip_tokens_ = nullptr;
   std::vector<PlanStep> ip_plan_;
+  // IP-Adapter Plus: the Resampler's geometry (num_queries = 0: the plain projection, or none) and its input
+  cfgpp_ip_resampler_desc ip_rs_{};
+  __half* ip_hidden_ = nullptr;  // [NB * seq_len][E]
 
   cudaGraph_t graph_ = nullptr;
   cudaGraphExec_t graph_exec_ = nullptr;

@@ -316,25 +316,40 @@ class NativeUNet(nv.NativeHandle):
                     nv.check(self.lib.cfgpp_ip_adapter_load_weight(self._h, key.encode(), nv.ptr(w), shape,
                                                                    c_int(w.dim()), c_int(nv.dtype_code(w)), st))
                 torch.cuda.synchronize(self.device)
-                nv.check(self.lib.cfgpp_ip_adapter_attach(self._h, c_int(adapter.n_tokens), c_int(adapter.embed_dim)))
+                if adapter.resampler is not None:  # IP-Adapter Plus
+                    r = adapter.resampler
+                    desc = (c_int * 7)(r["num_queries"], r["embed_dim"], r["seq_len"], r["dim"], r["heads"],
+                                       r["depth"], r["ff_mult"])  # cfgpp_ip_resampler_desc
+                    nv.check(self.lib.cfgpp_ip_adapter_attach_resampler(self._h, desc))
+                else:
+                    nv.check(self.lib.cfgpp_ip_adapter_attach(self._h, c_int(adapter.n_tokens),
+                                                              c_int(adapter.embed_dim)))
         self.ip_adapter = adapter
         self._ip_embeds = None
         self.batch, self.latent_hw, self._nsteps, self._bound, self._control_image = 0, (0, 0), 0, None, None
 
     def set_ip_image_embeds(self, embeds: torch.Tensor, force: bool = True) -> None:
-        """embeds [batch, E]: one image embedding per image of the prepared batch. The unconditional half gets zeros,
-        as diffusers' negative image embeds; the image projection and every block's K / V projection run here. With
-        force False, the same tensor object (same in-place version) already projected for this plan is not projected
-        again; any other tensor is (a new reference image with the same prompt)."""
-        assert embeds.dim() == 2 and embeds.shape[0] == self.batch, "one image embedding per image of the batch"
+        """embeds [batch, E]: one image embedding per image of the prepared batch; for an IP-Adapter Plus, the image
+        encoder's hidden states [batch, T, E] (IPAdapter.image_embeds gives either). The unconditional half gets what
+        diffusers gives it (IPAdapter.image_rows: zeros, or the hidden states of a zero image); the image projection and
+        every block's K / V projection run here. With force False, the same tensor object (same in-place version)
+        already projected for this plan is not projected again; any other tensor is (a new reference image with the
+        same prompt)."""
+        plus = self.ip_adapter is not None and self.ip_adapter.resampler is not None
+        assert embeds.dim() == (3 if plus else 2) and embeds.shape[0] == self.batch, \
+            "one image embedding (Plus: hidden states) per image of the batch"
         key = (embeds, embeds._version)
         if not force and self._ip_embeds is not None and self._ip_embeds[0] is embeds \
                 and self._ip_embeds[1] == key[1]:
             return
-        e = embeds.to(self.device, torch.float16)
-        rows = torch.cat([torch.zeros_like(e), e]).contiguous()
+        if plus:
+            rows = self.ip_adapter.image_rows(embeds).to(self.device)
+        else:
+            e = embeds.to(self.device, torch.float16)
+            rows = torch.cat([torch.zeros_like(e), e]).contiguous()
         with torch.cuda.device(self.device):
-            nv.check(self.lib.cfgpp_set_ip_image_embeds(self._h, nv.ptr(rows), nv.stream_ptr()))
+            fn = self.lib.cfgpp_set_ip_image_hidden_states if plus else self.lib.cfgpp_set_ip_image_embeds
+            nv.check(fn(self._h, nv.ptr(rows), nv.stream_ptr()))
         self._ip_embeds = key
 
     def set_ip_adapter_scale(self, scale: float) -> None:

@@ -154,7 +154,8 @@ def preprocess(images: Sequence, size: int = 224) -> torch.Tensor:
 
 
 class NativeCLIPVisionEncoder(nv.NativeHandle):
-    """Owner of one `cfgpp_clip_vision_handle`: `encode(pixel_values)` -> image_embeds (n, projection_dim) fp16."""
+    """Owner of one `cfgpp_clip_vision_handle`: `encode(pixel_values)` -> image_embeds (n, projection_dim) fp16, and
+    `encode_hidden(pixel_values, skip)` -> hidden_states[num_layers - skip] (n, T, hidden_size) fp16."""
 
     _prefix, _what = "_clip_vision", "vision encoder"
 
@@ -185,6 +186,22 @@ class NativeCLIPVisionEncoder(nv.NativeHandle):
                                                            c_int(xi.shape[0]), nv.ptr(out), nv.stream_ptr()))
                 outs.append(out)
         return torch.cat(outs)
+
+    def encode_hidden(self, pixel_values: torch.Tensor, skip: int = 1) -> torch.Tensor:
+        """hidden_states[num_layers - skip] of transformers' `output_hidden_states=True` (skip = 1: hidden_states[-2],
+        what IP-Adapter Plus reads; skip = 0: the last layer's output, before post_layernorm)."""
+        n, S = pixel_values.shape[0], self.cfg.image_size
+        assert tuple(pixel_values.shape[1:]) == (3, S, S), "pixel values (n, 3, image_size, image_size)"
+        x = pixel_values.to(self.device).contiguous()
+        T = self.cfg.num_positions
+        out = torch.empty((n, T, self.cfg.hidden_size), dtype=torch.float16, device=self.device)
+        with torch.cuda.device(self.device):
+            for i in range(0, n, 16):
+                xi = x[i:i + 16]
+                nv.check(self.lib.cfgpp_clip_vision_encode_hidden(self._h, nv.ptr(xi), c_int(nv.dtype_code(xi)),
+                                                                  c_int(xi.shape[0]), c_int(skip), nv.ptr(out[i:i + 16]),
+                                                                  nv.stream_ptr()))
+        return out
 
     @property
     def stats(self) -> dict:

@@ -268,6 +268,38 @@ int cfgpp_set_ip_image_embeds(cfgpp_handle* h, const void* embeds_dev, void* str
 /* The scale s (1.0 after create): one fp32 device word every decoupled cross-attention launch reads, written on
  * `stream`; never recaptures the step graph. */
 int cfgpp_set_ip_adapter_scale(cfgpp_handle* h, float scale, void* stream);
+/* ---- IP-Adapter Plus (diffusers IPAdapterPlusImageProjection, the Perceiver "Resampler"): the image tokens come from
+ * the image encoder's penultimate hidden states h [2*batch, seq_len, E] instead of one pooled embedding. Weights, loaded
+ * with cfgpp_ip_adapter_load_weight under the original checkpoint's `image_proj.*` keys (inner = 64 * heads,
+ * F = ff_mult * dim, D = cross_attention_dim):
+ *   image_proj.latents [1, Q, dim]; proj_in.{weight,bias} [dim, E], [dim]; proj_out.{weight,bias} [D, dim], [D];
+ *   norm_out.{weight,bias} [D]; per layer i: layers.{i}.0.norm1 (on x) / .norm2 (on the latents) {weight,bias} [dim],
+ *   layers.{i}.0.to_q.weight [inner, dim], layers.{i}.0.to_kv.weight [2 * inner, dim] (k rows first, then v),
+ *   layers.{i}.0.to_out.weight [dim, inner], layers.{i}.1.0.{weight,bias} [dim], layers.{i}.1.1.weight [F, dim],
+ *   layers.{i}.1.3.weight [dim, F]
+ * plus the per-block to_k_ip / to_v_ip above. Each Linear rounds once to fp16, every LayerNorm has eps 1e-5:
+ *   x = proj_in(h); lat = latents (per image)
+ *   per layer: kv = [LN0(x), LN1(lat)] (seq_len + Q rows), lat = to_out(SDPA(to_q(LN1(lat)), to_k(kv), to_v(kv))) + lat
+ *              (heads of 64, scale 1/8, no bias), lat = W2 gelu_erf(W1 LN_ff(lat)) + lat (bias-free)
+ *   tokens = norm_out(proj_out(lat))  [2*batch * Q, D]
+ * and the tokens feed every attn2 as the plain adapter's do. */
+typedef struct cfgpp_ip_resampler_desc {
+  int num_queries; /* Q, the image tokens: 1..64 (the Plus checkpoints: 16) */
+  int embed_dim;   /* E, the hidden-state width: a multiple of 64 (ViT-H/14: 1280) */
+  int seq_len;     /* rows of h per image (ViT-H/14 at 224: 257) */
+  int dim;         /* the Resampler's width: a multiple of 64, <= 2048 (SD v1.5 Plus: 768, SDXL Plus: 1280) */
+  int heads;       /* heads of 64 (12 / 20) */
+  int depth;       /* layers (4) */
+  int ff_mult;     /* feed-forward width / dim (4) */
+} cfgpp_ip_resampler_desc;
+/* Attach the loaded Plus adapter: like cfgpp_ip_adapter_attach (which, like cfgpp_ip_adapter_clear, also detaches a
+ * Resampler), and fails naming a key above that is missing or whose shape does not fit `desc`. */
+int cfgpp_ip_adapter_attach_resampler(cfgpp_handle* h, const cfgpp_ip_resampler_desc* desc);
+/* hidden_dev: (2*batch, seq_len, E) fp16 device tensor, rows in cfgpp_set_prompt's order (the unconditional half: the
+ * encoder's hidden states of an all-zero preprocessed image, as diffusers). Runs the Resampler and every block's K2 / V2
+ * projection now; the counterpart of cfgpp_set_ip_image_embeds, which refuses a Resampler (and this one, a plain
+ * adapter). */
+int cfgpp_set_ip_image_hidden_states(cfgpp_handle* h, const void* hidden_dev, void* stream);
 
 /* ---- AutoencoderKL decoder (SURVEY.md section 8 f2): replaces `self.vae.decode(zt / scaling_factor).sample` of
  * latent_sdxl.py:155-164 (VAE madebyollin/sdxl-vae-fp16-fix, :44) and latent_diffusion.py:123-129 on the same conv /
@@ -359,6 +391,11 @@ int cfgpp_clip_vision_finalize_weights(cfgpp_clip_vision_handle* h, void* stream
  * fp16 as the fp16 model's conv input); image_embeds_out: (batch, projection_dim) fp16. */
 int cfgpp_clip_vision_encode(cfgpp_clip_vision_handle* h, const void* pixel_values_dev, int dtype, int batch,
                              void* image_embeds_out, void* stream);
+/* The same images -> hidden_out (batch, T, hidden_size) fp16 = hidden_states[num_layers - skip] (T = (image_size /
+ * patch_size)^2 + 1; skip = 1: the penultimate layer IP-Adapter Plus reads; skip = num_layers: pre_layrnorm's output).
+ * No post_layernorm, no projection; the layers after the wanted one do not run. */
+int cfgpp_clip_vision_encode_hidden(cfgpp_clip_vision_handle* h, const void* pixel_values_dev, int dtype, int batch,
+                                    int skip, void* hidden_out, void* stream);
 int cfgpp_clip_vision_stats(cfgpp_clip_vision_handle* h, double* flops, size_t* workspace_bytes);
 
 /* ---- operator-level entry points (one kernel each; used by the kernel parity tests and micro-benchmarks) ----- */
@@ -426,6 +463,11 @@ int cfgpp_op_groupnorm(const void* x1, int C1, const void* x2, int C2, int B, in
                        const void* beta, float eps, int silu, void* out, void* stream);
 int cfgpp_op_layernorm(const void* x, int M, int C, const void* gamma, const void* beta, float eps, void* out,
                        void* stream);
+/* The two LayerNorms of an IP-Adapter Plus Resampler layer in one launch (C % 8 == 0, C <= 2048):
+ * kv [NB, T + Q, C]: rows (b, 0..T-1) = LN(x[b]; g0, b0), rows (b, T..T+Q-1) = LN(lat[b]; g1, b1), x [NB, T, C],
+ * lat [NB, Q, C]; q [NB, Q, C] = LN(lat; g1, b1) again. Every row equals cfgpp_op_layernorm's output for it, bit for bit. */
+int cfgpp_op_ip_ln_concat(const void* x, const void* lat, int NB, int T, int Q, int C, const void* g0, const void* b0,
+                          const void* g1, const void* b1, float eps, void* kv, void* q, void* stream);
 /* noise_dev (may be null): fp16 ancestral-noise table [slots][n]; the slot is coef_host->c3 (second_order bit 8).
  * lambda_dev (may be null): a per-image guidance table fp32 [batch] (device); element i of the n belongs to image
  * i / (n / batch) and mixes with lambda_dev[image]. NULL uses coef_host->lambda_ (batch is then ignored). */
