@@ -116,9 +116,9 @@ def refiner_components(ckpt_dir, device) -> dict:
                                             str(f["tokenizer_2/vocab.json"]), str(f["tokenizer_2/merges.txt"]))}
 
 
-def find_controlnet_files(ckpt_dir) -> Dict[str, Path]:
-    """A diffusers ControlNetModel directory: {'config': <dir>/config.json, 'weights':
-    <dir>/diffusion_pytorch_model[.fp16].safetensors}. Raises FileNotFoundError naming every missing file."""
+def _model_dir_files(ckpt_dir, what: str) -> Dict[str, Path]:
+    """{'config': <dir>/config.json, 'weights': <dir>/diffusion_pytorch_model[.fp16].safetensors} of a diffusers model
+    directory. Raises FileNotFoundError naming every missing file."""
     root = Path(ckpt_dir)
     found: Dict[str, Path] = {}
     missing = []
@@ -132,5 +132,16 @@ def find_controlnet_files(ckpt_dir) -> Dict[str, Path]:
     else:
         found["weights"] = w
     if missing:
-        raise FileNotFoundError("ControlNet directory is missing: " + ", ".join(missing))
+        raise FileNotFoundError(f"{what} directory is missing: " + ", ".join(missing))
     return found
+
+
+def find_controlnet_files(ckpt_dir) -> Dict[str, Path]:
+    """A diffusers ControlNetModel directory: {'config': <dir>/config.json, 'weights':
+    <dir>/diffusion_pytorch_model[.fp16].safetensors}. Raises FileNotFoundError naming every missing file."""
+    return _model_dir_files(ckpt_dir, "ControlNet")
+
+
+def find_t2i_adapter_files(ckpt_dir) -> Dict[str, Path]:
+    """A diffusers T2IAdapter directory (e.g. TencentARC/t2iadapter_canny_sd15v2), laid out as find_controlnet_files'."""
+    return _model_dir_files(ckpt_dir, "T2I-Adapter")

@@ -228,6 +228,24 @@ CFGPP_API int cfgpp_set_ip_adapter_scale(cfgpp_handle* h, float scale, void* str
   return guarded([&] { unet_of(h).set_ip_scale(scale, (cudaStream_t)stream); });
 }
 
+CFGPP_API int cfgpp_t2i_attach(cfgpp_handle* h, int n_features) {
+  return guarded([&] { unet_of(h).t2i_attach(n_features); });
+}
+
+CFGPP_API int cfgpp_set_t2i_features(cfgpp_handle* h, const void* const* features_dev, void* stream) {
+  return guarded([&] {
+    unet_of(h).set_t2i_features(reinterpret_cast<const __half* const*>(features_dev), (cudaStream_t)stream);
+  });
+}
+
+CFGPP_API int cfgpp_set_t2i_active(cfgpp_handle* h, int on, void* stream) {
+  return guarded([&] { unet_of(h).set_t2i_active(on, (cudaStream_t)stream); });
+}
+
+CFGPP_API int cfgpp_set_t2i_steps(cfgpp_handle* h, const int* on_host, int nsteps, void* stream) {
+  return guarded([&] { unet_of(h).set_t2i_steps(on_host, nsteps, (cudaStream_t)stream); });
+}
+
 // Debug aid (not in the public header): how many step graphs the handle has captured.
 CFGPP_API int cfgpp_dbg_graph_captures(cfgpp_handle* h, int* n) {
   return guarded([&] { *n = unet_of(h).graph_captures(); });

@@ -53,6 +53,18 @@ void run_image_to_nhwc(const void* x, int x_is_half, __half* out, int B, int C, 
                        cudaStream_t stream);
 void run_silu(__half* x, size_t n, cudaStream_t stream);
 
+// ---- t2i_adapter.cu ----------------------------------------------------------------------------------------
+// image [B,C,H,W] NCHW (fp16 or fp32) -> NHWC fp16 [B,H/f,W/f,C*f*f], channel c*f*f + i*f + j = x[b,c,f*y+i,f*x+j]
+void run_pixel_unshuffle(const void* x, int x_is_half, __half* out, int B, int C, int H, int W, int f,
+                         cudaStream_t stream);
+// NHWC 2x2 / stride-2 average pool over even H, W: fp16(((x00 + x01) + x10 + x11) / 4) in fp32 (torch's order)
+void run_avgpool2x2(const __half* x, __half* out, int B, int H, int W, int C, cudaStream_t stream);
+void run_relu(__half* x, size_t n, cudaStream_t stream);                        // in place, x > 0 ? x : +0
+void run_scale(const __half* x, float s, __half* out, size_t n, cudaStream_t stream);  // fp16(float(x) * s)
+// The T2I-Adapter's add into the UNet's down path, a launch of the step graph: when *on != 0, image n of h
+// [NB][per_image] becomes fp16(float(h) + float(feat[n % B])); when *on == 0 nothing is written. per_image % 8 == 0.
+void run_t2i_add(__half* h, const __half* feat, int NB, int B, size_t per_image, const int* on, cudaStream_t stream);
+
 enum StepMode : int {
   STEP_NONE = 0,        // only emit eps_uc / eps_c (the predict_noise seam)
   STEP_DDIM_CFGPP = 1,  // latent_diffusion.py:660-666, latent_sdxl.py:738-744 (fp32 state)
@@ -89,7 +101,9 @@ struct StepEntry {
   StepState s;
   float2 v_ab;          // v-prediction (a, b) = (sqrt(abar), sqrt(1 - abar)); unused by epsilon models
   float control_scale;  // ControlNet conditioning scale
+  int t2i_on;           // T2I-Adapter features added this step (nonzero) or not; fills the record's tail padding
 };
+static_assert(sizeof(StepEntry) == 64, "StepEntry is one 64-byte record");
 // The one device record every step consumer reads (timestep embedding, conv_in, zero convs, the step kernels).
 // noise: base of the ancestral noise table [slots][B,4,H,W] fp16, or null. lambda: the per-image guidance table [B]
 // fp32, or null for the entry's scalar cur.s.coef.lambda. Both are read from the record, so a captured graph survives

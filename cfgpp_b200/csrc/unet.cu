@@ -458,6 +458,9 @@ void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
   prompt_plan_.clear();
   ip_plan_.clear();
   ip_ready_ = false;
+  t2i_feat_.clear();
+  t2i_hw_.clear();
+  t2i_ready_ = false;
   res_.clear();
   res_hw_.clear();
   B_ = batch; NB_ = 2 * batch; H_ = h_lat; W_ = w_lat;
@@ -614,9 +617,11 @@ void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
       for (int j = 0; j < d_.layers_per_block; ++j) {
         const std::string rp = blk + ".resnets." + std::to_string(j);
         h = build_resnet(rp, h, nullptr, Cout, H, W, temb_off(rp));
-        if (d_.down_has_attn[i])
+        if (d_.down_has_attn[i]) {
           h = build_transformer(blk + ".attentions." + std::to_string(j), h, H, W, d_.transformer_layers[i],
                                 d_.num_heads[i]);
+          if (j == d_.layers_per_block - 1) add_t2i_feature(h, H, W);  // before the downsampler
+        }
         skips.push_back(h);
       }
       if (i != L - 1) {
@@ -624,12 +629,16 @@ void Unet::build(int batch, int h_lat, int w_lat, StepArgs* shared_args) {
         H /= 2; W /= 2;
         skips.push_back(h);
       }
+      if (!d_.down_has_attn[i]) add_t2i_feature(h, H, W);  // DownBlock2D: its output, in place under the skip
     }
     {
       const int Cm = d_.block_out_channels[L - 1];
       h = build_resnet("mid_block.resnets.0", h, nullptr, Cm, H, W, temb_off("mid_block.resnets.0"));
       h = build_transformer("mid_block.attentions.0", h, H, W, d_.transformer_layers[L - 1], d_.num_heads[L - 1]);
       h = build_resnet("mid_block.resnets.1", h, nullptr, Cm, H, W, temb_off("mid_block.resnets.1"));
+      add_t2i_feature(h, H, W);  // the feature left over (t2i_n_ = L + 1), of the last down placement's shape
+      CFGPP_REQUIRE(sizing_ || is_cn_ || static_cast<int>(t2i_feat_.size()) == t2i_n_,
+                    "internal: T2I-Adapter placements differ from the attached feature count");
     }
     if (!sizing_) {
       conv_in_out_ = h0.p;
@@ -737,6 +746,22 @@ void Unet::build_control_plan() {
   }
 }
 
+void Unet::add_t2i_feature(Act h, int H, int W) {
+  // in place on the block's output: its producer (proj_out, the downsample conv or a resnet's conv2) computes no row
+  // statistics, and every later reader (the next block's GroupNorm, the downsampler, the skip) runs after the add
+  if (sizing_ || is_cn_ || static_cast<int>(t2i_feat_.size()) >= t2i_n_) return;
+  const int k = static_cast<int>(t2i_feat_.size());
+  const size_t per_image = static_cast<size_t>(H) * W * h.C;
+  __half* feat = alloc_act(static_cast<size_t>(B_) * per_image);
+  t2i_feat_.push_back(Act{feat, h.C});
+  t2i_hw_.push_back(H * W);
+  const int NB = NB_, B = B_;
+  __half* hp = h.p;
+  const int* on = &args_->cur.t2i_on;
+  add_step("t2i_adapter.add" + std::to_string(k),
+           [=](cudaStream_t st) { run_t2i_add(hp, feat, NB, B, per_image, on, st); });
+}
+
 void Unet::run_plan(const std::vector<PlanStep>& plan, cudaStream_t stream) {
   for (const auto& s : plan) s.fn(stream);
 }
@@ -773,6 +798,11 @@ void Unet::require_control_ready() const {
   CFGPP_REQUIRE(!cn_ || cn_image_ready_, "a ControlNet is attached: call cfgpp_set_control_image for the prepared shape");
 }
 
+void Unet::require_t2i_ready() const {
+  CFGPP_REQUIRE(t2i_n_ == 0 || t2i_ready_,
+                "T2I-Adapter features are attached: call cfgpp_set_t2i_features for the prepared plan");
+}
+
 void Unet::upload_entries(cudaStream_t stream) {
   // pageable source: staged before the call returns; the stream orders it after a replay still reading the table
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(step_table_, entries_.data(), sizeof(StepEntry) * nsteps_, cudaMemcpyHostToDevice,
@@ -784,6 +814,7 @@ void Unet::stage_entry(float t, float in_scale, cudaStream_t stream) {
   e.s.t = t;
   e.s.in_scale = in_scale;
   e.control_scale = cn_scale_;
+  e.t2i_on = t2i_on_;
   // cudaMemcpyAsync from pageable memory stages the 64 bytes before returning: `e` may go out of scope
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(&args_->cur, &e, sizeof(e), cudaMemcpyHostToDevice, stream));
 }
@@ -824,6 +855,7 @@ void Unet::unet_forward(const void* z, int z_dtype, float t, float in_scale, __h
   require_fresh_prompt();
   require_control_ready();
   require_ip_ready();
+  require_t2i_ready();
   stage_entry(t, in_scale, stream);
   run_inputs(z, z_dtype == CFGPP_F16 ? 1 : 0, stream);
   run_body(stream);
@@ -844,6 +876,7 @@ std::vector<Unet::ProfEntry> Unet::profile_forward(const void* z, int z_dtype, f
   };
   require_control_ready();
   require_ip_ready();
+  require_t2i_ready();
   stage_entry(t, in_scale, stream);
   mark();
   auto run = [&](const std::vector<PlanStep>& plan, const std::string& prefix) {
@@ -898,6 +931,7 @@ void Unet::set_schedule(int method, int state_dtype, const cfgpp_step_state* ste
   for (int i = 0; i < nsteps; ++i) {
     std::memcpy(&entries_[i].s, &steps[i], sizeof(StepState));
     entries_[i].control_scale = cn_scale_;
+    entries_[i].t2i_on = t2i_on_;
   }
   v_ready_ = false;
   upload_entries(stream);
@@ -980,6 +1014,7 @@ void Unet::run_steps(int first_step, int nsteps, cudaStream_t stream) {
   require_fresh_prompt();
   require_control_ready();
   require_ip_ready();
+  require_t2i_ready();
   ensure_graph(stream);
   CFGPP_CHECK_CUDA(cudaMemcpyAsync(step_counter_, &first_step, sizeof(int), cudaMemcpyHostToDevice, stream));
   for (int i = 0; i < nsteps; ++i) CFGPP_CHECK_CUDA(cudaGraphLaunch(graph_exec_, stream));
@@ -1128,6 +1163,51 @@ void Unet::set_ip_scale(float scale, cudaStream_t stream) {
   // pageable source: staged before the call returns; the stream orders it after a replay still reading the word
   if (prepared_)
     CFGPP_CHECK_CUDA(cudaMemcpyAsync(&args_->ip_scale, &ip_scale_, sizeof(float), cudaMemcpyHostToDevice, stream));
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// T2I-Adapter
+// ------------------------------------------------------------------------------------------------------------
+void Unet::t2i_attach(int n_features) {
+  CFGPP_REQUIRE(!is_cn_, "T2I-Adapter features attach to a UNet handle, not a ControlNet");
+  const int L = d_.num_levels;
+  // the last down block has no downsampler, so the mid-block output always has its shape: an (L+1)-th feature lands
+  // there
+  CFGPP_REQUIRE(n_features == 0 || n_features == L || n_features == L + 1,
+                "a T2I-Adapter for this UNet has num_levels (" + std::to_string(L) + ") or num_levels + 1 features, "
+                "not " + std::to_string(n_features));
+  t2i_n_ = n_features;
+  // the plan changes shape: the next cfgpp_prepare builds it
+  prepared_ = false;
+  graph_valid_ = false;
+  nsteps_ = 0;
+  t2i_ready_ = false;
+}
+
+void Unet::set_t2i_features(const __half* const* features, cudaStream_t stream) {
+  CFGPP_REQUIRE(t2i_n_ > 0, "no T2I-Adapter features attached (cfgpp_t2i_attach)");
+  CFGPP_REQUIRE(prepared_, "call cfgpp_prepare first");
+  CFGPP_REQUIRE(features != nullptr, "null feature table");
+  for (int k = 0; k < t2i_n_; ++k) CFGPP_REQUIRE(features[k] != nullptr, "null T2I feature");
+  for (int k = 0; k < t2i_n_; ++k)
+    CFGPP_CHECK_CUDA(cudaMemcpyAsync(t2i_feat_[k].p, features[k],
+                                     static_cast<size_t>(B_) * t2i_hw_[k] * t2i_feat_[k].C * sizeof(__half),
+                                     cudaMemcpyDeviceToDevice, stream));
+  t2i_ready_ = true;
+}
+
+void Unet::set_t2i_active(int on, cudaStream_t stream) {
+  CFGPP_REQUIRE(!is_cn_, "the T2I word is set on the UNet handle");
+  t2i_on_ = on ? 1 : 0;
+  for (StepEntry& e : entries_) e.t2i_on = t2i_on_;
+  if (prepared_ && nsteps_ > 0) upload_entries(stream);
+}
+
+void Unet::set_t2i_steps(const int* on, int n, cudaStream_t stream) {
+  CFGPP_REQUIRE(prepared_ && nsteps_ > 0, "call cfgpp_set_schedule first");
+  CFGPP_REQUIRE(on != nullptr && n == nsteps_, "one T2I word per schedule entry");
+  for (int i = 0; i < n; ++i) entries_[i].t2i_on = on[i] ? 1 : 0;
+  upload_entries(stream);
 }
 
 void Unet::cond_embed(const void* image, int is_half, int B, int Hi, int Wi, __half* out, cudaStream_t stream) {

@@ -85,6 +85,11 @@ class Unet {
   // already set), and a copy of its tokens [2*batch * n_tokens][D] into tokens_out (may be null)
   void run_image_proj(__half* tokens_out, cudaStream_t stream);
   void set_ip_scale(float scale, cudaStream_t stream);
+  // ---- T2I-Adapter (see cfgpp_t2i_attach) ----
+  void t2i_attach(int n_features);  // 0 detaches
+  void set_t2i_features(const __half* const* features, cudaStream_t stream);
+  void set_t2i_active(int on, cudaStream_t stream);
+  void set_t2i_steps(const int* on_host, int n, cudaStream_t stream);
   // Eager un-fused forward with a CUDA-event pair around every plan entry (profiling aid for bench.py).
   struct ProfEntry {
     std::string name;
@@ -130,6 +135,9 @@ class Unet {
   void run_inputs(const void* z, int z_is_half, cudaStream_t stream);
   void require_control_ready() const;
   void require_ip_ready() const;
+  void require_t2i_ready() const;
+  // UNet handles with T2I features attached: the gated add of the next feature onto h (H x W), in body_plan_
+  void add_t2i_feature(Act h, int H, int W);
   void build_ip_resampler();  // ip_plan_ of an attached Resampler (ip_resampler.cu)
   void require_resampler_weights(const cfgpp_ip_resampler_desc& r) const;
   void upload_entries(cudaStream_t stream);  // entries_ -> step_table_
@@ -224,6 +232,14 @@ class Unet {
   // IP-Adapter Plus: the Resampler's geometry (num_queries = 0: the plain projection, or none) and its input
   cfgpp_ip_resampler_desc ip_rs_{};
   __half* ip_hidden_ = nullptr;  // [NB * seq_len][E]
+
+  // T2I-Adapter: t2i_n_ features (0: none), each a [B, HW, C] buffer of the prepared plan that one gated add per step
+  // adds into its placement (the body walk of build records them in order)
+  int t2i_n_ = 0;
+  int t2i_on_ = 1;           // the word of the un-fused forward and of a new schedule's entries
+  bool t2i_ready_ = false;   // features copied for the current plan
+  std::vector<Act> t2i_feat_;
+  std::vector<int> t2i_hw_;
 
   cudaGraph_t graph_ = nullptr;
   cudaGraphExec_t graph_exec_ = nullptr;

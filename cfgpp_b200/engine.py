@@ -39,6 +39,10 @@ class NativeUNet(nv.NativeHandle):
         self.ip_adapter = None  # the attached ip_adapter.IPAdapter
         self.ip_request = None  # the IPRequest of the running sample() call (bind_control applies it), else None
         self._ip_embeds = None  # the image embeds projected for the prepared plan
+        self.t2i_request = None  # the t2i_adapter.T2IRequest of the running sample() call (bind_control applies it)
+        self._t2i_n = 0  # T2I-Adapter features the native plan places
+        self._t2i_features = None  # the feature list copied into the prepared plan
+        self._t2i_flags = None  # the T2I word of every entry of the current schedule, else None
 
     def _create(self, desc, idx: int) -> None:
         nv.check(self.lib.cfgpp_create_ex(byref(desc), c_size_t(ctypes.sizeof(desc)), c_int(idx), byref(self._h)))
@@ -50,7 +54,7 @@ class NativeUNet(nv.NativeHandle):
         # a failing native prepare() leaves the handle unprepared: forget the old shape and the bound prompt first so
         # that the next call re-plans instead of running on freed buffers
         self.batch, self.latent_hw, self._nsteps, self._bound = 0, (0, 0), 0, None
-        self._control_image = self._ip_embeds = None
+        self._control_image = self._ip_embeds = self._t2i_features = None
         with torch.cuda.device(self.device):
             nv.check(self.lib.cfgpp_prepare(self._h, c_int(batch), c_int(h_lat), c_int(w_lat)))
         self.batch, self.latent_hw = batch, (h_lat, w_lat)
@@ -167,6 +171,9 @@ class NativeUNet(nv.NativeHandle):
         self.set_guidance(guidance)
         if control_scales is not None:
             self.set_control_scales(control_scales)
+        self._t2i_flags = None
+        if self.t2i_request is not None:  # the adapter_conditioning_factor cut, per entry
+            self.set_t2i_steps(self.t2i_request.entry_flags(steps))
 
     def set_guidance(self, guidance: Optional[Sequence[float]] = None):
         """One guidance scale per image of the prepared batch, rounded to fp32, used by every following step (fused
@@ -225,6 +232,8 @@ class NativeUNet(nv.NativeHandle):
         predict_noise, a v-prediction output turned into eps with the entry's own (a, b) as the fused step does, then
         the step kernel's update. Returns (z0t, zt)."""
         z = self.get_state(0)
+        if self._t2i_flags is not None:
+            self.set_t2i_active(self._t2i_flags[i])
         eps_uc, eps_c = self.predict_noise(z, step.t, step.in_scale)
         if self.v_prediction:
             a, b = self.v_coefs[i]
@@ -241,11 +250,14 @@ class NativeUNet(nv.NativeHandle):
     def bind_control(self, request, zt: torch.Tensor, uc, c, pooled=None, time_ids=None, force: bool = False):
         """Attach (or, with request None, detach) the request's ControlNet, prepare for zt's shape, bind the prompt and
         embed the control image: the engine set-up of one controlled or uncontrolled call. Engines are shared between
-        solvers, so an uncontrolled call detaches whatever an earlier call left attached."""
+        solvers, so an uncontrolled call detaches whatever an earlier call left attached. The IP-Adapter and the
+        T2I-Adapter of `ip_request` / `t2i_request` are attached (or detached) the same way."""
         b, _, h, w = zt.shape
         self.attach_controlnet(None if request is None else request.engine)
         ip = self.ip_request
         self.attach_ip_adapter(None if ip is None else ip.adapter)
+        t2i = self.t2i_request
+        self.attach_t2i(0 if t2i is None else len(t2i.features))
         self.prepare(b, h, w)
         self.bind_prompt(uc, c, pooled, time_ids, force=force)
         if request is not None:
@@ -253,6 +265,8 @@ class NativeUNet(nv.NativeHandle):
         if ip is not None:
             self.set_ip_image_embeds(ip.embeds, force=force)
             self.set_ip_adapter_scale(ip.scale)
+        if t2i is not None:
+            self.set_t2i_features(t2i.features, force=force)
 
     # ---- ControlNet ----------------------------------------------------------------------------------------------
     def attach_controlnet(self, cn) -> None:
@@ -356,6 +370,43 @@ class NativeUNet(nv.NativeHandle):
         """The scale s of every decoupled cross-attention: a device word, so the step graph is never recaptured."""
         with torch.cuda.device(self.device):
             nv.check(self.lib.cfgpp_set_ip_adapter_scale(self._h, c_float(float(scale)), nv.stream_ptr()))
+
+    # ---- T2I-Adapter ------------------------------------------------------------------------------------------
+    def attach_t2i(self, n_features: int) -> None:
+        """Expect n_features T2I-Adapter features (0 detaches). A change drops the plan: the next prepare() places one
+        gated add per feature in the down path, and set_t2i_features must run after it."""
+        if n_features == self._t2i_n:
+            return
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_t2i_attach(self._h, c_int(n_features)))
+        self._t2i_n, self._t2i_features = n_features, None
+        self.batch, self.latent_hw, self._nsteps, self._bound, self._control_image = 0, (0, 0), 0, None, None
+
+    def set_t2i_features(self, features: Sequence[torch.Tensor], force: bool = True) -> None:
+        """The adapter's features for the prepared batch (t2i_adapter.NativeT2IAdapter.features: (batch, h, w, C) NHWC
+        fp16 each), copied into the plan; both CFG halves add the same rows. With force False, the same list object
+        already copied for this plan is not copied again."""
+        if not force and self._t2i_features is features:
+            return
+        fs = [f.to(self.device, torch.float16).contiguous() for f in features]
+        assert len(fs) == self._t2i_n and all(f.shape[0] == self.batch for f in fs), "one feature row per image"
+        ptrs = (ctypes.c_void_p * len(fs))(*[f.data_ptr() for f in fs])
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_set_t2i_features(self._h, ptrs, nv.stream_ptr()))
+        self._t2i_features = features
+
+    def set_t2i_active(self, on: bool) -> None:
+        """Whether predict_noise (and every entry of a new schedule) adds the features; clears a per-entry table."""
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_set_t2i_active(self._h, c_int(1 if on else 0), nv.stream_ptr()))
+
+    def set_t2i_steps(self, flags: Sequence[bool]) -> None:
+        """Whether each entry of the current schedule adds the features (t2i_adapter.entry_flags), read on the device:
+        changing it never recaptures the step graph. set_schedule clears it; callback_step follows it."""
+        arr = (c_int * len(flags))(*[1 if f else 0 for f in flags])
+        with torch.cuda.device(self.device):
+            nv.check(self.lib.cfgpp_set_t2i_steps(self._h, arr, c_int(len(flags)), nv.stream_ptr()))
+        self._t2i_flags = list(flags)
 
     # ---- LoRA adapters ----------------------------------------------------------------------------------------
     MAX_LORAS_PER_WEIGHT = 4

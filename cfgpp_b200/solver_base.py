@@ -44,10 +44,12 @@ CONTROL_KWARGS = ("controlnet", "control_image", "controlnet_conditioning_scale"
 
 
 def refuse_control(kwargs: dict, what: str) -> None:
-    """The inversion / editing solvers take no ControlNet and no IP-Adapter."""
+    """The inversion / editing solvers take no ControlNet, no IP-Adapter and no T2I-Adapter."""
     if kwargs.get("controlnet") is not None or kwargs.get("control_image") is not None:
         raise ValueError(f"{what} does not take a ControlNet (text-to-image solvers only)")
     refuse_ip_adapter(kwargs, what)
+    if kwargs.get("t2i_adapter") is not None or kwargs.get("t2i_adapter_image") is not None:
+        raise ValueError(f"{what} does not take a T2I-Adapter (text-to-image solvers only)")
 
 
 def refuse_ip_adapter(kwargs: dict, what: str) -> None:
@@ -79,30 +81,43 @@ class SolverBase(K.KDiffusionMixin, LoraMixin):
     _control = None  # the ControlRequest of the running sample() call (controlnet.control_request), else None
 
     def _controlled(self, kwargs: dict, batch: int, lat_h: int, lat_w: int, run):
-        """run() under the ControlNet that sample()'s keyword arguments ask for (none: the engine is detached)."""
+        """run() under the ControlNet, IP-Adapter and T2I-Adapter that sample()'s keyword arguments ask for (none: the
+        engine is detached)."""
         from .controlnet import control_request
+        from .t2i_adapter import t2i_request
         ip = ip_request(kwargs, batch)
         if ip is not None and ip.adapter.base_cfg != self.unet.cfg:
             raise ValueError(f"ip_adapter was built for {ip.adapter.base_cfg.name}, this solver runs "
                              f"{self.unet.cfg.name} (IP-Adapter: SD v1.5 and SDXL)")
         self._control = control_request(kwargs, batch, 8 * lat_h, 8 * lat_w, self.device)
+        t2i = None
+        if kwargs.get("t2i_adapter") is not None or kwargs.get("t2i_adapter_image") is not None:
+            t2i = t2i_request(kwargs, self.unet.cfg, batch, 8 * lat_h, 8 * lat_w)
         if ip is not None:  # the engine's set-up (bind_control) attaches it; without one it detaches any adapter
             self.unet.ip_request = ip
+        if t2i is not None:  # likewise; the word starts on for the un-fused steps (a schedule sets its own)
+            self.unet.t2i_request = t2i
+            self.unet.set_t2i_active(True)
         try:
             return run()
         finally:
             self._control = None
             if ip is not None:
                 self.unet.ip_request = None
+            if t2i is not None:
+                self.unet.t2i_request = None
 
     def _control_entries(self, steps):
         """The conditioning scale of every entry of `steps`, or None when uncontrolled."""
         return None if self._control is None else self._control.entry_scales(steps)
 
     def _control_step(self, i: int, n: int) -> None:
-        """Sampler step i of n runs un-fused next: its UNet calls take that step's conditioning scale."""
+        """Sampler step i of n runs un-fused next: its UNet calls take that step's conditioning scale and T2I word."""
         if self._control is not None:
             self.unet.set_control_scale(self._control.step_scale(i, n))
+        t2i = getattr(self.unet, "t2i_request", None)
+        if t2i is not None:
+            self.unet.set_t2i_active(t2i.step_on(i, n))
 
     def _init_schedule(self, num_sampling: int, kind: str, device):
         """Sampling parameters (latent_diffusion.py:69-80, latent_sdxl.py:56-67 / :407-418)."""

@@ -82,7 +82,17 @@ def main():
     parser.add_argument("--ip_adapter_scale", type=float, default=1.0)
     parser.add_argument("--image_encoder", type=Path, default=None, metavar="DIR",
                         help="the adapter's CLIP image encoder (config.json + model.safetensors); default: synthetic")
+    parser.add_argument("--t2i_adapter", type=str, default=None, metavar="DIR",
+                        help="a diffusers T2IAdapter directory (config.json + diffusion_pytorch_model"
+                             "[.fp16].safetensors), or a name for seeded synthetic weights")
+    parser.add_argument("--t2i_adapter_image", type=Path, default=None,
+                        help="the adapter's conditioning map (sketch, canny, depth, ...) at exactly the output size; read "
+                             "as grayscale for a 1-channel adapter, RGB otherwise")
+    parser.add_argument("--adapter_conditioning_scale", type=float, default=1.0)
+    parser.add_argument("--adapter_conditioning_factor", type=float, default=1.0)
     args = parser.parse_args()
+    if (args.t2i_adapter is None) != (args.t2i_adapter_image is None):
+        raise SystemExit("--t2i_adapter and --t2i_adapter_image go together")
     if (args.controlnet is None) != (args.control_image is None):
         raise SystemExit("--controlnet and --control_image go together")
     if (args.ip_adapter is None) != (args.ip_adapter_image is None):
@@ -119,6 +129,14 @@ def main():
         control.update(ip_adapter=IPAdapter(args.ip_adapter, args.device, solver.cfg,
                                             image_encoder=str(args.image_encoder) if args.image_encoder else None),
                        ip_adapter_image=Image.open(args.ip_adapter_image), ip_adapter_scale=args.ip_adapter_scale)
+    if args.t2i_adapter is not None:
+        from cfgpp_b200.t2i_adapter import T2IAdapter
+        ad = T2IAdapter(args.t2i_adapter, args.device, base_cfg=solver.cfg)
+        control.update(t2i_adapter=ad, adapter_conditioning_scale=args.adapter_conditioning_scale,
+                       adapter_conditioning_factor=args.adapter_conditioning_factor,
+                       t2i_adapter_image=load_control_image(args.t2i_adapter_image, height, width,
+                                                            "L" if ad.cfg.in_channels == 1 else "RGB",
+                                                            "--t2i_adapter_image"))
     if sdxl:
         refiner = {}
         if args.denoising_end is not None:
@@ -141,14 +159,18 @@ def main():
     print(f"saved {out}")
 
 
-def load_control_image(path: Path, height: int, width: int) -> torch.Tensor:
-    """(1, 3, H, W) RGB in [0, 1]. The image must already have the output size: it is not resized."""
+def load_control_image(path: Path, height: int, width: int, mode: str = "RGB",
+                       flag: str = "--control_image") -> torch.Tensor:
+    """(1, 3, H, W) RGB (mode "RGB") or (1, 1, H, W) grayscale (mode "L") in [0, 1]. The image must already have the
+    output size: it is not resized."""
     import numpy as np
     from PIL import Image
-    img = Image.open(path).convert("RGB")
+    img = Image.open(path).convert(mode)
     if img.size != (width, height):
-        raise SystemExit(f"--control_image is {img.size[0]} x {img.size[1]}, the output is {width} x {height}")
-    return torch.from_numpy(np.asarray(img).copy()).permute(2, 0, 1)[None].float() / 255.0
+        raise SystemExit(f"{flag} is {img.size[0]} x {img.size[1]}, the output is {width} x {height}")
+    x = torch.from_numpy(np.asarray(img).copy())
+    x = x[None] if x.dim() == 2 else x.permute(2, 0, 1)
+    return x[None].float() / 255.0
 
 
 if __name__ == "__main__":

@@ -301,6 +301,61 @@ int cfgpp_ip_adapter_attach_resampler(cfgpp_handle* h, const cfgpp_ip_resampler_
  * adapter). */
 int cfgpp_set_ip_image_hidden_states(cfgpp_handle* h, const void* hidden_dev, void* stream);
 
+/* ---- T2I-Adapter (Mou et al. 2023; diffusers T2IAdapter, `full_adapter` / `full_adapter_xl`): spatial conditioning by
+ * four feature maps computed once per image and added into a UNet handle's down path at every step. An adapter handle
+ * holds the weights under diffusers' keys (`adapter.conv_in.*`, `adapter.body.{i}.in_conv.*`,
+ * `adapter.body.{i}.resnets.{j}.block1.*` (3x3), `adapter.body.{i}.resnets.{j}.block2.*` (1x1)) and runs, on an image
+ * x (batch, in_channels, H, W) in [0, 1], in fp16:
+ *   x = conv_in(pixel_unshuffle(fp16(x), downscale_factor))       (channel c*f*f + i*f + j holds pixel (f*y+i, f*x+j))
+ *   per block i: [x = avgpool2x2(x) if down] [x = in_conv(x) if cin != cout]
+ *                num_res_blocks x { x = fp16(fp16(block2(relu(block1(x)))) + x) };  feature_i = fp16(x * scale)
+ * full (SD):     blocks (c0,c0), (c0,c1,down), (c1,c2,down), (c2,c3,down): features at /f, /2f, /4f, /8f;
+ * full_xl (SDXL): blocks (c0,c0), (c0,c1), (c1,c2,down), (c3,c3) with c2 == c3: features at /f, /f, /2f, /2f.
+ * H and W must be multiples of the total factor (8f for full, 2f for full_xl): the average pool never pads. */
+typedef struct cfgpp_t2i_adapter_desc {
+  int kind;              /* 0: full_adapter (SD v1.5 / SD 2.x), 1: full_adapter_xl (SDXL) */
+  int in_channels;       /* 1 (sketch, canny) or 3 (RGB) */
+  int channels[4];       /* (320, 640, 1280, 1280) */
+  int num_res_blocks;    /* 2 */
+  int downscale_factor;  /* 8 (full) or 16 (full_xl) */
+} cfgpp_t2i_adapter_desc;
+typedef struct cfgpp_t2i_adapter_handle cfgpp_t2i_adapter_handle;
+int cfgpp_t2i_adapter_create(const cfgpp_t2i_adapter_desc* desc, int device, cfgpp_t2i_adapter_handle** out);
+int cfgpp_t2i_adapter_destroy(cfgpp_t2i_adapter_handle* ad);
+int cfgpp_t2i_adapter_load_weight(cfgpp_t2i_adapter_handle* ad, const char* key, const void* data_dev,
+                                  const int64_t* shape, int ndim, int dtype, void* stream);
+/* Checks every weight's exact shape (the error names the first missing or mis-shaped key) and packs the 3x3 convs. */
+int cfgpp_t2i_adapter_finalize_weights(cfgpp_t2i_adapter_handle* ad, void* stream);
+/* image_dev: (batch, in_channels, H, W) NCHW of `dtype` (fp16 / fp32), batch 1..8. features_out[k]: device buffers for
+ * feature k, NHWC fp16 (batch, h_k, w_k, channels_k), written already multiplied by `scale`. The launch plan is built
+ * for (batch, H, W) at the first call and kept until another shape arrives. */
+int cfgpp_t2i_adapter_forward(cfgpp_t2i_adapter_handle* ad, const void* image_dev, int dtype, int batch, int H, int W,
+                              float scale, void* const* features_out, void* stream);
+/* FLOPs of the prepared forward and its workspace bytes (0 before the first forward). */
+int cfgpp_t2i_adapter_stats(cfgpp_t2i_adapter_handle* ad, double* flops, size_t* workspace_bytes);
+/* On a UNet handle: expect n_features T2I-Adapter features (0 detaches). Either drops the prepared plan. The next
+ * cfgpp_prepare places feature k, in order, on (diffusers' down_intrablock_additional_residuals):
+ *   a CrossAttnDownBlock2D: the output of its last (resnet, attention) pair, before its downsampler (so the skip
+ *   tensor and the downsampler's input are the sum); a DownBlock2D: its output, after its downsampler if it has one;
+ *   a feature left after the down blocks: the mid-block output.
+ * It fails unless n_features is num_levels or num_levels + 1 (the last down block has no downsampler, so the mid-block
+ * output always has the last down placement's shape). Each placement is one launch in the step graph: rows r of h [2*batch, HW, C] become
+ *   h = fp16(float(h) + float(feature[r mod batch]))
+ * when the step's T2I word is on, and are left untouched (no write) when it is off. The adds come before an attached
+ * ControlNet's residuals; the ControlNet's own down path gets no features. */
+int cfgpp_t2i_attach(cfgpp_handle* h, int n_features);
+/* features_dev[k]: (batch, h_k, w_k, C_k) NHWC fp16 for the prepared shape, copied into the plan's buffers (both CFG
+ * halves read the same rows). cfgpp_run_steps / cfgpp_unet_forward of a handle with features attached fail until it
+ * has been called after the last cfgpp_prepare. */
+int cfgpp_set_t2i_features(cfgpp_handle* h, const void* const* features_dev, void* stream);
+/* The T2I word of cfgpp_unet_forward and of every entry of a new schedule (on = 1 after create); clears the per-entry
+ * table (enqueued on `stream`). */
+int cfgpp_set_t2i_active(cfgpp_handle* h, int on, void* stream);
+/* One word per entry of the current schedule (host [nsteps], nonzero = on), read on the device by the step selection:
+ * diffusers' `i < int(num_inference_steps * adapter_conditioning_factor)`. cfgpp_set_schedule and cfgpp_set_t2i_active
+ * clear it. */
+int cfgpp_set_t2i_steps(cfgpp_handle* h, const int* on_host, int nsteps, void* stream);
+
 /* ---- AutoencoderKL decoder (SURVEY.md section 8 f2): replaces `self.vae.decode(zt / scaling_factor).sample` of
  * latent_sdxl.py:155-164 (VAE madebyollin/sdxl-vae-fp16-fix, :44) and latent_diffusion.py:123-129 on the same conv /
  * GEMM / GroupNorm kernels. Weights under the diffusers AutoencoderKL keys (`post_quant_conv.*`, `decoder.*`). ----- */
@@ -513,6 +568,17 @@ int cfgpp_op_upsample2x(const void* x, void* out, int B, int H, int W, int C, vo
 int cfgpp_op_image_to_nhwc(const void* x, int dtype, void* out, int B, int C, int H, int W, int Cp, void* stream);
 /* In-place SiLU on n fp16 values: x = fp16(x / (1 + expf(-x))) in fp32. */
 int cfgpp_op_silu(void* x, size_t n, void* stream);
+/* T2I-Adapter: x [B,C,H,W] fp16 / fp32 (dtype) -> out [B,H/f,W/f,C*f*f] NHWC fp16, channel c*f*f + i*f + j = fp16(x[b,
+ * c, f*y+i, f*x+j]) (torch's pixel_unshuffle of fp16(x)); H, W multiples of f. */
+int cfgpp_op_pixel_unshuffle(const void* x, int dtype, void* out, int B, int C, int H, int W, int f, void* stream);
+/* NHWC 2x2 average pool, stride 2, even H, W: out = fp16(((x00 + x01) + x10 + x11) / 4) in fp32, C % 8 == 0. */
+int cfgpp_op_avgpool2x2(const void* x, void* out, int B, int H, int W, int C, void* stream);
+/* In-place ReLU on n fp16 values (x > 0 ? x : +0); out = fp16(x * s) on n fp16 values (out may be x). */
+int cfgpp_op_relu(void* x, size_t n, void* stream);
+int cfgpp_op_scale(const void* x, float s, void* out, size_t n, void* stream);
+/* The T2I gated add: when *on_dev (int, device) is nonzero, image n of h [NB][per_image] becomes fp16(float(h) +
+ * float(feat[n mod B])), feat [B][per_image]; when it is zero, nothing is written. per_image % 8 == 0. */
+int cfgpp_op_t2i_add(void* h, const void* feat, int NB, int B, size_t per_image, const int* on_dev, void* stream);
 /* AutoencoderKL decoder front: z [B,4,HW] of z_dtype -> fp16(w . fp16(z / scaling) + bias), w [4][4], out [B,4,HW]. */
 int cfgpp_op_vae_latent_prep(const void* z, int z_dtype, float scaling, const void* w, const void* bias, void* out,
                              int B, int HW, void* stream);
