@@ -2,7 +2,8 @@
 
 `test_gpu_gemm.py`, `test_gpu_norms.py` and `test_gpu_attention.py` walk these tables through their derivation
 functions; `test_production_lists_cpu.py` asserts that every full-size model, text tower, vision tower, ControlNet-capable
-UNet and IP-Adapter is listed, so a model added without sizes fails on any machine."""
+UNet, IP-Adapter (plain and Plus) and T2I-capable UNet is listed, so a model added without sizes fails on any
+machine."""
 
 # latent (h, w) per full-size UNet config of `config.CONFIGS`: the native resolution first, then the non-square sizes
 # whose levels are not multiples of 64 tokens (1216x832: 76x52 = 3952 tokens at level 1, 19x13 at level 3;
@@ -35,6 +36,25 @@ CONTROL_IMAGE_BATCHES = (1, 8)
 # (1280) and the ViT-H adapters for SDXL (1024); each projects one image embedding to IP_TOKENS image tokens
 IP_ADAPTERS = (("sd15", 1024), ("sdxl", 1280), ("sdxl", 1024))
 IP_TOKENS = 4
+
+# IP-Adapter Plus: (base UNet, ViT-H hidden width E); the Resampler (`ip_adapter.plus_geometry`) reads the tower's
+# penultimate hidden states and gives num_queries = 16 image tokens. It runs at UNet batch NB = 2, 4 and 16 (1, 2 and
+# 8 images with CFG)
+IP_PLUS_ADAPTERS = (("sd15", 1280), ("sdxl", 1280))
+IP_PLUS_NB = (2, 4, 16)
+
+# T2I-Adapters: base UNet -> latent (h, w) (the adapter image is 8h x 8w), for every UNet a T2I-Adapter conditions
+# (not the SDXL refiner: the refiner runs after the hand-off without features). The UNet's sizes, plus SD v1.5 at
+# 512x768, whose adapter levels are 96/48/24/12 wide and take the im2col A tile; the adapter runs for 1 image and the
+# engine's maximum of 8, on 3-channel and 1-channel (sketch, canny) images
+T2I_ADAPTER_SIZES = {
+    "sd15": ((64, 64), (64, 96)),
+    "sd2": ((96, 96), (96, 64)),
+    "sd2_base": ((64, 64),),
+    "sdxl": ((128, 128), (152, 104)),
+}
+T2I_ADAPTER_BATCHES = (1, 8)
+T2I_IN_CHANNELS = (3, 1)
 
 # CLIP vision towers of `vision_encoder` (`<name>_config`) and the image batches they encode
 VISION_TOWERS = {"vit_h": (1, 2, 8), "vit_bigg": (1, 2, 8)}
@@ -83,6 +103,11 @@ def unet_attn_launches(cfg, h, w, NB=4):
 def controlnet_sizes():
     """(model, h, w) over CONTROLNET_SIZES, in table order."""
     return [(m, h, w) for m, sizes in CONTROLNET_SIZES.items() for h, w in sizes]
+
+
+def t2i_sizes():
+    """(model, h, w) over T2I_ADAPTER_SIZES, in table order."""
+    return [(m, h, w) for m, sizes in T2I_ADAPTER_SIZES.items() for h, w in sizes]
 
 
 def vision_config(tower):

@@ -44,16 +44,18 @@ P·V at K = 16384). Every case asserts a finite output (except the overflow case
 
 The production launches are derived from the model configs at the sizes of `production.py` (every full-size UNet at
 each of its latent sizes, UNet batch 4; the VAE decoder and encoder at each image size; every text tower at
-M = B·77), run once per distinct launch signature in their production layouts; `test_unet_launch_list_matches_profile`
-checks the derived UNet GEMM and attention lists against the launches the native UNet reports. The LayerNorm-fold
-consumers run their shapes as plain linears here (the fold arithmetic has its own relative gate in
-`test_gpu_gemm_epilogues.py`)."""
+M = B·77; the ControlNets, vision towers, IP-Adapters and T2I-Adapters), run once per distinct launch signature in
+their production layouts; `test_unet_launch_list_matches_profile` checks the derived UNet GEMM and attention lists
+against the launches the native UNet reports, `test_t2i_adapter_launch_list_matches_plan_flops` the T2I-Adapter's
+against its plan's FLOPs. The LayerNorm-fold consumers run their shapes as plain linears here (the fold arithmetic has
+its own relative gate in `test_gpu_gemm_epilogues.py`)."""
 import zlib
 
 import pytest
 import torch
 import torch.nn.functional as F
 
+import production as P
 from test_gpu_norms import Gate, ulp16
 
 pytestmark = pytest.mark.gpu
@@ -61,7 +63,8 @@ dev = torch.device("cuda:0")
 EPS = 2.0 ** -23
 U = 2.0 ** -24
 PIECE = 1 << 24  # fp64 elements of one [rows, N] slice of the reference
-SEEN = {"bn": set(), "a_mode": set(), "streamk": set(), "pieces3": 0, "addend": set(), "cases": 0}
+SEEN = {"bn": set(), "a_mode": set(), "streamk": set(), "pieces3": 0, "addend": set(), "cases": 0, "forced": 0,
+        "t2i_conv": set()}
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -80,8 +83,9 @@ def gen(seed):
 
 # ------------------------------------------------------------------------------------------------ schedules
 
-def record(sched, modes, *, streamk=None, pieces3=False):
-    """Note what a gated launch covered; assert the path its test names."""
+def record(sched, modes, *, streamk=None, pieces3=False, forced=False):
+    """Note what a gated launch covered (`forced`: its tile width, stream-K split or A tile was forced); assert the
+    path its test names."""
     if streamk is not None:
         assert sched["streamk"] == streamk, f"expected stream-K {streamk}, schedule {sched}"
     if pieces3:
@@ -92,6 +96,7 @@ def record(sched, modes, *, streamk=None, pieces3=False):
     SEEN["pieces3"] += sched["max_pieces"] >= 3
     SEEN["addend"] |= modes
     SEEN["cases"] += 1
+    SEEN["forced"] += forced
 
 
 def addend_modes(addend, rpg, M):
@@ -315,7 +320,7 @@ def run_linear(what, a, w, *, bias=None, addend=None, rpg=1, a2=None, geglu=Fals
         sched["sk_kind"] = "natural"
     out = nv.op_linear(a, w, addend=addend, out=addend if in_place else None, **kw)
     modes = addend_modes(addend, rpg, M)
-    record(sched, modes, streamk=expect_sk, pieces3=pieces3)
+    record(sched, modes, streamk=expect_sk, pieces3=pieces3, forced=bool(force_bn or force_streamk))
     mode = "+".join(sorted(modes)) + (" in place" if in_place else "")
     tag = (f"{what} BN{sched['bn']} grid {sched['grid']} tiles {sched['tiles']}"
            f"{' stream-K x' + str(sched['max_pieces']) if sched['streamk'] else ''} {mode}")
@@ -340,7 +345,7 @@ def run_conv(what, x, w, *, bias=None, addend=None, rpg=1, stride=1, pad=1, forc
         assert sched["a_mode"] == expect_mode, f"{what}: expected the {expect_mode} A tile, schedule {sched}"
     out = nv.op_conv3x3_ex(x, w, addend=addend, **kw).reshape(M, w.shape[0])
     modes = addend_modes(addend, rpg, M)
-    record(sched, modes, streamk=expect_sk, pieces3=pieces3)
+    record(sched, modes, streamk=expect_sk, pieces3=pieces3, forced=bool(force_bn or force_im2col))
     mode = "+".join(sorted(modes))
     tag = (f"{what} s{stride}p{pad} {sched['a_mode']} BN{sched['bn']} tiles {sched['tiles']}"
            f"{' stream-K x' + str(sched['max_pieces']) if sched['streamk'] else ''} {mode}")
@@ -946,6 +951,37 @@ def controlnet_embed_launches(cn_cfg, h, w, B):
     return out
 
 
+def t2i_adapter_gemm_launches(cfg, H, W, B):
+    """The GEMM / conv launches of a T2I-Adapter (`t2i_adapter.T2IAdapterConfig`) on B images of H x W, as
+    `T2IAdapter::prepare` issues them: conv_in, a 3x3 conv over the pixel-unshuffled image (Cin = in_channels·f²);
+    per block, after the 2x2 pool of a down block, in_conv (a 1x1 conv as a linear) where the width changes, then per
+    resnet block1 (3x3 conv) and block2 (1x1 linear with the residual added in place). Names are the weights'
+    `adapter.*` keys; FLOPs 2·M·N·K, as `GemmOp::flops` counts them."""
+    f = cfg.downscale_factor
+    h, w, out = H // f, W // f, []
+
+    def conv(name, cin, cout):
+        out.append(dict(name=name, kind="conv", B=B, H=h, W=w, Cin=cin, Cout=cout, stride=1, pad=1,
+                        flops=2.0 * B * h * w * cout * 9 * cin))
+
+    def lin(name, N, K, **lay):
+        M = B * h * w
+        out.append(dict(name=name, kind="linear", M=M, N=N, K=K, flops=2.0 * M * N * K, **lay))
+
+    conv("adapter.conv_in", cfg.in_channels * f * f, cfg.channels[0])
+    for i, (cin, cout, down) in enumerate(cfg.blocks()):
+        p = f"adapter.body.{i}"
+        if down:
+            h, w = h // 2, w // 2
+        if cin != cout:
+            lin(f"{p}.in_conv", cout, cin)
+        for j in range(cfg.num_res_blocks):
+            conv(f"{p}.resnets.{j}.block1", cout, cout)
+            lin(f"{p}.resnets.{j}.block2", cout, cout, addend="in_place")
+    assert cfg.feature_shapes(H, W)[-1] == (cfg.channels[-1], h, w)
+    return out
+
+
 def zero_conv_launches(cn_cfg, h, w, NB=4):
     """The zero convs of `Unet::build_control_plan`: per ControlNet residual k (`residual_channels` order, the last one
     the mid block's) a 1x1 convolution as a linear over the residual's NB·HW rows, N = K = C, with the scaled-residual
@@ -981,13 +1017,35 @@ def vision_gemm_launches(vcfg, tower, B):
             dict(name=f"{tower} fc2", kind="linear", M=M, N=D, K=I, addend="residual")]
 
 
-def ip_adapter_gemm_launches(cfg, E, n_tokens, NB=4):
+def resampler_gemm_launches(g, D, T, NB):
+    """The GEMMs of an IP-Adapter Plus Resampler of geometry g (`ip_adapter.plus_geometry`) giving D-wide tokens, on
+    NB rows of T hidden states, as `Unet::build_ip_resampler` issues them (layer 0 stands for all: the layers share
+    their shapes): proj_in, per layer to_q, to_kv over the hidden states and the latents, to_out and the feed-forward
+    (in place into the latents), then proj_out. Names are the weights' `image_proj.*` keys."""
+    Q, E, dim, inner, F = g["num_queries"], g["embed_dim"], g["dim"], 64 * g["heads"], g["ff_mult"] * g["dim"]
+    lin = lambda n, M, N, K, **kw: dict(name="image_proj." + n, kind="linear", M=M, N=N, K=K, **kw)  # noqa: E731
+    return [lin("proj_in", NB * T, dim, E), lin("layers.0.0.to_q", NB * Q, inner, dim, bias=False),
+            lin("layers.0.0.to_kv", NB * (T + Q), 2 * inner, dim, bias=False),
+            lin("layers.0.0.to_out", NB * Q, dim, inner, bias=False, addend="in_place"),
+            lin("layers.0.1.1", NB * Q, F, dim, bias=False),
+            lin("layers.0.1.3", NB * Q, dim, F, bias=False, addend="in_place"),
+            lin("proj_out", NB * Q, D, dim)]
+
+
+def ip_adapter_gemm_launches(cfg, E, n_tokens, NB=4, resampler=False):
     """An IP-Adapter's GEMMs in the UNet's image plan at UNet batch NB: image_proj.proj (M = NB, N = n_tokens·D, K = E,
-    bias), then per transformer block attn2.to_kv_ip (M = NB·n_tokens, N = 2·Cp over heads zero-padded to 64-multiples,
-    K = D, no bias)."""
+    bias), or with `resampler` the Plus adapter's Resampler (`plus_geometry(cfg, E)`, over the hidden states of the
+    tower that E selects; n_tokens must be its num_queries), then per transformer block attn2.to_kv_ip
+    (M = NB·n_tokens, N = 2·Cp over heads zero-padded to 64-multiples, K = D, no bias)."""
     import production as P
     D = cfg.cross_attention_dim
-    out = [dict(name="image_proj.proj", kind="linear", M=NB, N=n_tokens * D, K=E)]
+    if resampler:
+        from cfgpp_b200 import ip_adapter as IP
+        g = IP.plus_geometry(cfg, E)
+        assert n_tokens == g["num_queries"], f"the Resampler gives {g['num_queries']} tokens, not {n_tokens}"
+        out = resampler_gemm_launches(g, D, IP.plus_encoder_config(cfg, E).num_positions, NB)
+    else:
+        out = [dict(name="image_proj.proj", kind="linear", M=NB, N=n_tokens * D, K=E)]
     for l in P.unet_attn_launches(cfg, 8, 8):  # the block list does not depend on the latent size
         if l["name"].endswith(".attn2.sdpa"):
             H, hd = l["heads"], l["hd"]
@@ -1014,7 +1072,8 @@ def unique_launches(launches):
 
 def production_lists():
     """{(model, size): [(case id, launch)]} over `production.py`: each UNet at each latent size, the VAE at each image
-    size, each text tower at each prompt batch. Launches are unique within a list, not across lists."""
+    size, each text tower at each prompt batch, and the ControlNets, vision towers, IP-Adapters (plain and Plus) and
+    T2I-Adapters. Launches are unique within a list, not across lists."""
     import production as P
     from cfgpp_b200 import config as C
     from cfgpp_b200.text_encoder import CLIP_CONFIGS
@@ -1037,6 +1096,38 @@ def production_lists():
     for m, E in P.IP_ADAPTERS:
         out[("ip_adapter", m, E)] = [(f"ip-{m}-E{E}-{i}-{l['name']}", l) for i, l in
                                      enumerate(unique_launches(ip_adapter_gemm_launches(C.CONFIGS[m](), E, P.IP_TOKENS)))]
+    out.update(adapter_production_lists())
+    return out
+
+
+def ip_plus_launches(m, E):
+    """An IP-Adapter Plus's launches (`ip_adapter_gemm_launches` with the Resampler) at every UNet batch of
+    IP_PLUS_NB, each name prefixed with its NB."""
+    from cfgpp_b200 import config as C, ip_adapter as IP
+    cfg = C.CONFIGS[m]()
+    Q = IP.plus_geometry(cfg, E)["num_queries"]
+    return [dict(l, name=f"NB{NB} {l['name']}") for NB in P.IP_PLUS_NB
+            for l in ip_adapter_gemm_launches(cfg, E, Q, NB, resampler=True)]
+
+
+def t2i_launches(m, h, w):
+    """A T2I-Adapter's launches for the UNet m on an h x w latent (8h x 8w images) at every batch and image channel
+    count of `production.py`, each name prefixed with them."""
+    from cfgpp_b200 import config as C, t2i_adapter as T
+    return [dict(l, name=f"B{B} C{ci} {l['name']}") for ci in P.T2I_IN_CHANNELS for B in P.T2I_ADAPTER_BATCHES
+            for l in t2i_adapter_gemm_launches(T.t2i_adapter_config(C.CONFIGS[m](), ci), 8 * h, 8 * w, B)]
+
+
+def adapter_production_lists():
+    """{("ip_adapter_plus", model, E): [(case id, launch)]} over IP_PLUS_ADAPTERS and {("t2i_adapter", model, size):
+    [(case id, launch)]} over T2I_ADAPTER_SIZES."""
+    out = {}
+    for m, E in P.IP_PLUS_ADAPTERS:
+        out[("ip_adapter_plus", m, E)] = [(f"ip-plus-{m}-E{E}-{i}-{l['name']}", l)
+                                          for i, l in enumerate(unique_launches(ip_plus_launches(m, E)))]
+    for m, h, w in P.t2i_sizes():
+        out[("t2i_adapter", m, (h, w))] = [(f"t2i-{P.size_tag(m, h, w)}-{i}-{l['name']}", l)
+                                           for i, l in enumerate(unique_launches(t2i_launches(m, h, w)))]
     return out
 
 
@@ -1099,7 +1190,9 @@ def run_production(l, family):
             addend, rpg = temb_all[:, l["temb_off"]:l["temb_off"] + Cout], (H // s) * (W // s)
         elif l.get("addend") == "residual":
             addend = mk(Mo, Cout)
-        out, _ = run_conv(name, x, w, bias=b, addend=addend, rpg=rpg, stride=s, pad=l["pad"], family=family)
+        out, sched = run_conv(name, x, w, bias=b, addend=addend, rpg=rpg, stride=s, pad=l["pad"], family=family)
+        if " adapter." in name:  # a T2I-Adapter convolution: its A tile and image batch
+            SEEN["t2i_conv"].add((sched["a_mode"], B))
         if "cout_real" in l:
             assert (out[:, l["cout_real"]:].view(torch.int16) == 0).all(), f"{name}: padded channels are not +0"
         return
@@ -1259,18 +1352,47 @@ def test_controlnet_launch_list_matches_profile(model, hw):
     check_launch_lists_against_profile(model, hw, hw, controlnet=True)
 
 
+@pytest.mark.parametrize("in_channels", P.T2I_IN_CHANNELS)
+@pytest.mark.parametrize("model", list(P.T2I_ADAPTER_SIZES))
+def test_t2i_adapter_launch_list_matches_plan_flops(model, in_channels):
+    """The native T2I-Adapter (synthetic weights) at every production size and batch: the GEMM FLOPs its plan counts
+    (`T2IAdapter::add_gemm`, GEMMs only) equal the sum over `t2i_adapter_gemm_launches`, so the derived list can
+    neither miss nor invent a launch."""
+    from cfgpp_b200 import config as C, t2i_adapter as T
+    cfg = T.t2i_adapter_config(C.CONFIGS[model](), in_channels)
+    ad = T.NativeT2IAdapter(cfg, T.synthetic_t2i_adapter_state_dict(cfg, seed=5, device=dev), dev)
+    try:
+        for h, w in P.T2I_ADAPTER_SIZES[model]:
+            for B in P.T2I_ADAPTER_BATCHES:
+                image = torch.rand(B, in_channels, 8 * h, 8 * w, generator=gen(B * h + w), device=dev)
+                feats = ad.features(image)
+                assert all(torch.isfinite(f).all() for f in feats)
+                got = ad.stats["flops"]
+                want = sum(l["flops"] for l in t2i_adapter_gemm_launches(cfg, 8 * h, 8 * w, B))
+                print(f"[gemm] t2i {model} C{in_channels} {8 * w}x{8 * h} B{B}: plan {got:.6g} FLOPs, derived {want:.6g}")
+                assert abs(got - want) <= 1e-9 * want, f"{model} {8 * w}x{8 * h} B{B}: plan {got}, derived {want}"
+    finally:
+        ad.close()
+
+
 # ================================================================================================= coverage (last)
 
 def test_zz_coverage():
-    """Over the module: every tile width, both conv A-tile modes, natural and forced stream-K, tiles of >= 3 pieces and
-    every addend mode (the ControlNet zero convs' scaled residual included) ran under the per-element gates."""
+    """Over the module: every tile width, both conv A-tile modes, natural and forced stream-K, tiles of >= 3 pieces,
+    every addend mode (the ControlNet zero convs' scaled residual included) and the T2I-Adapter's convolutions on both
+    A tiles at 1 and 8 images ran under the per-element gates. The 64-wide tile and the forced split are reached only
+    by the launches that force them (the sweeps), so they are asserted when forced launches ran."""
     if SEEN["cases"] < 500:
         pytest.skip(f"only {SEEN['cases']} gated launches ran: coverage is asserted over the whole module")
-    print(f"[gemm coverage] {SEEN['cases']} gated launches: BN {sorted(SEEN['bn'])}, A tile {sorted(SEEN['a_mode'])}, "
-          f"stream-K {sorted(str(s) for s in SEEN['streamk'])}, {SEEN['pieces3']} with >= 3 pieces per tile, "
-          f"addend {sorted(SEEN['addend'])}")
-    assert SEEN["bn"] >= {64, 128, 160, 256}
+    print(f"[gemm coverage] {SEEN['cases']} gated launches ({SEEN['forced']} forced): BN {sorted(SEEN['bn'])}, "
+          f"A tile {sorted(SEEN['a_mode'])}, stream-K {sorted(str(s) for s in SEEN['streamk'])}, {SEEN['pieces3']} with "
+          f">= 3 pieces per tile, addend {sorted(SEEN['addend'])}, T2I convs {sorted(SEEN['t2i_conv'])}")
+    assert SEEN["bn"] >= {128, 160, 256}
     assert SEEN["a_mode"] >= {"linear", "tiled", "im2col"}
-    assert SEEN["streamk"] >= {None, "natural", "forced"}
+    assert SEEN["streamk"] >= {None, "natural"}
     assert SEEN["pieces3"] > 0
     assert SEEN["addend"] >= {"none", "residual", "temb_staged", "temb_rows", "scaled_residual"}
+    assert SEEN["t2i_conv"] >= {(mode, B) for mode in ("tiled", "im2col") for B in (1, 8)}, SEEN["t2i_conv"]
+    if SEEN["forced"]:
+        assert 64 in SEEN["bn"]
+        assert "forced" in SEEN["streamk"]

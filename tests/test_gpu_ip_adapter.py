@@ -108,35 +108,38 @@ def test_fused_kernel_sweep(image, hd):
 
 
 def _attn2_cases():
-    """The distinct cross-attention launch shapes of SD v1.5 512² and SDXL 1024² / 1216x832 (`production.py`)."""
+    """The distinct cross-attention launch shapes of SD v1.5 512² and SDXL 1024² / 1216x832 (`production.py`), with
+    the plain adapter's IP_TOKENS image tokens and the Plus adapter's num_queries (`ip_adapter.plus_geometry`)."""
     import production as P
-    from cfgpp_b200 import config as C
+    from cfgpp_b200 import config as C, ip_adapter as IP
     seen, cases = set(), []
-    for m, h, w in P.unet_sizes():
-        if m not in ("sd15", "sdxl"):
-            continue
-        for l in P.unet_attn_launches(C.CONFIGS[m](), h, w):
-            shape = (l["heads"], l["Nq"], l["hd"])
-            if l["name"].endswith("attn2.sdpa") and shape not in seen:
-                seen.add(shape)
-                cases.append(pytest.param(*shape, id=f"{P.size_tag(m, h, w)}-H{shape[0]}-{shape[1]}-hd{shape[2]}"))
+    for n_img in (P.IP_TOKENS, IP.plus_geometry(C.CONFIGS["sd15"](), 1280)["num_queries"]):
+        for m, h, w in P.unet_sizes():
+            if m not in ("sd15", "sdxl"):
+                continue
+            for l in P.unet_attn_launches(C.CONFIGS[m](), h, w):
+                shape = (l["heads"], l["Nq"], l["hd"], n_img)
+                if l["name"].endswith("attn2.sdpa") and shape not in seen:
+                    seen.add(shape)
+                    tag = f"{P.size_tag(m, h, w)}-H{shape[0]}-{shape[1]}-hd{shape[2]}"
+                    cases.append(pytest.param(*shape, id=tag if n_img == P.IP_TOKENS else f"{tag}-img{n_img}"))
     return cases
 
 
-@pytest.mark.parametrize("H,Nq,hd", _attn2_cases())
+@pytest.mark.parametrize("H,Nq,hd,n_img", _attn2_cases())
 @pytest.mark.parametrize("s", [0.5, 1.0])
-def test_production_attn2_shapes(H, Nq, hd, s):
-    """Every attn2 launch of SD v1.5 512² and SDXL 1024² / 1216x832 at UNet batch 4 with 4 image tokens (every adapter
-    in scope), peaked text and image softmaxes, in the UNet's layouts: q from its own buffer, K / V and K2 / V2 column
-    slices of the prompt's and the image's K‖V buffers."""
+def test_production_attn2_shapes(H, Nq, hd, n_img, s):
+    """Every attn2 launch of SD v1.5 512² and SDXL 1024² / 1216x832 at UNet batch 4 with 4 image tokens (the plain
+    adapter) and 16 (IP-Adapter Plus), peaked text and image softmaxes, in the UNet's layouts: q from its own buffer,
+    K / V and K2 / V2 column slices of the prompt's and the image's K‖V buffers."""
     NB, hdp = 4, padded(hd)
-    g = gen(Nq * 31 + H * 7 + hd + int(4 * s))
+    g = gen(Nq * 31 + H * 7 + hd + int(4 * s) + 1000 * (n_img - 4))  # the 4-token cases keep their inputs
     q, k, v = family("peaked", g, NB, Nq, 77, H, hd)
     u = torch.zeros(H, hd, device=dev)
-    k2, v2 = image_tokens("peaked", g, NB, 4, H, hd, u)
+    k2, v2 = image_tokens("peaked", g, NB, n_img, H, hd, u)
     k, v = fused(heads(k, hdp), heads(v, hdp))
     k2, v2 = fused(heads(k2, hdp), heads(v2, hdp))
-    check_ip(f"NB{NB} H{H} {Nq}x77+4 hd{hd} s={s}", heads(q, hdp), k, v, k2, v2, s, H, hd)
+    check_ip(f"NB{NB} H{H} {Nq}x77+{n_img} hd{hd} s={s}", heads(q, hdp), k, v, k2, v2, s, H, hd)
 
 
 @pytest.mark.parametrize("hd", HEAD_DIMS)

@@ -1,20 +1,22 @@
 """IP-Adapter Plus on the GPU: the vision tower's hidden-state output, the Resampler's LayerNorm-concat kernel
-(`ln_concat_kernel`, norm.cu), every Resampler launch at the production sizes under the existing per-element gates, and
-the Plus adapter inside the UNet executor and through sample(). Every measured error is printed."""
+(`ln_concat_kernel`, norm.cu), the Resampler's attention and LayerNorm launches at the production sizes under the
+existing per-element gates (its GEMMs are in `test_gpu_gemm.py`'s production lists), and the Plus adapter inside the
+UNet executor and through sample(). Every measured error is printed."""
 import pytest
 import torch
 
 import ip_adapter_plus_oracle as PO
+import production as P
 from test_gpu_ip_adapter import TOL, _bind, _captures, _inputs, _native, _net, _trajectory, dev
 
 pytestmark = pytest.mark.gpu
 
-# (base UNet, Resampler geometry) of the released Plus adapters; both read ViT-H/14's 257 x 1280 hidden states
-PLUS = {"sd15": dict(num_queries=16, embed_dim=1280, dim=768, heads=12, depth=4, ff_mult=4),
-        "sdxl": dict(num_queries=16, embed_dim=1280, dim=1280, heads=20, depth=4, ff_mult=4)}
-D_OF = {"sd15": 768, "sdxl": 2048}
-T_VIT_H = 257
-RESAMPLER_NB = (2, 4, 16)
+
+def _geometry(name):
+    """(Resampler geometry, token width D, hidden-state rows T) of the Plus adapter of IP_PLUS_ADAPTERS for `name`."""
+    from cfgpp_b200 import config as C, ip_adapter as IP
+    cfg, E = C.CONFIGS[name](), dict(P.IP_PLUS_ADAPTERS)[name]
+    return IP.plus_geometry(cfg, E), cfg.cross_attention_dim, IP.plus_encoder_config(cfg, E).num_positions
 
 
 def _plus(cfg, key="plus-test"):
@@ -84,7 +86,7 @@ def test_ln_concat_kernel(NB, C):
     from test_gpu_norms import ln_check, ln_inputs
     from test_gpu_gemm import gen
     g = gen(1000 * NB + C)
-    T, Q = T_VIT_H, 16
+    T, Q = P.vision_config("vit_h").num_positions, 16
     x, g0, b0 = ln_inputs(g, NB * T, C, 100.0, const_every=7)
     lat, g1, b1 = ln_inputs(g, NB * Q, C, 100.0)
     x, lat = x.reshape(NB, T, C), lat.reshape(NB, Q, C)
@@ -99,38 +101,23 @@ def test_ln_concat_kernel(NB, C):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# every Resampler launch at the production sizes, under the existing per-element gates
+# the Resampler's attention and LayerNorms at the production sizes, under the existing per-element gates (its GEMMs
+# run in test_gpu_gemm.py's production lists)
 # ---------------------------------------------------------------------------------------------------------------
-def resampler_launches(name, NB):
-    """The GEMM launches of one Resampler (one layer stands for all: the layers share their shapes)."""
-    g, D = PLUS[name], D_OF[name]
-    T, Q, E, dim, inner, F = T_VIT_H, g["num_queries"], g["embed_dim"], g["dim"], 64 * g["heads"], g["ff_mult"] * g["dim"]
-    p = f"{name} plus NB{NB} "
-    lin = lambda n, M, N, K, **kw: dict(name=p + n, kind="linear", M=M, N=N, K=K, **kw)  # noqa: E731
-    return [lin("proj_in", NB * T, dim, E), lin("to_q", NB * Q, inner, dim, bias=False),
-            lin("to_kv", NB * (T + Q), 2 * inner, dim, bias=False),
-            lin("to_out", NB * Q, dim, inner, bias=False, addend="in_place"),
-            lin("ff.1", NB * Q, F, dim, bias=False), lin("ff.3", NB * Q, dim, F, bias=False, addend="in_place"),
-            lin("proj_out", NB * Q, D, dim)]
-
-
-@pytest.mark.parametrize("NB", RESAMPLER_NB)
-@pytest.mark.parametrize("name", ["sd15", "sdxl"])
+@pytest.mark.parametrize("NB", P.IP_PLUS_NB)
+@pytest.mark.parametrize("name", [m for m, _ in P.IP_PLUS_ADAPTERS])
 def test_resampler_production_launches(name, NB):
     from test_gpu_attention import check
-    from test_gpu_gemm import gen, run_production
+    from test_gpu_gemm import gen
     from test_gpu_norms import ln_check, ln_inputs
-    for l in resampler_launches(name, NB):
-        run_production(l, None)
-        run_production(l, "flat")
-    geo = PLUS[name]
-    T, Q, H, dim = T_VIT_H, geo["num_queries"], geo["heads"], geo["dim"]
+    geo, D, T = _geometry(name)
+    Q, H, dim = geo["num_queries"], geo["heads"], geo["dim"]
     inner = 64 * H
     g = gen(NB * 7 + H)
     q = torch.randn(NB, Q, inner, generator=g, device=dev).half()
     kvb = torch.randn(NB, T + Q, 2 * inner, generator=g, device=dev).half()
     check(f"{name} plus NB{NB} sdpa", q, kvb[..., :inner], kvb[..., inner:], H, 64)
-    for M, C in ((NB * Q, dim), (NB * Q, D_OF[name])):
+    for M, C in ((NB * Q, dim), (NB * Q, D)):
         ln_check(f"{name} plus NB{NB} layernorm {M}x{C}", *ln_inputs(g, M, C, 10.0))
 
 

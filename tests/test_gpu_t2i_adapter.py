@@ -13,7 +13,7 @@ import torch
 import torch.nn.functional as F
 
 import controlnet_oracle as CO
-import t2i_adapter_sizes as TS
+import production as P
 import t2i_adapter_oracle as TO
 from helpers import rel_l2
 
@@ -31,11 +31,13 @@ def _lib():
 # kernels
 # ---------------------------------------------------------------------------------------------------------------
 def _unshuffle_cases():
+    """(factor, channels, H, W) of every T2I production size, once each (SD v1.5 and SD 2-base share 512²)."""
+    from cfgpp_b200 import config as C, t2i_adapter as T
     out = []
-    for name, sizes in TS.T2I_ADAPTER_SIZES.items():
-        f = 8 if name == "sd15" else 16
-        for h, w in sizes:
-            for c in (1, 3):
+    for name, h, w in P.t2i_sizes():
+        f = T.t2i_adapter_config(C.CONFIGS[name]()).downscale_factor
+        for c in (1, 3):
+            if (f, c, 8 * h, 8 * w) not in out:
                 out.append((f, c, 8 * h, 8 * w))
     return out
 
@@ -94,10 +96,23 @@ def test_relu_and_scale_bit_exact():
         assert torch.equal(out.view(torch.int16)[ok], ref.view(torch.int16)[ok]) and torch.equal(out.isnan(), ~ok)
 
 
-@pytest.mark.parametrize("B,HW,C", [(1, 64 * 64, 320), (2, 32 * 32, 640), (4, 16 * 16, 1280), (8, 76 * 52, 320)])
+def _gated_add_cases():
+    """(B, HW, C) of every tensor a feature lands on (`unet_placements`) at every T2I production size, for B images
+    (UNet batch NB = 2B), once each."""
+    from cfgpp_b200 import config as C, t2i_adapter as T
+    out = []
+    for name, h, w in P.t2i_sizes():
+        for c, hh, ww in T.unet_placements(C.CONFIGS[name](), h, w):
+            for B in P.T2I_ADAPTER_BATCHES:
+                if (B, hh * ww, c) not in out:
+                    out.append((B, hh * ww, c))
+    return out
+
+
+@pytest.mark.parametrize("B,HW,C", _gated_add_cases())
 def test_gated_add(B, HW, C):
-    """On: bit for bit torch's fp16 add, rows b and B + b reading feature b. Off: not one bit written (-0.0 and NaN
-    included)."""
+    """At every placement of the production sizes. On: bit for bit torch's fp16 add, rows b and B + b reading feature
+    b. Off: not one bit written (-0.0 and NaN included)."""
     nv, lib = _lib()
     g = torch.Generator().manual_seed(B + C)
     h = torch.randn(2 * B, HW, C, generator=g).half().to(dev)
@@ -129,8 +144,8 @@ def _adapter(name, in_channels=3, seed=7):
 
 
 def _adapter_cases():
-    return [(name, h, w, b, c) for name, sizes in TS.T2I_ADAPTER_SIZES.items() for h, w in sizes
-            for b in TS.T2I_ADAPTER_BATCHES for c in (3, 1)]
+    return [(name, h, w, b, c) for name, h, w in P.t2i_sizes() for b in P.T2I_ADAPTER_BATCHES
+            for c in P.T2I_IN_CHANNELS]
 
 
 @pytest.mark.parametrize("name,h,w,B,C", _adapter_cases())

@@ -1,6 +1,6 @@
 """The production size table (`production.py`) and the per-element case lists derived from it, checked without a GPU:
-every full-size UNet config, text tower, vision tower, ControlNet-capable UNet and IP-Adapter has sizes, and the GEMM /
-conv, attention, GroupNorm and LayerNorm case lists cover every (model, size). A model added to `config.CONFIGS` or `text_encoder.CLIP_CONFIGS` without sizes fails here,
+every full-size UNet config, text tower, vision tower, ControlNet-capable UNet, IP-Adapter (plain and Plus) and
+T2I-capable UNet has sizes, and the GEMM / conv, attention, GroupNorm and LayerNorm case lists cover every (model, size). A model added to `config.CONFIGS` or `text_encoder.CLIP_CONFIGS` without sizes fails here,
 on any machine, before its kernels go unpinned."""
 import pytest
 
@@ -63,7 +63,8 @@ def assert_covered(what, lists, run, key_of):
 
 def test_gemm_cases_cover_every_model_and_size():
     lists = TG.production_lists()
-    lists = {k: v for k, v in lists.items() if k[0] not in ("controlnet", "ip_adapter") and k[0] not in P.VISION_TOWERS}
+    lists = {k: v for k, v in lists.items()
+             if k[0] not in ("controlnet", "ip_adapter", "ip_adapter_plus", "t2i_adapter") and k[0] not in P.VISION_TOWERS}
     assert set(lists) == expected_keys()
     run = {TG.signature(p.values[0]) for p in TG._production_cases()}
     assert_covered("GEMM", lists, run, lambda e: TG.signature(e[1]))
@@ -212,3 +213,98 @@ def test_vision_attention_cases_listed():
     run = {tuple(p.values) for p in TA._vision_cases()}
     assert_covered("vision attention", lists, run, lambda e: e[1])
     assert {s[3] for v in lists.values() for _, s in v} == {80, 104}
+
+
+# ------------------------------------------------------------------------------------------------ IP-Adapter Plus, T2I-Adapter
+
+REQUIRED_IP_PLUS = {("sd15", 1280), ("sdxl", 1280)}
+# the refiner runs the steps after an SDXL hand-off without the base's T2I features, and no released adapter targets it
+NO_T2I = {"sdxl_refiner"}
+# adapter sizes beyond the UNet's own: SD v1.5 at 512x768, whose adapter levels are 96/48/24/12 wide (the im2col A tile)
+T2I_EXTRA_SIZES = {"sd15": {(64, 96)}}
+
+
+def test_every_ip_plus_adapter_listed():
+    assert REQUIRED_IP_PLUS <= set(P.IP_PLUS_ADAPTERS)
+    assert {2, 4, 16} <= set(P.IP_PLUS_NB)
+
+
+def test_every_t2i_unet_has_sizes():
+    capable = [m for m in full_size(C.CONFIGS) if m not in NO_T2I]
+    assert set(P.T2I_ADAPTER_SIZES) == set(capable), "T2I-Adapter sizes are not listed for exactly the capable UNets"
+    for m in capable:
+        want = set(P.UNET_SIZES[m]) | T2I_EXTRA_SIZES.get(m, set())
+        assert set(P.T2I_ADAPTER_SIZES[m]) == want, f"{m}: T2I-Adapter sizes {P.T2I_ADAPTER_SIZES[m]}, want {want}"
+    assert set(P.T2I_ADAPTER_BATCHES) == {1, 8} and set(P.T2I_IN_CHANNELS) == {1, 3}
+
+
+def test_adapter_gemm_lists_run():
+    lists = TG.production_lists()
+    want = {("t2i_adapter", m, (h, w)) for m, h, w in P.t2i_sizes()}
+    want |= {("ip_adapter_plus", m, E) for m, E in P.IP_PLUS_ADAPTERS}
+    assert want <= set(lists)
+    run = {TG.signature(p.values[0]) for p in TG._production_cases()}
+    assert_covered("GEMM", {k: lists[k] for k in want}, run, lambda e: TG.signature(e[1]))
+
+
+@pytest.mark.parametrize("in_channels", P.T2I_IN_CHANNELS)
+@pytest.mark.parametrize("model", sorted(P.T2I_ADAPTER_SIZES))
+def test_t2i_launches_match_param_specs(model, in_channels):
+    """Every `adapter.*` weight of `t2i_adapter_param_specs` is the weight of exactly one derived launch, by name, with
+    its (N, K) (a 3x3 conv's K = 9·Cin), and every launch has a weight; block2 adds its residual in place."""
+    from cfgpp_b200 import t2i_adapter as T
+    cfg = T.t2i_adapter_config(C.CONFIGS[model](), in_channels)
+    specs = {k[:-len(".weight")]: shape for k, shape, _ in T.t2i_adapter_param_specs(cfg) if k.endswith(".weight")}
+    for h, w in P.T2I_ADAPTER_SIZES[model]:
+        for B in P.T2I_ADAPTER_BATCHES:
+            launches = TG.t2i_adapter_gemm_launches(cfg, 8 * h, 8 * w, B)
+            names = [l["name"] for l in launches]
+            assert sorted(names) == sorted(specs), f"{model} {h}x{w} B{B}: launches {names}, weights {sorted(specs)}"
+            for l in launches:
+                cout, cin, kh, kw = specs[l["name"]]
+                if l["kind"] == "conv":
+                    assert (kh, kw) == (3, 3) and (l["Cout"], 9 * l["Cin"], l["B"]) == (cout, 9 * cin, B), l["name"]
+                else:
+                    assert (kh, kw) == (1, 1) and (l["N"], l["K"]) == (cout, cin) and l["M"] % B == 0, l["name"]
+                assert (l.get("addend") == "in_place") == l["name"].endswith(".block2"), l["name"]
+            assert launches[0]["Cin"] == in_channels * cfg.downscale_factor ** 2
+            assert launches[0]["H"] * cfg.downscale_factor == 8 * h
+
+
+@pytest.mark.parametrize("model,E", sorted(REQUIRED_IP_PLUS))
+def test_ip_plus_launches_match_resampler_shapes(model, E):
+    """The Plus list's Resampler launches have the (N, K) of `resampler_shapes(plus_geometry(...), D)` for their weight
+    keys (one layer stands for all, the layers' shapes are equal), over every weight matrix; to_kv_ip runs at
+    M = NB·num_queries; there is no image_proj.proj."""
+    from cfgpp_b200 import ip_adapter as IP
+    cfg = C.CONFIGS[model]()
+    g = IP.plus_geometry(cfg, E)
+    shapes = IP.resampler_shapes(g, cfg.cross_attention_dim)
+    mats = {k[:-len(".weight")] for k, s in shapes.items() if k.endswith(".weight") and len(s) == 2}
+    T = IP.plus_encoder_config(cfg, E).num_positions
+    for NB in P.IP_PLUS_NB:
+        launches = [l for l in TG.ip_plus_launches(model, E) if l["name"].startswith(f"NB{NB} ")]
+        names = {l["name"][len(f"NB{NB} "):]: l for l in launches}
+        res = {n: l for n, l in names.items() if n.startswith("image_proj.")}
+        assert set(res) == {m for m in mats if not m.startswith("image_proj.layers.") or ".layers.0." in m}
+        for n, l in res.items():
+            assert (l["N"], l["K"]) == shapes[n + ".weight"], n
+            assert l["M"] == NB * (T + g["num_queries"] if n.endswith("to_kv") else
+                                   T if n.endswith("proj_in") else g["num_queries"]), n
+        kv = [l for n, l in names.items() if n.endswith(".attn2.to_kv_ip")]
+        assert len(kv) == len(IP.processor_blocks(cfg))
+        assert {l["M"] for l in kv} == {NB * g["num_queries"]}
+    assert g["num_queries"] == 16 and T == 257
+
+
+def test_adapter_lists_cover_their_edges():
+    """The T2I lists hold an in-place residual, convolutions at the 96/48/24/12-wide levels (the im2col A tile) and
+    both image batches; the Plus lists run to_kv_ip with 16 image tokens."""
+    lists = TG.production_lists()
+    t2i = [l for k, v in lists.items() if k[0] == "t2i_adapter" for _, l in v]
+    assert any(l.get("addend") == "in_place" for l in t2i)
+    convs = [l for l in t2i if l["kind"] == "conv"]
+    assert {96, 48, 24, 12} <= {l["W"] for l in convs}
+    assert {l["B"] for l in convs} == set(P.T2I_ADAPTER_BATCHES)
+    plus = [l for k, v in lists.items() if k[0] == "ip_adapter_plus" for _, l in v]
+    assert 4 * 16 in {l["M"] for l in plus if l["name"].endswith("to_kv_ip")}

@@ -8,7 +8,6 @@ import torch
 
 import controlnet_oracle as CO
 import production as P
-import t2i_adapter_sizes as TS
 import t2i_adapter_oracle as TO
 from cfgpp_b200 import config as C, t2i_adapter as T
 
@@ -70,8 +69,7 @@ def test_state_dict_key_census(name, in_channels):
 
 
 def _placement_cases():
-    cases = [(m, h, w) for m, sizes in TS.T2I_ADAPTER_SIZES.items() for h, w in sizes]
-    cases += [("sd2", h, w) for h, w in P.UNET_SIZES["sd2"]] + [("sd2_base", 64, 64)]
+    cases = P.t2i_sizes()
     from test_gpu_aspect_buckets import SDXL_BUCKETS  # latent (h, w) of every SDXL aspect-ratio bucket
     cases += [("sdxl", h, w) for h, w in SDXL_BUCKETS]
     cases += [("tiny_sd15", 32, 32), ("tiny_sd15", 16, 32), ("tiny_sd2", 16, 16), ("tiny_sdxl", 32, 32),
