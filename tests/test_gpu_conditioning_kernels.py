@@ -8,7 +8,8 @@ Then the two executors against chains of their per-element pinned ops, bit for b
 image_to_nhwc → (conv3x3 → SiLU)* → conv_out with the weights zero-padded in torch to the packed layout (pinning
 `packed_conv3x3`, the strides, the padded widths and where SiLU runs), and `NativeCLIPVisionEncoder.encode` equals
 patchify → patch GEMM → vision_embed → pre-LN → per layer (LN, qkv over heads padded in torch, attention, out_proj +
-residual, LN, fc1, activation, fc2 + residual) → class row → post-LN → projection."""
+residual, LN, fc1, activation, fc2 + residual) → class row → post-LN → projection (`vision_chain` of
+test_gpu_encoder_chains.py, which also pins the tower's hidden states)."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -191,51 +192,10 @@ def test_conditioning_embedding_equals_its_ops(model, B, S):
 
 # ---- composition: the CLIP vision tower -----------------------------------------------------------------------------
 
-def vision_chain(cfg, sd, px):
-    """image_embeds from the pinned ops, in `ClipVisionEncoder::encode` / `build_clip_layers` order."""
-    from cfgpp_b200 import _native as nv
-    D, I, H, P, S = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads, cfg.patch_size, cfg.image_size
-    hd = D // H
-    hdp = pad64(hd)
-    Cp, K, B, T, eps = H * hdp, 3 * P * P, px.shape[0], cfg.num_positions, cfg.layer_norm_eps
-    act = {"quick_gelu": 0, "gelu": 1}[cfg.hidden_act]
-    vm = "vision_model."
-
-    def w(k):
-        return sd[k].half()
-
-    patches = nv.op_clip_patchify(px, P, pad64(K))
-    wp = torch.zeros(D, pad64(K), dtype=torch.float16, device=dev)
-    wp[:, :K] = w(vm + "embeddings.patch_embedding.weight").reshape(D, K)
-    pe = nv.op_linear(patches, wp)
-    emb = nv.op_clip_vision_embed(pe, w(vm + "embeddings.class_embedding"),
-                                  w(vm + "embeddings.position_embedding.weight"), B)
-    x0 = nv.op_layernorm(emb, w(vm + "pre_layrnorm.weight"), w(vm + "pre_layrnorm.bias"), eps)
-    for l in range(cfg.num_hidden_layers):
-        p = f"{vm}encoder.layers.{l}."
-        wqkv = torch.zeros(3, H, hdp, D, dtype=torch.float16, device=dev)
-        bqkv = torch.zeros(3, H, hdp, dtype=torch.float16, device=dev)
-        for i, n in enumerate(("q_proj", "k_proj", "v_proj")):
-            wqkv[i, :, :hd] = w(p + f"self_attn.{n}.weight").view(H, hd, D)
-            bqkv[i, :, :hd] = w(p + f"self_attn.{n}.bias").view(H, hd)
-        wo = torch.zeros(D, H, hdp, dtype=torch.float16, device=dev)
-        wo[:, :, :hd] = w(p + "self_attn.out_proj.weight").view(D, H, hd)
-        ln = nv.op_layernorm(x0, w(p + "layer_norm1.weight"), w(p + "layer_norm1.bias"), eps)
-        qkv = nv.op_linear(ln, wqkv.reshape(3 * Cp, D), bqkv.reshape(-1)).view(B, T, 3 * Cp)
-        att = nv.op_attention(qkv[:, :, :Cp], qkv[:, :, Cp:2 * Cp], qkv[:, :, 2 * Cp:], H, head_dim=hd)
-        x1 = nv.op_linear(att.view(B * T, Cp), wo.reshape(D, Cp), w(p + "self_attn.out_proj.bias"), addend=x0)
-        ln = nv.op_layernorm(x1, w(p + "layer_norm2.weight"), w(p + "layer_norm2.bias"), eps)
-        m = nv.op_clip_activation(nv.op_linear(ln, w(p + "mlp.fc1.weight"), w(p + "mlp.fc1.bias")), act)
-        x0 = nv.op_linear(m, w(p + "mlp.fc2.weight"), w(p + "mlp.fc2.bias"), addend=x1)
-    cls = x0.view(B, T, D)[:, 0].contiguous()
-    cls = nv.op_layernorm(cls, w(vm + "post_layernorm.weight"), w(vm + "post_layernorm.bias"), eps)
-    out, _ = nv.op_small_linear(cls, w("visual_projection.weight"))
-    return out
-
-
 @pytest.mark.parametrize("tower,B", [("tiny_vision", 1), ("tiny_vision", 3), ("vit_h", 2), ("vit_bigg", 1)])
 def test_vision_tower_equals_its_ops(tower, B):
     from cfgpp_b200 import vision_encoder as V
+    from test_gpu_encoder_chains import vision_chain
     cfg = getattr(V, f"{tower}_config")()
     sd = V.synthetic_state_dict(cfg, seed=3, device=dev)
     enc = V.NativeCLIPVisionEncoder(cfg, sd, dev)
@@ -244,5 +204,5 @@ def test_vision_tower_equals_its_ops(tower, B):
         got = enc.encode(px)
     finally:
         enc.close()
-    want = vision_chain(cfg, sd, px)
+    want, _ = vision_chain(cfg, sd, px)
     assert_bits(f"{tower} B{B} image_embeds vs its ops", got, want)

@@ -427,9 +427,9 @@ def _run(name, B, h, w, t, in_scale=1.0, zdtype=torch.float32, add_rows="2B", se
                 e = torch.randn(B, ad.embed_dim, generator=g).half().to(dev)
             net.set_ip_image_embeds(e)
             net.set_ip_adapter_scale(scale)
-            if ad.resampler is not None:  # the Resampler's tokens, pinned on their own (test_gpu_ip_adapter_plus.py)
-                tokens = torch.empty(2 * B * ad.n_tokens, cfg.cross_attention_dim, dtype=torch.float16, device=dev)
-                nv.check(net.lib.cfgpp_dbg_ip_image_proj(net._h, nv.ptr(tokens), nv.stream_ptr()))
+            if ad.resampler is not None:  # the Resampler over the rows the engine hands it, unconditional rows first
+                from test_gpu_encoder_chains import resampler_chain
+                tokens = resampler_chain(ad.weights, ad.image_rows(e), ad.resampler, cfg.cross_attention_dim)
             else:  # image_proj: Linear(E -> T * D), then LayerNorm(D) of every token
                 rows = torch.cat([torch.zeros_like(e), e])
                 D, Tn = cfg.cross_attention_dim, ad.n_tokens
@@ -514,7 +514,7 @@ def test_t2i_adapter_equals_its_ops(name, B, hw, on):
                                             ("sd15", 1, 64, False), ("sdxl", 1, 128, True)])
 def test_ip_adapter_equals_its_ops(name, B, hw, plus):
     """The decoupled cross-attention over the image tokens at scale 0.6: image_proj (Linear + LayerNorm) for the
-    plain adapter, the pinned Resampler tokens for Plus, then every block's to_k_ip / to_v_ip."""
+    plain adapter, `resampler_chain` over the hidden-state rows for Plus, then every block's to_k_ip / to_v_ip."""
     from cfgpp_b200 import ip_adapter as IP
     cfg, _, _ = _unet(name)
     ad = IP.IPAdapter(f"chain-{name}", dev, cfg, image_proj="resampler" if plus else None)
